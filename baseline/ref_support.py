@@ -7,7 +7,7 @@ reference process.  Everything here is plain Python + numpy + NVML:
 * :func:`write_synthetic_mnist` writes idx files of MNIST's shape where ``torchvision.datasets.MNIST``
   expects them (the reference calls it with ``download=True``, ref: ddp_example.py:66-69; with the raw
   files present torchvision skips the download);
-* :class:`Clocks` samples SM clock / throttle reasons during the timed region (B200_PROFILING.md).
+* :class:`Clocks` samples SM clock / throttle reasons during the timed region.
 """
 from __future__ import annotations
 

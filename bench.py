@@ -12,7 +12,7 @@ N > 1 is launched one rank per GPU by ``python -m torch.distributed.run --nproc-
 Timed regions (both arms): W >= 3 untimed warm-up steps, then exactly K steps between
 barrier + torch.cuda.synchronize() on both sides, CUDA events on the launching stream, MAX over
 ranks.  ``value`` is the device-timed step with inputs rotating through a device-resident pool that
-is larger than L2 (164 MB > 126 MB).  ``e2e`` is the same step driven end to end through the framework's
+is larger than L2 (161 MB > 50 MB on an H100).  ``e2e`` is the same step driven end to end through the framework's
 own input path — ``data.MNIST`` on synthetic idx files -> ``DistributedSampler`` -> ``DataLoader(pin_memory=True)``
 -> H2D of every batch -> whole-step graph -> D2H of every loss — i.e. the loop of ``cli.dist_train``
 (ref: ddp_example.py:66-95).  Both arms print the same ``config`` dict; arm-specific facts live in ``details``.
@@ -32,7 +32,7 @@ sys.path.insert(0, ROOT)
 
 BATCH = 100                    # per GPU (ref: ddp_example.py:59)
 IMG = (1, 28, 28)
-POOL_BATCHES = 512             # 512 x 100 x 784 x 4 B = 160.6 MB of images  > 126 MB L2
+POOL_BATCHES = 512             # 512 x 100 x 784 x 4 B = 160.6 MB of images  > 50 MB L2
 LR = 1e-4                      # ref: ddp_example.py:62
 METRIC = "MNIST ConvNet DDP training throughput (images/sec, device-timed, max over ranks)"
 WINDOWS = 5                    # the K timed steps are also reported as 5 back-to-back windows (min / median / max)
@@ -50,6 +50,9 @@ def parse():
     p.add_argument("--conv-impl", default="auto", choices=["auto", "simt", "tcgen05"])
     p.add_argument("--skip-e2e", action="store_true")
     p.add_argument("--skip-verify", action="store_true", help="skip the pre-timing cross-check against torch autograd (+NCCL)")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="after the timed steps, write what the last timed step produced (its loss, the updated parameters and "
+                        "BatchNorm statistics) as DIR/<name>.npy, float32; rank 0 only")
     return p.parse_args()
 
 
@@ -58,10 +61,10 @@ def env_rank():
 
 
 def shared_config(world: int, syncbn: bool) -> dict:
-    """The benchmark configuration — byte-identical in both arms (the driver compares it)."""
+    """The benchmark configuration — byte-identical in both arms, so that their results can be compared."""
     return {"model": "ConvNet (ref ddp_example.py:22-41)", "global_batch": BATCH * world, "per_gpu_batch": BATCH, "seq_len": None,
             "parallelism": f"dp{world}", "optimizer": "SGD lr=1e-4", "syncbn": bool(syncbn),
-            "inputs": f"rotating pool of {POOL_BATCHES} batches = {POOL_BATCHES * BATCH * 784 * 4 / 1e6:.0f} MB > 126 MB L2 (no explicit L2 flush)",
+            "inputs": f"rotating pool of {POOL_BATCHES} batches = {POOL_BATCHES * BATCH * 784 * 4 / 1e6:.0f} MB > 50 MB L2 (no explicit L2 flush)",
             "e2e_inputs": "synthetic MNIST idx files -> dataset -> DistributedSampler -> DataLoader(pin_memory) -> H2D every step"}
 
 
@@ -76,9 +79,8 @@ def window_stats(marks):
     return {"n": len(per), "min_ms_per_step": min(per), "median_ms_per_step": statistics.median(per), "max_ms_per_step": max(per)}
 
 
-def ensure_synthetic_mnist(local_rank: int) -> str:
-    """Synthetic idx files where both arms' MNIST datasets look for them (./data/MNIST/raw); written once."""
-    data_root = os.path.join(os.getcwd(), "data")
+def ensure_synthetic_mnist(local_rank: int, data_root: str) -> str:
+    """Synthetic idx files where the MNIST datasets look for them (<data_root>/MNIST/raw); written once."""
     marker = os.path.join(data_root, "MNIST", "raw", ".synthetic_ready")
     if local_rank == 0 and not os.path.exists(marker):
         sys.path.insert(0, os.path.join(ROOT, "baseline"))
@@ -163,6 +165,18 @@ def verify_ours(pdt, ddp, criterion, dev, rank, world, x, y):
     out["oracle"] = "torch.nn modules + autograd (cuDNN/cuBLAS)" + (" + NCCL all_reduce / N" if world > 1 else "")
     out["ok"] = bool(out["params_identical_across_ranks"] and out["grad_max_rel_err"] < out["tolerance"] and out["loss_abs_err"] < 1e-3)
     return out
+
+
+def dump_outputs(out_dir, loss, module):
+    """What the last timed step hands back to its caller: the loss, and the parameters and BatchNorm statistics it updated."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": loss.detach().reshape(1)}
+    arrays.update({f"param.{k}": v.detach() for k, v in module.named_parameters()})
+    arrays.update({f"buffer.{k}": v.detach() for k, v in module.named_buffers() if v.is_floating_point()})
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.float().cpu().numpy())
 
 
 def run_ours(args):
@@ -272,10 +286,20 @@ def run_ours(args):
     with ClockSampler(gpu_index=local_rank, period_ms=100) as clocks:
         ms_dev, _, eager_launches, windows = timed(dev_step, W, K)
         final_loss = float(last["loss"].detach())
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, last["loss"], ddp.module)
         # ---- end to end through the framework's own input path (the loop of cli.dist_train) -----------
         e2e = None
+        private_root = None
         if not args.skip_e2e:
-            data_root = ensure_synthetic_mnist(local_rank)
+            # a directory of this run's own, outside the source tree (which may be read-only): rank 0 creates it and writes the
+            # files, every rank learns its path, and it is removed when the run ends
+            import tempfile
+
+            private_root = tempfile.mkdtemp(prefix="pdt_bench_mnist_") if rank == 0 else None
+            if world > 1:
+                private_root = pdt.distributed.all_gather_object(private_root)[0]
+            data_root = ensure_synthetic_mnist(local_rank, private_root)
             dataset = pdt.data.MNIST(root=data_root, train=True)
             sampler = pdt.DistributedSampler(dataset, num_replicas=world, rank=rank)
             loader = pdt.DataLoader(dataset=dataset, batch_size=BATCH, shuffle=False, num_workers=0, pin_memory=True, sampler=sampler,
@@ -378,6 +402,12 @@ def run_ours(args):
                                   "GraphedTrainStep(pinned images, pinned labels): H2D + whole-step graph replay; step.loss_to_host(): async D2H of every "
                                   "loss; blocking read of every 10th loss on rank 0, issued after the following step has been queued (the loop of "
                                   "cli.dist_train; cadence of ref ddp_example.py:93-95)"}
+    if private_root is not None:
+        pdt.distributed.barrier()   # every rank is done with the files
+        if rank == 0:
+            import shutil
+
+            shutil.rmtree(private_root, ignore_errors=True)
     pdt.destroy_process_group()
     if verify is not None and not verify["ok"]:
         if out is not None:
@@ -483,7 +513,7 @@ def run_reference(args):
         e2e_err = None
         if not args.skip_e2e:
             try:
-                ensure_synthetic_mnist(local_rank)
+                ensure_synthetic_mnist(local_rank, os.path.join(os.getcwd(), "data"))   # where ddp_example.py reads MNIST
                 e2e_ms = _reference_e2e(ref, args, rank, local_rank, world, W, K, base_port + 12)
             except Exception as e:  # noqa: BLE001
                 e2e_err = f"{type(e).__name__}: {e}"[:300]
@@ -565,6 +595,8 @@ def _reference_e2e(ref, args, rank, local_rank, world, W, K, port):
 
 def main():
     args = parse()
+    if args.dump_outputs and args.impl == "reference":
+        raise SystemExit("--dump-outputs writes what this framework's timed step computed; it is not available with --impl reference")
     if args.impl == "reference":
         out = run_reference(args)
     else:

@@ -1,9 +1,9 @@
-"""pytorch_distributed_train_b200 — a B200-native distributed data-parallel training engine.
+"""pytorch_distributed_train_b200 — a H100-native distributed data-parallel training engine.
 
 Same capabilities and entry points as the tutorial repo it replaces (spawn launcher,
 ``init_process_group``, ``DistributedDataParallel``, ``DistributedSampler``, ``SyncBatchNorm``,
-MNIST ConvNet training CLI), rebuilt B200-first: own C++ store / process groups / reducer, and
-sm_100a CUDA kernels for the gradient allreduce over NVLink peer memory and for the model's hot
+MNIST ConvNet training CLI), rebuilt H100-first: own C++ store / process groups / reducer, and
+sm_90a CUDA kernels for the gradient allreduce over NVLink peer memory and for the model's hot
 ops.  PyTorch is the tensor + autograd substrate only.
 """
 from __future__ import annotations

@@ -4,11 +4,11 @@ One shared object, three kinds of translation units:
 
 * torch-free C++ (store, sockets, CPU collectives, bucket planner) — plain ``g++``;
 * torch-facing C++ (comm facade, reducer, bindings, CUDA host glue) — ``g++`` with torch headers;
-* sm_100a CUDA (collective + compute kernels) — ``nvcc -gencode arch=compute_100a,code=sm_100a
+* sm_90a CUDA (collective + compute kernels) — ``nvcc -gencode arch=compute_90a,code=sm_90a
   -lineinfo``; these TUs never include torch headers so they compile in seconds and
   cross-compile on a GPU-less box.
 
-The ``.so`` is written next to the sources so it travels with a ``gpurun`` snapshot.
+The ``.so`` is written next to the sources, so the package imports straight from the source tree.
 Objects are cached under ``build/`` keyed by a content hash of the TU, its flags and every
 header in ``csrc/``.
 """
@@ -32,7 +32,7 @@ STAMP = PKG / "_C.stamp"
 
 CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 NVCC = os.path.join(CUDA_HOME, "bin", "nvcc")
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _torch_paths():
@@ -136,7 +136,7 @@ def build(verbose: bool = False, force: bool = False, ptxas_info: bool = False) 
         keys.append(key)
         obj = BUILD / f"{src.relative_to(CSRC).as_posix().replace('/', '__')}.{key}.o"
         objs.append(obj)
-    # The stamp travels with the .so (gpurun snapshot), so a box that has the library but not the
+    # The stamp travels with the .so, so a copy of the tree that has the library but not the
     # object cache does not rebuild.
     stamp = hashlib.sha256("".join(keys).encode()).hexdigest()
     if not force and OUT.exists() and STAMP.exists() and STAMP.read_text().strip() == stamp:

@@ -27,7 +27,7 @@ def _free_port() -> int:
 
 
 def build_parser() -> argparse.ArgumentParser:
-    p = argparse.ArgumentParser(description="B200-native DDP training (MNIST ConvNet / ResNet-18)")
+    p = argparse.ArgumentParser(description="H100-native DDP training (MNIST ConvNet / ResNet-18)")
     p.add_argument("-g", "--gpus", default=1, type=int, help="number of gpus per node")
     p.add_argument("--epochs", default=2, type=int, metavar="N", help="number of total epochs to run")
     p.add_argument("--backend", default="nccl", type=str, help="backend used for distributed train (nccl | gloo)")

@@ -33,7 +33,7 @@ py::class_<S, Store, std::shared_ptr<S>> bind_store(py::module_& m, const char* 
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "pytorch_distributed_train_b200 native runtime: stores, CPU/NVLink/NCCL collectives, reducer, sm_100a ops";
+  m.doc() = "pytorch_distributed_train_b200 native runtime: stores, CPU/NVLink/NCCL collectives, reducer, sm_90a ops";
 
   py::register_exception<TimeoutError>(m, "TimeoutError", PyExc_TimeoutError);
   py::register_exception<PeerClosedError>(m, "PeerClosedError", PyExc_ConnectionError);

@@ -1,6 +1,6 @@
 // Tensor-level collective interface implemented by every backend:
 //   CpuComm     – TCP mesh on host tensors (csrc/cpu)                        ["gloo" slot]
-//   SymmComm    – sm_100a kernels over NVLink peer / multicast memory (csrc/cuda) [product path]
+//   SymmComm    – sm_90a kernels over NVLink peer / multicast memory (csrc/cuda) [product path]
 //   NcclComm    – thin libnccl binding, measured baseline + oracle only       ["--comm nccl"]
 // Semantics follow the ProcessGroup contract the reference relies on
 // (ref: ddp_example.py:50,64; torch c10d ProcessGroup.hpp / Work.hpp): collectives are
@@ -31,8 +31,7 @@ class CommWork {
 };
 
 // A point in device time: an event on the compute (or comm) stream for CUDA backends, the host clock otherwise.
-// The reducer's logger is built on these so that its numbers are *device* times (SURVEY §2.3 B11: "CUDA-event
-// timers for fwd / bwd-compute / bwd-comm"), not host enqueue times.
+// The reducer's logger is built on these so that its numbers are *device* times, not host enqueue times.
 class DeviceStamp {
  public:
   virtual ~DeviceStamp() = default;
@@ -86,7 +85,7 @@ class Comm {
   virtual std::shared_ptr<DeviceStamp> stamp(bool on_comm_stream = false);
   virtual bool capturing() const { return false; }
 
-  // Flight recorder (SURVEY §5.5): ring of the last K collectives issued on this rank.
+  // Flight recorder: ring of the last K collectives issued on this rank.
   struct Record { uint64_t seq; std::string op; int64_t numel; std::string dtype; double t_enqueue; };
   std::vector<Record> flight_records() const;
 

@@ -63,7 +63,7 @@ class CpuBackend {
   std::shared_ptr<Work> recv(void* buf, size_t nbytes, int src);
   std::shared_ptr<Work> barrier();
 
-  // Fault injection for the failure tests (SURVEY §5.3): the next `n` ops on this rank
+  // Fault injection for the failure tests: the next `n` ops on this rank
   // sleep `ms` before running / are silently skipped.
   void inject_delay(int n_ops, int ms) { delay_ops_ = n_ops; delay_ms_ = ms; }
   void inject_skip(int n_ops) { skip_ops_ = n_ops; }

@@ -1,19 +1,20 @@
-// tcgen05 / TMEM / TMA kernels for sm_100a (hand-written PTX; no CUTLASS).
+// wgmma / TMA kernels for sm_90a (hand-written PTX; no CUTLASS).  The file and the "umma" kernel names date from the
+// first (Blackwell) version of the project; the kernels are Hopper's.
 //
 //  * gemm_tf32_umma_kernel — D[M,N] = A[M,K]·B[N,K]^T: both operands arrive by TMA
-//    (cp.async.bulk.tensor, SWIZZLE_128B), one elected thread issues tcgen05.mma.kind::tf32,
-//    the fp32 accumulator lives in TMEM and is read back with tcgen05.ld.  It is the self-test
+//    (cp.async.bulk.tensor, SWIZZLE_128B), one warpgroup issues wgmma.mma_async ... .tf32,
+//    the fp32 accumulator lives in its registers.  It is the self-test
 //    for every descriptor/barrier convention used below (tests/test_gpu_ops.py).
 //  * conv5x5_umma_kernel — the ConvNet's conv2 (88% of the model's FLOPs; ref:
 //    ddp_example.py:30) and its data gradient as an implicit GEMM: M = output pixels (128 per
 //    tile), N = output channels, K = 25 taps × input channels.  The im2col A-tile is never
 //    materialised in global memory: four producer warps gather it straight from the NHWC
 //    activation with 16-byte cp.async (zero-fill for the padding halo) into the 128B-swizzled
-//    K-major layout the UMMA descriptor expects; the repacked weights (B) are TMA-loaded once
+//    K-major layout the wgmma descriptor expects; the repacked weights (B) are TMA-loaded once
 //    per CTA and stay resident in smem; the epilogue adds the bias, folds the per-channel
 //    Σy/Σy² that BatchNorm needs (saving a full re-read of y) and writes the tile with a TMA
 //    store.  TF32 inputs / fp32 accumulate is the same numerics contract the reference gets from
-//    cuDNN (torch allows TF32 in convolutions by default; SURVEY §2.5).
+//    cuDNN (torch allows TF32 in convolutions by default).
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -27,6 +28,7 @@
 
 #include "conv_tcgen05.h"
 #include "umma_ptx.cuh"
+#include "wgrad_win.cuh"
 #include "cuda_utils.h"
 #include "grid_fold.cuh"
 #include "grid_sync.cuh"
@@ -42,21 +44,23 @@ constexpr int kChunkK = 32;            // fp32 elements per 128-byte swizzle row
 constexpr int kStageBytes = kTileM * 128;
 
 // =====================================================================================================
-// TF32 GEMM self-test:  one CTA per 128-row tile of D; 4-stage TMA ring; 128 threads
+// TF32 GEMM self-test:  one CTA per 128-row × NB-column tile of D; 4-stage TMA ring; 160 threads
+// (warps 0-3 = the wgmma warpgroup, warp 4 = TMA producer)
 // =====================================================================================================
-template <int NT>  // N tile = whole N, multiple of 16, <= 256; TMEM columns = next pow2 >= 32
+template <int NB>  // N block = 16, 32 or 64 columns
 struct GemmCfg {
   static constexpr int kStages = 4;
-  static constexpr int kTmemCols = NT <= 32 ? 32 : NT <= 64 ? 64 : NT <= 128 ? 128 : 256;
-  static constexpr int kBBytes = NT * 128;
+  static constexpr int kBBytes = NB * 128;
   static constexpr size_t kSmem = 1024 + kStages * (kStageBytes + kBBytes) + 256;
 };
 
-template <int NT>
-__global__ void __launch_bounds__(128, 1) gemm_tf32_umma_kernel(const __grid_constant__ CUtensorMap tm_a,
+template <int NB>
+__global__ void __launch_bounds__(160, 1) gemm_tf32_umma_kernel(const __grid_constant__ CUtensorMap tm_a,
                                                                 const __grid_constant__ CUtensorMap tm_b, float* __restrict__ d, int M,
                                                                 int N, int K) {
-  using Cfg = GemmCfg<NT>;
+  using Cfg = GemmCfg<NB>;
+  constexpr int kN = NB < 32 ? NB : 32;   // wgmma N per instruction
+  constexpr int kNI = NB / kN;            // instructions per 64-row half
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sa = smem;
@@ -64,71 +68,65 @@ __global__ void __launch_bounds__(128, 1) gemm_tf32_umma_kernel(const __grid_con
   uint64_t* bars = reinterpret_cast<uint64_t*>(sb + Cfg::kStages * Cfg::kBBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::kStages;
-  uint64_t* accum_full = bars + 2 * Cfg::kStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::kStages + 1);
 
-  const int warp = threadIdx.x >> 5;
-  const int m0 = blockIdx.x * kTileM;
+  const int tid = threadIdx.x, warp = tid >> 5;
+  const int m0 = blockIdx.x * kTileM, n0 = blockIdx.y * NB;
   const int nk = (K + kChunkK - 1) / kChunkK;
 
-  if (threadIdx.x == 0) {
+  if (tid == 0) {
     tma_prefetch_desc(&tm_a);
     tma_prefetch_desc(&tm_b);
-    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(accum_full, 1);
+    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 128); }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (elect_one()) {
       for (int kc = 0; kc < nk; ++kc) {
         const int s = kc % Cfg::kStages;
         mbar_wait(&empty[s], ((kc / Cfg::kStages) & 1) ^ 1);
         mbar_arrive_expect_tx(&full[s], kStageBytes + Cfg::kBBytes);
         tma_load_2d(sa + s * kStageBytes, &tm_a, &full[s], kc * kChunkK, m0);
-        tma_load_2d(sb + s * Cfg::kBBytes, &tm_b, &full[s], kc * kChunkK, 0);
+        tma_load_2d(sb + s * Cfg::kBBytes, &tm_b, &full[s], kc * kChunkK, n0);
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = umma_idesc_tf32(kTileM, NT);
-    for (int kc = 0; kc < nk; ++kc) {
-      const int s = kc % Cfg::kStages;
-      mbar_wait(&full[s], (kc / Cfg::kStages) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t a0 = smem_u32(sa + s * kStageBytes), b0 = smem_u32(sb + s * Cfg::kBBytes);
+    return;
+  }
+  float acc[2][kNI][kN / 2];
 #pragma unroll
-        for (int k = 0; k < kChunkK / 8; ++k)
-          umma_tf32(tmem_base, umma_desc_sw128(a0 + k * 32), umma_desc_sw128(b0 + k * 32), idesc, (kc | k) != 0);
-        umma_commit(&empty[s]);
-        if (kc == nk - 1) umma_commit(accum_full);
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < kNI; ++i)
+#pragma unroll
+      for (int e = 0; e < kN / 2; ++e) acc[h][i][e] = 0.f;
+  for (int kc = 0; kc < nk; ++kc) {
+    const int s = kc % Cfg::kStages;
+    mbar_wait(&full[s], (kc / Cfg::kStages) & 1);
+    const uint32_t a0 = smem_u32(sa + s * kStageBytes), b0 = smem_u32(sb + s * Cfg::kBBytes);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kChunkK / 8; ++k)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < kNI; ++i)
+          wgmma_tf32<kN>(acc[h][i], gmma_desc_kmajor<128>(a0 + h * 64 * 128 + k * 32), gmma_desc_kmajor<128>(b0 + i * kN * 128 + k * 32),
+                         (kc | k) != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    mbar_arrive(&empty[s]);
+  }
+  // epilogue straight from the register fragments
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < kNI; ++i)
+#pragma unroll
+      for (int e = 0; e < kN / 2; ++e) {
+        const int row = m0 + 64 * h + wgmma_frag_row(tid, e), col = n0 + i * kN + wgmma_frag_col(tid, e);
+        if (row < M && col < N) d[static_cast<size_t>(row) * N + col] = acc[h][i][e];
       }
-      __syncwarp();
-    }
-  }
-  // epilogue: all four warps, warp w owns TMEM lanes 32w..32w+31 = D rows m0+32w+lane
-  mbar_wait(accum_full, 0);
-  __syncwarp();  // tcgen05.ld is .sync.aligned: the elected producer/MMA lane must have rejoined
-  tc_fence_after();
-  const int row = m0 + warp * 32 + (threadIdx.x & 31);
-#pragma unroll 1
-  for (int c0 = 0; c0 < NT; c0 += 16) {
-    float v[16];
-    tmem_ld_32x32b_x16(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + c0, v);
-    if (row < M) {
-#pragma unroll
-      for (int j = 0; j < 16; j += 4)
-        if (c0 + j < N) *reinterpret_cast<float4*>(d + static_cast<size_t>(row) * N + c0 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<Cfg::kTmemCols>(tmem_base);
 }
 
 // =====================================================================================================
@@ -149,27 +147,25 @@ __global__ void repack_weights_kernel(const float* __restrict__ w, float* __rest
 }
 
 // =====================================================================================================
-// Implicit-GEMM 5x5 convolution on tcgen05
+// Implicit-GEMM 5x5 convolution on wgmma
 // =====================================================================================================
 template <int CK, int NOUT>
 struct ConvCfg {
   static constexpr int kTapsPerChunk = kChunkK / CK;                           // 2 (fwd) / 1 (dgrad)
   static constexpr int kChunks = (25 + kTapsPerChunk - 1) / kTapsPerChunk;     // 13 / 25
-  // 8 smem stages but only 3 cp.async groups in flight per thread: a chunk is signalled "full"
-  // kLag iterations after it was issued, so stages - kLag is the slack the MMA warp has to drain a
-  // stage before the producers need it back (4 stages / lag 3 left a slack of one stage and the
-  // mainloop ran at ~1.8k cycles per chunk — profiles/conv_umma_v1.md).
+  // 8 smem stages but only 3 cp.async groups in flight per thread: a chunk is multiplied kLag
+  // iterations after it was issued, so the copies of the next chunks overlap the MMAs.
   static constexpr int kStages = 8;
   static constexpr int kLag = 3;
   static constexpr int kBChunkBytes = NOUT * 128;
-  static constexpr int kTmemCols = 32;
-  static constexpr int kThreads = 192;                                         // 4 producer/epilogue warps + MMA warp + TMA warp
-  // alignment slack + A ring + resident B + output staging + (barriers, tmem slot, stat partials)
-  static constexpr size_t kSmem = 1024 + kStages * kStageBytes + kChunks * kBChunkBytes + kTileM * 128 + 2048;
+  static constexpr int kAccBytes = kTileM * (NOUT + 1) * 4;
+  static constexpr int kThreads = 160;                                         // 4 producer/MMA/epilogue warps + TMA warp
+  // alignment slack + A ring + resident B + output staging + accumulator rows + (barriers, stat partials)
+  static constexpr size_t kSmem = 1024 + kStages * kStageBytes + kChunks * kBChunkBytes + kTileM * 128 + kAccBytes + 2048;
 };
 
 template <int CK, int NOUT, bool FWD>
-__global__ void __launch_bounds__(192, 1) conv5x5_umma_kernel(const float* __restrict__ x, const __grid_constant__ CUtensorMap tm_b,
+__global__ void __launch_bounds__(160, 1) conv5x5_umma_kernel(const float* __restrict__ x, const __grid_constant__ CUtensorMap tm_b,
                                                               const __grid_constant__ CUtensorMap tm_y, const float* __restrict__ bias,
                                                               float* __restrict__ y, float* stats, ReduceScratch scr, int B, int H, int W,
                                                               int num_tiles) {
@@ -179,14 +175,9 @@ __global__ void __launch_bounds__(192, 1) conv5x5_umma_kernel(const float* __res
   uint8_t* sa = smem;                                                  // [stages][128 rows][128 B] swizzled
   uint8_t* sb = sa + Cfg::kStages * kStageBytes;                       // [chunks][NOUT rows][128 B] swizzled (TMA)
   uint8_t* sy = sb + Cfg::kChunks * Cfg::kBChunkBytes;                 // [128 rows][128 B] swizzled output staging
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sy + kTileM * 128);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + Cfg::kStages;
-  uint64_t* b_full = bars + 2 * Cfg::kStages;
-  uint64_t* acc_full = b_full + 1;
-  uint64_t* acc_empty = b_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(b_full + 3);
-  float* s_part = reinterpret_cast<float*>(tmem_slot + 2);             // [4 warps][2*NOUT] + [2*NOUT]
+  float* sacc = reinterpret_cast<float*>(sy + kTileM * 128);          // [128][NOUT + 1] accumulator rows
+  uint64_t* b_full = reinterpret_cast<uint64_t*>(sacc + kTileM * (NOUT + 1));
+  float* s_part = reinterpret_cast<float*>(b_full + 2);               // [4 warps][2*NOUT] + [2*NOUT]
   __shared__ int s_last;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -195,49 +186,35 @@ __global__ void __launch_bounds__(192, 1) conv5x5_umma_kernel(const float* __res
   if (tid == 0) {
     tma_prefetch_desc(&tm_b);
     if (FWD) tma_prefetch_desc(&tm_y);
-    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full[s], 128); mbar_init(&empty[s], 1); }
     mbar_init(b_full, 1);
-    mbar_init(acc_full, 1);
-    mbar_init(acc_empty, 128);
     fence_mbar_init();
   }
-  if (warp == 4) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 5) {
+  if (warp == 4) {
     // ---- weights: one TMA box per K-chunk, resident for the CTA's lifetime -------------------------
     if (elect_one()) {
       mbar_arrive_expect_tx(b_full, Cfg::kChunks * Cfg::kBChunkBytes);
       for (int c = 0; c < Cfg::kChunks; ++c) tma_load_2d(sb + c * Cfg::kBChunkBytes, &tm_b, b_full, c * kChunkK, 0);
     }
-  } else if (warp == 4) {
-    // ---- MMA issuer ------------------------------------------------------------------------------------
-    constexpr uint32_t idesc = umma_idesc_tf32(kTileM, NOUT);
-    mbar_wait(b_full, 0);
-    int g = 0, it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      mbar_wait(acc_empty, (it & 1) ^ 1);  // epilogue has drained the accumulator of the previous tile
-      tc_fence_after();
-      for (int c = 0; c < Cfg::kChunks; ++c, ++g) {
-        const int s = g % Cfg::kStages;
-        mbar_wait(&full[s], (g / Cfg::kStages) & 1);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a0 = smem_u32(sa + s * kStageBytes), b0 = smem_u32(sb + c * Cfg::kBChunkBytes);
-#pragma unroll
-          for (int k = 0; k < kChunkK / 8; ++k)
-            umma_tf32(tmem_base, umma_desc_sw128(a0 + k * 32), umma_desc_sw128(b0 + k * 32), idesc, (c | k) != 0);
-          umma_commit(&empty[s]);                       // smem stage may be refilled once these MMAs retire
-          if (c == Cfg::kChunks - 1) umma_commit(acc_full);
-        }
-        __syncwarp();
-      }
-    }
   } else {
-    // ---- warps 0-3: im2col producers, then epilogue ----------------------------------------------------
+    // ---- warps 0-3: im2col producers, wgmma issue (the chunk issued kLag iterations earlier), epilogue --------
+    // A stage is refilled kStages chunks after it was filled; its MMAs completed kStages − kLag iterations before.
+    static_assert(Cfg::kLag < Cfg::kStages, "conv5x5_umma: the lag must be shorter than the ring");
+    const uint64_t bdesc0 = gmma_desc_kmajor<128>(smem_u32(sb));
+    auto mma_chunk = [&](float (&acc)[2][NOUT / 2], int c, int s) {
+      const uint32_t a0 = smem_u32(sa + s * kStageBytes);
+      const uint64_t bd = bdesc0 + static_cast<uint64_t>((c * Cfg::kBChunkBytes) >> 4);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kChunkK / 8; ++k)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          wgmma_tf32<NOUT>(acc[h], gmma_desc_kmajor<128>(a0 + h * 64 * 128 + k * 32), bd + ((k * 32) >> 4), (c | k) != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+    };
+    mbar_wait(b_full, 0);
     const int u = tid & 7;                       // 16-byte column inside the 128-byte K row
     const int tap_in_chunk = (u * 4) / CK;       // which tap of the chunk this column belongs to
     const int c4 = (u * 4) % CK;                 // channel offset inside the tap
@@ -260,9 +237,13 @@ __global__ void __launch_bounds__(192, 1) conv5x5_umma_kernel(const float* __res
           row_w[j] = 0;
         }
       }
+      float acc[2][NOUT / 2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < NOUT / 2; ++e) acc[h][e] = 0.f;
       for (int c = 0; c < Cfg::kChunks; ++c, ++g) {
         const int s = g % Cfg::kStages;
-        mbar_wait(&empty[s], ((g / Cfg::kStages) & 1) ^ 1);
         const int tap = c * Cfg::kTapsPerChunk + tap_in_chunk;
         const int kh = tap / 5 - 2, kw = tap % 5 - 2;
         const int delta = (kh * W + kw) * CK + c4;
@@ -279,30 +260,25 @@ __global__ void __launch_bounds__(192, 1) conv5x5_umma_kernel(const float* __res
         if (c >= Cfg::kLag) {
           cp_async_wait<Cfg::kLag>();            // chunk c-kLag of this thread has landed
           fence_proxy_async_smem();              // generic-proxy writes → visible to the tensor core (async proxy)
-          mbar_arrive(&full[(g - Cfg::kLag) % Cfg::kStages]);
+          asm volatile("bar.sync 1, 128;" ::: "memory");   // ... and that of every producer thread
+          mma_chunk(acc, c - Cfg::kLag, (g - Cfg::kLag) % Cfg::kStages);
         }
       }
-      // drain this tile (its accumulator is needed now): signal the kLag chunks still in flight;
-      // the lag bookkeeping restarts with the next tile
+      // drain this tile (its accumulator is needed now): the kLag chunks still in flight; the lag bookkeeping restarts
+      // with the next tile
       cp_async_wait<0>();
       fence_proxy_async_smem();
+      asm volatile("bar.sync 1, 128;" ::: "memory");
 #pragma unroll
-      for (int q = Cfg::kLag; q >= 1; --q) mbar_arrive(&full[(g - q) % Cfg::kStages]);
+      for (int q = Cfg::kLag; q >= 1; --q) mma_chunk(acc, Cfg::kChunks - q, (g - q) % Cfg::kStages);
       // ---- epilogue ----------------------------------------------------------------------------------
-      mbar_wait(acc_full, it & 1);
-      __syncwarp();
-      tc_fence_after();
+#pragma unroll
+      for (int h = 0; h < 2; ++h) wgmma_frag_store<NOUT>(acc[h], sacc, NOUT + 1, 64 * h, tid);
+      asm volatile("bar.sync 1, 128;" ::: "memory");
       float v[NOUT];
 #pragma unroll
-      for (int c0 = 0; c0 < NOUT; c0 += 16) {
-        float t[16];
-        tmem_ld_32x32b_x16(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + c0, t);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[c0 + j] = t[j];
-      }
-      tc_fence_before();
-      mbar_arrive(acc_empty);
-      const int r = tid;  // 0..127 = tile row = TMEM lane
+      for (int j = 0; j < NOUT; ++j) v[j] = sacc[tid * (NOUT + 1) + j];
+      const int r = tid;  // 0..127 = tile row
       const int p = tile * kTileM + r;
       const bool valid = p < M;
       if (bias) {
@@ -354,19 +330,16 @@ __global__ void __launch_bounds__(192, 1) conv5x5_umma_kernel(const float* __res
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) tmem_dealloc<Cfg::kTmemCols>(tmem_base);
 }
 
 // =====================================================================================================
 // Implicit-GEMM 5x5 convolution, fully TMA-fed: the im2col A-tile of every filter tap is ONE
 // cp.async.bulk.tensor.4d...im2col instruction (hardware walks 128 consecutive output pixels through
 // W→H→N, applies the (kw,kh) tap offset and zero-fills the padding halo), so there are no producer
-// warps at all: warp 0 = TMA, warp 1 = MMA issue, warps 2-5 = epilogue on a double-buffered TMEM
-// accumulator (the epilogue of tile i overlaps the mainloop of tile i+1).
-//   CK = 16 (fwd):  rows of 64 B  → SWIZZLE_64B smem/UMMA layout, 2 MMAs (K=8) per tap
-//   CK = 32 (dgrad): rows of 128 B → SWIZZLE_128B,               4 MMAs per tap
+// warps at all: warp 4 = TMA, warps 0-3 = the warpgroup that issues the wgmma (two M = 64 halves of the
+// 128-pixel tile) and runs the epilogue from its register accumulators.
+//   CK = 16 (fwd):  rows of 64 B  → SWIZZLE_64B smem/wgmma layout, 2 K=8 steps per tap
+//   CK = 32 (dgrad): rows of 128 B → SWIZZLE_128B,                4 K=8 steps per tap
 // Weights: Bm[NOUT][25·CK] (K index = tap·CK + c), one TMA box per tap, resident in smem.
 // =====================================================================================================
 __device__ __forceinline__ void tma_load_im2col_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c, int w, int h, int n,
@@ -383,20 +356,20 @@ struct ConvTmaCfg {
   static constexpr int kRowB = CK * 4;                       // bytes per pixel per tap
   static constexpr int kATapBytes = kTileM * kRowB;          // 8 KB / 16 KB
   // One pipeline stage = one filter ROW (5 taps, 5 TMA loads on one mbarrier): the per-stage
-  // handshake (TMA issue → full → MMA wake-up → commit → empty) costs ~0.25 µs whatever the payload,
-  // and 25 one-tap stages per tile made the mainloop handshake-bound (profiles/op_bench.md).
+  // handshake (TMA issue → full → MMA → empty) costs the same whatever the payload, so a stage
+  // carries five taps rather than one.
   static constexpr int kTapsPerStage = 5;
   static constexpr int kAStageBytes = kTapsPerStage * kATapBytes;   // 40 KB / 80 KB
   static constexpr int kStages = CK == 16 ? 3 : 2;
   static constexpr int kBTapBytes = NOUT * kRowB;            // 2 KB
   static constexpr int kSyBytes = CK == 16 ? kTileM * 128 : 0;  // output staging only for the TMA-stored forward
-  static constexpr int kTmemCols = 64;                       // two 32-column accumulators
-  static constexpr int kThreads = 192;
-  static constexpr size_t kSmem = 2048 + kStages * kAStageBytes + 25 * kBTapBytes + kSyBytes + 2048;
+  static constexpr int kAccBytes = kTileM * (NOUT + 1) * 4;  // accumulator rows, one per epilogue thread
+  static constexpr int kThreads = 160;
+  static constexpr size_t kSmem = 2048 + kStages * kAStageBytes + 25 * kBTapBytes + kSyBytes + kAccBytes + 2048;
 };
 
 template <int CK, int NOUT, bool FWD>
-__global__ void __launch_bounds__(192, 1) conv5x5_umma_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_b,
+__global__ void __launch_bounds__(160, 1) conv5x5_umma_tma_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_b,
                                                                   const __grid_constant__ CUtensorMap tm_y, const float* __restrict__ bias,
                                                                   float* __restrict__ y, float* stats, ReduceScratch scr, int B, int H, int W,
                                                                   int num_tiles) {
@@ -407,14 +380,12 @@ __global__ void __launch_bounds__(192, 1) conv5x5_umma_tma_kernel(const __grid_c
   uint8_t* sb = sa + Cfg::kStages * Cfg::kAStageBytes;
   uint8_t* sy = sb + 25 * Cfg::kBTapBytes;
   sy = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(sy) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sy + Cfg::kSyBytes);
+  float* sacc = reinterpret_cast<float*>(sy + Cfg::kSyBytes);   // [128][NOUT + 1]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sacc + kTileM * (NOUT + 1));
   uint64_t* full = bars;
   uint64_t* empty = full + Cfg::kStages;
   uint64_t* b_full = empty + Cfg::kStages;
-  uint64_t* acc_full = b_full + 1;      // [2]
-  uint64_t* acc_empty = acc_full + 2;   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* s_part = reinterpret_cast<float*>(tmem_slot + 2);   // [4][2*NOUT] + [2*NOUT]
+  float* s_part = reinterpret_cast<float*>(b_full + 2);   // [4][2*NOUT] + [2*NOUT]
   __shared__ int s_last;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -423,18 +394,13 @@ __global__ void __launch_bounds__(192, 1) conv5x5_umma_tma_kernel(const __grid_c
     tma_prefetch_desc(&tm_x);
     tma_prefetch_desc(&tm_b);
     if (FWD) tma_prefetch_desc(&tm_y);
-    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 128); }
     mbar_init(b_full, 1);
-    for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 128); }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (elect_one()) {
       mbar_arrive_expect_tx(b_full, 25 * Cfg::kBTapBytes);
       for (int t = 0; t < 25; ++t) tma_load_2d(sb + t * Cfg::kBTapBytes, &tm_b, b_full, t * CK, 0);
@@ -454,53 +420,41 @@ __global__ void __launch_bounds__(192, 1) conv5x5_umma_tma_kernel(const __grid_c
         }
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = umma_idesc_tf32(kTileM, NOUT);
+  } else {
+    // ---- warps 0..3: wgmma issue + epilogue, thread = tile row -----------------------------------------------
+    const int et = tid, r = tid;
     mbar_wait(b_full, 0);
-    int g = 0, it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
-      mbar_wait(&acc_empty[as], ((it >> 1) & 1) ^ 1);
-      tc_fence_after();
+    int g = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      float acc[2][NOUT / 2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < NOUT / 2; ++e) acc[h][e] = 0.f;
       for (int kh = 0; kh < 5; ++kh, ++g) {
         const int s = g % Cfg::kStages;
         mbar_wait(&full[s], (g / Cfg::kStages) & 1);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a0 = smem_u32(sa + s * Cfg::kAStageBytes), b0 = smem_u32(sb + kh * 5 * Cfg::kBTapBytes);
+        const uint32_t a0 = smem_u32(sa + s * Cfg::kAStageBytes), b0 = smem_u32(sb + kh * 5 * Cfg::kBTapBytes);
+        wgmma_fence();
 #pragma unroll
-          for (int kw = 0; kw < 5; ++kw)
+        for (int kw = 0; kw < 5; ++kw)
 #pragma unroll
-            for (int k = 0; k < CK / 8; ++k)
-              umma_tf32(tmem_base + as * 32, umma_desc_kmajor<Cfg::kRowB>(a0 + kw * Cfg::kATapBytes + k * 32),
-                        umma_desc_kmajor<Cfg::kRowB>(b0 + kw * Cfg::kBTapBytes + k * 32), idesc, (kh | kw | k) != 0);
-          umma_commit(&empty[s]);
-          if (kh == 4) umma_commit(&acc_full[as]);
-        }
-        __syncwarp();
+          for (int k = 0; k < CK / 8; ++k)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              wgmma_tf32<NOUT>(acc[h], gmma_desc_kmajor<Cfg::kRowB>(a0 + kw * Cfg::kATapBytes + h * 64 * Cfg::kRowB + k * 32),
+                               gmma_desc_kmajor<Cfg::kRowB>(b0 + kw * Cfg::kBTapBytes + k * 32), (kh | kw | k) != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        mbar_arrive(&empty[s]);                 // this thread's share of the stage has been read
       }
-    }
-  } else {
-    // ---- epilogue warps 2..5: TMEM lane quadrant = warp % 4 ----------------------------------------------
-    const int et = tid - 64;                  // 0..127
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;           // tile row = TMEM lane
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
-      mbar_wait(&acc_full[as], (it >> 1) & 1);
-      __syncwarp();
-      tc_fence_after();
+      asm volatile("bar.sync 1, 128;" ::: "memory");   // the previous tile's rows have been read out of sacc
+#pragma unroll
+      for (int h = 0; h < 2; ++h) wgmma_frag_store<NOUT>(acc[h], sacc, NOUT + 1, 64 * h, tid);
+      asm volatile("bar.sync 1, 128;" ::: "memory");
       float v[NOUT];
 #pragma unroll
-      for (int c0 = 0; c0 < NOUT; c0 += 16) {
-        float t16[16];
-        tmem_ld_32x32b_x16(tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + as * 32 + c0, t16);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[c0 + j] = t16[j];
-      }
-      tc_fence_before();
-      mbar_arrive(&acc_empty[as]);            // the MMA warp may start the tile after next in this accumulator
+      for (int j = 0; j < NOUT; ++j) v[j] = sacc[r * (NOUT + 1) + j];
       const int p = tile * kTileM + r;
       const bool valid = p < M;
       if (bias) {
@@ -550,23 +504,19 @@ __global__ void __launch_bounds__(192, 1) conv5x5_umma_tma_kernel(const __grid_c
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<Cfg::kTmemCols>(tmem_base);
 }
 
 // =====================================================================================================
-// EXPERIMENTAL (not validated on hardware yet, not reachable unless impl == "win" is requested):
+// EXPERIMENTAL (not covered by the test suite, not reachable unless impl == "win" is requested):
 // "window" implicit-GEMM 5x5 convolution — every input pixel is loaded ONCE.
 //
-// ncu showed the im2col kernels above bound by the TMA gather's row rate (128 pixels × 25 taps = 3,200
-// rows per tile at ≈3.8 cycles/row, profiles/conv_tma_ncu.md).  Here a tile is R output rows of one image
+// The im2col kernels above gather 128 pixels × 25 taps = 3,200 rows per tile through TMA.  Here a tile is R output rows of one image
 // in *padded-width* coordinates (PW = W + 4 positions per row, M = R·PW ≤ 128 MMA rows of which R·W are real
 // outputs): ONE tiled TMA box {32 ch, PW, R + 4 rows} brings the zero-haloed patch (hardware OOB fill
 // provides the halo and, for C = 16, the upper half of the 128-byte row), and tap (kh, kw) is the same
-// buffer read through a K-major SWIZZLE_128B descriptor that starts (kh·PW + kw) rows in — the base-offset
-// field carries the swizzle phase of that start row.  Index math proven on the CPU by
-// tools/emulate_window_conv.py; descriptor addressing to be confirmed by tools/exp_rowshift.py.
+// buffer read through a K-major SWIZZLE_128B descriptor that starts (kh·PW + kw) rows in (base offset 0: the swizzle
+// phase follows the absolute address, tools/exp_rowshift.py).  Index math checked on the CPU by
+// tools/emulate_window_conv.py.
 // Weights: Bm[NOUT][25·32] (K index = tap·32 + c, zero padded for C = 16), resident in smem.
 // =====================================================================================================
 
@@ -575,16 +525,16 @@ struct ConvWinCfg {
   static constexpr int kRowB = 128;                          // bytes per padded position (32 floats, upper half zero for C=16)
   static constexpr int kPatchRowsMax = 256;                  // PW·(R+4) positions per tile, box limit
   static constexpr int kAStageBytes = kPatchRowsMax * kRowB + 1024;   // + slack: the last taps of padding rows read past the box
-  static constexpr int kStages = 3;
+  static constexpr int kStages = 2;
   static constexpr int kBTapBytes = NOUT * kRowB;            // 4 KB / 2 KB
   static constexpr int kSyBytes = kTileM * 128;              // row staging for the BN statistics
-  static constexpr int kTmemCols = 64;
-  static constexpr int kThreads = 192;
-  static constexpr size_t kSmem = 2048 + kStages * kAStageBytes + 25 * kBTapBytes + kSyBytes + 2048;
+  static constexpr int kAccBytes = kTileM * (NOUT + 1) * 4;  // accumulator rows, one per epilogue thread
+  static constexpr int kThreads = 160;
+  static constexpr size_t kSmem = 2048 + kStages * kAStageBytes + 25 * kBTapBytes + kSyBytes + kAccBytes + 2048;
 };
 
 template <int CK, int NOUT, bool FWD>
-__global__ void __launch_bounds__(192, 1) conv5x5_umma_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_b,
+__global__ void __launch_bounds__(160, 1) conv5x5_umma_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_b,
                                                                   const float* __restrict__ bias, float* __restrict__ y, float* stats,
                                                                   ReduceScratch scr, int B, int H, int W, int R, int num_tiles, int bo_mode) {
   using Cfg = ConvWinCfg<NOUT>;
@@ -593,14 +543,12 @@ __global__ void __launch_bounds__(192, 1) conv5x5_umma_win_kernel(const __grid_c
   uint8_t* sa = smem;                                        // stages start 1024-aligned (kAStageBytes % 1024 == 0)
   uint8_t* sb = sa + Cfg::kStages * Cfg::kAStageBytes;
   uint8_t* sy = sb + 25 * Cfg::kBTapBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sy + Cfg::kSyBytes);
+  float* sacc = reinterpret_cast<float*>(sy + Cfg::kSyBytes);   // [128][NOUT + 1]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sacc + kTileM * (NOUT + 1));
   uint64_t* full = bars;
   uint64_t* empty = full + Cfg::kStages;
   uint64_t* b_full = empty + Cfg::kStages;
-  uint64_t* acc_full = b_full + 1;      // [2]
-  uint64_t* acc_empty = acc_full + 2;   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* s_part = reinterpret_cast<float*>(tmem_slot + 2);   // [4][2*NOUT] + [2*NOUT]
+  float* s_part = reinterpret_cast<float*>(b_full + 2);   // [4][2*NOUT] + [2*NOUT]
   __shared__ int s_last;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -609,18 +557,13 @@ __global__ void __launch_bounds__(192, 1) conv5x5_umma_win_kernel(const __grid_c
   if (tid == 0) {
     tma_prefetch_desc(&tm_x);
     tma_prefetch_desc(&tm_b);
-    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 128); }
     mbar_init(b_full, 1);
-    for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 128); }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warpgroup_index() == 1) {
     if (elect_one()) {
       mbar_arrive_expect_tx(b_full, 25 * Cfg::kBTapBytes);
       for (int t = 0; t < 25; ++t) tma_load_2d(sb + t * Cfg::kBTapBytes, &tm_b, b_full, t * 32, 0);
@@ -634,60 +577,50 @@ __global__ void __launch_bounds__(192, 1) conv5x5_umma_win_kernel(const __grid_c
         tma_load_4d(sa + s * Cfg::kAStageBytes, &tm_x, &full[s], 0, -2, oh0 - 2, n);   // halo and channel pad: OOB zero fill
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = umma_idesc_tf32(kTileM, NOUT);
+  } else {
+    // ---- warps 0..3: wgmma issue + epilogue; thread = padded position of the tile --------------------------------
+    const int et = tid, r = tid;
+    const int rr = r / PW, owp = r - rr * PW;
+    const bool real = r < Mrows && owp < W;   // 4 of every PW positions (and rows ≥ R·PW) are padding
     mbar_wait(b_full, 0);
     int it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1, s = it % Cfg::kStages;
-      mbar_wait(&acc_empty[as], ((it >> 1) & 1) ^ 1);
+      const int s = it % Cfg::kStages;
+      const int n = tile / tiles_per_img, oh0 = (tile % tiles_per_img) * R;
       mbar_wait(&full[s], (it / Cfg::kStages) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t a0 = smem_u32(sa + s * Cfg::kAStageBytes), b0 = smem_u32(sb);
-        for (int kh = 0; kh < 5; ++kh) {
+      float acc[2][NOUT / 2];
 #pragma unroll
-          for (int kw = 0; kw < 5; ++kw) {
-            const uint32_t arow = a0 + static_cast<uint32_t>(kh * PW + kw) * Cfg::kRowB;
+      for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int k = 0; k < CK / 8; ++k) {   // C = 16: the zero upper half of the row is simply not multiplied
-              const uint32_t astart = arow + k * 32;
-              uint64_t ad = umma_desc_kmajor<128>(astart);
+        for (int e = 0; e < NOUT / 2; ++e) acc[h][e] = 0.f;
+      const uint32_t a0 = smem_u32(sa + s * Cfg::kAStageBytes), b0 = smem_u32(sb);
+      wgmma_fence();
+      for (int kh = 0; kh < 5; ++kh) {
+#pragma unroll
+        for (int kw = 0; kw < 5; ++kw) {
+          const uint32_t arow = a0 + static_cast<uint32_t>(kh * PW + kw) * Cfg::kRowB;
+#pragma unroll
+          for (int k = 0; k < CK / 8; ++k) {   // C = 16: the zero upper half of the row is simply not multiplied
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const uint32_t astart = arow + h * 64 * Cfg::kRowB + k * 32;
+              uint64_t ad = gmma_desc_kmajor<128>(astart);
               if (bo_mode) ad |= static_cast<uint64_t>((astart >> 7) & 7) << 49;
-              umma_tf32(tmem_base + as * 32, ad, umma_desc_kmajor<128>(b0 + (kh * 5 + kw) * Cfg::kBTapBytes + k * 32), idesc,
-                        (kh | kw | k) != 0);
+              wgmma_tf32<NOUT>(acc[h], ad, gmma_desc_kmajor<128>(b0 + (kh * 5 + kw) * Cfg::kBTapBytes + k * 32), (kh | kw | k) != 0);
             }
           }
         }
-        umma_commit(&empty[s]);
-        umma_commit(&acc_full[as]);
       }
-      __syncwarp();
-    }
-  } else {
-    // ---- epilogue warps 2..5: TMEM lane quadrant = warp % 4; lane = padded position of the tile -------------
-    const int et = tid - 64;                  // 0..127
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;           // tile row = TMEM lane = padded position
-    const int rr = r / PW, owp = r - rr * PW;
-    const bool real = r < Mrows && owp < W;   // 4 of every PW positions (and rows ≥ R·PW) are padding
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
-      const int n = tile / tiles_per_img, oh0 = (tile % tiles_per_img) * R;
-      mbar_wait(&acc_full[as], (it >> 1) & 1);
-      __syncwarp();
-      tc_fence_after();
+      wgmma_commit();
+      wgmma_wait<0>();
+      mbar_arrive(&empty[s]);
+      asm volatile("bar.sync 1, 128;" ::: "memory");   // the previous tile's rows have been read out of sacc
+#pragma unroll
+      for (int h = 0; h < 2; ++h) wgmma_frag_store<NOUT>(acc[h], sacc, NOUT + 1, 64 * h, tid);
+      asm volatile("bar.sync 1, 128;" ::: "memory");
       float v[NOUT];
 #pragma unroll
-      for (int c0 = 0; c0 < NOUT; c0 += 16) {
-        float t16[16];
-        tmem_ld_32x32b_x16(tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + as * 32 + c0, t16);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[c0 + j] = t16[j];
-      }
-      tc_fence_before();
-      mbar_arrive(&acc_empty[as]);
+      for (int j = 0; j < NOUT; ++j) v[j] = sacc[r * (NOUT + 1) + j];
       if (bias) {
 #pragma unroll
         for (int j = 0; j < NOUT; ++j) v[j] += bias[j];
@@ -728,9 +661,6 @@ __global__ void __launch_bounds__(192, 1) conv5x5_umma_win_kernel(const __grid_c
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<Cfg::kTmemCols>(tmem_base);
 }
 
 // Bm[NOUT][25·32]: K index = tap·32 + c, channels ≥ CK zero (window kernel: 128-byte rows for every C)
@@ -757,17 +687,15 @@ __global__ void repack_weights_dense_kernel(const float* __restrict__ w, float* 
 }
 
 // =====================================================================================================
-// conv2 weight gradient on tcgen05:   dWᵀ[m = tap·16+ci][co] = Σ_pixels xcol[p][m] · dy[p][co]
+// conv2 weight gradient on the tensor cores:   dWᵀ[m = tap·16+ci][co] = Σ_pixels xcol[p][m] · dy[p][co]
 //
-// The reduction runs over output pixels, i.e. over the *slow* dimension of both operands, so both
-// are fed to the tensor core MN-major (the 128-byte swizzle atom is 8 pixels × 32 contiguous
-// M/N values):
-//   A = im2col(x)   [128 pixels][128 of the 416 im2col columns]  gathered by cp.async (zero fill)
-//   B = dy tile     [128 pixels][32 channels]                    one TMA box per tile
-// M = 416 is covered by four 128-row accumulators living in TMEM for the CTA's whole lifetime
+// The reduction runs over output pixels, i.e. over the *slow* dimension of both operands (MN-major):
+//   A = im2col(x)   [64 pixels][128 of the 416 im2col columns]   gathered by cp.async (zero fill), 16-byte units XOR-swizzled
+//   B = dy tile     [128 pixels][32 channels]                    one TMA box per tile, SWIZZLE_128B
+// M = 416 is covered by four 128-row accumulators living in registers for the CTA's whole lifetime
 // (persistent split-K over pixel tiles); column 400 of the im2col is a column of ones, so the
 // bias gradient Σ_p dy[p][co] falls out of the same MMAs.  Each CTA deposits one partial
-// [416][32]; wgrad_fold_kernel sums the ≤148 partials in CTA order (deterministic) and scatters
+// [416][32]; wgrad_fold_kernel sums the ≤ #SM partials in CTA order (deterministic) and scatters
 // into torch's [co][ci][5][5] layout.
 // =====================================================================================================
 struct WgradCfg {
@@ -775,22 +703,16 @@ struct WgradCfg {
   static constexpr int kMTiles = 4;
   static constexpr int kHalfPix = 64;                 // pixels per A stage
   static constexpr int kStages = 4, kLag = 1;
-  static constexpr int kAStageBytes = 4 * 8 * 1024;   // [4 MN atoms][8 K blocks][8 rows][128 B]
+  static constexpr int kAStageBytes = kHalfPix * 512; // [64 pixels][128 im2col columns], 16-byte units XOR-swizzled
   static constexpr int kBStages = 2, kBStageBytes = kTileM * 128;
-  static constexpr int kTmemCols = 128;
-  static constexpr int kThreads = 192;
+  static constexpr int kThreads = 160;
   static constexpr size_t kSmem = 1024 + kStages * kAStageBytes + kBStages * kBStageBytes + 1024;
 };
 
-// MN-major descriptor for 32-bit (TF32) operands.  The only legal MN-major layout for TF32 is
-// SWIZZLE_128B_BASE32B (layout type 1): rows of 128 B = 32 consecutive M/N values, K atoms of FOUR
-// rows, and the XOR swizzle acts on 32-byte chunks (chunk32 ^= row % 4) — its TMA counterpart is
-// CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B.  LBO = byte stride between 32-element MN atoms, SBO = byte
-// stride between 4-row K atoms (512 B when the 8 rows of one MMA are contiguous).
-// [cf. UMMA::Layout_MN_SW128_32B_Atom and make_umma_desc<Major::MN>, cute/atom/mma_traits_sm100.hpp]
-// umma_desc_mn_sw128_32b: umma_ptx.cuh
-
-__global__ void __launch_bounds__(192, 1) conv5x5_wgrad_umma_kernel(const float* __restrict__ x, const __grid_constant__ CUtensorMap tm_dy,
+// Both GEMM operands have the pixels (the reduction dimension) outermost — MN-major — which TF32 wgmma does not
+// accept, so the four producer warps also run the MMAs, warp-level mma.sync m16n8k8 (wgrad_win.cuh): warp w owns
+// rows 32w .. 32w+31 of every 128-row M tile, and all four M tiles stay in registers across the CTA's pixel tiles.
+__global__ void __launch_bounds__(160, 1) conv5x5_wgrad_umma_kernel(const float* __restrict__ x, const __grid_constant__ CUtensorMap tm_dy,
                                                                     const float* __restrict__ ones, float* __restrict__ partials, int B,
                                                                     int H, int W, int num_tiles) {
   using Cfg = WgradCfg;
@@ -799,29 +721,19 @@ __global__ void __launch_bounds__(192, 1) conv5x5_wgrad_umma_kernel(const float*
   uint8_t* sa = smem;
   uint8_t* sb = sa + Cfg::kStages * Cfg::kAStageBytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sb + Cfg::kBStages * Cfg::kBStageBytes);
-  uint64_t* afull = bars;
-  uint64_t* aempty = afull + Cfg::kStages;
-  uint64_t* bfull = aempty + Cfg::kStages;
+  uint64_t* bfull = bars;
   uint64_t* bempty = bfull + Cfg::kBStages;
-  uint64_t* acc_full = bempty + Cfg::kBStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int M = B * H * W;
   if (tid == 0) {
     tma_prefetch_desc(&tm_dy);
-    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&afull[s], 128); mbar_init(&aempty[s], 1); }
-    for (int s = 0; s < Cfg::kBStages; ++s) { mbar_init(&bfull[s], 1); mbar_init(&bempty[s], 1); }
-    mbar_init(acc_full, 1);
+    for (int s = 0; s < Cfg::kBStages; ++s) { mbar_init(&bfull[s], 1); mbar_init(&bempty[s], 128); }
     fence_mbar_init();
   }
-  if (warp == 4) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 5) {
+  if (warp == 4) {
     if (elect_one()) {
       int it = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
@@ -831,118 +743,91 @@ __global__ void __launch_bounds__(192, 1) conv5x5_wgrad_umma_kernel(const float*
         tma_load_2d(sb + s * Cfg::kBStageBytes, &tm_dy, &bfull[s], 0, tile * kTileM);   // rows ≥ M arrive as zeros
       }
     }
-  } else if (warp == 4) {
-    constexpr uint32_t idesc = umma_idesc_tf32(kTileM, 32) | (1u << 15) | (1u << 16);  // A and B are MN-major
-    int g = 0, it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int bs = it % Cfg::kBStages;
-      mbar_wait(&bfull[bs], (it / Cfg::kBStages) & 1);
-      for (int mt = 0; mt < Cfg::kMTiles; ++mt) {
-        for (int h = 0; h < 2; ++h, ++g) {
-          const int s = g % Cfg::kStages;
-          mbar_wait(&afull[s], (g / Cfg::kStages) & 1);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t a0 = smem_u32(sa + s * Cfg::kAStageBytes), b0 = smem_u32(sb + bs * Cfg::kBStageBytes) + h * 8 * 1024;
+    return;
+  }
+  // ---- warps 0-3: im2col gather (64 pixels × 128 columns per stage), then the MMAs of the stage kLag behind --------
+  float acc[Cfg::kMTiles][2][4][4];
 #pragma unroll
-            for (int kb = 0; kb < 8; ++kb)
-              umma_tf32(tmem_base + mt * 32, umma_desc_mn_sw128_32b(a0 + kb * 1024, 8 * 1024, 512),
-                        umma_desc_mn_sw128_32b(b0 + kb * 1024, 1024, 512), idesc, (it | h | kb) != 0);
-            umma_commit(&aempty[s]);
-            if (mt == Cfg::kMTiles - 1 && h == 1) umma_commit(&bempty[bs]);
-          }
-          __syncwarp();
-        }
-      }
-    }
-    if (elect_one()) umma_commit(acc_full);
-    __syncwarp();
-  } else {
-    // ---- producers: im2col gather, 64 pixels × 128 columns per stage -------------------------------------
-    const int u = tid & 31;                 // 16-byte unit inside the 128-column row: tap_local = u/4, channels 4(u%4)..
-    const int tap_local = u >> 2, c4 = (u & 3) * 4;
-    const uint32_t unit_off = static_cast<uint32_t>(tap_local >> 1) * 8192u;
-    const int chunk = ((tap_local & 1) << 2) | (c4 >> 2);
-    int g = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      for (int mt = 0; mt < Cfg::kMTiles; ++mt) {
-        const int tap = mt * 8 + tap_local;
-        const int kh = tap / 5 - 2, kw = tap % 5 - 2;
-        for (int h = 0; h < 2; ++h, ++g) {
-          const int s = g % Cfg::kStages;
-          mbar_wait(&aempty[s], ((g / Cfg::kStages) & 1) ^ 1);
-          // rows r = t4 + 4j (t4 = tid/32): r/8 = j/2, r%8 = 4(j%2)+t4, r%4 = t4 ⇒ the swizzle term is a
-          // per-thread constant.  128B_BASE32B: the 32-byte chunk index (chunk >> 1) is XORed with (row % 4).
-          const int t4 = tid >> 5;
-          const uint32_t dst0 = smem_u32(sa + s * Cfg::kAStageBytes) + unit_off + t4 * 128 + (((((chunk >> 1) ^ t4) << 1) | (chunk & 1)) << 4);
-          int p = tile * kTileM + h * Cfg::kHalfPix + t4;
-          int ow = p % W, oh = (p / W) % H;               // NHWC: pixel p lives at x + 16 p, so only bounds need (oh, ow)
-          const int tap_delta = (kh * W + kw) * 16 + c4;
+  for (int mt = 0; mt < Cfg::kMTiles; ++mt)
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) acc[mt][j][nt][e] = 0.f;
+  // stage q (the q-th of the CTA) holds M tile (q / 2) % 4, pixel half q % 2 of the CTA's tile q / 8
+  auto mma_stage = [&](int q) {
+    const int mt = (q >> 1) & 3, h = q & 1, it = q >> 3, bs = it % Cfg::kBStages;
+    mbar_wait(&bfull[bs], (it / Cfg::kBStages) & 1);
+    const float* xs = reinterpret_cast<const float*>(sa + (q % Cfg::kStages) * Cfg::kAStageBytes);
+    const float* dys = reinterpret_cast<const float*>(sb + bs * Cfg::kBStageBytes);
+#pragma unroll
+    for (int m = 0; m < Cfg::kMTiles; ++m)
+      if (m == mt) wgrad_win_atom<Cfg::kHalfPix, 128>(acc[m], xs, 0, warp * 32, dys, h * Cfg::kHalfPix, lane);
+    if (mt == Cfg::kMTiles - 1 && h == 1) mbar_arrive(&bempty[bs]);   // the last stage of this pixel tile has read dy
+  };
+  const int u = tid & 31;                 // 16-byte unit inside the 128-column row: tap_local = u/4, channels 4(u%4)..
+  const int tap_local = u >> 2, c4 = (u & 3) * 4;
+  const int t4 = tid >> 5;                // this thread fills pixel rows t4 + 4j of a stage
+  int g = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    for (int mt = 0; mt < Cfg::kMTiles; ++mt) {
+      const int tap = mt * 8 + tap_local;
+      const int kh = tap / 5 - 2, kw = tap % 5 - 2;
+      for (int h = 0; h < 2; ++h, ++g) {
+        const int s = g % Cfg::kStages;
+        const uint32_t dst0 = smem_u32(sa + s * Cfg::kAStageBytes) + t4 * 512;   // row t4 + 4j, unit u stored at u ^ (row % 8)
+        int p = tile * kTileM + h * Cfg::kHalfPix + t4;
+        int ow = p % W, oh = (p / W) % H;               // NHWC: pixel p lives at x + 16 p, so only bounds need (oh, ow)
+        const int tap_delta = (kh * W + kw) * 16 + c4;
 #pragma unroll 4
-          for (int j = 0; j < 16; ++j) {
-            const float* src = x;
-            uint32_t bytes = 0;
-            if (p < M) {
-              if (tap < 25) {
-                const int ih = oh + kh, iw = ow + kw;
-                if (ih >= 0 && ih < H && iw >= 0 && iw < W) {
-                  src = x + static_cast<size_t>(p) * 16 + tap_delta;
-                  bytes = 16;
-                }
-              } else if (tap == 25 && c4 == 0) {
-                src = ones;  // {1,0,0,0}: im2col column 400 ≡ 1 → row 400 of dWᵀ is the bias gradient
+        for (int j = 0; j < 16; ++j) {
+          const float* src = x;
+          uint32_t bytes = 0;
+          if (p < M) {
+            if (tap < 25) {
+              const int ih = oh + kh, iw = ow + kw;
+              if (ih >= 0 && ih < H && iw >= 0 && iw < W) {
+                src = x + static_cast<size_t>(p) * 16 + tap_delta;
                 bytes = 16;
               }
+            } else if (tap == 25 && c4 == 0) {
+              src = ones;  // {1,0,0,0}: im2col column 400 ≡ 1 → row 400 of dWᵀ is the bias gradient
+              bytes = 16;
             }
-            cp_async_16(dst0 + (j >> 1) * 1024 + (j & 1) * 512, src, bytes);
-            p += 4;
-            ow += 4;
-            if (ow >= W) { ow -= W; oh = (oh + 1 == H) ? 0 : oh + 1; }
           }
-          cp_async_commit();
-          if (g >= Cfg::kLag) {
-            cp_async_wait<Cfg::kLag>();
-            fence_proxy_async_smem();
-            mbar_arrive(&afull[(g - Cfg::kLag) % Cfg::kStages]);
-          }
+          cp_async_16(dst0 + j * 2048 + ((u ^ (t4 | ((j & 1) << 2))) << 4), src, bytes);
+          p += 4;
+          ow += 4;
+          if (ow >= W) { ow -= W; oh = (oh + 1 == H) ? 0 : oh + 1; }
         }
-      }
-    }
-    cp_async_wait<0>();
-    fence_proxy_async_smem();
-#pragma unroll
-    for (int q = Cfg::kLag; q >= 1; --q) mbar_arrive(&afull[(g - q) % Cfg::kStages]);
-    // ---- epilogue: four accumulators → this CTA's partial [416][32] --------------------------------------
-    mbar_wait(acc_full, 0);
-    __syncwarp();
-    tc_fence_after();
-    for (int mt = 0; mt < Cfg::kMTiles; ++mt) {
-      const int m = mt * kTileM + tid;
-      float v[32];
-#pragma unroll
-      for (int c0 = 0; c0 < 32; c0 += 16) {
-        float t[16];
-        tmem_ld_32x32b_x16(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + mt * 32 + c0, t);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[c0 + j] = t[j];
-      }
-      if (m < Cfg::kMUsed) {
-        float* o = partials + (static_cast<size_t>(blockIdx.x) * Cfg::kMUsed + m) * 32;
-#pragma unroll
-        for (int q = 0; q < 8; ++q) *reinterpret_cast<float4*>(o + 4 * q) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+        cp_async_commit();
+        if (g >= Cfg::kLag) {
+          cp_async_wait<Cfg::kLag>();
+          asm volatile("bar.sync 1, 128;" ::: "memory");   // stage g - kLag has landed for every producer thread
+          mma_stage(g - Cfg::kLag);
+        }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) tmem_dealloc<Cfg::kTmemCols>(tmem_base);
+  cp_async_wait<0>();
+  asm volatile("bar.sync 1, 128;" ::: "memory");
+#pragma unroll
+  for (int q = Cfg::kLag; q >= 1; --q)
+    if (g - q >= 0) mma_stage(g - q);
+  // ---- this CTA's partial [416][32] ------------------------------------------------------------------------------
+#pragma unroll
+  for (int mt = 0; mt < Cfg::kMTiles; ++mt) {
+    const int m0 = mt * kTileM + warp * 32;
+    if (m0 < Cfg::kMUsed) wgrad_win_atom_store(acc[mt], partials + (static_cast<size_t>(blockIdx.x) * Cfg::kMUsed + m0) * 32, lane, Cfg::kMUsed - m0);
+  }
 }
 
 // dw[co][ci][tap] = Σ_cta partial[cta][tap*16+ci][co];  db[co] = Σ_cta partial[cta][400][co]
 __global__ void __launch_bounds__(256) wgrad_fold_kernel(const float* __restrict__ partials, int nparts, float* __restrict__ dw,
                                                          float* __restrict__ db) {
   // one CTA per im2col row m (401 of them): lane = output channel, the 8 warps stride over the
-  // per-CTA partials (≤ 148/8 = 19 loads each, two in flight), sub-sums folded in warp order
+  // per-CTA partials (≤ 132/8 = 17 loads each on an H100, two in flight), sub-sums folded in warp order
   __shared__ float s_sub[8][32];
   const int m = blockIdx.x, co = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const float* p = partials + static_cast<size_t>(m) * 32 + co;
@@ -969,137 +854,80 @@ __global__ void __launch_bounds__(256) wgrad_fold_kernel(const float* __restrict
 // conv2 weight gradient, fully TMA-fed ("window" formulation; used by the cooperative fused layers, whose activations
 // live in zero-haloed 18×18 frames):   dWᵀ[(kh, kw, ci)][co] = Σ_P  xpad[P + (kh−2)·18 + (kw−2)][ci] · dypad[P][co]
 // over the padded positions P of every image (dypad is zero outside the 14×14 interior, so the halo and the frame
-// padding contribute nothing).  Both operands are MN-major as in the kernel above, but the im2col gather is gone:
-// two horizontally adjacent taps of one pixel are 32 *contiguous* floats of the NHWC frame, so an A atom
-// [64 positions][2 taps × 16 ch] is ONE 2-D TMA box over an overlapping-row view of xpad (row pitch 64 B, row length
-// 128 B).  15 tap pairs (kh, {0-1, 2-3, 4-5}) → M = 480 (pair (kh,4-5) carries a dummy sixth column), four 128-row
-// TMEM accumulators; K = 256 positions per image in two 128-row tiles starting at the first interior position.
-// One CTA per image; per-CTA partial [512][32]; the bias gradient comes from per-image Σdy rows (layer-2 backward).
+// padding contribute nothing).  Two horizontally adjacent taps of one pixel are 32 *contiguous* floats of the NHWC
+// frame, so the 32-row M atom of tap pair (kh, kw/2) is a row of an overlapping-row view of xpad (row pitch 64 B, row
+// length 128 B) read (kh−2)·18 + (kw−2) rows from the position: each image's view (384 rows) and its 256 dy positions
+// from the first interior one arrive as eight TMA boxes, and the 15 tap pairs (q = 3·kh + kw/2; pair (kh, 4-5) carries
+// a dummy sixth column) are computed by four warps with mma.sync (wgrad_win.cuh), accumulated over the CTA's images in
+// registers.  One CTA per image at most; per-CTA partial [512][32] (rows q·32 + (kw&1)·16 + ci); the bias gradient
+// comes from per-image Σdy rows (layer-2 backward).
 // =====================================================================================================
 struct WgradWinCfg {
   static constexpr int kFrame = 18 * 18;              // padded positions per image
   static constexpr int kFirst = 2 * 18 + 2;           // first interior position
   static constexpr int kMRows = 512;
-  static constexpr int kStages = 5;
-  static constexpr int kAStageBytes = 4 * 8 * 1024;   // [4 pairs][64 positions][128 B]
-  static constexpr int kBStages = 2, kBStageBytes = kTileM * 128;
-  static constexpr int kTmemCols = 128;
-  static constexpr int kThreads = 192;
-  static constexpr size_t kSmem = 1024 + kStages * kAStageBytes + kBStages * kBStageBytes + 1024;
+  static constexpr int kABoxes = 6, kABytes = kABoxes * 64 * 128;   // overlapping-row view of one image, 64-row boxes
+  static constexpr int kBBytes = 2 * kTileM * 128;                   // dy at 256 positions
+  static constexpr int kThreads = 128;
+  static constexpr size_t kSmem = 1024 + kABytes + kBBytes + 1024;
 };
 
-__global__ void __launch_bounds__(192, 1) conv5x5_wgrad_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_dy,
+__global__ void __launch_bounds__(128, 1) conv5x5_wgrad_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_dy,
                                                                    float* __restrict__ partials, int B, const float* __restrict__ dysum,
                                                                    float* __restrict__ dw, float* __restrict__ db, GridSync gs) {
   using Cfg = WgradWinCfg;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sa = smem;
-  uint8_t* sb = sa + Cfg::kStages * Cfg::kAStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sb + Cfg::kBStages * Cfg::kBStageBytes);
-  uint64_t* afull = bars;
-  uint64_t* aempty = afull + Cfg::kStages;
-  uint64_t* bfull = aempty + Cfg::kStages;
-  uint64_t* bempty = bfull + Cfg::kBStages;
-  uint64_t* acc_full = bempty + Cfg::kBStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
+  uint8_t* sb = sa + Cfg::kABytes;
+  uint64_t* ld_full = reinterpret_cast<uint64_t*>(sb + Cfg::kBBytes);
 
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int num_tiles = 2 * B;   // (image, half)
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   GridBar bar(gs);
   if (tid == 0) {
     tma_prefetch_desc(&tm_x);
     tma_prefetch_desc(&tm_dy);
-    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&afull[s], 1); mbar_init(&aempty[s], 1); }
-    for (int s = 0; s < Cfg::kBStages; ++s) { mbar_init(&bfull[s], 1); mbar_init(&bempty[s], 1); }
-    mbar_init(acc_full, 1);
+    mbar_init(ld_full, 1);
     fence_mbar_init();
   }
-  if (warp == 4) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 5) {
-    if (elect_one()) {
-      int g = 0, it = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        const int n = tile >> 1, h = tile & 1;
-        const int row0 = n * Cfg::kFrame + Cfg::kFirst + 128 * h;          // first dy position of this K tile
-        const int bs = it % Cfg::kBStages;
-        mbar_wait(&bempty[bs], ((it / Cfg::kBStages) & 1) ^ 1);
-        mbar_arrive_expect_tx(&bfull[bs], Cfg::kBStageBytes);
-        tma_load_2d(sb + bs * Cfg::kBStageBytes, &tm_dy, &bfull[bs], 0, row0);
-        for (int mt = 0; mt < 4; ++mt) {
-          const int npairs = mt == 3 ? 3 : 4;                               // pair 15 does not exist
-          for (int half = 0; half < 2; ++half, ++g) {
-            const int s = g % Cfg::kStages;
-            mbar_wait(&aempty[s], ((g / Cfg::kStages) & 1) ^ 1);
-            mbar_arrive_expect_tx(&afull[s], npairs * 8192);
-            for (int a = 0; a < npairs; ++a) {
-              const int q = mt * 4 + a, kh = q / 3, kw = 2 * (q - kh * 3);
-              // x position of dy position P for tap (kh, kw): P + (kh-2)·18 + (kw-2); negative / past-the-end rows are zero-filled
-              tma_load_2d(sa + s * Cfg::kAStageBytes + a * 8192, &tm_x, &afull[s], 0, row0 + 64 * half + (kh - 2) * 18 + (kw - 2));
-            }
-          }
-        }
-      }
+  float acc[4][2][4][4];   // warp w: tap pairs q = 4w .. 4w+3
+#pragma unroll
+  for (int a = 0; a < 4; ++a)
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) acc[a][j][nt][e] = 0.f;
+  int it = 0;
+  for (int n = blockIdx.x; n < B; n += gridDim.x, ++it) {
+    if (tid == 0) {
+      const int frame0 = n * Cfg::kFrame;
+      mbar_arrive_expect_tx(ld_full, Cfg::kABytes + Cfg::kBBytes);
+      for (int bx = 0; bx < Cfg::kABoxes; ++bx) tma_load_2d(sa + bx * 8192, &tm_x, ld_full, 0, frame0 + 64 * bx);   // rows past the tensor are zero-filled
+      tma_load_2d(sb, &tm_dy, ld_full, 0, frame0 + Cfg::kFirst);
+      tma_load_2d(sb + kTileM * 128, &tm_dy, ld_full, 0, frame0 + Cfg::kFirst + kTileM);
     }
-  } else if (warp == 4) {
-    constexpr uint32_t idesc = umma_idesc_tf32(kTileM, 32) | (1u << 15) | (1u << 16);  // A and B are MN-major
-    int g = 0, it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int bs = it % Cfg::kBStages;
-      mbar_wait(&bfull[bs], (it / Cfg::kBStages) & 1);
-      for (int mt = 0; mt < 4; ++mt) {
-        for (int h = 0; h < 2; ++h, ++g) {
-          const int s = g % Cfg::kStages;
-          mbar_wait(&afull[s], (g / Cfg::kStages) & 1);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t a0 = smem_u32(sa + s * Cfg::kAStageBytes), b0 = smem_u32(sb + bs * Cfg::kBStageBytes) + h * 8 * 1024;
+    mbar_wait(ld_full, it & 1);
 #pragma unroll
-            for (int kb = 0; kb < 8; ++kb)
-              umma_tf32(tmem_base + mt * 32, umma_desc_mn_sw128_32b(a0 + kb * 1024, 8 * 1024, 512),
-                        umma_desc_mn_sw128_32b(b0 + kb * 1024, 1024, 512), idesc, (it | h | kb) != 0);
-            umma_commit(&aempty[s]);
-            if (mt == 3 && h == 1) umma_commit(&bempty[bs]);
-          }
-          __syncwarp();
-        }
-      }
+    for (int a = 0; a < 4; ++a) {
+      const int q = warp * 4 + a, kh = q / 3, kw = 2 * (q - kh * 3);
+      if (q < 15) wgrad_win_atom(acc[a], reinterpret_cast<const float*>(sa), Cfg::kFirst + (kh - 2) * 18 + (kw - 2), 0,
+                                 reinterpret_cast<const float*>(sb), 0, lane);
     }
-    if (elect_one()) umma_commit(acc_full);
-    __syncwarp();
-  } else {
-    // ---- epilogue (warps 0-3): four accumulators → this CTA's partial [512][32] ------------------------------------
-    mbar_wait(acc_full, 0);
-    __syncwarp();
-    tc_fence_after();
-    for (int mt = 0; mt < 4; ++mt) {
-      const int m = mt * kTileM + tid;
-      float v[32];
-#pragma unroll
-      for (int c0 = 0; c0 < 32; c0 += 16) {
-        float t[16];
-        tmem_ld_32x32b_x16(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + mt * 32 + c0, t);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[c0 + j] = t[j];
-      }
-      float* o = partials + (static_cast<size_t>(blockIdx.x) * Cfg::kMRows + m) * 32;
-#pragma unroll
-      for (int q = 0; q < 8; ++q) *reinterpret_cast<float4*>(o + 4 * q) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-    }
+    __syncthreads();   // every warp is done with this image's tiles before the next loads overwrite them
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) tmem_dealloc<Cfg::kTmemCols>(tmem_base);
+#pragma unroll
+  for (int a = 0; a < 4; ++a) {
+    const int q = warp * 4 + a;
+    if (q < 15) wgrad_win_atom_store(acc[a], partials + (static_cast<size_t>(blockIdx.x) * Cfg::kMRows + q * 32) * 32, lane);
+  }
   if (dw == nullptr) return;   // two-launch variant: wgrad_win_fold_kernel folds
   // ---- in-kernel fold (cooperative launch): after a grid barrier every CTA folds a share of the 400 × 32 outputs over the
   //      per-CTA partials in a fixed order — thread = (co, one of six partial classes), classes combined through smem ----------
   bar.sync(gs);
-  float* s_f = reinterpret_cast<float*>(smem);   // [6][32]
+  float* s_f = reinterpret_cast<float*>(smem);   // [4][32]
   const int co = tid & 31, part = tid >> 5, nparts = gridDim.x;
   for (int i = blockIdx.x; i < 401; i += gridDim.x) {
     float acc = 0.f;
@@ -1108,21 +936,21 @@ __global__ void __launch_bounds__(192, 1) conv5x5_wgrad_win_kernel(const __grid_
       const int m = (3 * kh + (kw >> 1)) * 32 + (kw & 1) * 16 + ci;
       const float* p = partials + static_cast<size_t>(m) * 32 + co;
       const size_t stride = static_cast<size_t>(Cfg::kMRows) * 32;
-      for (int c = part; c < nparts; c += 48) {   // eight independent L2 loads in flight
+      for (int c = part; c < nparts; c += 32) {   // eight independent L2 loads in flight
         float t[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) t[j] = (c + 6 * j < nparts) ? __ldcg(p + static_cast<size_t>(c + 6 * j) * stride) : 0.f;
+        for (int j = 0; j < 8; ++j) t[j] = (c + 4 * j < nparts) ? __ldcg(p + static_cast<size_t>(c + 4 * j) * stride) : 0.f;
 #pragma unroll
         for (int j = 0; j < 8; ++j) acc += t[j];
       }
     } else {
-      for (int n = part; n < B; n += 6) acc += __ldcg(dysum + static_cast<size_t>(n) * 32 + co);
+      for (int n = part; n < B; n += 4) acc += __ldcg(dysum + static_cast<size_t>(n) * 32 + co);
     }
     __syncthreads();
     s_f[part * 32 + co] = acc;
     __syncthreads();
     if (part == 0) {
-      const float tot = ((s_f[co] + s_f[32 + co]) + (s_f[64 + co] + s_f[96 + co])) + (s_f[128 + co] + s_f[160 + co]);
+      const float tot = (s_f[co] + s_f[32 + co]) + (s_f[64 + co] + s_f[96 + co]);
       if (i < 400) dw[(co * 16 + (i & 15)) * 25 + (i >> 4)] = tot;
       else if (db) db[co] = tot;
     }
@@ -1161,11 +989,10 @@ __global__ void __launch_bounds__(256) wgrad_win_fold_kernel(const float* __rest
 }
 
 // =====================================================================================================
-// Hardware probe for the next conv design (profiles/conv_tma_ncu.md §3): can a K-major swizzled A operand
-// start at an arbitrary ROW of a larger smem buffer?  A [256][ROWB/4] tile is loaded once by TMA; the MMA
-// reads rows [shift, shift+128) through a descriptor whose start address is base + shift·ROWB, with the
-// descriptor's base-offset field either 0 (mode 0) or (start >> 7) & 7 (mode 1, the documented rule for
-// starts that are not aligned to the swizzle repeat).  D[128][32] = A[shift:shift+128] · Bᵀ.
+// Hardware probe of the descriptor convention the window convolutions rely on: can a K-major swizzled A
+// operand start at an arbitrary ROW of a larger smem buffer?  A [256][ROWB/4] tile is loaded once by TMA;
+// the wgmma reads rows [shift, shift+128) through descriptors whose start address is base + shift·ROWB,
+// with the base-offset field either 0 (mode 0) or (start >> 7) & 7 (mode 1).  D[128][32] = A[shift:shift+128] · Bᵀ.
 // Not used by any product path; run by tools/exp_rowshift.py.
 // =====================================================================================================
 template <int ROWB>
@@ -1176,55 +1003,41 @@ __global__ void __launch_bounds__(128, 1) umma_rowshift_probe_kernel(const __gri
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sa = smem;                         // [256][ROWB]
   uint8_t* sb = smem + kRows * ROWB;          // [32][ROWB]   (1024-aligned: 256·ROWB is a multiple of 1024)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sb + 4096);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
-  const int warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) {
-    mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
+  uint64_t* bar = reinterpret_cast<uint64_t*>(sb + 4096);
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    mbar_init(bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<32>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (warp == 0 && elect_one()) {
-    mbar_arrive_expect_tx(&bars[0], kRows * ROWB + kN * ROWB);
-    tma_load_2d(sa, &tm_a, &bars[0], 0, 0);
-    tma_load_2d(sb, &tm_b, &bars[0], 0, 0);
+  if (tid == 0) {
+    mbar_arrive_expect_tx(bar, kRows * ROWB + kN * ROWB);
+    tma_load_2d(sa, &tm_a, bar, 0, 0);
+    tma_load_2d(sb, &tm_b, bar, 0, 0);
   }
-  if (warp == 1) {
-    mbar_wait(&bars[0], 0);
-    tc_fence_after();
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_tf32(kTileM, kN);
-      const uint32_t a0 = smem_u32(sa) + static_cast<uint32_t>(shift) * ROWB, b0 = smem_u32(sb);
+  mbar_wait(bar, 0);
+  float acc[2][16];
 #pragma unroll
-      for (int k = 0; k < kK / 8; ++k) {
-        const uint32_t astart = a0 + k * 32;
-        uint64_t ad = umma_desc_kmajor<ROWB>(astart);
-        if (mode == 1) ad |= static_cast<uint64_t>((astart >> 7) & 7) << 49;
-        umma_tf32(tmem_base, ad, umma_desc_kmajor<ROWB>(b0 + k * 32), idesc, k != 0);
-      }
-      umma_commit(&bars[1]);
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int e = 0; e < 16; ++e) acc[h][e] = 0.f;
+  const uint32_t a0 = smem_u32(sa) + static_cast<uint32_t>(shift) * ROWB, b0 = smem_u32(sb);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < kK / 8; ++k)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t astart = a0 + h * 64 * ROWB + k * 32;
+      uint64_t ad = gmma_desc_kmajor<ROWB>(astart);
+      if (mode == 1) ad |= static_cast<uint64_t>((astart >> 7) & 7) << 49;
+      wgmma_m64n32k8_tf32(acc[h], ad, gmma_desc_kmajor<ROWB>(b0 + k * 32), k != 0);
     }
-    __syncwarp();
-  }
-  mbar_wait(&bars[1], 0);
-  __syncwarp();
-  tc_fence_after();
-  const int row = warp * 32 + (threadIdx.x & 31);
+  wgmma_commit();
+  wgmma_wait<0>();
 #pragma unroll
-  for (int c0 = 0; c0 < kN; c0 += 16) {
-    float v[16];
-    tmem_ld_32x32b_x16(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + c0, v);
+  for (int h = 0; h < 2; ++h)
 #pragma unroll
-    for (int j = 0; j < 16; ++j) d[row * kN + c0 + j] = v[j];
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<32>(tmem_base);
+    for (int e = 0; e < 16; ++e) d[(64 * h + wgmma_frag_row(tid, e)) * kN + wgmma_frag_col(tid, e)] = acc[h][e];
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1404,7 +1217,7 @@ static int win_rows_per_tile(const ConvShape& s) {
   return R;
 }
 static int win_base_offset_mode() {
-  static const int m = [] { const char* e = getenv("PDT_WIN_BASE_OFFSET"); return e ? atoi(e) : 1; }();
+  static const int m = [] { const char* e = getenv("PDT_WIN_BASE_OFFSET"); return e ? atoi(e) : 0; }();
   return m;
 }
 
@@ -1469,7 +1282,7 @@ void launch_conv5x5_wgrad_tcgen05(const float* dy, const float* x, float* dw, fl
       ones_ready[dev] = true;
     }
   }
-  CUtensorMap tm_dy = make_tmap_2d(dy, 32, static_cast<uint64_t>(M), 32, kTileM, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
+  CUtensorMap tm_dy = make_tmap_2d(dy, 32, static_cast<uint64_t>(M), 32, kTileM, CU_TENSOR_MAP_SWIZZLE_128B);
   opt_in_smem(conv5x5_wgrad_umma_kernel, Cfg::kSmem);
   conv5x5_wgrad_umma_kernel<<<grid, Cfg::kThreads, Cfg::kSmem, st>>>(x, tm_dy, ones, scr.partials, s.B, s.H, s.W, tiles);
   check_launch("conv5x5_wgrad_umma");
@@ -1485,10 +1298,10 @@ void make_wgrad_win_tmaps(const float* x_pad, const float* dy_pad, int B, CUtens
   cuuint32_t box[2] = {32, 64};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = driver().cuTensorMapEncodeTiled(tm_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(x_pad), dims, strides, box, estr,
-                                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B,
+                                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) throw std::runtime_error("cuTensorMapEncodeTiled(overlapping rows) failed: " + cu_error(r));
-  *tm_dy = make_tmap_2d(dy_pad, 32, rows, 32, kTileM, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
+  *tm_dy = make_tmap_2d(dy_pad, 32, rows, 32, kTileM, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 void launch_conv5x5_wgrad_win(const float* dy_pad, const float* x_pad, const float* dysum, float* dw, float* db, int B, ReduceScratch scr,
@@ -1527,21 +1340,19 @@ void launch_gemm_tf32_tcgen05(const float* a, const float* b, float* d, int M, i
   if (N % 16 != 0 || N < 16 || N > 256) throw std::invalid_argument("gemm_tf32_tcgen05: N must be a multiple of 16 in [16, 256]");
   if (K % 4 != 0 || K < 4) throw std::invalid_argument("gemm_tf32_tcgen05: K must be a positive multiple of 4 (16-byte rows for TMA)");
   CUtensorMap tm_a = make_tmap_2d(a, static_cast<uint64_t>(K), static_cast<uint64_t>(M), kChunkK, kTileM);
-  const int grid = (M + kTileM - 1) / kTileM;
-#define PDT_GEMM_CASE(NT)                                                                    \
-  if (N <= NT) {                                                                             \
-    CUtensorMap tm_b = make_tmap_2d(b, static_cast<uint64_t>(K), static_cast<uint64_t>(N), kChunkK, NT); \
-    auto kern = gemm_tf32_umma_kernel<NT>;                                                   \
-    opt_in_smem(kern, GemmCfg<NT>::kSmem);                                                   \
-    kern<<<grid, 128, GemmCfg<NT>::kSmem, st>>>(tm_a, tm_b, d, M, N, K);                     \
+  const int mtiles = (M + kTileM - 1) / kTileM;
+#define PDT_GEMM_CASE(NB)                                                                    \
+  if (N <= NB || NB == 64) {                                                                 \
+    CUtensorMap tm_b = make_tmap_2d(b, static_cast<uint64_t>(K), static_cast<uint64_t>(N), kChunkK, NB); \
+    auto kern = gemm_tf32_umma_kernel<NB>;                                                   \
+    opt_in_smem(kern, GemmCfg<NB>::kSmem);                                                   \
+    kern<<<dim3(mtiles, (N + NB - 1) / NB), 160, GemmCfg<NB>::kSmem, st>>>(tm_a, tm_b, d, M, N, K); \
     check_launch("gemm_tf32_umma");                                                          \
     return;                                                                                  \
   }
   PDT_GEMM_CASE(16)
   PDT_GEMM_CASE(32)
   PDT_GEMM_CASE(64)
-  PDT_GEMM_CASE(128)
-  PDT_GEMM_CASE(256)
 #undef PDT_GEMM_CASE
 }
 

@@ -1,4 +1,4 @@
-// CUDA-side bindings: GPU communicators and the sm_100a operator library.
+// CUDA-side bindings: GPU communicators and the sm_90a operator library.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <pybind11/stl.h>
@@ -66,8 +66,7 @@ ReduceScratch scratch(const at::Tensor& like) {
   return r;
 }
 
-// The tensor-core weight gradient is the default (exact-integer GPU test green, 31.8 µs vs 70.7 µs SIMT
-// on B200, profiles/op_bench.md); PDT_WGRAD_TCGEN05=0 falls back to the SIMT kernel.
+// The tensor-core weight gradient is the default; PDT_WGRAD_TCGEN05=0 selects the SIMT kernel instead.
 bool wgrad_tcgen05_default() {
   static const bool on = [] {
     const char* e = getenv("PDT_WGRAD_TCGEN05");
@@ -605,7 +604,7 @@ void register_cuda_bindings(py::module_& m) {
     }
   });
 
-  // ---- tcgen05 GEMM self-test (D[M,N] = A[M,K]·B[N,K]^T in TF32) — validates descriptors/TMEM/TMA ---------
+  // ---- TF32 wgmma GEMM self-test (D[M,N] = A[M,K]·B[N,K]^T) — validates descriptors/TMA/accumulator layout ---
   m.def("umma_rowshift_probe", [](const at::Tensor& a, const at::Tensor& b, int64_t shift, int64_t mode) {
     chk(a, "a"); chk(b, "b");
     TORCH_CHECK(a.dim() == 2 && a.size(0) == 256 && (a.size(1) == 16 || a.size(1) == 32) && b.dim() == 2 && b.size(0) == 32 &&

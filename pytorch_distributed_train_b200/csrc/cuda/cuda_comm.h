@@ -12,7 +12,7 @@
 namespace pdt {
 
 // Stream-ordered completion handle: wait() makes the *current* stream wait for the collective
-// (ProcessGroupNCCL semantics the reference relies on, SURVEY §2.2 B5); never blocks the host.
+// (ProcessGroupNCCL semantics the reference relies on); never blocks the host.
 class CudaWork : public CommWork {
  public:
   CudaWork(int device, std::vector<at::Tensor> keep) : device_(device), keep_(std::move(keep)) {}

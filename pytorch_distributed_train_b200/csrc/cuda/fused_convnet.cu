@@ -1,19 +1,19 @@
 // Cooperative fused kernels for the reference ConvNet (ref: ddp_example.py:22-41) — one CTA per image.
 //
-// A ConvNet step is ~10 µs of work spread over dependent kernel boundaries (profiles/roofline.md): every per-op kernel
+// A ConvNet step is a few µs of arithmetic spread over dependent kernel boundaries and every per-op kernel
 // pays launch + ramp + drain + a grid-wide reduction.  Here everything that belongs to an image stays inside its CTA
-// (registers / shared memory / TMEM), and the only grid-wide dependencies — the BatchNorm batch statistics (forward), the
+// (registers / shared memory), and the only grid-wide dependencies — the BatchNorm batch statistics (forward), the
 // Σdz, Σdz·x̂ sums (backward) and the folds of the weight gradients — are device-side grid barriers in the middle of a
 // kernel instead of kernel boundaries.  A training step is three launches:
 //
 //   convnet_fwd_kernel         conv1 5x5 (1→16) ──barrier (Σy, Σy²)── BN + ReLU + MaxPool2 written straight into conv2's
-//                              swizzled smem patch ── conv2 5x5 (16→32) on tcgen05 (the 25 taps are row-shifted UMMA descriptors
-//                              into that patch; accumulators in TMEM) ──barrier── BN + ReLU + MaxPool2 + classifier
+//                              swizzled smem patch ── conv2 5x5 (16→32) on wgmma (the 25 taps are row-shifted descriptors
+//                              into that patch; accumulators in registers) ──barrier── BN + ReLU + MaxPool2 + classifier
 //                              (+ cross-entropy term and d(loss)/d(logits) when the targets are known)           (ref :25-34,40)
 //   convnet_l2_bwd_kernel<FC>  classifier backward + MaxPool/ReLU/BN backward ──barrier (Σdz, Σdz·x̂)── dy → conv2 data
-//                              gradient on tcgen05
+//                              gradient on wgmma
 //   convnet_l1_bwd_kernel<WG>  MaxPool/ReLU/BN backward ──barrier── conv1 weight gradient (mma.sync) ──barrier── folds,
-//                              while one extra warp computes conv2's weight gradient on tcgen05 (MN-major window) and — on one
+//                              while conv2's weight gradient is computed on mma.sync (MN-major window) and — on one
 //                              GPU — the threads that write the folded gradients apply the SGD update (SgdRider)
 //
 // convnet_l1_fwd_kernel / convnet_l2_fwd_kernel (one kernel per layer) and the <false> instantiations are the variants without
@@ -37,6 +37,7 @@
 #include "fused_convnet.h"
 #include "grid_sync.cuh"
 #include "umma_ptx.cuh"
+#include "wgrad_win.cuh"
 
 namespace pdt {
 
@@ -48,7 +49,7 @@ using namespace ptx;
 __device__ unsigned long long g_trace[4][160][12];
 __device__ int g_trace_on = 0;
 // The switch is read ONCE per kernel (TRACE_INIT, one global load whose latency overlaps the prologue); a stamp is then a predicated
-// branch on a register — a load of the switch per stamp cost ~0.2 µs each on the critical path (12 stamps in the forward kernel).
+// branch on a register — a load of the switch per stamp would put a global-memory latency on the critical path at every stamp.
 #define TRACE_INIT() const bool trace_on_ = (threadIdx.x == 0) && (*reinterpret_cast<volatile int*>(&g_trace_on) != 0)
 __device__ __forceinline__ void trace_stamp(bool on, int kernel, int phase) {
   if (on) {
@@ -288,43 +289,26 @@ convnet_l1_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w, 
 constexpr int kL1BwdSmem = (784 * 16 + kL1Warps * 512) * 4;
 
 // The conv2 weight gradient of an image needs nothing from layer-1 backward — only the dy / x frames that layer-2 backward
-// left in global memory — and layer-1 backward leaves the tensor cores, TMA and half of shared memory idle.  With WG the CTA
-// carries one extra warp that computes dW2ᵀ[(kh, kw, ci)][co] = Σ_P xpad[P + (kh−2)·18 + (kw−2)][ci] · dypad[P][co] of the same
-// image on tcgen05 while the 25 layer-1 warps do their SIMT work:
-//   * B (dy, MN-major): the 256 positions starting at the first interior one, two TMA boxes.
-//   * A (x, MN-major): the "window" trick of the forward pass, applied to an MN-major operand.  Row r of the overlapping-row view
-//     of the frame (pitch 64 B, length 128 B) holds positions r and r+1 = two horizontally adjacent taps × 16 channels, i.e. one
-//     32-wide M atom for K index r.  The whole image is loaded ONCE (384 rows, 48 KB); the atom of tap pair (kh, kw/2) for K
-//     position P is the same buffer read (kh−2)·18 + (kw−2) rows further down — a descriptor start address, not a copy
-//     (SWIZZLE_128B_ATOM_32B follows the absolute smem address, like the K-major case probed in profiles/r2/rowshift_probe.log).
-//     An M = 128 MMA takes four atoms at a uniform stride (the descriptor's LBO): tile kw/2 ∈ {0,1,2} stacks kh = 0..3 (stride
-//     18 rows), tile 3 holds kh = 4 with kw/2 = 0..3 (stride 2 rows; the fourth atom is a dummy).  The stand-alone kernel
-//     (conv_tcgen05.cu) materialises every tap pair by TMA instead: 491 KB of L2 reads per image where this one needs 48 KB.
-//   * four 128 × 32 accumulators in TMEM; 128 MMAs (K = 8 each); the per-CTA partial [512][32] is read out of TMEM by 16 of the
-//     layer-1 warps just before the kernel's second grid barrier and folded after it, next to the conv1 gradient.
-// One launch and one grid barrier less than running the two kernels back to back; the tensor-core work hides behind the SIMT phases.
+// left in global memory.  With WG the CTA carries one extra warp that TMA-loads both operands of the same image while the 25
+// layer-1 warps do their SIMT work, and 15 of those warps compute dW2ᵀ[(kh, kw, ci)][co] = Σ_P xpad[P + (kh−2)·18 + (kw−2)][ci] ·
+// dypad[P][co] on the tensor cores (wgrad_win.cuh) just before the kernel's second grid barrier; it is folded after it, next to
+// the conv1 gradient:
+//   * B (dy): the 256 positions starting at the first interior one, two TMA boxes.
+//   * A (x): the whole image's overlapping-row view (pitch 64 B, length 128 B: row r = positions r and r+1 = two horizontally
+//     adjacent taps × 16 channels), loaded ONCE (384 rows, 48 KB); the 32-row atom of tap pair (kh, kw/2) for position P is the
+//     same buffer read (kh−2)·18 + (kw−2) rows further down.  The per-CTA partial has 512 rows in four groups of four atoms:
+//     group kw/2 ∈ {0,1,2} stacks kh = 0..3 (stride 18 rows), group 3 holds kh = 4 with kw/2 = 0..2 (stride 2 rows; its fourth
+//     atom is unused).  The stand-alone kernel (conv_tcgen05.cu) orders the atoms by (kh, kw/2) instead.
+// One launch and one grid barrier less than running the two kernels back to back.
 struct L1WgCfg {
-  static constexpr int kThreads = kL1Threads + 32;        // + one warp: TMA loads, then the tcgen05 issue loop
+  static constexpr int kThreads = kL1Threads + 32;        // + one warp: the TMA loads
   static constexpr int kFrame = 18 * 18, kFirst = 2 * 18 + 2;
   // A window: rows [0, 384) of the image's overlapping-row view (row r = positions r, r+1 × 16 channels = 128 B), six 64-row boxes
   static constexpr int kABoxes = 6, kABytes = kABoxes * 64 * 128;
   static constexpr int kBBytes = 2 * 128 * 128;                    // both 128-position dy tiles of the image
-  static constexpr int kTmemCols = 128;
   static constexpr int kOff = (kL1BwdSmem + 1023) / 1024 * 1024;   // window starts 1024-aligned behind the layer-1 buffers
   static constexpr size_t kSmem = 1024 + kOff + kABytes + kBBytes + 256;
 };
-
-__device__ __forceinline__ uint32_t f32_to_tf32(float v) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
-  return r;
-}
-// D(16×8) += A(16×8, row) · B(8×8, col); fragments per the PTX ISA m16n8k8 .tf32 layout
-__device__ __forceinline__ void mma_m16n8k8_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 
 // One SGD update (the arithmetic of sgd_multi_kernel, ops_simt.cu) of element *p with gradient g.
 __device__ __forceinline__ void sgd_apply(float* p, float g, float* m, const SgdHyper& h, float lr) {
@@ -357,8 +341,6 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   uint8_t* sa = dsm_b + L1WgCfg::kOff;                              // WG: A window
   uint8_t* sb = sa + L1WgCfg::kABytes;                              // WG: dy tiles
   uint64_t* ld_full = reinterpret_cast<uint64_t*>(sb + L1WgCfg::kBBytes);
-  uint64_t* acc_full = ld_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
   __shared__ float xs[32 * 32];
   __shared__ float red[kL1Warps * 32];
   __shared__ float s_tmp[kL1Warps * 32];
@@ -368,24 +350,18 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
 
   if constexpr (WG) {
     if (warp == kL1Warps) {
-      // ================= tensor-core weight gradient of image n: one warp loads by TMA, then issues the MMAs =================
+      // ================= operands of the conv2 weight gradient of image n: one warp loads them by TMA =================
       using Cfg = L1WgCfg;
       if (lane == 0) {
         tma_prefetch_desc(&tm_x2);
         tma_prefetch_desc(&tm_dy2);
         mbar_init(ld_full, 1);
-        mbar_init(acc_full, 1);
         fence_mbar_init();
       }
       __syncwarp();
-      tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-      tc_fence_before();
-      asm volatile("bar.arrive 0, %0;" ::"n"(L1WgCfg::kThreads) : "memory");   // (1) the layer-1 warps sync on barrier 0 before they touch these
-      __syncwarp();
-      tc_fence_after();
-      const uint32_t tmem_base = *tmem_slot;
+      asm volatile("bar.arrive 0, %0;" ::"n"(L1WgCfg::kThreads) : "memory");   // (1) the layer-1 warps sync on barrier 0 before they wait on ld_full
       const int frame0 = n * Cfg::kFrame;
-      // the weight gradient has ~10 µs of slack: let the layer-1 warps have the L2 → SM path for their opening loads first
+      // let the layer-1 warps have the L2 → SM path for their opening loads first
       asm volatile("bar.sync 4, %0;" ::"n"(L1WgCfg::kThreads) : "memory");
       if (elect_one()) {
         mbar_arrive_expect_tx(ld_full, Cfg::kABytes + Cfg::kBBytes);
@@ -394,29 +370,6 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
         tma_load_2d(sb + 128 * 128, &tm_dy2, ld_full, 0, frame0 + Cfg::kFirst + 128);
       }
       __syncwarp();
-      mbar_wait(ld_full, 0);
-      tc_fence_after();
-      if (elect_one()) {
-        constexpr uint32_t idesc = umma_idesc_tf32(128, 32) | (1u << 15) | (1u << 16);  // A and B are MN-major
-        const uint32_t a_base = smem_u32(sa), b_base = smem_u32(sb);
-#pragma unroll 1
-        for (int mt = 0; mt < 4; ++mt) {
-          // first atom's row shift and the stride between the tile's four atoms
-          const int shift0 = mt < 3 ? (0 - 2) * 18 + 2 * mt - 2 : 2 * 18 - 2;
-          const uint32_t lbo = mt < 3 ? 18 * 128 : 2 * 128;
-#pragma unroll 1
-          for (int kc = 0; kc < 32; ++kc) {   // K = 256 positions in steps of 8
-            const uint32_t a0 = a_base + static_cast<uint32_t>(Cfg::kFirst + 8 * kc + shift0) * 128;
-            umma_tf32(tmem_base + mt * 32, umma_desc_mn_sw128_32b(a0, lbo, 512), umma_desc_mn_sw128_32b(b_base + kc * 1024, 1024, 512), idesc,
-                      kc != 0);
-          }
-        }
-        umma_commit(acc_full);
-      }
-      __syncwarp();
-      asm volatile("bar.sync 3, %0;" ::"n"(L1WgCfg::kThreads) : "memory");   // (2) the layer-1 warps have read the accumulators
-      tc_fence_after();
-      tmem_dealloc<Cfg::kTmemCols>(tmem_base);
       return;
     }
   }
@@ -525,7 +478,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   cta_sync<NAMED>();
   // conv1 weight gradient of this image on the tensor cores: dW[co][tap] = Σ_px dy[px][co] · x[px + tap] is a
   // 16 × 32 × 784 GEMM (taps 25..31 padded; tap 25 multiplies a column of ones → the bias gradient).  M = 16 is below
-  // tcgen05's minimum tile, so this is warp-level mma.sync m16n8k8 (TF32 in, fp32 accumulate): a warp takes every
+  // the 64-row wgmma tile, so this is warp-level mma.sync m16n8k8 (TF32 in, fp32 accumulate): a warp takes every
   // 25th group of 8 pixels, builds the A fragment from the staged dy and the four B fragments (8 taps each) straight
   // from the haloed image — no im2col buffer — and the 25 per-warp 16×32 accumulators are folded through smem.
   {
@@ -589,29 +542,26 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   }
   trace(1, 4);
   if constexpr (WG) {
-    // the tensor-core pipeline has been running since the kernel started; pick up its four 128 × 32 accumulators
-    // (16 warps: TMEM lane quarter = warp % 4, accumulator = warp / 4) and write this image's partial [512][32]
-    asm volatile("bar.sync 0, %0;" ::"n"(L1WgCfg::kThreads) : "memory");   // (1) mbarriers initialised, TMEM slot written (long ago)
-    if (warp < 16) {
-      mbar_wait(acc_full, 0);
-      __syncwarp();
-      tc_fence_after();
-      const uint32_t tmem_base = *tmem_slot;
-      const int mt = warp >> 2, lq = warp & 3;
-      float v[32];
+    // the operands have been loading since the kernel started: 15 warps take one 32-row atom each and write this image's
+    // partial [512][32]
+    asm volatile("bar.sync 0, %0;" ::"n"(L1WgCfg::kThreads) : "memory");   // (1) ld_full initialised (long ago)
+    if (warp < 15) {
+      mbar_wait(ld_full, 0);
+      const int mt = warp >> 2, a = warp & 3;   // atom a of group mt (group 3 has three)
+      const int shift0 = mt < 3 ? (0 - 2) * 18 + 2 * mt - 2 : 2 * 18 - 2;
+      const int stride = mt < 3 ? 18 : 2;
+
+      float acc[2][4][4];
 #pragma unroll
-      for (int c0 = 0; c0 < 32; c0 += 16) {
-        float t[16];
-        tmem_ld_32x32b_x16(tmem_base + (static_cast<uint32_t>(lq * 32) << 16) + mt * 32 + c0, t);
+      for (int j2 = 0; j2 < 2; ++j2)
 #pragma unroll
-        for (int j = 0; j < 16; ++j) v[c0 + j] = t[j];
-      }
-      float* o = wpart + (static_cast<size_t>(n) * 512 + mt * 128 + lq * 32 + lane) * 32;
+        for (int nt = 0; nt < 4; ++nt)
 #pragma unroll
-      for (int q = 0; q < 8; ++q) *reinterpret_cast<float4*>(o + 4 * q) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-      tc_fence_before();
+          for (int e = 0; e < 4; ++e) acc[j2][nt][e] = 0.f;
+      wgrad_win_atom<256, 32, 1>(acc, reinterpret_cast<const float*>(sa), L1WgCfg::kFirst + shift0 + a * stride, 0, reinterpret_cast<const float*>(sb), 0,
+                     lane);
+      wgrad_win_atom_store(acc, wpart + (static_cast<size_t>(n) * 512 + mt * 128 + a * 32) * 32, lane);
     }
-    asm volatile("bar.arrive 3, %0;" ::"n"(L1WgCfg::kThreads) : "memory");   // (2) TMEM may be released
     trace(1, 7);
   }
   bar.sync<NAMED>(gs);
@@ -706,12 +656,12 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
 }
 
 // =====================================================================================================================
-// Layer 2 — conv2 (16→32, 5x5) is 88 % of the model's FLOPs: tcgen05.  One CTA = one 14×14 image.
+// Layer 2 — conv2 (16→32, 5x5) is 88 % of the model's FLOPs: wgmma.  One CTA = one 14×14 image.
 // The zero-haloed input (18×18 positions × 128-byte rows, channels 16..31 zero-filled by TMA) is loaded ONCE; output
 // pixel (oh, ow) is MMA row p = oh·18 + ow of one of two M = 128 tiles (rows 0..125 ↔ oh 0..6, 126..251 ↔ oh 7..13;
 // ow ≥ 14 rows are padding), and filter tap (kh, kw) is the same buffer read through a K-major SWIZZLE_128B descriptor
 // that starts (kh·18 + kw) rows further in (swizzle phase follows the absolute address: verified on hardware by
-// tools/exp_rowshift.py, profiles/rowshift_probe.md).  Weights are swizzled into shared memory by the CTA itself.
+// tools/exp_rowshift.py).  Weights are swizzled into shared memory by the CTA itself.
 // =====================================================================================================================
 constexpr int kL2Threads = 256;
 constexpr int kPW = 18;                          // padded width
@@ -720,6 +670,50 @@ constexpr int kPatchBytes = kPatchRows * 128;    // 41,472
 constexpr int kPatchAlloc = 43008;               // + slack rows read by the padding rows of tile 1 (multiple of 1024)
 
 __device__ __forceinline__ uint32_t sw128_off(int row, int chunk16) { return static_cast<uint32_t>(row) * 128u + (static_cast<uint32_t>(chunk16 ^ (row & 7)) << 4); }
+
+// conv2 of one image on the tensor cores, issued by the warpgroup of warps 4..7 (wt = thread index inside it): per output
+// tile t, 25 taps × 2 K-steps of wgmma m64n32k8 per 64-row half, the A descriptors row-shifted into the haloed patch.  The
+// accumulators go straight into ys [pixel][32] (bias added; 16-byte chunks rotated by the pixel index, as the column reads
+// that follow expect).
+__device__ __forceinline__ void l2_conv_wgmma(const uint8_t* sa, const uint8_t* sb, const float* __restrict__ bias, float* ys, int wt) {
+  const uint64_t ad0 = gmma_desc_kmajor<128>(smem_u32(sa)), bd0 = gmma_desc_kmajor<128>(smem_u32(sb));
+#pragma unroll 1
+  for (int t = 0; t < 2; ++t) {
+    float acc[2][16];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int e = 0; e < 16; ++e) acc[h][e] = 0.f;
+    wgmma_fence();
+#pragma unroll 1
+    for (int kh = 0; kh < 5; ++kh) {
+      const uint64_t ad = ad0 + static_cast<uint64_t>(((7 * t + kh) * kPW * 128) >> 4);
+      const uint64_t bd = bd0 + static_cast<uint64_t>((kh * 5 * 4096) >> 4);
+#pragma unroll
+      for (int kw = 0; kw < 5; ++kw) {
+#pragma unroll
+        for (int k = 0; k < 2; ++k)   // K = 16 input channels = two K=8 steps; the zero upper half is never multiplied
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            wgmma_m64n32k8_tf32(acc[h], ad + ((h * 64 * 128 + kw * 128 + k * 32) >> 4), bd + ((kw * 4096 + k * 32) >> 4), (kh | kw | k) != 0);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int e = 0; e < 16; ++e) {
+        const int rr = 64 * h + wgmma_frag_row(wt, e), c = wgmma_frag_col(wt, e);
+        const int orow = rr / kPW, ow = rr - orow * kPW;
+        if (rr < 126 && ow < 14) {
+          const int pix = (7 * t + orow) * 14 + ow;
+          ys[pix * 32 + ((((c >> 2) + pix) & 7) << 2) + (c & 3)] = acc[h][e] + (bias ? __ldg(bias + c) : 0.f);
+        }
+      }
+    }
+  }
+}
 
 struct L2FwdSmem {
   static constexpr int kB = 25 * 32 * 128;       // weights: [tap][32 co][128 B] (ci 0..15 used)            102,400
@@ -745,8 +739,7 @@ convnet_l2_fwd_kernel(const __grid_constant__ CUtensorMap tm_x, const float* __r
   float* s_scale = misc + 576;                         // [32]
   float* s_shift = misc + 608;                         // [32]
 
-  __shared__ uint64_t bar_x, bar_mma;
-  __shared__ uint32_t tmem_slot;
+  __shared__ uint64_t bar_x;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = blockIdx.x, B = gridDim.x;
 
   GridBar bar(gs);
@@ -755,16 +748,12 @@ convnet_l2_fwd_kernel(const __grid_constant__ CUtensorMap tm_x, const float* __r
   if (tid == 0) {
     tma_prefetch_desc(&tm_x);
     mbar_init(&bar_x, 1);
-    mbar_init(&bar_mma, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<64>(&tmem_slot);
-  // zero the slack behind the patch (read only by padding rows, but keep NaNs out of TMEM)
+  // zero the slack behind the patch (read only by padding rows, but keep NaNs out of the accumulators)
   for (int i = tid; i < (kPatchAlloc - kPatchBytes) / 16; i += kL2Threads) reinterpret_cast<float4*>(sa + kPatchBytes)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  tc_fence_before();
+  fence_proxy_async_smem();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
   if (tid == 0) {
     mbar_arrive_expect_tx(&bar_x, kPatchBytes);
     tma_load_4d(sa, &tm_x, &bar_x, 0, 0, 0, n);        // the frame carries its zero halo; channels ≥ 16: out-of-bounds zero fill
@@ -791,60 +780,10 @@ convnet_l2_fwd_kernel(const __grid_constant__ CUtensorMap tm_x, const float* __r
   fence_proxy_async_smem();   // generic-proxy writes of B → visible to the tensor core
   __syncthreads();
   trace(2, 1);
-  if (warp == 0) {
+  // ---- conv2 + epilogue: the warpgroup of warps 4..7 ------------------------------------------------------------------------
+  if (warpgroup_index() == 1) {
     mbar_wait(&bar_x, 0);
-    tc_fence_after();
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_tf32(128, 32);
-      // the start-address field is the low 14 bits (bytes >> 4): a descriptor is advanced by plain integer adds
-      const uint64_t ad0 = umma_desc_kmajor<128>(smem_u32(sa)), bd0 = umma_desc_kmajor<128>(smem_u32(sb));
-#pragma unroll 1
-      for (int t = 0; t < 2; ++t) {
-#pragma unroll 1
-        for (int kh = 0; kh < 5; ++kh) {
-          const uint64_t ad = ad0 + static_cast<uint64_t>(((7 * t + kh) * kPW * 128) >> 4);
-          const uint64_t bd = bd0 + static_cast<uint64_t>((kh * 5 * 4096) >> 4);
-#pragma unroll
-          for (int kw = 0; kw < 5; ++kw) {
-#pragma unroll
-            for (int k = 0; k < 2; ++k)   // K = 16 input channels = two K=8 steps; the zero upper half is never multiplied
-              umma_tf32(tmem_base + t * 32, ad + ((kw * 128 + k * 32) >> 4), bd + ((kw * 4096 + k * 32) >> 4), idesc, (kh | kw | k) != 0);
-          }
-        }
-      }
-      umma_commit(&bar_mma);
-    }
-    __syncwarp();
-  }
-  // ---- epilogue: warps 4..7 own TMEM lane quadrants 0..3 ----------------------------------------------------------------
-  if (warp >= 4) {
-    mbar_wait(&bar_mma, 0);
-    __syncwarp();
-    tc_fence_after();
-    const int quad = warp & 3, rr = quad * 32 + lane;   // MMA row inside the tile
-    const int orow = rr / kPW, ow = rr - orow * kPW;
-#pragma unroll 1
-    for (int t = 0; t < 2; ++t) {
-      float v[32];
-#pragma unroll
-      for (int c0 = 0; c0 < 32; c0 += 16) {
-        float t16[16];
-        tmem_ld_32x32b_x16(tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + t * 32 + c0, t16);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[c0 + j] = t16[j];
-      }
-      if (rr < 126 && ow < 14) {
-        const int oh = 7 * t + orow, pix = oh * 14 + ow;
-        float4* yl = reinterpret_cast<float4*>(ys + pix * 32);
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          float4 o = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-          if (bias) { o.x += __ldg(bias + 4 * q); o.y += __ldg(bias + 4 * q + 1); o.z += __ldg(bias + 4 * q + 2); o.w += __ldg(bias + 4 * q + 3); }
-          yl[(q + pix) & 7] = o;   // rotate the 16-byte chunks by the pixel index: conflict-free column reads below
-        }
-      }
-    }
-    tc_fence_before();
+    l2_conv_wgmma(sa, sb, bias, ys, tid - 128);
   }
   __syncthreads();
   trace(2, 2);
@@ -955,17 +894,15 @@ convnet_l2_fwd_kernel(const __grid_constant__ CUtensorMap tm_x, const float* __r
     }
   }
 
-  tc_fence_before();
   __syncthreads();
   bar.finish(gs);
   trace(2, 7);
-  if (warp == 1) tmem_dealloc<64>(tmem_base);
 }
 
 // =====================================================================================================================
 // Whole forward pass in ONE kernel: layer 1 and layer 2 (+ classifier) of an image run in the same CTA, so the pooled
 // layer-1 activations never leave the SM on their way into conv2 — they are written straight into the swizzled,
-// zero-haloed shared-memory patch the tcgen05 descriptors read (the global copy is still written: backward needs it) —
+// zero-haloed shared-memory patch the wgmma descriptors read (the global copy is still written: backward needs it) —
 // and the conv2 weights are staged while conv1 computes.  Two grid barriers (BN1 and BN2 batch statistics), one launch.
 // =====================================================================================================================
 __global__ void __launch_bounds__(kL1Threads, 1)
@@ -992,19 +929,12 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
   __shared__ float s_tmp[kL1Warps * 32];
   __shared__ float s_tot[32];
   __shared__ float s_scale[16], s_shift[16];
-  __shared__ uint64_t bar_mma;
-  __shared__ uint32_t tmem_slot;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = blockIdx.x, B = gridDim.x;
   const L1Map m(tid);
   GridBar bar(gs);
   TRACE_INIT();
   trace(0, 0);
 
-  if (tid == 0) {
-    mbar_init(&bar_mma, 1);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc<64>(&tmem_slot);
   for (int i = tid; i < kPatchAlloc / 16; i += kL1Threads) reinterpret_cast<float4*>(sa)[i] = make_float4(0.f, 0.f, 0.f, 0.f);   // halo = 0
   l1_load_image(x + static_cast<size_t>(n) * 784, xs, tid);
   if (tid < 400) {
@@ -1018,10 +948,7 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
 #pragma unroll
     for (int tap = 0; tap < 25; ++tap) wv[tap] = __ldg(w2 + tid * 25 + tap);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
   trace(0, 11);
 
   // ---- layer 1 ------------------------------------------------------------------------------------------------------
@@ -1126,57 +1053,8 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
   fence_proxy_async_smem();   // generic-proxy writes of the patch and of the weights → visible to the tensor core
   __syncthreads();
   trace(0, 4);
-  // ---- layer 2: 100 MMAs, one elected thread -----------------------------------------------------------------------------
-  if (warp == 0) {
-    tc_fence_after();
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_tf32(128, 32);
-      const uint64_t ad0 = umma_desc_kmajor<128>(smem_u32(sa)), bd0 = umma_desc_kmajor<128>(smem_u32(sb));
-#pragma unroll 1
-      for (int t = 0; t < 2; ++t) {
-#pragma unroll 1
-        for (int kh = 0; kh < 5; ++kh) {
-          const uint64_t ad = ad0 + static_cast<uint64_t>(((7 * t + kh) * kPW * 128) >> 4);
-          const uint64_t bd = bd0 + static_cast<uint64_t>((kh * 5 * 4096) >> 4);
-#pragma unroll
-          for (int kw = 0; kw < 5; ++kw) {
-#pragma unroll
-            for (int k = 0; k < 2; ++k)
-              umma_tf32(tmem_base + t * 32, ad + ((kw * 128 + k * 32) >> 4), bd + ((kw * 4096 + k * 32) >> 4), idesc, (kh | kw | k) != 0);
-          }
-        }
-      }
-      umma_commit(&bar_mma);
-    }
-    __syncwarp();
-  }
-  if (warp >= 4 && warp < 8) {   // epilogue: TMEM lane quadrant = warp % 4
-    mbar_wait(&bar_mma, 0);
-    __syncwarp();
-    tc_fence_after();
-    const int quad = warp & 3, rr = quad * 32 + lane;
-    const int orow = rr / kPW, ow = rr - orow * kPW;
-#pragma unroll 1
-    for (int t = 0; t < 2; ++t) {
-#pragma unroll
-      for (int c0 = 0; c0 < 32; c0 += 16) {
-        float t16[16];
-        tmem_ld_32x32b_x16(tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + t * 32 + c0, t16);
-        if (rr < 126 && ow < 14) {
-          const int pix = (7 * t + orow) * 14 + ow;
-          float4* yl = reinterpret_cast<float4*>(ys + pix * 32);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int cq = (c0 >> 2) + q;
-            float4 o = make_float4(t16[4 * q], t16[4 * q + 1], t16[4 * q + 2], t16[4 * q + 3]);
-            if (b2) { o.x += __ldg(b2 + 4 * cq); o.y += __ldg(b2 + 4 * cq + 1); o.z += __ldg(b2 + 4 * cq + 2); o.w += __ldg(b2 + 4 * cq + 3); }
-            yl[(cq + pix) & 7] = o;
-          }
-        }
-      }
-    }
-    tc_fence_before();
-  }
+  // ---- layer 2: 200 wgmma (K = 8, M = 64 each) by the warpgroup of warps 4..7 --------------------------------------------
+  if (warpgroup_index() == 1) l2_conv_wgmma(sa, sb, b2, ys, tid - 128);
   __syncthreads();
   trace(0, 5);
   if (tid < 128) {
@@ -1314,9 +1192,6 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
     }
   }
   trace(0, 10);
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<64>(tmem_base);
 }
 
 // ---- layer 2 backward: pool/ReLU/BN backward + conv2 data gradient ---------------------------------------------------------
@@ -1331,7 +1206,7 @@ struct L2BwdSmem {
 // FC: the classifier's backward rides along.  The gradient of the pooled activations is not read from `dout` but computed
 // on the fly, d(out)[n][k] = Σ_j dlogits[n][j] · Wfc[j][k] (fc weights staged in smem once per CTA); the classifier's weight
 // gradient dWfc[j][k] = Σ_n dlogits[n][j] · out[n][k] is produced in 16-column slices, one slice per CTA (all images, fixed
-// order: deterministic, no partials), the bias gradient by the CTA that owns "slice 98".  One kernel and ~7 µs less per step.
+// order: deterministic, no partials), the bias gradient by the CTA that owns "slice 98".  One kernel less per step.
 template <bool FC>
 __global__ void __launch_bounds__(kL2Threads, 1)
 convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float* __restrict__ y /*[B,14,14,32]*/,
@@ -1345,7 +1220,7 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
                       int ncls, const float* __restrict__ loss_parts /*[B] or null*/, float* loss_out) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sa = smem;                                  // dy patch, written by the CTA in the TMA/UMMA SWIZZLE_128B layout
+  uint8_t* sa = smem;                                  // dy patch, written by the CTA in the TMA/wgmma SWIZZLE_128B layout
   uint8_t* sb = sa + kPatchAlloc;
   float* misc = reinterpret_cast<float*>(sb + L2BwdSmem::kB);   // 1024 floats
   float* s_part = misc;                                // [8][64]
@@ -1358,18 +1233,11 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
   float* s_fcw = misc + 1024;                                   // FC: [ncls][1568]
   float* s_dl = s_fcw + L2BwdSmem::kFcW / 4;                    // FC: [B][16] (columns >= ncls zero)
   float* s_pool = s_dl + L2BwdSmem::kFcDl / 4;                  // FC: [B][16] slice of the pooled activations
-  __shared__ uint64_t bar_mma;
-  __shared__ uint32_t tmem_slot;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = blockIdx.x, B = gridDim.x;
 
   GridBar bar(gs);
   TRACE_INIT();
   trace(3, 0);
-  if (tid == 0) {
-    mbar_init(&bar_mma, 1);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc<32>(&tmem_slot);
   if constexpr (FC) {
     // stage the classifier weights (cp.async, no registers, lands while the dgrad weights are built), every image's dlogits and this
     // CTA's first 16-column slice of the pooled activations (loads batched in registers: one L2 latency, not one per element)
@@ -1418,10 +1286,7 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
     }
   }
   if constexpr (FC) cp_async_wait<0>();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
   trace(3, 1);
 
   // thread = (channel c, window group g): windows pp = g, g+8, ... (≤ 7 per thread); y values stay in registers
@@ -1571,52 +1436,47 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
     dysum[static_cast<size_t>(n) * 32 + tid] = s;
   }
   trace(3, 5);
-  if (warp == 0) {
-    tc_fence_after();
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_tf32(128, 16);
-      const uint64_t ad0 = umma_desc_kmajor<128>(smem_u32(sa)), bd0 = umma_desc_kmajor<128>(smem_u32(sb));
-#pragma unroll 1
-      for (int t = 0; t < 2; ++t) {
-#pragma unroll 1
-        for (int kh = 0; kh < 5; ++kh) {
-          const uint64_t ad = ad0 + static_cast<uint64_t>(((7 * t + kh) * kPW * 128) >> 4);
-          const uint64_t bd = bd0 + static_cast<uint64_t>((kh * 5 * 2048) >> 4);
-#pragma unroll
-          for (int kw = 0; kw < 5; ++kw) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k)   // K = 32 output channels = four K=8 steps
-              umma_tf32(tmem_base + t * 16, ad + ((kw * 128 + k * 32) >> 4), bd + ((kw * 2048 + k * 32) >> 4), idesc, (kh | kw | k) != 0);
-          }
-        }
-      }
-      umma_commit(&bar_mma);
-    }
-    __syncwarp();
-  }
-  if (warp >= 4) {
-    mbar_wait(&bar_mma, 0);
-    __syncwarp();
-    tc_fence_after();
-    const int quad = warp & 3, rr = quad * 32 + lane;
-    const int orow = rr / kPW, ow = rr - orow * kPW;
+  // ---- conv2 data gradient: 400 wgmma m64n16k8 by the warpgroup of warps 4..7, accumulators straight to the dx frame -------
+  if (warpgroup_index() == 1) {
+    const int wt = tid - 128;
+    const uint64_t ad0 = gmma_desc_kmajor<128>(smem_u32(sa)), bd0 = gmma_desc_kmajor<128>(smem_u32(sb));
 #pragma unroll 1
     for (int t = 0; t < 2; ++t) {
-      float v[16];
-      tmem_ld_32x32b_x16(tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + t * 16, v);
-      if (rr < 126 && ow < 14) {
-        float4* o = reinterpret_cast<float4*>(dx + (static_cast<size_t>(n) * 324 + (7 * t + orow + 2) * 18 + ow + 2) * 16);
+      float acc[2][8];
 #pragma unroll
-        for (int q = 0; q < 4; ++q) o[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc[h][e] = 0.f;
+      wgmma_fence();
+#pragma unroll 1
+      for (int kh = 0; kh < 5; ++kh) {
+        const uint64_t ad = ad0 + static_cast<uint64_t>(((7 * t + kh) * kPW * 128) >> 4);
+        const uint64_t bd = bd0 + static_cast<uint64_t>((kh * 5 * 2048) >> 4);
+#pragma unroll
+        for (int kw = 0; kw < 5; ++kw) {
+#pragma unroll
+          for (int k = 0; k < 4; ++k)   // K = 32 output channels = four K=8 steps
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              wgmma_m64n16k8_tf32(acc[h], ad + ((h * 64 * 128 + kw * 128 + k * 32) >> 4), bd + ((kw * 2048 + k * 32) >> 4), (kh | kw | k) != 0);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          const int rr = 64 * h + wgmma_frag_row(wt, e), ci = wgmma_frag_col(wt, e);
+          const int orow = rr / kPW, ow = rr - orow * kPW;
+          if (rr < 126 && ow < 14) dx[(static_cast<size_t>(n) * 324 + (7 * t + orow + 2) * 18 + ow + 2) * 16 + ci] = acc[h][e];
+        }
       }
     }
-    tc_fence_before();
   }
-  tc_fence_before();
   __syncthreads();
   bar.finish(gs);
   trace(3, 6);
-  if (warp == 1) tmem_dealloc<32>(tmem_base);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

@@ -5,8 +5,7 @@
 // parallel, fixed row order) into a group partial; the last *group* to finish folds the
 // ≤ ceil(n/16) group partials and calls fin(i, total) for every output i.  The longest dependent
 // chain is ~16 + n/16 row loads split over width-wise thread groups, instead of n serial L2 round
-// trips in one thread (which cost 20-30 µs for the 300-400 CTA launches of the ConvNet step;
-// profiles/op_bench.md).  Summation order depends only on (n, width, thread count) ⇒ bit-reproducible.
+// trips in one thread.  Summation order depends only on (n, width, thread count) ⇒ bit-reproducible.
 // Counters are left at zero, so the same scratch serves the next launch / CUDA-graph replay.
 #pragma once
 #include <cuda_runtime.h>

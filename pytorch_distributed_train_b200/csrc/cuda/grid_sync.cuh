@@ -35,7 +35,7 @@ __device__ __forceinline__ void st_release_gpu(unsigned int* p, unsigned int v) 
 // after the barrier comes from L2 (ld.global.cg), the GPU's coherence point, so no trailing fence is needed.  Each CTA
 // tracks the epoch locally (read once at kernel start, +1 per barrier): no read of the word before arriving, nothing to
 // reset between launches or CUDA-graph replays, any grid size.  A flag-per-CTA variant (every CTA polling every flag)
-// was measured at 5.5 µs per barrier against 2-3 µs for the counter: 10^4 pollers on four cache lines (profiles/r2).
+// puts ~10^4 pollers on four cache lines and is slower than the counter.
 struct GridBar {
   unsigned int e;
   __device__ __forceinline__ explicit GridBar(GridSync gs) : e(gs.epoch ? *reinterpret_cast<volatile unsigned int*>(gs.epoch) : 0u) {}
@@ -46,7 +46,7 @@ struct GridBar {
     else __syncthreads();
   }
   // Split form: arrive() publishes this CTA's contribution, wait() blocks until every CTA has arrived.  Work placed between
-  // the two runs in the barrier's shadow (≈ 2 µs of latency plus the skew between CTAs) — it must not depend on other CTAs.
+  // the two runs in the barrier's shadow (the barrier latency plus the skew between CTAs) — it must not depend on other CTAs.
   template <int NAMED = 0>
   __device__ __forceinline__ void arrive(GridSync gs) {
     ++e;

@@ -1,5 +1,4 @@
-// Thin libnccl binding — the *measured baseline and correctness oracle* for the NVLink kernels
-// (SURVEY §2.3: "thin C++ NCCL binding as the measured baseline only"; `--comm nccl`).  The
+// Thin libnccl binding — the *measured baseline and correctness oracle* for the NVLink kernels (`--comm nccl`).  The
 // library is resolved with dlopen at first use so the extension imports on machines without it.
 #include <c10/cuda/CUDAGuard.h>
 #include <dlfcn.h>

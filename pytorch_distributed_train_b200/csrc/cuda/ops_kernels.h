@@ -1,4 +1,4 @@
-// Host launchers for the sm_100a compute kernels (no torch types; raw pointers + stream).
+// Host launchers for the sm_90a compute kernels (no torch types; raw pointers + stream).
 // Activation layout between fused layers is NHWC (= torch channels_last), fp32.
 #pragma once
 #include <cuda_runtime.h>
@@ -22,7 +22,7 @@ struct ReduceScratch {
   int counters;
 };
 
-// ---- SIMT direct convolution (conv1; conv2 fallback + oracle for the tcgen05 kernel) -------------
+// ---- SIMT direct convolution (conv1; conv2 fallback + oracle for the tensor-core kernels) -------------
 // x NHWC [B,H,W,Cin], w torch layout [Cout,Cin,5,5], bias [Cout] (nullable) → y NHWC [B,H,W,Cout].
 // stats (nullable): [2*Cout+1] = per-channel Σy, Σy², then the element count per channel.
 void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float* y, float* stats, ConvShape s,

@@ -1,10 +1,10 @@
-// sm_100a SIMT kernels for the ConvNet hot path (ref model: ddp_example.py:22-41) and the generic
+// sm_90a SIMT kernels for the ConvNet hot path (ref model: ddp_example.py:22-41) and the generic
 // BatchNorm pieces behind SyncBatchNorm.  They replace what the reference dispatches to
-// cuDNN/ATen (SURVEY §2.5 K1-K19): conv + bias + BN-statistics in one pass, BN-apply + ReLU +
+// cuDNN/ATen: conv + bias + BN-statistics in one pass, BN-apply + ReLU +
 // MaxPool in one pass (no int64 pool indices: the arg-max is recomputed in backward), fused
 // log-softmax/NLL, one multi-tensor SGD launch.  All cross-CTA reductions are deterministic
 // (per-CTA partials + last-CTA fold in fixed order), so runs are bit-reproducible.
-// conv2 (88% of the FLOPs) has a tcgen05/TMEM implementation in conv_tcgen05.cu; the SIMT
+// conv2 (88% of the FLOPs) has a tensor-core implementation in conv_tcgen05.cu; the SIMT
 // version here is its fallback and numerical oracle.
 #include <cuda_runtime.h>
 
@@ -518,7 +518,7 @@ __global__ void __launch_bounds__(256) bn_reduce_nchw_kernel(const float* __rest
 
 // Forward statistics in fp64: Σx, Σx² of channel c.  Downstream computes var = E[x²] − μ², which
 // amplifies the rounding of the two sums by μ²/σ²; fp32 sums made first-step gradients of a
-// SyncBN ResNet-18 differ from torch's (Welford) by 1 % (profiles/numerics_syncbn.md), fp64 sums
+// SyncBN ResNet-18 differ from torch's (Welford) by up to 1 %, fp64 sums
 // (and an fp64 exchange between ranks) bring that to 1e-5.  The kernel is bandwidth-bound either way.
 __global__ void __launch_bounds__(256) bn_stats_nchw_f64_kernel(const float* __restrict__ x, double* out, int N, int C, int HW, int S,
                                                                 ReduceScratch scr) {
@@ -809,8 +809,8 @@ void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float
                         cudaStream_t st) {
   constexpr int TH = 7;
   if (s.H % TH != 0) throw std::invalid_argument("conv5x5_fwd: H must be a multiple of 7");
-  // conv1 (1→16) one-CTA-per-image variant (784 threads, 100 CTAs): measured 23.5 µs vs 20.5 µs for the
-  // 400 quarter-image CTAs on B200 (profiles/op_bench_v1.md, v3) — kept for experiments, off by default
+  // conv1 (1→16) one-CTA-per-image variant (784 threads, 100 CTAs) instead of 400 quarter-image CTAs — kept for
+  // experiments, off by default (it was the slower of the two when the default was chosen; not re-measured on H100)
   static const bool whole_env = [] { const char* e = getenv("PDT_CONV1_WHOLE_IMAGE"); return e && e[0] == '1'; }();
   const bool whole_image = whole_env && s.Cin == 1 && s.Cout == 16 && s.H == 28 && s.W * 28 <= 1024;
   const int blocks = whole_image ? s.B : s.B * (s.H / TH);
@@ -855,7 +855,7 @@ void launch_conv5x5_wgrad(const float* dy, const float* x, float* dw, float* db,
   constexpr int TH = 7;
   if (s.H % TH != 0) throw std::invalid_argument("conv5x5_wgrad: H must be a multiple of 7");
   static const bool whole_env = [] { const char* e = getenv("PDT_CONV1_WHOLE_IMAGE"); return e && e[0] == '1'; }();
-  const bool whole_image = whole_env && s.Cin == 1 && s.Cout == 16 && s.H == 28;  // one CTA per image: slower (29.7 vs 25.5 µs)
+  const bool whole_image = whole_env && s.Cin == 1 && s.Cout == 16 && s.H == 28;  // one CTA per image (opt-in, see launch_conv5x5_fwd)
   const int blocks = whole_image ? s.B : s.B * (s.H / TH);
   const int width = 25 * s.Cin * s.Cout + s.Cout;
   if (static_cast<long long>(blocks) * width > scr.capacity_floats) throw std::invalid_argument("conv5x5_wgrad: reduction scratch too small");

@@ -81,9 +81,10 @@ SymmComm::SymmComm(std::shared_ptr<Store> store, int rank, int size, int device,
   store_ = store;
   heap_ = std::make_shared<SymmetricHeap>(std::move(store), rank, size, device, heap_bytes, timeout);
   if (const char* a = getenv("PDT_AR_ALGO")) algo_ = a;
-  // Measured one-shot / two-shot crossover (profiles/allreduce_sweep_{2,8}gpu.json): at N = 2 a one-shot push moves the
-  // same bytes as a two-shot and wins up to 4 MiB (20.8 vs 25.4 µs); at N = 8 it sends 7× the data and loses above
-  // 256 KiB (1 MiB: 24.9 vs 16.2 µs NVLS).  N = 4 is interpolated until it is measured.
+  // One-shot / two-shot crossover: at N = 2 a one-shot push moves the same bytes as a two-shot, so it stays ahead up to
+  // large messages; at N = 8 it sends 7× the data and falls behind much earlier.  These switch points were chosen on the
+  // previous NVLink generation and have not been re-measured on H100 (NVLink 4); tools/allreduce_sweep.py measures them,
+  // PDT_AR_ONESHOT_MAX overrides them.
   oneshot_max_ = size <= 2 ? (size_t(4) << 20) : size <= 4 ? (size_t(1) << 20) : (size_t(512) << 10);
   if (const char* m = getenv("PDT_AR_ONESHOT_MAX")) oneshot_max_ = static_cast<size_t>(atoll(m));
   if (const char* b = getenv("PDT_AR_BLOCKS")) cfg_.blocks = atoi(b);
@@ -173,7 +174,7 @@ void SymmComm::do_allreduce(at::Tensor& t, ReduceOp op, double scale, int channe
   std::string algo = algo_;
   if (algo == "auto") {
     if (slot_bytes * size_ <= half && nbytes <= oneshot_max_) algo = heap_->has_multicast() ? "oneshot_mc" : "oneshot";
-    // with two ranks the switch adds a hop and reduces nothing: peer loads beat NVLS (64 MiB: 137 vs 183 µs)
+    // with two ranks the switch adds a hop and reduces nothing: peer loads are preferred to NVLS
     else algo = (nvls_ok && size_ > 2) ? "nvls" : "twoshot";
   }
   if ((algo == "oneshot" || algo == "oneshot_mc") && slot_bytes * size_ > half) algo = nvls_ok ? "nvls" : "twoshot";

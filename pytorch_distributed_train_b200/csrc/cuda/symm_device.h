@@ -16,7 +16,7 @@ bool process_exiting();
 
 constexpr int kSymmMaxWorld = 8;       // one NVSwitch domain (single node, like the reference)
 constexpr int kSymmChannels = 4;       // independent flag/staging sets: one per concurrent stream
-constexpr int kSymmMaxBlocks = 160;    // >= 148 SMs: every CTA of a collective owns a flag row
+constexpr int kSymmMaxBlocks = 160;    // >= the SM count (132 on an H100 SXM): every CTA of a collective owns a flag row
 constexpr int kChanComm = 0;           // process-group collectives on the comm stream
 constexpr int kChanInline = 1;         // collectives fused into compute kernels on the caller's stream
 constexpr int kChanAux = 2;            // side uses (debug, tests)

@@ -1,6 +1,6 @@
-// sm_100a collective kernels over NVLink peer / multicast memory.
+// sm_90a collective kernels over NVLink peer / multicast memory.
 //
-// These are the product's communication path (BASELINE.json north star; SURVEY §5.8): the DDP
+// These are the product's communication path (BASELINE.json north star): the DDP
 // bucket allreduce, the per-step BatchNorm-buffer broadcast and SyncBatchNorm's statistic
 // exchange all run here, as plain kernel launches with device-side cross-GPU barriers, so they
 // can be issued from an autograd hook on a side stream *and* captured in a CUDA graph.  What the
@@ -376,6 +376,20 @@ __global__ void barrier_kernel(const __grid_constant__ SymmDev d) {
 }
 
 // ---- launch helpers -------------------------------------------------------------------------------------
+// SM count of the current device (cached per device): the two-shot kernels use at most one CTA per SM.
+int device_sm_count() {
+  static int cached[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64) dev = 0;
+  if (cached[dev] == 0) {
+    int n = 0;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = kSymmMaxBlocks;
+    cached[dev] = n;
+  }
+  return cached[dev];
+}
+
 int auto_blocks(size_t nvec, int threads, int cap) {
   size_t b = (nvec + static_cast<size_t>(threads) * 2 - 1) / (static_cast<size_t>(threads) * 2);
   return static_cast<int>(std::max<size_t>(1, std::min<size_t>(b, static_cast<size_t>(cap))));
@@ -490,7 +504,7 @@ void launch_allreduce_twoshot(const SymmDev& d, size_t buf_off, size_t count, in
   if (nvec == 0) return;
   const int threads = cfg.threads ? cfg.threads : 512;
   const size_t per = (nvec + d.world - 1) / d.world;
-  const int blocks = std::min(cfg.blocks ? cfg.blocks : auto_blocks(per, threads, 148), kSymmMaxBlocks);
+  const int blocks = std::min(cfg.blocks ? cfg.blocks : auto_blocks(per, threads, device_sm_count()), kSymmMaxBlocks);
   const float sc = static_cast<float>(scale);
   if (nvls) {
     if (!d.mc) throw std::runtime_error("twoshot nvls requested but the heap has no multicast mapping");

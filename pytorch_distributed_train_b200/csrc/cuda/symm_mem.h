@@ -1,6 +1,6 @@
 // Symmetric memory heap across the per-GPU processes of one node.
 //
-// This is the substrate of the NVLink-native backend (SURVEY §5.8): every rank owns one
+// This is the substrate of the NVLink-native backend: every rank owns one
 // physically contiguous heap (cuMemCreate), exports it as a POSIX fd, ships the fd to its peers
 // over an AF_UNIX socket (SCM_RIGHTS; names published through the Store) and maps every peer's
 // heap into its own address space, so a kernel can load/store any rank's memory directly over

@@ -1,5 +1,5 @@
-// Hand-written PTX wrappers for the Blackwell data path: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma /
-// commit / ld) and the shared-memory matrix descriptors.  Shared by conv_tcgen05.cu and fused_convnet.cu.
+// Hand-written PTX wrappers for the Hopper data path: mbarrier, TMA (cp.async.bulk.tensor), wgmma and the
+// shared-memory matrix descriptors.  Shared by conv_tcgen05.cu and fused_convnet.cu.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -40,8 +40,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
@@ -78,88 +76,78 @@ __device__ __forceinline__ void cp_async_16(uint32_t smem_dst, const void* gsrc,
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// TMEM
-template <int COLS> __device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "n"(COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS> __device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// ---------------------------------------------------------------------------------------------------
+// wgmma (sm_90a): one warpgroup (4 consecutive warps, the first a multiple of 4) issues the MMA; the fp32
+// accumulator lives in the registers of its 128 threads.  TF32 operands come from shared memory through
+// K-major matrix descriptors (TF32 wgmma has no MN-major form).
+// ---------------------------------------------------------------------------------------------------
+// Index of the calling thread's warpgroup, in a form the compiler knows to be warp-uniform: branching on it keeps the
+// wgmma of the taken side out of a "divergent path", where ptxas would serialise them.
+__device__ __forceinline__ int warpgroup_index() { return __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x) / 128, 0); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D[64×32] (+)= A[64×8] · B[32×8]ᵀ; accumulate = 0 overwrites D.
+__device__ __forceinline__ void wgmma_m64n32k8_tf32(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
       : "memory");
 }
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
+// D[64×16] (+)= A[64×8] · B[16×8]ᵀ
+__device__ __forceinline__ void wgmma_m64n16k8_tf32(float (&d)[8], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
       : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+}
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  static_assert(N == 16 || N == 32, "wgmma_tf32: N = 16 or 32");
+  if constexpr (N == 32) wgmma_m64n32k8_tf32(d, adesc, bdesc, accumulate);
+  else wgmma_m64n16k8_tf32(d, adesc, bdesc, accumulate);
+}
+// Accumulator fragment of an m64nN wgmma: element e of warpgroup thread wt (0..127) is D[frag_row][frag_col].
+__device__ __forceinline__ int wgmma_frag_row(int wt, int e) { return 16 * (wt >> 5) + ((wt & 31) >> 2) + 8 * ((e >> 1) & 1); }
+__device__ __forceinline__ int wgmma_frag_col(int wt, int e) { return 8 * (e >> 2) + 2 * (wt & 3) + (e & 1); }
+
+// Store the fragment of rows [row0, row0 + 64) into a row-major fp32 tile (pitch in floats), so that one thread can then
+// read a whole accumulator row.
+template <int N>
+__device__ __forceinline__ void wgmma_frag_store(const float (&d)[N / 2], float* tile, int pitch, int row0, int wt) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int e = 0; e < N / 2; ++e) tile[(row0 + wgmma_frag_row(wt, e)) * pitch + wgmma_frag_col(wt, e)] = d[e];
 }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_100 "version 1"):
-//   start address >> 4 | LBO (ignored for swizzled K-major, set to 1) << 16 | SBO = 1024 B (8 rows × 128 B) >> 4 << 32
-//   | version 1 << 46 | layout SWIZZLE_128B (2) << 61.       [cf. cute/arch/mma_sm100_desc.hpp]
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// K-major shared-memory matrix descriptor (sm_90 layout) for rows of ROWB bytes (128 → SWIZZLE_128B, 64 → SWIZZLE_64B):
+//   start address >> 4 | LBO (unused for swizzled K-major: 1) << 16 | SBO = 8 rows >> 4 << 32 | layout << 62.
+// The swizzle phase follows the absolute shared-memory address, so a descriptor may start at any row of a 1024-byte-aligned
+// buffer (the window convolutions read filter taps as row-shifted views of one patch).  The start-address field is the low
+// 14 bits, so descriptors are advanced by plain integer adds of (bytes >> 4).
+template <int ROWB>
+__device__ __forceinline__ uint64_t gmma_desc_kmajor(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>((8 * ROWB) >> 4) << 32;
+  d |= static_cast<uint64_t>(ROWB == 128 ? 1 : 2) << 62;
   return d;
 }
-// Instruction descriptor, kind::tf32: D=f32 (bits 4-5 = 1), A=B=TF32 (2 at bits 7-9 / 10-12), both K-major,
-// N>>3 at bits 17-22, M>>4 at bits 24-28.
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
-
 
 __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3) {
   asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(
                    smem_u32(smem_dst)),
                "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
-}
-
-// K-major descriptor for rows of ROWB bytes (64 → SWIZZLE_64B, layout type 4; 128 → SWIZZLE_128B, type 2);
-// SBO = 8 rows.
-template <int ROWB>
-__device__ __forceinline__ uint64_t umma_desc_kmajor(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>((8 * ROWB) >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(ROWB == 128 ? 2 : 4) << 61;
-  return d;
-}
-
-
-// MN-major operand, SWIZZLE_128B with 32-byte atoms (TMA: CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B).  LBO = byte stride between
-// 32-element MN atoms, SBO = byte stride between 4-row K atoms (512 B when the 8 rows of one MMA are contiguous).
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128_32b(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(1) << 61;
-  return d;
 }
 
 }  // namespace ptx

@@ -16,7 +16,7 @@
 namespace pdt {
 
 namespace {
-// uint8 → float32 × scale (ToTensor).  78,400 elements per MNIST batch: the scalar loop is ~0.2 ms, the AVX2 one ~10 µs —
+// uint8 → float32 × scale (ToTensor).  78,400 elements per MNIST batch: the AVX2 loop is an order of magnitude faster than the scalar one —
 // the difference between a loader that keeps up with a 0.1 ms training step and one that does not.
 #if defined(__x86_64__)
 __attribute__((target("avx2"), optimize("O3"))) void u8_to_f32_avx2(const uint8_t* __restrict p, float* __restrict o, int64_t n, float sc) {
@@ -88,7 +88,7 @@ void BatchStager::start(at::Tensor indices) {
   nbatches_ = drop_last_ ? n / batch_ : (n + batch_ - 1) / batch_;
   // Batches are numbered across epochs (consume_ never resets): the slots handed back in the previous epoch whose CUDA events are
   // still pending stay in the ring's normal reaping order instead of being waited for here — with a 75-step epoch (8 ranks) that
-  // wait (the device is ~15 steps behind the host) stalled the training thread for 3 ms per epoch (profiles/r2/e2e_stalls.md).
+  // wait (the device is ~15 steps behind the host) stalled the training thread for milliseconds per epoch.
   base_ = consume_;
   produce_ = 0;
   error_ = nullptr;
@@ -225,7 +225,7 @@ bool BatchStager::next(at::Tensor* images, at::Tensor* targets) {
   // The consumer moves on.  The batch handed out TWO calls ago goes back to the ring: its tensors are no longer referenced by an
   // ordinary `for batch in loader` loop (the loop variables and the iterator's own frame still hold the *previous* batch while this
   // call runs — releasing that one here made the retention check below re-allocate its pinned buffers on every step whenever the
-  // device was idle, 150 µs each).  Everything the consumer enqueued on its current stream for that batch precedes the event.
+  // device was idle).  Everything the consumer enqueued on its current stream for that batch precedes the event.
   if (prev_handed_ >= 0) {
     Slot& p = ring_[static_cast<size_t>(prev_handed_ % depth_)];
     std::shared_ptr<void> ev;
@@ -281,7 +281,7 @@ bool BatchStager::next(at::Tensor* images, at::Tensor* targets) {
   // Hand out FRESH tensor objects over the slot's buffers.  Their storage deleter keeps the buffers alive and counts the tensors
   // still in user hands — the retention check of the worker.  (Handing out the ring's own tensors and looking at use_count() does
   // not work: once a tensor has had a Python wrapper, the wrapper and the TensorImpl keep each other alive, so the count never
-  // returns to one and every refill re-allocated its pinned buffers, ~150 µs each.)
+  // returns to one and every refill re-allocated its pinned buffers.)
   {
     std::vector<int64_t> shp{s.rows};
     shp.insert(shp.end(), sample_shape_.begin(), sample_shape_.end());

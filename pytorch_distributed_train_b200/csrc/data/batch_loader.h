@@ -5,14 +5,14 @@
 // worker thread (no GIL, no intra-op thread pool) gathers the sampler's indices out of the dataset tensor, converts
 // uint8 → float32 on the way (ToTensor's 1/255), and writes straight into a ring of pinned buffers that is allocated
 // once — a graph-replayed step is ~0.1 ms, and a pool miss in the pinned allocator (cudaHostAlloc) or a descheduled
-// OpenMP worker was measured stalling the Python loader for 40-80 ms (profiles/r2/e2e_stalls.md).
+// OpenMP worker was measured stalling the Python loader for tens of milliseconds.
 //
 // Ring safety: a slot is refilled only after (1) the consumer has asked for a later batch, (2) the CUDA event recorded
 // on the consumer's stream at that moment has completed (so `.to(device, non_blocking=True)` copies out of the slot
 // are done), and (3) nobody else holds a reference to the slot's tensors — if the user kept a batch (list(loader)),
 // the slot gets fresh buffers instead of being overwritten.  The events are *queried by the consumer thread* (inside
 // next(), oldest first): a worker parked in cudaEventSynchronize spins inside the driver and slowed every CUDA call of
-// the training thread by 4× (14 → 58 µs per step, profiles/r2/e2e_stalls.md); the worker itself never touches CUDA.
+// the training thread by several times; the worker itself never touches CUDA.
 #pragma once
 #include <ATen/ATen.h>
 

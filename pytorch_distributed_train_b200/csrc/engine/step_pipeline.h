@@ -1,8 +1,8 @@
 // Host side of a graph-replayed training step (engine.GraphedTrainStep): everything the training thread does around
 // `cudaGraphLaunch` — staging the next batch into the step's input buffers on a copy stream, ordering it against the
 // replays that read / wrote those buffers, shipping every loss to pinned host memory on a side stream — as three native
-// calls instead of ~25 Python-level stream / event / copy operations (measured at 2 GPUs: 52 + 43 µs of host time per
-// step in Python against an 88 µs device step, i.e. the input loop was host-bound; profiles/r2/bench_history.md).
+// calls instead of ~25 Python-level stream / event / copy operations, whose host time was comparable to the device time
+// of a replayed step (the input loop was host-bound).
 //
 // Ordering per input buffer set i (two sets, one captured graph each):
 //   copy stream : wait done[i] (the replay that last read set i) → copy batch → record ready[i]

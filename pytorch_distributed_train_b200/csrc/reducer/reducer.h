@@ -95,7 +95,7 @@ class Reducer {
   // backward, but no collective is launched (a fused allreduce+update kernel consumes the flat buckets).
   void set_defer_comm(bool on) { defer_comm_ = on; }
   bool defer_comm() const { return defer_comm_; }
-  // Sub-bucket overlap (SURVEY §5.8 item 6): a bucket is reduced in up to `max_chunks` contiguous pieces of at least
+  // Sub-bucket overlap: a bucket is reduced in up to `max_chunks` contiguous pieces of at least
   // `min_chunk_bytes`, each launched from the autograd hook as soon as its last gradient is ready, so the transfer
   // of early layers' gradients overlaps the rest of backward even when the whole model fits one bucket.
   void set_chunking(int64_t min_chunk_bytes, int64_t max_chunks);

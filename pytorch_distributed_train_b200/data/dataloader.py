@@ -3,12 +3,11 @@
 sampler=train_sampler``; torch/utils/data/dataloader.py:773-805 for the contract:
 BatchSampler → fetch → collate → pin).
 
-B200-first changes (the host must keep a ~20 µs training step fed):
+H100-first changes (the host must keep a ~0.1 ms training step fed):
 
 * **batched gather**: datasets that expose ``gather(indices) -> tuple[Tensor, ...]`` (our MNIST and
   synthetic datasets do) are sliced with one ``index_select`` per field instead of a Python loop
-  over samples plus ``default_collate`` (the reference pays 100 PIL round trips per step here,
-  SURVEY §2.2 B16);
+  over samples plus ``default_collate`` (the reference pays 100 PIL round trips per step here);
 * **pinned batches**: every batch is copied into a fresh pinned tensor from torch's event-tracked caching host
   allocator (a free-list pop after warm-up), so a consumer that runs ahead of the GPU can never see a batch
   overwritten under a pending H2D copy;
@@ -95,7 +94,7 @@ def _pin_batch(batch):
         sig = (tuple(t.shape), t.dtype)
         if sig not in _WARM_POOL:
             # Pre-warm the allocator's free list for this batch signature: a pool miss later means cudaHostAlloc, which
-            # was measured stalling the loader for 40-80 ms in the middle of a run (profiles/r2/e2e_stalls.md).  A block
+            # was measured stalling the loader for tens of milliseconds in the middle of a run.  A block
             # is recycled only after the H2D copy out of it has completed, so a consumer that runs several steps ahead of
             # the GPU keeps a dozen blocks of each kind in flight.
             _WARM_POOL.add(sig)

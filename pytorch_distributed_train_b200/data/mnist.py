@@ -2,8 +2,7 @@
 
 The reference builds ``torchvision.datasets.MNIST(root='./data', train=True,
 transform=ToTensor(), download=True)`` (ref: ddp_example.py:66-69), which downloads four
-idx-ubyte archives and converts every sample through PIL on the training thread
-(SURVEY §2.2 B16 — its real wall-clock bottleneck).  Here:
+idx-ubyte archives and converts every sample through PIL on the training thread.  Here:
 
 * the idx files are parsed directly (``root/MNIST/raw/*-ubyte[.gz]``, the layout torchvision
   writes, so an existing download is picked up as is);

@@ -120,7 +120,7 @@ class DistributedSampler(Sampler):
 
     def indices_tensor(self) -> torch.Tensor:
         """This rank's indices of the current epoch as an int64 tensor — the same sequence ``__iter__`` yields, built with tensor ops
-        only (60,000 Python ints cost ~2 ms per epoch start, 25 training steps of the reference ConvNet) and cached while
+        only (60,000 Python ints cost milliseconds per epoch start, many training steps of the reference ConvNet) and cached while
         (seed, epoch) do not change: the reference never calls ``set_epoch``, so every epoch after the first restarts for free."""
         n = len(self.dataset)
         key = (self.seed, self.epoch, self.shuffle, n, self.num_replicas, self.rank, self.drop_last)

@@ -9,7 +9,7 @@ mesh backend, the NVLink symmetric-memory backend and the NCCL baseline binding 
 Backends
 --------
 ``"nccl"``  (the reference's default flag value, ref: ddp_example.py:105)
-    GPU group. ``comm="fused"`` (default): collectives are our sm_100a kernels over NVLink peer /
+    GPU group. ``comm="fused"`` (default): collectives are our sm_90a kernels over NVLink peer /
     multicast memory (``SymmComm``). ``comm="nccl"``: the thin libnccl binding, kept as the measured
     baseline and oracle. Also selectable via ``PDT_COMM``.
 ``"gloo"`` / ``"cpu"``

@@ -3,8 +3,8 @@ captured once and replayed with a single ``cudaGraphLaunch``.  With ``fuse_optim
 and a single-bucket model on the NVLink backend, the bucket allreduce and the SGD update are one
 kernel (``optim.SGD.fuse_with_ddp``).
 
-Why this exists: one ConvNet step is ≈10 µs of GPU work behind 60-80 kernel launches in the
-reference stack (SURVEY §0.3 fact 3, §2.5), so the step is launch/host bound.  The reference's DDP
+Why this exists: one ConvNet step is a few µs of arithmetic behind 60-80 kernel launches in the
+reference stack, so the step is launch/host bound.  The reference's DDP
 cannot be graph-captured as a whole because its gradient reduction is a host-side NCCL call per
 bucket; ours is a plain kernel launched from the autograd hook on the comm stream, so the reducer,
 the per-step buffer sync and the fused optimizer all land inside the graph.

@@ -3,9 +3,9 @@
 (``layer1.0.weight`` … ``fc.bias``) so checkpoints interchange and
 ``SyncBatchNorm.convert_sync_batchnorm`` finds the BatchNorm layers where it expects them.
 
-On a B200 the forward does not walk the ``nn.Sequential``s.  In training the whole forward is TWO cooperative
-sm_100a kernels with one CTA per image (``csrc/cuda/fused_convnet.cu``): conv1+BN1+ReLU+pool1, and
-conv2 (tcgen05, TMEM accumulators, TMA-loaded haloed image) +BN2+ReLU+pool2+classifier — the BatchNorm batch
+On an H100 the forward does not walk the ``nn.Sequential``s.  In training the whole forward is TWO cooperative
+sm_90a kernels with one CTA per image (``csrc/cuda/fused_convnet.cu``): conv1+BN1+ReLU+pool1, and
+conv2 (wgmma, register accumulators, haloed image in shared memory) +BN2+ReLU+pool2+classifier — the BatchNorm batch
 statistics cross a device-side grid barrier inside the kernel instead of a kernel boundary; backward is one such
 kernel per layer plus the tensor-core weight gradient.  Shapes the fused kernels do not cover (eval mode,
 SyncBatchNorm, batch > #SMs) run each ``layerN`` as two per-op kernels (implicit-GEMM conv with the BN statistics in
@@ -41,7 +41,7 @@ class ConvNet(nn.Module):
 
         ok = x.is_cuda and x.dtype == torch.float32 and ops.native_available()
         if self.fused is True and not ok:
-            raise RuntimeError("ConvNet(fused=True) needs float32 CUDA input and the native sm_100a runtime")
+            raise RuntimeError("ConvNet(fused=True) needs float32 CUDA input and the native sm_90a runtime")
         return ok
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:

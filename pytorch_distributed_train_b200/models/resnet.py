@@ -1,8 +1,8 @@
 """ResNet-18/34 for the larger-bucket / overlap-stress configuration (BASELINE.json config 4:
-"ResNet-18 on synthetic 3×224×224, DDP 8×B200").  Own implementation of the standard
+"ResNet-18 on synthetic 3×224×224, DDP 8×H100").  Own implementation of the standard
 architecture (He et al. 2015); parameter names follow the common torchvision layout
 (``conv1``, ``bn1``, ``layer{1..4}.{i}.conv{1,2}``, ``downsample.{0,1}``, ``fc``) so the bucket
-plan matches the numbers in SURVEY App. B (62 tensors, 46,758,048 B → 3 buckets).
+plan matches torch DDP's (62 tensors, 46,758,048 B → 3 buckets).
 """
 from __future__ import annotations
 

@@ -1,7 +1,7 @@
 """Cross-entropy loss (ref: ddp_example.py:61,87 ``nn.CrossEntropyLoss().cuda(gpu)``).
 
 On CUDA, float32 ``[B, C]`` logits with class-index targets and ``reduction='mean'`` run as one
-fused sm_100a kernel (log-softmax + NLL + mean, saving the softmax so backward is a single
+fused sm_90a kernel (log-softmax + NLL + mean, saving the softmax so backward is a single
 ``(softmax − onehot)/B`` pass) instead of the reference stack's ``_log_softmax`` +
 ``nll_loss_forward`` pair and their two backward kernels.  Everything else defers to the
 standard functional."""

@@ -1,4 +1,4 @@
-"""sm_100a operator library (Python face).  Every function here launches hand-written CUDA
+"""sm_90a operator library (Python face).  Every function here launches hand-written CUDA
 kernels from ``_C`` (csrc/cuda/*.cu); there is no eager fallback on a GPU: if the native runtime
 is missing on a CUDA machine the ops raise instead of silently running ATen kernels."""
 from __future__ import annotations
@@ -11,13 +11,13 @@ _HAS_NATIVE = hasattr(_C, "ops_ready")
 
 
 def native_available() -> bool:
-    """True when the compiled sm_100a kernels are present *and* a CUDA device is usable."""
+    """True when the compiled sm_90a kernels are present *and* a CUDA device is usable."""
     return _HAS_NATIVE and torch.cuda.is_available()
 
 
 def require_native(what: str) -> None:
     if not _HAS_NATIVE:
-        raise RuntimeError(f"{what}: the native sm_100a runtime (_C.so with CUDA kernels) is missing; "
+        raise RuntimeError(f"{what}: the native sm_90a runtime (_C.so with CUDA kernels) is missing; "
                            "run `python -m pytorch_distributed_train_b200._build`")
     if not torch.cuda.is_available():
         raise RuntimeError(f"{what}: no CUDA device available")

@@ -1,4 +1,4 @@
-"""Autograd bindings for the sm_100a kernels in ``_C`` (csrc/cuda/ops_simt.cu, conv_tcgen05.cu).
+"""Autograd bindings for the sm_90a kernels in ``_C`` (csrc/cuda/ops_simt.cu, conv_tcgen05.cu).
 
 Layout convention: activations between fused layers are NHWC in memory and are handed to PyTorch
 as ``channels_last`` tensors (logical NCHW shape), so module hooks / user code see ordinary tensors.
@@ -8,7 +8,7 @@ Gradient placement: when a parameter's ``.grad`` is ``None`` at backward time (t
 (``param._pdt_grad_view``), the weight-gradient kernels write **directly into the DDP bucket** and
 return an alias of that view; autograd adopts it as ``.grad`` and the reducer finds the gradient
 already in place — no per-parameter copy or scale kernels (the reference path spends ~20 tiny kernels
-per step there, SURVEY §2.5 K19).
+per step there).
 """
 from __future__ import annotations
 
@@ -254,7 +254,7 @@ class _FusedLayer1(torch.autograd.Function):
 
 
 class _FusedLayer2(torch.autograd.Function):
-    """conv2 (tcgen05) + BN2 + ReLU + pool2 (+ the classifier's logits, which ride on the pooled activations while they
+    """conv2 (wgmma) + BN2 + ReLU + pool2 (+ the classifier's logits, which ride on the pooled activations while they
     are still in shared memory) forward; pool/ReLU/BN backward + conv2 data gradient as one kernel backward.  The
     tensor-core weight gradient follows as its own kernel, or — the default — rides on layer 1's backward kernel."""
 
@@ -371,7 +371,7 @@ def conv_bn_relu_pool(x: torch.Tensor, conv: torch.nn.Conv2d, bn: torch.nn.Modul
     if conv.kernel_size != (5, 5) or conv.stride != (1, 1) or conv.padding != (2, 2) or conv.groups != 1:
         raise ValueError("conv_bn_relu_pool: only 5x5 / stride 1 / pad 2 convolutions are fused")
     if impl == "auto":
-        impl = os.environ.get("PDT_CONV_IMPL", "auto")  # auto = tcgen05 where implemented, SIMT elsewhere
+        impl = os.environ.get("PDT_CONV_IMPL", "auto")  # auto = tensor cores where implemented, SIMT elsewhere
     group = None
     training = bn.training
     if training and type(bn).__name__ == "SyncBatchNorm" and dist.is_initialized():
@@ -411,7 +411,7 @@ class _Conv5x5(torch.autograd.Function):
 
 
 def conv2d(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None, impl: str = "auto") -> torch.Tensor:
-    """5×5 / stride 1 / pad 2 convolution on our kernels (tcgen05 for 16→32 channels); returns a
+    """5×5 / stride 1 / pad 2 convolution on our kernels (tensor cores for 16→32 channels); returns a
     channels_last tensor."""
     return _Conv5x5.apply(x, weight, bias, impl)
 

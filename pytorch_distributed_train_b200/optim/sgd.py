@@ -2,9 +2,9 @@
 
 The reference uses ``torch.optim.SGD(model.parameters(), 1e-4)`` (ref: ddp_example.py:62,90,92),
 i.e. ``p -= lr·g`` through a foreach kernel, with ``zero_grad()`` dropping the gradients so
-autograd re-allocates them every backward (SURVEY §2.2 B17).  Ours:
+autograd re-allocates them every backward.  Ours:
 
-* the update for *all* parameters is one sm_100a kernel launch (``ops.sgd_step``) over a pointer
+* the update for *all* parameters is one sm_90a kernel launch (``ops.sgd_step``) over a pointer
   table — momentum, dampening, Nesterov and weight decay included — so it is graph-capturable
   and launch-count-free as the model grows;
 * ``lr`` lives in a device scalar when ``capturable=True`` so schedulers work under CUDA graphs;

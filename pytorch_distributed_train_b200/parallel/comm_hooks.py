@@ -3,7 +3,7 @@
 Interface parity: ``ddp.register_comm_hook(state, hook)`` with
 ``hook(state, bucket: GradBucket) -> Future[Tensor]`` (torch c10d comm.hpp:20-118,
 ddp_comm_hooks/default_hooks.py:35-175).  The bucket a hook receives holds *undivided* local
-gradients (observed behaviour of the reference stack, SURVEY App. B); the hook owns the
+gradients (observed behaviour of the reference stack); the hook owns the
 averaging.  The reference script itself installs no hook (ref: ddp_example.py:64) — the built-in
 path is the fused reduce kernel — so these are the optional surface.
 """

@@ -13,7 +13,7 @@ device_ids=[gpu])`` (ref: ddp_example.py:64; behaviour per torch/nn/parallel/dis
 * ``no_sync()``, ``register_comm_hook``, ``join()``, ``find_unused_parameters``, ``static_graph``,
   ``gradient_as_bucket_view``, ``bucket_cap_mb``, ``broadcast_buffers`` are supported.
 
-What is different (B200-first):
+What is different (H100-first):
 
 * the reducer is our own C++ (``_C.Reducer``); gradients live inside the bucket
   (``gradient_as_bucket_view=True`` by default) and on the NVLink backend the bucket is peer-mapped

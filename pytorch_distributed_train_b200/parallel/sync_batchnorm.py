@@ -11,7 +11,7 @@ peer-memory kernel with no host synchronisation, so the whole step stays CUDA-gr
 Backward all-reduces ``(Σdy, Σdy·(x-μ))`` exactly like the reference; ``dγ``/``dβ`` are left to
 DDP's bucket reduce.
 
-On CUDA the per-channel reductions and the elementwise passes run as our sm_100a kernels
+On CUDA the per-channel reductions and the elementwise passes run as our sm_90a kernels
 (``ops.bn_*``); on CPU the same math runs through torch ops so the logic is testable without a
 GPU (torch's own SyncBatchNorm refuses CPU tensors).
 """

@@ -1,4 +1,4 @@
-"""Checkpoint / resume (SURVEY §5.4).
+"""Checkpoint / resume.
 
 The reference saves nothing — the trained model is discarded at process exit (ref: ddp_example.py:96-97) —
 but a user switching from torch's DDP expects the usual surface to work: ``state_dict()`` keys carry the

@@ -1,7 +1,7 @@
-"""Sample SM clocks / throttle reasons *during* a timed region (B200_PROFILING.md "clocks line").
+"""Sample SM clocks / throttle reasons *during* a timed region.
 
 Primary source: NVML in-process (``pynvml``), polled every couple of milliseconds by a background
-thread — a 200-step timed region of the ConvNet lasts ~35 ms, far less than one ``nvidia-smi -lms``
+thread — a 200-step timed region of the ConvNet lasts tens of milliseconds, far less than one ``nvidia-smi -lms``
 period plus its start-up time.  Fallback: one long-lived ``nvidia-smi -lms`` process.
 ``summary()`` gives the JSON block bench.py prints."""
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""NVTX ranges (no-ops without CUDA) so phases show up in ncu/nsys timelines (SURVEY §5.1)."""
+"""NVTX ranges (no-ops without CUDA) so phases show up in ncu/nsys timelines."""
 from __future__ import annotations
 
 from contextlib import contextmanager

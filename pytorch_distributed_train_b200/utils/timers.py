@@ -55,7 +55,7 @@ _FLUSH = {}
 
 
 def l2_flush(device=None, nbytes: int = 256 << 20) -> None:
-    """Evict L2 (126 MB on B200) by overwriting a buffer larger than it."""
+    """Evict L2 (50 MB on H100) by overwriting a buffer larger than it."""
     if not torch.cuda.is_available():
         return
     dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)

@@ -1,4 +1,4 @@
-"""Host watchdog (SURVEY §5.3): the reference inherits NCCL's watchdog/heartbeat threads; ours is a
+"""Host watchdog: the reference inherits NCCL's watchdog/heartbeat threads; ours is a
 small thread that (a) publishes a heartbeat key in the store, (b) notices peers whose heartbeat
 stops and (c) aborts this process with a diagnostic (flight-recorder dump) instead of letting a
 device-side spin-wait hang forever.  Device-side waits additionally carry their own

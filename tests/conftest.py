@@ -17,7 +17,7 @@ _build.build()
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with `-m gpu` on a B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with `-m gpu` on an H100 box)")
     config.addinivalue_line("markers", "multigpu: needs >= 2 CUDA devices")
 
 

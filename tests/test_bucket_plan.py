@@ -1,4 +1,4 @@
-"""Bucket planner vs torch's _compute_bucket_assignment_by_size (oracle) — SURVEY §4.3."""
+"""Bucket planner vs torch's _compute_bucket_assignment_by_size (oracle)."""
 import sys
 
 import torch
@@ -33,7 +33,7 @@ def test_matches_torch_on_resnet18_forward_and_rebuilt_order():
     assert ours_r == ref_r
     sizes = [sum(ps[i].numel() * 4 for i in b) for b in ours_r]
     assert [len(b) for b in ours_r] == [2, 12, 48]
-    assert sizes == [2052000, 28852224, 15853824]  # SURVEY App. B
+    assert sizes == [2052000, 28852224, 15853824]  # torch DDP's plan for ResNet-18
 
 
 def test_mixed_dtypes_split():

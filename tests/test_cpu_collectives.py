@@ -188,7 +188,7 @@ def _debug_detail(rank, world):
 
 
 def test_debug_detail_names_mismatched_collectives_and_nan_check():
-    """SURVEY §5.2: collective fingerprint check + NaN check instead of a hang / silent corruption."""
+    """Collective fingerprint check + NaN check instead of a hang / silent corruption."""
     for msg, nan_msg in run_ranks(_debug_detail, 2):
         assert "collective mismatch at sequence number 2" in msg and "all_reduce" in msg and "broadcast" in msg
         assert "non-finite" in nan_msg

@@ -74,7 +74,7 @@ def test_cli_flags_match_reference():
     b = p.parse_args(["-g", "4", "--epochs", "3", "--backend", "gloo", "--syncbn"])
     assert (b.gpus, b.epochs, b.backend, b.syncbn) == (4, 3, "gloo", True)
     assert a.batch_size == 100 and a.lr == 1e-4  # ref: ddp_example.py:59,62
-    # the extras SURVEY §5.6 asks for, with defaults that reproduce the reference's behaviour
+    # the extra flags, with defaults that reproduce the reference's behaviour
     assert (a.comm, a.algo, a.data, a.model, a.steps, a.graph) == ("fused", "auto", "synthetic", "convnet", 0, False)
     assert p.parse_args(["--algo", "nvls", "--comm", "nccl", "--model", "resnet18"]).algo == "nvls"
 

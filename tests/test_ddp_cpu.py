@@ -1,5 +1,5 @@
 """DDP end-to-end on the CPU backend, world_size=2 (BASELINE.json config 1), with
-torch DDP + gloo as the oracle (SURVEY §4.3 integration tests a-d)."""
+torch DDP + gloo as the oracle."""
 import io
 import os
 
@@ -90,7 +90,7 @@ def test_matches_torch_ddp_gloo():
     info = a["info"]
     assert info["bucket_sizes"] == [116136] and info["total_parameter_size_bytes"] == 116136
     assert info["has_rebuilt_buckets"] and info["num_parameter_tensors"] == 10
-    # grad-ready order observed for the reference model (SURVEY App. B)
+    # grad-ready order observed for the reference model
     assert info["grad_ready_order"] == [9, 8, 6, 7, 4, 5, 2, 3, 0, 1]
     assert info["bucket_indices"] == [[9, 8, 6, 7, 4, 5, 2, 3, 0, 1]]
     assert info["world_size"] == 2 and info["module_name"] == "ConvNet"
@@ -413,7 +413,7 @@ def test_optimizer_fused_allreduce_matches_reducer_path(momentum):
 
 def _ckpt(rank, world, path, fuse):
     """Train 2 steps, checkpoint, train 2 more — versus a fresh process state restored from the checkpoint and
-    trained for the same 2 steps: identical parameters and momentum (SURVEY §5.4)."""
+    trained for the same 2 steps: identical parameters and momentum."""
     def fresh():
         torch.manual_seed(0)
         model = pdt.models.ConvNet()

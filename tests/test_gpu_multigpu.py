@@ -1,5 +1,5 @@
 """Multi-GPU tests of the NVLink backend (SymmComm) against NCCL / closed-form results, and of DDP /
-SyncBatchNorm end to end against the torch stack (SURVEY §4.3 "GPU distributed tests")."""
+SyncBatchNorm end to end against the torch stack."""
 import os
 
 import pytest
@@ -169,7 +169,7 @@ def test_ddp_convnet_matches_torch_ddp_nccl(syncbn):
     for r in res:
         assert max(abs(a - b) for a, b in zip(r["ours"], r["theirs"])) < 5e-3, (r["ours"], r["theirs"])
         # conv weight gradients behind a BatchNorm are ill-conditioned: TF32 (ours) vs fp32 cuDNN differ by up to
-        # 3.7e-2 of the max entry, the same as cuDNN-TF32 vs float64 (profiles/numerics.md, tables 1 and 3)
+        # 3.7e-2 of the max entry, the same as cuDNN-TF32 vs float64
         assert r["param_rel"] < 5e-2 and r["buf_abs"] < 5e-3, r
         assert r["copies"] == 0 and sum(r["buckets"]) == 116136
 
@@ -182,13 +182,13 @@ def _resnet(rank, world, syncbn, port):
     steps = 3
     # fp32 convolutions in both arms: with TF32 operand rounding a 1e-7 difference between our SyncBN arithmetic (fp64 sums) and
     # torch's (Welford) flips roundings in the next convolution, and layer4's BatchNorm over 4·2·2·world samples amplifies that to
-    # several percent of the gradient — a property of the comparison, not of either implementation (profiles/numerics.md §2)
+    # several percent of the gradient — a property of the comparison, not of either implementation
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
 
     def data(s):
         # seeds 77·(s+1)+rank: the batch of tools/numerics_probe.py.  With seed = rank the same comparison is off by up to 20 % in
-        # layer4 for OUR kernels and for our torch-op fallback math alike (profiles/r2/numerics_probe_r2.log, "resnet@test"): 8 samples
+        # layer4 for OUR kernels and for our torch-op fallback math alike: 8 samples
         # per rank reach layer4's BatchNorm at 2×2 resolution, and channels that are (almost) constant after the ReLU get
         # invstd = 1/sqrt(eps) = 316 — two correct ways of summing (fp64 Σx, Σx² here, Welford in torch) then disagree visibly.
         g = torch.Generator().manual_seed(77 * (s + 1) + rank)
@@ -390,7 +390,7 @@ def _absent_rank(rank, world, init, outdir):
 
 
 def test_absent_rank_trips_the_device_side_timeout(tmp_path):
-    """SURVEY §5.3: a rank that never joins a collective must produce a diagnostic within the
+    """A rank that never joins a collective must produce a diagnostic within the
     configured timeout on every waiting rank, not a hang."""
     import json
 
@@ -404,7 +404,7 @@ def test_absent_rank_trips_the_device_side_timeout(tmp_path):
 
 
 def _stress(rank, world):
-    """SURVEY §4.3 stress: 10k back-to-back collectives with randomised per-rank stream delays — the
+    """Stress: 10k back-to-back collectives with randomised per-rank stream delays — the
     flag/epoch protocol must neither deadlock nor let a fast rank overwrite a slot a slow rank is reading."""
     import random
 

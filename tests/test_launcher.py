@@ -1,4 +1,4 @@
-"""Launcher contract (ref: ddp_example.py:111; spawn.py:79-96,145-211; SURVEY §4.3)."""
+"""Launcher contract (ref: ddp_example.py:111; spawn.py:79-96,145-211)."""
 import os
 import signal
 import time

@@ -1,5 +1,5 @@
 """DistributedSampler index math vs torch.utils.data.DistributedSampler as the oracle
-(ref: ddp_example.py:70-72; SURVEY §4.3)."""
+(ref: ddp_example.py:70-72)."""
 import itertools
 
 import pytest
@@ -43,7 +43,7 @@ def test_shards_partition_dataset():
 
 
 def test_steps_per_epoch_match_reference():
-    # 600/300/150/75 steps at 1/2/4/8 GPUs with batch 100 (SURVEY App. B)
+    # 600/300/150/75 steps at 1/2/4/8 GPUs with batch 100
     ds = SyntheticMNIST(60000)
     for w, steps in [(1, 600), (2, 300), (4, 150), (8, 75)]:
         s = DistributedSampler(ds, w, 0)

@@ -1,4 +1,4 @@
-"""Store family (ref surface: TCPStore.hpp:83-121 op list; SURVEY §4.3 unit tests)."""
+"""Store family (ref surface: TCPStore.hpp:83-121 op list)."""
 import os
 import threading
 import time

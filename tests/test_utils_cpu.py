@@ -1,4 +1,4 @@
-"""Auxiliary subsystems on the CPU box: watchdog (SURVEY §5.3), rank-aware logging (§5.5), NVTX no-op (§5.1),
+"""Auxiliary subsystems on the CPU box: watchdog, rank-aware logging, NVTX no-op,
 clock sampler fallback, device-timer helpers that must degrade gracefully without a GPU."""
 import json
 import os

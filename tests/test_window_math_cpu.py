@@ -35,7 +35,7 @@ def window_wgrad(x_frames: torch.Tensor, dy_frames: torch.Tensor) -> torch.Tenso
         frame0 = n * FRAME
         window = view[frame0:frame0 + 6 * 64]                          # six 64-row TMA boxes = the A window in smem
         btile = torch.cat([dyf, torch.zeros(512, 32, dtype=dyf.dtype)])[frame0 + FIRST:frame0 + FIRST + 256]   # two 128-row boxes
-        acc = torch.zeros(4, 128, 32, dtype=xf.dtype)                  # four TMEM accumulators [M = 128][N = 32]
+        acc = torch.zeros(4, 128, 32, dtype=xf.dtype)                  # four accumulators [M = 128][N = 32]
         for mt in range(4):
             shift0 = (0 - 2) * 18 + 2 * mt - 2 if mt < 3 else 2 * 18 - 2
             lbo_rows = 18 if mt < 3 else 2

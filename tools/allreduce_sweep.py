@@ -2,11 +2,11 @@
 """Allreduce latency / bus-bandwidth sweep: our NVLink kernels vs the libnccl baseline
 (BASELINE.json config 5: "allreduce bus-bandwidth sweep 1KB–1GB at 2/4/8 GPUs vs reference NCCL").
 
-    python tools/allreduce_sweep.py --gpus 8 [--max-mb 256] [--out gpurun_out/sweep_8.json]
+    python tools/allreduce_sweep.py --gpus 8 [--max-mb 256] [--out sweep_8.json]
 
 Every number is device-timed with CUDA events on the launching stream, after warm-up, with a
 barrier + synchronize on both sides, and is the MAX over ranks.  busbw = 2(N-1)/N · bytes / t.
-Roofline (B200_PROFILING.md): t_min = bytes_that_must_cross_NVLink / 770 GB/s per direction per GPU;
+Roofline: t_min = bytes_that_must_cross_NVLink / 450 GB/s per direction per GPU (H100 SXM, NVLink 4 data sheet);
 one-shot push sends (N-1)·S, NVLS two-shot moves ≈ S in + S out per GPU, P2P two-shot 2·S·(N-1)/N.
 """
 import argparse
@@ -17,7 +17,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-LINK_GBS = 770.0
+LINK_GBS = 450.0
 
 
 def roofline_us(algo, nbytes, n):

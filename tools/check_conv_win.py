@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Hardware check of the experimental window conv kernels (impl="win") against the SIMT oracle.
 
-    PDT_WIN_BASE_OFFSET=1 python tools/check_conv_win.py     # descriptor base offset = (start >> 7) & 7  (default)
-    PDT_WIN_BASE_OFFSET=0 python tools/check_conv_win.py     # base offset 0 (pure address-based swizzle)
+    PDT_WIN_BASE_OFFSET=0 python tools/check_conv_win.py     # base offset 0: address-based swizzle (default, correct)
+    PDT_WIN_BASE_OFFSET=1 python tools/check_conv_win.py     # descriptor base offset = (start >> 7) & 7  (wrong on Hopper)
 
 Small-integer inputs make TF32 exact, so "max err" must be 0 for a correct kernel.  Also times both variants.
 """

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""CPU emulation of the index math of the planned "window" conv2 kernel (NOTES_NEXT.md §1).
+"""CPU emulation of the index math of the planned "window" conv2 kernel (conv_tcgen05.cu).
 
 The kernel will load, per tile, ONE zero-haloed patch of the NHWC input in padded-width coordinates
 (PW = W + 4 positions per padded image row) and feed the tensor core 25 row-shifted views of that single

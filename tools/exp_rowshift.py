@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Hardware experiment for the next conv2 design (profiles/conv_tma_ncu.md §3).
+"""Hardware check of the descriptor convention the window convolutions rely on (filter taps read as row-shifted descriptors).
 
-Question: with a K-major SWIZZLE_64B / SWIZZLE_128B operand in shared memory, may the UMMA
+Question: with a K-major SWIZZLE_64B / SWIZZLE_128B operand in shared memory, may the wgmma
 descriptor start at an arbitrary ROW of a larger TMA-loaded buffer (that is what turns 25 im2col
 gathers per pixel into one tiled load of the haloed patch)?  For every shift in 0..40 and for
 descriptor base-offset = 0 (mode 0) or (start >> 7) & 7 (mode 1) the kernel computes

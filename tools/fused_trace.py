@@ -34,7 +34,7 @@ _C.fused_convnet_trace_enable(False)
 names = {0: ("forward (whole)", ["start", "conv1 done", "stats partial written", "barrier 1 passed", "pooled patch in smem", "conv2 epilogue done",
                                  "stats 2 partial written", "barrier 2 passed", "pooled 2 in smem", "logits written", "end (incl. loss)", "prologue done (smem zeroed, weights requested)"]),
          1: ("l1_bwd (+conv2 wgrad)", ["start", "partial written", "barrier passed", "folded", "conv1 wgrad partial written", "barrier 2 passed", "end",
-                                       "conv2 wgrad read out of TMEM"]),
+                                       "conv2 wgrad (mma.sync)"]),
          2: ("l2_fwd", ["start", "B built + sync", "epilogue done", "partial written", "barrier passed", "folded", "pooled out written", "end"]),
          3: ("l2_bwd", ["start", "B built", "partial written", "barrier passed", "folded", "dy written", "end"])}
 def report(t, title):

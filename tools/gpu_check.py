@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Run the GPU test groups in separate processes (a device trap in one group must not poison the
-rest) and write logs + a summary under gpurun_out/.  Usage: python tools/gpu_check.py [group ...]"""
+rest) and write logs + a summary under tool_out/.  Usage: python tools/gpu_check.py [group ...]"""
 import json
 import os
 import subprocess
@@ -8,7 +8,7 @@ import sys
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-OUT = os.path.join(ROOT, "gpurun_out")
+OUT = os.path.join(ROOT, "tool_out")
 os.makedirs(OUT, exist_ok=True)
 
 GROUPS = {

@@ -124,7 +124,7 @@ def worker(rank, world, port):
             nn.functional.cross_entropy(net(x), y).backward()
             return {n: rel(p.grad.double(), oracle[n]) for n, p in net.named_parameters() if oracle[n].abs().max() > 1e-6}
 
-        out["precision_vs_fp64|ours(tf32 tcgen05 conv2)"] = arm(True, False)
+        out["precision_vs_fp64|ours(tf32 tensor-core conv2)"] = arm(True, False)
         out["precision_vs_fp64|torch cudnn allow_tf32=True (reference default)"] = arm(False, True)
         out["precision_vs_fp64|torch cudnn allow_tf32=False"] = arm(False, False)
         torch.backends.cudnn.allow_tf32 = False

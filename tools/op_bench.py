@@ -5,9 +5,9 @@ log-softmax + NLL, foreach SGD) — same box, same shapes (batch 100), same meth
 
 * every row is timed as a CUDA graph of REPS back-to-back launches (CUDA events around the replay, ÷ REPS), i.e. what
   the op costs inside a captured step, launch gap included, host overhead excluded — for both arms;
-* "cold" rows additionally overwrite a 256 MB buffer (> 126 MB L2) before a single eager launch.
+* "cold" rows additionally overwrite a 256 MB buffer (> 50 MB L2) before a single eager launch.
 
-Writes gpurun_out/op_bench.json and prints a table; tools/roofline_report.py turns it into profiles/*.md.
+Writes tool_out/op_bench.json and prints a table.
 """
 import json
 import os
@@ -106,9 +106,9 @@ def main():
     grads = [torch.randn_like(p) for p in params]
     dflat = torch.randn(B, 32, 7, 7, device=dev)
     ours = [
-        ("forward: conv1+BN+ReLU+pool + conv2(tcgen05)+BN+ReLU+pool + fc + cross-entropy (1 kernel)", fwd_whole),
-        ("backward A: classifier bwd + pool/ReLU/BN2 bwd + conv2 dgrad(tcgen05) (1 kernel)", l2_bwd_fc),
-        ("backward B: pool/ReLU/BN1 bwd + conv1 wgrad(mma.sync) + conv2 wgrad(tcgen05, window) (1 kernel)",
+        ("forward: conv1+BN+ReLU+pool + conv2(wgmma)+BN+ReLU+pool + fc + cross-entropy (1 kernel)", fwd_whole),
+        ("backward A: classifier bwd + pool/ReLU/BN2 bwd + conv2 dgrad(wgmma) (1 kernel)", l2_bwd_fc),
+        ("backward B: pool/ReLU/BN1 bwd + conv1 wgrad(mma.sync) + conv2 wgrad(mma.sync, window) (1 kernel)",
          lambda: _C.convnet_l1_bwd_wgrad(dp1, y1, x, sv1, g1, be1, dg1, dbe1, dw1, db1, dy2, p1, dysum, dw2, db2)),
         ("SGD, 10 tensors (1 kernel)", lambda: _C.sgd_multi(params, grads, [], 1e-4, None, 0.0, 0.0, 0.0, False, False, False)),
         ("(variant) cross-entropy fwd (+dlogits) as its own kernel", lambda: _C.cross_entropy_fwd(logits, tgt, True)),
@@ -176,8 +176,8 @@ def main():
     print(f"floor    {floor['us_in_graph']:8.2f} us in-graph   {floor['us_cold_eager']:8.2f} us cold eager   {floor['op']}")
     t_ours = sum(r["us_in_graph"] for r in rows if r["arm"] == "ours" and r["us_in_graph"] and not r["op"].startswith("(variant)"))
     print(f"ours, sum of the step's kernels in-graph: {t_ours:.1f} us")
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "op_bench.json"), "w") as f:
+    os.makedirs(os.path.join(ROOT, "tool_out"), exist_ok=True)
+    with open(os.path.join(ROOT, "tool_out", "op_bench.json"), "w") as f:
         json.dump(rows, f, indent=1)
 
 
