@@ -7,7 +7,7 @@
 #include <map>
 #include <mutex>
 
-#include "conv_tcgen05.h"
+#include "conv_wgmma.h"
 #include "fused_convnet.h"
 #include "cuda_comm.h"
 #include "cuda_utils.h"
@@ -66,13 +66,19 @@ ReduceScratch scratch(const at::Tensor& like) {
   return r;
 }
 
-// The tensor-core weight gradient is the default; PDT_WGRAD_TCGEN05=0 selects the SIMT kernel instead.
-bool wgrad_tcgen05_default() {
-  static const bool on = [] {
-    const char* e = getenv("PDT_WGRAD_TCGEN05");
-    return !(e && e[0] == '0');
-  }();
-  return on;
+// Kernel family of the per-op conv2, selected by the `impl` argument of the conv5x5_* bindings:
+//   auto, tma → TMA-im2col wgmma forward / data gradient;
+//   tcgen05   → the cp.async-gather wgmma kernel for forward / data gradient;
+//   simt      → the CUDA-core kernels for all three.
+// Both tensor-core choices compute the weight gradient with the mma.sync split-K kernel.  Shapes the tensor-core kernels
+// do not cover (conv1: K = 25) always take SIMT.
+enum class ConvImpl { kIm2col, kGather, kSimt };
+
+ConvImpl conv_impl(const std::string& impl) {
+  if (impl == "auto" || impl == "tma") return ConvImpl::kIm2col;
+  if (impl == "tcgen05") return ConvImpl::kGather;
+  TORCH_CHECK(impl == "simt", "conv5x5: impl must be one of auto, tma, tcgen05, simt (got '", impl, "')");
+  return ConvImpl::kSimt;
 }
 
 ConvShape conv_shape(const at::Tensor& x_nhwc, const at::Tensor& w) {
@@ -138,6 +144,7 @@ void register_cuda_bindings(py::module_& m) {
   // ---- convolution ---------------------------------------------------------------------------------
   m.def("conv5x5_fwd", [](const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> bias, bool want_stats, const std::string& impl,
                           bool zero_pad) {
+    const ConvImpl family = conv_impl(impl);
     chk(x, "x"); chk(w, "w");
     c10::cuda::CUDAGuard g(x.device());
     ConvShape s = conv_shape(x, w);
@@ -148,47 +155,35 @@ void register_cuda_bindings(py::module_& m) {
     // padded temporary (3 extra kernels)
     at::Tensor stats_full = !want_stats ? at::Tensor() : (zero_pad ? at::zeros({2 * s.Cout + 4}, x.options()) : at::empty({2 * s.Cout + 4}, x.options()));
     at::Tensor stats = want_stats ? stats_full.narrow(0, 0, 2 * s.Cout + 1) : at::Tensor();
-    // auto / tma → fully TMA-fed tcgen05 kernel; tcgen05 → cp.async-gather tcgen05 kernel; simt → CUDA cores.
-    // Shapes the tensor-core kernels do not cover (conv1: K = 25) always take the SIMT kernel.
-    const bool sup = conv_tcgen05_supported(s);
-    const bool tc = sup && impl == "tcgen05";
-    if (sup && impl == "win")  // experimental window kernel: explicit opt-in only
-      launch_conv5x5_fwd_win(x.data_ptr<float>(), w.data_ptr<float>(), opt_ptr(bias, "bias"), y.data_ptr<float>(),
-                             want_stats ? stats.data_ptr<float>() : nullptr, s, scratch(x), cur_stream(x));
-    else if (sup && (impl == "tma" || impl == "auto")) launch_conv5x5_fwd_tma(x.data_ptr<float>(), w.data_ptr<float>(), opt_ptr(bias, "bias"), y.data_ptr<float>(),
-                                              want_stats ? stats.data_ptr<float>() : nullptr, s, scratch(x), cur_stream(x));
-    else if (tc) launch_conv5x5_fwd_tcgen05(x.data_ptr<float>(), w.data_ptr<float>(), opt_ptr(bias, "bias"), y.data_ptr<float>(),
-                                       want_stats ? stats.data_ptr<float>() : nullptr, s, scratch(x), cur_stream(x));
-    else launch_conv5x5_fwd(x.data_ptr<float>(), w.data_ptr<float>(), opt_ptr(bias, "bias"), y.data_ptr<float>(),
-                            want_stats ? stats.data_ptr<float>() : nullptr, s, scratch(x), cur_stream(x));
+    const ConvImpl k = conv_wgmma_supported(s) ? family : ConvImpl::kSimt;
+    auto launch = k == ConvImpl::kIm2col ? launch_conv5x5_fwd_im2col : k == ConvImpl::kGather ? launch_conv5x5_fwd_gather : launch_conv5x5_fwd;
+    launch(x.data_ptr<float>(), w.data_ptr<float>(), opt_ptr(bias, "bias"), y.data_ptr<float>(), want_stats ? stats.data_ptr<float>() : nullptr, s,
+           scratch(x), cur_stream(x));
     return py::make_tuple(y, stats);  // stats is a view of the first 2C+1 entries of the zero-padded vector
   }, py::arg("x"), py::arg("w"), py::arg("bias") = py::none(), py::arg("want_stats") = true, py::arg("impl") = "auto",
      py::arg("zero_pad") = false);
 
   m.def("conv5x5_dgrad", [](const at::Tensor& dy, const at::Tensor& w, const std::string& impl) {
+    const ConvImpl family = conv_impl(impl);
     chk(dy, "dy"); chk(w, "w");
     c10::cuda::CUDAGuard g(dy.device());
     ConvShape s = conv_shape(dy, w);
     s.Cin = static_cast<int>(w.size(1));
     TORCH_CHECK(dy.size(3) == s.Cout, "conv5x5_dgrad: dy channels must equal weight Cout");
     at::Tensor dx = at::empty({s.B, s.H, s.W, s.Cin}, dy.options());
-    const bool sup = conv_tcgen05_supported(s);
-    const bool tc = sup && impl == "tcgen05";
-    if (sup && impl == "win") launch_conv5x5_dgrad_win(dy.data_ptr<float>(), w.data_ptr<float>(), dx.data_ptr<float>(), s, cur_stream(dy));
-    else if (sup && (impl == "tma" || impl == "auto")) launch_conv5x5_dgrad_tma(dy.data_ptr<float>(), w.data_ptr<float>(), dx.data_ptr<float>(), s, cur_stream(dy));
-    else if (tc) launch_conv5x5_dgrad_tcgen05(dy.data_ptr<float>(), w.data_ptr<float>(), dx.data_ptr<float>(), s, cur_stream(dy));
-    else launch_conv5x5_dgrad(dy.data_ptr<float>(), w.data_ptr<float>(), dx.data_ptr<float>(), s, cur_stream(dy));
+    const ConvImpl k = conv_wgmma_supported(s) ? family : ConvImpl::kSimt;
+    auto launch = k == ConvImpl::kIm2col ? launch_conv5x5_dgrad_im2col : k == ConvImpl::kGather ? launch_conv5x5_dgrad_gather : launch_conv5x5_dgrad;
+    launch(dy.data_ptr<float>(), w.data_ptr<float>(), dx.data_ptr<float>(), s, cur_stream(dy));
     return dx;
   }, py::arg("dy"), py::arg("w"), py::arg("impl") = "auto");
 
   m.def("conv5x5_wgrad", [](const at::Tensor& dy, const at::Tensor& x, at::Tensor dw, c10::optional<at::Tensor> db, const std::string& impl) {
+    const ConvImpl family = conv_impl(impl);
     chk(dy, "dy"); chk(x, "x"); chk(dw, "dw");
     c10::cuda::CUDAGuard g(dy.device());
     ConvShape s = conv_shape(x, dw);
-    const bool sup = conv_tcgen05_supported(s);
-    const bool tc = sup && (impl == "tcgen05" || ((impl == "auto" || impl == "tma" || impl == "win") && wgrad_tcgen05_default()));
-    if (tc) launch_conv5x5_wgrad_tcgen05(dy.data_ptr<float>(), x.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"), s, scratch(x), cur_stream(x));
-    else launch_conv5x5_wgrad(dy.data_ptr<float>(), x.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"), s, scratch(x), cur_stream(x));
+    auto launch = conv_wgmma_supported(s) && family != ConvImpl::kSimt ? launch_conv5x5_wgrad_mma : launch_conv5x5_wgrad;
+    launch(dy.data_ptr<float>(), x.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"), s, scratch(x), cur_stream(x));
   }, py::arg("dy"), py::arg("x"), py::arg("dw"), py::arg("db") = py::none(), py::arg("impl") = "auto");
 
   // ---- cooperative fused ConvNet layers (fused_convnet.cu): one CTA per image, grid barrier for the batch statistics ----
@@ -605,22 +600,12 @@ void register_cuda_bindings(py::module_& m) {
   });
 
   // ---- TF32 wgmma GEMM self-test (D[M,N] = A[M,K]·B[N,K]^T) — validates descriptors/TMA/accumulator layout ---
-  m.def("umma_rowshift_probe", [](const at::Tensor& a, const at::Tensor& b, int64_t shift, int64_t mode) {
-    chk(a, "a"); chk(b, "b");
-    TORCH_CHECK(a.dim() == 2 && a.size(0) == 256 && (a.size(1) == 16 || a.size(1) == 32) && b.dim() == 2 && b.size(0) == 32 &&
-                    b.size(1) == a.size(1), "umma_rowshift_probe: a [256, 16|32], b [32, same]");
-    c10::cuda::CUDAGuard g(a.device());
-    at::Tensor d = at::empty({128, 32}, a.options());
-    launch_umma_rowshift_probe(a.data_ptr<float>(), b.data_ptr<float>(), d.data_ptr<float>(), static_cast<int>(a.size(1)) * 4,
-                               static_cast<int>(shift), static_cast<int>(mode), cur_stream(a));
-    return d;
-  });
-  m.def("gemm_tf32_tcgen05", [](const at::Tensor& a, const at::Tensor& b) {
+  m.def("gemm_tf32_wgmma", [](const at::Tensor& a, const at::Tensor& b) {
     chk(a, "a"); chk(b, "b");
     c10::cuda::CUDAGuard g(a.device());
     TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && a.size(1) == b.size(1), "gemm_tf32: A [M,K], B [N,K]");
     at::Tensor d = at::empty({a.size(0), b.size(0)}, a.options());
-    launch_gemm_tf32_tcgen05(a.data_ptr<float>(), b.data_ptr<float>(), d.data_ptr<float>(), a.size(0), b.size(0), a.size(1), cur_stream(a));
+    launch_gemm_tf32_wgmma(a.data_ptr<float>(), b.data_ptr<float>(), d.data_ptr<float>(), a.size(0), b.size(0), a.size(1), cur_stream(a));
     return d;
   });
 }

@@ -3,8 +3,6 @@
 #include <atomic>
 #include <mutex>
 
-#include "symm_device.h"
-
 namespace pdt {
 
 namespace {
@@ -68,6 +66,25 @@ void mark_process_exiting() { g_exiting.store(true); }
 bool process_exiting() { return g_exiting.load(); }
 void count_kernel_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 long long kernel_launch_count() { return g_launches.load(std::memory_order_relaxed); }
+
+void check_launch(const char* what) {
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) throw std::runtime_error(std::string("launch of ") + what + " failed: " + cudaGetErrorString(e));
+  count_kernel_launch();
+}
+
+int sm_count() {
+  constexpr int kMaxDevices = 64;
+  static std::atomic<int> cached[kMaxDevices];   // 0 = not queried yet
+  int dev = 0;
+  PDT_CUDA_CHECK(cudaGetDevice(&dev));
+  int n = dev < kMaxDevices ? cached[dev].load(std::memory_order_relaxed) : 0;
+  if (n == 0) {
+    PDT_CUDA_CHECK(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
+    if (dev < kMaxDevices) cached[dev].store(n, std::memory_order_relaxed);
+  }
+  return n;
+}
 
 std::string cu_error(CUresult r) {
   const char* s = nullptr;

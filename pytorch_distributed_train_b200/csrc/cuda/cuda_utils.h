@@ -3,8 +3,10 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 
+#include <cstddef>
 #include <stdexcept>
 #include <string>
+#include <utility>
 
 namespace pdt {
 
@@ -56,5 +58,44 @@ std::string cu_error(CUresult r);
       throw std::runtime_error(std::string("CUDA driver error at ") + __FILE__ + ":" + std::to_string(__LINE__) + \
                                " (" #expr "): " + ::pdt::cu_error(_r));                              \
   } while (0)
+
+// Every launcher of this library reports here, so benchmarks can state how many of *our* kernels
+// ran in a timed region (during CUDA-graph capture: how many were recorded into the graph).
+void count_kernel_launch(int n = 1);
+long long kernel_launch_count();
+// Set from a Python atexit hook: destructors that would call into a dying CUDA driver skip their work.
+void mark_process_exiting();
+bool process_exiting();
+
+// Call right after a <<<...>>> launch: throws if the launch failed, counts it otherwise.
+void check_launch(const char* what);
+
+// Multiprocessor count of the current device (queried once per device).
+int sm_count();
+
+// Kernels that use more than the default 48 KB of dynamic shared memory must opt in first.
+template <typename K>
+void opt_in_smem(K kernel, size_t bytes) {
+  if (bytes > 48 * 1024) PDT_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes)));
+}
+
+// Cooperative launch: all CTAs are co-resident, so they may wait for each other at a grid barrier (grid_sync.cuh).
+template <typename... KArgs, typename... Args>
+void launch_cooperative(void (*kernel)(KArgs...), int grid, int block, size_t smem, cudaStream_t st, const char* what, Args&&... args) {
+  opt_in_smem(kernel, smem);
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(block);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeCooperative;
+  attr[0].val.cooperative = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+  if (e != cudaSuccess) throw std::runtime_error(std::string("launch of ") + what + " failed: " + cudaGetErrorString(e));
+  count_kernel_launch();
+}
 
 }  // namespace pdt

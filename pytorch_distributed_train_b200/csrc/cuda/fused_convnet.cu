@@ -28,15 +28,14 @@
 
 #include <algorithm>
 #include <cstdint>
-#include <cstdlib>
 #include <stdexcept>
 #include <string>
 
 #include "cuda_utils.h"
-#include "conv_tcgen05.h"
+#include "conv_wgmma.h"
 #include "fused_convnet.h"
 #include "grid_sync.cuh"
-#include "umma_ptx.cuh"
+#include "hopper_ptx.cuh"
 #include "wgrad_win.cuh"
 
 namespace pdt {
@@ -298,7 +297,7 @@ constexpr int kL1BwdSmem = (784 * 16 + kL1Warps * 512) * 4;
 //     adjacent taps × 16 channels), loaded ONCE (384 rows, 48 KB); the 32-row atom of tap pair (kh, kw/2) for position P is the
 //     same buffer read (kh−2)·18 + (kw−2) rows further down.  The per-CTA partial has 512 rows in four groups of four atoms:
 //     group kw/2 ∈ {0,1,2} stacks kh = 0..3 (stride 18 rows), group 3 holds kh = 4 with kw/2 = 0..2 (stride 2 rows; its fourth
-//     atom is unused).  The stand-alone kernel (conv_tcgen05.cu) orders the atoms by (kh, kw/2) instead.
+//     atom is unused).  The stand-alone kernel (conv_wgmma.cu) orders the atoms by (kh, kw/2) instead.
 // One launch and one grid barrier less than running the two kernels back to back.
 struct L1WgCfg {
   static constexpr int kThreads = kL1Threads + 32;        // + one warp: the TMA loads
@@ -660,8 +659,9 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
 // The zero-haloed input (18×18 positions × 128-byte rows, channels 16..31 zero-filled by TMA) is loaded ONCE; output
 // pixel (oh, ow) is MMA row p = oh·18 + ow of one of two M = 128 tiles (rows 0..125 ↔ oh 0..6, 126..251 ↔ oh 7..13;
 // ow ≥ 14 rows are padding), and filter tap (kh, kw) is the same buffer read through a K-major SWIZZLE_128B descriptor
-// that starts (kh·18 + kw) rows further in (swizzle phase follows the absolute address: verified on hardware by
-// tools/exp_rowshift.py).  Weights are swizzled into shared memory by the CTA itself.
+// that starts (kh·18 + kw) rows further in (the swizzle phase follows the absolute address; the bit-exact
+// tests/test_gpu_kernels.py::test_cooperative_layer2_exact_on_small_integers guards this).  Weights are swizzled into
+// shared memory by the CTA itself.
 // =====================================================================================================================
 constexpr int kL2Threads = 256;
 constexpr int kPW = 18;                          // padded width
@@ -1482,48 +1482,6 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
 // ---------------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------------
-void check_launch(const char* what) {
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("launch of ") + what + " failed: " + cudaGetErrorString(e));
-  count_kernel_launch();
-}
-
-bool cooperative_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("PDT_FUSED_COOPERATIVE");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
-
-template <typename... KArgs, typename... Args>
-void launch_coop(void (*kernel)(KArgs...), int grid, int block, size_t smem, cudaStream_t st, const char* what, Args&&... args) {
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) throw std::runtime_error(std::string("cudaFuncSetAttribute(smem) for ") + what + ": " + cudaGetErrorString(e));
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(block);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeCooperative;   // all CTAs co-resident: they wait for each other at the grid barrier
-  attr[0].val.cooperative = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = cooperative_enabled() ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
-  if (e != cudaSuccess) throw std::runtime_error(std::string("launch of ") + what + " failed: " + cudaGetErrorString(e));
-  count_kernel_launch();
-}
-
-int sm_count() {
-  int dev = 0, n = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  return n;
-}
-
 CUtensorMap make_patch_map(const float* base, int C, int W, int H, int N) {
   CUtensorMap m;
   cuuint64_t dims[4] = {static_cast<cuuint64_t>(C), static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H), static_cast<cuuint64_t>(N)};
@@ -1558,17 +1516,17 @@ void fused_convnet_trace_read(unsigned long long* host /*[4][160][12]*/) {
 void launch_convnet_l1_fwd(const float* x, const float* w, const float* bias, const float* gamma, const float* beta, float* y, float* out,
                            float* saved, float* running_mean, float* running_var, long long* nbt, float momentum, float eps, int B,
                            float* partials, GridSync gs, cudaStream_t st) {
-  launch_coop(convnet_l1_fwd_kernel, B, kL1Threads, 0, st, "convnet_l1_fwd", x, w, bias, gamma, beta, y, out, saved, running_mean, running_var, nbt,
-              momentum, eps, partials, gs);
+  launch_cooperative(convnet_l1_fwd_kernel, B, kL1Threads, 0, st, "convnet_l1_fwd", x, w, bias, gamma, beta, y, out, saved, running_mean, running_var, nbt,
+                     momentum, eps, partials, gs);
 }
 
 void launch_convnet_l1_bwd(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
                            float* dgamma, float* dbeta, float* dw, float* db, int B, float* partials, float* partials_w, GridSync gs,
                            cudaStream_t st) {
   CUtensorMap none{};
-  launch_coop(convnet_l1_bwd_kernel<false>, B, kL1Threads, static_cast<size_t>(kL1BwdSmem), st, "convnet_l1_bwd", dp, y, x, saved, gamma, beta, dgamma,
-              dbeta, dw, db, partials, partials_w, gs, none, none, static_cast<float*>(nullptr), static_cast<const float*>(nullptr),
-              static_cast<float*>(nullptr), static_cast<float*>(nullptr), SgdRider{});
+  launch_cooperative(convnet_l1_bwd_kernel<false>, B, kL1Threads, static_cast<size_t>(kL1BwdSmem), st, "convnet_l1_bwd", dp, y, x, saved, gamma, beta, dgamma,
+                     dbeta, dw, db, partials, partials_w, gs, none, none, static_cast<float*>(nullptr), static_cast<const float*>(nullptr),
+                     static_cast<float*>(nullptr), static_cast<float*>(nullptr), SgdRider{});
 }
 
 void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
@@ -1577,16 +1535,16 @@ void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* x
                                  SgdRider sgd) {
   CUtensorMap tm_x, tm_dy;
   make_wgrad_win_tmaps(x2_pad, dy2_pad, B, &tm_x, &tm_dy);
-  launch_coop(convnet_l1_bwd_kernel<true>, B, L1WgCfg::kThreads, L1WgCfg::kSmem, st, "convnet_l1_bwd_wgrad", dp, y, x, saved, gamma, beta, dgamma,
-              dbeta, dw, db, partials, partials_w, gs, tm_x, tm_dy, wpart, dysum2, dw2, db2, sgd);
+  launch_cooperative(convnet_l1_bwd_kernel<true>, B, L1WgCfg::kThreads, L1WgCfg::kSmem, st, "convnet_l1_bwd_wgrad", dp, y, x, saved, gamma, beta, dgamma,
+                     dbeta, dw, db, partials, partials_w, gs, tm_x, tm_dy, wpart, dysum2, dw2, db2, sgd);
 }
 
 void launch_convnet_l2_fwd(const float* x, const float* w, const float* bias, const float* gamma, const float* beta, float* y, float* out,
                            float* saved, float* running_mean, float* running_var, long long* nbt, float momentum, float eps,
                            const float* fcw, const float* fcb, float* logits, int ncls, int B, float* partials, GridSync gs, cudaStream_t st) {
   CUtensorMap tm_x = make_patch_map(x, 16, 18, 18, B);
-  launch_coop(convnet_l2_fwd_kernel, B, kL2Threads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_l2_fwd", tm_x, w, bias, gamma, beta, y, out,
-              saved, running_mean, running_var, nbt, momentum, eps, fcw, fcb, logits, ncls, partials, gs);
+  launch_cooperative(convnet_l2_fwd_kernel, B, kL2Threads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_l2_fwd", tm_x, w, bias, gamma, beta, y, out,
+                     saved, running_mean, running_var, nbt, momentum, eps, fcw, fcb, logits, ncls, partials, gs);
 }
 
 void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const float* g1, const float* be1, float* y1, float* p1, float* saved1,
@@ -1596,17 +1554,17 @@ void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const 
                         FusedCe ce) {
   if (logits != nullptr && ncls > 16) throw std::invalid_argument("convnet_fwd: the fused classifier handles at most 16 classes");
   if (ce.target != nullptr && logits == nullptr) throw std::invalid_argument("convnet_fwd: the fused cross-entropy needs the fused classifier");
-  launch_coop(convnet_fwd_kernel, B, kL1Threads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1, saved1, rm1, rv1,
-              nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials, gs, ce);
+  launch_cooperative(convnet_fwd_kernel, B, kL1Threads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1, saved1, rm1, rv1,
+                     nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials, gs, ce);
 }
 
 void launch_convnet_l2_bwd(const float* dout, const float* y, const float* saved, const float* gamma, const float* beta, const float* w,
                            float* dgamma, float* dbeta, float* dy, float* dx, float* dysum, int B, float* partials, GridSync gs,
                            cudaStream_t st) {
-  launch_coop(convnet_l2_bwd_kernel<false>, B, kL2Threads, static_cast<size_t>(L2BwdSmem::kTotal), st, "convnet_l2_bwd", dout, y, saved, gamma, beta, w,
-              dgamma, dbeta, dy, dx, dysum, partials, gs, static_cast<const float*>(nullptr), static_cast<const float*>(nullptr),
-              static_cast<const float*>(nullptr), static_cast<float*>(nullptr), static_cast<float*>(nullptr), 0, static_cast<const float*>(nullptr),
-              static_cast<float*>(nullptr));
+  launch_cooperative(convnet_l2_bwd_kernel<false>, B, kL2Threads, static_cast<size_t>(L2BwdSmem::kTotal), st, "convnet_l2_bwd", dout, y, saved, gamma, beta, w,
+                     dgamma, dbeta, dy, dx, dysum, partials, gs, static_cast<const float*>(nullptr), static_cast<const float*>(nullptr),
+                     static_cast<const float*>(nullptr), static_cast<float*>(nullptr), static_cast<float*>(nullptr), 0, static_cast<const float*>(nullptr),
+                     static_cast<float*>(nullptr));
 }
 
 void launch_convnet_l2_bwd_fc(const float* dlogits, const float* fcw, const float* pooled, float* dfcw, float* dfcb, int ncls, const float* y,
@@ -1614,9 +1572,9 @@ void launch_convnet_l2_bwd_fc(const float* dlogits, const float* fcw, const floa
                               float* dx, float* dysum, int B, float* partials, GridSync gs, cudaStream_t st, const float* loss_parts, float* loss_out) {
   if (ncls < 1 || ncls > 16) throw std::invalid_argument("convnet_l2_bwd_fc: 1..16 classes");
   if (B > 160) throw std::invalid_argument("convnet_l2_bwd_fc: batch too large for the staged dlogits");
-  launch_coop(convnet_l2_bwd_kernel<true>, B, kL2Threads, static_cast<size_t>(L2BwdSmem::kTotalFc), st, "convnet_l2_bwd_fc",
-              static_cast<const float*>(nullptr), y, saved, gamma, beta, w, dgamma, dbeta, dy, dx, dysum, partials, gs, dlogits, fcw, pooled, dfcw,
-              dfcb, ncls, loss_parts, loss_out);
+  launch_cooperative(convnet_l2_bwd_kernel<true>, B, kL2Threads, static_cast<size_t>(L2BwdSmem::kTotalFc), st, "convnet_l2_bwd_fc",
+                     static_cast<const float*>(nullptr), y, saved, gamma, beta, w, dgamma, dbeta, dy, dx, dysum, partials, gs, dlogits, fcw, pooled, dfcw,
+                     dfcb, ncls, loss_parts, loss_out);
 }
 
 }  // namespace pdt

@@ -6,8 +6,6 @@
 #include <cstddef>
 #include <cstdint>
 
-#include "symm_device.h"  // count_kernel_launch()
-
 namespace pdt {
 
 struct ConvShape {

@@ -4,27 +4,21 @@
 // MaxPool in one pass (no int64 pool indices: the arg-max is recomputed in backward), fused
 // log-softmax/NLL, one multi-tensor SGD launch.  All cross-CTA reductions are deterministic
 // (per-CTA partials + last-CTA fold in fixed order), so runs are bit-reproducible.
-// conv2 (88% of the FLOPs) has a tensor-core implementation in conv_tcgen05.cu; the SIMT
+// conv2 (88% of the FLOPs) has a tensor-core implementation in conv_wgmma.cu; the SIMT
 // version here is its fallback and numerical oracle.
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <cstdlib>
 #include <stdexcept>
 #include <string>
 
+#include "cuda_utils.h"
 #include "grid_fold.cuh"
 #include "ops_kernels.h"
 
 namespace pdt {
 
 namespace {
-
-void check_launch(const char* what) {
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("launch of ") + what + " failed: " + cudaGetErrorString(e));
-  count_kernel_launch();
-}
 
 // deterministic grid-wide fold: see grid_fold.cuh (two-level ticket tree, parallel row folds)
 
@@ -34,9 +28,8 @@ void check_launch(const char* what) {
 // TRANSPOSED=true computes the data gradient: weights are read as w[ci_k][co_k][24-tap].
 // =====================================================================================================
 template <int CIN, int COUT, int CPT, int TH, bool STATS, bool TRANSPOSED>
-__global__ void __launch_bounds__(TH >= 14 ? 1024 : 448) conv5x5_kernel(const float* __restrict__ x, const float* __restrict__ w,
-                                                      const float* __restrict__ bias, float* __restrict__ y, float* stats,
-                                                      ReduceScratch scr, int B, int H, int W) {
+__global__ void __launch_bounds__(448) conv5x5_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
+                                                      float* __restrict__ y, float* stats, ReduceScratch scr, int B, int H, int W) {
   constexpr int G = COUT / CPT;
   extern __shared__ __align__(16) float smem[];
   const int PW = W + 4, PH = TH + 4;
@@ -794,14 +787,6 @@ size_t conv_smem(int cin, int cout, int th, int w, int threads) {
   return (static_cast<size_t>(cin) * (th + 4) * (w + 4) + 4 + 25 * cin * cout + (threads / 32 + 1) * 2 * cout) * sizeof(float);
 }
 
-template <typename K>
-void set_smem(K kernel, size_t bytes) {
-  if (bytes > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
-    if (e != cudaSuccess) throw std::runtime_error(std::string("cudaFuncSetAttribute(smem): ") + cudaGetErrorString(e));
-  }
-}
-
 }  // namespace
 
 // ---- launchers ---------------------------------------------------------------------------------------
@@ -809,19 +794,10 @@ void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float
                         cudaStream_t st) {
   constexpr int TH = 7;
   if (s.H % TH != 0) throw std::invalid_argument("conv5x5_fwd: H must be a multiple of 7");
-  // conv1 (1→16) one-CTA-per-image variant (784 threads, 100 CTAs) instead of 400 quarter-image CTAs — kept for
-  // experiments, off by default (it was the slower of the two when the default was chosen; not re-measured on H100)
-  static const bool whole_env = [] { const char* e = getenv("PDT_CONV1_WHOLE_IMAGE"); return e && e[0] == '1'; }();
-  const bool whole_image = whole_env && s.Cin == 1 && s.Cout == 16 && s.H == 28 && s.W * 28 <= 1024;
-  const int blocks = whole_image ? s.B : s.B * (s.H / TH);
+  const int blocks = s.B * (s.H / TH);
   if (stats && (static_cast<long long>(blocks + blocks / kFoldGroup + 1) * 2 * s.Cout > scr.capacity_floats || blocks / kFoldGroup + 2 > scr.counters))
     throw std::invalid_argument("conv5x5_fwd: reduction scratch too small");
-  if (whole_image) {
-    const int threads = (28 * s.W + 31) / 32 * 32;
-    const size_t sm = conv_smem(1, 16, 28, s.W, threads);
-    if (stats) conv5x5_kernel<1, 16, 16, 28, true, false><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, scr, s.B, s.H, s.W);
-    else conv5x5_kernel<1, 16, 16, 28, false, false><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, scr, s.B, s.H, s.W);
-  } else if (s.Cin == 1 && s.Cout == 16) {
+  if (s.Cin == 1 && s.Cout == 16) {
     const int threads = (TH * s.W + 31) / 32 * 32;
     const size_t sm = conv_smem(1, 16, TH, s.W, threads);
     if (stats) conv5x5_kernel<1, 16, 16, TH, true, false><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, scr, s.B, s.H, s.W);
@@ -829,8 +805,8 @@ void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float
   } else if (s.Cin == 16 && s.Cout == 32) {
     const int threads = (TH * s.W * 4 + 31) / 32 * 32;
     const size_t sm = conv_smem(16, 32, TH, s.W, threads);
-    set_smem(conv5x5_kernel<16, 32, 8, TH, true, false>, sm);
-    set_smem(conv5x5_kernel<16, 32, 8, TH, false, false>, sm);
+    opt_in_smem(conv5x5_kernel<16, 32, 8, TH, true, false>, sm);
+    opt_in_smem(conv5x5_kernel<16, 32, 8, TH, false, false>, sm);
     if (stats) conv5x5_kernel<16, 32, 8, TH, true, false><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, scr, s.B, s.H, s.W);
     else conv5x5_kernel<16, 32, 8, TH, false, false><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, scr, s.B, s.H, s.W);
   } else {
@@ -846,7 +822,7 @@ void launch_conv5x5_dgrad(const float* dy, const float* w, float* dx, ConvShape 
   const int blocks = s.B * (s.H / TH);
   const int threads = (TH * s.W * 2 + 31) / 32 * 32;
   const size_t sm = conv_smem(32, 16, TH, s.W, threads);
-  set_smem(conv5x5_kernel<32, 16, 8, TH, false, true>, sm);
+  opt_in_smem(conv5x5_kernel<32, 16, 8, TH, false, true>, sm);
   conv5x5_kernel<32, 16, 8, TH, false, true><<<blocks, threads, sm, st>>>(dy, w, nullptr, dx, nullptr, ReduceScratch{}, s.B, s.H, s.W);
   check_launch("conv5x5_dgrad");
 }
@@ -854,24 +830,17 @@ void launch_conv5x5_dgrad(const float* dy, const float* w, float* dx, ConvShape 
 void launch_conv5x5_wgrad(const float* dy, const float* x, float* dw, float* db, ConvShape s, ReduceScratch scr, cudaStream_t st) {
   constexpr int TH = 7;
   if (s.H % TH != 0) throw std::invalid_argument("conv5x5_wgrad: H must be a multiple of 7");
-  static const bool whole_env = [] { const char* e = getenv("PDT_CONV1_WHOLE_IMAGE"); return e && e[0] == '1'; }();
-  const bool whole_image = whole_env && s.Cin == 1 && s.Cout == 16 && s.H == 28;  // one CTA per image (opt-in, see launch_conv5x5_fwd)
-  const int blocks = whole_image ? s.B : s.B * (s.H / TH);
+  const int blocks = s.B * (s.H / TH);
   const int width = 25 * s.Cin * s.Cout + s.Cout;
   if (static_cast<long long>(blocks) * width > scr.capacity_floats) throw std::invalid_argument("conv5x5_wgrad: reduction scratch too small");
-  const size_t xs_f = static_cast<size_t>(s.Cin) * ((whole_image ? 28 : TH) + 4) * (s.W + 4);
-  if (whole_image) {
-    const size_t fold_f = static_cast<size_t>(8) * 25 * 16;
-    const size_t sm = (xs_f + 4 + static_cast<size_t>(28) * s.W * s.Cout + fold_f) * sizeof(float);
-    set_smem(conv5x5_wgrad_kernel<1, 16, 28>, sm);
-    conv5x5_wgrad_kernel<1, 16, 28><<<blocks, 256, sm, st>>>(dy, x, scr.partials, s.B, s.H, s.W);
-  } else if (s.Cin == 1 && s.Cout == 16) {
+  const size_t xs_f = static_cast<size_t>(s.Cin) * (TH + 4) * (s.W + 4);
+  if (s.Cin == 1 && s.Cout == 16) {
     const size_t fold_f = static_cast<size_t>(8) * 25 * 16;  // [warps][P*COUT] after dys
     const size_t sm = (xs_f + 4 + static_cast<size_t>(TH) * s.W * s.Cout + fold_f) * sizeof(float);
     conv5x5_wgrad_kernel<1, 16, TH><<<blocks, 256, sm, st>>>(dy, x, scr.partials, s.B, s.H, s.W);
   } else if (s.Cin == 16 && s.Cout == 32) {
     const size_t sm = (xs_f + 4 + static_cast<size_t>(TH) * s.W * s.Cout) * sizeof(float);
-    set_smem(conv5x5_wgrad_kernel<16, 32, TH>, sm);
+    opt_in_smem(conv5x5_wgrad_kernel<16, 32, TH>, sm);
     conv5x5_wgrad_kernel<16, 32, TH><<<blocks, 256, sm, st>>>(dy, x, scr.partials, s.B, s.H, s.W);
   } else {
     throw std::invalid_argument("conv5x5_wgrad: supported channel configs are 1→16 and 16→32");

@@ -6,14 +6,6 @@
 
 namespace pdt {
 
-// Every launcher of this library reports here, so benchmarks can state how many of *our* kernels
-// ran in a timed region (during CUDA-graph capture: how many were recorded into the graph).
-void count_kernel_launch(int n = 1);
-long long kernel_launch_count();
-// Set from a Python atexit hook: destructors that would call into a dying CUDA driver skip their work.
-void mark_process_exiting();
-bool process_exiting();
-
 constexpr int kSymmMaxWorld = 8;       // one NVSwitch domain (single node, like the reference)
 constexpr int kSymmChannels = 4;       // independent flag/staging sets: one per concurrent stream
 constexpr int kSymmMaxBlocks = 160;    // >= the SM count (132 on an H100 SXM): every CTA of a collective owns a flag row

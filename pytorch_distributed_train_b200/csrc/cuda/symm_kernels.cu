@@ -15,6 +15,7 @@
 #include <stdexcept>
 #include <string>
 
+#include "cuda_utils.h"
 #include "symm_kernels.h"
 
 namespace pdt {
@@ -376,29 +377,9 @@ __global__ void barrier_kernel(const __grid_constant__ SymmDev d) {
 }
 
 // ---- launch helpers -------------------------------------------------------------------------------------
-// SM count of the current device (cached per device): the two-shot kernels use at most one CTA per SM.
-int device_sm_count() {
-  static int cached[64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) dev = 0;
-  if (cached[dev] == 0) {
-    int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = kSymmMaxBlocks;
-    cached[dev] = n;
-  }
-  return cached[dev];
-}
-
 int auto_blocks(size_t nvec, int threads, int cap) {
   size_t b = (nvec + static_cast<size_t>(threads) * 2 - 1) / (static_cast<size_t>(threads) * 2);
   return static_cast<int>(std::max<size_t>(1, std::min<size_t>(b, static_cast<size_t>(cap))));
-}
-
-void check_launch(const char* what) {
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("launch of ") + what + " failed: " + cudaGetErrorString(e));
-  count_kernel_launch();
 }
 
 // Which (dtype, op) pairs get a kernel.  SUM exists for every dtype (it is what DDP, SyncBatchNorm and the object
@@ -504,7 +485,8 @@ void launch_allreduce_twoshot(const SymmDev& d, size_t buf_off, size_t count, in
   if (nvec == 0) return;
   const int threads = cfg.threads ? cfg.threads : 512;
   const size_t per = (nvec + d.world - 1) / d.world;
-  const int blocks = std::min(cfg.blocks ? cfg.blocks : auto_blocks(per, threads, device_sm_count()), kSymmMaxBlocks);
+  // the two-shot kernels use at most one CTA per SM
+  const int blocks = std::min(cfg.blocks ? cfg.blocks : auto_blocks(per, threads, sm_count()), kSymmMaxBlocks);
   const float sc = static_cast<float>(scale);
   if (nvls) {
     if (!d.mc) throw std::runtime_error("twoshot nvls requested but the heap has no multicast mapping");

@@ -1,11 +1,11 @@
 // conv2 (16→32, 5×5) weight gradient of one image in the "window" formulation, shared by the stand-alone kernel
-// (conv_tcgen05.cu) and the layer-1 backward kernel that carries it along (fused_convnet.cu):
+// (conv_wgmma.cu) and the layer-1 backward kernel that carries it along (fused_convnet.cu):
 //   dWᵀ[(kh, kw, ci)][co] = Σ_P xpad[P + (kh−2)·18 + (kw−2)][ci] · dypad[P][co]
 // over the 256 padded positions P from the first interior one.  Two horizontally adjacent taps of one position are 32
 // contiguous floats of the NHWC frame, so a 32-row "atom" of the M dimension (tap pair × 16 channels) is one row of the
 // overlapping-row view of the frame (row r = positions r, r+1).  Both operands have the reduction dimension (positions)
 // outermost — MN-major — which TF32 wgmma does not accept, so this is warp-level mma.sync m16n8k8 reading the swizzled
-// tiles directly.  The im2col weight gradient (conv_tcgen05.cu) uses the same per-warp step.
+// tiles directly.  The im2col weight gradient (conv_wgmma.cu) uses the same per-warp step.
 // Trade-off: on the previous (Blackwell) generation these MMAs ran asynchronously from one extra warp while the layer-1
 // SIMT warps worked; here they are synchronous warp-level MMAs.  In the layer-1 backward kernel they run on 15 of its warps
 // just before the second grid barrier, i.e. on the critical path of the step: about 13 µs of the ~40 µs layer-1 backward

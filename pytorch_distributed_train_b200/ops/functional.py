@@ -1,4 +1,4 @@
-"""Autograd bindings for the sm_90a kernels in ``_C`` (csrc/cuda/ops_simt.cu, conv_tcgen05.cu).
+"""Autograd bindings for the sm_90a kernels in ``_C`` (csrc/cuda/ops_simt.cu, conv_wgmma.cu).
 
 Layout convention: activations between fused layers are NHWC in memory and are handed to PyTorch
 as ``channels_last`` tensors (logical NCHW shape), so module hooks / user code see ordinary tensors.
@@ -189,8 +189,7 @@ class sgd_rider_enabled:
 def _wgrad_rides_on_layer1() -> bool:
     """conv2's weight gradient runs on the tensor cores *inside* the layer-1 backward kernel (two extra warps per CTA)
     instead of as a kernel of its own between the two layer kernels.  PDT_WGRAD_MERGED=0 restores the separate launch."""
-    return (os.environ.get("PDT_WGRAD_MERGED", "1") != "0" and os.environ.get("PDT_WGRAD_WIN", "1") != "0"
-            and hasattr(_C, "convnet_l1_bwd_wgrad"))
+    return os.environ.get("PDT_WGRAD_MERGED", "1") != "0" and hasattr(_C, "convnet_l1_bwd_wgrad")
 
 
 class _FusedLayer1(torch.autograd.Function):
@@ -306,11 +305,8 @@ class _FusedLayer2(torch.autograd.Function):
             return dp1, None, None, dg, dbe, None, None, None, None, None, dfcw, dfcb, None, None, None
         dw = _grad_dst(w_p, w)
         db = _grad_dst(b_p, b_p) if b_p is not None else None
-        if os.environ.get("PDT_WGRAD_WIN", "1") != "0":
-            # dy and p1 are zero-haloed frames: every operand of the tensor-core weight gradient arrives by TMA
-            _C.conv5x5_wgrad_win(dy, p1, dysum, dw, db)
-        else:  # im2col-gather kernel on the frames' interiors
-            _C.conv5x5_wgrad(dy[:, 2:16, 2:16, :].contiguous(), p1[:, 2:16, 2:16, :].contiguous(), dw, db, "auto")
+        # dy and p1 are zero-haloed frames: every operand of the tensor-core weight gradient arrives by TMA
+        _C.conv5x5_wgrad_win(dy, p1, dysum, dw, db)
         return dp1, dw, db, dg, dbe, None, None, None, None, None, dfcw, dfcb, None, None, None
 
 

@@ -30,16 +30,16 @@ def nhwc(t):
     return t.permute(0, 2, 3, 1).contiguous()
 
 
-def test_native_runtime_is_loaded():
-    assert ops.native_available() and hasattr(_C, "SymmComm") and hasattr(_C, "gemm_tf32_tcgen05")
+def test_native_cuda_runtime_is_loaded():
+    assert ops.native_available() and hasattr(_C, "SymmComm") and hasattr(_C, "gemm_tf32_wgmma")
     assert torch.cuda.get_device_capability(0) == (9, 0), "these kernels are built for sm_90a only"
 
 
 @pytest.mark.parametrize("M,N,K", [(128, 32, 32), (128, 32, 416), (256, 16, 800), (19600, 32, 416), (1000, 64, 100), (77, 256, 64)])
-def test_gemm_tf32_tcgen05(M, N, K):
+def test_gemm_tf32_wgmma(M, N, K):
     a = torch.randn(M, K, device=dev())
     b = torch.randn(N, K, device=dev())
-    d = _C.gemm_tf32_tcgen05(a, b)
+    d = _C.gemm_tf32_wgmma(a, b)
     ref = a.double() @ b.double().t()
     err = (d.double() - ref).abs().max().item()
     scale = ref.abs().max().item()
@@ -47,7 +47,7 @@ def test_gemm_tf32_tcgen05(M, N, K):
     # exactness on tf32-representable inputs: proves operand layout / descriptors, not just "close"
     ai = torch.randint(-4, 5, (M, K), device=dev()).float()
     bi = torch.randint(-4, 5, (N, K), device=dev()).float()
-    assert torch.equal(_C.gemm_tf32_tcgen05(ai, bi), ai @ bi.t())
+    assert torch.equal(_C.gemm_tf32_wgmma(ai, bi), ai @ bi.t())
 
 
 @pytest.mark.parametrize("cin,cout,H,impl", [(1, 16, 28, "simt"), (16, 32, 14, "simt"), (16, 32, 14, "tcgen05")])
@@ -70,7 +70,7 @@ def test_conv5x5_forward_and_stats(cin, cout, H, impl, B):
     assert torch.equal(y, y2) and torch.equal(stats, stats2)
 
 
-def test_conv_tcgen05_exact_on_small_integers():
+def test_conv_gather_exact_on_small_integers():
     x = torch.randint(-3, 4, (5, 16, 14, 14), device=dev()).float()
     w = torch.randint(-2, 3, (32, 16, 5, 5), device=dev()).float()
     y, _ = _C.conv5x5_fwd(nhwc(x), w, None, False, "tcgen05")

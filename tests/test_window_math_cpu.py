@@ -1,18 +1,14 @@
-"""CPU emulation of the index arithmetic of the tensor-core "window" kernels (no GPU): what the descriptors address, not how fast.
+"""CPU emulation of the index arithmetic of the tensor-core "window" weight gradient (no GPU): what the descriptors address, not
+how fast.
 
-* forward / data gradient (K-major patch, 25 row-shifted descriptors): tools/emulate_window_conv.py, run here as a test;
-* weight gradient riding on layer-1 backward (csrc/cuda/fused_convnet.cu, L1WgCfg): ONE overlapping-row view of the zero-haloed
-  x frame (row r = positions r and r+1 × 16 channels = a 32-wide MN-major atom), four M = 128 tiles whose four atoms sit at a
-  uniform row stride (the descriptor's LBO) — tiles 0-2 stack kh = 0..3 at 18 rows for kw/2 = 0,1,2; tile 3 stacks kw/2 = 0..3 at
-  2 rows for kh = 4 — K = 256 positions from the first interior one in 32 steps of 8, and the fold's accumulator-row → (kh, kw, ci)
-  mapping.  Checked against torch.nn.grad.conv2d_weight in float64.
+The weight gradient riding on layer-1 backward (csrc/cuda/fused_convnet.cu, L1WgCfg) reads ONE overlapping-row view of the zero-haloed
+x frame (row r = positions r and r+1 × 16 channels = a 32-wide MN-major atom), four M = 128 tiles whose four atoms sit at a
+uniform row stride (the descriptor's LBO) — tiles 0-2 stack kh = 0..3 at 18 rows for kw/2 = 0,1,2; tile 3 stacks kw/2 = 0..3 at
+2 rows for kh = 4 — K = 256 positions from the first interior one in 32 steps of 8, and the fold's accumulator-row → (kh, kw, ci)
+mapping.  Checked against torch.nn.grad.conv2d_weight in float64.
 """
-import importlib.util
-import os
-
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PW, FRAME, FIRST = 18, 18 * 18, 2 * 18 + 2
 
 
@@ -62,10 +58,3 @@ def test_window_weight_gradient_addressing_matches_conv2d_weight():
         assert (got - ref).abs().max().item() < 1e-10
     # the window never reaches outside its six boxes, and the dummy fourth atom of tile 3 (kw/2 = 3) is the only garbage column block
     assert FIRST + 8 * 31 + (2 * 18 - 2) + 3 * 2 + 7 < 6 * 64 and FIRST + (0 - 2) * 18 - 2 == 0
-
-
-def test_window_forward_and_dgrad_addressing():
-    spec = importlib.util.spec_from_file_location("emulate_window_conv", os.path.join(ROOT, "tools", "emulate_window_conv.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    assert mod.main() == 0

@@ -12,10 +12,10 @@ OUT = os.path.join(ROOT, "tool_out")
 os.makedirs(OUT, exist_ok=True)
 
 GROUPS = {
-    "loaded": ["tests/test_gpu_kernels.py::test_native_runtime_is_loaded"],
-    "gemm": ["tests/test_gpu_kernels.py::test_gemm_tf32_tcgen05"],
+    "loaded": ["tests/test_gpu_kernels.py::test_native_cuda_runtime_is_loaded"],
+    "gemm": ["tests/test_gpu_kernels.py::test_gemm_tf32_wgmma"],
     "conv_fwd": ["tests/test_gpu_kernels.py::test_conv5x5_forward_and_stats"],
-    "conv_exact": ["tests/test_gpu_kernels.py::test_conv_tcgen05_exact_on_small_integers"],
+    "conv_exact": ["tests/test_gpu_kernels.py::test_conv_gather_exact_on_small_integers"],
     "conv_bwd": ["tests/test_gpu_kernels.py::test_conv5x5_backward"],
     "conv_tma": ["tests/test_gpu_kernels.py::test_conv_tma_im2col_exact"],
     "bn_pool": ["tests/test_gpu_kernels.py::test_bn_relu_pool_forward_backward", "tests/test_gpu_kernels.py::test_generic_bn_kernels_match_torch"],
