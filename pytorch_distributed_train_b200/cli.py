@@ -8,7 +8,8 @@ GPU → init_process_group over TCP → seed → model → optional SyncBN → D
 Extra flags cover what the reference hard-codes: ``--init-method`` (its LAN address
 ``tcp://10.9.1.2:34567`` only works on the author's network, ref: ddp_example.py:110; we default
 to loopback with a free port), ``--data synthetic|mnist``, ``--model``, ``--comm fused|nccl``, ``--algo``,
-``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--lr``, ``--checkpoint`` / ``--resume``.
+``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw), ``--lr``,
+``--momentum``, ``--weight-decay``, ``--checkpoint`` / ``--resume``.
 """
 from __future__ import annotations
 
@@ -41,8 +42,12 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--data-root", default="./data", type=str)
     p.add_argument("--model", default="convnet", choices=["convnet", "resnet18"])
     p.add_argument("--batch-size", default=100, type=int, help="per-GPU batch size (reference: 100)")
-    p.add_argument("--lr", default=1e-4, type=float, help="SGD learning rate (reference: 1e-4)")
-    p.add_argument("--momentum", default=0.0, type=float)
+    p.add_argument("--optimizer", default="sgd", choices=["sgd", "adam", "adamw"],
+                   help="optimizer: SGD (the reference's), Adam or AdamW, each a native multi-tensor kernel")
+    p.add_argument("--lr", default=1e-4, type=float, help="learning rate (reference: 1e-4)")
+    p.add_argument("--momentum", default=None, type=float, help="SGD momentum (default 0; not accepted with Adam / AdamW)")
+    p.add_argument("--weight-decay", default=None, type=float,
+                   help="weight decay (default: 0 for SGD and Adam, 1e-2 for AdamW, torch's defaults)")
     p.add_argument("--steps", default=0, type=int, help="stop each epoch after this many steps (0 = full epoch)")
     p.add_argument("--samples", default=60000, type=int, help="synthetic dataset size")
     p.add_argument("--graph", default=False, action="store_true", help="capture the whole training step in a CUDA graph")
@@ -52,6 +57,22 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--set-epoch", default=False, action="store_true",
                    help="call sampler.set_epoch(e) each epoch (the reference does not)")
     return p
+
+
+def make_optimizer(args, params):
+    """The optimizer ``--optimizer`` / ``--lr`` / ``--momentum`` / ``--weight-decay`` describe."""
+    import pytorch_distributed_train_b200 as pdt
+
+    kw = {} if args.weight_decay is None else {"weight_decay": args.weight_decay}
+    if args.optimizer == "sgd":
+        return pdt.optim.SGD(params, args.lr, momentum=args.momentum or 0.0, **kw)
+    cls = pdt.optim.Adam if args.optimizer == "adam" else pdt.optim.AdamW
+    return cls(params, args.lr, **kw)
+
+
+def check_args(p: argparse.ArgumentParser, args) -> None:
+    if args.optimizer != "sgd" and args.momentum is not None:
+        p.error(f"--momentum applies to SGD only; {args.optimizer} takes its moments from its betas")
 
 
 def dist_train(gpu: int, args) -> None:
@@ -85,7 +106,7 @@ def dist_train(gpu: int, args) -> None:
     model.to(device)
     batch_size = args.batch_size
     criterion = pdt.nn.CrossEntropyLoss().to(device)
-    optimizer = pdt.optim.SGD(model.parameters(), args.lr, momentum=args.momentum)
+    optimizer = make_optimizer(args, model.parameters())
     model = pdt.DistributedDataParallel(model, device_ids=[gpu] if use_cuda else None)
 
     if args.data == "mnist" and args.model == "convnet":
@@ -156,7 +177,9 @@ def dist_train(gpu: int, args) -> None:
 
 
 def main(argv=None) -> None:
-    args = build_parser().parse_args(argv)
+    p = build_parser()
+    args = p.parse_args(argv)
+    check_args(p, args)
     args.world_size = args.gpus  # one process per GPU (ref: ddp_example.py:109)
     if args.init_method is None:
         args.init_method = f"tcp://127.0.0.1:{_free_port()}"

@@ -243,8 +243,60 @@ void register_cuda_bindings(py::module_& m) {
                     dysum2.numel() == static_cast<int64_t>(B) * 32 && dw2.numel() == 12800, "convnet_l1_bwd_wgrad: layer-2 shape mismatch");
     // sgd = (params[10], prev_grads[4], momentum_bufs[10] or [], lr, lr_tensor, momentum, dampening, weight_decay, nesterov, maximize, first_step):
     // parameters in the order conv1.w, conv1.b, bn1.w, bn1.b, conv2.w, conv2.b, fc.w, fc.b, bn2.w, bn2.b (entries may be None)
+    // or the Adam rider: ("adam", params[10], prev_grads[4], exp_avgs[10], exp_avg_sqs[10], steps[10], lr, lr_tensor, beta1, beta2,
+    // eps, weight_decay, decoupled, maximize), steps being fp32 scalars on the device
+    static const int64_t want[10] = {400, 16, 16, 16, 12800, 32, -1, -1, 32, 32};
+    ReduceScratch scr = scratch(x);
+    const size_t l1_floats = static_cast<size_t>(B) * (64 + 512);
+    TORCH_CHECK(static_cast<long long>(l1_floats) + static_cast<long long>(B) * 512 * 32 <= scr.capacity_floats, "convnet_l1_bwd_wgrad: scratch too small");
+    if (!sgd.is_none() && py::isinstance<py::tuple>(sgd) && py::len(sgd) > 0 && py::isinstance<py::str>(sgd.cast<py::tuple>()[0])) {
+      auto t = sgd.cast<py::tuple>();
+      TORCH_CHECK(t.size() == 14 && t[0].cast<std::string>() == "adam", "convnet_l1_bwd_wgrad: adam tuple of 14 entries expected");
+      auto params = t[1].cast<std::vector<c10::optional<at::Tensor>>>();
+      auto prev = t[2].cast<std::vector<c10::optional<at::Tensor>>>();
+      auto ms = t[3].cast<std::vector<c10::optional<at::Tensor>>>();
+      auto vs = t[4].cast<std::vector<c10::optional<at::Tensor>>>();
+      auto steps = t[5].cast<std::vector<c10::optional<at::Tensor>>>();
+      TORCH_CHECK(params.size() == 10 && prev.size() == 4 && ms.size() == 10 && vs.size() == 10 && steps.size() == 10,
+                  "convnet_l1_bwd_wgrad: adam lists have the wrong length");
+      AdamRider rider;
+      for (int k = 0; k < 10; ++k) {
+        if (!params[k].has_value() || !params[k]->defined()) continue;
+        chk(*params[k], "adam param");
+        const int64_t numel = params[k]->numel();
+        TORCH_CHECK(want[k] < 0 || numel == want[k], "convnet_l1_bwd_wgrad: adam parameter ", k, " has the wrong size");
+        TORCH_CHECK(ms[k].has_value() && vs[k].has_value() && steps[k].has_value(), "convnet_l1_bwd_wgrad: adam state of parameter ", k, " missing");
+        chk(*ms[k], "exp_avg"); chk(*vs[k], "exp_avg_sq"); chk(*steps[k], "step");
+        TORCH_CHECK(ms[k]->numel() == numel && vs[k]->numel() == numel && steps[k]->numel() == 1, "convnet_l1_bwd_wgrad: adam state of parameter ", k,
+                    " has the wrong size");
+        rider.p[k] = params[k]->data_ptr<float>();
+        rider.m[k] = ms[k]->data_ptr<float>();
+        rider.v[k] = vs[k]->data_ptr<float>();
+        rider.step[k] = steps[k]->data_ptr<float>();
+        if (k >= 6) {
+          TORCH_CHECK(prev[k - 6].has_value() && prev[k - 6]->numel() == numel, "convnet_l1_bwd_wgrad: gradient of adam parameter ", k, " missing");
+          chk(*prev[k - 6], "adam gradient");
+          rider.g_prev[k - 6] = prev[k - 6]->data_ptr<float>();
+          rider.n_prev[k - 6] = static_cast<int>(numel);
+        }
+      }
+      TORCH_CHECK(rider.p[0] && rider.p[4], "convnet_l1_bwd_wgrad: the convolution weights must take part in the fused update");
+      rider.h = AdamHyper{t[6].cast<double>(), t[8].cast<double>(), t[9].cast<double>(), static_cast<float>(t[10].cast<double>()),
+                          static_cast<float>(t[11].cast<double>()), t[12].cast<bool>() ? 1 : 0, t[13].cast<bool>() ? 1 : 0, nullptr};
+      if (!t[7].is_none()) {
+        at::Tensor lrt = t[7].cast<at::Tensor>();
+        chk(lrt, "lr_tensor");
+        rider.h.lr_dev = lrt.data_ptr<float>();
+      }
+      rider.on = 1;
+      launch_convnet_l1_bwd_wgrad(dp.data_ptr<float>(), y.data_ptr<float>(), x.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"),
+                                  opt_ptr(beta, "beta"), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"),
+                                  dy2_pad.data_ptr<float>(), x2_pad.data_ptr<float>(), dysum2.data_ptr<float>(), dw2.data_ptr<float>(),
+                                  opt_mut(db2, "db2"), B, scr.partials, scr.partials + static_cast<size_t>(B) * 64, scr.partials + l1_floats,
+                                  GridSync{scr.counter + 512, scr.counter + 520}, cur_stream(x), rider);
+      return;
+    }
     SgdRider rider;
-    std::vector<at::Tensor> keep;   // keeps converted tensors alive until the launch
     if (!sgd.is_none()) {
       auto t = sgd.cast<py::tuple>();
       TORCH_CHECK(t.size() == 11, "convnet_l1_bwd_wgrad: sgd tuple of 11 entries expected");
@@ -252,7 +304,6 @@ void register_cuda_bindings(py::module_& m) {
       auto prev = t[1].cast<std::vector<c10::optional<at::Tensor>>>();
       auto bufs = t[2].cast<std::vector<c10::optional<at::Tensor>>>();
       TORCH_CHECK(params.size() == 10 && prev.size() == 4 && (bufs.empty() || bufs.size() == 10), "convnet_l1_bwd_wgrad: sgd lists have the wrong length");
-      static const int64_t want[10] = {400, 16, 16, 16, 12800, 32, -1, -1, 32, 32};
       const double momentum = t[5].cast<double>();
       for (int k = 0; k < 10; ++k) {
         if (!params[k].has_value() || !params[k]->defined()) continue;
@@ -281,9 +332,6 @@ void register_cuda_bindings(py::module_& m) {
       }
       rider.on = 1;
     }
-    ReduceScratch scr = scratch(x);
-    const size_t l1_floats = static_cast<size_t>(B) * (64 + 512);
-    TORCH_CHECK(static_cast<long long>(l1_floats) + static_cast<long long>(B) * 512 * 32 <= scr.capacity_floats, "convnet_l1_bwd_wgrad: scratch too small");
     launch_convnet_l1_bwd_wgrad(dp.data_ptr<float>(), y.data_ptr<float>(), x.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"),
                                 opt_ptr(beta, "beta"), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"),
                                 dy2_pad.data_ptr<float>(), x2_pad.data_ptr<float>(), dysum2.data_ptr<float>(), dw2.data_ptr<float>(),
@@ -596,6 +644,39 @@ void register_cuda_bindings(py::module_& m) {
         tl.n[i] = static_cast<int>(p.numel());
       }
       launch_sgd_multi(tl, h, st);
+    }
+  });
+  m.def("adam_multi", [](std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avgs,
+                         std::vector<at::Tensor> exp_avg_sqs, std::vector<at::Tensor> steps, double lr, c10::optional<at::Tensor> lr_tensor,
+                         double beta1, double beta2, double eps, double weight_decay, bool decoupled, bool maximize) {
+    const size_t n = params.size();
+    TORCH_CHECK(grads.size() == n && exp_avgs.size() == n && exp_avg_sqs.size() == n && steps.size() == n, "adam_multi: list lengths differ");
+    if (n == 0) return;
+    c10::cuda::CUDAGuard g(params[0].device());
+    AdamHyper h{lr, beta1, beta2, static_cast<float>(eps), static_cast<float>(weight_decay), decoupled ? 1 : 0, maximize ? 1 : 0, nullptr};
+    if (lr_tensor.has_value() && lr_tensor->defined()) { chk(*lr_tensor, "lr_tensor"); h.lr_dev = lr_tensor->data_ptr<float>(); }
+    cudaStream_t st = cur_stream(params[0]);
+    // the ticket word of the step hand-over (adam_multi_kernel); launches on one device are ordered by the compute stream, and
+    // every launch leaves the word at zero
+    unsigned int* ticket = scratch(params[0]).counter + 536;
+    for (size_t base = 0; base < n; base += AdamTensorList::kMax) {
+      AdamTensorList tl;
+      tl.count = static_cast<int>(std::min<size_t>(AdamTensorList::kMax, n - base));
+      for (int i = 0; i < tl.count; ++i) {
+        const size_t j = base + i;
+        chk(params[j], "param"); chk(grads[j], "grad"); chk(exp_avgs[j], "exp_avg"); chk(exp_avg_sqs[j], "exp_avg_sq"); chk(steps[j], "step");
+        const int64_t numel = params[j].numel();
+        TORCH_CHECK(grads[j].numel() == numel && exp_avgs[j].numel() == numel && exp_avg_sqs[j].numel() == numel && steps[j].numel() == 1 &&
+                        numel < (int64_t(1) << 31), "adam_multi: bad tensor sizes");
+        TORCH_CHECK(params[j].device() == params[0].device() && steps[j].device() == params[0].device(), "adam_multi: all tensors on one device");
+        tl.p[i] = params[j].data_ptr<float>();
+        tl.g[i] = grads[j].data_ptr<float>();
+        tl.m[i] = exp_avgs[j].data_ptr<float>();
+        tl.v[i] = exp_avg_sqs[j].data_ptr<float>();
+        tl.step[i] = steps[j].data_ptr<float>();
+        tl.n[i] = static_cast<int>(numel);
+      }
+      launch_adam_multi(tl, h, ticket, st);
     }
   });
 

@@ -30,6 +30,7 @@
 #include <cstdint>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 
 #include "cuda_utils.h"
 #include "conv_wgmma.h"
@@ -322,14 +323,53 @@ __device__ __forceinline__ void sgd_apply(float* p, float g, float* m, const Sgd
   *p = fmaf(-lr, gv, pv);
 }
 
-template <bool WG>
+// Per-launch factors of the Adam rider, formed once per CTA before the first grid barrier (kAdamLr: index of the first
+// non-parameter entry): step size lr/bc1 [10], sqrt(bc2) [10], AdamW decay 1 − lr·wd, 1 − β1, β2, 1 − β2.
+constexpr int kAdamLr = 20, kAdamFactors = 24;
+__device__ __forceinline__ void adam_factors(const AdamRider& r, float* f, int tid) {
+  if (tid < 10 && r.step[tid]) {
+    const double lr = r.h.lr_dev ? static_cast<double>(__ldg(r.h.lr_dev)) : r.h.lr;
+    const double s = static_cast<double>(*r.step[tid] + 1.f);
+    f[tid] = static_cast<float>(lr / (1.0 - pow(r.h.beta1, s)));
+    f[10 + tid] = static_cast<float>(sqrt(1.0 - pow(r.h.beta2, s)));
+    if (tid == 0) {
+      f[kAdamLr] = static_cast<float>(1.0 - lr * r.h.weight_decay);
+      f[kAdamLr + 1] = static_cast<float>(1.0 - r.h.beta1);
+      f[kAdamLr + 2] = static_cast<float>(r.h.beta2);
+      f[kAdamLr + 3] = static_cast<float>(1.0 - r.h.beta2);
+    }
+  }
+}
+
+// One Adam update (the arithmetic of adam_multi_kernel, ops_simt.cu) of element i of parameter k with gradient g.
+__device__ __forceinline__ void adam_apply(const AdamRider& r, int k, int i, float g, const float* f) {
+  float gv = r.h.maximize ? -g : g;
+  float* p = r.p[k] + i;
+  float* m = r.m[k] + i;
+  float* v = r.v[k] + i;
+  float pv = *p;
+  if (r.h.weight_decay != 0.f) {
+    if (r.h.decoupled) pv *= f[kAdamLr];
+    else gv = fmaf(r.h.weight_decay, pv, gv);
+  }
+  const float mv = fmaf(f[kAdamLr + 1], gv - *m, *m);
+  const float vv = fmaf(f[kAdamLr + 3] * gv, gv, f[kAdamLr + 2] * *v);
+  *m = mv;
+  *v = vv;
+  *p = fmaf(-f[k], mv / (sqrtf(vv) / f[10 + k] + r.h.eps), pv);
+}
+
+template <bool WG, class Rider = SgdRider>
 __global__ void __launch_bounds__(WG ? L1WgCfg::kThreads : kL1Threads, 1)
 convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y, const float* __restrict__ x, const float* __restrict__ saved,
                       const float* __restrict__ gamma, const float* __restrict__ beta, float* dgamma, float* dbeta, float* dw, float* db,
                       float* partials, float* partials_w, GridSync gs,
                       // WG only: conv2 weight gradient of the same image
                       const __grid_constant__ CUtensorMap tm_x2, const __grid_constant__ CUtensorMap tm_dy2, float* __restrict__ wpart,
-                      const float* __restrict__ dysum2, float* dw2, float* db2, const __grid_constant__ SgdRider sr) {
+                      const float* __restrict__ dysum2, float* dw2, float* db2, const __grid_constant__ Rider sr) {
+  constexpr bool kAdam = std::is_same_v<Rider, AdamRider>;
+  static_assert(kAdam || std::is_same_v<Rider, SgdRider>, "convnet_l1_bwd_kernel: SgdRider or AdamRider");
+  static_assert(WG || !kAdam, "the Adam rider rides on the kernel with the conv2 weight gradient");
   constexpr int NAMED = WG ? kL1Threads : 0;
   extern __shared__ __align__(16) uint8_t dsm_raw[];
   // WG: everything is placed relative to a 1024-aligned base (the swizzled TMA tiles need it)
@@ -340,6 +380,8 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   uint8_t* sa = dsm_b + L1WgCfg::kOff;                              // WG: A window
   uint8_t* sb = sa + L1WgCfg::kABytes;                              // WG: dy tiles
   uint64_t* ld_full = reinterpret_cast<uint64_t*>(sb + L1WgCfg::kBBytes);
+  float* adam_f = reinterpret_cast<float*>(sb + L1WgCfg::kBBytes + 64);   // Adam rider: kAdamFactors floats behind the barrier word
+  static_assert(64 + kAdamFactors * sizeof(float) <= 256, "Adam rider factors must fit the tail of the dynamic shared memory");
   __shared__ float xs[32 * 32];
   __shared__ float red[kL1Warps * 32];
   __shared__ float s_tmp[kL1Warps * 32];
@@ -386,6 +428,9 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
     s_invstd[tid] = invstd;
     s_scale[tid] = g * invstd;
     s_shift[tid] = b - mean * g * invstd;
+  }
+  if constexpr (kAdam) {
+    if (sr.on) adam_factors(sr, adam_f, tid);   // reads the step counts: before the first grid barrier
   }
   cta_sync<NAMED>();
 
@@ -443,14 +488,16 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   }
   trace(1, 1);
   bar.arrive<NAMED>(gs);
-  const float sgd_lr = sr.on ? (sr.h.lr_dev ? __ldg(sr.h.lr_dev) : sr.h.lr) : 0.f;
+  // (each update below is spelled out for both riders: the SGD instantiation keeps the code it had before the Adam rider existed)
+  const float sgd_lr = sr.on ? (sr.h.lr_dev ? __ldg(sr.h.lr_dev) : static_cast<float>(sr.h.lr)) : 0.f;
   if (sr.on) {
     // in the barrier's shadow: the optimizer step of the parameters whose gradients were complete before this kernel started
     // (classifier, bn2) — nothing in this kernel reads them
 #pragma unroll
     for (int t = 0; t < 4; ++t)
       for (int i = n * kL1Threads + tid; i < sr.n_prev[t]; i += B * kL1Threads)
-        sgd_apply(sr.p[6 + t] + i, __ldg(sr.g_prev[t] + i), sr.m[6 + t] ? sr.m[6 + t] + i : nullptr, sr.h, sgd_lr);
+        if constexpr (kAdam) adam_apply(sr, 6 + t, i, __ldg(sr.g_prev[t] + i), adam_f);
+        else sgd_apply(sr.p[6 + t] + i, __ldg(sr.g_prev[t] + i), sr.m[6 + t] ? sr.m[6 + t] + i : nullptr, sr.h, sgd_lr);
   }
   bar.wait<NAMED>(gs);
   trace(1, 2);
@@ -576,18 +623,31 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
     if (lane == 0) {
       if (tap < 25) {
         dw[co * 25 + tap] = s;
-        if (sr.on) sgd_apply(sr.p[0] + co * 25 + tap, s, sr.m[0] ? sr.m[0] + co * 25 + tap : nullptr, sr.h, sgd_lr);
+        if constexpr (kAdam) { if (sr.on) adam_apply(sr, 0, co * 25 + tap, s, adam_f); }
+        else if (sr.on) sgd_apply(sr.p[0] + co * 25 + tap, s, sr.m[0] ? sr.m[0] + co * 25 + tap : nullptr, sr.h, sgd_lr);
       } else if (db) {
         db[co] = s;
-        if (sr.on && sr.p[1]) sgd_apply(sr.p[1] + co, s, sr.m[1] ? sr.m[1] + co : nullptr, sr.h, sgd_lr);
+        if constexpr (kAdam) { if (sr.on && sr.p[1]) adam_apply(sr, 1, co, s, adam_f); }
+        else if (sr.on && sr.p[1]) sgd_apply(sr.p[1] + co, s, sr.m[1] ? sr.m[1] + co : nullptr, sr.h, sgd_lr);
       }
     }
   }
   if (sr.on && n == 0 && tid < 16) {
     // BatchNorm-1 affine parameters: their gradients are the totals this CTA folded after the first barrier.  Every CTA read
     // gamma / beta before that barrier, so updating them here (after the second one) races with nobody.
-    if (sr.p[3]) sgd_apply(sr.p[3] + tid, s_tot[tid], sr.m[3] ? sr.m[3] + tid : nullptr, sr.h, sgd_lr);
-    if (sr.p[2]) sgd_apply(sr.p[2] + tid, s_tot[16 + tid], sr.m[2] ? sr.m[2] + tid : nullptr, sr.h, sgd_lr);
+    if constexpr (kAdam) {
+      if (sr.p[3]) adam_apply(sr, 3, tid, s_tot[tid], adam_f);
+      if (sr.p[2]) adam_apply(sr, 2, tid, s_tot[16 + tid], adam_f);
+    } else {
+      if (sr.p[3]) sgd_apply(sr.p[3] + tid, s_tot[tid], sr.m[3] ? sr.m[3] + tid : nullptr, sr.h, sgd_lr);
+      if (sr.p[2]) sgd_apply(sr.p[2] + tid, s_tot[16 + tid], sr.m[2] ? sr.m[2] + tid : nullptr, sr.h, sgd_lr);
+    }
+  }
+  if constexpr (kAdam) {
+    // every CTA read the step counts before the first grid barrier and this is after the last one
+    if (sr.on && n == 0 && tid == 0)
+      for (int k = 0; k < 10; ++k)
+        if (sr.step[k]) *sr.step[k] += 1.f;
   }
   if constexpr (WG) {
     // conv2 weight gradient: CTA n folds outputs n, n + B, … of the 400 (tap, ci) rows × 32 co (+ row 400: the bias, from the
@@ -641,10 +701,12 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
           if (i < 400) {
             const int e = (lane * 16 + (i & 15)) * 25 + (i >> 4);
             dw2[e] = tot;
-            if (sr.on) sgd_apply(sr.p[4] + e, tot, sr.m[4] ? sr.m[4] + e : nullptr, sr.h, sgd_lr);
+            if constexpr (kAdam) { if (sr.on) adam_apply(sr, 4, e, tot, adam_f); }
+            else if (sr.on) sgd_apply(sr.p[4] + e, tot, sr.m[4] ? sr.m[4] + e : nullptr, sr.h, sgd_lr);
           } else if (db2) {
             db2[lane] = tot;
-            if (sr.on && sr.p[5]) sgd_apply(sr.p[5] + lane, tot, sr.m[5] ? sr.m[5] + lane : nullptr, sr.h, sgd_lr);
+            if constexpr (kAdam) { if (sr.on && sr.p[5]) adam_apply(sr, 5, lane, tot, adam_f); }
+            else if (sr.on && sr.p[5]) sgd_apply(sr.p[5] + lane, tot, sr.m[5] ? sr.m[5] + lane : nullptr, sr.h, sgd_lr);
           }
         }
       }
@@ -1529,15 +1591,22 @@ void launch_convnet_l1_bwd(const float* dp, const float* y, const float* x, cons
                      static_cast<float*>(nullptr), static_cast<float*>(nullptr), SgdRider{});
 }
 
+template <class Rider>
 void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
                                  float* dgamma, float* dbeta, float* dw, float* db, const float* dy2_pad, const float* x2_pad, const float* dysum2,
                                  float* dw2, float* db2, int B, float* partials, float* partials_w, float* wpart, GridSync gs, cudaStream_t st,
-                                 SgdRider sgd) {
+                                 Rider rider) {
   CUtensorMap tm_x, tm_dy;
   make_wgrad_win_tmaps(x2_pad, dy2_pad, B, &tm_x, &tm_dy);
-  launch_cooperative(convnet_l1_bwd_kernel<true>, B, L1WgCfg::kThreads, L1WgCfg::kSmem, st, "convnet_l1_bwd_wgrad", dp, y, x, saved, gamma, beta, dgamma,
-                     dbeta, dw, db, partials, partials_w, gs, tm_x, tm_dy, wpart, dysum2, dw2, db2, sgd);
+  launch_cooperative(convnet_l1_bwd_kernel<true, Rider>, B, L1WgCfg::kThreads, L1WgCfg::kSmem, st, "convnet_l1_bwd_wgrad", dp, y, x, saved, gamma, beta,
+                     dgamma, dbeta, dw, db, partials, partials_w, gs, tm_x, tm_dy, wpart, dysum2, dw2, db2, rider);
 }
+template void launch_convnet_l1_bwd_wgrad<SgdRider>(const float*, const float*, const float*, const float*, const float*, const float*, float*,
+                                                    float*, float*, float*, const float*, const float*, const float*, float*, float*, int, float*,
+                                                    float*, float*, GridSync, cudaStream_t, SgdRider);
+template void launch_convnet_l1_bwd_wgrad<AdamRider>(const float*, const float*, const float*, const float*, const float*, const float*, float*,
+                                                     float*, float*, float*, const float*, const float*, const float*, float*, float*, int, float*,
+                                                     float*, float*, GridSync, cudaStream_t, AdamRider);
 
 void launch_convnet_l2_fwd(const float* x, const float* w, const float* bias, const float* gamma, const float* beta, float* y, float* out,
                            float* saved, float* running_mean, float* running_var, long long* nbt, float momentum, float eps,

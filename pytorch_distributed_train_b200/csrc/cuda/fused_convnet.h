@@ -36,14 +36,27 @@ struct SgdRider {
   int n_prev[4] = {};
   SgdHyper h{};
 };
+// The same rider with the Adam / AdamW update (the arithmetic of adam_multi_kernel).  Every CTA reads the ten step counts before
+// the kernel's first grid barrier; one thread writes step + 1 after the last one.
+struct AdamRider {
+  int on = 0;
+  float* p[10] = {};
+  float* m[10] = {};           // exp_avg
+  float* v[10] = {};           // exp_avg_sq
+  float* step[10] = {};        // fp32 step counts on the device
+  const float* g_prev[4] = {};
+  int n_prev[4] = {};
+  AdamHyper h{};
+};
 
 // Layer-1 backward with the conv2 weight gradient of the same image running on the tensor cores next to it (two extra warps):
 // dy2_pad [B,18,18,32] / x2_pad [B,18,18,16] frames and dysum2 [B,32] from layer-2 backward → dw2 [32,16,5,5], db2 [32].
-// wpart: B·512·32 floats of scratch, disjoint from partials / partials_w.
+// wpart: B·512·32 floats of scratch, disjoint from partials / partials_w.  Rider: SgdRider or AdamRider.
+template <class Rider = SgdRider>
 void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
                                  float* dgamma, float* dbeta, float* dw, float* db, const float* dy2_pad, const float* x2_pad, const float* dysum2,
                                  float* dw2, float* db2, int B, float* partials, float* partials_w, float* wpart, GridSync gs, cudaStream_t st,
-                                 SgdRider sgd = SgdRider{});
+                                 Rider rider = Rider{});
 // x [B,18,18,16] frame → y [B,14,14,32], out [B,32,7,7] NCHW, saved [64]; logits [B,ncls] = fc(out) when logits != nullptr.
 // partials: B·64 floats.
 void launch_convnet_l2_fwd(const float* x, const float* w, const float* bias, const float* gamma, const float* beta, float* y, float* out,

@@ -91,4 +91,27 @@ struct SgdHyper {
 };
 void launch_sgd_multi(const SgdTensorList& tl, SgdHyper h, cudaStream_t st);
 
+// Adam / AdamW with torch's single-tensor arithmetic.  `step` is the per-parameter fp32 step count on the device (torch's
+// capturable layout): the launch uses step + 1 for the bias corrections and leaves step + 1 behind, so a replayed CUDA graph
+// advances it.
+struct AdamTensorList {
+  static constexpr int kMax = 48;
+  float* p[kMax];
+  const float* g[kMax];
+  float* m[kMax];     // exp_avg
+  float* v[kMax];     // exp_avg_sq
+  float* step[kMax];
+  int n[kMax];
+  int count;
+};
+struct AdamHyper {
+  double lr, beta1, beta2;   // double, as torch's host-side bias corrections are
+  float eps, weight_decay;
+  int decoupled, maximize;   // decoupled: AdamW (p *= 1 - lr·wd); else Adam (g += wd·p)
+  const float* lr_dev;       // optional device-resident learning rate (graph-capturable schedules)
+};
+// ticket: one zeroed counter word; every block takes a ticket after it has read its step, the last one advances all steps and
+// resets the word to zero.
+void launch_adam_multi(const AdamTensorList& tl, AdamHyper h, unsigned int* ticket, cudaStream_t st);
+
 }  // namespace pdt

@@ -783,6 +783,50 @@ __global__ void __launch_bounds__(256) sgd_multi_kernel(SgdTensorList tl, SgdHyp
   }
 }
 
+// =====================================================================================================
+// Multi-tensor Adam / AdamW: same layout as sgd_multi_kernel.  Thread 0 of every block reads its tensor's step s and forms
+// the bias corrections of step s + 1 in double; the block that takes the last ticket writes s + 1 back for every tensor
+// (no block reads a step after it has taken its ticket) and resets the ticket word for the next launch.
+// =====================================================================================================
+__global__ void __launch_bounds__(256) adam_multi_kernel(AdamTensorList tl, AdamHyper h, unsigned int* ticket) {
+  const int t = blockIdx.y;
+  __shared__ float s_f[3];
+  if (threadIdx.x == 0) {
+    const double lr = h.lr_dev ? static_cast<double>(*h.lr_dev) : h.lr;
+    const double s = static_cast<double>(*tl.step[t] + 1.f);
+    s_f[0] = static_cast<float>(lr / (1.0 - pow(h.beta1, s)));   // step size lr / bc1
+    s_f[1] = static_cast<float>(sqrt(1.0 - pow(h.beta2, s)));    // sqrt(bc2)
+    s_f[2] = static_cast<float>(1.0 - lr * h.weight_decay);      // AdamW's decay factor
+    __threadfence();
+    if (atomicAdd(ticket, 1u) == gridDim.x * gridDim.y - 1) {
+      __threadfence();
+      for (int i = 0; i < tl.count; ++i) *tl.step[i] += 1.f;
+      atomicExch(ticket, 0u);
+    }
+  }
+  __syncthreads();
+  const int n = tl.n[t];
+  float* __restrict__ p = tl.p[t];
+  const float* __restrict__ g = tl.g[t];
+  float* __restrict__ m = tl.m[t];
+  float* __restrict__ v = tl.v[t];
+  const float step_size = s_f[0], bc2s = s_f[1], decay = s_f[2];
+  const float omb1 = static_cast<float>(1.0 - h.beta1), b2 = static_cast<float>(h.beta2), omb2 = static_cast<float>(1.0 - h.beta2);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float gv = h.maximize ? -g[i] : g[i];
+    float pv = p[i];
+    if (h.weight_decay != 0.f) {
+      if (h.decoupled) pv *= decay;
+      else gv = fmaf(h.weight_decay, pv, gv);
+    }
+    const float mv = fmaf(omb1, gv - m[i], m[i]);
+    const float vv = fmaf(omb2 * gv, gv, b2 * v[i]);
+    m[i] = mv;
+    v[i] = vv;
+    p[i] = fmaf(-step_size, mv / (sqrtf(vv) / bc2s + h.eps), pv);
+  }
+}
+
 size_t conv_smem(int cin, int cout, int th, int w, int threads) {
   return (static_cast<size_t>(cin) * (th + 4) * (w + 4) + 4 + 25 * cin * cout + (threads / 32 + 1) * 2 * cout) * sizeof(float);
 }
@@ -956,6 +1000,15 @@ void launch_sgd_multi(const SgdTensorList& tl, SgdHyper h, cudaStream_t st) {
   const int bx = std::max(1, std::min(64, (maxn + 1023) / 1024));
   sgd_multi_kernel<<<dim3(bx, tl.count), 256, 0, st>>>(tl, h);
   check_launch("sgd_multi");
+}
+
+void launch_adam_multi(const AdamTensorList& tl, AdamHyper h, unsigned int* ticket, cudaStream_t st) {
+  if (tl.count == 0) return;
+  int maxn = 0;
+  for (int i = 0; i < tl.count; ++i) maxn = std::max(maxn, tl.n[i]);
+  const int bx = std::max(1, std::min(64, (maxn + 1023) / 1024));
+  adam_multi_kernel<<<dim3(bx, tl.count), 256, 0, st>>>(tl, h, ticket);
+  check_launch("adam_multi");
 }
 
 }  // namespace pdt

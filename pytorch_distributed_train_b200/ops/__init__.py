@@ -24,7 +24,7 @@ def require_native(what: str) -> None:
 
 
 if _HAS_NATIVE:
-    from .functional import (bn_apply, bn_backward_apply, bn_backward_reduce, bn_finalize, bn_local_stats,  # noqa: F401
+    from .functional import (adam_step, bn_apply, bn_backward_apply, bn_backward_reduce, bn_finalize, bn_local_stats,  # noqa: F401
                              conv_bn_relu_pool, conv2d, cross_entropy, linear, sgd_step)
 else:  # CPU-only build of the extension: keep the names importable, fail loudly on use
     def _missing(name):
@@ -33,6 +33,6 @@ else:  # CPU-only build of the extension: keep the names importable, fail loudly
         f.__name__ = name
         return f
 
-    for _n in ("bn_apply", "bn_backward_apply", "bn_backward_reduce", "bn_finalize", "bn_local_stats", "conv_bn_relu_pool",
+    for _n in ("adam_step", "bn_apply", "bn_backward_apply", "bn_backward_reduce", "bn_finalize", "bn_local_stats", "conv_bn_relu_pool",
                "conv2d", "cross_entropy", "linear", "sgd_step"):
         globals()[_n] = _missing(_n)

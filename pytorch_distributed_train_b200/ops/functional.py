@@ -164,8 +164,9 @@ class upcoming_targets:
         return False
 
 
-# The optimizer whose update rides on the last backward kernel (optim.SGD.ride_on_backward, armed by engine.GraphedTrainStep when the
-# gradient reduction does not already carry it, i.e. on one GPU): {"params": [...10 parameters...], "args": callable -> hyper-parameters}
+# The optimizer whose update rides on the last backward kernel (optim.SGD / optim.Adam .ride_on_backward, armed by
+# engine.GraphedTrainStep when the gradient reduction does not already carry it, i.e. on one GPU):
+# {"kind": "sgd" | "adam", "params": [...10 parameters...], "args": callable -> the rider tuple of convnet_l1_bwd_wgrad, "owner": optimizer}
 _sgd_rider: Optional[dict] = None
 _sgd_rider_enabled = False
 
@@ -484,6 +485,14 @@ def sgd_step(params, grads, momentum_bufs, lr, momentum=0.0, dampening=0.0, weig
              maximize=False, first_step=False, lr_tensor=None) -> None:
     _C.sgd_multi(list(params), list(grads), list(momentum_bufs) if momentum_bufs else [], float(lr), lr_tensor, float(momentum),
                  float(dampening), float(weight_decay), bool(nesterov), bool(maximize), bool(first_step))
+
+
+def adam_step(params, grads, exp_avgs, exp_avg_sqs, steps, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0,
+              decoupled=False, maximize=False, lr_tensor=None) -> None:
+    """One Adam (``decoupled=False``) or AdamW update of every tensor, one kernel launch per 48 tensors.  ``steps`` are the fp32
+    step counts on the device: the launch uses step + 1 for the bias corrections and stores it, so a replayed graph advances it."""
+    _C.adam_multi(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), list(steps), float(lr), lr_tensor, float(beta1),
+                  float(beta2), float(eps), float(weight_decay), bool(decoupled), bool(maximize))
 
 
 # ---- generic (NCHW) BatchNorm pieces used by parallel.SyncBatchNorm ------------------------------------------

@@ -1,3 +1,4 @@
+from .adam import Adam, AdamW
 from .sgd import SGD
 
-__all__ = ["SGD"]
+__all__ = ["Adam", "AdamW", "SGD"]

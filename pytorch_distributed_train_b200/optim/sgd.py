@@ -12,7 +12,8 @@ autograd re-allocates them every backward.  Ours:
   no copy into the bucket next step). ``set_to_none=True`` (the reference's default behaviour)
   still works — the reducer re-homes gradients on the next backward.
 
-Bookkeeping (param_groups / state_dict) comes from ``torch.optim.Optimizer``.
+Bookkeeping (param_groups / state_dict) comes from ``torch.optim.Optimizer``; the device-resident learning rate and the
+riding checks are shared with ``Adam`` (``_riding.RidingOptimizer``).
 """
 from __future__ import annotations
 
@@ -20,8 +21,10 @@ from typing import Iterable, Optional
 
 import torch
 
+from ._riding import RidingOptimizer
 
-class SGD(torch.optim.Optimizer):
+
+class SGD(RidingOptimizer):
     def __init__(self, params: Iterable, lr: float = 1e-3, momentum: float = 0.0, dampening: float = 0.0,
                  weight_decay: float = 0.0, nesterov: bool = False, maximize: bool = False,
                  capturable: bool = False, fused: Optional[bool] = None):
@@ -39,29 +42,6 @@ class SGD(torch.optim.Optimizer):
         self._ddp = None            # set by fuse_with_ddp()
         self._fused_active = False
         self._flat_momentum = None
-        self._lr_dev = {}           # group index -> (device scalar, last host value) when capturable
-
-    # ---- device-resident learning rate (CUDA-graph friendly schedulers) ------------------------------
-    def _lr_tensor(self, gi: int, group, device) -> Optional[torch.Tensor]:
-        if not group.get("capturable") or device.type != "cuda":
-            return None
-        ent = self._lr_dev.get(gi)
-        if ent is None:
-            ent = [torch.full((1,), float(group["lr"]), dtype=torch.float32, device=device), float(group["lr"])]
-            self._lr_dev[gi] = ent
-        elif ent[1] != float(group["lr"]) and not torch.cuda.is_current_stream_capturing():
-            ent[0].fill_(float(group["lr"]))
-            ent[1] = float(group["lr"])
-        return ent[0]
-
-    def sync_lr(self) -> None:
-        """Push ``param_groups[i]['lr']`` into the device scalars a captured step reads (call between
-        graph replays after a scheduler step; a no-op when nothing changed)."""
-        for gi, group in enumerate(self.param_groups):
-            ent = self._lr_dev.get(gi)
-            if ent is not None and ent[1] != float(group["lr"]):
-                ent[0].fill_(float(group["lr"]))
-                ent[1] = float(group["lr"])
 
     # ---- single GPU: the update rides on the model's last backward kernel ---------------------------------
     def ride_on_backward(self, model) -> bool:
@@ -72,33 +52,9 @@ class SGD(torch.optim.Optimizer):
 
         Same contract as :meth:`fuse_with_ddp`: between ``backward()`` and ``step()`` the parameters are already updated.  Returns
         False (and changes nothing) when the model / optimizer combination does not qualify."""
-        import os
-
-        from .. import distributed as dist
-        from ..ops import functional as OF
-
-        if os.environ.get("PDT_SGD_RIDER", "1") == "0":
+        params = self._qualify_rider(model)
+        if params is None:
             return False
-        group_ = getattr(model, "process_group", None)
-        world = group_.size() if group_ is not None else (dist.get_world_size() if dist.is_initialized() else 1)
-        if world > 1:
-            return False   # the gradients still have to be averaged: the reduce kernels carry the update (fuse_with_ddp)
-        inner = getattr(model, "module", model)
-        try:
-            c1, b1, c2, b2, fc = inner.layer1[0], inner.layer1[1], inner.layer2[0], inner.layer2[1], inner.fc
-            params = [c1.weight, c1.bias, b1.weight, b1.bias, c2.weight, c2.bias, fc.weight, fc.bias, b2.weight, b2.bias]
-        except (AttributeError, IndexError, TypeError):
-            return False
-        if len(self.param_groups) != 1 or any(q is None for q in params):
-            return False
-        group = self.param_groups[0]
-        mine = group["params"]
-        if len(mine) != len(params) or {id(q) for q in mine} != {id(q) for q in params}:
-            return False
-        if not all(q.is_cuda and q.dtype == torch.float32 and q.is_contiguous() for q in params):
-            return False
-        self._rider_params = params
-        self._rode = False
 
         def args(prev_grads):
             if getattr(self, "_fused_active", False):   # the reduce kernels carry the update (N >= 2)
@@ -120,16 +76,8 @@ class SGD(torch.optim.Optimizer):
             return (params, list(prev_grads), bufs, float(g["lr"]), self._lr_tensor(0, g, params[0].device), float(g["momentum"]),
                     float(g["dampening"]), float(g["weight_decay"]), bool(g["nesterov"]), bool(g["maximize"]), first)
 
-        OF._sgd_rider = {"params": params, "args": args, "owner": self}
+        self._arm_rider("sgd", params, args)
         return True
-
-    def stop_riding(self) -> None:
-        """Undo :meth:`ride_on_backward`."""
-        from ..ops import functional as OF
-
-        if OF._sgd_rider is not None and OF._sgd_rider.get("owner") is self:
-            OF._sgd_rider = None
-        self._rode = False
 
     # ---- DDP fusion: the update rides on the gradient reduction ----------------------------------------
     def fuse_with_ddp(self, ddp) -> "SGD":

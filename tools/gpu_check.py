@@ -22,6 +22,7 @@ GROUPS = {
     "head_sgd": ["tests/test_gpu_kernels.py::test_linear_and_cross_entropy", "tests/test_gpu_kernels.py::test_fused_sgd_matches_torch"],
     "convnet": ["tests/test_gpu_kernels.py::test_convnet_fused_matches_unfused"],
     "ddp1": ["tests/test_gpu_kernels.py::test_single_gpu_ddp_and_graphed_step"],
+    "adam": ["tests/test_adam.py"],
 }
 
 
