@@ -9,7 +9,7 @@ Extra flags cover what the reference hard-codes: ``--init-method`` (its LAN addr
 ``tcp://10.9.1.2:34567`` only works on the author's network, ref: ddp_example.py:110; we default
 to loopback with a free port), ``--data synthetic|mnist``, ``--model``, ``--comm fused|nccl``, ``--algo``,
 ``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw), ``--lr``,
-``--momentum``, ``--weight-decay``, ``--checkpoint`` / ``--resume``.
+``--momentum``, ``--weight-decay``, ``--clip-grad-norm``, ``--checkpoint`` / ``--resume``.
 """
 from __future__ import annotations
 
@@ -48,6 +48,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--momentum", default=None, type=float, help="SGD momentum (default 0; not accepted with Adam / AdamW)")
     p.add_argument("--weight-decay", default=None, type=float,
                    help="weight decay (default: 0 for SGD and Adam, 1e-2 for AdamW, torch's defaults)")
+    p.add_argument("--clip-grad-norm", default=None, type=float, metavar="MAX",
+                   help="clip the global gradient norm (L2) to MAX before every optimizer step (default: off)")
     p.add_argument("--steps", default=0, type=int, help="stop each epoch after this many steps (0 = full epoch)")
     p.add_argument("--samples", default=60000, type=int, help="synthetic dataset size")
     p.add_argument("--graph", default=False, action="store_true", help="capture the whole training step in a CUDA graph")
@@ -73,6 +75,8 @@ def make_optimizer(args, params):
 def check_args(p: argparse.ArgumentParser, args) -> None:
     if args.optimizer != "sgd" and args.momentum is not None:
         p.error(f"--momentum applies to SGD only; {args.optimizer} takes its moments from its betas")
+    if args.clip_grad_norm is not None and not args.clip_grad_norm > 0:
+        p.error(f"--clip-grad-norm must be positive (got {args.clip_grad_norm})")
 
 
 def dist_train(gpu: int, args) -> None:
@@ -123,7 +127,8 @@ def dist_train(gpu: int, args) -> None:
         from pytorch_distributed_train_b200.engine import GraphedTrainStep
 
         step_fn = GraphedTrainStep(model, criterion, optimizer, example_inputs=(
-            torch.zeros((batch_size,) + shape, device=device), torch.zeros(batch_size, dtype=torch.int64, device=device)))
+            torch.zeros((batch_size,) + shape, device=device), torch.zeros(batch_size, dtype=torch.int64, device=device)),
+            max_grad_norm=args.clip_grad_norm)
 
     first_epoch = 0
     if args.resume:
@@ -154,6 +159,8 @@ def dist_train(gpu: int, args) -> None:
                 loss = criterion(outputs, labels)
                 optimizer.zero_grad()
                 loss.backward()
+                if args.clip_grad_norm is not None:
+                    pdt.nn.utils.clip_grad_norm_(model.parameters(), args.clip_grad_norm)
                 optimizer.step()
                 handle = loss
             if pending is not None and gpu == 0:

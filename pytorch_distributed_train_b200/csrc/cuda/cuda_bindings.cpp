@@ -4,6 +4,7 @@
 #include <pybind11/stl.h>
 #include <torch/extension.h>
 
+#include <cmath>
 #include <map>
 #include <mutex>
 
@@ -244,14 +245,39 @@ void register_cuda_bindings(py::module_& m) {
     // sgd = (params[10], prev_grads[4], momentum_bufs[10] or [], lr, lr_tensor, momentum, dampening, weight_decay, nesterov, maximize, first_step):
     // parameters in the order conv1.w, conv1.b, bn1.w, bn1.b, conv2.w, conv2.b, fc.w, fc.b, bn2.w, bn2.b (entries may be None)
     // or the Adam rider: ("adam", params[10], prev_grads[4], exp_avgs[10], exp_avg_sqs[10], steps[10], lr, lr_tensor, beta1, beta2,
-    // eps, weight_decay, decoupled, maximize), steps being fp32 scalars on the device
+    // eps, weight_decay, decoupled, maximize), steps being fp32 scalars on the device.  Either tuple may end in a clip entry
+    // (max_norm, norm_type 2 or inf, norm_out): gradient-norm clipping in front of the update (ClipRider); norm_out receives the norm.
     static const int64_t want[10] = {400, 16, 16, 16, 12800, 32, -1, -1, 32, 32};
     ReduceScratch scr = scratch(x);
     const size_t l1_floats = static_cast<size_t>(B) * (64 + 512);
-    TORCH_CHECK(static_cast<long long>(l1_floats) + static_cast<long long>(B) * 512 * 32 <= scr.capacity_floats, "convnet_l1_bwd_wgrad: scratch too small");
+    TORCH_CHECK(static_cast<long long>(l1_floats) + static_cast<long long>(B) * 512 * 32 + B <= scr.capacity_floats, "convnet_l1_bwd_wgrad: scratch too small");
+    auto launch = [&](auto rider) {
+      launch_convnet_l1_bwd_wgrad(dp.data_ptr<float>(), y.data_ptr<float>(), x.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"),
+                                  opt_ptr(beta, "beta"), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"),
+                                  dy2_pad.data_ptr<float>(), x2_pad.data_ptr<float>(), dysum2.data_ptr<float>(), dw2.data_ptr<float>(),
+                                  opt_mut(db2, "db2"), B, scr.partials, scr.partials + static_cast<size_t>(B) * 64, scr.partials + l1_floats,
+                                  GridSync{scr.counter + 512, scr.counter + 520}, cur_stream(x), rider);
+    };
+    // the clip entry of a rider tuple → the clipping variant of the rider
+    auto clipped = [&](auto base, const py::handle& entry) {
+      auto c = entry.cast<py::tuple>();
+      TORCH_CHECK(c.size() == 3, "convnet_l1_bwd_wgrad: clip entry (max_norm, norm_type, norm_out) expected");
+      const double norm_type = c[1].cast<double>();
+      TORCH_CHECK(norm_type == 2.0 || (std::isinf(norm_type) && norm_type > 0), "convnet_l1_bwd_wgrad: clip norm_type must be 2 or inf");
+      at::Tensor out = c[2].cast<at::Tensor>();
+      chk(out, "norm_out");
+      TORCH_CHECK(out.numel() == 1, "convnet_l1_bwd_wgrad: norm_out must have one element");
+      ClipRider<decltype(base)> r;
+      static_cast<decltype(base)&>(r) = base;
+      r.max_norm = static_cast<float>(c[0].cast<double>());
+      r.norm_inf = std::isinf(norm_type) ? 1 : 0;
+      r.norm_out = out.data_ptr<float>();
+      r.part = scr.partials + l1_floats + static_cast<size_t>(B) * 512 * 32;
+      return r;
+    };
     if (!sgd.is_none() && py::isinstance<py::tuple>(sgd) && py::len(sgd) > 0 && py::isinstance<py::str>(sgd.cast<py::tuple>()[0])) {
       auto t = sgd.cast<py::tuple>();
-      TORCH_CHECK(t.size() == 14 && t[0].cast<std::string>() == "adam", "convnet_l1_bwd_wgrad: adam tuple of 14 entries expected");
+      TORCH_CHECK((t.size() == 14 || t.size() == 15) && t[0].cast<std::string>() == "adam", "convnet_l1_bwd_wgrad: adam tuple of 14 or 15 entries expected");
       auto params = t[1].cast<std::vector<c10::optional<at::Tensor>>>();
       auto prev = t[2].cast<std::vector<c10::optional<at::Tensor>>>();
       auto ms = t[3].cast<std::vector<c10::optional<at::Tensor>>>();
@@ -289,17 +315,14 @@ void register_cuda_bindings(py::module_& m) {
         rider.h.lr_dev = lrt.data_ptr<float>();
       }
       rider.on = 1;
-      launch_convnet_l1_bwd_wgrad(dp.data_ptr<float>(), y.data_ptr<float>(), x.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"),
-                                  opt_ptr(beta, "beta"), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"),
-                                  dy2_pad.data_ptr<float>(), x2_pad.data_ptr<float>(), dysum2.data_ptr<float>(), dw2.data_ptr<float>(),
-                                  opt_mut(db2, "db2"), B, scr.partials, scr.partials + static_cast<size_t>(B) * 64, scr.partials + l1_floats,
-                                  GridSync{scr.counter + 512, scr.counter + 520}, cur_stream(x), rider);
+      if (t.size() == 15) launch(clipped(rider, t[14]));
+      else launch(rider);
       return;
     }
     SgdRider rider;
     if (!sgd.is_none()) {
       auto t = sgd.cast<py::tuple>();
-      TORCH_CHECK(t.size() == 11, "convnet_l1_bwd_wgrad: sgd tuple of 11 entries expected");
+      TORCH_CHECK(t.size() == 11 || t.size() == 12, "convnet_l1_bwd_wgrad: sgd tuple of 11 or 12 entries expected");
       auto params = t[0].cast<std::vector<c10::optional<at::Tensor>>>();
       auto prev = t[1].cast<std::vector<c10::optional<at::Tensor>>>();
       auto bufs = t[2].cast<std::vector<c10::optional<at::Tensor>>>();
@@ -331,12 +354,12 @@ void register_cuda_bindings(py::module_& m) {
         rider.h.lr_dev = lrt.data_ptr<float>();
       }
       rider.on = 1;
+      if (t.size() == 12) {
+        launch(clipped(rider, t[11]));
+        return;
+      }
     }
-    launch_convnet_l1_bwd_wgrad(dp.data_ptr<float>(), y.data_ptr<float>(), x.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"),
-                                opt_ptr(beta, "beta"), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"),
-                                dy2_pad.data_ptr<float>(), x2_pad.data_ptr<float>(), dysum2.data_ptr<float>(), dw2.data_ptr<float>(),
-                                opt_mut(db2, "db2"), B, scr.partials, scr.partials + static_cast<size_t>(B) * 64, scr.partials + l1_floats,
-                                GridSync{scr.counter + 512, scr.counter + 520}, cur_stream(x), rider);
+    launch(rider);
   }, py::arg("dp"), py::arg("y"), py::arg("x"), py::arg("saved"), py::arg("gamma"), py::arg("beta"), py::arg("dgamma"), py::arg("dbeta"),
      py::arg("dw"), py::arg("db"), py::arg("dy2_pad"), py::arg("x2_pad"), py::arg("dysum2"), py::arg("dw2"), py::arg("db2"),
      py::arg("sgd") = py::none());
@@ -677,6 +700,66 @@ void register_cuda_bindings(py::module_& m) {
         tl.n[i] = static_cast<int>(numel);
       }
       launch_adam_multi(tl, h, ticket, st);
+    }
+  });
+  // Gradient-norm clipping: returns the total norm (a 0-d view of a [2] buffer whose second element is the clip coefficient);
+  // scale=False stops after the norm kernel (grad_scale then applies the coefficient).
+  m.def("grad_norm_clip", [](std::vector<at::Tensor> grads, double max_norm, double norm_type, bool scale) {
+    TORCH_CHECK(!grads.empty(), "grad_norm_clip: no gradients");
+    TORCH_CHECK(norm_type == 2.0 || (std::isinf(norm_type) && norm_type > 0), "grad_norm_clip: norm_type must be 2 or inf");
+    c10::cuda::CUDAGuard g(grads[0].device());
+    std::vector<GradTensorList> tables;
+    for (size_t base = 0; base < grads.size(); base += GradTensorList::kMax) {
+      GradTensorList tl;
+      tl.count = static_cast<int>(std::min<size_t>(GradTensorList::kMax, grads.size() - base));
+      for (int i = 0; i < tl.count; ++i) {
+        at::Tensor& gr = grads[base + i];
+        chk(gr, "grad");
+        TORCH_CHECK(gr.device() == grads[0].device(), "grad_norm_clip: all gradients on one device");
+        TORCH_CHECK(gr.numel() < (int64_t(1) << 31), "grad_norm_clip: gradient too large");
+        tl.g[i] = gr.data_ptr<float>();
+        tl.n[i] = static_cast<int>(gr.numel());
+      }
+      tables.push_back(tl);
+    }
+    int total = 0;
+    for (const auto& tl : tables) total += grad_multi_blocks_x(tl) * tl.count;
+    ReduceScratch scr = scratch(grads[0]);
+    TORCH_CHECK(total <= scr.capacity_floats, "grad_norm_clip: too many gradients for the reduction scratch");
+    at::Tensor out = at::empty({2}, grads[0].options());
+    cudaStream_t st = cur_stream(grads[0]);
+    // the ticket word of the fold (grad_norm_multi_kernel): launches on one device are ordered by the compute stream, and every
+    // set leaves the word at zero
+    GradNormArgs a{scr.partials, 0, total, 0, std::isinf(norm_type) ? 1 : 0, static_cast<float>(max_norm), out.data_ptr<float>(),
+                   scr.counter + 544};
+    for (size_t k = 0; k < tables.size(); ++k) {
+      a.last = k + 1 == tables.size() ? 1 : 0;
+      launch_grad_norm_multi(tables[k], a, st);
+      a.part_base += grad_multi_blocks_x(tables[k]) * tables[k].count;
+    }
+    if (scale)
+      for (const auto& tl : tables) launch_grad_scale_multi(tl, out.data_ptr<float>() + 1, st);
+    return out.select(0, 0);
+  }, py::arg("grads"), py::arg("max_norm"), py::arg("norm_type") = 2.0, py::arg("scale") = true);
+  // g *= the clip coefficient stored behind `norm` (a tensor returned by grad_norm_clip)
+  m.def("grad_scale", [](std::vector<at::Tensor> grads, const at::Tensor& norm) {
+    TORCH_CHECK(norm.is_cuda() && norm.scalar_type() == at::kFloat && norm.dim() == 0 &&
+                    norm.storage().nbytes() >= (static_cast<size_t>(norm.storage_offset()) + 2) * sizeof(float),
+                "grad_scale: norm must be a tensor returned by grad_norm_clip");
+    if (grads.empty()) return;
+    c10::cuda::CUDAGuard g(norm.device());
+    cudaStream_t st = cur_stream(norm);
+    for (size_t base = 0; base < grads.size(); base += GradTensorList::kMax) {
+      GradTensorList tl;
+      tl.count = static_cast<int>(std::min<size_t>(GradTensorList::kMax, grads.size() - base));
+      for (int i = 0; i < tl.count; ++i) {
+        at::Tensor& gr = grads[base + i];
+        chk(gr, "grad");
+        TORCH_CHECK(gr.device() == norm.device() && gr.numel() < (int64_t(1) << 31), "grad_scale: bad gradient");
+        tl.g[i] = gr.data_ptr<float>();
+        tl.n[i] = static_cast<int>(gr.numel());
+      }
+      launch_grad_scale_multi(tl, norm.data_ptr<float>() + 1, st);
     }
   });
 

@@ -359,6 +359,12 @@ __device__ __forceinline__ void adam_apply(const AdamRider& r, int k, int i, flo
   *p = fmaf(-f[k], mv / (sqrtf(vv) / f[10 + k] + r.h.eps), pv);
 }
 
+// Gradient-norm clipping (ClipRider): one gradient element g into a thread's accumulator — Σg², or max |g| keeping a NaN.
+template <class R>
+__device__ __forceinline__ float clip_acc(const R& r, float acc, float g) { return r.norm_inf ? nan_max(fabsf(g), acc) : fmaf(g, g, acc); }
+template <class R>
+__device__ __forceinline__ float clip_comb(const R& r, float a, float b) { return r.norm_inf ? nan_max(a, b) : a + b; }
+
 template <bool WG, class Rider = SgdRider>
 __global__ void __launch_bounds__(WG ? L1WgCfg::kThreads : kL1Threads, 1)
 convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y, const float* __restrict__ x, const float* __restrict__ saved,
@@ -367,9 +373,10 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
                       // WG only: conv2 weight gradient of the same image
                       const __grid_constant__ CUtensorMap tm_x2, const __grid_constant__ CUtensorMap tm_dy2, float* __restrict__ wpart,
                       const float* __restrict__ dysum2, float* dw2, float* db2, const __grid_constant__ Rider sr) {
-  constexpr bool kAdam = std::is_same_v<Rider, AdamRider>;
-  static_assert(kAdam || std::is_same_v<Rider, SgdRider>, "convnet_l1_bwd_kernel: SgdRider or AdamRider");
-  static_assert(WG || !kAdam, "the Adam rider rides on the kernel with the conv2 weight gradient");
+  constexpr bool kClip = std::is_same_v<Rider, ClipRider<SgdRider>> || std::is_same_v<Rider, ClipRider<AdamRider>>;
+  constexpr bool kAdam = std::is_same_v<Rider, AdamRider> || std::is_same_v<Rider, ClipRider<AdamRider>>;
+  static_assert(kAdam || std::is_base_of_v<SgdRider, Rider>, "convnet_l1_bwd_kernel: SgdRider or AdamRider, or either in a ClipRider");
+  static_assert(WG || !(kAdam || kClip), "the Adam and clipping riders ride on the kernel with the conv2 weight gradient");
   constexpr int NAMED = WG ? kL1Threads : 0;
   extern __shared__ __align__(16) uint8_t dsm_raw[];
   // WG: everything is placed relative to a 1024-aligned base (the swizzled TMA tiles need it)
@@ -388,6 +395,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   __shared__ float s_tot[32];
   __shared__ float s_scale[16], s_shift[16], s_mean[16], s_invstd[16];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = blockIdx.x, B = gridDim.x;
+  float* s_clip = red + 512;   // ClipRider: per-warp norm partials + the coefficient (s_db below takes red[0, 512) only)
 
   if constexpr (WG) {
     if (warp == kL1Warps) {
@@ -490,7 +498,18 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   bar.arrive<NAMED>(gs);
   // (each update below is spelled out for both riders: the SGD instantiation keeps the code it had before the Adam rider existed)
   const float sgd_lr = sr.on ? (sr.h.lr_dev ? __ldg(sr.h.lr_dev) : static_cast<float>(sr.h.lr)) : 0.f;
-  if (sr.on) {
+  if constexpr (kClip) {
+    // in the barrier's shadow: the norm partial of the parameters whose gradients were complete before this kernel started
+    // (classifier, bn2); their update waits for the coefficient
+    float ca = 0.f;
+#pragma unroll
+    for (int t = 0; t < 4; ++t)
+      if (sr.p[6 + t])
+        for (int i = n * kL1Threads + tid; i < sr.n_prev[t]; i += B * kL1Threads) ca = clip_acc(sr, ca, __ldg(sr.g_prev[t] + i));
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) ca = clip_comb(sr, ca, __shfl_xor_sync(0xffffffffu, ca, off));
+    if (lane == 0) s_clip[warp] = ca;
+  } else if (sr.on) {
     // in the barrier's shadow: the optimizer step of the parameters whose gradients were complete before this kernel started
     // (classifier, bn2) — nothing in this kernel reads them
 #pragma unroll
@@ -612,6 +631,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   }
   bar.sync<NAMED>(gs);
   trace(1, 5);
+  float ca = 0.f;   // ClipRider: this thread's share of the norm of the gradients folded from here on
   // every CTA folds a few of the 16 × 26 outputs over the B partial rows: one warp per output, fixed order
   for (int j = n + warp * B; j < 512; j += kL1Warps * B) {
     const int co = j >> 5, tap = j & 31;
@@ -623,11 +643,13 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
     if (lane == 0) {
       if (tap < 25) {
         dw[co * 25 + tap] = s;
-        if constexpr (kAdam) { if (sr.on) adam_apply(sr, 0, co * 25 + tap, s, adam_f); }
+        if constexpr (kClip) ca = clip_acc(sr, ca, s);
+        else if constexpr (kAdam) { if (sr.on) adam_apply(sr, 0, co * 25 + tap, s, adam_f); }
         else if (sr.on) sgd_apply(sr.p[0] + co * 25 + tap, s, sr.m[0] ? sr.m[0] + co * 25 + tap : nullptr, sr.h, sgd_lr);
       } else if (db) {
         db[co] = s;
-        if constexpr (kAdam) { if (sr.on && sr.p[1]) adam_apply(sr, 1, co, s, adam_f); }
+        if constexpr (kClip) { if (sr.p[1]) ca = clip_acc(sr, ca, s); }
+        else if constexpr (kAdam) { if (sr.on && sr.p[1]) adam_apply(sr, 1, co, s, adam_f); }
         else if (sr.on && sr.p[1]) sgd_apply(sr.p[1] + co, s, sr.m[1] ? sr.m[1] + co : nullptr, sr.h, sgd_lr);
       }
     }
@@ -635,7 +657,10 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   if (sr.on && n == 0 && tid < 16) {
     // BatchNorm-1 affine parameters: their gradients are the totals this CTA folded after the first barrier.  Every CTA read
     // gamma / beta before that barrier, so updating them here (after the second one) races with nobody.
-    if constexpr (kAdam) {
+    if constexpr (kClip) {
+      if (sr.p[3]) ca = clip_acc(sr, ca, s_tot[tid]);
+      if (sr.p[2]) ca = clip_acc(sr, ca, s_tot[16 + tid]);
+    } else if constexpr (kAdam) {
       if (sr.p[3]) adam_apply(sr, 3, tid, s_tot[tid], adam_f);
       if (sr.p[2]) adam_apply(sr, 2, tid, s_tot[16 + tid], adam_f);
     } else {
@@ -643,7 +668,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
       if (sr.p[2]) sgd_apply(sr.p[2] + tid, s_tot[16 + tid], sr.m[2] ? sr.m[2] + tid : nullptr, sr.h, sgd_lr);
     }
   }
-  if constexpr (kAdam) {
+  if constexpr (kAdam && !kClip) {
     // every CTA read the step counts before the first grid barrier and this is after the last one
     if (sr.on && n == 0 && tid == 0)
       for (int k = 0; k < 10; ++k)
@@ -701,15 +726,70 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
           if (i < 400) {
             const int e = (lane * 16 + (i & 15)) * 25 + (i >> 4);
             dw2[e] = tot;
-            if constexpr (kAdam) { if (sr.on) adam_apply(sr, 4, e, tot, adam_f); }
+            if constexpr (kClip) ca = clip_acc(sr, ca, tot);
+            else if constexpr (kAdam) { if (sr.on) adam_apply(sr, 4, e, tot, adam_f); }
             else if (sr.on) sgd_apply(sr.p[4] + e, tot, sr.m[4] ? sr.m[4] + e : nullptr, sr.h, sgd_lr);
           } else if (db2) {
             db2[lane] = tot;
-            if constexpr (kAdam) { if (sr.on && sr.p[5]) adam_apply(sr, 5, lane, tot, adam_f); }
+            if constexpr (kClip) { if (sr.p[5]) ca = clip_acc(sr, ca, tot); }
+            else if constexpr (kAdam) { if (sr.on && sr.p[5]) adam_apply(sr, 5, lane, tot, adam_f); }
             else if (sr.on && sr.p[5]) sgd_apply(sr.p[5] + lane, tot, sr.m[5] ? sr.m[5] + lane : nullptr, sr.h, sgd_lr);
           }
         }
       }
+    }
+  }
+  if constexpr (kClip) {
+    // every gradient has been seen: one partial per CTA, one more grid barrier, then every CTA folds the B partials in the same
+    // order and derives the same coefficient bit for bit
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) ca = clip_comb(sr, ca, __shfl_xor_sync(0xffffffffu, ca, off));
+    if (lane == 0) s_clip[warp] = clip_comb(sr, s_clip[warp], ca);
+    cta_sync<NAMED>();
+    if (tid == 0) {
+      float s = s_clip[0];
+      for (int w = 1; w < kL1Warps; ++w) s = clip_comb(sr, s, s_clip[w]);
+      sr.part[n] = s;
+    }
+    bar.sync<NAMED>(gs);
+    if (warp == 0) {
+      double d = 0.0;
+      for (int r = lane; r < B; r += 32) {
+        const double v = static_cast<double>(__ldcg(sr.part + r));
+        d = sr.norm_inf ? nan_max(d, v) : d + v;
+      }
+#pragma unroll
+      for (int off = 16; off >= 1; off >>= 1) {
+        const double o = __shfl_xor_sync(0xffffffffu, d, off);
+        d = sr.norm_inf ? nan_max(d, o) : d + o;
+      }
+      if (lane == 0) {
+        const float norm = static_cast<float>(sr.norm_inf ? d : sqrt(d));
+        s_clip[kL1Warps] = clip_coef(norm, sr.max_norm);
+        if (n == 0) *sr.norm_out = norm;
+      }
+    }
+    cta_sync<NAMED>();
+    const float coef = s_clip[kL1Warps];
+    // grid-stride pass over the ten gradients (read from L2: other CTAs wrote them): .grad becomes the clipped gradient, as after
+    // clip_grad_norm_, and the update takes it
+#pragma unroll
+    for (int k = 0; k < 10; ++k) {
+      float* gk = k == 0 ? dw : k == 1 ? db : k == 2 ? dgamma : k == 3 ? dbeta : k == 4 ? dw2 : k == 5 ? db2 : const_cast<float*>(sr.g_prev[k - 6]);
+      const int nk = k == 0 ? 400 : k == 4 ? 12800 : k == 5 ? 32 : k < 6 ? 16 : sr.n_prev[k - 6];
+      if (!sr.p[k] || !gk) continue;
+      for (int i = n * kL1Threads + tid; i < nk; i += B * kL1Threads) {
+        const float gv = __ldcg(gk + i) * coef;
+        gk[i] = gv;
+        if constexpr (kAdam) adam_apply(sr, k, i, gv, adam_f);
+        else sgd_apply(sr.p[k] + i, gv, sr.m[k] ? sr.m[k] + i : nullptr, sr.h, sgd_lr);
+      }
+    }
+    if constexpr (kAdam) {
+      // every CTA read the step counts before the first grid barrier and this is after the last one
+      if (n == 0 && tid == 0)
+        for (int k = 0; k < 10; ++k)
+          if (sr.step[k]) *sr.step[k] += 1.f;
     }
   }
   bar.finish(gs);
@@ -1607,6 +1687,14 @@ template void launch_convnet_l1_bwd_wgrad<SgdRider>(const float*, const float*, 
 template void launch_convnet_l1_bwd_wgrad<AdamRider>(const float*, const float*, const float*, const float*, const float*, const float*, float*,
                                                      float*, float*, float*, const float*, const float*, const float*, float*, float*, int, float*,
                                                      float*, float*, GridSync, cudaStream_t, AdamRider);
+template void launch_convnet_l1_bwd_wgrad<ClipRider<SgdRider>>(const float*, const float*, const float*, const float*, const float*,
+                                                               const float*, float*, float*, float*, float*, const float*, const float*,
+                                                               const float*, float*, float*, int, float*, float*, float*, GridSync, cudaStream_t,
+                                                               ClipRider<SgdRider>);
+template void launch_convnet_l1_bwd_wgrad<ClipRider<AdamRider>>(const float*, const float*, const float*, const float*, const float*,
+                                                                const float*, float*, float*, float*, float*, const float*, const float*,
+                                                                const float*, float*, float*, int, float*, float*, float*, GridSync, cudaStream_t,
+                                                                ClipRider<AdamRider>);
 
 void launch_convnet_l2_fwd(const float* x, const float* w, const float* bias, const float* gamma, const float* beta, float* y, float* out,
                            float* saved, float* running_mean, float* running_var, long long* nbt, float momentum, float eps,

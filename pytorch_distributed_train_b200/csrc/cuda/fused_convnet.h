@@ -48,10 +48,22 @@ struct AdamRider {
   int n_prev[4] = {};
   AdamHyper h{};
 };
+// Either rider with gradient-norm clipping in front of the update (torch.nn.utils.clip_grad_norm_, norm_type 2 or inf).  Every CTA
+// adds up the squares (or the max |g|) of the gradient elements it sees — those of parameters 6..9 in the shadow of the first
+// grid barrier, those of 0..5 as it folds them — and writes one partial; after one more grid barrier every CTA folds the B
+// partials in the same order (fp64), derives the same coefficient, and in a grid-stride pass writes g·coef back to every
+// gradient and applies the update with it.  CTA 0 stores the norm.
+template <class Base>
+struct ClipRider : Base {
+  float max_norm = 0.f;
+  int norm_inf = 0;            // 1: max |g|, 0: Euclidean norm
+  float* norm_out = nullptr;   // the total norm (fp32 scalar)
+  float* part = nullptr;       // [B] per-CTA partials
+};
 
 // Layer-1 backward with the conv2 weight gradient of the same image running on the tensor cores next to it (two extra warps):
 // dy2_pad [B,18,18,32] / x2_pad [B,18,18,16] frames and dysum2 [B,32] from layer-2 backward → dw2 [32,16,5,5], db2 [32].
-// wpart: B·512·32 floats of scratch, disjoint from partials / partials_w.  Rider: SgdRider or AdamRider.
+// wpart: B·512·32 floats of scratch, disjoint from partials / partials_w.  Rider: SgdRider or AdamRider, or either one in a ClipRider.
 template <class Rider = SgdRider>
 void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
                                  float* dgamma, float* dbeta, float* dw, float* db, const float* dy2_pad, const float* x2_pad, const float* dysum2,

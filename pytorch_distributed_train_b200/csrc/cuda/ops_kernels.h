@@ -114,4 +114,40 @@ struct AdamHyper {
 // resets the word to zero.
 void launch_adam_multi(const AdamTensorList& tl, AdamHyper h, unsigned int* ticket, cudaStream_t st);
 
+// Gradient-norm clipping (torch.nn.utils.clip_grad_norm_ with norm_type 2 or inf) as two launches per table set: the norm, then
+// the scale.  A set of more than kMax tensors is split into tables launched back to back; every block of every table writes one
+// partial (fp32 Σg² or max |g|), and the block of the last table that takes the last ticket folds all partials of the set in
+// index order in fp64, so the norm is the same bit for bit from run to run.
+struct GradTensorList {
+  static constexpr int kMax = 48;
+  float* g[kMax];
+  int n[kMax];
+  int count;
+};
+struct GradNormArgs {
+  float* partials;       // one float per block of every table of the set
+  int part_base;         // index of this table's first partial
+  int part_total;        // partials of the whole set
+  int last;              // this is the set's last table: its last block folds
+  int norm_inf;          // 1: max |g|, 0: Euclidean norm
+  float max_norm;
+  float* out;            // [0] total norm, [1] clip coefficient min(max_norm / (norm + 1e-6), 1) (NaN propagates)
+  unsigned int* ticket;  // one zeroed counter word; the last block resets it
+};
+int grad_multi_blocks_x(const GradTensorList& tl);   // blockIdx.x extent of a table's launches
+void launch_grad_norm_multi(const GradTensorList& tl, GradNormArgs a, cudaStream_t st);
+// g *= *coef for every tensor of the table
+void launch_grad_scale_multi(const GradTensorList& tl, const float* coef, cudaStream_t st);
+
+#ifdef __CUDACC__
+// max that keeps a NaN (fmaxf drops it), as torch's inf-norm does
+__device__ __forceinline__ float nan_max(float a, float b) { return (a != a || a > b) ? a : b; }
+__device__ __forceinline__ double nan_max(double a, double b) { return (a != a || a > b) ? a : b; }
+// torch's clip coefficient, op for op in fp32: reciprocal(norm + 1e-6) · max_norm, then clamp(max=1), which keeps a NaN
+__device__ __forceinline__ float clip_coef(float norm, float max_norm) {
+  const float c = (1.f / (norm + 1e-6f)) * max_norm;
+  return c > 1.f ? 1.f : c;
+}
+#endif
+
 }  // namespace pdt

@@ -827,6 +827,72 @@ __global__ void __launch_bounds__(256) adam_multi_kernel(AdamTensorList tl, Adam
   }
 }
 
+// =====================================================================================================
+// Gradient-norm clipping: same layout as sgd_multi_kernel.  grad_norm_multi_kernel: every block writes one partial (fp32 Σg² or
+// max |g| of the elements it strides over, reduced over the block in a fixed order); on the set's last table, the block that
+// takes the last ticket folds the partials of every table in index order in fp64 and stores the norm and torch's clip
+// coefficient.  grad_scale_multi_kernel multiplies every gradient by that coefficient, read from device memory.
+// =====================================================================================================
+__global__ void __launch_bounds__(256) grad_norm_multi_kernel(GradTensorList tl, GradNormArgs a) {
+  const int t = blockIdx.y;
+  const int n = tl.n[t];
+  const float* __restrict__ g = tl.g[t];
+  float acc = 0.f;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float v = g[i];
+    acc = a.norm_inf ? nan_max(fabsf(v), acc) : fmaf(v, v, acc);
+  }
+  __shared__ float s_w[8];
+  __shared__ double s_d[256];
+  __shared__ bool s_last;
+#pragma unroll
+  for (int off = 16; off >= 1; off >>= 1) {
+    const float o = __shfl_xor_sync(0xffffffffu, acc, off);
+    acc = a.norm_inf ? nan_max(acc, o) : acc + o;
+  }
+  if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = s_w[0];
+    for (int w = 1; w < 8; ++w) s = a.norm_inf ? nan_max(s, s_w[w]) : s + s_w[w];
+    a.partials[a.part_base + t * gridDim.x + blockIdx.x] = s;
+    bool last = false;
+    if (a.last) {
+      __threadfence();
+      last = atomicAdd(a.ticket, 1u) == gridDim.x * gridDim.y - 1;
+    }
+    s_last = last;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  double d = 0.0;
+  for (int i = threadIdx.x; i < a.part_total; i += blockDim.x) {
+    const double v = static_cast<double>(__ldcg(a.partials + i));
+    d = a.norm_inf ? nan_max(d, v) : d + v;
+  }
+  s_d[threadIdx.x] = d;
+  __syncthreads();
+  for (int h = 128; h >= 1; h >>= 1) {
+    if (threadIdx.x < h) s_d[threadIdx.x] = a.norm_inf ? nan_max(s_d[threadIdx.x], s_d[threadIdx.x + h]) : s_d[threadIdx.x] + s_d[threadIdx.x + h];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const float norm = static_cast<float>(a.norm_inf ? s_d[0] : sqrt(s_d[0]));
+    a.out[0] = norm;
+    a.out[1] = clip_coef(norm, a.max_norm);
+    atomicExch(a.ticket, 0u);
+  }
+}
+
+__global__ void __launch_bounds__(256) grad_scale_multi_kernel(GradTensorList tl, const float* coef) {
+  const int t = blockIdx.y;
+  const int n = tl.n[t];
+  float* __restrict__ g = tl.g[t];
+  const float c = *coef;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) g[i] *= c;
+}
+
 size_t conv_smem(int cin, int cout, int th, int w, int threads) {
   return (static_cast<size_t>(cin) * (th + 4) * (w + 4) + 4 + 25 * cin * cout + (threads / 32 + 1) * 2 * cout) * sizeof(float);
 }
@@ -1009,6 +1075,24 @@ void launch_adam_multi(const AdamTensorList& tl, AdamHyper h, unsigned int* tick
   const int bx = std::max(1, std::min(64, (maxn + 1023) / 1024));
   adam_multi_kernel<<<dim3(bx, tl.count), 256, 0, st>>>(tl, h, ticket);
   check_launch("adam_multi");
+}
+
+int grad_multi_blocks_x(const GradTensorList& tl) {
+  int maxn = 0;
+  for (int i = 0; i < tl.count; ++i) maxn = std::max(maxn, tl.n[i]);
+  return std::max(1, std::min(64, (maxn + 1023) / 1024));
+}
+
+void launch_grad_norm_multi(const GradTensorList& tl, GradNormArgs a, cudaStream_t st) {
+  if (tl.count == 0) return;
+  grad_norm_multi_kernel<<<dim3(grad_multi_blocks_x(tl), tl.count), 256, 0, st>>>(tl, a);
+  check_launch("grad_norm_multi");
+}
+
+void launch_grad_scale_multi(const GradTensorList& tl, const float* coef, cudaStream_t st) {
+  if (tl.count == 0) return;
+  grad_scale_multi_kernel<<<dim3(grad_multi_blocks_x(tl), tl.count), 256, 0, st>>>(tl, coef);
+  check_launch("grad_scale_multi");
 }
 
 }  // namespace pdt

@@ -20,6 +20,13 @@ broadcast: every rank must have finished step k before anyone leaves the broadca
 safe as is — this is the ConvNet/ResNet case; (b) otherwise the step is captured twice (the second
 capture starts on the other half) and replays alternate between the two graphs, which reproduces
 exactly the eager alternation.
+
+Gradient-norm clipping (``max_grad_norm``, as ``torch.nn.utils.clip_grad_norm_`` between backward and ``optimizer.step()``):
+on one GPU, when the update rides on the last backward kernel, that kernel clips before it updates (still three launches);
+otherwise the native clip runs between backward and ``step()`` inside the graph (two launches).  With clipping the optimizer
+is not fused into the gradient reduction: the reducer averages, the step clips, then ``step()`` runs.  The averaged gradients
+are bitwise identical on every rank and the norm is reproducible bit for bit, so every rank derives the same coefficient
+without a collective.
 """
 from __future__ import annotations
 
@@ -32,7 +39,8 @@ import torch
 
 class GraphedTrainStep:
     def __init__(self, model, criterion, optimizer, example_inputs: Sequence[torch.Tensor], warmup: int = 3,
-                 zero_grad_set_to_none: bool = True, fuse_optimizer: bool = True, double_buffer_inputs: bool = True):
+                 zero_grad_set_to_none: bool = True, fuse_optimizer: bool = True, double_buffer_inputs: bool = True,
+                 max_grad_norm: Optional[float] = None, norm_type: float = 2.0):
         if not torch.cuda.is_available():
             raise RuntimeError("GraphedTrainStep needs CUDA")
         self.model, self.criterion, self.optimizer = model, criterion, optimizer
@@ -49,13 +57,30 @@ class GraphedTrainStep:
         self._last = 0
         self._seed: Optional[torch.Tensor] = None   # d(loss)/d(loss) = 1, allocated once (autograd would fill a new one per step)
         self.fused_optimizer = False
-        if fuse_optimizer and hasattr(optimizer, "fuse_with_ddp") and hasattr(model, "enable_optimizer_fusion"):
+        # gradient-norm clipping: the total norm of the last replay's gradients (a device scalar per captured graph, alternating
+        # with them as static_loss does)
+        if max_grad_norm is not None and not float(max_grad_norm) > 0:
+            raise ValueError(f"max_grad_norm must be positive, got {max_grad_norm}")
+        self.max_grad_norm = None if max_grad_norm is None else float(max_grad_norm)
+        self.norm_type = float(norm_type)
+        self.grad_norm: Optional[torch.Tensor] = None
+        self._clip_params = [p for g in optimizer.param_groups for p in g["params"]]
+        self._rider_norms = [torch.zeros((), device=self.static_inputs[0].device) for _ in range(2)] if self.max_grad_norm is not None else []
+        self._riding = False
+        if fuse_optimizer and self.max_grad_norm is None and hasattr(optimizer, "fuse_with_ddp") and hasattr(model, "enable_optimizer_fusion"):
             optimizer.fuse_with_ddp(model)
             warmup = max(warmup, 4)  # bucket rebuild after step 1, fusion switches on after step 2
         if fuse_optimizer and hasattr(optimizer, "ride_on_backward"):
-            optimizer.ride_on_backward(model)   # one GPU: the update rides on the model's last backward kernel (no-op when it cannot)
+            # one GPU: the update (and the clipping) rides on the model's last backward kernel (no-op when it cannot)
+            self._riding = bool(self._ride(0))
         self._capture(warmup)
         self.fused_optimizer = bool(getattr(optimizer, "_fused_active", False))
+
+    def _ride(self, k: int) -> bool:
+        """(Re-)arm the riding update; with clipping, the rider stores the norm in the device scalar of graph k."""
+        if self.max_grad_norm is None:
+            return self.optimizer.ride_on_backward(self.model)
+        return self.optimizer.ride_on_backward(self.model, clip=(self.max_grad_norm, self.norm_type, self._rider_norms[k]))
 
     def _eager_step(self, inputs=None):
         inputs = self.static_inputs if inputs is None else inputs
@@ -72,8 +97,16 @@ class GraphedTrainStep:
             self._seed._pdt_unit_seed = True   # lets ops that pre-compute their unit-gradient backward skip the scaling kernel
         with OF.sgd_rider_enabled():   # an optimizer armed with ride_on_backward may apply its update inside this backward pass
             loss.backward(self._seed)
+        norm = None
+        if self.max_grad_norm is not None:
+            if getattr(self.optimizer, "_rode", False):
+                norm = OF._sgd_rider["clip"][2]   # the backward kernel clipped and updated
+            else:
+                from ..nn.utils import clip_grad_norm_
+
+                norm = clip_grad_norm_(self._clip_params, self.max_grad_norm, self.norm_type)
         self.optimizer.step()
-        return loss
+        return loss, norm
 
     def _capture(self, warmup: int):
         dev = self.static_inputs[0].device
@@ -93,22 +126,26 @@ class GraphedTrainStep:
         torch.cuda.synchronize(dev)
         comm = getattr(self.model, "comm", None)
         parity = (lambda: list(comm.parity_state())) if hasattr(comm, "parity_state") else (lambda: [])
-        self.graphs, self.losses = [], []
+        self.graphs, self.losses, self.norms = [], [], []
         p0 = parity()
         for k in range(2):
+            if self._riding and self.max_grad_norm is not None:
+                self._ride(k)   # each graph's rider stores the norm in its own scalar
             g = torch.cuda.CUDAGraph()
             before = _C.kernel_launch_count()
             with torch.cuda.graph(g, stream=side):
-                loss = self._eager_step(self.input_sets[k % len(self.input_sets)])
+                loss, norm = self._eager_step(self.input_sets[k % len(self.input_sets)])
             # how many of *our* kernels one replay runs (ATen glue kernels are not counted)
             self.kernels_per_replay = int(_C.kernel_launch_count() - before)
             self.graphs.append(g)
             self.losses.append(loss)
+            self.norms.append(norm)
             torch.cuda.synchronize(dev)
             ordered = getattr(self.model, "syncs_buffers_every_step", None)
             if not self.double_buffer and (parity() == p0 or (ordered is not None and ordered())):
                 break  # even number of staged collectives per step, or case (a): one graph replays safely
         self.graph, self.static_loss = self.graphs[0], self.losses[0]
+        self.grad_norm = None
         # the host side of a replay (input staging on a copy stream, ordering against the replays that use the buffers, losses to pinned
         # memory on a side stream) is native: csrc/engine/step_pipeline.cpp
         self._io = _C.StepPipeline(dev.index if dev.index is not None else torch.cuda.current_device(), len(self.graphs), self.static_loss)
@@ -126,6 +163,7 @@ class GraphedTrainStep:
         self.replays += 1
         self._last = i
         self.static_loss = self.losses[i]
+        self.grad_norm = self.norms[i]
         return self.static_loss
 
     def loss_to_host(self) -> "HostLoss":

@@ -1,4 +1,5 @@
 """Layers whose CUDA path is our own kernels."""
+from . import utils
 from .loss import CrossEntropyLoss
 
-__all__ = ["CrossEntropyLoss"]
+__all__ = ["CrossEntropyLoss", "utils"]

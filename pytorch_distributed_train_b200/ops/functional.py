@@ -174,7 +174,9 @@ _sgd_rider_enabled = False
 class sgd_rider_enabled:
     """The armed optimizer may ride on backward passes started inside this context only (engine.GraphedTrainStep wraps its step in it):
     a backward pass anywhere else — gradient inspection, clipping experiments, an eager loop — never updates parameters behind the
-    caller's back."""
+    caller's back.  Inside it the parameters are already updated when backward returns, so a clip call of the user's own between
+    backward and step sees the updated model; clipping is expressible through ``GraphedTrainStep(max_grad_norm=…)``, which lets the
+    rider clip the gradients before it applies the update."""
 
     def __enter__(self):
         global _sgd_rider_enabled
@@ -493,6 +495,19 @@ def adam_step(params, grads, exp_avgs, exp_avg_sqs, steps, lr, beta1=0.9, beta2=
     step counts on the device: the launch uses step + 1 for the bias corrections and stores it, so a replayed graph advances it."""
     _C.adam_multi(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), list(steps), float(lr), lr_tensor, float(beta1),
                   float(beta2), float(eps), float(weight_decay), bool(decoupled), bool(maximize))
+
+
+def grad_norm_clip(grads, max_norm, norm_type=2.0, scale=True) -> torch.Tensor:
+    """The total ``norm_type`` norm (2 or inf) of fp32 contiguous gradients on one device, and — with ``scale`` — every gradient
+    multiplied by torch's clip coefficient ``min(max_norm / (norm + 1e-6), 1)``: two launches per 48 tensors, graph-capturable,
+    the norm the same bit for bit from run to run.  Returns the norm as a 0-d device tensor; ``scale=False`` stops after the
+    norm, and ``grad_scale(grads, norm)`` applies the coefficient later."""
+    return _C.grad_norm_clip(list(grads), float(max_norm), float(norm_type), bool(scale))
+
+
+def grad_scale(grads, norm: torch.Tensor) -> None:
+    """Multiply every gradient by the clip coefficient of ``norm``, a tensor returned by :func:`grad_norm_clip`."""
+    _C.grad_scale(list(grads), norm)
 
 
 # ---- generic (NCHW) BatchNorm pieces used by parallel.SyncBatchNorm ------------------------------------------

@@ -2,6 +2,7 @@
 graph reads, and the checks that decide whether the update may ride on the reference ConvNet's last backward kernel."""
 from __future__ import annotations
 
+import math
 import os
 from typing import List, Optional
 
@@ -68,12 +69,30 @@ class RidingOptimizer(torch.optim.Optimizer):
             return None
         return params
 
-    def _arm_rider(self, kind: str, params, args) -> None:
+    @staticmethod
+    def _clip_qualifies(clip, params) -> bool:
+        """``clip = (max_norm, norm_type, norm_out)`` can ride: norm type 2 or inf, ``norm_out`` one fp32 element on the
+        parameters' device."""
+        max_norm, norm_type, out = clip
+        return (float(norm_type) in (2.0, math.inf) and isinstance(out, torch.Tensor) and out.numel() == 1
+                and out.dtype == torch.float32 and out.device == params[0].device)
+
+    def _arm_rider(self, kind: str, params, args, clip=None) -> None:
         from ..ops import functional as OF
+
+        if clip is not None:
+            # the rider tuple gains a trailing clip entry: the kernel clips the gradients to max_norm before the update and stores
+            # the total norm in norm_out
+            entry = (float(clip[0]), float(clip[1]), clip[2])
+            plain = args
+
+            def args(prev_grads):
+                t = plain(prev_grads)
+                return None if t is None else tuple(t) + (entry,)
 
         self._riding_params = params
         self._rode = False
-        OF._sgd_rider = {"kind": kind, "params": params, "args": args, "owner": self}
+        OF._sgd_rider = {"kind": kind, "params": params, "args": args, "owner": self, "clip": clip}
 
     def stop_riding(self) -> None:
         """Undo :meth:`ride_on_backward`."""

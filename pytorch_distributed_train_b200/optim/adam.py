@@ -101,12 +101,12 @@ class Adam(RidingOptimizer):
                     st["step"] = s.to(device=p.device, dtype=torch.float32).reshape(())
 
     # ---- single GPU: the update rides on the model's last backward kernel ---------------------------------
-    def ride_on_backward(self, model) -> bool:
+    def ride_on_backward(self, model, clip=None) -> bool:
         """Let the reference ConvNet's last backward kernel apply this optimizer's update (csrc/cuda/fused_convnet.cu: AdamRider).
-        Same contract and preconditions as :meth:`SGD.ride_on_backward`; ``amsgrad`` and ``fused=False`` do not ride.  Returns False
-        (and changes nothing) when the model / optimizer combination does not qualify."""
+        Same contract, preconditions and ``clip = (max_norm, norm_type, norm_out)`` as :meth:`SGD.ride_on_backward`; ``amsgrad`` and
+        ``fused=False`` do not ride.  Returns False (and changes nothing) when the model / optimizer combination does not qualify."""
         params = self._qualify_rider(model)
-        if params is None:
+        if params is None or (clip is not None and not self._clip_qualifies(clip, params)):
             return False
         group = self.param_groups[0]
         if group["amsgrad"] or group["fused"] is False:
@@ -125,7 +125,7 @@ class Adam(RidingOptimizer):
                     [st["step"] for st in states], float(g["lr"]), self._lr_tensor(0, g, params[0].device), float(beta1), float(beta2),
                     float(g["eps"]), float(g["weight_decay"]), bool(g["decoupled_weight_decay"]), bool(g["maximize"]))
 
-        self._arm_rider("adam", params, args)
+        self._arm_rider("adam", params, args, clip)
         return True
 
     # ---- the update ---------------------------------------------------------------------------------------------

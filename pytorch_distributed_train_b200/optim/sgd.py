@@ -44,16 +44,20 @@ class SGD(RidingOptimizer):
         self._flat_momentum = None
 
     # ---- single GPU: the update rides on the model's last backward kernel ---------------------------------
-    def ride_on_backward(self, model) -> bool:
+    def ride_on_backward(self, model, clip=None) -> bool:
         """Let the reference ConvNet's last backward kernel apply this optimizer's update (csrc/cuda/fused_convnet.cu: SgdRider): the
         thread that writes a folded gradient element updates the parameter with the value still in its register; the parameters whose
         gradients are complete earlier are updated in the shadow of that kernel's first grid barrier.  ``step()`` then has only
         bookkeeping left.  Used by ``engine.GraphedTrainStep`` when the gradient reduction does not already carry the update (one GPU).
 
+        ``clip = (max_norm, norm_type, norm_out)``: the kernel clips the gradient norm first, as ``clip_grad_norm_`` would
+        (ClipRider: one more grid barrier, then every gradient is scaled and updated in one pass; ``.grad`` reads the clipped
+        gradient and ``norm_out``, one fp32 element on the device, the total norm).  ``norm_type`` must be 2 or inf.
+
         Same contract as :meth:`fuse_with_ddp`: between ``backward()`` and ``step()`` the parameters are already updated.  Returns
         False (and changes nothing) when the model / optimizer combination does not qualify."""
         params = self._qualify_rider(model)
-        if params is None:
+        if params is None or (clip is not None and not self._clip_qualifies(clip, params)):
             return False
 
         def args(prev_grads):
@@ -76,7 +80,7 @@ class SGD(RidingOptimizer):
             return (params, list(prev_grads), bufs, float(g["lr"]), self._lr_tensor(0, g, params[0].device), float(g["momentum"]),
                     float(g["dampening"]), float(g["weight_decay"]), bool(g["nesterov"]), bool(g["maximize"]), first)
 
-        self._arm_rider("sgd", params, args)
+        self._arm_rider("sgd", params, args, clip)
         return True
 
     # ---- DDP fusion: the update rides on the gradient reduction ----------------------------------------
@@ -92,9 +96,11 @@ class SGD(RidingOptimizer):
         of the early ones.  The last chunk also carries DDP's per-step BatchNorm-buffer broadcast.
         ``step()`` then only has bookkeeping left; ``.grad`` reads as the averaged gradient, as in the reference.
 
-        Contract: between ``backward()`` and ``step()`` the parameters are already updated — gradient clipping or a
-        skipped ``step()`` are not expressible in this mode.  Takes effect on the first ``step()`` after the reducer
-        has settled its bucket layout; until then (and whenever the preconditions fail) the ordinary path runs."""
+        Contract: between ``backward()`` and ``step()`` the parameters are already updated — a clip call of the user's own
+        there sees an already-updated model, and a skipped ``step()`` is not expressible in this mode.  Clipping is expressible
+        through ``engine.GraphedTrainStep(max_grad_norm=…)``, which does not fuse the optimizer into the reduction then.  Takes
+        effect on the first ``step()`` after the reducer has settled its bucket layout; until then (and whenever the
+        preconditions fail) the ordinary path runs."""
         self._ddp = ddp
         return self
 

@@ -5,11 +5,17 @@
   torch AdamW(capturable=True, foreach=True) (torch's multi-tensor kernels, replayed inside the same graph)
   torch AdamW(capturable=True, fused=True)   (torch's fused kernel, replayed inside the same graph)
 
+With ``--max-grad-norm X`` four more arms clip the global gradient norm to X in the same rounds:
+
+  pdt SGD / pdt AdamW with clipping, riding   (the last backward kernel clips, then updates: still 3 launches)
+  pdt AdamW with clipping, not riding          (GraphedTrainStep(fuse_optimizer=False): native clip + Adam kernel after backward)
+  torch clip_grad_norm_(foreach=True) + AdamW(capturable=True, fused=True) in the same graph
+
 Every optimizer gets its own model (same initial weights) and its own ``engine.GraphedTrainStep``.  Inputs rotate through a
 device-resident pool larger than L2, as in bench.py; the steps are timed with CUDA events, in rounds that alternate between the
 optimizers so that clock drift hits all of them alike.  Prints the card, its power limit and one JSON line.
 
-Usage: python tools/optim_step_bench.py [--steps 200] [--warmup 20] [--rounds 5]
+Usage: python tools/optim_step_bench.py [--steps 200] [--warmup 20] [--rounds 5] [--max-grad-norm 1.0]
 """
 import argparse
 import json
@@ -34,11 +40,28 @@ def power_limit_w():
         return None
 
 
+class _TorchClip:
+    """torch.optim optimizer whose step() first runs torch.nn.utils.clip_grad_norm_(foreach=True): the torch arm of the clipped
+    step, captured in the same graph as ours."""
+
+    def __init__(self, opt, params, max_norm):
+        self.opt, self.params, self.max_norm = opt, params, max_norm
+        self.param_groups = opt.param_groups
+
+    def zero_grad(self, set_to_none=True):
+        self.opt.zero_grad(set_to_none=set_to_none)
+
+    def step(self):
+        torch.nn.utils.clip_grad_norm_(self.params, self.max_norm, foreach=True)
+        self.opt.step()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=200, help="timed steps per optimizer and round")
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--max-grad-norm", type=float, default=None, help="also time the arms that clip the gradient norm to this value")
     args = ap.parse_args()
 
     import pytorch_distributed_train_b200 as pdt
@@ -59,13 +82,25 @@ def main():
         "torch_adamw_foreach": lambda ps: torch.optim.AdamW(ps, lr, capturable=True, foreach=True),
         "torch_adamw_fused": lambda ps: torch.optim.AdamW(ps, lr, capturable=True, fused=True),
     }
+    # name -> GraphedTrainStep keyword arguments of the arm
+    kwargs = {name: {} for name in makers}
+    if args.max_grad_norm is not None:
+        mg = args.max_grad_norm
+        makers.update({
+            "pdt_sgd_clip": lambda ps: pdt.optim.SGD(ps, lr),
+            "pdt_adamw_clip": lambda ps: pdt.optim.AdamW(ps, lr),
+            "pdt_adamw_clip_unfused": lambda ps: pdt.optim.AdamW(ps, lr),
+            "torch_clip_adamw_fused": lambda ps: _TorchClip(torch.optim.AdamW(ps, lr, capturable=True, fused=True), ps, mg),
+        })
+        kwargs.update({"pdt_sgd_clip": {"max_grad_norm": mg}, "pdt_adamw_clip": {"max_grad_norm": mg},
+                       "pdt_adamw_clip_unfused": {"max_grad_norm": mg, "fuse_optimizer": False}, "torch_clip_adamw_fused": {}})
     crit = pdt.nn.CrossEntropyLoss()
     steps = {}
     for name, make in makers.items():
         model = pdt.models.ConvNet().to(dev)
         model.load_state_dict(init)
-        opt = make(model.parameters())
-        steps[name] = (GraphedTrainStep(model, crit, opt, (xs[0], ys[0]), warmup=3), opt)
+        opt = make(list(model.parameters()))
+        steps[name] = (GraphedTrainStep(model, crit, opt, (xs[0], ys[0]), warmup=3, **kwargs[name]), opt)
         if hasattr(opt, "stop_riding"):
             opt.stop_riding()   # the captured graph keeps the rider; disarm it so that the next model captures on its own
 
@@ -98,6 +133,7 @@ def main():
         "kernels_per_replay": {name: steps[name][0].kernels_per_replay for name in makers},
         "ms_per_step_median": {name: round(statistics.median(v), 5) for name, v in per.items()},
         "ms_per_step_min": {name: round(min(v), 5) for name, v in per.items()},
+        "max_grad_norm": args.max_grad_norm,
     }
     print(f"{result['card']}, power limit {result['power_limit_w']} W")
     for name in makers:
