@@ -847,7 +847,7 @@ void launch_conv5x5_fwd_gather(const float* x, const float* w, const float* bias
   using Cfg = ConvCfg<16, 32>;
   const int M = s.B * s.H * s.W;
   const int tiles = (M + kTileM - 1) / kTileM;
-  if (stats && (static_cast<long long>(tiles + tiles / kFoldGroup + 1) * 64 > scr.capacity_floats || tiles / kFoldGroup + 2 > scr.counters))
+  if (stats && (static_cast<long long>(tiles + tiles / kFoldGroup + 1) * 64 > scr.capacity_floats || tiles / kFoldGroup + 2 > scr.fold_counters))
     throw std::invalid_argument("conv5x5 gather: scratch too small");
   const int kpad = Cfg::kChunks * kChunkK;
   float* bm = repack_buffer(0, static_cast<size_t>(32) * kpad);
@@ -885,7 +885,7 @@ void launch_conv5x5_fwd_im2col(const float* x, const float* w, const float* bias
   using Cfg = ConvTmaCfg<16, 32>;
   const int M = s.B * s.H * s.W;
   const int tiles = (M + kTileM - 1) / kTileM;
-  if (stats && (static_cast<long long>(tiles + tiles / kFoldGroup + 1) * 64 > scr.capacity_floats || tiles / kFoldGroup + 2 > scr.counters))
+  if (stats && (static_cast<long long>(tiles + tiles / kFoldGroup + 1) * 64 > scr.capacity_floats || tiles / kFoldGroup + 2 > scr.fold_counters))
     throw std::invalid_argument("conv5x5 im2col: scratch too small");
   float* bm = repack_buffer(3, static_cast<size_t>(32) * 400);
   repack_weights_dense_kernel<true><<<(32 * 400 + 255) / 256, 256, 0, st>>>(w, bm, 32, 16);

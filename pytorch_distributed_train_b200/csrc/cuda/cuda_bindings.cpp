@@ -54,18 +54,20 @@ ReduceScratch scratch(const at::Tensor& like) {
   auto it = per_dev.find(dev);
   if (it == per_dev.end()) {
     Scratch s;
-    const int64_t cap = 4 << 20;  // 4 Mi floats = 16 MiB
-    s.partials = at::empty({cap}, like.options().dtype(at::kFloat));
-    s.counter = at::zeros({1024}, like.options().dtype(at::kInt));
+    s.partials = at::empty({kScratchFloats}, like.options().dtype(at::kFloat));
+    s.counter = at::zeros({kCounterWords}, like.options().dtype(at::kInt));   // layout: ops_kernels.h
     it = per_dev.emplace(dev, std::move(s)).first;
   }
   ReduceScratch r;
   r.partials = it->second.partials.data_ptr<float>();
   r.counter = reinterpret_cast<unsigned int*>(it->second.counter.data_ptr<int>());
   r.capacity_floats = static_cast<int>(it->second.partials.numel());
-  r.counters = static_cast<int>(it->second.counter.numel());
+  r.fold_counters = kFoldCounterWords;
   return r;
 }
+
+// The grid barrier of the cooperative kernels lives in the fixed words behind the fold region.
+GridSync grid_sync(const ReduceScratch& r) { return GridSync{r.counter + kGridEpochWord, r.counter + kGridArrivalWord}; }
 
 // Kernel family of the per-op conv2, selected by the `impl` argument of the conv5x5_* bindings:
 //   auto, tma → TMA-im2col wgmma forward / data gradient;
@@ -213,7 +215,7 @@ void register_cuda_bindings(py::module_& m) {
     launch_convnet_l1_fwd(x.data_ptr<float>(), w.data_ptr<float>(), opt_ptr(bias, "bias"), opt_ptr(gamma, "gamma"), opt_ptr(beta, "beta"),
                           y.data_ptr<float>(), out.data_ptr<float>(), saved.data_ptr<float>(), opt_mut(running_mean, "running_mean"),
                           opt_mut(running_var, "running_var"), nbt_p, static_cast<float>(momentum), static_cast<float>(eps), B, scr.partials,
-                          GridSync{scr.counter + 512, scr.counter + 520}, cur_stream(x));
+                          grid_sync(scr), cur_stream(x));
     return py::make_tuple(out, y, saved);
   });
   m.def("convnet_l1_bwd", [](const at::Tensor& dp, const at::Tensor& y, const at::Tensor& x, const at::Tensor& saved,
@@ -228,7 +230,7 @@ void register_cuda_bindings(py::module_& m) {
     launch_convnet_l1_bwd(dp.data_ptr<float>(), y.data_ptr<float>(), x.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"),
                           opt_ptr(beta, "beta"), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"), B,
                           scr.partials, scr.partials + static_cast<size_t>(B) * 64,
-                          GridSync{scr.counter + 512, scr.counter + 520}, cur_stream(x));
+                          grid_sync(scr), cur_stream(x));
   });
   m.def("convnet_l1_bwd_wgrad", [](const at::Tensor& dp, const at::Tensor& y, const at::Tensor& x, const at::Tensor& saved,
                                    c10::optional<at::Tensor> gamma, c10::optional<at::Tensor> beta, at::Tensor dgamma, at::Tensor dbeta, at::Tensor dw,
@@ -256,7 +258,7 @@ void register_cuda_bindings(py::module_& m) {
                                   opt_ptr(beta, "beta"), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"),
                                   dy2_pad.data_ptr<float>(), x2_pad.data_ptr<float>(), dysum2.data_ptr<float>(), dw2.data_ptr<float>(),
                                   opt_mut(db2, "db2"), B, scr.partials, scr.partials + static_cast<size_t>(B) * 64, scr.partials + l1_floats,
-                                  GridSync{scr.counter + 512, scr.counter + 520}, cur_stream(x), rider);
+                                  grid_sync(scr), cur_stream(x), rider);
     };
     // the clip entry of a rider tuple → the clipping variant of the rider
     auto clipped = [&](auto base, const py::handle& entry) {
@@ -392,7 +394,7 @@ void register_cuda_bindings(py::module_& m) {
                           opt_mut(running_var, "running_var"), nbt_p, static_cast<float>(momentum), static_cast<float>(eps),
                           ncls ? fcw->data_ptr<float>() : nullptr, ncls ? opt_ptr(fcb, "fc bias") : nullptr,
                           ncls ? logits.data_ptr<float>() : nullptr, ncls, B, scr.partials,
-                          GridSync{scr.counter + 512, scr.counter + 520}, cur_stream(x));
+                          grid_sync(scr), cur_stream(x));
     return py::make_tuple(out, y, saved, logits);
   });
   m.def("convnet_fwd", [](const at::Tensor& x, const at::Tensor& w1, c10::optional<at::Tensor> b1, c10::optional<at::Tensor> g1,
@@ -423,19 +425,19 @@ void register_cuda_bindings(py::module_& m) {
       TORCH_CHECK(target->numel() == B, "convnet_fwd: one target per image expected");
       loss = at::empty({}, x.options());
       dlogits = at::empty({B, ncls}, x.options());
-      loss_parts = at::empty({B}, x.options());
+      loss_parts = at::empty({B + 1}, x.options());   // one term per image, then the number of counted images
       ce.target = reinterpret_cast<const long long*>(target->data_ptr<int64_t>());
       ce.loss_parts = loss_parts.data_ptr<float>();
       ce.loss = defer_loss_mean ? nullptr : loss.data_ptr<float>();   // deferred: convnet_l2_bwd_fc(…, loss_parts, loss) writes it
       ce.dlogits = dlogits.data_ptr<float>();
-      ce.counter = scr.counter + 528;
+      ce.counter = scr.counter + kCeCounterWord;
     }
     launch_convnet_fwd(x.data_ptr<float>(), w1.data_ptr<float>(), opt_ptr(b1, "b1"), opt_ptr(g1, "g1"), opt_ptr(be1, "be1"), y1.data_ptr<float>(),
                        p1.data_ptr<float>(), saved1.data_ptr<float>(), opt_mut(rm1, "rm1"), opt_mut(rv1, "rv1"), nbt_ptr(nbt1), static_cast<float>(mom1),
                        static_cast<float>(eps1), w2.data_ptr<float>(), opt_ptr(b2, "b2"), opt_ptr(g2, "g2"), opt_ptr(be2, "be2"), y2.data_ptr<float>(),
                        out.data_ptr<float>(), saved2.data_ptr<float>(), opt_mut(rm2, "rm2"), opt_mut(rv2, "rv2"), nbt_ptr(nbt2), static_cast<float>(mom2),
                        static_cast<float>(eps2), fcw.data_ptr<float>(), opt_ptr(fcb, "fc bias"), logits.data_ptr<float>(), ncls, B, scr.partials,
-                       GridSync{scr.counter + 512, scr.counter + 520}, cur_stream(x), ce);
+                       grid_sync(scr), cur_stream(x), ce);
     return py::make_tuple(p1, y1, saved1, out, y2, saved2, logits, loss, dlogits, loss_parts);
   }, py::arg("x"), py::arg("w1"), py::arg("b1"), py::arg("g1"), py::arg("be1"), py::arg("rm1"), py::arg("rv1"), py::arg("nbt1"), py::arg("mom1"),
      py::arg("eps1"), py::arg("w2"), py::arg("b2"), py::arg("g2"), py::arg("be2"), py::arg("rm2"), py::arg("rv2"), py::arg("nbt2"), py::arg("mom2"),
@@ -453,7 +455,7 @@ void register_cuda_bindings(py::module_& m) {
     ReduceScratch scr = scratch(y);
     launch_convnet_l2_bwd(dout.data_ptr<float>(), y.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"), opt_ptr(beta, "beta"),
                           w.data_ptr<float>(), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dy.data_ptr<float>(), dx.data_ptr<float>(),
-                          dysum.data_ptr<float>(), B, scr.partials, GridSync{scr.counter + 512, scr.counter + 520},
+                          dysum.data_ptr<float>(), B, scr.partials, grid_sync(scr),
                           cur_stream(y));
     return py::make_tuple(dy, dx, dysum);
   });
@@ -470,6 +472,8 @@ void register_cuda_bindings(py::module_& m) {
                     pooled.numel() == static_cast<int64_t>(B) * 1568 && dfcw.numel() == fcw.numel() && y.numel() == static_cast<int64_t>(B) * 6272 &&
                     w.numel() == 12800 && dgamma.numel() == 32 && dbeta.numel() == 32, "convnet_l2_bwd_fc: shape mismatch");
     TORCH_CHECK(reinterpret_cast<uintptr_t>(fcw.data_ptr()) % 16 == 0, "convnet_l2_bwd_fc: fc weight must be 16-byte aligned");
+    TORCH_CHECK(!loss_parts.has_value() || !loss_parts->defined() || (loss_parts->numel() == B + 1 && loss_out.has_value() && loss_out->defined()),
+                "convnet_l2_bwd_fc: loss_parts must be the [B + 1] tensor of convnet_fwd, and loss_out given with it");
     at::Tensor dy = at::empty({B, 18, 18, 32}, y.options());
     at::Tensor dx = at::empty({B, 18, 18, 16}, y.options());
     at::Tensor dysum = at::empty({B, 32}, y.options());
@@ -477,7 +481,7 @@ void register_cuda_bindings(py::module_& m) {
     launch_convnet_l2_bwd_fc(dlogits.data_ptr<float>(), fcw.data_ptr<float>(), pooled.data_ptr<float>(), dfcw.data_ptr<float>(), opt_mut(dfcb, "dfcb"),
                              ncls, y.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"), opt_ptr(beta, "beta"), w.data_ptr<float>(),
                              dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dy.data_ptr<float>(), dx.data_ptr<float>(), dysum.data_ptr<float>(), B,
-                             scr.partials, GridSync{scr.counter + 512, scr.counter + 520}, cur_stream(y), opt_ptr(loss_parts, "loss_parts"),
+                             scr.partials, grid_sync(scr), cur_stream(y), opt_ptr(loss_parts, "loss_parts"),
                              opt_mut(loss_out, "loss_out"));
     return py::make_tuple(dy, dx, dysum);
   }, py::arg("dlogits"), py::arg("fcw"), py::arg("pooled"), py::arg("dfcw"), py::arg("dfcb"), py::arg("y"), py::arg("saved"), py::arg("gamma"),
@@ -490,26 +494,34 @@ void register_cuda_bindings(py::module_& m) {
                     dysum.numel() == static_cast<int64_t>(B) * 32 && dw.numel() == 12800, "conv5x5_wgrad_win: shape mismatch");
     ReduceScratch scr = scratch(dy_pad);
     launch_conv5x5_wgrad_win(dy_pad.data_ptr<float>(), x_pad.data_ptr<float>(), dysum.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"), B,
-                             scr, cur_stream(dy_pad), GridSync{scr.counter + 512, scr.counter + 520});
+                             scr, cur_stream(dy_pad), grid_sync(scr));
   }, py::arg("dy_pad"), py::arg("x_pad"), py::arg("dysum"), py::arg("dw"), py::arg("db") = py::none());
 
   // ---- BN + ReLU + pool ------------------------------------------------------------------------------
   m.def("bn_relu_pool_fwd", [](const at::Tensor& y, const at::Tensor& stats, c10::optional<at::Tensor> gamma, c10::optional<at::Tensor> beta,
                                c10::optional<at::Tensor> running_mean, c10::optional<at::Tensor> running_var,
-                               c10::optional<at::Tensor> nbt, double momentum, double eps, bool out_nchw) {
+                               c10::optional<at::Tensor> nbt, double momentum, double eps, bool out_nchw, bool mean_var) {
     chk(y, "y"); chk(stats, "stats");
     c10::cuda::CUDAGuard g(y.device());
+    TORCH_CHECK(y.dim() == 4, "bn_relu_pool_fwd: y [B,H,W,C] expected");
     const int B = y.size(0), H = y.size(1), W = y.size(2), C = y.size(3);
-    TORCH_CHECK(stats.numel() == 2 * C + 1, "bn_relu_pool_fwd: stats must have 2C+1 entries");
+    if (mean_var) {
+      TORCH_CHECK(stats.numel() == 2 * C, "bn_relu_pool_fwd: mean_var stats must have 2C entries (mean, var)");
+      TORCH_CHECK(!(running_mean.has_value() && running_mean->defined()) && !(running_var.has_value() && running_var->defined()) &&
+                      !(nbt.has_value() && nbt->defined()), "bn_relu_pool_fwd: mean_var statistics update no running statistics");
+    } else {
+      TORCH_CHECK(stats.numel() == 2 * C + 1, "bn_relu_pool_fwd: stats must have 2C+1 entries");
+    }
     at::Tensor out = out_nchw ? at::empty({B, C, H / 2, W / 2}, y.options()) : at::empty({B, H / 2, W / 2, C}, y.options());
     at::Tensor saved = at::empty({2 * C}, y.options());
     long long* nbt_p = nullptr;
     if (nbt.has_value() && nbt->defined()) { chk(*nbt, "num_batches_tracked", at::kLong); nbt_p = reinterpret_cast<long long*>(nbt->data_ptr<int64_t>()); }
     launch_bn_relu_pool_fwd(y.data_ptr<float>(), stats.data_ptr<float>(), opt_ptr(gamma, "gamma"), opt_ptr(beta, "beta"), out.data_ptr<float>(),
                             saved.data_ptr<float>(), opt_mut(running_mean, "running_mean"), opt_mut(running_var, "running_var"), nbt_p,
-                            static_cast<float>(momentum), static_cast<float>(eps), B, H, W, C, out_nchw, cur_stream(y));
+                            static_cast<float>(momentum), static_cast<float>(eps), B, H, W, C, out_nchw, mean_var, cur_stream(y));
     return py::make_tuple(out, saved);
-  });
+  }, py::arg("y"), py::arg("stats"), py::arg("gamma"), py::arg("beta"), py::arg("running_mean"), py::arg("running_var"), py::arg("nbt"),
+     py::arg("momentum"), py::arg("eps"), py::arg("out_nchw"), py::arg("mean_var") = false);
   m.def("bn_relu_pool_bwd_reduce", [](const at::Tensor& dout, const at::Tensor& y, const at::Tensor& saved, c10::optional<at::Tensor> gamma,
                                       c10::optional<at::Tensor> beta, bool dout_nchw, c10::optional<at::Tensor> dgamma_out,
                                       c10::optional<at::Tensor> dbeta_out) {
@@ -681,7 +693,7 @@ void register_cuda_bindings(py::module_& m) {
     cudaStream_t st = cur_stream(params[0]);
     // the ticket word of the step hand-over (adam_multi_kernel); launches on one device are ordered by the compute stream, and
     // every launch leaves the word at zero
-    unsigned int* ticket = scratch(params[0]).counter + 536;
+    unsigned int* ticket = scratch(params[0]).counter + kAdamTicketWord;
     for (size_t base = 0; base < n; base += AdamTensorList::kMax) {
       AdamTensorList tl;
       tl.count = static_cast<int>(std::min<size_t>(AdamTensorList::kMax, n - base));
@@ -731,7 +743,7 @@ void register_cuda_bindings(py::module_& m) {
     // the ticket word of the fold (grad_norm_multi_kernel): launches on one device are ordered by the compute stream, and every
     // set leaves the word at zero
     GradNormArgs a{scr.partials, 0, total, 0, std::isinf(norm_type) ? 1 : 0, static_cast<float>(max_norm), out.data_ptr<float>(),
-                   scr.counter + 544};
+                   scr.counter + kClipTicketWord};
     for (size_t k = 0; k < tables.size(); ++k) {
       a.last = k + 1 == tables.size() ? 1 : 0;
       launch_grad_norm_multi(tables[k], a, st);

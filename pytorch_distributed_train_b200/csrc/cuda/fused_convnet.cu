@@ -1216,10 +1216,24 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
   trace(0, 6);
   bar.arrive(gs);
   float* fcs = reinterpret_cast<float*>(sb + 8192);   // classifier weights, staged behind the pooled activations (conv2's weights are dead)
-  const bool fc_staged = logits != nullptr && (reinterpret_cast<uintptr_t>(fcw) & 15) == 0;
+  // only where they fit before ys, which is still being read: up to 15 classes; 16 are read from global memory
+  const bool fc_staged = logits != nullptr && (reinterpret_cast<uintptr_t>(fcw) & 15) == 0 && ncls * 1568 * 4 <= L2FwdSmem::kB - 8192;
   if (fc_staged) {
     for (int i = tid; i < ncls * 392; i += kL1Threads) cp_async_16(smem_u32(fcs + 4 * i), fcw + 4 * i, 16);
     cp_async_commit();
+  }
+  __shared__ int s_counted;
+  if (ce.target != nullptr && warp == 0) {
+    // in the barrier's shadow: the cross-entropy's mean is over the images whose target lies in [0, ncls) (torch's ignore_index);
+    // every CTA counts them, B ≤ one per SM
+    int counted = 0;
+#pragma unroll 4
+    for (int r = lane; r < B; r += 32) {
+      const long long tr = ce.target[r];
+      counted += (tr >= 0 && tr < ncls) ? 1 : 0;
+    }
+    counted = __reduce_add_sync(0xffffffffu, counted);
+    if (lane == 0) s_counted = counted;
   }
   for (int i = tid; i < 196 * 8; i += kL1Threads) {   // in the barrier's shadow: conv2's output for the backward pass
     const int pix = i >> 3, q = i & 7;
@@ -1298,7 +1312,9 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
       }
       trace(0, 9);
       if (ce.target != nullptr) {
-        // cross-entropy of this image and its gradient for a unit incoming gradient
+        // cross-entropy of this image and its gradient for a unit incoming gradient, divided by the number of counted images; an
+        // ignored image adds no term and gets a zero gradient
+        const int counted = s_counted;
         float mx = lg;
 #pragma unroll
         for (int off = 16; off >= 1; off >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
@@ -1309,8 +1325,10 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
         const long long t = ce.target[n];
         const bool t_ok = t >= 0 && t < ncls;
         const float lt = __shfl_sync(0xffffffffu, lg, t_ok ? static_cast<int>(t) : 0);
-        if (lane < ncls) ce.dlogits[static_cast<size_t>(n) * ncls + lane] = (e / ssum - (t == lane ? 1.f : 0.f)) / static_cast<float>(B);
+        if (lane < ncls)
+          ce.dlogits[static_cast<size_t>(n) * ncls + lane] = t_ok ? (e / ssum - (t == lane ? 1.f : 0.f)) / static_cast<float>(counted) : 0.f;
         if (lane == 0) ce.loss_parts[n] = t_ok ? mx + __logf(ssum) - lt : 0.f;
+        if (lane == 0 && n == 0) ce.loss_parts[B] = static_cast<float>(counted);   // for a mean folded later
         if (ce.loss != nullptr) {   // batch mean now (otherwise layer-2 backward folds it: ce.loss == nullptr)
           int last = 0;
           if (lane == 0) {
@@ -1325,7 +1343,7 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
 #pragma unroll
             for (int off = 16; off >= 1; off >>= 1) sl += __shfl_xor_sync(0xffffffffu, sl, off);
             if (lane == 0) {
-              *ce.loss = sl / static_cast<float>(B);
+              *ce.loss = sl / static_cast<float>(counted);
               *ce.counter = 0u;
             }
           }
@@ -1528,12 +1546,13 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
           for (int r = 0; r < B; ++r) a += s_dl[r * 16 + tid];
           dfcb[tid] = a;
         }
-        if (loss_parts != nullptr && warp == 7) {   // the forward kernel left one cross-entropy term per image: batch mean, fixed order
+        if (loss_parts != nullptr && warp == 7) {   // the forward kernel left one cross-entropy term per image and the number of
+          const float counted = __ldg(loss_parts + B);   // counted images after them: batch mean, fixed order
           float sl = 0.f;
           for (int r = lane; r < B; r += 32) sl += __ldg(loss_parts + r);
 #pragma unroll
           for (int off = 16; off >= 1; off >>= 1) sl += __shfl_xor_sync(0xffffffffu, sl, off);
-          if (lane == 0) *loss_out = sl / static_cast<float>(B);
+          if (lane == 0) *loss_out = sl / counted;
         }
       }
     }

@@ -75,11 +75,12 @@ void launch_convnet_l2_fwd(const float* x, const float* w, const float* bias, co
                            float* saved, float* running_mean, float* running_var, long long* nbt, float momentum, float eps,
                            const float* fcw, const float* fcb, float* logits, int ncls, int B, float* partials, GridSync gs, cudaStream_t st);
 // Optional rider of the whole-forward kernel: the mean cross-entropy of the logits against `target` and its gradient
-// (softmax − onehot)/B, computed by the CTA that owns the image; the batch mean is folded by the CTA that finishes last
-// (arrival counter, fixed summation order).  target == nullptr: off.
+// (softmax − onehot)/n, computed by the CTA that owns the image; the batch mean is folded by the CTA that finishes last
+// (arrival counter, fixed summation order).  n counts the images whose target is in [0, ncls); the others (ignore_index) add
+// no term and get a zero gradient, and n = 0 gives a NaN loss, as in torch.  target == nullptr: off.
 struct FusedCe {
   const long long* target = nullptr;   // [B]
-  float* loss_parts = nullptr;         // [B] scratch
+  float* loss_parts = nullptr;         // [B + 1] scratch: one term per image, then n
   float* loss = nullptr;               // scalar; nullptr = the mean is folded later (launch_convnet_l2_bwd_fc)
   float* dlogits = nullptr;            // [B, ncls]
   unsigned int* counter = nullptr;     // zero before first use; reset by the kernel
@@ -101,6 +102,6 @@ void launch_convnet_l2_bwd(const float* dout, const float* y, const float* saved
 void launch_convnet_l2_bwd_fc(const float* dlogits, const float* fcw, const float* pooled, float* dfcw, float* dfcb, int ncls, const float* y,
                               const float* saved, const float* gamma, const float* beta, const float* w, float* dgamma, float* dbeta, float* dy,
                               float* dx, float* dysum, int B, float* partials, GridSync gs, cudaStream_t st,
-                              const float* loss_parts = nullptr, float* loss_out = nullptr);   // batch mean of the forward kernel's CE terms
+                              const float* loss_parts = nullptr, float* loss_out = nullptr);   // mean of the forward kernel's CE terms
 
 }  // namespace pdt

@@ -55,7 +55,8 @@ __device__ __forceinline__ float fold_rows(const float* rows, int nrows, int wid
 
 // blk_vals: this contributor's `width` partial values (visible to all participating threads).
 // bid / nblk: linear id of this contributor and the number of contributors.
-// scr.partials must hold (nblk + ceil(nblk/16)) * width floats; scr.counter ≥ 1 + ceil(nblk/16) zeroed uints.
+// scr.partials must hold (nblk + ceil(nblk/16)) * width floats; the fold region of scr.counter (ops_kernels.h: words
+// [0, scr.fold_counters), which no fixed counter word shares) must hold 1 + ceil(nblk/16) zeroed uints.
 // s_flag: one int of shared memory; s_tmp: ≥ nthreads floats of shared memory.
 template <typename Sync, typename Fin>
 __device__ __forceinline__ void grid_fold(const float* blk_vals, int width, int bid, int nblk, ReduceScratch scr, float* s_tmp, int* s_flag,

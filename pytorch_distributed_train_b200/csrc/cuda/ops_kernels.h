@@ -12,13 +12,32 @@ struct ConvShape {
   int B, H, W, Cin, Cout;  // 5x5, stride 1, pad 2 ("same")
 };
 
-// Scratch for deterministic cross-CTA reductions: partials[max_blocks][width] + a ticket counter.
+// Scratch for deterministic cross-CTA reductions: partials[max_blocks][width] + ticket counters.
 struct ReduceScratch {
   float* partials;
-  unsigned int* counter;  // `counters` ticket words; zero before first use, kernels leave them at zero
+  unsigned int* counter;  // the per-device counter words laid out below; zero before first use, kernels leave them at zero
   int capacity_floats;
-  int counters;
+  int fold_counters;      // words of the fold region, counter[0, fold_counters)
 };
+
+// Per-device reduction scratch: kScratchFloats partial floats and kCounterWords counter words.  The counter words are:
+//   [0, kFoldCounterWords)  the fold region: grid_fold's group counter [0] and one ticket [1 + g] per group of 16 contributors,
+//                           or the single ticket [0] of a last-block fold.  Every per-op fold launch checks that its
+//                           1 + ceil(blocks / 16) words fit; the region is large enough that the partials run out first.
+//   kGridEpochWord          epoch of the cooperative kernels' grid barrier (GridBar): only ever increases, never reset
+//   kGridArrivalWord        arrival count of that barrier
+//   kCeCounterWord          arrival counter of the whole-forward kernel's cross-entropy mean
+//   kAdamTicketWord         step hand-over ticket of adam_multi
+//   kClipTicketWord         fold ticket of grad_norm_clip
+// Each fixed word sits in a 32-byte sector of its own.
+constexpr int kScratchFloats = 4 << 20;                   // 16 MiB
+constexpr int kFoldCounterWords = kScratchFloats / 64;    // a fold of width ≥ 4 fills the partials before it runs out of tickets
+constexpr int kGridEpochWord = kFoldCounterWords;
+constexpr int kGridArrivalWord = kFoldCounterWords + 8;
+constexpr int kCeCounterWord = kFoldCounterWords + 16;
+constexpr int kAdamTicketWord = kFoldCounterWords + 24;
+constexpr int kClipTicketWord = kFoldCounterWords + 32;
+constexpr int kCounterWords = kFoldCounterWords + 40;
 
 // ---- SIMT direct convolution (conv1; conv2 fallback + oracle for the tensor-core kernels) -------------
 // x NHWC [B,H,W,Cin], w torch layout [Cout,Cin,5,5], bias [Cout] (nullable) → y NHWC [B,H,W,Cout].
@@ -31,12 +50,14 @@ void launch_conv5x5_dgrad(const float* dy, const float* w, float* dx, ConvShape 
 void launch_conv5x5_wgrad(const float* dy, const float* x, float* dw, float* db, ConvShape s, ReduceScratch scr, cudaStream_t st);
 
 // ---- BatchNorm(train) + ReLU + MaxPool2x2, fused -----------------------------------------------------
-// y NHWC [B,H,W,C]; stats [2C+1] (Σ, Σ², n — already all-reduced when SyncBN is on).
+// Every bn_relu_pool launcher takes C ∈ {4, 8, 16, 32, 64} and even H, W.
+// y NHWC [B,H,W,C]; stats [2C+1] (Σ, Σ², n — already all-reduced when SyncBN is on), or with mean_var [2C] = mean, variance
+// (eval mode: the running statistics, used as they are).
 // out: pooled [B,H/2,W/2,C] NHWC, or NCHW when out_nchw. saved [2C] ← mean, invstd.
 // running_mean/var (nullable) updated with `momentum` (unbiased var), nbt (nullable, int64) += 1.
 void launch_bn_relu_pool_fwd(const float* y, const float* stats, const float* gamma, const float* beta, float* out, float* saved,
                              float* running_mean, float* running_var, long long* nbt, float momentum, float eps, int B, int H,
-                             int W, int C, bool out_nchw, cudaStream_t st);
+                             int W, int C, bool out_nchw, bool mean_var, cudaStream_t st);
 // Pass 1 of backward: sums [2C] ← Σdz, Σdz·x̂ over the *local* batch (dz = grad at the BN output,
 // i.e. pooled grad routed to the arg-max position and masked by ReLU).  Also dγ = Σdz·x̂, dβ = Σdz.
 void launch_bn_relu_pool_bwd_reduce(const float* dout, const float* y, const float* saved, const float* gamma, const float* beta,
@@ -67,11 +88,14 @@ void launch_linear_fwd(const float* x, const float* w, const float* b, float* ou
 // dx[B,K] = dout·w (nullable); dw[N,K] = dout^T·x; db[N] = Σ dout
 void launch_linear_bwd(const float* dout, const float* x, const float* w, float* dx, float* dw, float* db, int B, int K, int N,
                        cudaStream_t st);
-// loss (scalar, mean over B) and probs[B,C] (softmax, kept for backward)
-// emit_grad: `probs` receives (softmax − onehot)/B instead (the backward of a mean loss with unit incoming gradient)
+// Cross-entropy with torch's ignore_index semantics: a row whose target is outside [0, C) (ignore_index) adds nothing, the mean is
+// over the n rows whose target is in [0, C), and with n = 0 the loss is NaN and every gradient zero.
+// loss (scalar, mean over the n rows) and probs[B,C] (softmax, kept for backward)
+// emit_grad: `probs` receives (softmax − onehot)/n instead, zero in ignored rows (the backward of a mean loss with unit incoming
+// gradient)
 void launch_cross_entropy_fwd(const float* logits, const long long* target, float* loss, float* probs, int B, int C, cudaStream_t st,
                               bool emit_grad = false);
-// dlogits = (probs - onehot) * (*dloss) / B
+// dlogits = (probs - onehot) * (*dloss) / n, zero in ignored rows
 void launch_cross_entropy_bwd(const float* probs, const long long* target, const float* dloss, float* dlogits, int B, int C,
                               cudaStream_t st);
 

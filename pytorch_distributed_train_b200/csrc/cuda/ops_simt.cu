@@ -254,12 +254,14 @@ __global__ void __launch_bounds__(256) fold_partials_kernel(const float* __restr
 // =====================================================================================================
 // BatchNorm(train) + ReLU + MaxPool 2x2
 // =====================================================================================================
-__device__ __forceinline__ void bn_coeffs(const float* stats, const float* gamma, const float* beta, float eps, int C, float* s_scale,
-                                          float* s_shift, float* s_mean, float* s_invstd) {
+// mean_var: stats = [mean, var] as they are (eval mode), not [Σ, Σ², n]: rebuilding var = E[y²] − mean² from running statistics
+// would cancel away the variance's digits when |mean| ≫ std
+__device__ __forceinline__ void bn_coeffs(const float* stats, const float* gamma, const float* beta, float eps, int C, int mean_var,
+                                          float* s_scale, float* s_shift, float* s_mean, float* s_invstd) {
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    const float n = fmaxf(stats[2 * C], 1.f);
-    const float mean = stats[c] / n;
-    const float var = fmaxf(stats[C + c] / n - mean * mean, 0.f);
+    const float n = mean_var ? 1.f : fmaxf(stats[2 * C], 1.f);
+    const float mean = mean_var ? stats[c] : stats[c] / n;
+    const float var = mean_var ? stats[C + c] : fmaxf(stats[C + c] / n - mean * mean, 0.f);
     const float invstd = rsqrtf(var + eps);
     const float g = gamma ? gamma[c] : 1.f, b = beta ? beta[c] : 0.f;
     s_mean[c] = mean;
@@ -273,9 +275,9 @@ __global__ void __launch_bounds__(256) bn_relu_pool_fwd_kernel(const float* __re
                                                                const float* __restrict__ gamma, const float* __restrict__ beta,
                                                                float* __restrict__ out, float* saved, float* running_mean,
                                                                float* running_var, long long* nbt, float momentum, float eps, int B,
-                                                               int H, int W, int C, int out_nchw) {
+                                                               int H, int W, int C, int out_nchw, int mean_var) {
   __shared__ float s_scale[64], s_shift[64], s_mean[64], s_invstd[64];
-  bn_coeffs(stats, gamma, beta, eps, C, s_scale, s_shift, s_mean, s_invstd);
+  bn_coeffs(stats, gamma, beta, eps, C, mean_var, s_scale, s_shift, s_mean, s_invstd);
   __syncthreads();
   if (blockIdx.x == 0) {
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
@@ -720,12 +722,25 @@ __global__ void __launch_bounds__(256) linear_bwd_kernel(const float* __restrict
   if (db && static_cast<int>(blockIdx.x) == dx_blocks && threadIdx.x < N) db[threadIdx.x] = bsum;
 }
 
-// emit_grad: write d(loss)/d(logits) = (softmax − onehot)/B instead of the softmax — the whole backward of a mean
+// Rows whose target lies in [0, C), counted by every thread of the block (ignore_index: torch's mean is over these rows only).
+__device__ __forceinline__ int ce_counted_rows(const long long* __restrict__ target, int B, int C) {
+  int n = 0;
+  for (int r0 = 0; r0 < B; r0 += blockDim.x) {
+    const int r = r0 + threadIdx.x;
+    const long long t = r < B ? target[r] : -1;
+    n += __syncthreads_count(t >= 0 && t < C);
+  }
+  return n;
+}
+
+// emit_grad: write d(loss)/d(logits) = (softmax − onehot)/n instead of the softmax — the whole backward of a mean
 // cross-entropy whose incoming gradient is 1, produced by the forward launch (the backward kernel disappears).
+// Ignored rows (target outside [0, C)) add no loss term and get a zero gradient; n counts the others (0 ⇒ NaN loss, as torch).
 __global__ void __launch_bounds__(256) cross_entropy_fwd_kernel(const float* __restrict__ logits, const long long* __restrict__ target,
                                                                 float* loss, float* __restrict__ probs, int B, int C, int emit_grad) {
   float local = 0.f;
-  const float invB = 1.f / static_cast<float>(B);
+  const int counted = ce_counted_rows(target, B, C);
+  const float invN = 1.f / static_cast<float>(counted);
   for (int r = threadIdx.x; r < B; r += blockDim.x) {
     const float* l = logits + static_cast<size_t>(r) * C;
     float m = l[0];
@@ -734,11 +749,12 @@ __global__ void __launch_bounds__(256) cross_entropy_fwd_kernel(const float* __r
     for (int c = 0; c < C; ++c) s += __expf(l[c] - m);
     const float inv = 1.f / s, lse = m + __logf(s);
     const long long t = target[r];
+    const bool counted_row = t >= 0 && t < C;
     for (int c = 0; c < C; ++c) {
       const float p = __expf(l[c] - m) * inv;
-      probs[static_cast<size_t>(r) * C + c] = emit_grad ? (p - (t == c ? 1.f : 0.f)) * invB : p;
+      probs[static_cast<size_t>(r) * C + c] = !emit_grad ? p : counted_row ? (p - (t == c ? 1.f : 0.f)) * invN : 0.f;
     }
-    if (t >= 0 && t < C) local += lse - l[t];
+    if (counted_row) local += lse - l[t];
   }
   // fixed-order block reduction (deterministic)
   __shared__ float red[256];
@@ -748,16 +764,18 @@ __global__ void __launch_bounds__(256) cross_entropy_fwd_kernel(const float* __r
     if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
     __syncthreads();
   }
-  if (threadIdx.x == 0) *loss = red[0] / static_cast<float>(B);
+  if (threadIdx.x == 0) *loss = red[0] / static_cast<float>(counted);
 }
 
-__global__ void cross_entropy_bwd_kernel(const float* __restrict__ probs, const long long* __restrict__ target,
-                                         const float* __restrict__ dloss, float* __restrict__ dlogits, int B, int C) {
+__global__ void __launch_bounds__(256) cross_entropy_bwd_kernel(const float* __restrict__ probs, const long long* __restrict__ target,
+                                                                const float* __restrict__ dloss, float* __restrict__ dlogits, int B, int C) {
+  const int counted = ce_counted_rows(target, B, C);
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * C) return;
   const int r = i / C, c = i % C;
-  const float g = (dloss ? *dloss : 1.f) / static_cast<float>(B);
-  dlogits[i] = (probs[i] - (target[r] == c ? 1.f : 0.f)) * g;
+  const long long t = target[r];
+  const float g = (dloss ? *dloss : 1.f) / static_cast<float>(counted);
+  dlogits[i] = (t >= 0 && t < C) ? (probs[i] - (t == c ? 1.f : 0.f)) * g : 0.f;
 }
 
 // =====================================================================================================
@@ -905,7 +923,7 @@ void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float
   constexpr int TH = 7;
   if (s.H % TH != 0) throw std::invalid_argument("conv5x5_fwd: H must be a multiple of 7");
   const int blocks = s.B * (s.H / TH);
-  if (stats && (static_cast<long long>(blocks + blocks / kFoldGroup + 1) * 2 * s.Cout > scr.capacity_floats || blocks / kFoldGroup + 2 > scr.counters))
+  if (stats && (static_cast<long long>(blocks + blocks / kFoldGroup + 1) * 2 * s.Cout > scr.capacity_floats || blocks / kFoldGroup + 2 > scr.fold_counters))
     throw std::invalid_argument("conv5x5_fwd: reduction scratch too small");
   if (s.Cin == 1 && s.Cout == 16) {
     const int threads = (TH * s.W + 31) / 32 * 32;
@@ -960,23 +978,31 @@ void launch_conv5x5_wgrad(const float* dy, const float* x, float* dw, float* db,
   check_launch("fold_partials");
 }
 
+// The backward kernel takes a thread's channel quad from threadIdx.x % (C/4), which needs 256 % (C/4) == 0, and reduces the
+// quads of a warp with a shuffle tree over C/4 lanes, which needs a power of two: C ∈ {4, 8, 16, 32, 64}.  Pooling takes even H, W.
+static void check_bn_relu_pool_shape(int C, int H, int W, const char* what) {
+  if (!(C == 4 || C == 8 || C == 16 || C == 32 || C == 64) || H % 2 || W % 2)
+    throw std::invalid_argument(std::string(what) + ": C must be 4, 8, 16, 32 or 64, and H and W even");
+}
+
 void launch_bn_relu_pool_fwd(const float* y, const float* stats, const float* gamma, const float* beta, float* out, float* saved,
                              float* running_mean, float* running_var, long long* nbt, float momentum, float eps, int B, int H, int W,
-                             int C, bool out_nchw, cudaStream_t st) {
-  if (C % 4 != 0 || C > 64 || H % 2 || W % 2) throw std::invalid_argument("bn_relu_pool: C%4==0, C<=64, even H/W required");
+                             int C, bool out_nchw, bool mean_var, cudaStream_t st) {
+  check_bn_relu_pool_shape(C, H, W, "bn_relu_pool_fwd");
   const long long total = static_cast<long long>(B) * (H / 2) * (W / 2) * (C / 4);
   bn_relu_pool_fwd_kernel<<<static_cast<int>((total + 255) / 256), 256, 0, st>>>(y, stats, gamma, beta, out, saved, running_mean, running_var,
-                                                                                 nbt, momentum, eps, B, H, W, C, out_nchw ? 1 : 0);
+                                                                                 nbt, momentum, eps, B, H, W, C, out_nchw ? 1 : 0,
+                                                                                 mean_var ? 1 : 0);
   check_launch("bn_relu_pool_fwd");
 }
 
 void launch_bn_relu_pool_bwd_reduce(const float* dout, const float* y, const float* saved, const float* gamma, const float* beta, float* sums,
                                     float* dgamma, float* dbeta, int B, int H, int W, int C, bool dout_nchw, ReduceScratch scr,
                                     cudaStream_t st) {
-  if (C % 4 != 0 || C > 64) throw std::invalid_argument("bn_relu_pool_bwd: C%4==0, C<=64 required");
+  check_bn_relu_pool_shape(C, H, W, "bn_relu_pool_bwd_reduce");
   const long long total = static_cast<long long>(B) * (H / 2) * (W / 2) * (C / 4);
   const int blocks = static_cast<int>((total + 255) / 256);
-  if (static_cast<long long>(blocks + blocks / kFoldGroup + 1) * 2 * C > scr.capacity_floats || blocks / kFoldGroup + 2 > scr.counters)
+  if (static_cast<long long>(blocks + blocks / kFoldGroup + 1) * 2 * C > scr.capacity_floats || blocks / kFoldGroup + 2 > scr.fold_counters)
     throw std::invalid_argument("bn_relu_pool_bwd: reduction scratch too small");
   bn_relu_pool_bwd_kernel<false><<<blocks, 256, 0, st>>>(dout, y, saved, gamma, beta, sums, dgamma, dbeta, nullptr, nullptr, B, H, W, C,
                                                          dout_nchw ? 1 : 0, scr);
@@ -986,6 +1012,7 @@ void launch_bn_relu_pool_bwd_reduce(const float* dout, const float* y, const flo
 void launch_bn_relu_pool_bwd_apply(const float* dout, const float* y, const float* saved, const float* gamma, const float* beta,
                                    const float* sums, const float* count, float* dy, int B, int H, int W, int C, bool dout_nchw,
                                    cudaStream_t st) {
+  check_bn_relu_pool_shape(C, H, W, "bn_relu_pool_bwd_apply");
   const long long total = static_cast<long long>(B) * (H / 2) * (W / 2) * (C / 4);
   bn_relu_pool_bwd_kernel<true><<<static_cast<int>((total + 255) / 256), 256, 0, st>>>(dout, y, saved, gamma, beta, const_cast<float*>(sums), nullptr,
                                                                                        nullptr, count, dy, B, H, W, C, dout_nchw ? 1 : 0,

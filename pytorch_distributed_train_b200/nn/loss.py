@@ -2,9 +2,10 @@
 
 On CUDA, float32 ``[B, C]`` logits with class-index targets and ``reduction='mean'`` run as one
 fused sm_90a kernel (log-softmax + NLL + mean, saving the softmax so backward is a single
-``(softmax − onehot)/B`` pass) instead of the reference stack's ``_log_softmax`` +
-``nll_loss_forward`` pair and their two backward kernels.  Everything else defers to the
-standard functional."""
+``(softmax − onehot)/n`` pass) instead of the reference stack's ``_log_softmax`` +
+``nll_loss_forward`` pair and their two backward kernels.  As in torch, rows whose target is
+``ignore_index`` (-100) add nothing and get a zero gradient, ``n`` counts the other rows, and a
+batch with n = 0 gives a NaN loss.  Everything else defers to the standard functional."""
 from __future__ import annotations
 
 import torch
