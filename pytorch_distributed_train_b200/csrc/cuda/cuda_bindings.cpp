@@ -45,8 +45,12 @@ float* opt_mut(c10::optional<at::Tensor>& t, const char* name) {
 // stream at a time (the compute stream), which is what serialises access.
 struct Scratch {
   at::Tensor partials, counter;
+  // conv2's weight-gradient partials per image ([one per SM][512][32]), written by the layer-2 backward kernel and folded by the
+  // layer-1 one: a buffer of their own, so that no per-op kernel launched between the two (on any stream) can overwrite them
+  at::Tensor wgrad;
+  int wgrad_batch = 0;   // batch whose partials wgrad holds and nobody has folded yet (0: none)
 };
-ReduceScratch scratch(const at::Tensor& like) {
+Scratch& scratch_entry(const at::Tensor& like) {
   static std::mutex mu;
   static auto& per_dev = *new std::map<int, Scratch>();  // leaked on purpose: CUDA tensors must not die at static teardown
   std::lock_guard<std::mutex> g(mu);
@@ -56,14 +60,33 @@ ReduceScratch scratch(const at::Tensor& like) {
     Scratch s;
     s.partials = at::empty({kScratchFloats}, like.options().dtype(at::kFloat));
     s.counter = at::zeros({kCounterWords}, like.options().dtype(at::kInt));   // layout: ops_kernels.h
+    s.wgrad = at::empty({static_cast<int64_t>(at::cuda::getDeviceProperties(dev)->multiProcessorCount) * 512 * 32}, like.options().dtype(at::kFloat));
     it = per_dev.emplace(dev, std::move(s)).first;
   }
+  return it->second;
+}
+ReduceScratch scratch(const at::Tensor& like) {
+  Scratch& s = scratch_entry(like);
   ReduceScratch r;
-  r.partials = it->second.partials.data_ptr<float>();
-  r.counter = reinterpret_cast<unsigned int*>(it->second.counter.data_ptr<int>());
-  r.capacity_floats = static_cast<int>(it->second.partials.numel());
+  r.partials = s.partials.data_ptr<float>();
+  r.counter = reinterpret_cast<unsigned int*>(s.counter.data_ptr<int>());
+  r.capacity_floats = static_cast<int>(s.partials.numel());
   r.fold_counters = kFoldCounterWords;
   return r;
+}
+// Where the layer-2 backward kernel of a batch of B leaves conv2's per-image weight-gradient partials for the layer-1 one.
+float* conv2_wgrad_partials(const at::Tensor& like, int B, const char* what) {
+  Scratch& s = scratch_entry(like);
+  TORCH_CHECK(static_cast<int64_t>(B) * 512 * 32 <= s.wgrad.numel(), what, ": batch ", B, " exceeds one CTA per SM");
+  return s.wgrad.data_ptr<float>();
+}
+
+// conv2's input frame p1 [B,18,18,16] of the layer-2 backward bindings, or nullptr when not given.
+const float* conv2_input(const c10::optional<at::Tensor>& p1, int B, const char* what) {
+  if (!p1.has_value() || !p1->defined()) return nullptr;
+  chk(*p1, "p1");
+  TORCH_CHECK(p1->numel() == static_cast<int64_t>(B) * 324 * 16, what, ": p1 must be the [B,18,18,16] frame of layer 1");
+  return p1->data_ptr<float>();
 }
 
 // The grid barrier of the cooperative kernels lives in the fixed words behind the fold region.
@@ -234,16 +257,28 @@ void register_cuda_bindings(py::module_& m) {
   });
   m.def("convnet_l1_bwd_wgrad", [](const at::Tensor& dp, const at::Tensor& y, const at::Tensor& x, const at::Tensor& saved,
                                    c10::optional<at::Tensor> gamma, c10::optional<at::Tensor> beta, at::Tensor dgamma, at::Tensor dbeta, at::Tensor dw,
-                                   c10::optional<at::Tensor> db, const at::Tensor& dy2_pad, const at::Tensor& x2_pad, const at::Tensor& dysum2,
-                                   at::Tensor dw2, c10::optional<at::Tensor> db2, py::object sgd) {
+                                   c10::optional<at::Tensor> db, c10::optional<at::Tensor> dy2_pad, c10::optional<at::Tensor> x2_pad,
+                                   const at::Tensor& dysum2, at::Tensor dw2, c10::optional<at::Tensor> db2, py::object sgd) {
     chk(dp, "dp"); chk(y, "y"); chk(x, "x"); chk(saved, "saved"); chk(dgamma, "dgamma"); chk(dbeta, "dbeta"); chk(dw, "dw");
-    chk(dy2_pad, "dy2_pad"); chk(x2_pad, "x2_pad"); chk(dysum2, "dysum2"); chk(dw2, "dw2");
+    chk(dysum2, "dysum2"); chk(dw2, "dw2");
     c10::cuda::CUDAGuard g(x.device());
     const int B = static_cast<int>(y.size(0));
     TORCH_CHECK(dp.numel() == static_cast<int64_t>(B) * 5184 && x.numel() == static_cast<int64_t>(B) * 784 && dw.numel() == 400 &&
                     dgamma.numel() == 16 && dbeta.numel() == 16, "convnet_l1_bwd_wgrad: layer-1 shape mismatch");
-    TORCH_CHECK(dy2_pad.numel() == static_cast<int64_t>(B) * 324 * 32 && x2_pad.numel() == static_cast<int64_t>(B) * 324 * 16 &&
-                    dysum2.numel() == static_cast<int64_t>(B) * 32 && dw2.numel() == 12800, "convnet_l1_bwd_wgrad: layer-2 shape mismatch");
+    TORCH_CHECK(dysum2.numel() == static_cast<int64_t>(B) * 32 && dw2.numel() == 12800, "convnet_l1_bwd_wgrad: layer-2 shape mismatch");
+    // conv2's per-image weight-gradient partials: from the given frames, or (both None) left by convnet_l2_bwd(_fc)(…, p1) of this batch
+    const bool frames = dy2_pad.has_value() && dy2_pad->defined();
+    TORCH_CHECK(frames == (x2_pad.has_value() && x2_pad->defined()), "convnet_l1_bwd_wgrad: dy2_pad and x2_pad are given together or not at all");
+    float* wpart = conv2_wgrad_partials(x, B, "convnet_l1_bwd_wgrad");
+    Scratch& entry = scratch_entry(x);
+    if (frames) {
+      chk(*dy2_pad, "dy2_pad"); chk(*x2_pad, "x2_pad");
+      TORCH_CHECK(dy2_pad->numel() == static_cast<int64_t>(B) * 324 * 32 && x2_pad->numel() == static_cast<int64_t>(B) * 324 * 16,
+                  "convnet_l1_bwd_wgrad: layer-2 frame shape mismatch");
+    } else {
+      TORCH_CHECK(entry.wgrad_batch == B, "convnet_l1_bwd_wgrad: without dy2_pad / x2_pad it folds the partials of convnet_l2_bwd(_fc)(…, p1) "
+                  "of the same batch, and none are pending");
+    }
     // sgd = (params[10], prev_grads[4], momentum_bufs[10] or [], lr, lr_tensor, momentum, dampening, weight_decay, nesterov, maximize, first_step):
     // parameters in the order conv1.w, conv1.b, bn1.w, bn1.b, conv2.w, conv2.b, fc.w, fc.b, bn2.w, bn2.b (entries may be None)
     // or the Adam rider: ("adam", params[10], prev_grads[4], exp_avgs[10], exp_avg_sqs[10], steps[10], lr, lr_tensor, beta1, beta2,
@@ -252,13 +287,14 @@ void register_cuda_bindings(py::module_& m) {
     static const int64_t want[10] = {400, 16, 16, 16, 12800, 32, -1, -1, 32, 32};
     ReduceScratch scr = scratch(x);
     const size_t l1_floats = static_cast<size_t>(B) * (64 + 512);
-    TORCH_CHECK(static_cast<long long>(l1_floats) + static_cast<long long>(B) * 512 * 32 + B <= scr.capacity_floats, "convnet_l1_bwd_wgrad: scratch too small");
+    TORCH_CHECK(static_cast<long long>(l1_floats) + B <= scr.capacity_floats, "convnet_l1_bwd_wgrad: scratch too small");
     auto launch = [&](auto rider) {
+      if (frames) launch_conv2_wgrad_partials(dy2_pad->data_ptr<float>(), x2_pad->data_ptr<float>(), B, wpart, cur_stream(x));
       launch_convnet_l1_bwd_wgrad(dp.data_ptr<float>(), y.data_ptr<float>(), x.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"),
                                   opt_ptr(beta, "beta"), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"),
-                                  dy2_pad.data_ptr<float>(), x2_pad.data_ptr<float>(), dysum2.data_ptr<float>(), dw2.data_ptr<float>(),
-                                  opt_mut(db2, "db2"), B, scr.partials, scr.partials + static_cast<size_t>(B) * 64, scr.partials + l1_floats,
-                                  grid_sync(scr), cur_stream(x), rider);
+                                  wpart, dysum2.data_ptr<float>(), dw2.data_ptr<float>(), opt_mut(db2, "db2"), B, scr.partials,
+                                  scr.partials + static_cast<size_t>(B) * 64, grid_sync(scr), cur_stream(x), rider);
+      entry.wgrad_batch = 0;
     };
     // the clip entry of a rider tuple → the clipping variant of the rider
     auto clipped = [&](auto base, const py::handle& entry) {
@@ -274,7 +310,7 @@ void register_cuda_bindings(py::module_& m) {
       r.max_norm = static_cast<float>(c[0].cast<double>());
       r.norm_inf = std::isinf(norm_type) ? 1 : 0;
       r.norm_out = out.data_ptr<float>();
-      r.part = scr.partials + l1_floats + static_cast<size_t>(B) * 512 * 32;
+      r.part = scr.partials + l1_floats;
       return r;
     };
     if (!sgd.is_none() && py::isinstance<py::tuple>(sgd) && py::len(sgd) > 0 && py::isinstance<py::str>(sgd.cast<py::tuple>()[0])) {
@@ -442,27 +478,32 @@ void register_cuda_bindings(py::module_& m) {
   }, py::arg("x"), py::arg("w1"), py::arg("b1"), py::arg("g1"), py::arg("be1"), py::arg("rm1"), py::arg("rv1"), py::arg("nbt1"), py::arg("mom1"),
      py::arg("eps1"), py::arg("w2"), py::arg("b2"), py::arg("g2"), py::arg("be2"), py::arg("rm2"), py::arg("rv2"), py::arg("nbt2"), py::arg("mom2"),
      py::arg("eps2"), py::arg("fcw"), py::arg("fcb"), py::arg("target") = py::none(), py::arg("defer_loss_mean") = false);
+  // p1 (conv2's input frame [B,18,18,16], optional): conv2's per-image weight-gradient partials are computed inside the kernel for
+  // convnet_l1_bwd_wgrad(…, None, None, …) to fold, and the dy frame is not written (None in its place).
   m.def("convnet_l2_bwd", [](const at::Tensor& dout, const at::Tensor& y, const at::Tensor& saved, c10::optional<at::Tensor> gamma,
-                             c10::optional<at::Tensor> beta, const at::Tensor& w, at::Tensor dgamma, at::Tensor dbeta) {
+                             c10::optional<at::Tensor> beta, const at::Tensor& w, at::Tensor dgamma, at::Tensor dbeta, c10::optional<at::Tensor> p1) {
     chk(dout, "dout"); chk(y, "y"); chk(saved, "saved"); chk(w, "w"); chk(dgamma, "dgamma"); chk(dbeta, "dbeta");
     c10::cuda::CUDAGuard g(y.device());
     const int B = static_cast<int>(y.size(0));
     TORCH_CHECK(dout.numel() == static_cast<int64_t>(B) * 1568 && y.numel() == static_cast<int64_t>(B) * 6272 && w.numel() == 12800 &&
                     dgamma.numel() == 32 && dbeta.numel() == 32, "convnet_l2_bwd: shape mismatch");
-    at::Tensor dy = at::empty({B, 18, 18, 32}, y.options());
+    const float* x2 = conv2_input(p1, B, "convnet_l2_bwd");
+    at::Tensor dy = x2 ? at::Tensor() : at::empty({B, 18, 18, 32}, y.options());
     at::Tensor dx = at::empty({B, 18, 18, 16}, y.options());
     at::Tensor dysum = at::empty({B, 32}, y.options());
     ReduceScratch scr = scratch(y);
+    float* wpart = x2 ? conv2_wgrad_partials(y, B, "convnet_l2_bwd") : nullptr;
     launch_convnet_l2_bwd(dout.data_ptr<float>(), y.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"), opt_ptr(beta, "beta"),
-                          w.data_ptr<float>(), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dy.data_ptr<float>(), dx.data_ptr<float>(),
-                          dysum.data_ptr<float>(), B, scr.partials, grid_sync(scr),
-                          cur_stream(y));
-    return py::make_tuple(dy, dx, dysum);
-  });
+                          w.data_ptr<float>(), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), x2 ? nullptr : dy.data_ptr<float>(), dx.data_ptr<float>(),
+                          dysum.data_ptr<float>(), B, scr.partials, grid_sync(scr), cur_stream(y), x2, wpart);
+    if (x2) scratch_entry(y).wgrad_batch = B;
+    return py::make_tuple(x2 ? py::none() : py::cast(dy), dx, dysum);
+  }, py::arg("dout"), py::arg("y"), py::arg("saved"), py::arg("gamma"), py::arg("beta"), py::arg("w"), py::arg("dgamma"), py::arg("dbeta"),
+     py::arg("p1") = py::none());
   m.def("convnet_l2_bwd_fc", [](const at::Tensor& dlogits, const at::Tensor& fcw, const at::Tensor& pooled, at::Tensor dfcw, c10::optional<at::Tensor> dfcb,
                                 const at::Tensor& y, const at::Tensor& saved, c10::optional<at::Tensor> gamma, c10::optional<at::Tensor> beta,
                                 const at::Tensor& w, at::Tensor dgamma, at::Tensor dbeta, c10::optional<at::Tensor> loss_parts,
-                                c10::optional<at::Tensor> loss_out) {
+                                c10::optional<at::Tensor> loss_out, c10::optional<at::Tensor> p1) {
     chk(dlogits, "dlogits"); chk(fcw, "fc weight"); chk(pooled, "pooled"); chk(dfcw, "dfcw");
     chk(y, "y"); chk(saved, "saved"); chk(w, "w"); chk(dgamma, "dgamma"); chk(dbeta, "dbeta");
     c10::cuda::CUDAGuard g(y.device());
@@ -474,18 +515,22 @@ void register_cuda_bindings(py::module_& m) {
     TORCH_CHECK(reinterpret_cast<uintptr_t>(fcw.data_ptr()) % 16 == 0, "convnet_l2_bwd_fc: fc weight must be 16-byte aligned");
     TORCH_CHECK(!loss_parts.has_value() || !loss_parts->defined() || (loss_parts->numel() == B + 1 && loss_out.has_value() && loss_out->defined()),
                 "convnet_l2_bwd_fc: loss_parts must be the [B + 1] tensor of convnet_fwd, and loss_out given with it");
-    at::Tensor dy = at::empty({B, 18, 18, 32}, y.options());
+    const float* x2 = conv2_input(p1, B, "convnet_l2_bwd_fc");
+    at::Tensor dy = x2 ? at::Tensor() : at::empty({B, 18, 18, 32}, y.options());
     at::Tensor dx = at::empty({B, 18, 18, 16}, y.options());
     at::Tensor dysum = at::empty({B, 32}, y.options());
     ReduceScratch scr = scratch(y);
+    float* wpart = x2 ? conv2_wgrad_partials(y, B, "convnet_l2_bwd_fc") : nullptr;
     launch_convnet_l2_bwd_fc(dlogits.data_ptr<float>(), fcw.data_ptr<float>(), pooled.data_ptr<float>(), dfcw.data_ptr<float>(), opt_mut(dfcb, "dfcb"),
                              ncls, y.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"), opt_ptr(beta, "beta"), w.data_ptr<float>(),
-                             dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dy.data_ptr<float>(), dx.data_ptr<float>(), dysum.data_ptr<float>(), B,
-                             scr.partials, grid_sync(scr), cur_stream(y), opt_ptr(loss_parts, "loss_parts"),
-                             opt_mut(loss_out, "loss_out"));
-    return py::make_tuple(dy, dx, dysum);
+                             dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), x2 ? nullptr : dy.data_ptr<float>(), dx.data_ptr<float>(),
+                             dysum.data_ptr<float>(), B, scr.partials, grid_sync(scr), cur_stream(y), opt_ptr(loss_parts, "loss_parts"),
+                             opt_mut(loss_out, "loss_out"), x2, wpart);
+    if (x2) scratch_entry(y).wgrad_batch = B;
+    return py::make_tuple(x2 ? py::none() : py::cast(dy), dx, dysum);
   }, py::arg("dlogits"), py::arg("fcw"), py::arg("pooled"), py::arg("dfcw"), py::arg("dfcb"), py::arg("y"), py::arg("saved"), py::arg("gamma"),
-     py::arg("beta"), py::arg("w"), py::arg("dgamma"), py::arg("dbeta"), py::arg("loss_parts") = py::none(), py::arg("loss_out") = py::none());
+     py::arg("beta"), py::arg("w"), py::arg("dgamma"), py::arg("dbeta"), py::arg("loss_parts") = py::none(), py::arg("loss_out") = py::none(),
+     py::arg("p1") = py::none());
   m.def("conv5x5_wgrad_win", [](const at::Tensor& dy_pad, const at::Tensor& x_pad, const at::Tensor& dysum, at::Tensor dw, c10::optional<at::Tensor> db) {
     chk(dy_pad, "dy_pad"); chk(x_pad, "x_pad"); chk(dysum, "dysum"); chk(dw, "dw");
     c10::cuda::CUDAGuard g(dy_pad.device());

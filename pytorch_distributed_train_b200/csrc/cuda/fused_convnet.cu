@@ -10,11 +10,13 @@
 //                              swizzled smem patch ── conv2 5x5 (16→32) on wgmma (the 25 taps are row-shifted descriptors
 //                              into that patch; accumulators in registers) ──barrier── BN + ReLU + MaxPool2 + classifier
 //                              (+ cross-entropy term and d(loss)/d(logits) when the targets are known)           (ref :25-34,40)
-//   convnet_l2_bwd_kernel<FC>  classifier backward + MaxPool/ReLU/BN backward ──barrier (Σdz, Σdz·x̂)── dy → conv2 data
-//                              gradient on wgmma
-//   convnet_l1_bwd_kernel<WG>  MaxPool/ReLU/BN backward ──barrier── conv1 weight gradient (mma.sync) ──barrier── folds,
-//                              while conv2's weight gradient is computed on mma.sync (MN-major window) and — on one
-//                              GPU — the threads that write the folded gradients apply the SGD update (SgdRider)
+//   convnet_l2_bwd_kernel<FC, WG>  classifier backward + MaxPool/ReLU/BN backward ──barrier (Σdz, Σdz·x̂)── dy → conv2 data
+//                              gradient on wgmma (warps 4..7), next to it conv2's weight-gradient partial of the image on
+//                              mma.sync (warps 0..3, joined by 4..7 when their wgmma are done; MN-major window; A operand
+//                              loaded by TMA in the barrier's shadow)
+//   convnet_l1_bwd_kernel<WG>  MaxPool/ReLU/BN backward ──barrier── conv1 weight gradient (mma.sync) ──barrier── conv1 fold;
+//                              conv2's weight gradient is folded in the shadow of the first barrier, and — on one GPU — the
+//                              threads that write the folded gradients apply the optimizer update (SgdRider / AdamRider)
 //
 // convnet_l1_fwd_kernel / convnet_l2_fwd_kernel (one kernel per layer) and the <false> instantiations are the variants without
 // the riders (PDT_FUSED_WHOLE_FWD / PDT_FC_MERGED / PDT_WGRAD_MERGED = 0); all of them are exercised by tests/test_gpu_kernels.py.
@@ -60,17 +62,9 @@ __device__ __forceinline__ void trace_stamp(bool on, int kernel, int phase) {
 }
 #define trace(kernel, phase) trace_stamp(trace_on_, kernel, phase)
 
-// CTA-wide sync of the first NAMED threads (named barrier 1) or of the whole CTA (NAMED = 0): kernels with extra
-// role warps keep their "main" threads in step without involving the others.
-template <int NAMED>
-__device__ __forceinline__ void cta_sync() {
-  if constexpr (NAMED > 0) asm volatile("bar.sync 1, %0;" ::"n"(NAMED) : "memory");
-  else __syncthreads();
-}
-
 // Sum `rows` partial rows of `W` floats (written by other CTAs before a grid barrier) in a fixed order.
-// Called by all (main) threads; the totals land in s_out[0..W).  s_tmp: [4][W] floats.  Needs >= 4*W threads.
-template <int W, int NAMED = 0>
+// Called by all threads; the totals land in s_out[0..W).  s_tmp: [4][W] floats.  Needs >= 4*W threads.
+template <int W>
 __device__ __forceinline__ void fold_rows(const float* __restrict__ partials, int rows, float* s_tmp, float* s_out) {
   const int tid = threadIdx.x;
   if (tid < 4 * W) {
@@ -85,14 +79,14 @@ __device__ __forceinline__ void fold_rows(const float* __restrict__ partials, in
     }
     s_tmp[grp * W + col] = s;
   }
-  cta_sync<NAMED>();
+  __syncthreads();
   if (tid < W) s_out[tid] = (s_tmp[tid] + s_tmp[W + tid]) + (s_tmp[2 * W + tid] + s_tmp[3 * W + tid]);
-  cta_sync<NAMED>();
+  __syncthreads();
 }
 
 // The same with every thread of a THREADS-wide CTA loading: G = THREADS / W row classes, one L2 round trip for up to 8·G rows.
 // s_tmp: [G][W] floats.
-template <int W, int THREADS, int NAMED = 0>
+template <int W, int THREADS>
 __device__ __forceinline__ void fold_rows_wide(const float* __restrict__ partials, int rows, float* s_tmp, float* s_out) {
   constexpr int G = THREADS / W;
   const int tid = threadIdx.x;
@@ -108,14 +102,14 @@ __device__ __forceinline__ void fold_rows_wide(const float* __restrict__ partial
     }
     s_tmp[grp * W + col] = s;
   }
-  cta_sync<NAMED>();
+  __syncthreads();
   if (tid < W) {
     float tot = 0.f;
 #pragma unroll
     for (int g = 0; g < G; ++g) tot += s_tmp[g * W + tid];
     s_out[tid] = tot;
   }
-  cta_sync<NAMED>();
+  __syncthreads();
 }
 
 // Warp-level reduction of 32 per-thread values with 31 shuffles: after the call lane l holds Σ_lanes v[l] in v[0].
@@ -156,10 +150,9 @@ struct L1Map {
   }
 };
 
-template <int NAMED = 0>
 __device__ __forceinline__ void l1_load_image(const float* __restrict__ x, float* xs /*[32][32]*/, int tid) {
   for (int i = tid; i < 1024; i += kL1Threads) xs[i] = 0.f;
-  cta_sync<NAMED>();
+  __syncthreads();
   if (tid < 784) {
     const int rr = tid / 28, cc = tid - rr * 28;
     xs[(rr + 2) * 32 + cc + 2] = x[tid];
@@ -284,31 +277,82 @@ convnet_l1_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w, 
   trace(0, 5);
 }
 
-// ---- layer 1 backward (+ conv2 weight gradient riding along) ---------------------------------------------------------------
-// dynamic smem: dys [784][16] | fold [25 warps][16 co][32 taps]   (+ WG: the tensor-core weight-gradient pipeline, below)
+// ---- layer 1 backward (+ the fold of conv2's weight gradient riding along) ---------------------------------------------------
+// dynamic smem: dys [784][16] | fold [25 warps][16 co][32 taps]
 constexpr int kL1BwdSmem = (784 * 16 + kL1Warps * 512) * 4;
 
-// The conv2 weight gradient of an image needs nothing from layer-1 backward — only the dy / x frames that layer-2 backward
-// left in global memory.  With WG the CTA carries one extra warp that TMA-loads both operands of the same image while the 25
-// layer-1 warps do their SIMT work, and 15 of those warps compute dW2ᵀ[(kh, kw, ci)][co] = Σ_P xpad[P + (kh−2)·18 + (kw−2)][ci] ·
-// dypad[P][co] on the tensor cores (wgrad_win.cuh) just before the kernel's second grid barrier; it is folded after it, next to
-// the conv1 gradient:
-//   * B (dy): the 256 positions starting at the first interior one, two TMA boxes.
-//   * A (x): the whole image's overlapping-row view (pitch 64 B, length 128 B: row r = positions r and r+1 = two horizontally
-//     adjacent taps × 16 channels), loaded ONCE (384 rows, 48 KB); the 32-row atom of tap pair (kh, kw/2) for position P is the
-//     same buffer read (kh−2)·18 + (kw−2) rows further down.  The per-CTA partial has 512 rows in four groups of four atoms:
-//     group kw/2 ∈ {0,1,2} stacks kh = 0..3 (stride 18 rows), group 3 holds kh = 4 with kw/2 = 0..2 (stride 2 rows; its fourth
-//     atom is unused).  The stand-alone kernel (conv_wgmma.cu) orders the atoms by (kh, kw/2) instead.
-// One launch and one grid barrier less than running the two kernels back to back.
-struct L1WgCfg {
-  static constexpr int kThreads = kL1Threads + 32;        // + one warp: the TMA loads
-  static constexpr int kFrame = 18 * 18, kFirst = 2 * 18 + 2;
-  // A window: rows [0, 384) of the image's overlapping-row view (row r = positions r, r+1 × 16 channels = 128 B), six 64-row boxes
-  static constexpr int kABoxes = 6, kABytes = kABoxes * 64 * 128;
-  static constexpr int kBBytes = 2 * 128 * 128;                    // both 128-position dy tiles of the image
-  static constexpr int kOff = (kL1BwdSmem + 1023) / 1024 * 1024;   // window starts 1024-aligned behind the layer-1 buffers
-  static constexpr size_t kSmem = 1024 + kOff + kABytes + kBBytes + 256;
+// conv2's weight gradient in the window formulation (wgrad_win.cuh): dW2ᵀ[(kh, kw, ci)][co] = Σ_P xpad[P + (kh−2)·18 + (kw−2)][ci] ·
+// dypad[P][co] over the 256 positions P from the first interior one, per image, on mma.sync.
+//   * B (dy): the layer-2 backward kernel's own swizzled dy patch (rows = padded positions, zero halo), from row kFirst on.
+//   * A (x): the whole image's overlapping-row view of the layer-1 output frame (pitch 64 B, length 128 B: row r = positions r and
+//     r+1 = two horizontally adjacent taps × 16 channels), loaded ONCE by TMA (six 64-row boxes, 48 KB, 1024-aligned); the 32-row
+//     atom of tap pair (kh, kw/2) for position P is the same buffer read (kh−2)·18 + (kw−2) rows further down.
+// The per-image partial has 512 rows in four groups of four atoms: group kw/2 ∈ {0,1,2} stacks kh = 0..3 (stride 18 rows), group 3
+// holds kh = 4 with kw/2 = 0..2 (stride 2 rows; its fourth atom is unused).  The stand-alone kernel (conv_wgmma.cu) orders the
+// atoms by (kh, kw/2) instead.  The layer-1 backward kernel folds the B partials in the shadow of its first grid barrier.
+struct Conv2WgCfg {
+  static constexpr int kFrame = 18 * 18, kFirst = 2 * 18 + 2, kAtoms = 15;
+  static constexpr int kABoxes = 6, kABytes = kABoxes * 64 * 128;   // A window: rows [0, 384) of the image's overlapping-row view
+  static constexpr int kBBytes = 2 * 128 * 128;                     // stand-alone: both 128-position dy tiles of the image
 };
+
+// TMA of image n's A window into the 1024-aligned buffer `win` (rows past the tensor are zero-filled).  One thread.
+__device__ __forceinline__ void conv2_wgrad_load_window(uint8_t* win, const CUtensorMap* tm_x2, uint64_t* bar, int n) {
+  for (int bx = 0; bx < Conv2WgCfg::kABoxes; ++bx) tma_load_2d(win + bx * 8192, tm_x2, bar, 0, n * Conv2WgCfg::kFrame + 64 * bx);
+}
+
+// The atoms of image n's partial, one warp per atom at a time, each warp taking the next one from the shared counter *next (zero
+// before the first call): warps that join late take fewer.  An atom is computed the same way whichever warp takes it, so the result
+// does not depend on the order.  win / dys are the shared addresses of the A window and of the dy tile whose row dyrow0 is position
+// kFirst; wpart_n = the image's [512][32] partial.
+__device__ __forceinline__ void conv2_wgrad_atoms(uint32_t win, uint32_t dys, int dyrow0, float* wpart_n, int* next, int lane) {
+#pragma unroll 1
+  for (;;) {
+    int atom = 0;
+    if (lane == 0) atom = atomicAdd(next, 1);
+    atom = __shfl_sync(0xffffffffu, atom, 0);
+    if (atom >= Conv2WgCfg::kAtoms) break;
+    const int mt = atom >> 2, a = atom & 3;   // atom a of group mt (group 3 has three)
+    const int shift0 = mt < 3 ? (0 - 2) * 18 + 2 * mt - 2 : 2 * 18 - 2;
+    const int stride = mt < 3 ? 18 : 2;
+    float acc[2][4][4];
+#pragma unroll
+    for (int j2 = 0; j2 < 2; ++j2)
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) acc[j2][nt][e] = 0.f;
+    wgrad_win_atom_smem<256, 32>(acc, win, Conv2WgCfg::kFirst + shift0 + a * stride, 0, dys, dyrow0, lane);
+    wgrad_win_atom_store(acc, wpart_n + (mt * 128 + a * 32) * 32, lane);
+  }
+}
+
+// The per-image partials from given dy / x frames (the layer-1 backward binding's stand-alone form): one CTA per image, one warp
+// per atom; both operands by TMA (dy: the 256 positions from kFirst, two 128-row boxes).
+constexpr int kConv2WgThreads = Conv2WgCfg::kAtoms * 32;
+constexpr size_t kConv2WgSmem = 1024 + Conv2WgCfg::kABytes + Conv2WgCfg::kBBytes;
+__global__ void __launch_bounds__(kConv2WgThreads, 1)
+conv2_wgrad_partials_kernel(const __grid_constant__ CUtensorMap tm_x2, const __grid_constant__ CUtensorMap tm_dy2, float* __restrict__ wpart) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* win = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sd = win + Conv2WgCfg::kABytes;
+  __shared__ uint64_t ld_full;
+  __shared__ int next_atom;
+  const int n = blockIdx.x;
+  if (threadIdx.x == 0) {
+    next_atom = 0;
+    mbar_init(&ld_full, 1);
+    fence_mbar_init();
+    mbar_arrive_expect_tx(&ld_full, Conv2WgCfg::kABytes + Conv2WgCfg::kBBytes);
+    conv2_wgrad_load_window(win, &tm_x2, &ld_full, n);
+    const int first = n * Conv2WgCfg::kFrame + Conv2WgCfg::kFirst;
+    tma_load_2d(sd, &tm_dy2, &ld_full, 0, first);
+    tma_load_2d(sd + 128 * 128, &tm_dy2, &ld_full, 0, first + 128);
+  }
+  __syncthreads();
+  mbar_wait(&ld_full, 0);
+  conv2_wgrad_atoms(smem_u32(win), smem_u32(sd), 0, wpart + static_cast<size_t>(n) * 512 * 32, &next_atom, threadIdx.x & 31);
+}
 
 // One SGD update (the arithmetic of sgd_multi_kernel, ops_simt.cu) of element *p with gradient g.
 __device__ __forceinline__ void sgd_apply(float* p, float g, float* m, const SgdHyper& h, float lr) {
@@ -366,29 +410,20 @@ template <class R>
 __device__ __forceinline__ float clip_comb(const R& r, float a, float b) { return r.norm_inf ? nan_max(a, b) : a + b; }
 
 template <bool WG, class Rider = SgdRider>
-__global__ void __launch_bounds__(WG ? L1WgCfg::kThreads : kL1Threads, 1)
+__global__ void __launch_bounds__(kL1Threads, 1)
 convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y, const float* __restrict__ x, const float* __restrict__ saved,
                       const float* __restrict__ gamma, const float* __restrict__ beta, float* dgamma, float* dbeta, float* dw, float* db,
                       float* partials, float* partials_w, GridSync gs,
-                      // WG only: conv2 weight gradient of the same image
-                      const __grid_constant__ CUtensorMap tm_x2, const __grid_constant__ CUtensorMap tm_dy2, float* __restrict__ wpart,
-                      const float* __restrict__ dysum2, float* dw2, float* db2, const __grid_constant__ Rider sr) {
+                      // WG only: conv2's weight gradient, folded from the per-image partials [B][512][32] and Σdy rows [B][32]
+                      const float* __restrict__ wpart, const float* __restrict__ dysum2, float* dw2, float* db2, const __grid_constant__ Rider sr) {
   constexpr bool kClip = std::is_same_v<Rider, ClipRider<SgdRider>> || std::is_same_v<Rider, ClipRider<AdamRider>>;
   constexpr bool kAdam = std::is_same_v<Rider, AdamRider> || std::is_same_v<Rider, ClipRider<AdamRider>>;
   static_assert(kAdam || std::is_base_of_v<SgdRider, Rider>, "convnet_l1_bwd_kernel: SgdRider or AdamRider, or either in a ClipRider");
   static_assert(WG || !(kAdam || kClip), "the Adam and clipping riders ride on the kernel with the conv2 weight gradient");
-  constexpr int NAMED = WG ? kL1Threads : 0;
-  extern __shared__ __align__(16) uint8_t dsm_raw[];
-  // WG: everything is placed relative to a 1024-aligned base (the swizzled TMA tiles need it)
-  uint8_t* dsm_b = WG ? reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(dsm_raw) + 1023) & ~uintptr_t(1023)) : dsm_raw;
-  float* dsm = reinterpret_cast<float*>(dsm_b);
+  extern __shared__ __align__(16) float dsm[];
   float* dys = dsm;                  // [784][16]
   float* fold = dsm + 784 * 16;      // [25 warps][16][32]
-  uint8_t* sa = dsm_b + L1WgCfg::kOff;                              // WG: A window
-  uint8_t* sb = sa + L1WgCfg::kABytes;                              // WG: dy tiles
-  uint64_t* ld_full = reinterpret_cast<uint64_t*>(sb + L1WgCfg::kBBytes);
-  float* adam_f = reinterpret_cast<float*>(sb + L1WgCfg::kBBytes + 64);   // Adam rider: kAdamFactors floats behind the barrier word
-  static_assert(64 + kAdamFactors * sizeof(float) <= 256, "Adam rider factors must fit the tail of the dynamic shared memory");
+  __shared__ float adam_f[kAdam ? kAdamFactors : 1];   // Adam rider: the per-launch factors
   __shared__ float xs[32 * 32];
   __shared__ float red[kL1Warps * 32];
   __shared__ float s_tmp[kL1Warps * 32];
@@ -397,38 +432,12 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = blockIdx.x, B = gridDim.x;
   float* s_clip = red + 512;   // ClipRider: per-warp norm partials + the coefficient (s_db below takes red[0, 512) only)
 
-  if constexpr (WG) {
-    if (warp == kL1Warps) {
-      // ================= operands of the conv2 weight gradient of image n: one warp loads them by TMA =================
-      using Cfg = L1WgCfg;
-      if (lane == 0) {
-        tma_prefetch_desc(&tm_x2);
-        tma_prefetch_desc(&tm_dy2);
-        mbar_init(ld_full, 1);
-        fence_mbar_init();
-      }
-      __syncwarp();
-      asm volatile("bar.arrive 0, %0;" ::"n"(L1WgCfg::kThreads) : "memory");   // (1) the layer-1 warps sync on barrier 0 before they wait on ld_full
-      const int frame0 = n * Cfg::kFrame;
-      // let the layer-1 warps have the L2 → SM path for their opening loads first
-      asm volatile("bar.sync 4, %0;" ::"n"(L1WgCfg::kThreads) : "memory");
-      if (elect_one()) {
-        mbar_arrive_expect_tx(ld_full, Cfg::kABytes + Cfg::kBBytes);
-        for (int bx = 0; bx < Cfg::kABoxes; ++bx) tma_load_2d(sa + bx * 8192, &tm_x2, ld_full, 0, frame0 + 64 * bx);   // rows past the tensor are zero-filled
-        tma_load_2d(sb, &tm_dy2, ld_full, 0, frame0 + Cfg::kFirst);
-        tma_load_2d(sb + 128 * 128, &tm_dy2, ld_full, 0, frame0 + Cfg::kFirst + 128);
-      }
-      __syncwarp();
-      return;
-    }
-  }
-
   const L1Map m(tid);
   GridBar bar(gs);
   TRACE_INIT();
   trace(1, 0);
 
-  l1_load_image<NAMED>(x + static_cast<size_t>(n) * 784, xs, tid);
+  l1_load_image(x + static_cast<size_t>(n) * 784, xs, tid);
   if (tid < 16) {
     const float mean = saved[tid], invstd = saved[16 + tid];
     const float g = gamma ? gamma[tid] : 1.f, b = beta ? beta[tid] : 0.f;
@@ -440,7 +449,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   if constexpr (kAdam) {
     if (sr.on) adam_factors(sr, adam_f, tid);   // reads the step counts: before the first grid barrier
   }
-  cta_sync<NAMED>();
+  __syncthreads();
 
   float yv[16], dz[16];
   {
@@ -465,7 +474,6 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
     zmax[j] = t;
     mine |= (z == t ? 1u : 0u) << j;
   }
-  if constexpr (WG) asm volatile("bar.arrive 4, %0;" ::"n"(L1WgCfg::kThreads) : "memory");   // y / dp have arrived: the tensor-core warp may load
   unsigned int lower = 0;  // positions of the window that come before this one
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
@@ -487,7 +495,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
     warp_transpose_reduce32(v, lane);
     red[warp * 32 + lane] = v[0];
   }
-  cta_sync<NAMED>();
+  __syncthreads();
   if (tid < 32) {
     float s = 0.f;
 #pragma unroll 5
@@ -495,20 +503,17 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
     partials[static_cast<size_t>(n) * 32 + tid] = s;
   }
   trace(1, 1);
-  bar.arrive<NAMED>(gs);
+  bar.arrive(gs);
   // (each update below is spelled out for both riders: the SGD instantiation keeps the code it had before the Adam rider existed)
   const float sgd_lr = sr.on ? (sr.h.lr_dev ? __ldg(sr.h.lr_dev) : static_cast<float>(sr.h.lr)) : 0.f;
+  float ca = 0.f;   // ClipRider: this thread's share of the gradient norm
   if constexpr (kClip) {
     // in the barrier's shadow: the norm partial of the parameters whose gradients were complete before this kernel started
-    // (classifier, bn2); their update waits for the coefficient
-    float ca = 0.f;
+    // (classifier, bn2, and below conv2); their update waits for the coefficient
 #pragma unroll
     for (int t = 0; t < 4; ++t)
       if (sr.p[6 + t])
         for (int i = n * kL1Threads + tid; i < sr.n_prev[t]; i += B * kL1Threads) ca = clip_acc(sr, ca, __ldg(sr.g_prev[t] + i));
-#pragma unroll
-    for (int off = 16; off >= 1; off >>= 1) ca = clip_comb(sr, ca, __shfl_xor_sync(0xffffffffu, ca, off));
-    if (lane == 0) s_clip[warp] = ca;
   } else if (sr.on) {
     // in the barrier's shadow: the optimizer step of the parameters whose gradients were complete before this kernel started
     // (classifier, bn2) — nothing in this kernel reads them
@@ -518,9 +523,83 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
         if constexpr (kAdam) adam_apply(sr, 6 + t, i, __ldg(sr.g_prev[t] + i), adam_f);
         else sgd_apply(sr.p[6 + t] + i, __ldg(sr.g_prev[t] + i), sr.m[6 + t] ? sr.m[6 + t] + i : nullptr, sr.h, sgd_lr);
   }
-  bar.wait<NAMED>(gs);
+  if constexpr (WG) {
+    // in the barrier's shadow: conv2's weight gradient, complete before this kernel started (the layer-2 backward kernel wrote the
+    // per-image partials), and its optimizer step — nothing in this kernel reads conv2's parameters.  CTA n folds outputs n, n + B,
+    // … of the 400 (tap, ci) rows × 32 co (+ row 400: the bias, from the per-image Σdy rows) over the B per-image partials — warp =
+    // one of 25 partial classes, lane = co, classes combined through smem in a fixed order, up to five outputs per round so that
+    // ~20 L2 loads per thread are in flight
+    float* s_f = fold;   // [5][25][32]
+    constexpr size_t kStride = 512 * 32;
+    for (int base = n; base < 401; base += 5 * B) {
+      float acc[5];
+      const float* src[5];
+      size_t stride[5];
+#pragma unroll
+      for (int u = 0; u < 5; ++u) {
+        const int i = base + u * B;
+        if (i < 400) {
+          const int tap = i >> 4, ci = i & 15, kh = tap / 5, kw = tap - kh * 5;
+          // accumulator row of (kh, kw, ci): tiles 0-2 = kw/2 with kh 0..3 stacked, tile 3 = kh 4 with kw/2 stacked
+          const int mrow = (kh < 4 ? (kw >> 1) * 128 + kh * 32 : 384 + (kw >> 1) * 32) + (kw & 1) * 16 + ci;
+          src[u] = wpart + static_cast<size_t>(mrow) * 32 + lane;
+          stride[u] = kStride;
+        } else {
+          src[u] = i == 400 ? dysum2 + lane : nullptr;   // row 400: the bias gradient from the per-image Σdy rows
+          stride[u] = 32;
+        }
+        acc[u] = 0.f;
+      }
+      for (int c0 = warp; c0 < B; c0 += 4 * kL1Warps) {   // 5 outputs × 4 rows = 20 independent L2 loads in flight per thread
+        float t[5][4];
+#pragma unroll
+        for (int u = 0; u < 5; ++u)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int c = c0 + j * kL1Warps;
+            t[u][j] = (src[u] != nullptr && c < B) ? __ldcg(src[u] + static_cast<size_t>(c) * stride[u]) : 0.f;
+          }
+#pragma unroll
+        for (int u = 0; u < 5; ++u)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) acc[u] += t[u][j];
+      }
+      __syncthreads();
+#pragma unroll
+      for (int u = 0; u < 5; ++u) s_f[(u * kL1Warps + warp) * 32 + lane] = acc[u];
+      __syncthreads();
+      if (tid < 160) {
+        const int u = tid >> 5, i = base + u * B;
+        if (i <= 400) {
+          float tot = 0.f;
+#pragma unroll 5
+          for (int wi = 0; wi < kL1Warps; ++wi) tot += s_f[(u * kL1Warps + wi) * 32 + lane];
+          if (i < 400) {
+            const int e = (lane * 16 + (i & 15)) * 25 + (i >> 4);
+            dw2[e] = tot;
+            if constexpr (kClip) ca = clip_acc(sr, ca, tot);
+            else if constexpr (kAdam) { if (sr.on) adam_apply(sr, 4, e, tot, adam_f); }
+            else if (sr.on) sgd_apply(sr.p[4] + e, tot, sr.m[4] ? sr.m[4] + e : nullptr, sr.h, sgd_lr);
+          } else if (db2) {
+            db2[lane] = tot;
+            if constexpr (kClip) { if (sr.p[5]) ca = clip_acc(sr, ca, tot); }
+            else if constexpr (kAdam) { if (sr.on && sr.p[5]) adam_apply(sr, 5, lane, tot, adam_f); }
+            else if (sr.on && sr.p[5]) sgd_apply(sr.p[5] + lane, tot, sr.m[5] ? sr.m[5] + lane : nullptr, sr.h, sgd_lr);
+          }
+        }
+      }
+    }
+    trace(1, 7);
+  }
+  if constexpr (kClip) {
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) ca = clip_comb(sr, ca, __shfl_xor_sync(0xffffffffu, ca, off));
+    if (lane == 0) s_clip[warp] = ca;
+    ca = 0.f;
+  }
+  bar.wait(gs);
   trace(1, 2);
-  fold_rows_wide<32, kL1Threads, NAMED>(partials, B, s_tmp, s_tot);  // [0..16) Σdz, [16..32) Σdz·x̂
+  fold_rows_wide<32, kL1Threads>(partials, B, s_tmp, s_tot);  // [0..16) Σdz, [16..32) Σdz·x̂
   trace(1, 3);
   if (n == 0 && tid < 16) {
     if (dbeta) dbeta[tid] = s_tot[tid];
@@ -540,7 +619,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
       dst[q] = make_float4(o[0], o[1], o[2], o[3]);
     }
   }
-  cta_sync<NAMED>();
+  __syncthreads();
   // conv1 weight gradient of this image on the tensor cores: dW[co][tap] = Σ_px dy[px][co] · x[px + tap] is a
   // 16 × 32 × 784 GEMM (taps 25..31 padded; tap 25 multiplies a column of ones → the bias gradient).  M = 16 is below
   // the 64-row wgmma tile, so this is warp-level mma.sync m16n8k8 (TF32 in, fp32 accumulate): a warp takes every
@@ -589,10 +668,10 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
     const int co = tid & 15, part = tid >> 4;
     for (int p = part; p < 784; p += 32) dbp += dys[p * 16 + co];
   }
-  cta_sync<NAMED>();
+  __syncthreads();
   float* s_db = red;   // [32 parts][16]  (the statistics scratch is free again)
   if (tid < 512) s_db[tid] = dbp;
-  cta_sync<NAMED>();
+  __syncthreads();
   if (tid < 512) {
     float sacc = 0.f;
     if ((tid & 31) == 25) {
@@ -606,32 +685,8 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
     partials_w[static_cast<size_t>(n) * 512 + tid] = sacc;   // index = co·32 + tap  (tap 25 = bias, 26..31 unused)
   }
   trace(1, 4);
-  if constexpr (WG) {
-    // the operands have been loading since the kernel started: 15 warps take one 32-row atom each and write this image's
-    // partial [512][32]
-    asm volatile("bar.sync 0, %0;" ::"n"(L1WgCfg::kThreads) : "memory");   // (1) ld_full initialised (long ago)
-    if (warp < 15) {
-      mbar_wait(ld_full, 0);
-      const int mt = warp >> 2, a = warp & 3;   // atom a of group mt (group 3 has three)
-      const int shift0 = mt < 3 ? (0 - 2) * 18 + 2 * mt - 2 : 2 * 18 - 2;
-      const int stride = mt < 3 ? 18 : 2;
-
-      float acc[2][4][4];
-#pragma unroll
-      for (int j2 = 0; j2 < 2; ++j2)
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-          for (int e = 0; e < 4; ++e) acc[j2][nt][e] = 0.f;
-      wgrad_win_atom<256, 32, 1>(acc, reinterpret_cast<const float*>(sa), L1WgCfg::kFirst + shift0 + a * stride, 0, reinterpret_cast<const float*>(sb), 0,
-                     lane);
-      wgrad_win_atom_store(acc, wpart + (static_cast<size_t>(n) * 512 + mt * 128 + a * 32) * 32, lane);
-    }
-    trace(1, 7);
-  }
-  bar.sync<NAMED>(gs);
+  bar.sync(gs);
   trace(1, 5);
-  float ca = 0.f;   // ClipRider: this thread's share of the norm of the gradients folded from here on
   // every CTA folds a few of the 16 × 26 outputs over the B partial rows: one warp per output, fixed order
   for (int j = n + warp * B; j < 512; j += kL1Warps * B) {
     const int co = j >> 5, tap = j & 31;
@@ -674,84 +729,19 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
       for (int k = 0; k < 10; ++k)
         if (sr.step[k]) *sr.step[k] += 1.f;
   }
-  if constexpr (WG) {
-    // conv2 weight gradient: CTA n folds outputs n, n + B, … of the 400 (tap, ci) rows × 32 co (+ row 400: the bias, from the
-    // per-image Σdy rows) over the B per-image partials — warp = one of 25 partial classes, lane = co, classes combined
-    // through smem in a fixed order, up to five outputs per round so that ~20 L2 loads per thread are in flight
-    float* s_f = fold;   // [5][25][32]
-    constexpr size_t kStride = 512 * 32;
-    for (int base = n; base < 401; base += 5 * B) {
-      float acc[5];
-      const float* src[5];
-      size_t stride[5];
-#pragma unroll
-      for (int u = 0; u < 5; ++u) {
-        const int i = base + u * B;
-        if (i < 400) {
-          const int tap = i >> 4, ci = i & 15, kh = tap / 5, kw = tap - kh * 5;
-          // accumulator row of (kh, kw, ci): tiles 0-2 = kw/2 with kh 0..3 stacked, tile 3 = kh 4 with kw/2 stacked
-          const int mrow = (kh < 4 ? (kw >> 1) * 128 + kh * 32 : 384 + (kw >> 1) * 32) + (kw & 1) * 16 + ci;
-          src[u] = wpart + static_cast<size_t>(mrow) * 32 + lane;
-          stride[u] = kStride;
-        } else {
-          src[u] = i == 400 ? dysum2 + lane : nullptr;   // row 400: the bias gradient from the per-image Σdy rows
-          stride[u] = 32;
-        }
-        acc[u] = 0.f;
-      }
-      for (int c0 = warp; c0 < B; c0 += 4 * kL1Warps) {   // 5 outputs × 4 rows = 20 independent L2 loads in flight per thread
-        float t[5][4];
-#pragma unroll
-        for (int u = 0; u < 5; ++u)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int c = c0 + j * kL1Warps;
-            t[u][j] = (src[u] != nullptr && c < B) ? __ldcg(src[u] + static_cast<size_t>(c) * stride[u]) : 0.f;
-          }
-#pragma unroll
-        for (int u = 0; u < 5; ++u)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) acc[u] += t[u][j];
-      }
-      cta_sync<NAMED>();
-#pragma unroll
-      for (int u = 0; u < 5; ++u) s_f[(u * kL1Warps + warp) * 32 + lane] = acc[u];
-      cta_sync<NAMED>();
-      if (tid < 160) {
-        const int u = tid >> 5, i = base + u * B;
-        if (i <= 400) {
-          float tot = 0.f;
-#pragma unroll 5
-          for (int wi = 0; wi < kL1Warps; ++wi) tot += s_f[(u * kL1Warps + wi) * 32 + lane];
-          if (i < 400) {
-            const int e = (lane * 16 + (i & 15)) * 25 + (i >> 4);
-            dw2[e] = tot;
-            if constexpr (kClip) ca = clip_acc(sr, ca, tot);
-            else if constexpr (kAdam) { if (sr.on) adam_apply(sr, 4, e, tot, adam_f); }
-            else if (sr.on) sgd_apply(sr.p[4] + e, tot, sr.m[4] ? sr.m[4] + e : nullptr, sr.h, sgd_lr);
-          } else if (db2) {
-            db2[lane] = tot;
-            if constexpr (kClip) { if (sr.p[5]) ca = clip_acc(sr, ca, tot); }
-            else if constexpr (kAdam) { if (sr.on && sr.p[5]) adam_apply(sr, 5, lane, tot, adam_f); }
-            else if (sr.on && sr.p[5]) sgd_apply(sr.p[5] + lane, tot, sr.m[5] ? sr.m[5] + lane : nullptr, sr.h, sgd_lr);
-          }
-        }
-      }
-    }
-  }
   if constexpr (kClip) {
     // every gradient has been seen: one partial per CTA, one more grid barrier, then every CTA folds the B partials in the same
     // order and derives the same coefficient bit for bit
 #pragma unroll
     for (int off = 16; off >= 1; off >>= 1) ca = clip_comb(sr, ca, __shfl_xor_sync(0xffffffffu, ca, off));
     if (lane == 0) s_clip[warp] = clip_comb(sr, s_clip[warp], ca);
-    cta_sync<NAMED>();
+    __syncthreads();
     if (tid == 0) {
       float s = s_clip[0];
       for (int w = 1; w < kL1Warps; ++w) s = clip_comb(sr, s, s_clip[w]);
       sr.part[n] = s;
     }
-    bar.sync<NAMED>(gs);
+    bar.sync(gs);
     if (warp == 0) {
       double d = 0.0;
       for (int r = lane; r < B; r += 32) {
@@ -769,7 +759,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
         if (n == 0) *sr.norm_out = norm;
       }
     }
-    cta_sync<NAMED>();
+    __syncthreads();
     const float coef = s_clip[kL1Warps];
     // grid-stride pass over the ten gradients (read from L2: other CTAs wrote them): .grad becomes the clipped gradient, as after
     // clip_grad_norm_, and the update takes it
@@ -1361,13 +1351,21 @@ struct L2BwdSmem {
   // FC (the classifier's backward rides along): fc weights [16][1568] | dlogits [B ≤ 160][16] | pooled slice [B ≤ 160][16]
   static constexpr int kFcW = 16 * 1568 * 4, kFcDl = 160 * 16 * 4, kFcP = 160 * 16 * 4;
   static constexpr int kTotalFc = kTotal + kFcW + kFcDl + kFcP;
+  // WG: conv2's A window (Conv2WgCfg) at the same 1024-aligned offset as the fc weights — over them once they are dead (FC), or
+  // behind everything else
+  static constexpr int kWin = kPatchAlloc + kB + 4096;
+  static constexpr int kTotalWg = kTotal + Conv2WgCfg::kABytes;
+  static_assert(kWin % 1024 == 0 && Conv2WgCfg::kABytes <= kFcW, "conv2 weight-gradient window placement");
 };
 
 // FC: the classifier's backward rides along.  The gradient of the pooled activations is not read from `dout` but computed
 // on the fly, d(out)[n][k] = Σ_j dlogits[n][j] · Wfc[j][k] (fc weights staged in smem once per CTA); the classifier's weight
 // gradient dWfc[j][k] = Σ_n dlogits[n][j] · out[n][k] is produced in 16-column slices, one slice per CTA (all images, fixed
 // order: deterministic, no partials), the bias gradient by the CTA that owns "slice 98".  One kernel less per step.
-template <bool FC>
+// WG: conv2's weight gradient partial of the image (Conv2WgCfg) is computed here, by warps 0..3 while warps 4..7 run the data
+// gradient's asynchronous wgmma (and warps 4..7 once that is done): its B operand is the dy patch this kernel builds anyway, its A operand (the layer-1 output frame)
+// arrives by TMA in the shadow of the grid barrier.  The global dy frame is then not written: nothing reads it.
+template <bool FC, bool WG>
 __global__ void __launch_bounds__(kL2Threads, 1)
 convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float* __restrict__ y /*[B,14,14,32]*/,
                       const float* __restrict__ saved, const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -1377,7 +1375,10 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
                       // FC only
                       const float* __restrict__ dlogits /*[B,ncls]*/, const float* __restrict__ fcw /*[ncls,1568]*/,
                       const float* __restrict__ pooled /*[B,1568] = forward's out*/, float* dfcw /*[ncls,1568]*/, float* dfcb /*[ncls]*/,
-                      int ncls, const float* __restrict__ loss_parts /*[B] or null*/, float* loss_out) {
+                      int ncls, const float* __restrict__ loss_parts /*[B] or null*/, float* loss_out,
+                      // WG only
+                      const __grid_constant__ CUtensorMap tm_x2 /*overlapping-row view of the layer-1 output frame*/,
+                      float* __restrict__ wpart /*[B][512][32]*/) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sa = smem;                                  // dy patch, written by the CTA in the TMA/wgmma SWIZZLE_128B layout
@@ -1393,11 +1394,26 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
   float* s_fcw = misc + 1024;                                   // FC: [ncls][1568]
   float* s_dl = s_fcw + L2BwdSmem::kFcW / 4;                    // FC: [B][16] (columns >= ncls zero)
   float* s_pool = s_dl + L2BwdSmem::kFcDl / 4;                  // FC: [B][16] slice of the pooled activations
+  uint8_t* s_win = smem + L2BwdSmem::kWin;                      // WG: conv2's A window
+  __shared__ uint64_t win_full;
+  __shared__ int next_atom;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = blockIdx.x, B = gridDim.x;
 
   GridBar bar(gs);
   TRACE_INIT();
   trace(3, 0);
+  if constexpr (WG) {
+    if (tid == 0) {
+      next_atom = 0;
+      tma_prefetch_desc(&tm_x2);
+      mbar_init(&win_full, 1);
+      fence_mbar_init();
+      if constexpr (!FC) {   // a region of its own: load now
+        mbar_arrive_expect_tx(&win_full, Conv2WgCfg::kABytes);
+        conv2_wgrad_load_window(s_win, &tm_x2, &win_full, n);
+      }
+    }
+  }
   if constexpr (FC) {
     // stage the classifier weights (cp.async, no registers, lands while the dgrad weights are built), every image's dlogits and this
     // CTA's first 16-column slice of the pooled activations (loads batched in registers: one L2 latency, not one per element)
@@ -1495,6 +1511,15 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
   s_part[g * 64 + c] = s1;
   s_part[g * 64 + 32 + c] = s2;
   __syncthreads();
+  if constexpr (WG && FC) {
+    // the classifier weights are dead: the window goes over them (their cp.async writes and generic reads are ordered before the
+    // TMA writes by the proxy fence) and lands in the shadow of the grid barrier
+    if (tid == 0) {
+      fence_proxy_async_smem();
+      mbar_arrive_expect_tx(&win_full, Conv2WgCfg::kABytes);
+      conv2_wgrad_load_window(s_win, &tm_x2, &win_full, n);
+    }
+  }
   if (tid < 64) {
     float s = 0.f;
 #pragma unroll
@@ -1505,9 +1530,11 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
   bar.arrive(gs);
   // ---- in the shadow of the grid barrier: work that no other CTA waits for ----
   // zero halo of the global dy frame (the weight gradient sums over all 324 positions)
-  for (int i = tid; i < 324 * 8; i += kL2Threads) {
-    const int P = i >> 3, pr = P / 18, pc = P - pr * 18;
-    if (pr < 2 || pr >= 16 || pc < 2 || pc >= 16) reinterpret_cast<float4*>(dy + (static_cast<size_t>(n) * 324 + P) * 32)[i & 7] = make_float4(0.f, 0.f, 0.f, 0.f);
+  if constexpr (!WG) {
+    for (int i = tid; i < 324 * 8; i += kL2Threads) {
+      const int P = i >> 3, pr = P / 18, pc = P - pr * 18;
+      if (pr < 2 || pr >= 16 || pc < 2 || pc >= 16) reinterpret_cast<float4*>(dy + (static_cast<size_t>(n) * 324 + P) * 32)[i & 7] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
   }
   if constexpr (FC) {
     // classifier weight gradient, slice = 16 consecutive columns (98 slices; "slice 98" = the bias): thread = (column, class).
@@ -1580,7 +1607,7 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
           const float xh = (yv[k][d] - mu) * is;
           const float v = sc * ((d == arg[k] ? dzv[k] : 0.f) - m1 - xh * m2);
           const int P = (oh + 2) * kPW + ow + 2;
-          dy[(static_cast<size_t>(n) * 324 + P) * 32 + c] = v;                      // frame for the weight-gradient kernel (TMA)
+          if constexpr (!WG) dy[(static_cast<size_t>(n) * 324 + P) * 32 + c] = v;  // frame for the weight-gradient kernel (TMA)
           *reinterpret_cast<float*>(sa + sw128_off(P, c >> 2) + (c & 3) * 4) = v;   // same frame in smem for the data-gradient MMAs
           dsum += v;
         }
@@ -1635,6 +1662,13 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
       }
     }
   }
+  if constexpr (WG) {
+    // ---- conv2 weight-gradient partial of this image, one 32-row atom per warp at a time: warps 0..3 start next to the wgmma,
+    // warps 4..7 join when their data gradient is done ---------------------------------------------------------------------
+    mbar_wait(&win_full, 0);
+    conv2_wgrad_atoms(smem_u32(s_win), smem_u32(sa), Conv2WgCfg::kFirst, wpart + static_cast<size_t>(n) * 512 * 32, &next_atom, lane);
+    trace(3, 7);
+  }
   __syncthreads();
   bar.finish(gs);
   trace(3, 6);
@@ -1684,36 +1718,35 @@ void launch_convnet_l1_fwd(const float* x, const float* w, const float* bias, co
 void launch_convnet_l1_bwd(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
                            float* dgamma, float* dbeta, float* dw, float* db, int B, float* partials, float* partials_w, GridSync gs,
                            cudaStream_t st) {
-  CUtensorMap none{};
   launch_cooperative(convnet_l1_bwd_kernel<false>, B, kL1Threads, static_cast<size_t>(kL1BwdSmem), st, "convnet_l1_bwd", dp, y, x, saved, gamma, beta, dgamma,
-                     dbeta, dw, db, partials, partials_w, gs, none, none, static_cast<float*>(nullptr), static_cast<const float*>(nullptr),
+                     dbeta, dw, db, partials, partials_w, gs, static_cast<const float*>(nullptr), static_cast<const float*>(nullptr),
                      static_cast<float*>(nullptr), static_cast<float*>(nullptr), SgdRider{});
+}
+
+void launch_conv2_wgrad_partials(const float* dy2_pad, const float* x2_pad, int B, float* wpart, cudaStream_t st) {
+  CUtensorMap tm_x, tm_dy;
+  make_wgrad_win_tmaps(x2_pad, dy2_pad, B, &tm_x, &tm_dy);
+  opt_in_smem(conv2_wgrad_partials_kernel, kConv2WgSmem);
+  conv2_wgrad_partials_kernel<<<B, kConv2WgThreads, kConv2WgSmem, st>>>(tm_x, tm_dy, wpart);
+  check_launch("conv2_wgrad_partials");
 }
 
 template <class Rider>
 void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
-                                 float* dgamma, float* dbeta, float* dw, float* db, const float* dy2_pad, const float* x2_pad, const float* dysum2,
-                                 float* dw2, float* db2, int B, float* partials, float* partials_w, float* wpart, GridSync gs, cudaStream_t st,
-                                 Rider rider) {
-  CUtensorMap tm_x, tm_dy;
-  make_wgrad_win_tmaps(x2_pad, dy2_pad, B, &tm_x, &tm_dy);
-  launch_cooperative(convnet_l1_bwd_kernel<true, Rider>, B, L1WgCfg::kThreads, L1WgCfg::kSmem, st, "convnet_l1_bwd_wgrad", dp, y, x, saved, gamma, beta,
-                     dgamma, dbeta, dw, db, partials, partials_w, gs, tm_x, tm_dy, wpart, dysum2, dw2, db2, rider);
+                                 float* dgamma, float* dbeta, float* dw, float* db, const float* wpart, const float* dysum2, float* dw2, float* db2,
+                                 int B, float* partials, float* partials_w, GridSync gs, cudaStream_t st, Rider rider) {
+  launch_cooperative(convnet_l1_bwd_kernel<true, Rider>, B, kL1Threads, static_cast<size_t>(kL1BwdSmem), st, "convnet_l1_bwd_wgrad", dp, y, x, saved,
+                     gamma, beta, dgamma, dbeta, dw, db, partials, partials_w, gs, wpart, dysum2, dw2, db2, rider);
 }
-template void launch_convnet_l1_bwd_wgrad<SgdRider>(const float*, const float*, const float*, const float*, const float*, const float*, float*,
-                                                    float*, float*, float*, const float*, const float*, const float*, float*, float*, int, float*,
-                                                    float*, float*, GridSync, cudaStream_t, SgdRider);
-template void launch_convnet_l1_bwd_wgrad<AdamRider>(const float*, const float*, const float*, const float*, const float*, const float*, float*,
-                                                     float*, float*, float*, const float*, const float*, const float*, float*, float*, int, float*,
-                                                     float*, float*, GridSync, cudaStream_t, AdamRider);
-template void launch_convnet_l1_bwd_wgrad<ClipRider<SgdRider>>(const float*, const float*, const float*, const float*, const float*,
-                                                               const float*, float*, float*, float*, float*, const float*, const float*,
-                                                               const float*, float*, float*, int, float*, float*, float*, GridSync, cudaStream_t,
-                                                               ClipRider<SgdRider>);
-template void launch_convnet_l1_bwd_wgrad<ClipRider<AdamRider>>(const float*, const float*, const float*, const float*, const float*,
-                                                                const float*, float*, float*, float*, float*, const float*, const float*,
-                                                                const float*, float*, float*, int, float*, float*, float*, GridSync, cudaStream_t,
-                                                                ClipRider<AdamRider>);
+#define PDT_L1_BWD_WGRAD(R)                                                                                                            \
+  template void launch_convnet_l1_bwd_wgrad<R>(const float*, const float*, const float*, const float*, const float*, const float*, float*, \
+                                               float*, float*, float*, const float*, const float*, float*, float*, int, float*, float*,       \
+                                               GridSync, cudaStream_t, R);
+PDT_L1_BWD_WGRAD(SgdRider)
+PDT_L1_BWD_WGRAD(AdamRider)
+PDT_L1_BWD_WGRAD(ClipRider<SgdRider>)
+PDT_L1_BWD_WGRAD(ClipRider<AdamRider>)
+#undef PDT_L1_BWD_WGRAD
 
 void launch_convnet_l2_fwd(const float* x, const float* w, const float* bias, const float* gamma, const float* beta, float* y, float* out,
                            float* saved, float* running_mean, float* running_var, long long* nbt, float momentum, float eps,
@@ -1736,21 +1769,28 @@ void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const 
 
 void launch_convnet_l2_bwd(const float* dout, const float* y, const float* saved, const float* gamma, const float* beta, const float* w,
                            float* dgamma, float* dbeta, float* dy, float* dx, float* dysum, int B, float* partials, GridSync gs,
-                           cudaStream_t st) {
-  launch_cooperative(convnet_l2_bwd_kernel<false>, B, kL2Threads, static_cast<size_t>(L2BwdSmem::kTotal), st, "convnet_l2_bwd", dout, y, saved, gamma, beta, w,
-                     dgamma, dbeta, dy, dx, dysum, partials, gs, static_cast<const float*>(nullptr), static_cast<const float*>(nullptr),
-                     static_cast<const float*>(nullptr), static_cast<float*>(nullptr), static_cast<float*>(nullptr), 0, static_cast<const float*>(nullptr),
-                     static_cast<float*>(nullptr));
+                           cudaStream_t st, const float* x2, float* wpart) {
+  CUtensorMap tm_x2{};
+  if (x2 != nullptr) make_wgrad_win_xmap(x2, B, &tm_x2);
+  auto kernel = x2 != nullptr ? convnet_l2_bwd_kernel<false, true> : convnet_l2_bwd_kernel<false, false>;
+  launch_cooperative(kernel, B, kL2Threads, static_cast<size_t>(x2 != nullptr ? L2BwdSmem::kTotalWg : L2BwdSmem::kTotal), st, "convnet_l2_bwd", dout,
+                     y, saved, gamma, beta, w, dgamma, dbeta, dy, dx, dysum, partials, gs, static_cast<const float*>(nullptr),
+                     static_cast<const float*>(nullptr), static_cast<const float*>(nullptr), static_cast<float*>(nullptr), static_cast<float*>(nullptr), 0,
+                     static_cast<const float*>(nullptr), static_cast<float*>(nullptr), tm_x2, wpart);
 }
 
 void launch_convnet_l2_bwd_fc(const float* dlogits, const float* fcw, const float* pooled, float* dfcw, float* dfcb, int ncls, const float* y,
                               const float* saved, const float* gamma, const float* beta, const float* w, float* dgamma, float* dbeta, float* dy,
-                              float* dx, float* dysum, int B, float* partials, GridSync gs, cudaStream_t st, const float* loss_parts, float* loss_out) {
+                              float* dx, float* dysum, int B, float* partials, GridSync gs, cudaStream_t st, const float* loss_parts, float* loss_out,
+                              const float* x2, float* wpart) {
   if (ncls < 1 || ncls > 16) throw std::invalid_argument("convnet_l2_bwd_fc: 1..16 classes");
   if (B > 160) throw std::invalid_argument("convnet_l2_bwd_fc: batch too large for the staged dlogits");
-  launch_cooperative(convnet_l2_bwd_kernel<true>, B, kL2Threads, static_cast<size_t>(L2BwdSmem::kTotalFc), st, "convnet_l2_bwd_fc",
-                     static_cast<const float*>(nullptr), y, saved, gamma, beta, w, dgamma, dbeta, dy, dx, dysum, partials, gs, dlogits, fcw, pooled, dfcw,
-                     dfcb, ncls, loss_parts, loss_out);
+  CUtensorMap tm_x2{};
+  if (x2 != nullptr) make_wgrad_win_xmap(x2, B, &tm_x2);
+  auto kernel = x2 != nullptr ? convnet_l2_bwd_kernel<true, true> : convnet_l2_bwd_kernel<true, false>;
+  launch_cooperative(kernel, B, kL2Threads, static_cast<size_t>(L2BwdSmem::kTotalFc), st, "convnet_l2_bwd_fc", static_cast<const float*>(nullptr), y, saved,
+                     gamma, beta, w, dgamma, dbeta, dy, dx, dysum, partials, gs, dlogits, fcw, pooled, dfcw, dfcb, ncls, loss_parts, loss_out, tm_x2,
+                     wpart);
 }
 
 }  // namespace pdt

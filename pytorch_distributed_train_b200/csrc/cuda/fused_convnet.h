@@ -50,7 +50,7 @@ struct AdamRider {
 };
 // Either rider with gradient-norm clipping in front of the update (torch.nn.utils.clip_grad_norm_, norm_type 2 or inf).  Every CTA
 // adds up the squares (or the max |g|) of the gradient elements it sees — those of parameters 6..9 in the shadow of the first
-// grid barrier, those of 0..5 as it folds them — and writes one partial; after one more grid barrier every CTA folds the B
+// grid barrier, those of 0..5 as it folds them (4, 5 in that shadow too) — and writes one partial; after one more grid barrier every CTA folds the B
 // partials in the same order (fp64), derives the same coefficient, and in a grid-stride pass writes g·coef back to every
 // gradient and applies the update with it.  CTA 0 stores the norm.
 template <class Base>
@@ -61,14 +61,15 @@ struct ClipRider : Base {
   float* part = nullptr;       // [B] per-CTA partials
 };
 
-// Layer-1 backward with the conv2 weight gradient of the same image running on the tensor cores next to it (two extra warps):
-// dy2_pad [B,18,18,32] / x2_pad [B,18,18,16] frames and dysum2 [B,32] from layer-2 backward → dw2 [32,16,5,5], db2 [32].
-// wpart: B·512·32 floats of scratch, disjoint from partials / partials_w.  Rider: SgdRider or AdamRider, or either one in a ClipRider.
+// conv2's weight gradient per image (wpart [B][512][32], the layout of launch_convnet_l2_bwd's WG form) from given frames:
+// dy2_pad [B,18,18,32] (zero halo), x2_pad [B,18,18,16].  One CTA per image, not cooperative.
+void launch_conv2_wgrad_partials(const float* dy2_pad, const float* x2_pad, int B, float* wpart, cudaStream_t st);
+// Layer-1 backward that also folds conv2's weight gradient: the per-image partials wpart and Σdy rows dysum2 [B,32] → dw2
+// [32,16,5,5], db2 [32], in the shadow of the kernel's first grid barrier.  Rider: SgdRider or AdamRider, or either one in a ClipRider.
 template <class Rider = SgdRider>
 void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
-                                 float* dgamma, float* dbeta, float* dw, float* db, const float* dy2_pad, const float* x2_pad, const float* dysum2,
-                                 float* dw2, float* db2, int B, float* partials, float* partials_w, float* wpart, GridSync gs, cudaStream_t st,
-                                 Rider rider = Rider{});
+                                 float* dgamma, float* dbeta, float* dw, float* db, const float* wpart, const float* dysum2, float* dw2, float* db2,
+                                 int B, float* partials, float* partials_w, GridSync gs, cudaStream_t st, Rider rider = Rider{});
 // x [B,18,18,16] frame → y [B,14,14,32], out [B,32,7,7] NCHW, saved [64]; logits [B,ncls] = fc(out) when logits != nullptr.
 // partials: B·64 floats.
 void launch_convnet_l2_fwd(const float* x, const float* w, const float* bias, const float* gamma, const float* beta, float* y, float* out,
@@ -95,13 +96,17 @@ void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const 
                         FusedCe ce = FusedCe{});
 // dout [B,32,7,7] → dgamma/dbeta [32], dy [B,18,18,32] frame with zero halo (gradient at the conv2 output), dx [B,18,18,16] frame
 // (data gradient, interior written), dysum [B,32] (per-image Σdy: the conv2 bias gradient is the sum of its rows).
+// x2 != nullptr (conv2's input frame [B,18,18,16]): conv2's weight-gradient partials per image go to wpart [B][512][32] instead,
+// and dy is not written.
 void launch_convnet_l2_bwd(const float* dout, const float* y, const float* saved, const float* gamma, const float* beta, const float* w,
-                           float* dgamma, float* dbeta, float* dy, float* dx, float* dysum, int B, float* partials, GridSync gs, cudaStream_t st);
+                           float* dgamma, float* dbeta, float* dy, float* dx, float* dysum, int B, float* partials, GridSync gs, cudaStream_t st,
+                           const float* x2 = nullptr, float* wpart = nullptr);
 // The same with the classifier's backward riding along: d(out) is computed from dlogits [B,ncls] and the fc weights [ncls,1568]
 // inside the kernel; dfcw [ncls,1568] / dfcb [ncls] are produced from `pooled` = the forward's out [B,1568].  ncls ≤ 16.
 void launch_convnet_l2_bwd_fc(const float* dlogits, const float* fcw, const float* pooled, float* dfcw, float* dfcb, int ncls, const float* y,
                               const float* saved, const float* gamma, const float* beta, const float* w, float* dgamma, float* dbeta, float* dy,
                               float* dx, float* dysum, int B, float* partials, GridSync gs, cudaStream_t st,
-                              const float* loss_parts = nullptr, float* loss_out = nullptr);   // mean of the forward kernel's CE terms
+                              const float* loss_parts = nullptr, float* loss_out = nullptr,   // mean of the forward kernel's CE terms
+                              const float* x2 = nullptr, float* wpart = nullptr);             // as for launch_convnet_l2_bwd
 
 }  // namespace pdt

@@ -192,8 +192,9 @@ class sgd_rider_enabled:
 
 
 def _wgrad_rides_on_layer1() -> bool:
-    """conv2's weight gradient runs on the tensor cores *inside* the layer-1 backward kernel (two extra warps per CTA)
-    instead of as a kernel of its own between the two layer kernels.  PDT_WGRAD_MERGED=0 restores the separate launch."""
+    """conv2's weight gradient rides on the two backward kernels instead of running as a kernel of its own between them: the
+    layer-2 kernel computes the per-image partials next to its data gradient, the layer-1 kernel folds them (and applies the
+    riding optimizer's update).  PDT_WGRAD_MERGED=0 restores the separate launch."""
     return os.environ.get("PDT_WGRAD_MERGED", "1") != "0" and hasattr(_C, "convnet_l1_bwd_wgrad")
 
 
@@ -237,7 +238,7 @@ class _FusedLayer1(torch.autograd.Function):
         pending = ctx.link.pop("wgrad", None) if ctx.link is not None else None
         dw2 = db2 = None
         if pending is not None:
-            dy2, p1, dysum2 = pending
+            dy2, p1, dysum2 = pending   # dy2 = p1 = None: layer 2's kernel left the per-image partials
             dw2 = _grad_dst(w2_p, w2_p)
             db2 = _grad_dst(b2_p, b2_p) if b2_p is not None else None
             sgd = None
@@ -260,7 +261,8 @@ class _FusedLayer1(torch.autograd.Function):
 class _FusedLayer2(torch.autograd.Function):
     """conv2 (wgmma) + BN2 + ReLU + pool2 (+ the classifier's logits, which ride on the pooled activations while they
     are still in shared memory) forward; pool/ReLU/BN backward + conv2 data gradient as one kernel backward.  The
-    tensor-core weight gradient follows as its own kernel, or — the default — rides on layer 1's backward kernel."""
+    tensor-core weight gradient follows as its own kernel, or — the default — its per-image partials are computed in this
+    node's kernel and folded by layer 1's backward kernel."""
 
     @staticmethod
     def forward(ctx, p1, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, fcw, fcb, whole=None, link=None, fc_rides=False):
@@ -289,6 +291,9 @@ class _FusedLayer2(torch.autograd.Function):
         dfcw = dfcb = None
         if ctx.link is not None:   # do the gradients written here become `.grad` as they are (nothing to accumulate into)?
             ctx.link["prev_fresh"] = ctx.fc_rides and all(q is None or q.grad is None for q in (fcw_p, fcb_p, g_p, be_p))
+        # layer 1's backward kernel folds (and layer 1's node returns) conv2's weight / bias gradient; this kernel computes the
+        # per-image partials (given p1) for it
+        rides = ctx.link is not None and ctx.needs_input_grad[0]
         if ctx.fc_rides:
             p1, y, saved, gamma, beta, w, out, fcw = ctx.saved_tensors
             if dout is not None:
@@ -296,13 +301,13 @@ class _FusedLayer2(torch.autograd.Function):
             dfcw = _grad_dst(fcw_p, fcw)
             dfcb = _grad_dst(fcb_p, fcb_p) if fcb_p is not None else None
             lp, lo = ctx.ce_deferred if ctx.ce_deferred is not None else (None, None)
-            dy, dp1, dysum = _C.convnet_l2_bwd_fc(dlogits.contiguous(), fcw, out, dfcw, dfcb, y, saved, gamma, beta, w, dg, dbe, lp, lo)
+            dy, dp1, dysum = _C.convnet_l2_bwd_fc(dlogits.contiguous(), fcw, out, dfcw, dfcb, y, saved, gamma, beta, w, dg, dbe, lp, lo,
+                                                  p1 if rides else None)
         else:
             p1, y, saved, gamma, beta, w = ctx.saved_tensors
-            dy, dp1, dysum = _C.convnet_l2_bwd(dout.contiguous(), y, saved, gamma, beta, w, dg, dbe)
-        if ctx.link is not None and ctx.needs_input_grad[0]:
-            # layer 1's backward kernel computes (and layer 1's node returns) conv2's weight / bias gradient
-            ctx.link["wgrad"] = (dy, p1, dysum)
+            dy, dp1, dysum = _C.convnet_l2_bwd(dout.contiguous(), y, saved, gamma, beta, w, dg, dbe, p1 if rides else None)
+        if rides:
+            ctx.link["wgrad"] = (None, None, dysum)
             # for the optimizer rider of layer 1's kernel: WHERE these gradients were written — addresses, not tensors (an extra
             # reference would make autograd's AccumulateGrad clone the gradient instead of adopting the bucket view)
             ctx.link["prev"] = ((fcw_p, dfcw.data_ptr() if dfcw is not None else 0), (fcb_p, dfcb.data_ptr() if dfcb is not None else 0),

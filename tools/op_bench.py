@@ -96,8 +96,8 @@ def main():
     dwf, dbf = torch.empty_like(wf), torch.empty_like(bf)
     dg2, dbe2 = torch.empty(32, device=dev), torch.empty(32, device=dev)
 
-    def l2_bwd_fc():
-        return _C.convnet_l2_bwd_fc(dlog, wf, p2, dwf, dbf, y2, sv2, g2, be2, w2, dg2, dbe2, lparts, loss)
+    def l2_bwd_fc(p1=None):
+        return _C.convnet_l2_bwd_fc(dlog, wf, p2, dwf, dbf, y2, sv2, g2, be2, w2, dg2, dbe2, lparts, loss, p1)
 
     dy2, dp1, dysum = l2_bwd_fc()
     dw2, db2 = torch.empty_like(w2), torch.empty_like(b2)
@@ -107,8 +107,12 @@ def main():
     dflat = torch.randn(B, 32, 7, 7, device=dev)
     ours = [
         ("forward: conv1+BN+ReLU+pool + conv2(wgmma)+BN+ReLU+pool + fc + cross-entropy (1 kernel)", fwd_whole),
-        ("backward A: classifier bwd + pool/ReLU/BN2 bwd + conv2 dgrad(wgmma) (1 kernel)", l2_bwd_fc),
-        ("backward B: pool/ReLU/BN1 bwd + conv1 wgrad(mma.sync) + conv2 wgrad(mma.sync, window) (1 kernel)",
+        ("backward A: classifier bwd + pool/ReLU/BN2 bwd + conv2 dgrad(wgmma) + conv2 wgrad partials(mma.sync, window) (1 kernel)",
+         lambda: l2_bwd_fc(p1)),
+        ("backward A + B: the row above, then pool/ReLU/BN1 bwd + conv1 wgrad(mma.sync) + conv2 wgrad fold (2 kernels)",
+         lambda: (l2_bwd_fc(p1), _C.convnet_l1_bwd_wgrad(dp1, y1, x, sv1, g1, be1, dg1, dbe1, dw1, db1, None, None, dysum, dw2, db2))),
+        ("(variant) layer-2 bwd without the conv2 wgrad partials", l2_bwd_fc),
+        ("(variant) conv2 wgrad partials from given frames + layer-1 bwd with the fold (2 kernels)",
          lambda: _C.convnet_l1_bwd_wgrad(dp1, y1, x, sv1, g1, be1, dg1, dbe1, dw1, db1, dy2, p1, dysum, dw2, db2)),
         ("SGD, 10 tensors (1 kernel)", lambda: _C.sgd_multi(params, grads, [], 1e-4, None, 0.0, 0.0, 0.0, False, False, False)),
         ("(variant) cross-entropy fwd (+dlogits) as its own kernel", lambda: _C.cross_entropy_fwd(logits, tgt, True)),
