@@ -947,12 +947,7 @@ void launch_conv5x5_wgrad_mma(const float* dy, const float* x, float* dw, float*
   check_launch("wgrad_fold");
 }
 
-void make_wgrad_win_xmap(const float* x_pad, int B, CUtensorMap* tm_x) {
-  // the driver call needs a current context on this thread, and the layer-2 backward kernel may be the first CUDA work of an
-  // autograd worker thread: cudaSetDevice makes the runtime's primary context current
-  int dev = 0;
-  PDT_CUDA_CHECK(cudaGetDevice(&dev));
-  PDT_CUDA_CHECK(cudaSetDevice(dev));
+void make_wgrad_win_tmaps(const float* x_pad, const float* dy_pad, int B, CUtensorMap* tm_x, CUtensorMap* tm_dy) {
   const uint64_t rows = static_cast<uint64_t>(B) * WgradWinCfg::kFrame;
   // overlapping-row view of the haloed NHWC frames: row r = the 32 floats starting at position r (two adjacent pixels × 16 ch)
   cuuint64_t dims[2] = {32, rows - 1};
@@ -963,11 +958,7 @@ void make_wgrad_win_xmap(const float* x_pad, int B, CUtensorMap* tm_x) {
                                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) throw std::runtime_error("cuTensorMapEncodeTiled(overlapping rows) failed: " + cu_error(r));
-}
-
-void make_wgrad_win_tmaps(const float* x_pad, const float* dy_pad, int B, CUtensorMap* tm_x, CUtensorMap* tm_dy) {
-  make_wgrad_win_xmap(x_pad, B, tm_x);
-  *tm_dy = make_tmap_2d(dy_pad, 32, static_cast<uint64_t>(B) * WgradWinCfg::kFrame, 32, kTileM, CU_TENSOR_MAP_SWIZZLE_128B);
+  *tm_dy = make_tmap_2d(dy_pad, 32, rows, 32, kTileM, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 void launch_conv5x5_wgrad_win(const float* dy_pad, const float* x_pad, const float* dysum, float* dw, float* db, int B, ReduceScratch scr,

@@ -31,7 +31,6 @@ void launch_conv5x5_wgrad_mma(const float* dy, const float* x, float* dw, float*
 // Tensor maps of the window weight gradient: tm_x = overlapping-row view of the x frame [B,18,18,16] (row pitch 64 B, row length
 // 128 B, box 64 rows), tm_dy = the dy frame [B,18,18,32] as rows of 32 floats (box 128 rows); both SWIZZLE_128B.
 void make_wgrad_win_tmaps(const float* x_pad, const float* dy_pad, int B, CUtensorMap* tm_x, CUtensorMap* tm_dy);
-void make_wgrad_win_xmap(const float* x_pad, int B, CUtensorMap* tm_x);   // tm_x alone
 // Window formulation for zero-haloed 18×18 frames (cooperative fused layers): dy_pad [B,18,18,32], x_pad [B,18,18,16], dysum [B,32]
 // (per-image Σdy rows, folded into db).  All operands arrive by TMA: no im2col gather.  One cooperative launch: the per-CTA
 // partials are folded after the grid barrier gs.

@@ -60,7 +60,7 @@ Scratch& scratch_entry(const at::Tensor& like) {
     Scratch s;
     s.partials = at::empty({kScratchFloats}, like.options().dtype(at::kFloat));
     s.counter = at::zeros({kCounterWords}, like.options().dtype(at::kInt));   // layout: ops_kernels.h
-    s.wgrad = at::empty({static_cast<int64_t>(at::cuda::getDeviceProperties(dev)->multiProcessorCount) * 512 * 32}, like.options().dtype(at::kFloat));
+    s.wgrad = at::empty({static_cast<int64_t>(at::cuda::getDeviceProperties(dev)->multiProcessorCount) * 400 * 32}, like.options().dtype(at::kFloat));
     it = per_dev.emplace(dev, std::move(s)).first;
   }
   return it->second;
@@ -77,7 +77,7 @@ ReduceScratch scratch(const at::Tensor& like) {
 // Where the layer-2 backward kernel of a batch of B leaves conv2's per-image weight-gradient partials for the layer-1 one.
 float* conv2_wgrad_partials(const at::Tensor& like, int B, const char* what) {
   Scratch& s = scratch_entry(like);
-  TORCH_CHECK(static_cast<int64_t>(B) * 512 * 32 <= s.wgrad.numel(), what, ": batch ", B, " exceeds one CTA per SM");
+  TORCH_CHECK(static_cast<int64_t>(B) * 400 * 32 <= s.wgrad.numel(), what, ": batch ", B, " exceeds one CTA per SM");
   return s.wgrad.data_ptr<float>();
 }
 

@@ -12,8 +12,7 @@
 //                              (+ cross-entropy term and d(loss)/d(logits) when the targets are known)           (ref :25-34,40)
 //   convnet_l2_bwd_kernel<FC, WG>  classifier backward + MaxPool/ReLU/BN backward ──barrier (Σdz, Σdz·x̂)── dy → conv2 data
 //                              gradient on wgmma (warps 4..7), next to it conv2's weight-gradient partial of the image on
-//                              mma.sync (warps 0..3, joined by 4..7 when their wgmma are done; MN-major window; A operand
-//                              loaded by TMA in the barrier's shadow)
+//                              wgmma (warps 0..3; K-major copies of x, written in the barrier's shadow, and of dy)
 //   convnet_l1_bwd_kernel<WG>  MaxPool/ReLU/BN backward ──barrier── conv1 weight gradient (mma.sync) ──barrier── conv1 fold;
 //                              conv2's weight gradient is folded in the shadow of the first barrier, and — on one GPU — the
 //                              threads that write the folded gradients apply the optimizer update (SgdRider / AdamRider)
@@ -281,77 +280,144 @@ convnet_l1_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w, 
 // dynamic smem: dys [784][16] | fold [25 warps][16 co][32 taps]
 constexpr int kL1BwdSmem = (784 * 16 + kL1Warps * 512) * 4;
 
-// conv2's weight gradient in the window formulation (wgrad_win.cuh): dW2ᵀ[(kh, kw, ci)][co] = Σ_P xpad[P + (kh−2)·18 + (kw−2)][ci] ·
-// dypad[P][co] over the 256 positions P from the first interior one, per image, on mma.sync.
-//   * B (dy): the layer-2 backward kernel's own swizzled dy patch (rows = padded positions, zero halo), from row kFirst on.
-//   * A (x): the whole image's overlapping-row view of the layer-1 output frame (pitch 64 B, length 128 B: row r = positions r and
-//     r+1 = two horizontally adjacent taps × 16 channels), loaded ONCE by TMA (six 64-row boxes, 48 KB, 1024-aligned); the 32-row
-//     atom of tap pair (kh, kw/2) for position P is the same buffer read (kh−2)·18 + (kw−2) rows further down.
-// The per-image partial has 512 rows in four groups of four atoms: group kw/2 ∈ {0,1,2} stacks kh = 0..3 (stride 18 rows), group 3
-// holds kh = 4 with kw/2 = 0..2 (stride 2 rows; its fourth atom is unused).  The stand-alone kernel (conv_wgmma.cu) orders the
-// atoms by (kh, kw/2) instead.  The layer-1 backward kernel folds the B partials in the shadow of its first grid barrier.
-struct Conv2WgCfg {
-  static constexpr int kFrame = 18 * 18, kFirst = 2 * 18 + 2, kAtoms = 15;
-  static constexpr int kABoxes = 6, kABytes = kABoxes * 64 * 128;   // A window: rows [0, 384) of the image's overlapping-row view
-  static constexpr int kBBytes = 2 * 128 * 128;                     // stand-alone: both 128-position dy tiles of the image
+// conv2's weight gradient of one image on wgmma: dW2ᵀ[(kh, kw, ci)][co] = Σ_P x[P + 18·kh + kw][ci] · dy[kFirst + P][co] over the
+// 256 positions P ∈ [0, 256) of the zero-haloed 18 × 18 frames from the first interior one (kFirst; x index 0 is tap (0, 0) of
+// position kFirst).  M = (tap, ci), N = co, K = P.  TF32 wgmma wants both operands K-major, i.e. with positions innermost, while
+// the NHWC frames have channels innermost, so both are written transposed into shared memory, in the no-swizzle canonical layout
+// (core matrix = 8 rows × 4 positions, 128 contiguous bytes), already rounded by cvt.rna — the tensor core then reads them exactly.
+//   * A: four residue copies X_r of the x frame.  X_r holds block (cg, q) = x[4q + r + i][8·cg + row] (row 0..7, i 0..3) in
+//     128-byte slot 2q + 9·cg.  Tap (kh, kw) with off = 18·kh + kw reads copy off mod 4 from block q = off / 4; taps kh, kh + 2,
+//     kh + 4, kh + 6 are 36 positions = 18 slots apart, so with M-group g = 2j + cg one descriptor (LBO = 256, SBO = 1152) covers
+//     an M = 64 tile of four kh × 16 channels.  Per kw two tiles: kh ∈ {0, 2, 4, 6} and {1, 3, 5, 7}; kh > 4 are pad rows,
+//     computed from whatever lies there and not stored.  Positions ≥ 324 are written as zeros (they meet dy = 0, and 0 × NaN
+//     would poison real rows).
+//   * B: dyᵀ, block (co-group, K-chunk kc of four positions) at kc·512 + cog·128 (LBO = 512, SBO = 128).
+// 10 tiles × 32 K-steps = 320 wgmma m64n32k8 per image; the partial is [400][32], rows in (kh, kw, ci) order.
+struct Conv2Wg {
+  static constexpr int kFrame = 18 * 18, kFirst = 2 * 18 + 2;
+  static constexpr int kXBlocks = 83;                       // q = 0..82: covers every real tap (off ≤ 76) over 64 K-chunks
+  static constexpr int kXCopy = (2 * (kXBlocks - 1) + 9 + 1) * 128;   // 175 slots, 22,400 B
+  static constexpr int kLbo = 256, kSbo = 1152;
+  // bytes from the first copy up to the end of the farthest pad-row read: copy 3, tile kh ∈ {1, 3, 5, 7} at kw = 1 (off 19, block
+  // 4), M-group 7, K-step 31, second core matrix
+  static constexpr int kXReach = 3 * kXCopy + 2 * 4 * 128 + 7 * kSbo + 31 * 512 + kLbo + 128;
+  static constexpr int kXBytes = (kXReach + 1023) / 1024 * 1024;
+  static constexpr int kDyT = 64 * 512;                     // dyᵀ: 32 co × 256 positions
 };
 
-// TMA of image n's A window into the 1024-aligned buffer `win` (rows past the tensor are zero-filled).  One thread.
-__device__ __forceinline__ void conv2_wgrad_load_window(uint8_t* win, const CUtensorMap* tm_x2, uint64_t* bar, int n) {
-  for (int bx = 0; bx < Conv2WgCfg::kABoxes; ++bx) tma_load_2d(win + bx * 8192, tm_x2, bar, 0, n * Conv2WgCfg::kFrame + 64 * bx);
+// Byte offset of dy[kFirst + p][co] in dyᵀ (p < 256).
+__device__ __forceinline__ uint32_t conv2_dyt_off(int co, int p) {
+  return static_cast<uint32_t>((p >> 2) * 512 + (co >> 3) * 128 + (co & 7) * 16 + (p & 3) * 4);
+}
+__device__ __forceinline__ float tf32_round(float v) { return __uint_as_float(f32_to_tf32(v)); }
+
+// The four residue copies of one image's x frame (frame = its [324][16] floats, read-only in this kernel) by the NT threads of the
+// CTA, in two halves so that the loads can be issued long before the copies' region is free: task (ci, q) loads positions
+// 4q .. 4q + 6 of channel ci (zero past the frame) and writes one 16-byte core-matrix row into each copy.
+template <int NT>
+struct Conv2WgX {
+  static constexpr int kTasks = 16 * Conv2Wg::kXBlocks, kPer = (kTasks + NT - 1) / NT;
+  float v[kPer][7];
+  __device__ __forceinline__ void load(const float* __restrict__ frame, int tid) {
+#pragma unroll
+    for (int u = 0; u < kPer; ++u) {
+      const int i = tid + u * NT, ci = i & 15, q = i >> 4;
+#pragma unroll
+      for (int k = 0; k < 7; ++k) {
+        const int pos = 4 * q + k;
+        v[u][k] = (i < kTasks && pos < Conv2Wg::kFrame) ? __ldg(frame + pos * 16 + ci) : 0.f;   // rounded in store(): no wait here
+      }
+    }
+  }
+  __device__ __forceinline__ void store(uint8_t* xt, int tid) const {
+#pragma unroll
+    for (int u = 0; u < kPer; ++u) {
+      const int i = tid + u * NT, ci = i & 15, q = i >> 4;
+      if (i < kTasks) {
+        uint8_t* dst = xt + (2 * q + 9 * (ci >> 3)) * 128 + (ci & 7) * 16;
+        float t[7];
+#pragma unroll
+        for (int k = 0; k < 7; ++k) t[k] = tf32_round(v[u][k]);
+#pragma unroll
+        for (int r = 0; r < 4; ++r) *reinterpret_cast<float4*>(dst + r * Conv2Wg::kXCopy) = make_float4(t[r], t[r + 1], t[r + 2], t[r + 3]);
+      }
+    }
+  }
+};
+
+// The 64 wgmma of column kw (its two tiles, 32 K-steps each) into a, as one commit group.  A loop, not unrolled code: the kernel
+// runs it once per launch, and every SM would fetch straight-line code from L2 at the same time.
+__device__ __forceinline__ void conv2_wgrad_issue(float (&a)[2][16], uint32_t xt, uint64_t bd, int kw) {
+  uint64_t ad[2];
+#pragma unroll
+  for (int par = 0; par < 2; ++par) {
+    const int off = 18 * par + kw;
+    ad[par] = gmma_desc_kmajor_noswz<Conv2Wg::kLbo, Conv2Wg::kSbo>(xt + (off & 3) * Conv2Wg::kXCopy + (off >> 2) * 256);
+  }
+  wgmma_fence();
+#pragma unroll 4
+  for (int s = 0; s < 32; ++s)
+#pragma unroll
+    for (int par = 0; par < 2; ++par) wgmma_m64n32k8_tf32(a[par], ad[par] + s * (512 >> 4), bd + s * (1024 >> 4), s != 0);
+  wgmma_commit();
+}
+// Rows kh ≤ 4 of column kw's accumulators to the image's partial.
+__device__ __forceinline__ void conv2_wgrad_store(const float (&a)[2][16], float* __restrict__ wpart_n, int kw, int wt) {
+#pragma unroll
+  for (int par = 0; par < 2; ++par)
+#pragma unroll
+    for (int e = 0; e < 16; e += 2) {
+      const int row = wgmma_frag_row(wt, e), g = row >> 3, kh = par + 2 * (g >> 1);
+      if (kh < 5) {
+        const int prow = (kh * 5 + kw) * 16 + 8 * (g & 1) + (row & 7);
+        *reinterpret_cast<float2*>(wpart_n + prow * 32 + wgmma_frag_col(wt, e)) = make_float2(a[par][e], a[par][e + 1]);
+      }
+    }
 }
 
-// The atoms of image n's partial, one warp per atom at a time, each warp taking the next one from the shared counter *next (zero
-// before the first call): warps that join late take fewer.  An atom is computed the same way whichever warp takes it, so the result
-// does not depend on the order.  win / dys are the shared addresses of the A window and of the dy tile whose row dyrow0 is position
-// kFirst; wpart_n = the image's [512][32] partial.
-__device__ __forceinline__ void conv2_wgrad_atoms(uint32_t win, uint32_t dys, int dyrow0, float* wpart_n, int* next, int lane) {
+// The per-image partial from the K-major operands (xt, dyt: shared addresses), issued by one warpgroup (wt = thread index in it):
+// column kw + 1 is in flight while the accumulators of column kw are stored.  The same instructions in the same order wherever
+// it runs, so the stand-alone kernel reproduces the layer-2 backward kernel bit for bit.
+__device__ __forceinline__ void conv2_wgrad_wgmma(uint32_t xt, uint32_t dyt, float* __restrict__ wpart_n, int wt) {
+  const uint64_t bd = gmma_desc_kmajor_noswz<512, 128>(dyt);
+  float acc0[2][16], acc1[2][16];
+  conv2_wgrad_issue(acc0, xt, bd, 0);
 #pragma unroll 1
-  for (;;) {
-    int atom = 0;
-    if (lane == 0) atom = atomicAdd(next, 1);
-    atom = __shfl_sync(0xffffffffu, atom, 0);
-    if (atom >= Conv2WgCfg::kAtoms) break;
-    const int mt = atom >> 2, a = atom & 3;   // atom a of group mt (group 3 has three)
-    const int shift0 = mt < 3 ? (0 - 2) * 18 + 2 * mt - 2 : 2 * 18 - 2;
-    const int stride = mt < 3 ? 18 : 2;
-    float acc[2][4][4];
-#pragma unroll
-    for (int j2 = 0; j2 < 2; ++j2)
-#pragma unroll
-      for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) acc[j2][nt][e] = 0.f;
-    wgrad_win_atom_smem<256, 32>(acc, win, Conv2WgCfg::kFirst + shift0 + a * stride, 0, dys, dyrow0, lane);
-    wgrad_win_atom_store(acc, wpart_n + (mt * 128 + a * 32) * 32, lane);
+  for (int kw = 1; kw < 5; kw += 2) {
+    conv2_wgrad_issue(acc1, xt, bd, kw);
+    wgmma_wait<1>();
+    conv2_wgrad_store(acc0, wpart_n, kw - 1, wt);
+    conv2_wgrad_issue(acc0, xt, bd, kw + 1);
+    wgmma_wait<1>();
+    conv2_wgrad_store(acc1, wpart_n, kw, wt);
   }
+  wgmma_wait<0>();
+  conv2_wgrad_store(acc0, wpart_n, 4, wt);
 }
 
-// The per-image partials from given dy / x frames (the layer-1 backward binding's stand-alone form): one CTA per image, one warp
-// per atom; both operands by TMA (dy: the 256 positions from kFirst, two 128-row boxes).
-constexpr int kConv2WgThreads = Conv2WgCfg::kAtoms * 32;
-constexpr size_t kConv2WgSmem = 1024 + Conv2WgCfg::kABytes + Conv2WgCfg::kBBytes;
-__global__ void __launch_bounds__(kConv2WgThreads, 1)
-conv2_wgrad_partials_kernel(const __grid_constant__ CUtensorMap tm_x2, const __grid_constant__ CUtensorMap tm_dy2, float* __restrict__ wpart) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* win = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sd = win + Conv2WgCfg::kABytes;
-  __shared__ uint64_t ld_full;
-  __shared__ int next_atom;
-  const int n = blockIdx.x;
-  if (threadIdx.x == 0) {
-    next_atom = 0;
-    mbar_init(&ld_full, 1);
-    fence_mbar_init();
-    mbar_arrive_expect_tx(&ld_full, Conv2WgCfg::kABytes + Conv2WgCfg::kBBytes);
-    conv2_wgrad_load_window(win, &tm_x2, &ld_full, n);
-    const int first = n * Conv2WgCfg::kFrame + Conv2WgCfg::kFirst;
-    tma_load_2d(sd, &tm_dy2, &ld_full, 0, first);
-    tma_load_2d(sd + 128 * 128, &tm_dy2, &ld_full, 0, first + 128);
+// The per-image partials from given dy / x frames (the layer-1 backward binding's stand-alone form): one CTA = one warpgroup per
+// image writes the operands from the frames and runs conv2_wgrad_wgmma.
+constexpr size_t kConv2WgSmem = Conv2Wg::kXBytes + Conv2Wg::kDyT;
+__global__ void __launch_bounds__(128, 1)
+conv2_wgrad_partials_kernel(const float* __restrict__ dy2_pad, const float* __restrict__ x2_pad, float* __restrict__ wpart) {
+  extern __shared__ __align__(1024) uint8_t smem_wg[];
+  uint8_t* dyt = smem_wg + Conv2Wg::kXBytes;
+  const int n = blockIdx.x, tid = threadIdx.x;
+  {
+    Conv2WgX<128> xr;
+    xr.load(x2_pad + static_cast<size_t>(n) * Conv2Wg::kFrame * 16, tid);
+    xr.store(smem_wg, tid);
   }
+  const float* dyf = dy2_pad + (static_cast<size_t>(n) * Conv2Wg::kFrame + Conv2Wg::kFirst) * 32;
+  for (int i = tid; i < 32 * 64; i += 128) {   // task (co, kc): positions 4kc .. 4kc + 3 of channel co, one 16-byte row
+    const int co = i & 31, kc = i >> 5;
+    const float* src = dyf + 4 * kc * 32 + co;
+    *reinterpret_cast<float4*>(dyt + conv2_dyt_off(co, 4 * kc)) =
+        make_float4(tf32_round(__ldg(src)), tf32_round(__ldg(src + 32)), tf32_round(__ldg(src + 64)), tf32_round(__ldg(src + 96)));
+  }
+  fence_proxy_async_smem();
   __syncthreads();
-  mbar_wait(&ld_full, 0);
-  conv2_wgrad_atoms(smem_u32(win), smem_u32(sd), 0, wpart + static_cast<size_t>(n) * 512 * 32, &next_atom, threadIdx.x & 31);
+  conv2_wgrad_wgmma(smem_u32(smem_wg), smem_u32(dyt), wpart + static_cast<size_t>(n) * 400 * 32, tid);
 }
 
 // One SGD update (the arithmetic of sgd_multi_kernel, ops_simt.cu) of element *p with gradient g.
@@ -414,7 +480,7 @@ __global__ void __launch_bounds__(kL1Threads, 1)
 convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y, const float* __restrict__ x, const float* __restrict__ saved,
                       const float* __restrict__ gamma, const float* __restrict__ beta, float* dgamma, float* dbeta, float* dw, float* db,
                       float* partials, float* partials_w, GridSync gs,
-                      // WG only: conv2's weight gradient, folded from the per-image partials [B][512][32] and Σdy rows [B][32]
+                      // WG only: conv2's weight gradient, folded from the per-image partials [B][400][32] and Σdy rows [B][32]
                       const float* __restrict__ wpart, const float* __restrict__ dysum2, float* dw2, float* db2, const __grid_constant__ Rider sr) {
   constexpr bool kClip = std::is_same_v<Rider, ClipRider<SgdRider>> || std::is_same_v<Rider, ClipRider<AdamRider>>;
   constexpr bool kAdam = std::is_same_v<Rider, AdamRider> || std::is_same_v<Rider, ClipRider<AdamRider>>;
@@ -526,11 +592,12 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   if constexpr (WG) {
     // in the barrier's shadow: conv2's weight gradient, complete before this kernel started (the layer-2 backward kernel wrote the
     // per-image partials), and its optimizer step — nothing in this kernel reads conv2's parameters.  CTA n folds outputs n, n + B,
-    // … of the 400 (tap, ci) rows × 32 co (+ row 400: the bias, from the per-image Σdy rows) over the B per-image partials — warp =
+    // … of the 400 (tap, ci) rows × 32 co (+ row 400: the bias, from the per-image Σdy rows) over the B per-image partials [400][32],
+    // whose row i is that output row — warp =
     // one of 25 partial classes, lane = co, classes combined through smem in a fixed order, up to five outputs per round so that
     // ~20 L2 loads per thread are in flight
     float* s_f = fold;   // [5][25][32]
-    constexpr size_t kStride = 512 * 32;
+    constexpr size_t kStride = 400 * 32;
     for (int base = n; base < 401; base += 5 * B) {
       float acc[5];
       const float* src[5];
@@ -539,10 +606,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
       for (int u = 0; u < 5; ++u) {
         const int i = base + u * B;
         if (i < 400) {
-          const int tap = i >> 4, ci = i & 15, kh = tap / 5, kw = tap - kh * 5;
-          // accumulator row of (kh, kw, ci): tiles 0-2 = kw/2 with kh 0..3 stacked, tile 3 = kh 4 with kw/2 stacked
-          const int mrow = (kh < 4 ? (kw >> 1) * 128 + kh * 32 : 384 + (kw >> 1) * 32) + (kw & 1) * 16 + ci;
-          src[u] = wpart + static_cast<size_t>(mrow) * 32 + lane;
+          src[u] = wpart + static_cast<size_t>(i) * 32 + lane;
           stride[u] = kStride;
         } else {
           src[u] = i == 400 ? dysum2 + lane : nullptr;   // row 400: the bias gradient from the per-image Σdy rows
@@ -1351,20 +1415,22 @@ struct L2BwdSmem {
   // FC (the classifier's backward rides along): fc weights [16][1568] | dlogits [B ≤ 160][16] | pooled slice [B ≤ 160][16]
   static constexpr int kFcW = 16 * 1568 * 4, kFcDl = 160 * 16 * 4, kFcP = 160 * 16 * 4;
   static constexpr int kTotalFc = kTotal + kFcW + kFcDl + kFcP;
-  // WG: conv2's A window (Conv2WgCfg) at the same 1024-aligned offset as the fc weights — over them once they are dead (FC), or
-  // behind everything else
-  static constexpr int kWin = kPatchAlloc + kB + 4096;
-  static constexpr int kTotalWg = kTotal + Conv2WgCfg::kABytes;
-  static_assert(kWin % 1024 == 0 && Conv2WgCfg::kABytes <= kFcW, "conv2 weight-gradient window placement");
+  // WG: conv2's weight-gradient operands (Conv2Wg).  The x copies are written in the grid barrier's shadow over the fc weights, dead
+  // by then (FC), and dyᵀ after the barrier over the end of the fc weights and the dlogits / pooled slices, which the classifier's
+  // weight gradient in the shadow was the last to read.  The same offsets without FC.
+  static constexpr int kXT = kPatchAlloc + kB + 4096;
+  static constexpr int kDyT = kXT + Conv2Wg::kXBytes;
+  static constexpr int kTotalWg = 1024 + kDyT + Conv2Wg::kDyT;
+  static_assert(Conv2Wg::kXBytes <= kFcW && kTotalWg <= 227 * 1024, "conv2 weight-gradient operand placement");
 };
 
 // FC: the classifier's backward rides along.  The gradient of the pooled activations is not read from `dout` but computed
 // on the fly, d(out)[n][k] = Σ_j dlogits[n][j] · Wfc[j][k] (fc weights staged in smem once per CTA); the classifier's weight
 // gradient dWfc[j][k] = Σ_n dlogits[n][j] · out[n][k] is produced in 16-column slices, one slice per CTA (all images, fixed
 // order: deterministic, no partials), the bias gradient by the CTA that owns "slice 98".  One kernel less per step.
-// WG: conv2's weight gradient partial of the image (Conv2WgCfg) is computed here, by warps 0..3 while warps 4..7 run the data
-// gradient's asynchronous wgmma (and warps 4..7 once that is done): its B operand is the dy patch this kernel builds anyway, its A operand (the layer-1 output frame)
-// arrives by TMA in the shadow of the grid barrier.  The global dy frame is then not written: nothing reads it.
+// WG: conv2's weight-gradient partial of the image (Conv2Wg) is computed here on wgmma, issued by warpgroup 0 while warpgroup 1 issues
+// the data gradient's: the x copies are written from conv2's input frame x2 in the shadow of the grid barrier, dyᵀ from the
+// registers that write the dy patch.  The global dy frame is then not written: nothing reads it.
 template <bool FC, bool WG>
 __global__ void __launch_bounds__(kL2Threads, 1)
 convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float* __restrict__ y /*[B,14,14,32]*/,
@@ -1377,8 +1443,7 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
                       const float* __restrict__ pooled /*[B,1568] = forward's out*/, float* dfcw /*[ncls,1568]*/, float* dfcb /*[ncls]*/,
                       int ncls, const float* __restrict__ loss_parts /*[B] or null*/, float* loss_out,
                       // WG only
-                      const __grid_constant__ CUtensorMap tm_x2 /*overlapping-row view of the layer-1 output frame*/,
-                      float* __restrict__ wpart /*[B][512][32]*/) {
+                      const float* __restrict__ x2 /*[B,18,18,16] = conv2's input frame*/, float* __restrict__ wpart /*[B][400][32]*/) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sa = smem;                                  // dy patch, written by the CTA in the TMA/wgmma SWIZZLE_128B layout
@@ -1394,26 +1459,16 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
   float* s_fcw = misc + 1024;                                   // FC: [ncls][1568]
   float* s_dl = s_fcw + L2BwdSmem::kFcW / 4;                    // FC: [B][16] (columns >= ncls zero)
   float* s_pool = s_dl + L2BwdSmem::kFcDl / 4;                  // FC: [B][16] slice of the pooled activations
-  uint8_t* s_win = smem + L2BwdSmem::kWin;                      // WG: conv2's A window
-  __shared__ uint64_t win_full;
-  __shared__ int next_atom;
+  uint8_t* s_xt = smem + L2BwdSmem::kXT;                        // WG: conv2's x copies
+  uint8_t* s_dyt = smem + L2BwdSmem::kDyT;                      // WG: conv2's dyᵀ
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = blockIdx.x, B = gridDim.x;
 
   GridBar bar(gs);
   TRACE_INIT();
   trace(3, 0);
-  if constexpr (WG) {
-    if (tid == 0) {
-      next_atom = 0;
-      tma_prefetch_desc(&tm_x2);
-      mbar_init(&win_full, 1);
-      fence_mbar_init();
-      if constexpr (!FC) {   // a region of its own: load now
-        mbar_arrive_expect_tx(&win_full, Conv2WgCfg::kABytes);
-        conv2_wgrad_load_window(s_win, &tm_x2, &win_full, n);
-      }
-    }
-  }
+  // WG: the loads of conv2's x copies, written in the grid barrier's shadow (the forward kernel wrote x2)
+  Conv2WgX<kL2Threads> xr;
+  if constexpr (WG) xr.load(x2 + static_cast<size_t>(n) * Conv2Wg::kFrame * 16, tid);
   if constexpr (FC) {
     // stage the classifier weights (cp.async, no registers, lands while the dgrad weights are built), every image's dlogits and this
     // CTA's first 16-column slice of the pooled activations (loads batched in registers: one L2 latency, not one per element)
@@ -1511,15 +1566,6 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
   s_part[g * 64 + c] = s1;
   s_part[g * 64 + 32 + c] = s2;
   __syncthreads();
-  if constexpr (WG && FC) {
-    // the classifier weights are dead: the window goes over them (their cp.async writes and generic reads are ordered before the
-    // TMA writes by the proxy fence) and lands in the shadow of the grid barrier
-    if (tid == 0) {
-      fence_proxy_async_smem();
-      mbar_arrive_expect_tx(&win_full, Conv2WgCfg::kABytes);
-      conv2_wgrad_load_window(s_win, &tm_x2, &win_full, n);
-    }
-  }
   if (tid < 64) {
     float s = 0.f;
 #pragma unroll
@@ -1529,6 +1575,8 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
   trace(3, 2);
   bar.arrive(gs);
   // ---- in the shadow of the grid barrier: work that no other CTA waits for ----
+  // conv2's x copies, over the classifier weights (dead since the __syncthreads above)
+  if constexpr (WG) xr.store(s_xt, tid);
   // zero halo of the global dy frame (the weight gradient sums over all 324 positions)
   if constexpr (!WG) {
     for (int i = tid; i < 324 * 8; i += kL2Threads) {
@@ -1608,12 +1656,21 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
           const float v = sc * ((d == arg[k] ? dzv[k] : 0.f) - m1 - xh * m2);
           const int P = (oh + 2) * kPW + ow + 2;
           if constexpr (!WG) dy[(static_cast<size_t>(n) * 324 + P) * 32 + c] = v;  // frame for the weight-gradient kernel (TMA)
+          else *reinterpret_cast<float*>(s_dyt + conv2_dyt_off(c, P - Conv2Wg::kFirst)) = tf32_round(v);   // conv2's dyᵀ
           *reinterpret_cast<float*>(sa + sw128_off(P, c >> 2) + (c & 3) * 4) = v;   // same frame in smem for the data-gradient MMAs
           dsum += v;
         }
       }
     }
     s_part[g * 64 + c] = dsum;
+    if constexpr (WG) {
+      // the 60 halo positions of dyᵀ's window: P = 18·pr + 16 .. 18·pr + 19 for pr = 2..14, then 286..293
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const int h = g + 8 * k;
+        if (h < 60) *reinterpret_cast<float*>(s_dyt + conv2_dyt_off(c, (h < 52 ? 18 * (2 + (h >> 2)) + 16 + (h & 3) : 286 + h - 52) - Conv2Wg::kFirst)) = 0.f;
+      }
+    }
   }
   fence_proxy_async_smem();
   __syncthreads();
@@ -1624,8 +1681,16 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
     dysum[static_cast<size_t>(n) * 32 + tid] = s;
   }
   trace(3, 5);
-  // ---- conv2 data gradient: 400 wgmma m64n16k8 by the warpgroup of warps 4..7, accumulators straight to the dx frame -------
-  if (warpgroup_index() == 1) {
+  // ---- conv2 data gradient: 400 wgmma m64n16k8 by the warpgroup of warps 4..7, accumulators straight to the dx frame; next to
+  // it (WG) conv2's weight-gradient partial, 320 wgmma m64n32k8 by warps 0..3 ---------------------------------------------------
+  const int wg = warpgroup_index();
+  if constexpr (WG) {
+    if (wg == 0) {
+      conv2_wgrad_wgmma(smem_u32(s_xt), smem_u32(s_dyt), wpart + static_cast<size_t>(n) * 400 * 32, tid);
+      trace(3, 7);
+    }
+  }
+  if (wg == 1) {
     const int wt = tid - 128;
     const uint64_t ad0 = gmma_desc_kmajor<128>(smem_u32(sa)), bd0 = gmma_desc_kmajor<128>(smem_u32(sb));
 #pragma unroll 1
@@ -1661,13 +1726,6 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
         }
       }
     }
-  }
-  if constexpr (WG) {
-    // ---- conv2 weight-gradient partial of this image, one 32-row atom per warp at a time: warps 0..3 start next to the wgmma,
-    // warps 4..7 join when their data gradient is done ---------------------------------------------------------------------
-    mbar_wait(&win_full, 0);
-    conv2_wgrad_atoms(smem_u32(s_win), smem_u32(sa), Conv2WgCfg::kFirst, wpart + static_cast<size_t>(n) * 512 * 32, &next_atom, lane);
-    trace(3, 7);
   }
   __syncthreads();
   bar.finish(gs);
@@ -1724,10 +1782,8 @@ void launch_convnet_l1_bwd(const float* dp, const float* y, const float* x, cons
 }
 
 void launch_conv2_wgrad_partials(const float* dy2_pad, const float* x2_pad, int B, float* wpart, cudaStream_t st) {
-  CUtensorMap tm_x, tm_dy;
-  make_wgrad_win_tmaps(x2_pad, dy2_pad, B, &tm_x, &tm_dy);
   opt_in_smem(conv2_wgrad_partials_kernel, kConv2WgSmem);
-  conv2_wgrad_partials_kernel<<<B, kConv2WgThreads, kConv2WgSmem, st>>>(tm_x, tm_dy, wpart);
+  conv2_wgrad_partials_kernel<<<B, 128, kConv2WgSmem, st>>>(dy2_pad, x2_pad, wpart);
   check_launch("conv2_wgrad_partials");
 }
 
@@ -1770,13 +1826,11 @@ void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const 
 void launch_convnet_l2_bwd(const float* dout, const float* y, const float* saved, const float* gamma, const float* beta, const float* w,
                            float* dgamma, float* dbeta, float* dy, float* dx, float* dysum, int B, float* partials, GridSync gs,
                            cudaStream_t st, const float* x2, float* wpart) {
-  CUtensorMap tm_x2{};
-  if (x2 != nullptr) make_wgrad_win_xmap(x2, B, &tm_x2);
   auto kernel = x2 != nullptr ? convnet_l2_bwd_kernel<false, true> : convnet_l2_bwd_kernel<false, false>;
   launch_cooperative(kernel, B, kL2Threads, static_cast<size_t>(x2 != nullptr ? L2BwdSmem::kTotalWg : L2BwdSmem::kTotal), st, "convnet_l2_bwd", dout,
                      y, saved, gamma, beta, w, dgamma, dbeta, dy, dx, dysum, partials, gs, static_cast<const float*>(nullptr),
                      static_cast<const float*>(nullptr), static_cast<const float*>(nullptr), static_cast<float*>(nullptr), static_cast<float*>(nullptr), 0,
-                     static_cast<const float*>(nullptr), static_cast<float*>(nullptr), tm_x2, wpart);
+                     static_cast<const float*>(nullptr), static_cast<float*>(nullptr), x2, wpart);
 }
 
 void launch_convnet_l2_bwd_fc(const float* dlogits, const float* fcw, const float* pooled, float* dfcw, float* dfcb, int ncls, const float* y,
@@ -1785,11 +1839,10 @@ void launch_convnet_l2_bwd_fc(const float* dlogits, const float* fcw, const floa
                               const float* x2, float* wpart) {
   if (ncls < 1 || ncls > 16) throw std::invalid_argument("convnet_l2_bwd_fc: 1..16 classes");
   if (B > 160) throw std::invalid_argument("convnet_l2_bwd_fc: batch too large for the staged dlogits");
-  CUtensorMap tm_x2{};
-  if (x2 != nullptr) make_wgrad_win_xmap(x2, B, &tm_x2);
   auto kernel = x2 != nullptr ? convnet_l2_bwd_kernel<true, true> : convnet_l2_bwd_kernel<true, false>;
-  launch_cooperative(kernel, B, kL2Threads, static_cast<size_t>(L2BwdSmem::kTotalFc), st, "convnet_l2_bwd_fc", static_cast<const float*>(nullptr), y, saved,
-                     gamma, beta, w, dgamma, dbeta, dy, dx, dysum, partials, gs, dlogits, fcw, pooled, dfcw, dfcb, ncls, loss_parts, loss_out, tm_x2,
+  const int smem = x2 != nullptr ? std::max(L2BwdSmem::kTotalFc, L2BwdSmem::kTotalWg) : L2BwdSmem::kTotalFc;
+  launch_cooperative(kernel, B, kL2Threads, static_cast<size_t>(smem), st, "convnet_l2_bwd_fc", static_cast<const float*>(nullptr), y, saved,
+                     gamma, beta, w, dgamma, dbeta, dy, dx, dysum, partials, gs, dlogits, fcw, pooled, dfcw, dfcb, ncls, loss_parts, loss_out, x2,
                      wpart);
 }
 

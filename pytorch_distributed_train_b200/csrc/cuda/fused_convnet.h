@@ -61,7 +61,7 @@ struct ClipRider : Base {
   float* part = nullptr;       // [B] per-CTA partials
 };
 
-// conv2's weight gradient per image (wpart [B][512][32], the layout of launch_convnet_l2_bwd's WG form) from given frames:
+// conv2's weight gradient per image (wpart [B][400][32], rows (kh, kw, ci), the layout of launch_convnet_l2_bwd's WG form) from given frames:
 // dy2_pad [B,18,18,32] (zero halo), x2_pad [B,18,18,16].  One CTA per image, not cooperative.
 void launch_conv2_wgrad_partials(const float* dy2_pad, const float* x2_pad, int B, float* wpart, cudaStream_t st);
 // Layer-1 backward that also folds conv2's weight gradient: the per-image partials wpart and Σdy rows dysum2 [B,32] → dw2
@@ -96,7 +96,7 @@ void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const 
                         FusedCe ce = FusedCe{});
 // dout [B,32,7,7] → dgamma/dbeta [32], dy [B,18,18,32] frame with zero halo (gradient at the conv2 output), dx [B,18,18,16] frame
 // (data gradient, interior written), dysum [B,32] (per-image Σdy: the conv2 bias gradient is the sum of its rows).
-// x2 != nullptr (conv2's input frame [B,18,18,16]): conv2's weight-gradient partials per image go to wpart [B][512][32] instead,
+// x2 != nullptr (conv2's input frame [B,18,18,16]): conv2's weight-gradient partials per image go to wpart [B][400][32] instead,
 // and dy is not written.
 void launch_convnet_l2_bwd(const float* dout, const float* y, const float* saved, const float* gamma, const float* beta, const float* w,
                            float* dgamma, float* dbeta, float* dy, float* dx, float* dysum, int B, float* partials, GridSync gs, cudaStream_t st,

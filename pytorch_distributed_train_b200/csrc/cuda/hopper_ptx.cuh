@@ -144,6 +144,15 @@ __device__ __forceinline__ uint64_t gmma_desc_kmajor(uint32_t smem_addr) {
   return d;
 }
 
+// K-major descriptor without swizzle (layout 0, "interleave"): a core matrix of 8 rows × 16 bytes is 128 contiguous bytes (row i
+// at byte 16·i); LBO = byte step between core matrices along K, SBO = byte step between 8-row groups along M / N.  16-byte
+// alignment suffices; advanced like the swizzled one, by adds of (bytes >> 4).
+template <int LBO, int SBO>
+__device__ __forceinline__ uint64_t gmma_desc_kmajor_noswz(uint32_t smem_addr) {
+  static_assert(LBO % 16 == 0 && SBO % 16 == 0 && LBO < (1 << 18) && SBO < (1 << 18), "gmma_desc_kmajor_noswz: 16-byte multiples below 256 KB");
+  return static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4) | static_cast<uint64_t>(LBO >> 4) << 16 | static_cast<uint64_t>(SBO >> 4) << 32;
+}
+
 __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3) {
   asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(
                    smem_u32(smem_dst)),

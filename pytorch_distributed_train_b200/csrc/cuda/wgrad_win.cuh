@@ -1,20 +1,13 @@
-// conv2 (16→32, 5×5) weight gradient of one image in the "window" formulation, shared by the stand-alone kernel
-// (conv_wgmma.cu) and the layer-2 backward kernel that carries it along (fused_convnet.cu):
+// conv2 (16→32, 5×5) weight gradient in the "window" formulation on warp-level mma.sync, for the per-op kernels of
+// conv_wgmma.cu:
 //   dWᵀ[(kh, kw, ci)][co] = Σ_P xpad[P + (kh−2)·18 + (kw−2)][ci] · dypad[P][co]
-// over the 256 padded positions P from the first interior one.  Two horizontally adjacent taps of one position are 32
+// over the padded positions P from the first interior one.  Two horizontally adjacent taps of one position are 32
 // contiguous floats of the NHWC frame, so a 32-row "atom" of the M dimension (tap pair × 16 channels) is one row of the
 // overlapping-row view of the frame (row r = positions r, r+1).  Both operands have the reduction dimension (positions)
-// outermost — MN-major — which TF32 wgmma does not accept, so this is warp-level mma.sync m16n8k8 reading the swizzled
-// tiles directly.  The im2col weight gradient (conv_wgmma.cu) uses the same per-warp step.
-// Trade-off: on the previous (Blackwell) generation these MMAs ran asynchronously from one extra warp while the layer-1
-// SIMT warps worked; here they are synchronous warp-level MMAs.  In the fused step they run in the layer-2 backward kernel, on
-// the warpgroup that has nothing to do while the other one waits for its asynchronous wgmma data gradient (dy is already in
-// that kernel's shared memory), and the layer-1 backward kernel folds the per-image partials in the shadow of its first grid
-// barrier.  Until then they ran inside the layer-1 backward kernel, on 15 of its warps just before its second grid barrier:
-// about 13 µs of the critical path of the ~99 µs replayed step at batch 100 (H100 SXM, 700 W limit; tools/fused_trace.py).  On the
-// idle warps of the layer-2 kernel they cost that kernel ~11 µs and save the layer-1 kernel ~15 µs; the step is ~8 µs shorter
-// (H100 80GB HBM3, 400 W limit).
-// Feeding wgmma instead would need a K-major (transposed) copy of both operands in shared memory.
+// outermost — MN-major — which TF32 wgmma does not accept, so this is mma.sync m16n8k8 reading the swizzled TMA tiles
+// directly.  The im2col weight gradient (conv_wgmma.cu) uses the same per-warp step.
+// The fused step does not use it: its layer-2 backward kernel writes K-major (transposed, TF32-rounded) copies of both operands
+// into shared memory and issues wgmma (conv2_wgrad_wgmma, fused_convnet.cu).
 #pragma once
 #include <cstdint>
 
@@ -62,44 +55,6 @@ __device__ __forceinline__ void wgrad_win_atom(float (&acc)[2][4][4], const floa
     }
     const uint32_t a0[4] = {f32_to_tf32(xa[c0]), f32_to_tf32(xa[c1]), f32_to_tf32(xb[c0 ^ 16]), f32_to_tf32(xb[c1 ^ 16])};
     const uint32_t a1[4] = {f32_to_tf32(xa[c2]), f32_to_tf32(xa[c3]), f32_to_tf32(xb[c2 ^ 16]), f32_to_tf32(xb[c3 ^ 16])};
-#pragma unroll
-    for (int nt = 0; nt < 4; ++nt) {
-      mma_m16n8k8_tf32(acc[0][nt], a0, b[nt][0], b[nt][1]);
-      mma_m16n8k8_tf32(acc[1][nt], a1, b[nt][0], b[nt][1]);
-    }
-  }
-}
-
-__device__ __forceinline__ float lds_f32(uint32_t addr) {
-  float v;
-  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
-  return v;
-}
-
-// wgrad_win_atom on tiles given by their shared-memory addresses (xs, dys: byte addresses, 1024-aligned tiles): the operand
-// loads are ld.shared whatever pointer arithmetic placed the tiles.  Same loads, roundings and MMAs in the same order.
-template <int KPOS = 256, int XPITCH = 32, int UNROLL = 2>
-__device__ __forceinline__ void wgrad_win_atom_smem(float (&acc)[2][4][4], uint32_t xs, int xrow0, int xcol0, uint32_t dys, int dyrow0,
-                                                    int lane) {
-  const int g = lane >> 2, t4 = lane & 3;
-  const int kx = ((xrow0 + t4) & 7) << 2, kd = ((dyrow0 + t4) & 7) << 2;
-  const int c0 = (xcol0 + g) ^ kx, c1 = (xcol0 + g + 8) ^ kx, c2 = (xcol0 + g + 16) ^ kx, c3 = (xcol0 + g + 24) ^ kx;
-  uint32_t xa = xs + static_cast<uint32_t>((xrow0 + t4) * XPITCH) * 4u;
-  uint32_t da = dys + static_cast<uint32_t>((dyrow0 + t4) * 32) * 4u;
-#pragma unroll UNROLL
-  for (int p0 = 0; p0 < KPOS; p0 += 8, xa += 8 * XPITCH * 4, da += 8 * 32 * 4) {
-    const uint32_t xb = xa + 4 * XPITCH * 4;
-    const uint32_t db = da + 4 * 32 * 4;
-    uint32_t b[4][2];
-#pragma unroll
-    for (int nt = 0; nt < 4; ++nt) {
-      b[nt][0] = f32_to_tf32(lds_f32(da + 4u * ((8 * nt + g) ^ kd)));
-      b[nt][1] = f32_to_tf32(lds_f32(db + 4u * ((8 * nt + g) ^ kd ^ 16)));
-    }
-    const uint32_t a0[4] = {f32_to_tf32(lds_f32(xa + 4u * c0)), f32_to_tf32(lds_f32(xa + 4u * c1)), f32_to_tf32(lds_f32(xb + 4u * (c0 ^ 16))),
-                            f32_to_tf32(lds_f32(xb + 4u * (c1 ^ 16)))};
-    const uint32_t a1[4] = {f32_to_tf32(lds_f32(xa + 4u * c2)), f32_to_tf32(lds_f32(xa + 4u * c3)), f32_to_tf32(lds_f32(xb + 4u * (c2 ^ 16))),
-                            f32_to_tf32(lds_f32(xb + 4u * (c3 ^ 16)))};
 #pragma unroll
     for (int nt = 0; nt < 4; ++nt) {
       mma_m16n8k8_tf32(acc[0][nt], a0, b[nt][0], b[nt][1]);
