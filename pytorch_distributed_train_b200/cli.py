@@ -9,11 +9,12 @@ Extra flags cover what the reference hard-codes: ``--init-method`` (its LAN addr
 ``tcp://10.9.1.2:34567`` only works on the author's network, ref: ddp_example.py:110; we default
 to loopback with a free port), ``--data synthetic|mnist``, ``--model``, ``--comm fused|nccl``, ``--algo``,
 ``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw), ``--lr``,
-``--momentum``, ``--weight-decay``, ``--clip-grad-norm``, ``--checkpoint`` / ``--resume``.
+``--momentum``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--checkpoint`` / ``--resume``.
 """
 from __future__ import annotations
 
 import argparse
+import contextlib
 import socket
 import sys
 from datetime import datetime
@@ -50,7 +51,10 @@ def build_parser() -> argparse.ArgumentParser:
                    help="weight decay (default: 0 for SGD and Adam, 1e-2 for AdamW, torch's defaults)")
     p.add_argument("--clip-grad-norm", default=None, type=float, metavar="MAX",
                    help="clip the global gradient norm (L2) to MAX before every optimizer step (default: off)")
-    p.add_argument("--steps", default=0, type=int, help="stop each epoch after this many steps (0 = full epoch)")
+    p.add_argument("--accumulation-steps", default=1, type=int, metavar="K",
+                   help="gradient accumulation: K micro-batches of --batch-size images per optimizer step, each backward of loss / K "
+                        "(default 1)")
+    p.add_argument("--steps", default=0, type=int, help="stop each epoch after this many (optimizer) steps (0 = full epoch)")
     p.add_argument("--samples", default=60000, type=int, help="synthetic dataset size")
     p.add_argument("--graph", default=False, action="store_true", help="capture the whole training step in a CUDA graph")
     p.add_argument("--log-interval", default=10, type=int)
@@ -77,6 +81,10 @@ def check_args(p: argparse.ArgumentParser, args) -> None:
         p.error(f"--momentum applies to SGD only; {args.optimizer} takes its moments from its betas")
     if args.clip_grad_norm is not None and not args.clip_grad_norm > 0:
         p.error(f"--clip-grad-norm must be positive (got {args.clip_grad_norm})")
+    if args.accumulation_steps < 1:
+        p.error(f"--accumulation-steps must be at least 1 (got {args.accumulation_steps})")
+    if args.graph and args.gpus >= 2 and args.accumulation_steps > 1:
+        p.error("--graph with --accumulation-steps > 1 runs on one GPU only (-g 1)")
 
 
 def dist_train(gpu: int, args) -> None:
@@ -109,6 +117,7 @@ def dist_train(gpu: int, args) -> None:
     device = torch.device("cuda", gpu) if use_cuda else torch.device("cpu")
     model.to(device)
     batch_size = args.batch_size
+    accum = args.accumulation_steps
     criterion = pdt.nn.CrossEntropyLoss().to(device)
     optimizer = make_optimizer(args, model.parameters())
     model = pdt.DistributedDataParallel(model, device_ids=[gpu] if use_cuda else None)
@@ -119,7 +128,8 @@ def dist_train(gpu: int, args) -> None:
         n = args.samples if args.model == "convnet" else min(args.samples, 4096)
         train_dataset = pdata.SyntheticMNIST(n, seed=0, num_classes=10 if args.model == "convnet" else 1000, image_shape=shape)
     train_sampler = pdt.DistributedSampler(train_dataset, num_replicas=args.world_size, rank=rank)
-    train_loader = pdt.DataLoader(dataset=train_dataset, batch_size=batch_size, shuffle=False, num_workers=0,
+    # one loader batch = one optimizer step: `accum` micro-batches of batch_size images
+    train_loader = pdt.DataLoader(dataset=train_dataset, batch_size=accum * batch_size, shuffle=False, num_workers=0,
                                   pin_memory=use_cuda, sampler=train_sampler)
 
     step_fn = None
@@ -127,8 +137,8 @@ def dist_train(gpu: int, args) -> None:
         from pytorch_distributed_train_b200.engine import GraphedTrainStep
 
         step_fn = GraphedTrainStep(model, criterion, optimizer, example_inputs=(
-            torch.zeros((batch_size,) + shape, device=device), torch.zeros(batch_size, dtype=torch.int64, device=device)),
-            max_grad_norm=args.clip_grad_norm)
+            torch.zeros((accum * batch_size,) + shape, device=device), torch.zeros(accum * batch_size, dtype=torch.int64, device=device)),
+            max_grad_norm=args.clip_grad_norm, accumulation_steps=accum)
 
     first_epoch = 0
     if args.resume:
@@ -147,7 +157,7 @@ def dist_train(gpu: int, args) -> None:
         for i, (images, labels) in enumerate(train_loader):
             if args.steps and i >= args.steps:
                 break
-            graphed = step_fn is not None and images.shape[0] == batch_size
+            graphed = step_fn is not None and images.shape[0] == accum * batch_size
             if graphed:
                 # the (pinned) host batch goes straight into the captured step's input buffers; the copy overlaps the previous step
                 step_fn(images, labels)
@@ -155,10 +165,20 @@ def dist_train(gpu: int, args) -> None:
             else:
                 images = images.to(device, non_blocking=True)
                 labels = labels.to(device, non_blocking=True)
-                outputs = model(images)
-                loss = criterion(outputs, labels)
                 optimizer.zero_grad()
-                loss.backward()
+                if accum == 1:
+                    outputs = model(images)
+                    loss = criterion(outputs, labels)
+                    loss.backward()
+                else:
+                    # micro-batches of batch_size rows (a short last batch gives fewer); the gradient reduction runs on the last one
+                    micro = list(zip(images.split(batch_size), labels.split(batch_size)))
+                    loss = 0.0
+                    for j, (x, t) in enumerate(micro):
+                        with model.no_sync() if j + 1 < len(micro) else contextlib.nullcontext():
+                            part = criterion(model(x), t) / len(micro)
+                            part.backward()
+                        loss = loss + part.detach()
                 if args.clip_grad_norm is not None:
                     pdt.nn.utils.clip_grad_norm_(model.parameters(), args.clip_grad_norm)
                 optimizer.step()

@@ -258,7 +258,7 @@ void register_cuda_bindings(py::module_& m) {
   m.def("convnet_l1_bwd_wgrad", [](const at::Tensor& dp, const at::Tensor& y, const at::Tensor& x, const at::Tensor& saved,
                                    c10::optional<at::Tensor> gamma, c10::optional<at::Tensor> beta, at::Tensor dgamma, at::Tensor dbeta, at::Tensor dw,
                                    c10::optional<at::Tensor> db, c10::optional<at::Tensor> dy2_pad, c10::optional<at::Tensor> x2_pad,
-                                   const at::Tensor& dysum2, at::Tensor dw2, c10::optional<at::Tensor> db2, py::object sgd) {
+                                   const at::Tensor& dysum2, at::Tensor dw2, c10::optional<at::Tensor> db2, py::object sgd, bool accumulate) {
     chk(dp, "dp"); chk(y, "y"); chk(x, "x"); chk(saved, "saved"); chk(dgamma, "dgamma"); chk(dbeta, "dbeta"); chk(dw, "dw");
     chk(dysum2, "dysum2"); chk(dw2, "dw2");
     c10::cuda::CUDAGuard g(x.device());
@@ -284,6 +284,8 @@ void register_cuda_bindings(py::module_& m) {
     // or the Adam rider: ("adam", params[10], prev_grads[4], exp_avgs[10], exp_avg_sqs[10], steps[10], lr, lr_tensor, beta1, beta2,
     // eps, weight_decay, decoupled, maximize), steps being fp32 scalars on the device.  Either tuple may end in a clip entry
     // (max_norm, norm_type 2 or inf, norm_out): gradient-norm clipping in front of the update (ClipRider); norm_out receives the norm.
+    // accumulate: gradient accumulation — dgamma, dbeta, dw, db, dw2, db2 are added to (they hold the earlier micro-batches' sum), and
+    // the rider updates with the accumulated gradients.
     static const int64_t want[10] = {400, 16, 16, 16, 12800, 32, -1, -1, 32, 32};
     ReduceScratch scr = scratch(x);
     const size_t l1_floats = static_cast<size_t>(B) * (64 + 512);
@@ -293,7 +295,7 @@ void register_cuda_bindings(py::module_& m) {
       launch_convnet_l1_bwd_wgrad(dp.data_ptr<float>(), y.data_ptr<float>(), x.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"),
                                   opt_ptr(beta, "beta"), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"),
                                   wpart, dysum2.data_ptr<float>(), dw2.data_ptr<float>(), opt_mut(db2, "db2"), B, scr.partials,
-                                  scr.partials + static_cast<size_t>(B) * 64, grid_sync(scr), cur_stream(x), rider);
+                                  scr.partials + static_cast<size_t>(B) * 64, grid_sync(scr), cur_stream(x), rider, accumulate);
       entry.wgrad_batch = 0;
     };
     // the clip entry of a rider tuple → the clipping variant of the rider
@@ -400,7 +402,7 @@ void register_cuda_bindings(py::module_& m) {
     launch(rider);
   }, py::arg("dp"), py::arg("y"), py::arg("x"), py::arg("saved"), py::arg("gamma"), py::arg("beta"), py::arg("dgamma"), py::arg("dbeta"),
      py::arg("dw"), py::arg("db"), py::arg("dy2_pad"), py::arg("x2_pad"), py::arg("dysum2"), py::arg("dw2"), py::arg("db2"),
-     py::arg("sgd") = py::none());
+     py::arg("sgd") = py::none(), py::arg("accumulate") = false);
   m.def("convnet_l2_fwd", [](const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> bias, c10::optional<at::Tensor> gamma,
                              c10::optional<at::Tensor> beta, c10::optional<at::Tensor> running_mean, c10::optional<at::Tensor> running_var,
                              c10::optional<at::Tensor> nbt, double momentum, double eps, c10::optional<at::Tensor> fcw,
@@ -438,7 +440,7 @@ void register_cuda_bindings(py::module_& m) {
                           double mom1, double eps1, const at::Tensor& w2, c10::optional<at::Tensor> b2, c10::optional<at::Tensor> g2,
                           c10::optional<at::Tensor> be2, c10::optional<at::Tensor> rm2, c10::optional<at::Tensor> rv2, c10::optional<at::Tensor> nbt2,
                           double mom2, double eps2, const at::Tensor& fcw, c10::optional<at::Tensor> fcb, c10::optional<at::Tensor> target,
-                          bool defer_loss_mean) {
+                          bool defer_loss_mean, double grad_scale) {
     chk(x, "x"); chk(w1, "w1"); chk(w2, "w2"); chk(fcw, "fc weight");
     c10::cuda::CUDAGuard g(x.device());
     TORCH_CHECK(x.numel() % 784 == 0 && w1.numel() == 400 && w2.numel() == 12800 && fcw.dim() == 2 && fcw.size(1) == 1568 && fcw.size(0) <= 16,
@@ -454,7 +456,10 @@ void register_cuda_bindings(py::module_& m) {
       return reinterpret_cast<long long*>(t->data_ptr<int64_t>());
     };
     ReduceScratch scr = scratch(x);
-    FusedCe ce;
+    TORCH_CHECK(grad_scale > 0.0, "convnet_fwd: grad_scale must be positive");
+    // grad_scale (gradient accumulation over k micro-batches: 1/k): the loss is grad_scale · mean cross-entropy, dlogits its gradient
+    ScaledCe ce;
+    ce.scale = static_cast<float>(grad_scale);
     at::Tensor loss, dlogits, loss_parts;
     if (target.has_value() && target->defined()) {
       chk(*target, "target", at::kLong);
@@ -477,7 +482,8 @@ void register_cuda_bindings(py::module_& m) {
     return py::make_tuple(p1, y1, saved1, out, y2, saved2, logits, loss, dlogits, loss_parts);
   }, py::arg("x"), py::arg("w1"), py::arg("b1"), py::arg("g1"), py::arg("be1"), py::arg("rm1"), py::arg("rv1"), py::arg("nbt1"), py::arg("mom1"),
      py::arg("eps1"), py::arg("w2"), py::arg("b2"), py::arg("g2"), py::arg("be2"), py::arg("rm2"), py::arg("rv2"), py::arg("nbt2"), py::arg("mom2"),
-     py::arg("eps2"), py::arg("fcw"), py::arg("fcb"), py::arg("target") = py::none(), py::arg("defer_loss_mean") = false);
+     py::arg("eps2"), py::arg("fcw"), py::arg("fcb"), py::arg("target") = py::none(), py::arg("defer_loss_mean") = false,
+     py::arg("grad_scale") = 1.0);
   // p1 (conv2's input frame [B,18,18,16], optional): conv2's per-image weight-gradient partials are computed inside the kernel for
   // convnet_l1_bwd_wgrad(…, None, None, …) to fold, and the dy frame is not written (None in its place).
   m.def("convnet_l2_bwd", [](const at::Tensor& dout, const at::Tensor& y, const at::Tensor& saved, c10::optional<at::Tensor> gamma,
@@ -503,7 +509,7 @@ void register_cuda_bindings(py::module_& m) {
   m.def("convnet_l2_bwd_fc", [](const at::Tensor& dlogits, const at::Tensor& fcw, const at::Tensor& pooled, at::Tensor dfcw, c10::optional<at::Tensor> dfcb,
                                 const at::Tensor& y, const at::Tensor& saved, c10::optional<at::Tensor> gamma, c10::optional<at::Tensor> beta,
                                 const at::Tensor& w, at::Tensor dgamma, at::Tensor dbeta, c10::optional<at::Tensor> loss_parts,
-                                c10::optional<at::Tensor> loss_out, c10::optional<at::Tensor> p1) {
+                                c10::optional<at::Tensor> loss_out, c10::optional<at::Tensor> p1, bool accumulate) {
     chk(dlogits, "dlogits"); chk(fcw, "fc weight"); chk(pooled, "pooled"); chk(dfcw, "dfcw");
     chk(y, "y"); chk(saved, "saved"); chk(w, "w"); chk(dgamma, "dgamma"); chk(dbeta, "dbeta");
     c10::cuda::CUDAGuard g(y.device());
@@ -516,6 +522,8 @@ void register_cuda_bindings(py::module_& m) {
     TORCH_CHECK(!loss_parts.has_value() || !loss_parts->defined() || (loss_parts->numel() == B + 1 && loss_out.has_value() && loss_out->defined()),
                 "convnet_l2_bwd_fc: loss_parts must be the [B + 1] tensor of convnet_fwd, and loss_out given with it");
     const float* x2 = conv2_input(p1, B, "convnet_l2_bwd_fc");
+    // accumulate: dfcw, dfcb, dgamma, dbeta (and loss_out) hold the earlier micro-batches' sum and are added to
+    TORCH_CHECK(!accumulate || x2 != nullptr, "convnet_l2_bwd_fc: accumulate mode is the variant with conv2's weight-gradient partials (p1)");
     at::Tensor dy = x2 ? at::Tensor() : at::empty({B, 18, 18, 32}, y.options());
     at::Tensor dx = at::empty({B, 18, 18, 16}, y.options());
     at::Tensor dysum = at::empty({B, 32}, y.options());
@@ -525,12 +533,12 @@ void register_cuda_bindings(py::module_& m) {
                              ncls, y.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"), opt_ptr(beta, "beta"), w.data_ptr<float>(),
                              dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), x2 ? nullptr : dy.data_ptr<float>(), dx.data_ptr<float>(),
                              dysum.data_ptr<float>(), B, scr.partials, grid_sync(scr), cur_stream(y), opt_ptr(loss_parts, "loss_parts"),
-                             opt_mut(loss_out, "loss_out"), x2, wpart);
+                             opt_mut(loss_out, "loss_out"), x2, wpart, accumulate);
     if (x2) scratch_entry(y).wgrad_batch = B;
     return py::make_tuple(x2 ? py::none() : py::cast(dy), dx, dysum);
   }, py::arg("dlogits"), py::arg("fcw"), py::arg("pooled"), py::arg("dfcw"), py::arg("dfcb"), py::arg("y"), py::arg("saved"), py::arg("gamma"),
      py::arg("beta"), py::arg("w"), py::arg("dgamma"), py::arg("dbeta"), py::arg("loss_parts") = py::none(), py::arg("loss_out") = py::none(),
-     py::arg("p1") = py::none());
+     py::arg("p1") = py::none(), py::arg("accumulate") = false);
   m.def("conv5x5_wgrad_win", [](const at::Tensor& dy_pad, const at::Tensor& x_pad, const at::Tensor& dysum, at::Tensor dw, c10::optional<at::Tensor> db) {
     chk(dy_pad, "dy_pad"); chk(x_pad, "x_pad"); chk(dysum, "dysum"); chk(dw, "dw");
     c10::cuda::CUDAGuard g(dy_pad.device());

@@ -475,7 +475,9 @@ __device__ __forceinline__ float clip_acc(const R& r, float acc, float g) { retu
 template <class R>
 __device__ __forceinline__ float clip_comb(const R& r, float a, float b) { return r.norm_inf ? nan_max(a, b) : a + b; }
 
-template <bool WG, class Rider = SgdRider>
+// ACC (accumulate mode, gradient accumulation over micro-batches): every gradient this kernel writes — dgamma, dbeta, the conv1 fold
+// dw / db and the conv2 fold dw2 / db2 — becomes g = g_old + v, and the rider updates with (and clips) that accumulated value.
+template <bool WG, class Rider = SgdRider, bool ACC = false>
 __global__ void __launch_bounds__(kL1Threads, 1)
 convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y, const float* __restrict__ x, const float* __restrict__ saved,
                       const float* __restrict__ gamma, const float* __restrict__ beta, float* dgamma, float* dbeta, float* dw, float* db,
@@ -486,6 +488,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   constexpr bool kAdam = std::is_same_v<Rider, AdamRider> || std::is_same_v<Rider, ClipRider<AdamRider>>;
   static_assert(kAdam || std::is_base_of_v<SgdRider, Rider>, "convnet_l1_bwd_kernel: SgdRider or AdamRider, or either in a ClipRider");
   static_assert(WG || !(kAdam || kClip), "the Adam and clipping riders ride on the kernel with the conv2 weight gradient");
+  static_assert(WG || !ACC, "accumulate mode is a variant of the kernel with the conv2 weight gradient");
   extern __shared__ __align__(16) float dsm[];
   float* dys = dsm;                  // [784][16]
   float* fold = dsm + 784 * 16;      // [25 warps][16][32]
@@ -640,11 +643,13 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
           for (int wi = 0; wi < kL1Warps; ++wi) tot += s_f[(u * kL1Warps + wi) * 32 + lane];
           if (i < 400) {
             const int e = (lane * 16 + (i & 15)) * 25 + (i >> 4);
+            if constexpr (ACC) tot = dw2[e] + tot;
             dw2[e] = tot;
             if constexpr (kClip) ca = clip_acc(sr, ca, tot);
             else if constexpr (kAdam) { if (sr.on) adam_apply(sr, 4, e, tot, adam_f); }
             else if (sr.on) sgd_apply(sr.p[4] + e, tot, sr.m[4] ? sr.m[4] + e : nullptr, sr.h, sgd_lr);
           } else if (db2) {
+            if constexpr (ACC) tot = db2[lane] + tot;
             db2[lane] = tot;
             if constexpr (kClip) { if (sr.p[5]) ca = clip_acc(sr, ca, tot); }
             else if constexpr (kAdam) { if (sr.on && sr.p[5]) adam_apply(sr, 5, lane, tot, adam_f); }
@@ -666,8 +671,13 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   fold_rows_wide<32, kL1Threads>(partials, B, s_tmp, s_tot);  // [0..16) Σdz, [16..32) Σdz·x̂
   trace(1, 3);
   if (n == 0 && tid < 16) {
-    if (dbeta) dbeta[tid] = s_tot[tid];
-    if (dgamma) dgamma[tid] = s_tot[16 + tid];
+    if constexpr (ACC) {   // s_tot keeps this batch's sums: the data gradient below needs them
+      if (dbeta) dbeta[tid] = dbeta[tid] + s_tot[tid];
+      if (dgamma) dgamma[tid] = dgamma[tid] + s_tot[16 + tid];
+    } else {
+      if (dbeta) dbeta[tid] = s_tot[tid];
+      if (dgamma) dgamma[tid] = s_tot[16 + tid];
+    }
   }
   const float inv_cnt = 1.f / (static_cast<float>(B) * 784.f);
   if (m.valid) {
@@ -761,11 +771,13 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
     for (int off = 16; off >= 1; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
     if (lane == 0) {
       if (tap < 25) {
+        if constexpr (ACC) s = dw[co * 25 + tap] + s;
         dw[co * 25 + tap] = s;
         if constexpr (kClip) ca = clip_acc(sr, ca, s);
         else if constexpr (kAdam) { if (sr.on) adam_apply(sr, 0, co * 25 + tap, s, adam_f); }
         else if (sr.on) sgd_apply(sr.p[0] + co * 25 + tap, s, sr.m[0] ? sr.m[0] + co * 25 + tap : nullptr, sr.h, sgd_lr);
       } else if (db) {
+        if constexpr (ACC) s = db[co] + s;
         db[co] = s;
         if constexpr (kClip) { if (sr.p[1]) ca = clip_acc(sr, ca, s); }
         else if constexpr (kAdam) { if (sr.on && sr.p[1]) adam_apply(sr, 1, co, s, adam_f); }
@@ -776,7 +788,20 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   if (sr.on && n == 0 && tid < 16) {
     // BatchNorm-1 affine parameters: their gradients are the totals this CTA folded after the first barrier.  Every CTA read
     // gamma / beta before that barrier, so updating them here (after the second one) races with nobody.
-    if constexpr (kClip) {
+    if constexpr (ACC) {
+      // accumulate mode: the gradients are what this thread wrote above (batch sums added to the earlier micro-batches')
+      const float gbeta = dbeta ? dbeta[tid] : 0.f, ggamma = dgamma ? dgamma[tid] : 0.f;
+      if constexpr (kClip) {
+        if (sr.p[3]) ca = clip_acc(sr, ca, gbeta);
+        if (sr.p[2]) ca = clip_acc(sr, ca, ggamma);
+      } else if constexpr (kAdam) {
+        if (sr.p[3]) adam_apply(sr, 3, tid, gbeta, adam_f);
+        if (sr.p[2]) adam_apply(sr, 2, tid, ggamma, adam_f);
+      } else {
+        if (sr.p[3]) sgd_apply(sr.p[3] + tid, gbeta, sr.m[3] ? sr.m[3] + tid : nullptr, sr.h, sgd_lr);
+        if (sr.p[2]) sgd_apply(sr.p[2] + tid, ggamma, sr.m[2] ? sr.m[2] + tid : nullptr, sr.h, sgd_lr);
+      }
+    } else if constexpr (kClip) {
       if (sr.p[3]) ca = clip_acc(sr, ca, s_tot[tid]);
       if (sr.p[2]) ca = clip_acc(sr, ca, s_tot[16 + tid]);
     } else if constexpr (kAdam) {
@@ -1100,14 +1125,20 @@ convnet_l2_fwd_kernel(const __grid_constant__ CUtensorMap tm_x, const float* __r
 // layer-1 activations never leave the SM on their way into conv2 — they are written straight into the swizzled,
 // zero-haloed shared-memory patch the wgmma descriptors read (the global copy is still written: backward needs it) —
 // and the conv2 weights are staged while conv1 computes.  Two grid barriers (BN1 and BN2 batch statistics), one launch.
+// Ce = ScaledCe: the cross-entropy rider computes scale · (mean cross-entropy) and its gradient (gradient accumulation: 1/k).
 // =====================================================================================================================
+__device__ __forceinline__ float ce_scale(const FusedCe&) { return 1.f; }
+__device__ __forceinline__ float ce_scale(const ScaledCe& ce) { return ce.scale; }
+
+template <class Ce = FusedCe>
 __global__ void __launch_bounds__(kL1Threads, 1)
 convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ g1,
                    const float* __restrict__ be1, float* __restrict__ y1, float* __restrict__ p1, float* saved1, float* rm1, float* rv1,
                    long long* nbt1, float mom1, float eps1, const float* __restrict__ w2, const float* __restrict__ b2,
                    const float* __restrict__ g2, const float* __restrict__ be2, float* __restrict__ y2, float* __restrict__ out, float* saved2,
                    float* rm2, float* rv2, long long* nbt2, float mom2, float eps2, const float* __restrict__ fcw,
-                   const float* __restrict__ fcb, float* __restrict__ logits, int ncls, float* partials, GridSync gs, FusedCe ce) {
+                   const float* __restrict__ fcb, float* __restrict__ logits, int ncls, float* partials, GridSync gs, Ce ce) {
+  constexpr bool kScaled = std::is_same_v<Ce, ScaledCe>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sa = smem;                                  // conv2 input patch, written by this CTA's layer-1 epilogue
@@ -1379,10 +1410,16 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
         const long long t = ce.target[n];
         const bool t_ok = t >= 0 && t < ncls;
         const float lt = __shfl_sync(0xffffffffu, lg, t_ok ? static_cast<int>(t) : 0);
-        if (lane < ncls)
-          ce.dlogits[static_cast<size_t>(n) * ncls + lane] = t_ok ? (e / ssum - (t == lane ? 1.f : 0.f)) / static_cast<float>(counted) : 0.f;
+        if (lane < ncls) {
+          // ScaledCe: the rounding of autograd's grad · scale behind the unscaled loss
+          if constexpr (kScaled)
+            ce.dlogits[static_cast<size_t>(n) * ncls + lane] = (t_ok ? (e / ssum - (t == lane ? 1.f : 0.f)) / static_cast<float>(counted) : 0.f) * ce.scale;
+          else
+            ce.dlogits[static_cast<size_t>(n) * ncls + lane] = t_ok ? (e / ssum - (t == lane ? 1.f : 0.f)) / static_cast<float>(counted) : 0.f;
+        }
         if (lane == 0) ce.loss_parts[n] = t_ok ? mx + __logf(ssum) - lt : 0.f;
-        if (lane == 0 && n == 0) ce.loss_parts[B] = static_cast<float>(counted);   // for a mean folded later
+        // for a mean folded later (ScaledCe: the divisor is the count over the scale)
+        if (lane == 0 && n == 0) ce.loss_parts[B] = kScaled ? static_cast<float>(counted) / ce_scale(ce) : static_cast<float>(counted);
         if (ce.loss != nullptr) {   // batch mean now (otherwise layer-2 backward folds it: ce.loss == nullptr)
           int last = 0;
           if (lane == 0) {
@@ -1397,7 +1434,7 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
 #pragma unroll
             for (int off = 16; off >= 1; off >>= 1) sl += __shfl_xor_sync(0xffffffffu, sl, off);
             if (lane == 0) {
-              *ce.loss = sl / static_cast<float>(counted);
+              *ce.loss = sl / (kScaled ? static_cast<float>(counted) / ce_scale(ce) : static_cast<float>(counted));
               *ce.counter = 0u;
             }
           }
@@ -1431,7 +1468,9 @@ struct L2BwdSmem {
 // WG: conv2's weight-gradient partial of the image (Conv2Wg) is computed here on wgmma, issued by warpgroup 0 while warpgroup 1 issues
 // the data gradient's: the x copies are written from conv2's input frame x2 in the shadow of the grid barrier, dyᵀ from the
 // registers that write the dy patch.  The global dy frame is then not written: nothing reads it.
-template <bool FC, bool WG>
+// ACC (accumulate mode, gradient accumulation over micro-batches): every gradient this kernel writes — dfcw, dfcb, dgamma, dbeta —
+// and the folded loss become g = g_old + v, one fp32 add, the rounding of autograd's accumulation of a temporary.
+template <bool FC, bool WG, bool ACC = false>
 __global__ void __launch_bounds__(kL2Threads, 1)
 convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float* __restrict__ y /*[B,14,14,32]*/,
                       const float* __restrict__ saved, const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -1444,6 +1483,7 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
                       int ncls, const float* __restrict__ loss_parts /*[B] or null*/, float* loss_out,
                       // WG only
                       const float* __restrict__ x2 /*[B,18,18,16] = conv2's input frame*/, float* __restrict__ wpart /*[B][400][32]*/) {
+  static_assert(!ACC || (FC && WG), "accumulate mode is a variant of the kernel with the classifier and conv2's weight gradient");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sa = smem;                                  // dy patch, written by the CTA in the TMA/wgmma SWIZZLE_128B layout
@@ -1613,13 +1653,16 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
             for (int u = 0; u < 4; ++u) a[u] = fmaf(s_dl[(r + u) * 16 + j], s_pool[(r + u) * 16 + kl], a[u]);
           }
           for (; r < B; ++r) a[0] = fmaf(s_dl[r * 16 + j], s_pool[r * 16 + kl], a[0]);
-          dfcw[static_cast<size_t>(j) * 1568 + slice * 16 + kl] = (a[0] + a[1]) + (a[2] + a[3]);
+          float* dst = dfcw + static_cast<size_t>(j) * 1568 + slice * 16 + kl;
+          if constexpr (ACC) *dst = *dst + ((a[0] + a[1]) + (a[2] + a[3]));
+          else *dst = (a[0] + a[1]) + (a[2] + a[3]);
         }
       } else {
         if (dfcb != nullptr && tid < ncls) {
           float a = 0.f;
           for (int r = 0; r < B; ++r) a += s_dl[r * 16 + tid];
-          dfcb[tid] = a;
+          if constexpr (ACC) dfcb[tid] = dfcb[tid] + a;
+          else dfcb[tid] = a;
         }
         if (loss_parts != nullptr && warp == 7) {   // the forward kernel left one cross-entropy term per image and the number of
           const float counted = __ldg(loss_parts + B);   // counted images after them: batch mean, fixed order
@@ -1627,7 +1670,8 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
           for (int r = lane; r < B; r += 32) sl += __ldg(loss_parts + r);
 #pragma unroll
           for (int off = 16; off >= 1; off >>= 1) sl += __shfl_xor_sync(0xffffffffu, sl, off);
-          if (lane == 0) *loss_out = sl / counted;
+          if constexpr (ACC) { if (lane == 0) *loss_out = *loss_out + sl / counted; }
+          else if (lane == 0) *loss_out = sl / counted;
         }
       }
     }
@@ -1637,8 +1681,13 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
   fold_rows<64>(partials, B, s_tmp, s_tot);
   trace(3, 4);
   if (n == 0 && tid < 32) {
-    if (dbeta) dbeta[tid] = s_tot[tid];
-    if (dgamma) dgamma[tid] = s_tot[32 + tid];
+    if constexpr (ACC) {
+      if (dbeta) dbeta[tid] = dbeta[tid] + s_tot[tid];
+      if (dgamma) dgamma[tid] = dgamma[tid] + s_tot[32 + tid];
+    } else {
+      if (dbeta) dbeta[tid] = s_tot[tid];
+      if (dgamma) dgamma[tid] = s_tot[32 + tid];
+    }
   }
   {
     const float inv_cnt = 1.f / (static_cast<float>(B) * 196.f);
@@ -1790,14 +1839,15 @@ void launch_conv2_wgrad_partials(const float* dy2_pad, const float* x2_pad, int 
 template <class Rider>
 void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
                                  float* dgamma, float* dbeta, float* dw, float* db, const float* wpart, const float* dysum2, float* dw2, float* db2,
-                                 int B, float* partials, float* partials_w, GridSync gs, cudaStream_t st, Rider rider) {
-  launch_cooperative(convnet_l1_bwd_kernel<true, Rider>, B, kL1Threads, static_cast<size_t>(kL1BwdSmem), st, "convnet_l1_bwd_wgrad", dp, y, x, saved,
+                                 int B, float* partials, float* partials_w, GridSync gs, cudaStream_t st, Rider rider, bool accumulate) {
+  auto kernel = accumulate ? convnet_l1_bwd_kernel<true, Rider, true> : convnet_l1_bwd_kernel<true, Rider>;
+  launch_cooperative(kernel, B, kL1Threads, static_cast<size_t>(kL1BwdSmem), st, "convnet_l1_bwd_wgrad", dp, y, x, saved,
                      gamma, beta, dgamma, dbeta, dw, db, partials, partials_w, gs, wpart, dysum2, dw2, db2, rider);
 }
 #define PDT_L1_BWD_WGRAD(R)                                                                                                            \
   template void launch_convnet_l1_bwd_wgrad<R>(const float*, const float*, const float*, const float*, const float*, const float*, float*, \
                                                float*, float*, float*, const float*, const float*, float*, float*, int, float*, float*,       \
-                                               GridSync, cudaStream_t, R);
+                                               GridSync, cudaStream_t, R, bool);
 PDT_L1_BWD_WGRAD(SgdRider)
 PDT_L1_BWD_WGRAD(AdamRider)
 PDT_L1_BWD_WGRAD(ClipRider<SgdRider>)
@@ -1816,11 +1866,19 @@ void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const 
                         float* rm1, float* rv1, long long* nbt1, float mom1, float eps1, const float* w2, const float* b2, const float* g2,
                         const float* be2, float* y2, float* out, float* saved2, float* rm2, float* rv2, long long* nbt2, float mom2, float eps2,
                         const float* fcw, const float* fcb, float* logits, int ncls, int B, float* partials, GridSync gs, cudaStream_t st,
-                        FusedCe ce) {
+                        ScaledCe ce) {
   if (logits != nullptr && ncls > 16) throw std::invalid_argument("convnet_fwd: the fused classifier handles at most 16 classes");
   if (ce.target != nullptr && logits == nullptr) throw std::invalid_argument("convnet_fwd: the fused cross-entropy needs the fused classifier");
-  launch_cooperative(convnet_fwd_kernel, B, kL1Threads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1, saved1, rm1, rv1,
-                     nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials, gs, ce);
+  if (!(ce.scale > 0.f)) throw std::invalid_argument("convnet_fwd: the cross-entropy scale must be positive");
+  if (ce.target != nullptr && ce.scale != 1.f) {
+    launch_cooperative(convnet_fwd_kernel<ScaledCe>, B, kL1Threads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1,
+                       saved1, rm1, rv1, nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials,
+                       gs, ce);
+    return;
+  }
+  launch_cooperative(convnet_fwd_kernel<FusedCe>, B, kL1Threads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1, saved1,
+                     rm1, rv1, nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials, gs,
+                     static_cast<const FusedCe&>(ce));
 }
 
 void launch_convnet_l2_bwd(const float* dout, const float* y, const float* saved, const float* gamma, const float* beta, const float* w,
@@ -1836,10 +1894,12 @@ void launch_convnet_l2_bwd(const float* dout, const float* y, const float* saved
 void launch_convnet_l2_bwd_fc(const float* dlogits, const float* fcw, const float* pooled, float* dfcw, float* dfcb, int ncls, const float* y,
                               const float* saved, const float* gamma, const float* beta, const float* w, float* dgamma, float* dbeta, float* dy,
                               float* dx, float* dysum, int B, float* partials, GridSync gs, cudaStream_t st, const float* loss_parts, float* loss_out,
-                              const float* x2, float* wpart) {
+                              const float* x2, float* wpart, bool accumulate) {
   if (ncls < 1 || ncls > 16) throw std::invalid_argument("convnet_l2_bwd_fc: 1..16 classes");
   if (B > 160) throw std::invalid_argument("convnet_l2_bwd_fc: batch too large for the staged dlogits");
-  auto kernel = x2 != nullptr ? convnet_l2_bwd_kernel<true, true> : convnet_l2_bwd_kernel<true, false>;
+  if (accumulate && x2 == nullptr) throw std::invalid_argument("convnet_l2_bwd_fc: accumulate mode needs conv2's input frame (x2)");
+  auto kernel = accumulate ? convnet_l2_bwd_kernel<true, true, true>
+                           : x2 != nullptr ? convnet_l2_bwd_kernel<true, true> : convnet_l2_bwd_kernel<true, false>;
   const int smem = x2 != nullptr ? std::max(L2BwdSmem::kTotalFc, L2BwdSmem::kTotalWg) : L2BwdSmem::kTotalFc;
   launch_cooperative(kernel, B, kL2Threads, static_cast<size_t>(smem), st, "convnet_l2_bwd_fc", static_cast<const float*>(nullptr), y, saved,
                      gamma, beta, w, dgamma, dbeta, dy, dx, dysum, partials, gs, dlogits, fcw, pooled, dfcw, dfcb, ncls, loss_parts, loss_out, x2,

@@ -66,10 +66,13 @@ struct ClipRider : Base {
 void launch_conv2_wgrad_partials(const float* dy2_pad, const float* x2_pad, int B, float* wpart, cudaStream_t st);
 // Layer-1 backward that also folds conv2's weight gradient: the per-image partials wpart and Σdy rows dysum2 [B,32] → dw2
 // [32,16,5,5], db2 [32], in the shadow of the kernel's first grid barrier.  Rider: SgdRider or AdamRider, or either one in a ClipRider.
+// accumulate: gradient accumulation — every gradient written (dgamma, dbeta, dw, db, dw2, db2) becomes g_old + this batch's value, and
+// the rider updates with (and clips) the accumulated gradient.
 template <class Rider = SgdRider>
 void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
                                  float* dgamma, float* dbeta, float* dw, float* db, const float* wpart, const float* dysum2, float* dw2, float* db2,
-                                 int B, float* partials, float* partials_w, GridSync gs, cudaStream_t st, Rider rider = Rider{});
+                                 int B, float* partials, float* partials_w, GridSync gs, cudaStream_t st, Rider rider = Rider{},
+                                 bool accumulate = false);
 // x [B,18,18,16] frame → y [B,14,14,32], out [B,32,7,7] NCHW, saved [64]; logits [B,ncls] = fc(out) when logits != nullptr.
 // partials: B·64 floats.
 void launch_convnet_l2_fwd(const float* x, const float* w, const float* bias, const float* gamma, const float* beta, float* y, float* out,
@@ -86,14 +89,21 @@ struct FusedCe {
   float* dlogits = nullptr;            // [B, ncls]
   unsigned int* counter = nullptr;     // zero before first use; reset by the kernel
 };
+// The same rider with a gradient scale: the loss is scale · (mean cross-entropy) and dlogits its gradient, i.e. the unscaled
+// gradient times scale, rounded as autograd's grad · scale would be.  Gradient accumulation over k micro-batches uses 1/k (torch's
+// loss / k convention).  The mean's divisor loss_parts[B] becomes n / scale, so a mean folded later carries the scale too.
+struct ScaledCe : FusedCe {
+  float scale = 1.f;
+};
 
 // The whole training forward in one launch: layer 1 and layer 2 (+ classifier, ncls ≤ 16) of an image in the same CTA; the
 // pooled layer-1 activations go into conv2's shared-memory patch directly.  partials: B·(32 + 64) floats.
+// ce.scale != 1 (with targets) runs the ScaledCe instantiation; otherwise the kernel without the scale.
 void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const float* g1, const float* be1, float* y1, float* p1, float* saved1,
                         float* rm1, float* rv1, long long* nbt1, float mom1, float eps1, const float* w2, const float* b2, const float* g2,
                         const float* be2, float* y2, float* out, float* saved2, float* rm2, float* rv2, long long* nbt2, float mom2, float eps2,
                         const float* fcw, const float* fcb, float* logits, int ncls, int B, float* partials, GridSync gs, cudaStream_t st,
-                        FusedCe ce = FusedCe{});
+                        ScaledCe ce = ScaledCe{});
 // dout [B,32,7,7] → dgamma/dbeta [32], dy [B,18,18,32] frame with zero halo (gradient at the conv2 output), dx [B,18,18,16] frame
 // (data gradient, interior written), dysum [B,32] (per-image Σdy: the conv2 bias gradient is the sum of its rows).
 // x2 != nullptr (conv2's input frame [B,18,18,16]): conv2's weight-gradient partials per image go to wpart [B][400][32] instead,
@@ -107,6 +117,7 @@ void launch_convnet_l2_bwd_fc(const float* dlogits, const float* fcw, const floa
                               const float* saved, const float* gamma, const float* beta, const float* w, float* dgamma, float* dbeta, float* dy,
                               float* dx, float* dysum, int B, float* partials, GridSync gs, cudaStream_t st,
                               const float* loss_parts = nullptr, float* loss_out = nullptr,   // mean of the forward kernel's CE terms
-                              const float* x2 = nullptr, float* wpart = nullptr);             // as for launch_convnet_l2_bwd
+                              const float* x2 = nullptr, float* wpart = nullptr,              // as for launch_convnet_l2_bwd
+                              bool accumulate = false);   // dfcw, dfcb, dgamma, dbeta, loss_out += this batch's values (needs x2)
 
 }  // namespace pdt

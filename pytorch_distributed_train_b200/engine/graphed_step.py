@@ -27,22 +27,58 @@ otherwise the native clip runs between backward and ``step()`` inside the graph 
 is not fused into the gradient reduction: the reducer averages, the step clips, then ``step()`` runs.  The averaged gradients
 are bitwise identical on every rank and the norm is reproducible bit for bit, so every rank derives the same coefficient
 without a collective.
+
+Gradient accumulation (``accumulation_steps=k``): the step's inputs carry k micro-batches of b rows each (micro-batch i is rows
+[i·b, (i+1)·b)); one captured step runs k forward/backward passes and one update on the summed gradient of ``loss / k`` (torch's
+convention; BatchNorm uses per-micro-batch statistics and updates its running statistics k times).  On the reference ConvNet
+whose ten gradients all come from the two fused backward kernels, with a criterion that returns the fused cross-entropy
+unchanged, the forward kernel emits the gradient of ``loss / k``, the backward kernels of micro-batches 2..k add into the
+gradients of micro-batch 1 (accumulate mode, ops.functional.accumulate_into) and the update — with the clipping — rides on the
+last micro-batch's backward: 3k launches, no AccumulateGrad add, no separate optimizer or clip kernel.  Any other model,
+criterion or configuration accumulates through autograd.  One GPU only for now: for a model whose gradients are reduced across
+ranks the micro-batches 1..k−1 would have to skip the reduction (``no_sync``) inside the captured step.
 """
 from __future__ import annotations
 
 from typing import Optional, Sequence
 
+import contextlib
 import os
 
 import torch
 
 
 class GraphedTrainStep:
+    # private switch for comparisons (tools/accum_step_bench.py): False accumulates through autograd even where the fused backward
+    # kernels could add in place
+    _accumulate_in_kernel = True
+
     def __init__(self, model, criterion, optimizer, example_inputs: Sequence[torch.Tensor], warmup: int = 3,
                  zero_grad_set_to_none: bool = True, fuse_optimizer: bool = True, double_buffer_inputs: bool = True,
-                 max_grad_norm: Optional[float] = None, norm_type: float = 2.0):
+                 max_grad_norm: Optional[float] = None, norm_type: float = 2.0, accumulation_steps: int = 1):
         if not torch.cuda.is_available():
             raise RuntimeError("GraphedTrainStep needs CUDA")
+        k = int(accumulation_steps)
+        if k != accumulation_steps or k < 1:
+            raise ValueError(f"accumulation_steps must be a positive integer, got {accumulation_steps}")
+        if k > 1:
+            rows = {int(t.shape[0]) for t in example_inputs}
+            if len(rows) != 1 or next(iter(rows)) % k != 0:
+                raise ValueError(f"accumulation_steps={k}: every input must have the same number of rows, a multiple of {k} "
+                                 f"(got {sorted(rows)})")
+            # a model that reduces its gradients across ranks (DistributedDataParallel) would need the reduction skipped on all but the
+            # last micro-batch; an unwrapped model accumulates locally whatever the default group's size
+            group_ = getattr(model, "process_group", None)
+            if group_ is not None and group_.size() > 1:
+                raise NotImplementedError("GraphedTrainStep(accumulation_steps > 1) runs on one GPU only: at world size >= 2 the "
+                                          "micro-batches before the last would have to skip the gradient reduction (no_sync) inside "
+                                          "the captured step")
+        self.accumulation_steps = k
+        # ``step`` of the last eager or captured step: whether micro-batches 2..k accumulated inside the fused backward kernels
+        self.accumulates_in_kernel = False
+        # whether the forward kernel may emit the cross-entropy already scaled by 1/k: decided by the first (unscaled) eager step, True
+        # when the criterion returned the fused cross-entropy itself on every micro-batch (None: not decided yet)
+        self._prescale: Optional[bool] = None
         self.model, self.criterion, self.optimizer = model, criterion, optimizer
         self.static_inputs = [t.clone() for t in example_inputs]
         # two input buffers, one captured graph each: the next batch's copy into the step's static inputs (host→device from pinned
@@ -86,17 +122,100 @@ class GraphedTrainStep:
         inputs = self.static_inputs if inputs is None else inputs
         from ..ops import functional as OF
 
+        if self.accumulation_steps > 1:
+            return self._finish_step(self._accumulate(inputs))
+
         # the step owns the targets before the model runs: a model whose forward kernel can fold the loss in does so
         # (ops.functional.upcoming_targets); the criterion then finds value and gradient ready
         with OF.upcoming_targets(inputs[1] if len(inputs) == 2 else None, loss_read_after_backward=True):
             out = self.model(inputs[0])
         loss = self.criterion(out, *inputs[1:])
         self.optimizer.zero_grad(set_to_none=self.set_to_none)
+        with OF.sgd_rider_enabled():   # an optimizer armed with ride_on_backward may apply its update inside this backward pass
+            loss.backward(self._unit_seed(loss))
+        return self._finish_step(loss)
+
+    def _unit_seed(self, loss):
         if self._seed is None or self._seed.shape != loss.shape or self._seed.dtype != loss.dtype:
             self._seed = torch.ones_like(loss)
             self._seed._pdt_unit_seed = True   # lets ops that pre-compute their unit-gradient backward skip the scaling kernel
-        with OF.sgd_rider_enabled():   # an optimizer armed with ride_on_backward may apply its update inside this backward pass
-            loss.backward(self._seed)
+        return self._seed
+
+    def _accumulate(self, inputs):
+        """Forward and backward of the k micro-batches; returns the mean of their losses.  Micro-batches 2..k add into the gradient
+        buffers micro-batch 1 left — inside the fused backward kernels when micro-batch 1 showed that they wrote every gradient and
+        the loss is the fused cross-entropy's (scaled by 1/k in the forward kernel, its mean folded by a backward kernel), through
+        autograd's accumulation otherwise.  The riding update is enabled for the last micro-batch's backward only.
+
+        The forward kernel scales the cross-entropy, and a backward kernel folds its mean, only for a criterion that returns it
+        unchanged (pdt.nn.CrossEntropyLoss): a criterion that computes anything from it (``ce * w``, ``ce + reg``) would see — and
+        scale once more — the scaled value, and would read the loss before backward has folded it.  The first eager step therefore
+        runs unscaled with the mean folded by the forward kernel and backpropagates ``loss / k``; it records whether the criterion's
+        result was the fused cross-entropy itself, and only then do later steps let the kernels scale and fold.  A criterion that
+        changes its mind later is an error, not a silently doubled scale."""
+        from ..ops import functional as OF
+
+        k = self.accumulation_steps
+        b = inputs[0].shape[0] // k
+        scale = 1.0 / k
+        grad_scale = scale if self._prescale else 1.0
+        returns_ce = True
+        params = [p for p in self.model.parameters() if p.requires_grad]
+        self.optimizer.zero_grad(set_to_none=self.set_to_none)
+        kept = None     # (gradient buffers of micro-batch 1, its loss buffer): the in-kernel accumulation's destinations
+        total = None
+        for i in range(k):
+            micro = [t[i * b:(i + 1) * b] for t in inputs]
+            OF.reset_fused_ce_consumed()
+            with OF.upcoming_targets(micro[1] if len(micro) == 2 else None, loss_read_after_backward=bool(self._prescale),
+                                     grad_scale=grad_scale):
+                out = self.model(micro[0])
+            loss = self.criterion(out, *micro[1:])
+            consumed = OF.fused_ce_consumed()
+            # the criterion's result is the one fused cross-entropy of this forward, as cross_entropy returned it
+            is_ce = (len(consumed) == 1 and consumed[0] == (id(loss), grad_scale)
+                     and getattr(loss, "_pdt_loss_scale", None) == grad_scale)
+            returns_ce = returns_ce and is_ce
+            if grad_scale != 1.0 and not is_ce:
+                raise RuntimeError("gradient accumulation: the forward kernel scaled the cross-entropy by 1/k because the criterion "
+                                   "returned it unchanged in the first step, but this time the criterion computed something else from "
+                                   "it; the scale would be applied twice")
+            prescaled = grad_scale != 1.0
+            fused_loss = prescaled and getattr(loss, "_pdt_loss_deferred", False)
+            part = loss if prescaled else loss / k
+            into = None
+            if kept is not None and fused_loss:
+                for p in params:
+                    p.grad = None   # the kernels add into the kept buffers and hand them back as fresh gradients
+                into = OF.accumulate_into(kept[0], kept[1])
+            OF.reset_fused_backward_params()
+            riding = OF.sgd_rider_enabled() if i == k - 1 else contextlib.nullcontext()
+            with (into if into is not None else contextlib.nullcontext()), riding:
+                part.backward(self._unit_seed(part))
+            if into is not None:
+                lost = into.leftover() + [p for p in kept[0] if p.grad is None]
+                if lost:
+                    raise RuntimeError(f"gradient accumulation: {len(lost)} gradient(s) of micro-batch {i + 1} were not added in the fused "
+                                       "backward kernels")
+                # the sums, where .grad holds them now (a DDP reducer that has just rebuilt its buckets copies them into the new ones)
+                kept = ({p: p.grad for p in kept[0]}, kept[1])
+            if i == 0:
+                wrote = OF.fused_backward_params()
+                grads = {p: p.grad for p in params if p.grad is not None}
+                if (self._accumulate_in_kernel and fused_loss and wrote is not None and {id(p) for p in wrote if p is not None} == {id(p) for p in grads}
+                        and all(g.is_contiguous() for g in grads.values())):
+                    kept = (grads, part.detach())
+            self.accumulates_in_kernel = kept is not None
+            if into is None or total is None:
+                total = part if total is None else total + part.detach()
+        if self._prescale is None:
+            self._prescale = returns_ce
+        return total   # in-kernel: micro-batch 1's loss buffer, to which the later folds added
+
+    def _finish_step(self, loss):
+        """Clipping (unless the riding update did it) and the optimizer step after the backward pass(es)."""
+        from ..ops import functional as OF
+
         norm = None
         if self.max_grad_norm is not None:
             if getattr(self.optimizer, "_rode", False):

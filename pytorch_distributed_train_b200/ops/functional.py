@@ -145,25 +145,86 @@ _upcoming_target: Optional[torch.Tensor] = None
 
 
 _loss_read_after_backward = False
+_upcoming_grad_scale = 1.0
 
 
 class upcoming_targets:
     """``loss_read_after_backward=True`` (a captured step: nobody looks at the loss before the whole step has run) lets the
-    batch mean of the per-image loss terms be folded by the first backward kernel instead of by the forward kernel's tail."""
+    batch mean of the per-image loss terms be folded by the first backward kernel instead of by the forward kernel's tail.
 
-    def __init__(self, target: Optional[torch.Tensor], loss_read_after_backward: bool = False):
-        self.target, self.late = target, loss_read_after_backward
+    ``grad_scale`` (gradient accumulation over k micro-batches: 1/k) makes the forward kernel produce ``grad_scale · loss`` and its
+    gradient, so backward seeded with one yields torch's ``(loss / k).backward()`` with no scaling kernel.  That is right only when
+    the criterion's result IS the cross-entropy ``cross_entropy`` returned (its ``_pdt_loss_scale`` says by how much it is scaled):
+    a criterion that computes anything from it (``ce * w``, ``ce + reg``) would see the scaled value.  ``fused_ce_consumed`` lists
+    every fused cross-entropy handed out since ``reset_fused_ce_consumed``, so the caller can check that before it scales."""
+
+    def __init__(self, target: Optional[torch.Tensor], loss_read_after_backward: bool = False, grad_scale: float = 1.0):
+        if not float(grad_scale) > 0:
+            raise ValueError(f"grad_scale must be positive, got {grad_scale}")
+        self.target, self.late, self.scale = target, loss_read_after_backward, float(grad_scale)
 
     def __enter__(self):
-        global _upcoming_target, _loss_read_after_backward
-        self.prev = (_upcoming_target, _loss_read_after_backward)
-        _upcoming_target, _loss_read_after_backward = self.target, self.late
+        global _upcoming_target, _loss_read_after_backward, _upcoming_grad_scale
+        self.prev = (_upcoming_target, _loss_read_after_backward, _upcoming_grad_scale)
+        _upcoming_target, _loss_read_after_backward, _upcoming_grad_scale = self.target, self.late, self.scale
         return self
 
     def __exit__(self, *exc):
-        global _upcoming_target, _loss_read_after_backward
-        _upcoming_target, _loss_read_after_backward = self.prev
+        global _upcoming_target, _loss_read_after_backward, _upcoming_grad_scale
+        _upcoming_target, _loss_read_after_backward, _upcoming_grad_scale = self.prev
         return False
+
+
+# Gradient accumulation inside the two fused backward kernels (engine.GraphedTrainStep(accumulation_steps=k)).  On micro-batches 2..k
+# the engine sets every .grad to None and hands the buffers micro-batch 1 left back through `accumulate_into`: the fused nodes take
+# them as their destinations, launch their kernels in accumulate mode (g = g_old + v) and return them, and autograd adopts the sums
+# as fresh gradients — no AccumulateGrad add, and the optimizer rider's fresh-gradient checks hold on the last micro-batch.  A writer
+# that overwrites (the per-op kernels, the stand-alone conv2 weight gradient, the stand-alone classifier backward) never consults
+# this, so the engine arms it only when `fused_backward_params` shows that the fused kernels wrote every gradient of micro-batch 1.
+_accumulate: Optional[dict] = None     # {"grads": {id(param): buffer}, "loss": tensor the loss fold adds to, or None}
+_fused_backward_params: Optional[list] = None
+
+
+class accumulate_into:
+    """Inside this context the fused backward kernels add into ``grads`` ({parameter: buffer}) instead of writing fresh gradients,
+    and the deferred loss fold adds into ``loss``.  ``leftover()`` lists the parameters whose buffer no kernel took."""
+
+    def __init__(self, grads: dict, loss: Optional[torch.Tensor] = None):
+        self.state = {"grads": {id(p): g for p, g in grads.items()}, "loss": loss}
+        self.params = {id(p): p for p in grads}
+
+    def __enter__(self):
+        global _accumulate
+        self.prev, _accumulate = _accumulate, self.state
+        return self
+
+    def __exit__(self, *exc):
+        global _accumulate
+        _accumulate = self.prev
+        return False
+
+    def leftover(self) -> list:
+        return [self.params[i] for i in self.state["grads"]]
+
+
+def fused_backward_params() -> Optional[list]:
+    """The parameters whose gradients the last backward pass wrote through the two fused ConvNet backward kernels — all ten, the
+    classifier's and conv2's included — or None when that pass took any other writer.  Reset with ``reset_fused_backward_params``."""
+    return _fused_backward_params
+
+
+def reset_fused_backward_params() -> None:
+    global _fused_backward_params
+    _fused_backward_params = None
+
+
+def _take_accumulated(params) -> Optional[list]:
+    """Under ``accumulate_into``: the kept buffers of ``params`` (None entries stay None) as fresh aliases autograd may adopt, when
+    every one of them has one; None otherwise (nothing is taken)."""
+    acc = _accumulate
+    if acc is None or not all(p is None or id(p) in acc["grads"] for p in params):
+        return None
+    return [None if p is None else acc["grads"].pop(id(p)).detach().view(p.shape) for p in params]
 
 
 # The optimizer whose update rides on the last backward kernel (optim.SGD / optim.Adam .ride_on_backward, armed by
@@ -215,7 +276,7 @@ class _FusedLayer1(torch.autograd.Function):
             out, y, saved, p2, y2, saved2, logits, loss, dlogits, loss_parts = _C.convnet_fwd(
                 x, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, c2.weight, c2.bias, bn2.weight, bn2.bias,
                 bn2.running_mean, bn2.running_var, bn2.num_batches_tracked, float(bn2.momentum), float(bn2.eps), fc.weight, fc.bias,
-                whole.get("target"), defer)
+                whole.get("target"), defer, float(whole.get("grad_scale", 1.0)))
             whole["layer2"] = (p2, y2, saved2, logits)
             whole["ce"] = (loss, dlogits)
             whole["ce_deferred"] = (loss_parts, loss) if defer else None
@@ -228,19 +289,30 @@ class _FusedLayer1(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dp):
+        global _fused_backward_params
         x, y, saved, gamma, beta = ctx.saved_tensors
         w_p, b_p, g_p, be_p, w2_p, b2_p = ctx.params
-        dw = _grad_dst(w_p, w_p)
-        db = _grad_dst(b_p, b_p) if b_p is not None else None
-        dg = _grad_dst(g_p, gamma)
-        dbe = _grad_dst(be_p, beta)
+        pending = ctx.link.get("wgrad") if ctx.link is not None else None
+        # gradient accumulation (accumulate_into): the buffers of the earlier micro-batches, added to by the kernel
+        # (only when layer 2's kernel accumulated too)
+        acc = _take_accumulated((w_p, b_p, g_p, be_p, w2_p, b2_p)) if pending is not None and ctx.link.get("accumulated") else None
+        if acc is not None:
+            dw, db, dg, dbe = acc[:4]
+        else:
+            dw = _grad_dst(w_p, w_p)
+            db = _grad_dst(b_p, b_p) if b_p is not None else None
+            dg = _grad_dst(g_p, gamma)
+            dbe = _grad_dst(be_p, beta)
         fresh = all(q is None or q.grad is None for q in (w_p, b_p, g_p, be_p, w2_p, b2_p))
         pending = ctx.link.pop("wgrad", None) if ctx.link is not None else None
         dw2 = db2 = None
         if pending is not None:
             dy2, p1, dysum2 = pending   # dy2 = p1 = None: layer 2's kernel left the per-image partials
-            dw2 = _grad_dst(w2_p, w2_p)
-            db2 = _grad_dst(b2_p, b2_p) if b2_p is not None else None
+            if acc is not None:
+                dw2, db2 = acc[4:]
+            else:
+                dw2 = _grad_dst(w2_p, w2_p)
+                db2 = _grad_dst(b2_p, b2_p) if b2_p is not None else None
             sgd = None
             prev = ctx.link.pop("prev", None)
             rider = _sgd_rider if _sgd_rider_enabled else None
@@ -252,7 +324,11 @@ class _FusedLayer1(torch.autograd.Function):
                     grads = [q.grad if q is not None else None for q, _ in prev[:4]]
                     if all((g is None and ptr == 0) or (g is not None and g.data_ptr() == ptr) for g, (_, ptr) in zip(grads, prev[:4])):
                         sgd = rider["args"](grads)   # None when the optimizer cannot ride this iteration
-            _C.convnet_l1_bwd_wgrad(dp.contiguous(), y, x, saved, gamma, beta, dg, dbe, dw, db, dy2, p1, dysum2, dw2, db2, sgd)
+            _C.convnet_l1_bwd_wgrad(dp.contiguous(), y, x, saved, gamma, beta, dg, dbe, dw, db, dy2, p1, dysum2, dw2, db2, sgd,
+                                    accumulate=acc is not None)
+            prev = prev if prev is not None else ()
+            if len(prev) == 5 and prev[0][1] != 0:   # the classifier's gradient came from layer 2's kernel: all ten are the fused kernels'
+                _fused_backward_params = [w_p, b_p, g_p, be_p, w2_p, b2_p] + [q for q, _ in prev[:4]]
         else:
             _C.convnet_l1_bwd(dp.contiguous(), y, x, saved, gamma, beta, dg, dbe, dw, db)
         return None, dw, db, dg, dbe, None, None, None, None, None, dw2, db2, None, None
@@ -286,23 +362,36 @@ class _FusedLayer2(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout, dlogits):
         w_p, b_p, g_p, be_p, fcw_p, fcb_p = ctx.params
-        dg = _grad_dst(g_p, ctx.saved_tensors[3])
-        dbe = _grad_dst(be_p, ctx.saved_tensors[4])
-        dfcw = dfcb = None
-        if ctx.link is not None:   # do the gradients written here become `.grad` as they are (nothing to accumulate into)?
-            ctx.link["prev_fresh"] = ctx.fc_rides and all(q is None or q.grad is None for q in (fcw_p, fcb_p, g_p, be_p))
         # layer 1's backward kernel folds (and layer 1's node returns) conv2's weight / bias gradient; this kernel computes the
         # per-image partials (given p1) for it
         rides = ctx.link is not None and ctx.needs_input_grad[0]
+        # gradient accumulation (accumulate_into): this kernel and layer 1's add into the earlier micro-batches' buffers
+        acc = _take_accumulated((g_p, be_p, fcw_p, fcb_p)) if ctx.fc_rides and rides else None
+        if acc is not None:
+            ctx.link["accumulated"] = True
+            dg, dbe = acc[:2]
+        else:
+            dg = _grad_dst(g_p, ctx.saved_tensors[3])
+            dbe = _grad_dst(be_p, ctx.saved_tensors[4])
+        dfcw = dfcb = None
+        if ctx.link is not None:   # do the gradients written here become `.grad` as they are (nothing to accumulate into)?
+            ctx.link["prev_fresh"] = ctx.fc_rides and all(q is None or q.grad is None for q in (fcw_p, fcb_p, g_p, be_p))
         if ctx.fc_rides:
             p1, y, saved, gamma, beta, w, out, fcw = ctx.saved_tensors
             if dout is not None:
                 raise RuntimeError("fused ConvNet: the pooled activations of the fused classifier path must not be used outside the model")
-            dfcw = _grad_dst(fcw_p, fcw)
-            dfcb = _grad_dst(fcb_p, fcb_p) if fcb_p is not None else None
             lp, lo = ctx.ce_deferred if ctx.ce_deferred is not None else (None, None)
+            if acc is not None:
+                dfcw, dfcb = acc[2:]
+                if lp is not None:   # the step's loss adds up over the micro-batches too
+                    lo = _accumulate["loss"]
+                    if lo is None:
+                        raise RuntimeError("gradient accumulation: the deferred loss of this micro-batch has no buffer to add into")
+            else:
+                dfcw = _grad_dst(fcw_p, fcw)
+                dfcb = _grad_dst(fcb_p, fcb_p) if fcb_p is not None else None
             dy, dp1, dysum = _C.convnet_l2_bwd_fc(dlogits.contiguous(), fcw, out, dfcw, dfcb, y, saved, gamma, beta, w, dg, dbe, lp, lo,
-                                                  p1 if rides else None)
+                                                  p1 if rides else None, accumulate=acc is not None)
         else:
             p1, y, saved, gamma, beta, w = ctx.saved_tensors
             dy, dp1, dysum = _C.convnet_l2_bwd(dout.contiguous(), y, saved, gamma, beta, w, dg, dbe, p1 if rides else None)
@@ -353,6 +442,7 @@ def fused_convnet_forward(x: torch.Tensor, model) -> torch.Tensor:
                 and t.shape[0] == x.shape[0] and t.is_contiguous() and torch.is_grad_enabled()):
             whole["target"] = t
             whole["defer_loss_mean"] = bool(_loss_read_after_backward and fc_rides)
+            whole["grad_scale"] = _upcoming_grad_scale
     # conv2's weight gradient is produced by layer 1's backward kernel: layer 1's node owns (w2, b2) for autograd, `link` carries
     # the operands from layer 2's backward to it.  Only when conv1's parameters need gradients (layer 1's backward runs at all).
     link = {} if (_wgrad_rides_on_layer1() and c1.weight.requires_grad and c2.weight.requires_grad) else None
@@ -363,7 +453,8 @@ def fused_convnet_forward(x: torch.Tensor, model) -> torch.Tensor:
                                     b2_bn.num_batches_tracked, float(b2_bn.momentum), float(b2_bn.eps), fc.weight, fc.bias, whole, link, fc_rides)
     if whole is not None and whole.get("target") is not None:
         logits = logits if fc_rides else _FusedClassifier.apply(p2, fc.weight, fc.bias, logits)
-        logits._pdt_ce = (whole["target"],) + whole["ce"]   # (target, loss, dlogits) for ops.cross_entropy
+        # (target, loss, dlogits, scale of loss and gradient, loss folded by layer 2's backward kernel) for ops.cross_entropy
+        logits._pdt_ce = (whole["target"],) + whole["ce"] + (float(whole.get("grad_scale", 1.0)), whole["ce_deferred"] is not None)
         return logits
     if fc_rides:
         return logits
@@ -482,11 +573,29 @@ class _CrossEntropyPrecomputed(torch.autograd.Function):
         return grad0 * dloss, None, None
 
 
+_fused_ce_consumed: list = []   # the losses cross_entropy built from the forward kernel's cross-entropy (as id, scale)
+
+
+def reset_fused_ce_consumed() -> None:
+    _fused_ce_consumed.clear()
+
+
+def fused_ce_consumed() -> list:
+    """``(id(loss), scale)`` of every loss ``cross_entropy`` built from the forward kernel's cross-entropy since the last
+    ``reset_fused_ce_consumed``: a caller that wants the loss pre-scaled (``upcoming_targets(grad_scale=…)``) checks that its
+    criterion returned exactly one of them, unchanged."""
+    return list(_fused_ce_consumed)
+
+
 def cross_entropy(logits: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
     """Mean cross-entropy over the batch: fused log-softmax + NLL (ref: ddp_example.py:61,87)."""
     pre = getattr(logits, "_pdt_ce", None)
     if pre is not None and pre[0] is target:
-        return _CrossEntropyPrecomputed.apply(logits, pre[1], pre[2])
+        loss = _CrossEntropyPrecomputed.apply(logits, pre[1], pre[2])
+        loss._pdt_loss_scale = pre[3]   # upcoming_targets(grad_scale=…): the value and its gradient are grad_scale · the mean
+        loss._pdt_loss_deferred = pre[4]
+        _fused_ce_consumed.append((id(loss), pre[3]))
+        return loss
     return _CrossEntropy.apply(logits, target)
 
 
