@@ -29,7 +29,6 @@
 #include "wgrad_win.cuh"
 #include "cuda_utils.h"
 #include "grid_fold.cuh"
-#include "grid_sync.cuh"
 
 namespace pdt {
 
@@ -679,113 +678,6 @@ __global__ void __launch_bounds__(256) wgrad_fold_kernel(const float* __restrict
   }
 }
 
-// =====================================================================================================
-// conv2 weight gradient, fully TMA-fed ("window" formulation; used by the cooperative fused layers, whose activations
-// live in zero-haloed 18×18 frames):   dWᵀ[(kh, kw, ci)][co] = Σ_P  xpad[P + (kh−2)·18 + (kw−2)][ci] · dypad[P][co]
-// over the padded positions P of every image (dypad is zero outside the 14×14 interior, so the halo and the frame
-// padding contribute nothing).  Two horizontally adjacent taps of one pixel are 32 *contiguous* floats of the NHWC
-// frame, so the 32-row M atom of tap pair (kh, kw/2) is a row of an overlapping-row view of xpad (row pitch 64 B, row
-// length 128 B) read (kh−2)·18 + (kw−2) rows from the position: each image's view (384 rows) and its 256 dy positions
-// from the first interior one arrive as eight TMA boxes, and the 15 tap pairs (q = 3·kh + kw/2; pair (kh, 4-5) carries
-// a dummy sixth column) are computed by four warps with mma.sync (wgrad_win.cuh), accumulated over the CTA's images in
-// registers.  One CTA per image at most; per-CTA partial [512][32] (rows q·32 + (kw&1)·16 + ci); the bias gradient
-// comes from per-image Σdy rows (layer-2 backward).
-// =====================================================================================================
-struct WgradWinCfg {
-  static constexpr int kFrame = 18 * 18;              // padded positions per image
-  static constexpr int kFirst = 2 * 18 + 2;           // first interior position
-  static constexpr int kMRows = 512;
-  static constexpr int kABoxes = 6, kABytes = kABoxes * 64 * 128;   // overlapping-row view of one image, 64-row boxes
-  static constexpr int kBBytes = 2 * kTileM * 128;                   // dy at 256 positions
-  static constexpr int kThreads = 128;
-  static constexpr size_t kSmem = 1024 + kABytes + kBBytes + 1024;
-};
-
-__global__ void __launch_bounds__(128, 1) conv5x5_wgrad_win_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_dy,
-                                                                   float* __restrict__ partials, int B, const float* __restrict__ dysum,
-                                                                   float* __restrict__ dw, float* __restrict__ db, GridSync gs) {
-  using Cfg = WgradWinCfg;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sa = smem;
-  uint8_t* sb = sa + Cfg::kABytes;
-  uint64_t* ld_full = reinterpret_cast<uint64_t*>(sb + Cfg::kBBytes);
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  GridBar bar(gs);
-  if (tid == 0) {
-    tma_prefetch_desc(&tm_x);
-    tma_prefetch_desc(&tm_dy);
-    mbar_init(ld_full, 1);
-    fence_mbar_init();
-  }
-  __syncthreads();
-  float acc[4][2][4][4];   // warp w: tap pairs q = 4w .. 4w+3
-#pragma unroll
-  for (int a = 0; a < 4; ++a)
-#pragma unroll
-    for (int j = 0; j < 2; ++j)
-#pragma unroll
-      for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) acc[a][j][nt][e] = 0.f;
-  int it = 0;
-  for (int n = blockIdx.x; n < B; n += gridDim.x, ++it) {
-    if (tid == 0) {
-      const int frame0 = n * Cfg::kFrame;
-      mbar_arrive_expect_tx(ld_full, Cfg::kABytes + Cfg::kBBytes);
-      for (int bx = 0; bx < Cfg::kABoxes; ++bx) tma_load_2d(sa + bx * 8192, &tm_x, ld_full, 0, frame0 + 64 * bx);   // rows past the tensor are zero-filled
-      tma_load_2d(sb, &tm_dy, ld_full, 0, frame0 + Cfg::kFirst);
-      tma_load_2d(sb + kTileM * 128, &tm_dy, ld_full, 0, frame0 + Cfg::kFirst + kTileM);
-    }
-    mbar_wait(ld_full, it & 1);
-#pragma unroll
-    for (int a = 0; a < 4; ++a) {
-      const int q = warp * 4 + a, kh = q / 3, kw = 2 * (q - kh * 3);
-      if (q < 15) wgrad_win_atom(acc[a], reinterpret_cast<const float*>(sa), Cfg::kFirst + (kh - 2) * 18 + (kw - 2), 0,
-                                 reinterpret_cast<const float*>(sb), 0, lane);
-    }
-    __syncthreads();   // every warp is done with this image's tiles before the next loads overwrite them
-  }
-#pragma unroll
-  for (int a = 0; a < 4; ++a) {
-    const int q = warp * 4 + a;
-    if (q < 15) wgrad_win_atom_store(acc[a], partials + (static_cast<size_t>(blockIdx.x) * Cfg::kMRows + q * 32) * 32, lane);
-  }
-  if (dw == nullptr) return;   // per-CTA partials only, no fold
-  // ---- in-kernel fold (cooperative launch): after a grid barrier every CTA folds a share of the 400 × 32 outputs over the
-  //      per-CTA partials in a fixed order — thread = (co, one of six partial classes), classes combined through smem ----------
-  bar.sync(gs);
-  float* s_f = reinterpret_cast<float*>(smem);   // [4][32]
-  const int co = tid & 31, part = tid >> 5, nparts = gridDim.x;
-  for (int i = blockIdx.x; i < 401; i += gridDim.x) {
-    float acc = 0.f;
-    if (i < 400) {
-      const int tap = i >> 4, ci = i & 15, kh = tap / 5, kw = tap - kh * 5;
-      const int m = (3 * kh + (kw >> 1)) * 32 + (kw & 1) * 16 + ci;
-      const float* p = partials + static_cast<size_t>(m) * 32 + co;
-      const size_t stride = static_cast<size_t>(Cfg::kMRows) * 32;
-      for (int c = part; c < nparts; c += 32) {   // eight independent L2 loads in flight
-        float t[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) t[j] = (c + 4 * j < nparts) ? __ldcg(p + static_cast<size_t>(c + 4 * j) * stride) : 0.f;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc += t[j];
-      }
-    } else {
-      for (int n = part; n < B; n += 4) acc += __ldcg(dysum + static_cast<size_t>(n) * 32 + co);
-    }
-    __syncthreads();
-    s_f[part * 32 + co] = acc;
-    __syncthreads();
-    if (part == 0) {
-      const float tot = (s_f[co] + s_f[32 + co]) + (s_f[64 + co] + s_f[96 + co]);
-      if (i < 400) dw[(co * 16 + (i & 15)) * 25 + (i >> 4)] = tot;
-      else if (db) db[co] = tot;
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------
@@ -945,32 +837,6 @@ void launch_conv5x5_wgrad_mma(const float* dy, const float* x, float* dw, float*
   check_launch("conv5x5_wgrad_mma");
   wgrad_fold_kernel<<<401, 256, 0, st>>>(scr.partials, grid, dw, db);
   check_launch("wgrad_fold");
-}
-
-void make_wgrad_win_tmaps(const float* x_pad, const float* dy_pad, int B, CUtensorMap* tm_x, CUtensorMap* tm_dy) {
-  const uint64_t rows = static_cast<uint64_t>(B) * WgradWinCfg::kFrame;
-  // overlapping-row view of the haloed NHWC frames: row r = the 32 floats starting at position r (two adjacent pixels × 16 ch)
-  cuuint64_t dims[2] = {32, rows - 1};
-  cuuint64_t strides[1] = {64};
-  cuuint32_t box[2] = {32, 64};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = driver().cuTensorMapEncodeTiled(tm_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(x_pad), dims, strides, box, estr,
-                                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                               CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) throw std::runtime_error("cuTensorMapEncodeTiled(overlapping rows) failed: " + cu_error(r));
-  *tm_dy = make_tmap_2d(dy_pad, 32, rows, 32, kTileM, CU_TENSOR_MAP_SWIZZLE_128B);
-}
-
-void launch_conv5x5_wgrad_win(const float* dy_pad, const float* x_pad, const float* dysum, float* dw, float* db, int B, ReduceScratch scr,
-                              cudaStream_t st, GridSync gs) {
-  using Cfg = WgradWinCfg;
-  const int grid = std::min(B, sm_count());
-  if (static_cast<long long>(grid) * Cfg::kMRows * 32 > scr.capacity_floats) throw std::invalid_argument("conv5x5 wgrad (window): scratch too small");
-  CUtensorMap tm_x, tm_dy;
-  make_wgrad_win_tmaps(x_pad, dy_pad, B, &tm_x, &tm_dy);
-  // one CTA per SM at most: the fold happens after a grid barrier inside the kernel
-  launch_cooperative(conv5x5_wgrad_win_kernel, grid, Cfg::kThreads, Cfg::kSmem, st, "conv5x5_wgrad_win", tm_x, tm_dy, scr.partials, B, dysum,
-                     dw, db, gs);
 }
 
 void launch_gemm_tf32_wgmma(const float* a, const float* b, float* d, int M, int N, int K, cudaStream_t st) {

@@ -3,7 +3,6 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 
-#include "grid_sync.cuh"
 #include "ops_kernels.h"
 
 namespace pdt {
@@ -27,15 +26,6 @@ void launch_conv5x5_dgrad_im2col(const float* dy, const float* w, float* dx, Con
 // dw [32,16,5,5], db [32] (nullable) from dy NHWC [B,H,W,32] and x NHWC [B,H,W,16]: persistent split-K over
 // pixel tiles with MN-major operands (mma.sync), four register-resident accumulator tiles, deterministic fold of the per-CTA partials.
 void launch_conv5x5_wgrad_mma(const float* dy, const float* x, float* dw, float* db, ConvShape s, ReduceScratch scr, cudaStream_t st);
-
-// Tensor maps of the window weight gradient: tm_x = overlapping-row view of the x frame [B,18,18,16] (row pitch 64 B, row length
-// 128 B, box 64 rows), tm_dy = the dy frame [B,18,18,32] as rows of 32 floats (box 128 rows); both SWIZZLE_128B.
-void make_wgrad_win_tmaps(const float* x_pad, const float* dy_pad, int B, CUtensorMap* tm_x, CUtensorMap* tm_dy);
-// Window formulation for zero-haloed 18×18 frames (cooperative fused layers): dy_pad [B,18,18,32], x_pad [B,18,18,16], dysum [B,32]
-// (per-image Σdy rows, folded into db).  All operands arrive by TMA: no im2col gather.  One cooperative launch: the per-CTA
-// partials are folded after the grid barrier gs.
-void launch_conv5x5_wgrad_win(const float* dy_pad, const float* x_pad, const float* dysum, float* dw, float* db, int B, ReduceScratch scr,
-                              cudaStream_t st, GridSync gs);
 
 // D[M,N] = A[M,K] · B[N,K]^T, fp32 in/out, TF32 tensor-core math (K % 4 == 0, N % 16 == 0, N <= 256).
 void launch_gemm_tf32_wgmma(const float* a, const float* b, float* d, int M, int N, int K, cudaStream_t st);

@@ -220,41 +220,6 @@ void register_cuda_bindings(py::module_& m) {
     fused_convnet_trace_read(reinterpret_cast<unsigned long long*>(t.data_ptr<int64_t>()));
     return t;
   });
-  m.def("convnet_l1_fwd", [](const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> bias, c10::optional<at::Tensor> gamma,
-                             c10::optional<at::Tensor> beta, c10::optional<at::Tensor> running_mean, c10::optional<at::Tensor> running_var,
-                             c10::optional<at::Tensor> nbt, double momentum, double eps) {
-    chk(x, "x"); chk(w, "w");
-    c10::cuda::CUDAGuard g(x.device());
-    TORCH_CHECK(x.numel() % 784 == 0 && w.numel() == 400, "convnet_l1_fwd: x [B,1,28,28] and w [16,1,5,5] expected");
-    const int B = static_cast<int>(x.numel() / 784);
-    TORCH_CHECK(fused_convnet_supported(B), "convnet_l1_fwd: batch ", B, " exceeds one CTA per SM");
-    at::Tensor y = at::empty({B, 28, 28, 16}, x.options());
-    at::Tensor out = at::empty({B, 18, 18, 16}, x.options());   // zero-haloed frame
-    at::Tensor saved = at::empty({32}, x.options());
-    long long* nbt_p = nullptr;
-    if (nbt.has_value() && nbt->defined()) { chk(*nbt, "num_batches_tracked", at::kLong); nbt_p = reinterpret_cast<long long*>(nbt->data_ptr<int64_t>()); }
-    ReduceScratch scr = scratch(x);
-    TORCH_CHECK(static_cast<long long>(B) * 512 <= scr.capacity_floats, "fused convnet: reduction scratch too small");
-    launch_convnet_l1_fwd(x.data_ptr<float>(), w.data_ptr<float>(), opt_ptr(bias, "bias"), opt_ptr(gamma, "gamma"), opt_ptr(beta, "beta"),
-                          y.data_ptr<float>(), out.data_ptr<float>(), saved.data_ptr<float>(), opt_mut(running_mean, "running_mean"),
-                          opt_mut(running_var, "running_var"), nbt_p, static_cast<float>(momentum), static_cast<float>(eps), B, scr.partials,
-                          grid_sync(scr), cur_stream(x));
-    return py::make_tuple(out, y, saved);
-  });
-  m.def("convnet_l1_bwd", [](const at::Tensor& dp, const at::Tensor& y, const at::Tensor& x, const at::Tensor& saved,
-                             c10::optional<at::Tensor> gamma, c10::optional<at::Tensor> beta, at::Tensor dgamma, at::Tensor dbeta, at::Tensor dw,
-                             c10::optional<at::Tensor> db) {
-    chk(dp, "dp"); chk(y, "y"); chk(x, "x"); chk(saved, "saved"); chk(dgamma, "dgamma"); chk(dbeta, "dbeta"); chk(dw, "dw");
-    c10::cuda::CUDAGuard g(x.device());
-    const int B = static_cast<int>(y.size(0));
-    TORCH_CHECK(dp.numel() == static_cast<int64_t>(B) * 5184 && x.numel() == static_cast<int64_t>(B) * 784 && dw.numel() == 400 &&
-                    dgamma.numel() == 16 && dbeta.numel() == 16, "convnet_l1_bwd: shape mismatch");
-    ReduceScratch scr = scratch(x);
-    launch_convnet_l1_bwd(dp.data_ptr<float>(), y.data_ptr<float>(), x.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"),
-                          opt_ptr(beta, "beta"), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"), B,
-                          scr.partials, scr.partials + static_cast<size_t>(B) * 64,
-                          grid_sync(scr), cur_stream(x));
-  });
   m.def("convnet_l1_bwd_wgrad", [](const at::Tensor& dp, const at::Tensor& y, const at::Tensor& x, const at::Tensor& saved,
                                    c10::optional<at::Tensor> gamma, c10::optional<at::Tensor> beta, at::Tensor dgamma, at::Tensor dbeta, at::Tensor dw,
                                    c10::optional<at::Tensor> db, c10::optional<at::Tensor> dy2_pad, c10::optional<at::Tensor> x2_pad,
@@ -266,7 +231,8 @@ void register_cuda_bindings(py::module_& m) {
     TORCH_CHECK(dp.numel() == static_cast<int64_t>(B) * 5184 && x.numel() == static_cast<int64_t>(B) * 784 && dw.numel() == 400 &&
                     dgamma.numel() == 16 && dbeta.numel() == 16, "convnet_l1_bwd_wgrad: layer-1 shape mismatch");
     TORCH_CHECK(dysum2.numel() == static_cast<int64_t>(B) * 32 && dw2.numel() == 12800, "convnet_l1_bwd_wgrad: layer-2 shape mismatch");
-    // conv2's per-image weight-gradient partials: from the given frames, or (both None) left by convnet_l2_bwd(_fc)(…, p1) of this batch
+    // conv2's per-image weight-gradient partials: from the given frames (the tests' reference), or (both None) left by
+    // convnet_l2_bwd_fc(…, p1) of this batch
     const bool frames = dy2_pad.has_value() && dy2_pad->defined();
     TORCH_CHECK(frames == (x2_pad.has_value() && x2_pad->defined()), "convnet_l1_bwd_wgrad: dy2_pad and x2_pad are given together or not at all");
     float* wpart = conv2_wgrad_partials(x, B, "convnet_l1_bwd_wgrad");
@@ -276,7 +242,7 @@ void register_cuda_bindings(py::module_& m) {
       TORCH_CHECK(dy2_pad->numel() == static_cast<int64_t>(B) * 324 * 32 && x2_pad->numel() == static_cast<int64_t>(B) * 324 * 16,
                   "convnet_l1_bwd_wgrad: layer-2 frame shape mismatch");
     } else {
-      TORCH_CHECK(entry.wgrad_batch == B, "convnet_l1_bwd_wgrad: without dy2_pad / x2_pad it folds the partials of convnet_l2_bwd(_fc)(…, p1) "
+      TORCH_CHECK(entry.wgrad_batch == B, "convnet_l1_bwd_wgrad: without dy2_pad / x2_pad it folds the partials of convnet_l2_bwd_fc(…, p1) "
                   "of the same batch, and none are pending");
     }
     // sgd = (params[10], prev_grads[4], momentum_bufs[10] or [], lr, lr_tensor, momentum, dampening, weight_decay, nesterov, maximize, first_step):
@@ -403,38 +369,6 @@ void register_cuda_bindings(py::module_& m) {
   }, py::arg("dp"), py::arg("y"), py::arg("x"), py::arg("saved"), py::arg("gamma"), py::arg("beta"), py::arg("dgamma"), py::arg("dbeta"),
      py::arg("dw"), py::arg("db"), py::arg("dy2_pad"), py::arg("x2_pad"), py::arg("dysum2"), py::arg("dw2"), py::arg("db2"),
      py::arg("sgd") = py::none(), py::arg("accumulate") = false);
-  m.def("convnet_l2_fwd", [](const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> bias, c10::optional<at::Tensor> gamma,
-                             c10::optional<at::Tensor> beta, c10::optional<at::Tensor> running_mean, c10::optional<at::Tensor> running_var,
-                             c10::optional<at::Tensor> nbt, double momentum, double eps, c10::optional<at::Tensor> fcw,
-                             c10::optional<at::Tensor> fcb) {
-    chk(x, "x"); chk(w, "w");
-    c10::cuda::CUDAGuard g(x.device());
-    TORCH_CHECK(x.dim() == 4 && x.size(1) == 18 && x.size(2) == 18 && x.size(3) == 16 && w.numel() == 12800,
-                "convnet_l2_fwd: x [B,18,18,16] (zero-haloed NHWC frame) and w [32,16,5,5] expected");
-    const int B = static_cast<int>(x.size(0));
-    TORCH_CHECK(fused_convnet_supported(B), "convnet_l2_fwd: batch ", B, " exceeds one CTA per SM");
-    at::Tensor y = at::empty({B, 14, 14, 32}, x.options());
-    at::Tensor out = at::empty({B, 32, 7, 7}, x.options());
-    at::Tensor saved = at::empty({64}, x.options());
-    at::Tensor logits;
-    int ncls = 0;
-    if (fcw.has_value() && fcw->defined()) {
-      chk(*fcw, "fc weight");
-      TORCH_CHECK(fcw->dim() == 2 && fcw->size(1) == 1568, "convnet_l2_fwd: fc weight [classes, 1568] expected");
-      ncls = static_cast<int>(fcw->size(0));
-      logits = at::empty({B, ncls}, x.options());
-    }
-    long long* nbt_p = nullptr;
-    if (nbt.has_value() && nbt->defined()) { chk(*nbt, "num_batches_tracked", at::kLong); nbt_p = reinterpret_cast<long long*>(nbt->data_ptr<int64_t>()); }
-    ReduceScratch scr = scratch(x);
-    launch_convnet_l2_fwd(x.data_ptr<float>(), w.data_ptr<float>(), opt_ptr(bias, "bias"), opt_ptr(gamma, "gamma"), opt_ptr(beta, "beta"),
-                          y.data_ptr<float>(), out.data_ptr<float>(), saved.data_ptr<float>(), opt_mut(running_mean, "running_mean"),
-                          opt_mut(running_var, "running_var"), nbt_p, static_cast<float>(momentum), static_cast<float>(eps),
-                          ncls ? fcw->data_ptr<float>() : nullptr, ncls ? opt_ptr(fcb, "fc bias") : nullptr,
-                          ncls ? logits.data_ptr<float>() : nullptr, ncls, B, scr.partials,
-                          grid_sync(scr), cur_stream(x));
-    return py::make_tuple(out, y, saved, logits);
-  });
   m.def("convnet_fwd", [](const at::Tensor& x, const at::Tensor& w1, c10::optional<at::Tensor> b1, c10::optional<at::Tensor> g1,
                           c10::optional<at::Tensor> be1, c10::optional<at::Tensor> rm1, c10::optional<at::Tensor> rv1, c10::optional<at::Tensor> nbt1,
                           double mom1, double eps1, const at::Tensor& w2, c10::optional<at::Tensor> b2, c10::optional<at::Tensor> g2,
@@ -485,27 +419,8 @@ void register_cuda_bindings(py::module_& m) {
      py::arg("eps2"), py::arg("fcw"), py::arg("fcb"), py::arg("target") = py::none(), py::arg("defer_loss_mean") = false,
      py::arg("grad_scale") = 1.0);
   // p1 (conv2's input frame [B,18,18,16], optional): conv2's per-image weight-gradient partials are computed inside the kernel for
-  // convnet_l1_bwd_wgrad(…, None, None, …) to fold, and the dy frame is not written (None in its place).
-  m.def("convnet_l2_bwd", [](const at::Tensor& dout, const at::Tensor& y, const at::Tensor& saved, c10::optional<at::Tensor> gamma,
-                             c10::optional<at::Tensor> beta, const at::Tensor& w, at::Tensor dgamma, at::Tensor dbeta, c10::optional<at::Tensor> p1) {
-    chk(dout, "dout"); chk(y, "y"); chk(saved, "saved"); chk(w, "w"); chk(dgamma, "dgamma"); chk(dbeta, "dbeta");
-    c10::cuda::CUDAGuard g(y.device());
-    const int B = static_cast<int>(y.size(0));
-    TORCH_CHECK(dout.numel() == static_cast<int64_t>(B) * 1568 && y.numel() == static_cast<int64_t>(B) * 6272 && w.numel() == 12800 &&
-                    dgamma.numel() == 32 && dbeta.numel() == 32, "convnet_l2_bwd: shape mismatch");
-    const float* x2 = conv2_input(p1, B, "convnet_l2_bwd");
-    at::Tensor dy = x2 ? at::Tensor() : at::empty({B, 18, 18, 32}, y.options());
-    at::Tensor dx = at::empty({B, 18, 18, 16}, y.options());
-    at::Tensor dysum = at::empty({B, 32}, y.options());
-    ReduceScratch scr = scratch(y);
-    float* wpart = x2 ? conv2_wgrad_partials(y, B, "convnet_l2_bwd") : nullptr;
-    launch_convnet_l2_bwd(dout.data_ptr<float>(), y.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"), opt_ptr(beta, "beta"),
-                          w.data_ptr<float>(), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), x2 ? nullptr : dy.data_ptr<float>(), dx.data_ptr<float>(),
-                          dysum.data_ptr<float>(), B, scr.partials, grid_sync(scr), cur_stream(y), x2, wpart);
-    if (x2) scratch_entry(y).wgrad_batch = B;
-    return py::make_tuple(x2 ? py::none() : py::cast(dy), dx, dysum);
-  }, py::arg("dout"), py::arg("y"), py::arg("saved"), py::arg("gamma"), py::arg("beta"), py::arg("w"), py::arg("dgamma"), py::arg("dbeta"),
-     py::arg("p1") = py::none());
+  // convnet_l1_bwd_wgrad(…, None, None, …) to fold, and the dy frame is not written (None in its place).  The training step always
+  // passes p1; the dy frame of the form without it, fed to convnet_l1_bwd_wgrad, is the tests' reference for those partials.
   m.def("convnet_l2_bwd_fc", [](const at::Tensor& dlogits, const at::Tensor& fcw, const at::Tensor& pooled, at::Tensor dfcw, c10::optional<at::Tensor> dfcb,
                                 const at::Tensor& y, const at::Tensor& saved, c10::optional<at::Tensor> gamma, c10::optional<at::Tensor> beta,
                                 const at::Tensor& w, at::Tensor dgamma, at::Tensor dbeta, c10::optional<at::Tensor> loss_parts,
@@ -539,17 +454,6 @@ void register_cuda_bindings(py::module_& m) {
   }, py::arg("dlogits"), py::arg("fcw"), py::arg("pooled"), py::arg("dfcw"), py::arg("dfcb"), py::arg("y"), py::arg("saved"), py::arg("gamma"),
      py::arg("beta"), py::arg("w"), py::arg("dgamma"), py::arg("dbeta"), py::arg("loss_parts") = py::none(), py::arg("loss_out") = py::none(),
      py::arg("p1") = py::none(), py::arg("accumulate") = false);
-  m.def("conv5x5_wgrad_win", [](const at::Tensor& dy_pad, const at::Tensor& x_pad, const at::Tensor& dysum, at::Tensor dw, c10::optional<at::Tensor> db) {
-    chk(dy_pad, "dy_pad"); chk(x_pad, "x_pad"); chk(dysum, "dysum"); chk(dw, "dw");
-    c10::cuda::CUDAGuard g(dy_pad.device());
-    const int B = static_cast<int>(dy_pad.size(0));
-    TORCH_CHECK(dy_pad.numel() == static_cast<int64_t>(B) * 324 * 32 && x_pad.numel() == static_cast<int64_t>(B) * 324 * 16 &&
-                    dysum.numel() == static_cast<int64_t>(B) * 32 && dw.numel() == 12800, "conv5x5_wgrad_win: shape mismatch");
-    ReduceScratch scr = scratch(dy_pad);
-    launch_conv5x5_wgrad_win(dy_pad.data_ptr<float>(), x_pad.data_ptr<float>(), dysum.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"), B,
-                             scr, cur_stream(dy_pad), grid_sync(scr));
-  }, py::arg("dy_pad"), py::arg("x_pad"), py::arg("dysum"), py::arg("dw"), py::arg("db") = py::none());
-
   // ---- BN + ReLU + pool ------------------------------------------------------------------------------
   m.def("bn_relu_pool_fwd", [](const at::Tensor& y, const at::Tensor& stats, c10::optional<at::Tensor> gamma, c10::optional<at::Tensor> beta,
                                c10::optional<at::Tensor> running_mean, c10::optional<at::Tensor> running_var,

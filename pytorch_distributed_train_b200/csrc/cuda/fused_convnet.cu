@@ -10,15 +10,12 @@
 //                              swizzled smem patch ── conv2 5x5 (16→32) on wgmma (the 25 taps are row-shifted descriptors
 //                              into that patch; accumulators in registers) ──barrier── BN + ReLU + MaxPool2 + classifier
 //                              (+ cross-entropy term and d(loss)/d(logits) when the targets are known)           (ref :25-34,40)
-//   convnet_l2_bwd_kernel<FC, WG>  classifier backward + MaxPool/ReLU/BN backward ──barrier (Σdz, Σdz·x̂)── dy → conv2 data
+//   convnet_l2_bwd_kernel<WG>  classifier backward + MaxPool/ReLU/BN backward ──barrier (Σdz, Σdz·x̂)── dy → conv2 data
 //                              gradient on wgmma (warps 4..7), next to it conv2's weight-gradient partial of the image on
 //                              wgmma (warps 0..3; K-major copies of x, written in the barrier's shadow, and of dy)
-//   convnet_l1_bwd_kernel<WG>  MaxPool/ReLU/BN backward ──barrier── conv1 weight gradient (mma.sync) ──barrier── conv1 fold;
+//   convnet_l1_bwd_kernel      MaxPool/ReLU/BN backward ──barrier── conv1 weight gradient (mma.sync) ──barrier── conv1 fold;
 //                              conv2's weight gradient is folded in the shadow of the first barrier, and — on one GPU — the
 //                              threads that write the folded gradients apply the optimizer update (SgdRider / AdamRider)
-//
-// convnet_l1_fwd_kernel / convnet_l2_fwd_kernel (one kernel per layer) and the <false> instantiations are the variants without
-// the riders (PDT_FUSED_WHOLE_FWD / PDT_FC_MERGED / PDT_WGRAD_MERGED = 0); all of them are exercised by tests/test_gpu_kernels.py.
 //
 // All cross-CTA sums are "every CTA writes one partial row, barrier, every CTA folds the rows in the same fixed order",
 // so results are bit-reproducible and identical in every CTA.  The kernels are launched cooperatively (all CTAs
@@ -47,6 +44,7 @@ namespace {
 using namespace ptx;
 
 // ---- optional phase trace (PDT_FUSED_TRACE=1): globaltimer stamps of thread 0 of every CTA, read back by tools ----------
+// Kernel slots: 0 forward, 1 layer-1 backward, 3 layer-2 backward (slot 2 is unused).
 __device__ unsigned long long g_trace[4][160][12];
 __device__ int g_trace_on = 0;
 // The switch is read ONCE per kernel (TRACE_INIT, one global load whose latency overlaps the prologue); a stamp is then a predicated
@@ -156,124 +154,6 @@ __device__ __forceinline__ void l1_load_image(const float* __restrict__ x, float
     const int rr = tid / 28, cc = tid - rr * 28;
     xs[(rr + 2) * 32 + cc + 2] = x[tid];
   }
-}
-
-__global__ void __launch_bounds__(kL1Threads, 1)
-convnet_l1_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
-                      const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ y, float* __restrict__ out,
-                      float* saved, float* running_mean, float* running_var, long long* nbt, float momentum, float eps,
-                      float* partials, GridSync gs) {
-  __shared__ float xs[32 * 32];
-  __shared__ __align__(16) float ws[25 * 16];
-  __shared__ float red[kL1Warps * 32];
-  __shared__ float s_tmp[4 * 32];
-  __shared__ float s_tot[32];
-  __shared__ float s_scale[16], s_shift[16];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = blockIdx.x, B = gridDim.x;
-  const L1Map m(tid);
-  GridBar bar(gs);
-  TRACE_INIT();
-  trace(0, 0);
-
-  l1_load_image(x + static_cast<size_t>(n) * 784, xs, tid);
-  if (tid < 400) {
-    const int tap = tid >> 4, co = tid & 15;
-    ws[tid] = w[co * 25 + tap];
-  }
-  __syncthreads();
-
-  float acc[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) acc[j] = bias ? __ldg(bias + j) : 0.f;
-#pragma unroll 1
-  for (int kh = 0; kh < 5; ++kh) {
-#pragma unroll
-    for (int kw = 0; kw < 5; ++kw) {
-      const float xv = xs[(m.r + kh) * 32 + m.c + kw];
-      const float4* wt = reinterpret_cast<const float4*>(ws + (kh * 5 + kw) * 16);
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float4 wv = wt[q];
-        acc[4 * q + 0] = fmaf(xv, wv.x, acc[4 * q + 0]);
-        acc[4 * q + 1] = fmaf(xv, wv.y, acc[4 * q + 1]);
-        acc[4 * q + 2] = fmaf(xv, wv.z, acc[4 * q + 2]);
-        acc[4 * q + 3] = fmaf(xv, wv.w, acc[4 * q + 3]);
-      }
-    }
-  }
-  trace(0, 1);
-  {
-    float v[32];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      v[j] = m.valid ? acc[j] : 0.f;
-      v[16 + j] = m.valid ? acc[j] * acc[j] : 0.f;
-    }
-    warp_transpose_reduce32(v, lane);
-    red[warp * 32 + lane] = v[0];
-  }
-  __syncthreads();
-  if (tid < 32) {
-    float s = 0.f;
-#pragma unroll 5
-    for (int wi = 0; wi < kL1Warps; ++wi) s += red[wi * 32 + tid];
-    partials[static_cast<size_t>(n) * 32 + tid] = s;
-  }
-  trace(0, 2);
-  bar.sync(gs);
-  trace(0, 3);
-  fold_rows<32>(partials, B, s_tmp, s_tot);
-  trace(0, 4);
-  if (tid < 16) {
-    const float cnt = static_cast<float>(B) * 784.f;
-    const float mean = s_tot[tid] / cnt;
-    const float var = fmaxf(s_tot[16 + tid] / cnt - mean * mean, 0.f);
-    const float invstd = rsqrtf(var + eps);
-    const float g = gamma ? gamma[tid] : 1.f, b = beta ? beta[tid] : 0.f;
-    s_scale[tid] = g * invstd;
-    s_shift[tid] = b - mean * g * invstd;
-    if (n == 0) {
-      saved[tid] = mean;
-      saved[16 + tid] = invstd;
-      if (running_mean) {
-        const float unbiased = var * (cnt / fmaxf(cnt - 1.f, 1.f));
-        running_mean[tid] = (1.f - momentum) * running_mean[tid] + momentum * mean;
-        running_var[tid] = (1.f - momentum) * running_var[tid] + momentum * unbiased;
-      }
-      if (nbt && tid == 0) *nbt += 1;
-    }
-  }
-  __syncthreads();
-  float z[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    float t = fmaxf(fmaf(acc[j], s_scale[j], s_shift[j]), 0.f);
-    t = fmaxf(t, __shfl_xor_sync(0xffffffffu, t, 1));
-    t = fmaxf(t, __shfl_xor_sync(0xffffffffu, t, 2));
-    z[j] = t;
-  }
-  if (m.valid) {  // lane d of the window writes channels 4d..4d+3: one 64-byte row per window
-    float4 o;
-    if (m.d == 0) o = make_float4(z[0], z[1], z[2], z[3]);
-    else if (m.d == 1) o = make_float4(z[4], z[5], z[6], z[7]);
-    else if (m.d == 2) o = make_float4(z[8], z[9], z[10], z[11]);
-    else o = make_float4(z[12], z[13], z[14], z[15]);
-    reinterpret_cast<float4*>(out + ((static_cast<size_t>(n) * 18 + m.ph + 2) * 18 + m.pw + 2) * 16)[m.d] = o;
-  }
-  // the 2-position halo of the frame is zero: layer 2 reads it as the convolution's zero padding (forward: one TMA box
-  // per image; weight gradient: overlapping-row TMA view), so nobody has to special-case the image border
-  for (int i = tid; i < 324 * 4; i += kL1Threads) {
-    const int P = i >> 2, pr = P / 18, pc = P - pr * 18;
-    if (pr < 2 || pr >= 16 || pc < 2 || pc >= 16) reinterpret_cast<float4*>(out + (static_cast<size_t>(n) * 324 + P) * 16)[i & 3] = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-  if (m.valid) {  // conv output is kept for the backward pass (BatchNorm needs x̂ at every position); stored last: nothing
-                  // in this kernel waits for these 50 KB per CTA, least of all the fence in front of the grid barrier
-    float4* yp = reinterpret_cast<float4*>(y + ((static_cast<size_t>(n) * 28 + m.r) * 28 + m.c) * 16);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) yp[q] = make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
-  }
-  bar.finish(gs);
-  trace(0, 5);
 }
 
 // ---- layer 1 backward (+ the fold of conv2's weight gradient riding along) ---------------------------------------------------
@@ -477,18 +357,16 @@ __device__ __forceinline__ float clip_comb(const R& r, float a, float b) { retur
 
 // ACC (accumulate mode, gradient accumulation over micro-batches): every gradient this kernel writes — dgamma, dbeta, the conv1 fold
 // dw / db and the conv2 fold dw2 / db2 — becomes g = g_old + v, and the rider updates with (and clips) that accumulated value.
-template <bool WG, class Rider = SgdRider, bool ACC = false>
+template <class Rider = SgdRider, bool ACC = false>
 __global__ void __launch_bounds__(kL1Threads, 1)
 convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y, const float* __restrict__ x, const float* __restrict__ saved,
                       const float* __restrict__ gamma, const float* __restrict__ beta, float* dgamma, float* dbeta, float* dw, float* db,
                       float* partials, float* partials_w, GridSync gs,
-                      // WG only: conv2's weight gradient, folded from the per-image partials [B][400][32] and Σdy rows [B][32]
+                      // conv2's weight gradient, folded from the per-image partials [B][400][32] and Σdy rows [B][32]
                       const float* __restrict__ wpart, const float* __restrict__ dysum2, float* dw2, float* db2, const __grid_constant__ Rider sr) {
   constexpr bool kClip = std::is_same_v<Rider, ClipRider<SgdRider>> || std::is_same_v<Rider, ClipRider<AdamRider>>;
   constexpr bool kAdam = std::is_same_v<Rider, AdamRider> || std::is_same_v<Rider, ClipRider<AdamRider>>;
   static_assert(kAdam || std::is_base_of_v<SgdRider, Rider>, "convnet_l1_bwd_kernel: SgdRider or AdamRider, or either in a ClipRider");
-  static_assert(WG || !(kAdam || kClip), "the Adam and clipping riders ride on the kernel with the conv2 weight gradient");
-  static_assert(WG || !ACC, "accumulate mode is a variant of the kernel with the conv2 weight gradient");
   extern __shared__ __align__(16) float dsm[];
   float* dys = dsm;                  // [784][16]
   float* fold = dsm + 784 * 16;      // [25 warps][16][32]
@@ -592,7 +470,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
         if constexpr (kAdam) adam_apply(sr, 6 + t, i, __ldg(sr.g_prev[t] + i), adam_f);
         else sgd_apply(sr.p[6 + t] + i, __ldg(sr.g_prev[t] + i), sr.m[6 + t] ? sr.m[6 + t] + i : nullptr, sr.h, sgd_lr);
   }
-  if constexpr (WG) {
+  {
     // in the barrier's shadow: conv2's weight gradient, complete before this kernel started (the layer-2 backward kernel wrote the
     // per-image partials), and its optimizer step — nothing in this kernel reads conv2's parameters.  CTA n folds outputs n, n + B,
     // … of the 400 (tap, ci) rows × 32 co (+ row 400: the bias, from the per-image Σdy rows) over the B per-image partials [400][32],
@@ -942,184 +820,6 @@ struct L2FwdSmem {
   static constexpr int kTotal = 1024 + kPatchAlloc + kB + kYs + 8192;
 };
 
-__global__ void __launch_bounds__(kL2Threads, 1)
-convnet_l2_fwd_kernel(const __grid_constant__ CUtensorMap tm_x, const float* __restrict__ w, const float* __restrict__ bias,
-                      const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ y, float* __restrict__ out,
-                      float* saved, float* running_mean, float* running_var, long long* nbt, float momentum, float eps,
-                      const float* __restrict__ fcw, const float* __restrict__ fcb, float* __restrict__ logits, int ncls,
-                      float* partials, GridSync gs) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sa = smem;                                  // input patch (TMA, SWIZZLE_128B)
-  uint8_t* sb = sa + kPatchAlloc;                      // weights
-  float* ys = reinterpret_cast<float*>(sb + L2FwdSmem::kB);
-  float* misc = ys + 196 * 32;                         // 2048 floats
-  float* s_part = misc;                                // [4][64]
-  float* s_tmp = misc + 256;                           // [4][64]
-  float* s_tot = misc + 512;                           // [64]
-  float* s_scale = misc + 576;                         // [32]
-  float* s_shift = misc + 608;                         // [32]
-
-  __shared__ uint64_t bar_x;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = blockIdx.x, B = gridDim.x;
-
-  GridBar bar(gs);
-  TRACE_INIT();
-  trace(2, 0);
-  if (tid == 0) {
-    tma_prefetch_desc(&tm_x);
-    mbar_init(&bar_x, 1);
-    fence_mbar_init();
-  }
-  // zero the slack behind the patch (read only by padding rows, but keep NaNs out of the accumulators)
-  for (int i = tid; i < (kPatchAlloc - kPatchBytes) / 16; i += kL2Threads) reinterpret_cast<float4*>(sa + kPatchBytes)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  fence_proxy_async_smem();
-  __syncthreads();
-  if (tid == 0) {
-    mbar_arrive_expect_tx(&bar_x, kPatchBytes);
-    tma_load_4d(sa, &tm_x, &bar_x, 0, 0, 0, n);        // the frame carries its zero halo; channels ≥ 16: out-of-bounds zero fill
-  }
-  // B[tap][co][ci] = w[co][ci][tap], K-major rows of 128 B, SWIZZLE_128B
-  {
-    // thread = two (co, ci) pairs; a pair's 25 taps are contiguous in w (a warp reads 3,200 contiguous bytes) and land
-    // 4,096 B apart in smem (one swizzled K-major tile per tap): all 50 loads are in flight before the first store
-    float wv[2][25];
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      const float* src = w + (tid + j * kL2Threads) * 25;
-#pragma unroll
-      for (int tap = 0; tap < 25; ++tap) wv[j][tap] = __ldg(src + tap);
-    }
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      const int pair = tid + j * kL2Threads, co = pair >> 4, ci = pair & 15;
-      uint8_t* dst = sb + sw128_off(co, ci >> 2) + (ci & 3) * 4;
-#pragma unroll
-      for (int tap = 0; tap < 25; ++tap) *reinterpret_cast<float*>(dst + tap * 4096) = wv[j][tap];
-    }
-  }
-  fence_proxy_async_smem();   // generic-proxy writes of B → visible to the tensor core
-  __syncthreads();
-  trace(2, 1);
-  // ---- conv2 + epilogue: the warpgroup of warps 4..7 ------------------------------------------------------------------------
-  if (warpgroup_index() == 1) {
-    mbar_wait(&bar_x, 0);
-    l2_conv_wgmma(sa, sb, bias, ys, tid - 128);
-  }
-  __syncthreads();
-  trace(2, 2);
-  // ---- per-channel Σy, Σy² of this image: thread = (channel, quarter of the pixels) --------------------------------------
-  if (tid < 128) {
-    const int c = tid & 31, part = tid >> 5;
-    float s1 = 0.f, s2 = 0.f;
-    for (int p = part * 49; p < part * 49 + 49; ++p) {
-      const float val = ys[p * 32 + ((((c >> 2) + p) & 7) << 2) + (c & 3)];
-      s1 += val;
-      s2 = fmaf(val, val, s2);
-    }
-    s_part[part * 64 + c] = s1;
-    s_part[part * 64 + 32 + c] = s2;
-  }
-  __syncthreads();
-  if (tid < 64) partials[static_cast<size_t>(n) * 64 + tid] = (s_part[tid] + s_part[64 + tid]) + (s_part[128 + tid] + s_part[192 + tid]);
-  trace(2, 3);
-  bar.sync(gs);
-  trace(2, 4);
-  // conv output → global (kept for backward), after the barrier: un-rotate the 16-byte chunks on the way out
-  for (int i = tid; i < 196 * 8; i += kL2Threads) {
-    const int pix = i >> 3, q = i & 7;
-    reinterpret_cast<float4*>(y + (static_cast<size_t>(n) * 196 + pix) * 32)[q] = reinterpret_cast<const float4*>(ys + pix * 32)[(q + pix) & 7];
-  }
-  fold_rows<64>(partials, B, s_tmp, s_tot);
-  trace(2, 5);
-  if (tid < 32) {
-    const float cnt = static_cast<float>(B) * 196.f;
-    const float mean = s_tot[tid] / cnt;
-    const float var = fmaxf(s_tot[32 + tid] / cnt - mean * mean, 0.f);
-    const float invstd = rsqrtf(var + eps);
-    const float g = gamma ? gamma[tid] : 1.f, b = beta ? beta[tid] : 0.f;
-    s_scale[tid] = g * invstd;
-    s_shift[tid] = b - mean * g * invstd;
-    if (n == 0) {
-      saved[tid] = mean;
-      saved[32 + tid] = invstd;
-      if (running_mean) {
-        const float unbiased = var * (cnt / fmaxf(cnt - 1.f, 1.f));
-        running_mean[tid] = (1.f - momentum) * running_mean[tid] + momentum * mean;
-        running_var[tid] = (1.f - momentum) * running_var[tid] + momentum * unbiased;
-      }
-      if (nbt && tid == 0) *nbt += 1;
-    }
-  }
-  __syncthreads();
-  // ---- BN + ReLU + MaxPool 2×2 → NCHW [32][7][7] (the flatten order of the classifier, ref :39) ------------------------
-  float* pool = reinterpret_cast<float*>(sb);   // the weights are dead after the MMAs: reuse their space
-  for (int i = tid; i < 1568; i += kL2Threads) {
-    const int c = i & 31, pp = i >> 5, ph = pp / 7, pw = pp - ph * 7;
-    const float sc = s_scale[c], sh = s_shift[c];
-    float mx = 0.f;   // the ReLU floor doubles as the identity of max
-#pragma unroll
-    for (int d = 0; d < 4; ++d) {
-      const int p = (2 * ph + (d >> 1)) * 14 + 2 * pw + (d & 1);
-      mx = fmaxf(mx, fmaf(ys[p * 32 + ((((c >> 2) + p) & 7) << 2) + (c & 3)], sc, sh));
-    }
-    pool[c * 49 + pp] = mx;
-  }
-  __syncthreads();
-  for (int i = tid; i < 1568; i += kL2Threads) out[static_cast<size_t>(n) * 1568 + i] = pool[i];
-  trace(2, 6);
-  // ---- classifier head riding on the pooled activations still in shared memory: logits = fc(pool) ----------------------
-  if (logits != nullptr && ncls <= 16) {
-    // thread t owns features t, t+256, … (≤ 7) for every class: all weight loads are independent and in flight together
-    float pv[7];
-#pragma unroll
-    for (int j = 0; j < 7; ++j) pv[j] = (tid + j * kL2Threads < 1568) ? pool[tid + j * kL2Threads] : 0.f;
-    float accv[16];
-#pragma unroll
-    for (int c16 = 0; c16 < 16; ++c16) {
-      float sacc = 0.f;
-      if (c16 < ncls) {
-        const float* wr = fcw + static_cast<size_t>(c16) * 1568 + tid;
-#pragma unroll
-        for (int j = 0; j < 7; ++j)
-          if (tid + j * kL2Threads < 1568) sacc = fmaf(pv[j], __ldg(wr + j * kL2Threads), sacc);
-      }
-      accv[c16] = sacc;
-    }
-#pragma unroll
-    for (int c16 = 0; c16 < 16; ++c16) {
-#pragma unroll
-      for (int off = 16; off >= 1; off >>= 1) accv[c16] += __shfl_xor_sync(0xffffffffu, accv[c16], off);
-    }
-    float* s_fc = s_part;   // [8 warps][16]
-    if (lane == 0) {
-#pragma unroll
-      for (int c16 = 0; c16 < 16; ++c16) s_fc[warp * 16 + c16] = accv[c16];
-    }
-    __syncthreads();
-    if (tid < ncls) {
-      float sfin = fcb ? fcb[tid] : 0.f;
-#pragma unroll
-      for (int w8 = 0; w8 < 8; ++w8) sfin += s_fc[w8 * 16 + tid];
-      logits[static_cast<size_t>(n) * ncls + tid] = sfin;
-    }
-  } else if (logits != nullptr) {
-    // warp k computes classes k, k+8, ...: 1568-long dot products, lanes stride the features
-    for (int cls = warp; cls < ncls; cls += kL2Threads / 32) {
-      const float* wr = fcw + static_cast<size_t>(cls) * 1568;
-      float s = 0.f;
-      for (int k = lane; k < 1568; k += 32) s = fmaf(pool[k], __ldg(wr + k), s);
-#pragma unroll
-      for (int off = 16; off >= 1; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-      if (lane == 0) logits[static_cast<size_t>(n) * ncls + cls] = s + (fcb ? fcb[cls] : 0.f);
-    }
-  }
-
-  __syncthreads();
-  bar.finish(gs);
-  trace(2, 7);
-}
-
 // =====================================================================================================================
 // Whole forward pass in ONE kernel: layer 1 and layer 2 (+ classifier) of an image run in the same CTA, so the pooled
 // layer-1 activations never leave the SM on their way into conv2 — they are written straight into the swizzled,
@@ -1449,41 +1149,42 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
 struct L2BwdSmem {
   static constexpr int kB = 25 * 16 * 128;       // dgrad weights: [tap][16 ci][128 B = 32 co]                  51,200
   static constexpr int kTotal = 1024 + kPatchAlloc + kB + 4096;
-  // FC (the classifier's backward rides along): fc weights [16][1568] | dlogits [B ≤ 160][16] | pooled slice [B ≤ 160][16]
+  // the classifier's backward: fc weights [16][1568] | dlogits [B ≤ 160][16] | pooled slice [B ≤ 160][16]
   static constexpr int kFcW = 16 * 1568 * 4, kFcDl = 160 * 16 * 4, kFcP = 160 * 16 * 4;
   static constexpr int kTotalFc = kTotal + kFcW + kFcDl + kFcP;
   // WG: conv2's weight-gradient operands (Conv2Wg).  The x copies are written in the grid barrier's shadow over the fc weights, dead
-  // by then (FC), and dyᵀ after the barrier over the end of the fc weights and the dlogits / pooled slices, which the classifier's
-  // weight gradient in the shadow was the last to read.  The same offsets without FC.
+  // by then, and dyᵀ after the barrier over the end of the fc weights and the dlogits / pooled slices, which the classifier's
+  // weight gradient in the shadow was the last to read.
   static constexpr int kXT = kPatchAlloc + kB + 4096;
   static constexpr int kDyT = kXT + Conv2Wg::kXBytes;
   static constexpr int kTotalWg = 1024 + kDyT + Conv2Wg::kDyT;
   static_assert(Conv2Wg::kXBytes <= kFcW && kTotalWg <= 227 * 1024, "conv2 weight-gradient operand placement");
 };
 
-// FC: the classifier's backward rides along.  The gradient of the pooled activations is not read from `dout` but computed
-// on the fly, d(out)[n][k] = Σ_j dlogits[n][j] · Wfc[j][k] (fc weights staged in smem once per CTA); the classifier's weight
+// The classifier's backward rides along: the gradient of the pooled activations is computed on the fly,
+// d(out)[n][k] = Σ_j dlogits[n][j] · Wfc[j][k] (fc weights staged in smem once per CTA); the classifier's weight
 // gradient dWfc[j][k] = Σ_n dlogits[n][j] · out[n][k] is produced in 16-column slices, one slice per CTA (all images, fixed
-// order: deterministic, no partials), the bias gradient by the CTA that owns "slice 98".  One kernel less per step.
+// order: deterministic, no partials), the bias gradient by the CTA that owns "slice 98".
 // WG: conv2's weight-gradient partial of the image (Conv2Wg) is computed here on wgmma, issued by warpgroup 0 while warpgroup 1 issues
 // the data gradient's: the x copies are written from conv2's input frame x2 in the shadow of the grid barrier, dyᵀ from the
 // registers that write the dy patch.  The global dy frame is then not written: nothing reads it.
-// ACC (accumulate mode, gradient accumulation over micro-batches): every gradient this kernel writes — dfcw, dfcb, dgamma, dbeta —
-// and the folded loss become g = g_old + v, one fp32 add, the rounding of autograd's accumulation of a temporary.
-template <bool FC, bool WG, bool ACC = false>
+// WG = false writes the dy frame instead and no partials.  No training step runs it: it is the reference the tests feed to
+// conv2_wgrad_partials_kernel, and the two together are the only bit-exact check of the K-major operand copies the WG form writes.
+// ACC (accumulate mode, gradient accumulation over micro-batches, needs WG): every gradient this kernel writes — dfcw, dfcb, dgamma,
+// dbeta — and the folded loss become g = g_old + v, one fp32 add, the rounding of autograd's accumulation of a temporary.
+template <bool WG, bool ACC = false>
 __global__ void __launch_bounds__(kL2Threads, 1)
-convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float* __restrict__ y /*[B,14,14,32]*/,
+convnet_l2_bwd_kernel(const float* __restrict__ y /*[B,14,14,32]*/,
                       const float* __restrict__ saved, const float* __restrict__ gamma, const float* __restrict__ beta,
                       const float* __restrict__ w, float* dgamma, float* dbeta, float* __restrict__ dy /*[B,18,18,32] zero-haloed frame*/,
                       float* __restrict__ dx /*[B,18,18,16] frame, interior written*/, float* __restrict__ dysum /*[B,32]*/,
                       float* partials, GridSync gs,
-                      // FC only
                       const float* __restrict__ dlogits /*[B,ncls]*/, const float* __restrict__ fcw /*[ncls,1568]*/,
                       const float* __restrict__ pooled /*[B,1568] = forward's out*/, float* dfcw /*[ncls,1568]*/, float* dfcb /*[ncls]*/,
                       int ncls, const float* __restrict__ loss_parts /*[B] or null*/, float* loss_out,
                       // WG only
                       const float* __restrict__ x2 /*[B,18,18,16] = conv2's input frame*/, float* __restrict__ wpart /*[B][400][32]*/) {
-  static_assert(!ACC || (FC && WG), "accumulate mode is a variant of the kernel with the classifier and conv2's weight gradient");
+  static_assert(WG || !ACC, "accumulate mode is a variant of the kernel with conv2's weight gradient");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sa = smem;                                  // dy patch, written by the CTA in the TMA/wgmma SWIZZLE_128B layout
@@ -1496,9 +1197,9 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
   float* s_shift = misc + 864;
   float* s_mean = misc + 896;
   float* s_invstd = misc + 928;
-  float* s_fcw = misc + 1024;                                   // FC: [ncls][1568]
-  float* s_dl = s_fcw + L2BwdSmem::kFcW / 4;                    // FC: [B][16] (columns >= ncls zero)
-  float* s_pool = s_dl + L2BwdSmem::kFcDl / 4;                  // FC: [B][16] slice of the pooled activations
+  float* s_fcw = misc + 1024;                                   // [ncls][1568]
+  float* s_dl = s_fcw + L2BwdSmem::kFcW / 4;                    // [B][16] (columns >= ncls zero)
+  float* s_pool = s_dl + L2BwdSmem::kFcDl / 4;                  // [B][16] slice of the pooled activations
   uint8_t* s_xt = smem + L2BwdSmem::kXT;                        // WG: conv2's x copies
   uint8_t* s_dyt = smem + L2BwdSmem::kDyT;                      // WG: conv2's dyᵀ
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = blockIdx.x, B = gridDim.x;
@@ -1509,7 +1210,7 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
   // WG: the loads of conv2's x copies, written in the grid barrier's shadow (the forward kernel wrote x2)
   Conv2WgX<kL2Threads> xr;
   if constexpr (WG) xr.load(x2 + static_cast<size_t>(n) * Conv2Wg::kFrame * 16, tid);
-  if constexpr (FC) {
+  {
     // stage the classifier weights (cp.async, no registers, lands while the dgrad weights are built), every image's dlogits and this
     // CTA's first 16-column slice of the pooled activations (loads batched in registers: one L2 latency, not one per element)
     for (int i = tid; i < ncls * 392; i += kL2Threads) cp_async_16(smem_u32(s_fcw + 4 * i), fcw + 4 * i, 16);
@@ -1556,7 +1257,7 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
       for (int tap = 0; tap < 25; ++tap) *reinterpret_cast<float*>(dst + (24 - tap) * 2048) = wv[j][tap];
     }
   }
-  if constexpr (FC) cp_async_wait<0>();
+  cp_async_wait<0>();
   __syncthreads();
   trace(3, 1);
 
@@ -1581,20 +1282,16 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
         const float z = fmaf(yv[k][d], sc, sh);
         if (z > best) { best = z; arg[k] = d; }
       }
-      float go;
-      if constexpr (FC) {
-        const float* wk = s_fcw + c * 49 + pp;       // bank = (17·c + pp) mod 32: conflict-free across the warp's 32 channels
-        const float* dl = s_dl + n * 16;
-        float g0 = 0.f, g1 = 0.f;
+      // d(out) of this window from the classifier: Σ_j dlogits[n][j] · Wfc[j][c·49 + pp]
+      const float* wk = s_fcw + c * 49 + pp;       // bank = (17·c + pp) mod 32: conflict-free across the warp's 32 channels
+      const float* dl = s_dl + n * 16;
+      float g0 = 0.f, g1 = 0.f;
 #pragma unroll
-        for (int j = 0; j < 16; j += 2) {            // independent smem loads (classes >= ncls: dlogits column is zero, weight not read)
-          g0 = fmaf(dl[j], j < ncls ? wk[j * 1568] : 0.f, g0);
-          g1 = fmaf(dl[j + 1], j + 1 < ncls ? wk[(j + 1) * 1568] : 0.f, g1);
-        }
-        go = g0 + g1;
-      } else {
-        go = dout[static_cast<size_t>(n) * 1568 + c * 49 + pp];
+      for (int j = 0; j < 16; j += 2) {            // independent smem loads (classes >= ncls: dlogits column is zero, weight not read)
+        g0 = fmaf(dl[j], j < ncls ? wk[j * 1568] : 0.f, g0);
+        g1 = fmaf(dl[j + 1], j + 1 < ncls ? wk[(j + 1) * 1568] : 0.f, g1);
       }
+      const float go = g0 + g1;
       dzv[k] = best > 0.f ? go : 0.f;
       float xh = 0.f;
 #pragma unroll
@@ -1624,7 +1321,7 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
       if (pr < 2 || pr >= 16 || pc < 2 || pc >= 16) reinterpret_cast<float4*>(dy + (static_cast<size_t>(n) * 324 + P) * 32)[i & 7] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
   }
-  if constexpr (FC) {
+  {
     // classifier weight gradient, slice = 16 consecutive columns (98 slices; "slice 98" = the bias): thread = (column, class).
     // The first slice of this CTA (slice n) was staged at kernel start.
     const int kl = tid & 15, j = tid >> 4;
@@ -1781,23 +1478,11 @@ convnet_l2_bwd_kernel(const float* __restrict__ dout /*[B,32,7,7]*/, const float
   trace(3, 6);
 }
 
+}  // namespace
+
 // ---------------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------------
-CUtensorMap make_patch_map(const float* base, int C, int W, int H, int N) {
-  CUtensorMap m;
-  cuuint64_t dims[4] = {static_cast<cuuint64_t>(C), static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H), static_cast<cuuint64_t>(N)};
-  cuuint64_t strides[3] = {static_cast<cuuint64_t>(C) * 4, static_cast<cuuint64_t>(W) * C * 4, static_cast<cuuint64_t>(H) * W * C * 4};
-  cuuint32_t box[4] = {32, static_cast<cuuint32_t>(W), static_cast<cuuint32_t>(H), 1};   // the whole (already haloed) frame
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = driver().cuTensorMapEncodeTiled(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), dims, strides, box, estr,
-                                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) throw std::runtime_error("cuTensorMapEncodeTiled(fused conv2 patch) failed: " + cu_error(r));
-  return m;
-}
-
-}  // namespace
 
 bool fused_convnet_supported(int B) { return B >= 1 && B <= sm_count(); }
 
@@ -1815,21 +1500,6 @@ void fused_convnet_trace_read(unsigned long long* host /*[4][160][12]*/) {
   PDT_CUDA_CHECK(cudaMemcpyFromSymbol(host, g_trace, sizeof(unsigned long long) * 4 * 160 * 12));
 }
 
-void launch_convnet_l1_fwd(const float* x, const float* w, const float* bias, const float* gamma, const float* beta, float* y, float* out,
-                           float* saved, float* running_mean, float* running_var, long long* nbt, float momentum, float eps, int B,
-                           float* partials, GridSync gs, cudaStream_t st) {
-  launch_cooperative(convnet_l1_fwd_kernel, B, kL1Threads, 0, st, "convnet_l1_fwd", x, w, bias, gamma, beta, y, out, saved, running_mean, running_var, nbt,
-                     momentum, eps, partials, gs);
-}
-
-void launch_convnet_l1_bwd(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
-                           float* dgamma, float* dbeta, float* dw, float* db, int B, float* partials, float* partials_w, GridSync gs,
-                           cudaStream_t st) {
-  launch_cooperative(convnet_l1_bwd_kernel<false>, B, kL1Threads, static_cast<size_t>(kL1BwdSmem), st, "convnet_l1_bwd", dp, y, x, saved, gamma, beta, dgamma,
-                     dbeta, dw, db, partials, partials_w, gs, static_cast<const float*>(nullptr), static_cast<const float*>(nullptr),
-                     static_cast<float*>(nullptr), static_cast<float*>(nullptr), SgdRider{});
-}
-
 void launch_conv2_wgrad_partials(const float* dy2_pad, const float* x2_pad, int B, float* wpart, cudaStream_t st) {
   opt_in_smem(conv2_wgrad_partials_kernel, kConv2WgSmem);
   conv2_wgrad_partials_kernel<<<B, 128, kConv2WgSmem, st>>>(dy2_pad, x2_pad, wpart);
@@ -1840,7 +1510,7 @@ template <class Rider>
 void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
                                  float* dgamma, float* dbeta, float* dw, float* db, const float* wpart, const float* dysum2, float* dw2, float* db2,
                                  int B, float* partials, float* partials_w, GridSync gs, cudaStream_t st, Rider rider, bool accumulate) {
-  auto kernel = accumulate ? convnet_l1_bwd_kernel<true, Rider, true> : convnet_l1_bwd_kernel<true, Rider>;
+  auto kernel = accumulate ? convnet_l1_bwd_kernel<Rider, true> : convnet_l1_bwd_kernel<Rider>;
   launch_cooperative(kernel, B, kL1Threads, static_cast<size_t>(kL1BwdSmem), st, "convnet_l1_bwd_wgrad", dp, y, x, saved,
                      gamma, beta, dgamma, dbeta, dw, db, partials, partials_w, gs, wpart, dysum2, dw2, db2, rider);
 }
@@ -1853,14 +1523,6 @@ PDT_L1_BWD_WGRAD(AdamRider)
 PDT_L1_BWD_WGRAD(ClipRider<SgdRider>)
 PDT_L1_BWD_WGRAD(ClipRider<AdamRider>)
 #undef PDT_L1_BWD_WGRAD
-
-void launch_convnet_l2_fwd(const float* x, const float* w, const float* bias, const float* gamma, const float* beta, float* y, float* out,
-                           float* saved, float* running_mean, float* running_var, long long* nbt, float momentum, float eps,
-                           const float* fcw, const float* fcb, float* logits, int ncls, int B, float* partials, GridSync gs, cudaStream_t st) {
-  CUtensorMap tm_x = make_patch_map(x, 16, 18, 18, B);
-  launch_cooperative(convnet_l2_fwd_kernel, B, kL2Threads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_l2_fwd", tm_x, w, bias, gamma, beta, y, out,
-                     saved, running_mean, running_var, nbt, momentum, eps, fcw, fcb, logits, ncls, partials, gs);
-}
 
 void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const float* g1, const float* be1, float* y1, float* p1, float* saved1,
                         float* rm1, float* rv1, long long* nbt1, float mom1, float eps1, const float* w2, const float* b2, const float* g2,
@@ -1881,16 +1543,6 @@ void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const 
                      static_cast<const FusedCe&>(ce));
 }
 
-void launch_convnet_l2_bwd(const float* dout, const float* y, const float* saved, const float* gamma, const float* beta, const float* w,
-                           float* dgamma, float* dbeta, float* dy, float* dx, float* dysum, int B, float* partials, GridSync gs,
-                           cudaStream_t st, const float* x2, float* wpart) {
-  auto kernel = x2 != nullptr ? convnet_l2_bwd_kernel<false, true> : convnet_l2_bwd_kernel<false, false>;
-  launch_cooperative(kernel, B, kL2Threads, static_cast<size_t>(x2 != nullptr ? L2BwdSmem::kTotalWg : L2BwdSmem::kTotal), st, "convnet_l2_bwd", dout,
-                     y, saved, gamma, beta, w, dgamma, dbeta, dy, dx, dysum, partials, gs, static_cast<const float*>(nullptr),
-                     static_cast<const float*>(nullptr), static_cast<const float*>(nullptr), static_cast<float*>(nullptr), static_cast<float*>(nullptr), 0,
-                     static_cast<const float*>(nullptr), static_cast<float*>(nullptr), x2, wpart);
-}
-
 void launch_convnet_l2_bwd_fc(const float* dlogits, const float* fcw, const float* pooled, float* dfcw, float* dfcb, int ncls, const float* y,
                               const float* saved, const float* gamma, const float* beta, const float* w, float* dgamma, float* dbeta, float* dy,
                               float* dx, float* dysum, int B, float* partials, GridSync gs, cudaStream_t st, const float* loss_parts, float* loss_out,
@@ -1898,12 +1550,10 @@ void launch_convnet_l2_bwd_fc(const float* dlogits, const float* fcw, const floa
   if (ncls < 1 || ncls > 16) throw std::invalid_argument("convnet_l2_bwd_fc: 1..16 classes");
   if (B > 160) throw std::invalid_argument("convnet_l2_bwd_fc: batch too large for the staged dlogits");
   if (accumulate && x2 == nullptr) throw std::invalid_argument("convnet_l2_bwd_fc: accumulate mode needs conv2's input frame (x2)");
-  auto kernel = accumulate ? convnet_l2_bwd_kernel<true, true, true>
-                           : x2 != nullptr ? convnet_l2_bwd_kernel<true, true> : convnet_l2_bwd_kernel<true, false>;
+  auto kernel = accumulate ? convnet_l2_bwd_kernel<true, true> : x2 != nullptr ? convnet_l2_bwd_kernel<true> : convnet_l2_bwd_kernel<false>;
   const int smem = x2 != nullptr ? std::max(L2BwdSmem::kTotalFc, L2BwdSmem::kTotalWg) : L2BwdSmem::kTotalFc;
-  launch_cooperative(kernel, B, kL2Threads, static_cast<size_t>(smem), st, "convnet_l2_bwd_fc", static_cast<const float*>(nullptr), y, saved,
-                     gamma, beta, w, dgamma, dbeta, dy, dx, dysum, partials, gs, dlogits, fcw, pooled, dfcw, dfcb, ncls, loss_parts, loss_out, x2,
-                     wpart);
+  launch_cooperative(kernel, B, kL2Threads, static_cast<size_t>(smem), st, "convnet_l2_bwd_fc", y, saved, gamma, beta, w, dgamma, dbeta, dy,
+                     dx, dysum, partials, gs, dlogits, fcw, pooled, dfcw, dfcb, ncls, loss_parts, loss_out, x2, wpart);
 }
 
 }  // namespace pdt

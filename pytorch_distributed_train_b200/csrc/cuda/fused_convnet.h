@@ -9,21 +9,14 @@ namespace pdt {
 
 // One CTA per image, all co-resident: the batch must not exceed the number of SMs.
 bool fused_convnet_supported(int B);
-// Phase trace of the cooperative kernels (globaltimer stamps of thread 0 of every CTA): [kernel 0..3][CTA][phase].
+// Phase trace of the cooperative kernels (globaltimer stamps of thread 0 of every CTA): [kernel slot 0..3][CTA][phase], slots
+// 0 forward, 1 layer-1 backward, 3 layer-2 backward.
 void fused_convnet_trace_enable(bool on);
 void fused_convnet_trace_read(unsigned long long* host);
 
-// Activations between the two layers live in zero-haloed 18×18 NHWC frames ([B,18,18,C], interior = rows/cols 2..15):
-// layer 2 reads the halo as the convolution's zero padding (one TMA box per image, row-shifted descriptors per tap).
-// x [B,28,28] → y [B,28,28,16] (conv1 + bias, kept for backward), out [B,18,18,16] frame (BN + ReLU + pool), saved [32] = mean, invstd.
-// partials: B·32 floats of scratch.
-void launch_convnet_l1_fwd(const float* x, const float* w, const float* bias, const float* gamma, const float* beta, float* y, float* out,
-                           float* saved, float* running_mean, float* running_var, long long* nbt, float momentum, float eps, int B,
-                           float* partials, GridSync gs, cudaStream_t st);
-// dp [B,18,18,16] frame (interior read) → dgamma/dbeta [16], dw [16,1,5,5], db [16].  partials: B·32, partials_w: B·512 floats.
-void launch_convnet_l1_bwd(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
-                           float* dgamma, float* dbeta, float* dw, float* db, int B, float* partials, float* partials_w, GridSync gs,
-                           cudaStream_t st);
+// Activations between the two layers live in zero-haloed 18×18 NHWC frames ([B,18,18,C], interior = rows/cols 2..15): the
+// kernels read the halo as the convolution's zero padding.
+
 // Optional rider of the last backward kernel: the SGD update of every parameter of the model.  Parameters 0..5 (conv1.w, conv1.b,
 // bn1.w, bn1.b, conv2.w, conv2.b) get their gradient inside this kernel — the thread that writes the folded gradient element applies
 // the update with the value still in its register; parameters 6..9 (gradients complete before the launch: classifier, bn2) are updated
@@ -61,11 +54,13 @@ struct ClipRider : Base {
   float* part = nullptr;       // [B] per-CTA partials
 };
 
-// conv2's weight gradient per image (wpart [B][400][32], rows (kh, kw, ci), the layout of launch_convnet_l2_bwd's WG form) from given frames:
-// dy2_pad [B,18,18,32] (zero halo), x2_pad [B,18,18,16].  One CTA per image, not cooperative.
+// conv2's weight gradient per image (wpart [B][400][32], rows (kh, kw, ci), the layout launch_convnet_l2_bwd_fc writes given x2) from
+// given frames: dy2_pad [B,18,18,32] (zero halo), x2_pad [B,18,18,16].  One CTA per image, not cooperative.  No training step runs it:
+// with the dy frame of launch_convnet_l2_bwd_fc without x2 it is the tests' bit-exact reference for the partials backward A computes.
 void launch_conv2_wgrad_partials(const float* dy2_pad, const float* x2_pad, int B, float* wpart, cudaStream_t st);
-// Layer-1 backward that also folds conv2's weight gradient: the per-image partials wpart and Σdy rows dysum2 [B,32] → dw2
-// [32,16,5,5], db2 [32], in the shadow of the kernel's first grid barrier.  Rider: SgdRider or AdamRider, or either one in a ClipRider.
+// Layer-1 backward: dp [B,18,18,16] frame (interior read) → dgamma/dbeta [16], dw [16,1,5,5], db [16]; it also folds conv2's weight
+// gradient: the per-image partials wpart and Σdy rows dysum2 [B,32] → dw2 [32,16,5,5], db2 [32], in the shadow of the kernel's first
+// grid barrier.  partials: B·32, partials_w: B·512 floats.  Rider: SgdRider or AdamRider, or either one in a ClipRider.
 // accumulate: gradient accumulation — every gradient written (dgamma, dbeta, dw, db, dw2, db2) becomes g_old + this batch's value, and
 // the rider updates with (and clips) the accumulated gradient.
 template <class Rider = SgdRider>
@@ -73,11 +68,6 @@ void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* x
                                  float* dgamma, float* dbeta, float* dw, float* db, const float* wpart, const float* dysum2, float* dw2, float* db2,
                                  int B, float* partials, float* partials_w, GridSync gs, cudaStream_t st, Rider rider = Rider{},
                                  bool accumulate = false);
-// x [B,18,18,16] frame → y [B,14,14,32], out [B,32,7,7] NCHW, saved [64]; logits [B,ncls] = fc(out) when logits != nullptr.
-// partials: B·64 floats.
-void launch_convnet_l2_fwd(const float* x, const float* w, const float* bias, const float* gamma, const float* beta, float* y, float* out,
-                           float* saved, float* running_mean, float* running_var, long long* nbt, float momentum, float eps,
-                           const float* fcw, const float* fcb, float* logits, int ncls, int B, float* partials, GridSync gs, cudaStream_t st);
 // Optional rider of the whole-forward kernel: the mean cross-entropy of the logits against `target` and its gradient
 // (softmax − onehot)/n, computed by the CTA that owns the image; the batch mean is folded by the CTA that finishes last
 // (arrival counter, fixed summation order).  n counts the images whose target is in [0, ncls); the others (ignore_index) add
@@ -97,27 +87,27 @@ struct ScaledCe : FusedCe {
 };
 
 // The whole training forward in one launch: layer 1 and layer 2 (+ classifier, ncls ≤ 16) of an image in the same CTA; the
-// pooled layer-1 activations go into conv2's shared-memory patch directly.  partials: B·(32 + 64) floats.
+// pooled layer-1 activations go into conv2's shared-memory patch directly.  x [B,28,28] → y1 [B,28,28,16] (conv1 + bias, kept for
+// backward), p1 [B,18,18,16] frame (BN + ReLU + pool), saved1 [32] = mean, invstd; y2 [B,14,14,32], out [B,32,7,7] NCHW, saved2
+// [64]; logits [B,ncls].  partials: B·(32 + 64) floats.
 // ce.scale != 1 (with targets) runs the ScaledCe instantiation; otherwise the kernel without the scale.
 void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const float* g1, const float* be1, float* y1, float* p1, float* saved1,
                         float* rm1, float* rv1, long long* nbt1, float mom1, float eps1, const float* w2, const float* b2, const float* g2,
                         const float* be2, float* y2, float* out, float* saved2, float* rm2, float* rv2, long long* nbt2, float mom2, float eps2,
                         const float* fcw, const float* fcb, float* logits, int ncls, int B, float* partials, GridSync gs, cudaStream_t st,
                         ScaledCe ce = ScaledCe{});
-// dout [B,32,7,7] → dgamma/dbeta [32], dy [B,18,18,32] frame with zero halo (gradient at the conv2 output), dx [B,18,18,16] frame
-// (data gradient, interior written), dysum [B,32] (per-image Σdy: the conv2 bias gradient is the sum of its rows).
+// Layer-2 backward with the classifier's backward riding along: d(out) is computed from dlogits [B,ncls] and the fc weights
+// [ncls,1568] inside the kernel; dfcw [ncls,1568] / dfcb [ncls] are produced from `pooled` = the forward's out [B,1568].  ncls ≤ 16.
+// → dgamma/dbeta [32], dy [B,18,18,32] frame with zero halo (gradient at the conv2 output), dx [B,18,18,16] frame (data gradient,
+// interior written), dysum [B,32] (per-image Σdy: the conv2 bias gradient is the sum of its rows).
 // x2 != nullptr (conv2's input frame [B,18,18,16]): conv2's weight-gradient partials per image go to wpart [B][400][32] instead,
-// and dy is not written.
-void launch_convnet_l2_bwd(const float* dout, const float* y, const float* saved, const float* gamma, const float* beta, const float* w,
-                           float* dgamma, float* dbeta, float* dy, float* dx, float* dysum, int B, float* partials, GridSync gs, cudaStream_t st,
-                           const float* x2 = nullptr, float* wpart = nullptr);
-// The same with the classifier's backward riding along: d(out) is computed from dlogits [B,ncls] and the fc weights [ncls,1568]
-// inside the kernel; dfcw [ncls,1568] / dfcb [ncls] are produced from `pooled` = the forward's out [B,1568].  ncls ≤ 16.
+// and dy is not written.  The training step always passes x2; without it the kernel is the tests' reference (see
+// launch_conv2_wgrad_partials).
 void launch_convnet_l2_bwd_fc(const float* dlogits, const float* fcw, const float* pooled, float* dfcw, float* dfcb, int ncls, const float* y,
                               const float* saved, const float* gamma, const float* beta, const float* w, float* dgamma, float* dbeta, float* dy,
                               float* dx, float* dysum, int B, float* partials, GridSync gs, cudaStream_t st,
                               const float* loss_parts = nullptr, float* loss_out = nullptr,   // mean of the forward kernel's CE terms
-                              const float* x2 = nullptr, float* wpart = nullptr,              // as for launch_convnet_l2_bwd
+                              const float* x2 = nullptr, float* wpart = nullptr,
                               bool accumulate = false);   // dfcw, dfcb, dgamma, dbeta, loss_out += this batch's values (needs x2)
 
 }  // namespace pdt

@@ -1,13 +1,9 @@
-// conv2 (16→32, 5×5) weight gradient in the "window" formulation on warp-level mma.sync, for the per-op kernels of
-// conv_wgmma.cu:
-//   dWᵀ[(kh, kw, ci)][co] = Σ_P xpad[P + (kh−2)·18 + (kw−2)][ci] · dypad[P][co]
-// over the padded positions P from the first interior one.  Two horizontally adjacent taps of one position are 32
-// contiguous floats of the NHWC frame, so a 32-row "atom" of the M dimension (tap pair × 16 channels) is one row of the
-// overlapping-row view of the frame (row r = positions r, r+1).  Both operands have the reduction dimension (positions)
-// outermost — MN-major — which TF32 wgmma does not accept, so this is mma.sync m16n8k8 reading the swizzled TMA tiles
-// directly.  The im2col weight gradient (conv_wgmma.cu) uses the same per-warp step.
-// The fused step does not use it: its layer-2 backward kernel writes K-major (transposed, TF32-rounded) copies of both operands
-// into shared memory and issues wgmma (conv2_wgrad_wgmma, fused_convnet.cu).
+// Warp-level mma.sync step of the per-op conv2 (16→32, 5×5) weight gradient (conv5x5_wgrad_mma_kernel, conv_wgmma.cu):
+// one warp accumulates a 32-row "atom" of dWᵀ (rows of the im2col tile × 32 output channels) over pixel positions.  Both
+// operands have the reduction dimension (positions) outermost — MN-major — which TF32 wgmma does not accept, so this is
+// mma.sync m16n8k8 reading the swizzled TMA tiles directly.  fused_convnet.cu takes its TF32 conversion and mma.sync
+// wrappers; its own conv2 weight gradient writes K-major (transposed, TF32-rounded) copies of both operands into shared memory
+// and issues wgmma (conv2_wgrad_wgmma).
 #pragma once
 #include <cstdint>
 
@@ -31,7 +27,7 @@ __device__ __forceinline__ void mma_m16n8k8_tf32(float (&c)[4], const uint32_t (
 // The four rows a fragment load touches differ in r mod 8, so the loads below are free of bank conflicts.
 
 // One warp: acc (32 rows of an atom × 32 output channels) += Σ_{P < KPOS} x[P][i] · dy[P][co], where x[P][i] is element
-// (xrow0 + P, xcol0 + i) of the swizzled tile xs (the window kernels: row xrow0 + P of the overlapping-row view) and dy[P][co]
+// (xrow0 + P, xcol0 + i) of the swizzled tile xs and dy[P][co]
 // element (dyrow0 + P, co) of the swizzled tile dys ([rows][32]).  acc[j][nt][e] holds D[16j + g + 8·(e >> 1)][8nt + 2·t4 + (e & 1)]
 // with g = lane / 4, t4 = lane % 4.  UNROLL: K steps per loop iteration (1 where registers are scarce).
 template <int KPOS = 256, int XPITCH = 32, int UNROLL = 2>

@@ -3,14 +3,14 @@
 (``layer1.0.weight`` … ``fc.bias``) so checkpoints interchange and
 ``SyncBatchNorm.convert_sync_batchnorm`` finds the BatchNorm layers where it expects them.
 
-On an H100 the forward does not walk the ``nn.Sequential``s.  In training the whole forward is TWO cooperative
-sm_90a kernels with one CTA per image (``csrc/cuda/fused_convnet.cu``): conv1+BN1+ReLU+pool1, and
-conv2 (wgmma, register accumulators, haloed image in shared memory) +BN2+ReLU+pool2+classifier — the BatchNorm batch
-statistics cross a device-side grid barrier inside the kernel instead of a kernel boundary; backward is one such
-kernel per layer plus the tensor-core weight gradient.  Shapes the fused kernels do not cover (eval mode,
-SyncBatchNorm, batch > #SMs) run each ``layerN`` as two per-op kernels (implicit-GEMM conv with the BN statistics in
-its epilogue, then BN-apply+ReLU+MaxPool) and the classifier as one linear kernel.  The same modules fall back to
-the stock layers on CPU (plumbing tests) or when ``fused=False``.
+On an H100 the forward does not walk the ``nn.Sequential``s.  In training the whole forward is ONE cooperative
+sm_90a kernel with one CTA per image (``csrc/cuda/fused_convnet.cu``): conv1+BN1+ReLU+pool1 → conv2 (wgmma, register
+accumulators, haloed image in shared memory) +BN2+ReLU+pool2+classifier — the BatchNorm batch statistics cross a
+device-side grid barrier inside the kernel instead of a kernel boundary; backward is one such kernel per layer, with the
+classifier's backward and conv2's weight gradient riding along.  What the fused kernels do not cover (eval mode,
+SyncBatchNorm, batch > #SMs, a partially frozen model) runs each ``layerN`` as two per-op kernels (implicit-GEMM conv with the
+BN statistics in its epilogue, then BN-apply+ReLU+MaxPool) and the classifier as one linear kernel.  The same modules fall back
+to the stock layers on CPU (plumbing tests) or when ``fused=False``.
 """
 from __future__ import annotations
 
@@ -50,7 +50,7 @@ class ConvNet(nn.Module):
             from ..ops import functional as OF
 
             if torch.is_grad_enabled() and OF.fused_convnet_ok(x, self):
-                # one cooperative kernel per layer (conv + BN statistics barrier + BN/ReLU/pool [+ classifier])
+                # one cooperative kernel for the forward (conv + BN statistics barrier + BN/ReLU/pool, per layer, + classifier)
                 return OF.fused_convnet_forward(x, self)
             out = ops.conv_bn_relu_pool(x, self.layer1[0], self.layer1[1])
             out = ops.conv_bn_relu_pool(out, self.layer2[0], self.layer2[1])

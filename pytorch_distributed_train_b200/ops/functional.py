@@ -121,9 +121,10 @@ class _ConvBnReluPool(torch.autograd.Function):
 # =====================================================================================================
 def fused_convnet_ok(x: torch.Tensor, model) -> bool:
     """The per-image cooperative kernels cover exactly the reference architecture (ref: ddp_example.py:22-41) in
-    training mode with local BatchNorm statistics and a classifier of at most 16 classes (the width of the fused classifier
-    and its backward); everything else takes the per-op kernels."""
-    if os.environ.get("PDT_FUSED_LAYERS", "1") == "0" or not hasattr(_C, "convnet_l1_fwd"):
+    training mode with local BatchNorm statistics, a classifier of at most 16 classes (the width of the fused classifier
+    and its backward) and every parameter trainable (the two fused backward kernels write all ten gradients); everything
+    else, a partially frozen model included, takes the per-op kernels."""
+    if os.environ.get("PDT_FUSED_LAYERS", "1") == "0" or not hasattr(_C, "convnet_fwd"):
         return False
     c1, b1, c2, b2, fc = model.layer1[0], model.layer1[1], model.layer2[0], model.layer2[1], model.fc
     if not (x.dim() == 4 and x.shape[1:] == (1, 28, 28) and x.is_contiguous() and _C.fused_convnet_supported(x.shape[0])):
@@ -135,6 +136,11 @@ def fused_convnet_ok(x: torch.Tensor, model) -> bool:
     for bn in (b1, b2):
         if not bn.training or type(bn).__name__ == "SyncBatchNorm" or not bn.track_running_stats or bn.momentum is None or not bn.affine:
             return False
+    params = (c1.weight, c1.bias, b1.weight, b1.bias, c2.weight, c2.bias, b2.weight, b2.bias, fc.weight, fc.bias)
+    if not all(p is None or p.requires_grad for p in params):
+        return False
+    if fc.weight.data_ptr() % 16 != 0:
+        return False   # layer 2's backward kernel stages the classifier weights in 16-byte copies
     return all(p.is_contiguous() for p in (c1.weight, c2.weight, fc.weight))
 
 
@@ -179,8 +185,8 @@ class upcoming_targets:
 # the engine sets every .grad to None and hands the buffers micro-batch 1 left back through `accumulate_into`: the fused nodes take
 # them as their destinations, launch their kernels in accumulate mode (g = g_old + v) and return them, and autograd adopts the sums
 # as fresh gradients — no AccumulateGrad add, and the optimizer rider's fresh-gradient checks hold on the last micro-batch.  A writer
-# that overwrites (the per-op kernels, the stand-alone conv2 weight gradient, the stand-alone classifier backward) never consults
-# this, so the engine arms it only when `fused_backward_params` shows that the fused kernels wrote every gradient of micro-batch 1.
+# that overwrites (the per-op kernels) never consults this, so the engine arms it only when `fused_backward_params` shows that the
+# fused kernels wrote every gradient of micro-batch 1.
 _accumulate: Optional[dict] = None     # {"grads": {id(param): buffer}, "loss": tensor the loss fold adds to, or None}
 _fused_backward_params: Optional[list] = None
 
@@ -209,7 +215,7 @@ class accumulate_into:
 
 def fused_backward_params() -> Optional[list]:
     """The parameters whose gradients the last backward pass wrote through the two fused ConvNet backward kernels — all ten, the
-    classifier's and conv2's included — or None when that pass took any other writer.  Reset with ``reset_fused_backward_params``."""
+    classifier's and conv2's included — or None when that pass did not run them.  Reset with ``reset_fused_backward_params``."""
     return _fused_backward_params
 
 
@@ -252,36 +258,26 @@ class sgd_rider_enabled:
         return False
 
 
-def _wgrad_rides_on_layer1() -> bool:
-    """conv2's weight gradient rides on the two backward kernels instead of running as a kernel of its own between them: the
-    layer-2 kernel computes the per-image partials next to its data gradient, the layer-1 kernel folds them (and applies the
-    riding optimizer's update).  PDT_WGRAD_MERGED=0 restores the separate launch."""
-    return os.environ.get("PDT_WGRAD_MERGED", "1") != "0" and hasattr(_C, "convnet_l1_bwd_wgrad")
-
-
 class _FusedLayer1(torch.autograd.Function):
-    """conv1 + BN1 + ReLU + pool1 forward, and its whole backward, as one cooperative kernel each.
+    """conv1 + BN1 + ReLU + pool1 forward — the node of the whole-forward launch — and its whole backward as one cooperative kernel.
 
-    ``w2`` / ``b2`` (conv2's parameters) are inputs of this node on purpose: when conv2's weight gradient rides on the
-    layer-1 backward kernel, *this* node returns it, so autograd (and DDP's reducer hooks behind it) sees the gradient
-    only after the kernel that produces it has been launched."""
+    ``w2`` / ``b2`` (conv2's parameters) are inputs of this node on purpose: conv2's weight gradient rides on the layer-1
+    backward kernel, so *this* node returns it, and autograd (and DDP's reducer hooks behind it) sees the gradient only after
+    the kernel that produces it has been launched."""
 
     @staticmethod
-    def forward(ctx, x, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, w2=None, b2=None, whole=None, link=None):
-        if whole is not None:
-            # ONE launch for the whole forward pass (csrc/cuda/fused_convnet.cu: convnet_fwd_kernel): layer 2 and the
-            # classifier of an image run in the same CTA; their results are handed to the next autograd nodes through `whole`
-            c2, bn2, fc = whole["conv2"], whole["bn2"], whole["fc"]
-            defer = bool(whole.get("defer_loss_mean", False))
-            out, y, saved, p2, y2, saved2, logits, loss, dlogits, loss_parts = _C.convnet_fwd(
-                x, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, c2.weight, c2.bias, bn2.weight, bn2.bias,
-                bn2.running_mean, bn2.running_var, bn2.num_batches_tracked, float(bn2.momentum), float(bn2.eps), fc.weight, fc.bias,
-                whole.get("target"), defer, float(whole.get("grad_scale", 1.0)))
-            whole["layer2"] = (p2, y2, saved2, logits)
-            whole["ce"] = (loss, dlogits)
-            whole["ce_deferred"] = (loss_parts, loss) if defer else None
-        else:
-            out, y, saved = _C.convnet_l1_fwd(x, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps)
+    def forward(ctx, x, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, w2, b2, whole, link):
+        # ONE launch for the whole forward pass (csrc/cuda/fused_convnet.cu: convnet_fwd_kernel): layer 2 and the
+        # classifier of an image run in the same CTA; their results are handed to the next autograd nodes through `whole`
+        c2, bn2, fc = whole["conv2"], whole["bn2"], whole["fc"]
+        defer = bool(whole.get("defer_loss_mean", False))
+        out, y, saved, p2, y2, saved2, logits, loss, dlogits, loss_parts = _C.convnet_fwd(
+            x, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, c2.weight, c2.bias, bn2.weight, bn2.bias,
+            bn2.running_mean, bn2.running_var, bn2.num_batches_tracked, float(bn2.momentum), float(bn2.eps), fc.weight, fc.bias,
+            whole.get("target"), defer, float(whole.get("grad_scale", 1.0)))
+        whole["layer2"] = (p2, y2, saved2, logits)
+        whole["ce"] = (loss, dlogits)
+        whole["ce_deferred"] = (loss_parts, loss) if defer else None
         ctx.save_for_backward(x, y, saved, gamma, beta)
         ctx.params = (w, b, gamma, beta, w2, b2)
         ctx.link = link
@@ -291,174 +287,111 @@ class _FusedLayer1(torch.autograd.Function):
     def backward(ctx, dp):
         global _fused_backward_params
         x, y, saved, gamma, beta = ctx.saved_tensors
-        w_p, b_p, g_p, be_p, w2_p, b2_p = ctx.params
-        pending = ctx.link.get("wgrad") if ctx.link is not None else None
+        params = ctx.params   # w, b, gamma, beta, w2, b2
         # gradient accumulation (accumulate_into): the buffers of the earlier micro-batches, added to by the kernel
         # (only when layer 2's kernel accumulated too)
-        acc = _take_accumulated((w_p, b_p, g_p, be_p, w2_p, b2_p)) if pending is not None and ctx.link.get("accumulated") else None
+        acc = _take_accumulated(params) if ctx.link.get("accumulated") else None
         if acc is not None:
-            dw, db, dg, dbe = acc[:4]
+            dw, db, dg, dbe, dw2, db2 = acc
         else:
+            w_p, b_p, g_p, be_p, w2_p, b2_p = params
             dw = _grad_dst(w_p, w_p)
             db = _grad_dst(b_p, b_p) if b_p is not None else None
             dg = _grad_dst(g_p, gamma)
             dbe = _grad_dst(be_p, beta)
-        fresh = all(q is None or q.grad is None for q in (w_p, b_p, g_p, be_p, w2_p, b2_p))
-        pending = ctx.link.pop("wgrad", None) if ctx.link is not None else None
-        dw2 = db2 = None
-        if pending is not None:
-            dy2, p1, dysum2 = pending   # dy2 = p1 = None: layer 2's kernel left the per-image partials
-            if acc is not None:
-                dw2, db2 = acc[4:]
-            else:
-                dw2 = _grad_dst(w2_p, w2_p)
-                db2 = _grad_dst(b2_p, b2_p) if b2_p is not None else None
-            sgd = None
-            prev = ctx.link.pop("prev", None)
-            rider = _sgd_rider if _sgd_rider_enabled else None
-            if rider is not None and prev is not None and prev[4] and fresh:
-                mine = [w_p, b_p, g_p, be_p, w2_p, b2_p] + [q for q, _ in prev[:4]]
-                if len(mine) == len(rider["params"]) and all(a is b for a, b in zip(mine, rider["params"])):
-                    # autograd has accumulated layer 2's gradients by now (AccumulateGrad runs as soon as its input is ready): they
-                    # must be exactly the tensors layer 2's kernel wrote
-                    grads = [q.grad if q is not None else None for q, _ in prev[:4]]
-                    if all((g is None and ptr == 0) or (g is not None and g.data_ptr() == ptr) for g, (_, ptr) in zip(grads, prev[:4])):
-                        sgd = rider["args"](grads)   # None when the optimizer cannot ride this iteration
-            _C.convnet_l1_bwd_wgrad(dp.contiguous(), y, x, saved, gamma, beta, dg, dbe, dw, db, dy2, p1, dysum2, dw2, db2, sgd,
-                                    accumulate=acc is not None)
-            prev = prev if prev is not None else ()
-            if len(prev) == 5 and prev[0][1] != 0:   # the classifier's gradient came from layer 2's kernel: all ten are the fused kernels'
-                _fused_backward_params = [w_p, b_p, g_p, be_p, w2_p, b2_p] + [q for q, _ in prev[:4]]
-        else:
-            _C.convnet_l1_bwd(dp.contiguous(), y, x, saved, gamma, beta, dg, dbe, dw, db)
+            dw2 = _grad_dst(w2_p, w2_p)
+            db2 = _grad_dst(b2_p, b2_p) if b2_p is not None else None
+        fresh = all(q is None or q.grad is None for q in params)
+        # layer 2's kernel left conv2's per-image weight-gradient partials; this kernel folds them with its Σdy rows
+        dysum2 = ctx.link.pop("dysum")
+        prev = ctx.link.pop("prev")
+        sgd = None
+        rider = _sgd_rider if _sgd_rider_enabled else None
+        if rider is not None and prev[4] and fresh:
+            mine = list(params) + [q for q, _ in prev[:4]]
+            if len(mine) == len(rider["params"]) and all(a is b for a, b in zip(mine, rider["params"])):
+                # autograd has accumulated layer 2's gradients by now (AccumulateGrad runs as soon as its input is ready): they
+                # must be exactly the tensors layer 2's kernel wrote
+                grads = [q.grad if q is not None else None for q, _ in prev[:4]]
+                if all((g is None and ptr == 0) or (g is not None and g.data_ptr() == ptr) for g, (_, ptr) in zip(grads, prev[:4])):
+                    sgd = rider["args"](grads)   # None when the optimizer cannot ride this iteration
+        _C.convnet_l1_bwd_wgrad(dp.contiguous(), y, x, saved, gamma, beta, dg, dbe, dw, db, None, None, dysum2, dw2, db2, sgd,
+                                accumulate=acc is not None)
+        _fused_backward_params = list(params) + [q for q, _ in prev[:4]]
         return None, dw, db, dg, dbe, None, None, None, None, None, dw2, db2, None, None
 
 
 class _FusedLayer2(torch.autograd.Function):
-    """conv2 (wgmma) + BN2 + ReLU + pool2 (+ the classifier's logits, which ride on the pooled activations while they
-    are still in shared memory) forward; pool/ReLU/BN backward + conv2 data gradient as one kernel backward.  The
-    tensor-core weight gradient follows as its own kernel, or — the default — its per-image partials are computed in this
-    node's kernel and folded by layer 1's backward kernel."""
+    """conv2 (wgmma) + BN2 + ReLU + pool2 + the classifier's logits, forward (produced by the whole-forward launch of layer 1's
+    node); the classifier's backward + pool/ReLU/BN backward + conv2 data gradient + the per-image partials of conv2's weight
+    gradient as one kernel backward.  Layer 1's backward kernel folds those partials."""
 
     @staticmethod
-    def forward(ctx, p1, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, fcw, fcb, whole=None, link=None, fc_rides=False):
-        if whole is not None and "layer2" in whole:
-            out, y, saved, logits = whole.pop("layer2")   # produced by the whole-forward launch of layer 1's node
-        else:
-            out, y, saved, logits = _C.convnet_l2_fwd(p1, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, fcw, fcb)
+    def forward(ctx, p1, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, fcw, fcb, whole, link):
+        out, y, saved, logits = whole.pop("layer2")
         ctx.params = (w, b, gamma, beta, fcw, fcb)
         ctx.link = link
-        ctx.fc_rides = fc_rides
-        ctx.ce_deferred = whole.get("ce_deferred") if (whole is not None and fc_rides) else None
-        if fc_rides:
-            # the classifier's backward runs inside this node's backward kernel: the logits are this node's differentiable output
-            ctx.save_for_backward(p1, y, saved, gamma, beta, w, out, fcw)
-            ctx.set_materialize_grads(False)
-        else:
-            ctx.save_for_backward(p1, y, saved, gamma, beta, w)
-            ctx.mark_non_differentiable(logits)
+        ctx.ce_deferred = whole.get("ce_deferred")
+        # the classifier's backward runs inside this node's backward kernel: the logits are this node's differentiable output
+        ctx.save_for_backward(p1, y, saved, gamma, beta, w, out, fcw)
+        ctx.set_materialize_grads(False)
         return out, logits  # [B,32,7,7] NCHW, [B,classes]
 
     @staticmethod
     def backward(ctx, dout, dlogits):
         w_p, b_p, g_p, be_p, fcw_p, fcb_p = ctx.params
-        # layer 1's backward kernel folds (and layer 1's node returns) conv2's weight / bias gradient; this kernel computes the
-        # per-image partials (given p1) for it
-        rides = ctx.link is not None and ctx.needs_input_grad[0]
+        p1, y, saved, gamma, beta, w, out, fcw = ctx.saved_tensors
+        if dout is not None:
+            raise RuntimeError("fused ConvNet: the pooled activations of the fused classifier path must not be used outside the model")
+        # do the gradients written here become `.grad` as they are (nothing to accumulate into)?
+        fresh = all(q is None or q.grad is None for q in (fcw_p, fcb_p, g_p, be_p))
         # gradient accumulation (accumulate_into): this kernel and layer 1's add into the earlier micro-batches' buffers
-        acc = _take_accumulated((g_p, be_p, fcw_p, fcb_p)) if ctx.fc_rides and rides else None
+        acc = _take_accumulated((g_p, be_p, fcw_p, fcb_p))
+        ctx.link["accumulated"] = acc is not None
+        lp, lo = ctx.ce_deferred if ctx.ce_deferred is not None else (None, None)
         if acc is not None:
-            ctx.link["accumulated"] = True
-            dg, dbe = acc[:2]
+            dg, dbe, dfcw, dfcb = acc
+            if lp is not None:   # the step's loss adds up over the micro-batches too
+                lo = _accumulate["loss"]
+                if lo is None:
+                    raise RuntimeError("gradient accumulation: the deferred loss of this micro-batch has no buffer to add into")
         else:
-            dg = _grad_dst(g_p, ctx.saved_tensors[3])
-            dbe = _grad_dst(be_p, ctx.saved_tensors[4])
-        dfcw = dfcb = None
-        if ctx.link is not None:   # do the gradients written here become `.grad` as they are (nothing to accumulate into)?
-            ctx.link["prev_fresh"] = ctx.fc_rides and all(q is None or q.grad is None for q in (fcw_p, fcb_p, g_p, be_p))
-        if ctx.fc_rides:
-            p1, y, saved, gamma, beta, w, out, fcw = ctx.saved_tensors
-            if dout is not None:
-                raise RuntimeError("fused ConvNet: the pooled activations of the fused classifier path must not be used outside the model")
-            lp, lo = ctx.ce_deferred if ctx.ce_deferred is not None else (None, None)
-            if acc is not None:
-                dfcw, dfcb = acc[2:]
-                if lp is not None:   # the step's loss adds up over the micro-batches too
-                    lo = _accumulate["loss"]
-                    if lo is None:
-                        raise RuntimeError("gradient accumulation: the deferred loss of this micro-batch has no buffer to add into")
-            else:
-                dfcw = _grad_dst(fcw_p, fcw)
-                dfcb = _grad_dst(fcb_p, fcb_p) if fcb_p is not None else None
-            dy, dp1, dysum = _C.convnet_l2_bwd_fc(dlogits.contiguous(), fcw, out, dfcw, dfcb, y, saved, gamma, beta, w, dg, dbe, lp, lo,
-                                                  p1 if rides else None, accumulate=acc is not None)
-        else:
-            p1, y, saved, gamma, beta, w = ctx.saved_tensors
-            dy, dp1, dysum = _C.convnet_l2_bwd(dout.contiguous(), y, saved, gamma, beta, w, dg, dbe, p1 if rides else None)
-        if rides:
-            ctx.link["wgrad"] = (None, None, dysum)
-            # for the optimizer rider of layer 1's kernel: WHERE these gradients were written — addresses, not tensors (an extra
-            # reference would make autograd's AccumulateGrad clone the gradient instead of adopting the bucket view)
-            ctx.link["prev"] = ((fcw_p, dfcw.data_ptr() if dfcw is not None else 0), (fcb_p, dfcb.data_ptr() if dfcb is not None else 0),
-                                (g_p, dg.data_ptr()), (be_p, dbe.data_ptr()), ctx.link.pop("prev_fresh", False))
-            return dp1, None, None, dg, dbe, None, None, None, None, None, dfcw, dfcb, None, None, None
-        dw = _grad_dst(w_p, w)
-        db = _grad_dst(b_p, b_p) if b_p is not None else None
-        # dy and p1 are zero-haloed frames: every operand of the tensor-core weight gradient arrives by TMA
-        _C.conv5x5_wgrad_win(dy, p1, dysum, dw, db)
-        return dp1, dw, db, dg, dbe, None, None, None, None, None, dfcw, dfcb, None, None, None
-
-
-class _FusedClassifier(torch.autograd.Function):
-    """Autograd node of the classifier whose forward value was already produced by the layer-2 kernel."""
-
-    @staticmethod
-    def forward(ctx, feat, w, b, logits):
-        ctx.save_for_backward(feat, w)
-        ctx.params = (w, b)
-        return logits.view_as(logits)
-
-    @staticmethod
-    def backward(ctx, dout):
-        feat, w = ctx.saved_tensors
-        w_p, b_p = ctx.params
-        dw = _grad_dst(w_p, w)
-        db = _grad_dst(b_p, b_p) if b_p is not None else None
-        dx = _C.linear_bwd(dout.contiguous(), feat.reshape(feat.shape[0], -1), w, True, dw, db)
-        return dx.view_as(feat), dw, db, None
+            dg = _grad_dst(g_p, gamma)
+            dbe = _grad_dst(be_p, beta)
+            dfcw = _grad_dst(fcw_p, fcw)
+            dfcb = _grad_dst(fcb_p, fcb_p) if fcb_p is not None else None
+        # given p1, the kernel computes conv2's per-image weight-gradient partials for layer 1's kernel to fold
+        _, dp1, dysum = _C.convnet_l2_bwd_fc(dlogits.contiguous(), fcw, out, dfcw, dfcb, y, saved, gamma, beta, w, dg, dbe, lp, lo, p1,
+                                             accumulate=acc is not None)
+        ctx.link["dysum"] = dysum
+        # for the optimizer rider of layer 1's kernel: WHERE these gradients were written — addresses, not tensors (an extra
+        # reference would make autograd's AccumulateGrad clone the gradient instead of adopting the bucket view)
+        ctx.link["prev"] = ((fcw_p, dfcw.data_ptr()), (fcb_p, dfcb.data_ptr() if dfcb is not None else 0),
+                            (g_p, dg.data_ptr()), (be_p, dbe.data_ptr()), fresh)
+        return dp1, None, None, dg, dbe, None, None, None, None, None, dfcw, dfcb, None, None
 
 
 def fused_convnet_forward(x: torch.Tensor, model) -> torch.Tensor:
-    """The reference ConvNet's training forward as ONE kernel (two with PDT_FUSED_WHOLE_FWD=0) (ref: ddp_example.py:36-41)."""
+    """The reference ConvNet's training forward as ONE kernel (ref: ddp_example.py:36-41)."""
     c1, b1, c2, b2_bn, fc = model.layer1[0], model.layer1[1], model.layer2[0], model.layer2[1], model.fc
-    # the classifier's backward rides on layer 2's backward kernel (PDT_FC_MERGED=0: separate linear_bwd launch)
-    fc_rides = (os.environ.get("PDT_FC_MERGED", "1") != "0" and hasattr(_C, "convnet_l2_bwd_fc") and fc.weight.shape[0] <= 16
-                and fc.weight.requires_grad and c2.weight.requires_grad and fc.weight.data_ptr() % 16 == 0)
-    whole = None
-    if os.environ.get("PDT_FUSED_WHOLE_FWD", "1") != "0" and fc.weight.shape[0] <= 16 and hasattr(_C, "convnet_fwd"):
-        whole = {"conv2": c2, "bn2": b2_bn, "fc": fc}
-        t = _upcoming_target
-        if (t is not None and os.environ.get("PDT_FUSED_CE", "1") != "0" and t.is_cuda and t.dtype == torch.int64 and t.dim() == 1
-                and t.shape[0] == x.shape[0] and t.is_contiguous() and torch.is_grad_enabled()):
-            whole["target"] = t
-            whole["defer_loss_mean"] = bool(_loss_read_after_backward and fc_rides)
-            whole["grad_scale"] = _upcoming_grad_scale
+    whole = {"conv2": c2, "bn2": b2_bn, "fc": fc}
+    t = _upcoming_target
+    if (t is not None and t.is_cuda and t.dtype == torch.int64 and t.dim() == 1 and t.shape[0] == x.shape[0] and t.is_contiguous()
+            and torch.is_grad_enabled()):
+        whole["target"] = t
+        whole["defer_loss_mean"] = bool(_loss_read_after_backward)
+        whole["grad_scale"] = _upcoming_grad_scale
     # conv2's weight gradient is produced by layer 1's backward kernel: layer 1's node owns (w2, b2) for autograd, `link` carries
-    # the operands from layer 2's backward to it.  Only when conv1's parameters need gradients (layer 1's backward runs at all).
-    link = {} if (_wgrad_rides_on_layer1() and c1.weight.requires_grad and c2.weight.requires_grad) else None
-    w2, b2 = (c2.weight, c2.bias) if link is not None else (None, None)
+    # the operands from layer 2's backward to it
+    link = {}
     p1 = _FusedLayer1.apply(x, c1.weight, c1.bias, b1.weight, b1.bias, b1.running_mean, b1.running_var, b1.num_batches_tracked,
-                            float(b1.momentum), float(b1.eps), w2, b2, whole, link)
-    p2, logits = _FusedLayer2.apply(p1, c2.weight, c2.bias, b2_bn.weight, b2_bn.bias, b2_bn.running_mean, b2_bn.running_var,
-                                    b2_bn.num_batches_tracked, float(b2_bn.momentum), float(b2_bn.eps), fc.weight, fc.bias, whole, link, fc_rides)
-    if whole is not None and whole.get("target") is not None:
-        logits = logits if fc_rides else _FusedClassifier.apply(p2, fc.weight, fc.bias, logits)
+                            float(b1.momentum), float(b1.eps), c2.weight, c2.bias, whole, link)
+    _, logits = _FusedLayer2.apply(p1, c2.weight, c2.bias, b2_bn.weight, b2_bn.bias, b2_bn.running_mean, b2_bn.running_var,
+                                   b2_bn.num_batches_tracked, float(b2_bn.momentum), float(b2_bn.eps), fc.weight, fc.bias, whole, link)
+    if whole.get("target") is not None:
         # (target, loss, dlogits, scale of loss and gradient, loss folded by layer 2's backward kernel) for ops.cross_entropy
         logits._pdt_ce = (whole["target"],) + whole["ce"] + (float(whole.get("grad_scale", 1.0)), whole["ce_deferred"] is not None)
-        return logits
-    if fc_rides:
-        return logits
-    return _FusedClassifier.apply(p2, fc.weight, fc.bias, logits)
+    return logits
 
 
 def conv_bn_relu_pool(x: torch.Tensor, conv: torch.nn.Conv2d, bn: torch.nn.Module, out_nchw: Optional[bool] = None,

@@ -1,6 +1,6 @@
 """conv2's weight gradient split over the two backward kernels: the layer-2 backward kernel computes the per-image partials
 (given conv2's input frame p1), the layer-1 backward kernel folds them.  Checked against the stand-alone form of the layer-1
-binding fed the dy frame of the non-riding layer-2 kernel (bit for bit), against float64, and in a graphed training step against
+binding fed the dy frame the layer-2 kernel writes without p1 (bit for bit), against float64, and in a graphed training step against
 the same step without the optimizer riding on the backward kernels."""
 import pytest
 import torch
@@ -26,26 +26,23 @@ def _layer_inputs(B, ncls, seed):
     r = lambda *s: torch.randn(*s, device=dev(), generator=g)   # noqa: E731
     x1 = torch.rand(B, 1, 28, 28, device=dev(), generator=g)
     w1, b1, g1, be1 = r(16, 1, 5, 5) * 0.2, r(16) * 0.1, torch.rand(16, device=dev(), generator=g) + 0.5, r(16) * 0.1
-    p1, y1, sv1 = _C.convnet_l1_fwd(x1, w1, b1, g1, be1, None, None, None, 0.1, 1e-5)
     w2, b2, g2, be2 = r(32, 16, 5, 5) * 0.05, r(32) * 0.1, torch.rand(32, device=dev(), generator=g) + 0.5, r(32) * 0.1
     fcw, fcb = r(ncls, 1568) * 0.02, r(ncls) * 0.1
-    out, y2, sv2, _ = _C.convnet_l2_fwd(p1, w2, b2, g2, be2, None, None, None, 0.1, 1e-5, fcw, fcb)
-    dlogits, dout = r(B, ncls) / B, r(B, 32, 7, 7)
+    p1, y1, sv1, out, y2, sv2, *_ = _C.convnet_fwd(x1, w1, b1, g1, be1, None, None, None, 0.1, 1e-5, w2, b2, g2, be2, None, None, None,
+                                                   0.1, 1e-5, fcw, fcb)
+    dlogits = r(B, ncls) / B
     dp1 = torch.zeros(B, 18, 18, 16, device=dev())
     dp1[:, 2:16, 2:16, :] = r(B, 14, 14, 16)
     return dict(x1=x1, g1=g1, be1=be1, p1=p1, y1=y1, sv1=sv1, w2=w2, g2=g2, be2=be2, fcw=fcw, out=out, y2=y2, sv2=sv2,
-                dlogits=dlogits, dout=dout, dp1=dp1)
+                dlogits=dlogits, dp1=dp1)
 
 
-def _layer2_bwd(d, fc, p1=None):
-    """(dy or None, dx, dysum, [dg, dbe, dfcw, dfcb]) of the layer-2 backward kernel, the classifier riding on it or not."""
-    grads = [torch.full((32,), 7.0, device=dev()), torch.full((32,), 7.0, device=dev())]
-    if fc:
-        grads += [torch.full_like(d["fcw"], 7.0), torch.full((d["fcw"].shape[0],), 7.0, device=dev())]
-        res = _C.convnet_l2_bwd_fc(d["dlogits"], d["fcw"], d["out"], grads[2], grads[3], d["y2"], d["sv2"], d["g2"], d["be2"], d["w2"],
-                                   grads[0], grads[1], p1=p1)
-    else:
-        res = _C.convnet_l2_bwd(d["dout"], d["y2"], d["sv2"], d["g2"], d["be2"], d["w2"], grads[0], grads[1], p1=p1)
+def _layer2_bwd(d, p1=None):
+    """(dy or None, dx, dysum, [dg, dbe, dfcw, dfcb]) of the layer-2 backward kernel."""
+    grads = [torch.full((32,), 7.0, device=dev()), torch.full((32,), 7.0, device=dev()), torch.full_like(d["fcw"], 7.0),
+             torch.full((d["fcw"].shape[0],), 7.0, device=dev())]
+    res = _C.convnet_l2_bwd_fc(d["dlogits"], d["fcw"], d["out"], grads[2], grads[3], d["y2"], d["sv2"], d["g2"], d["be2"], d["w2"],
+                               grads[0], grads[1], p1=p1)
     return (*res, grads)
 
 
@@ -55,14 +52,13 @@ def _l1_outputs():
 
 
 @pytest.mark.parametrize("ncls", [10, 16])
-@pytest.mark.parametrize("fc", [True, False], ids=["fc_rides", "fc_apart"])
 @pytest.mark.parametrize("B", [1, 3, 100, "sms"])
-def test_layer2_partials_folded_by_layer1_match_the_standalone_path(B, fc, ncls):
+def test_layer2_partials_folded_by_layer1_match_the_standalone_path(B, ncls):
     if B == "sms":
         B = torch.cuda.get_device_properties(0).multi_processor_count
-    d = _layer_inputs(B, ncls, seed=B * 31 + ncls + (7 if fc else 0))
-    dy, dx, dysum, grads = _layer2_bwd(d, fc)
-    none, dx_r, dysum_r, grads_r = _layer2_bwd(d, fc, p1=d["p1"])
+    d = _layer_inputs(B, ncls, seed=B * 31 + ncls + 7)
+    dy, dx, dysum, grads = _layer2_bwd(d)
+    none, dx_r, dysum_r, grads_r = _layer2_bwd(d, p1=d["p1"])
     assert none is None, "with p1 the layer-2 kernel does not write the dy frame"
     # everything else the layer-2 kernel produces is unchanged
     assert torch.equal(dx_r[:, 2:16, 2:16, :], dx[:, 2:16, 2:16, :]) and torch.equal(dysum_r, dysum)
@@ -70,20 +66,18 @@ def test_layer2_partials_folded_by_layer1_match_the_standalone_path(B, fc, ncls)
         assert torch.equal(got, want)
 
     common = (d["dp1"], d["y1"], d["x1"], d["sv1"], d["g1"], d["be1"])
-    plain = _l1_outputs()
-    _C.convnet_l1_bwd(*common, *plain)
     ref, chain = _l1_outputs(), _l1_outputs()
     dw_ref, db_ref = torch.full((32, 16, 5, 5), 7.0, device=dev()), torch.full((32,), 7.0, device=dev())
     dw_c, db_c = torch.full_like(dw_ref, 7.0), torch.full_like(db_ref, 7.0)
-    # the stand-alone form (per-image kernel on the given frames, then layer 1), fed the non-riding kernel's dy frame
+    # the stand-alone form (per-image kernel on the given frames, then layer 1), fed the dy frame of the form without p1
     _C.convnet_l1_bwd_wgrad(*common, *ref, dy, d["p1"], dysum, dw_ref, db_ref)
     # the chain: layer 2 (p1 given) left the partials, layer 1 folds them.  Layer 2 runs again so that its partials are the pending ones.
-    _layer2_bwd(d, fc, p1=d["p1"])
+    _layer2_bwd(d, p1=d["p1"])
     _C.convnet_l1_bwd_wgrad(*common, *chain, None, None, dysum_r, dw_c, db_c)
     assert torch.equal(dw_c, dw_ref), (dw_c - dw_ref).abs().max().item()
     assert torch.equal(db_c, db_ref)
-    for got, want, ref_out in zip(chain, plain, ref):
-        assert torch.equal(got, want) and torch.equal(ref_out, want)
+    for got, want in zip(chain, ref):
+        assert torch.equal(got, want)
 
     # float64 conv2d_weight on the TF32-rounded (rna) operands; the kernel accumulates in fp32 (256 positions per image, then B rows)
     xi = tf32_rna(d["p1"][:, 2:16, 2:16, :]).permute(0, 3, 1, 2).double()
@@ -100,7 +94,7 @@ def test_layer1_without_frames_needs_pending_partials():
     d = _layer_inputs(3, 10, seed=5)
     common = (d["dp1"], d["y1"], d["x1"], d["sv1"], d["g1"], d["be1"])
     dw2, db2 = torch.empty(32, 16, 5, 5, device=dev()), torch.empty(32, device=dev())
-    _layer2_bwd(d, True, p1=d["p1"])
+    _layer2_bwd(d, p1=d["p1"])
     _C.convnet_l1_bwd_wgrad(*common, *_l1_outputs(), None, None, torch.zeros(3, 32, device=dev()), dw2, db2)
     with pytest.raises(RuntimeError, match="none are pending"):   # consumed by the call above
         _C.convnet_l1_bwd_wgrad(*common, *_l1_outputs(), None, None, torch.zeros(3, 32, device=dev()), dw2, db2)

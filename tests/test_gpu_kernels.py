@@ -225,16 +225,13 @@ def test_convnet_fused_matches_unfused(syncbn_module):
     assert torch.allclose(net(x).double(), ref(x.double()), atol=3e-2, rtol=1e-2)
 
 
-@pytest.mark.parametrize("riders", ["11", "00", "10", "01"])
 @pytest.mark.parametrize("B", [100, 3, "sms"])   # "sms": one image per SM, i.e. one CTA on every SM of the device
-def test_cooperative_fused_layers_match_per_op_kernels(B, riders, monkeypatch):
-    """csrc/cuda/fused_convnet.cu (one cooperative kernel per layer and direction, grid barrier for the batch
-    statistics) against the per-op kernels on the same weights and data: same TF32 convolution, same fp32 rest —
-    only summation orders differ."""
+def test_cooperative_fused_layers_match_per_op_kernels(B, monkeypatch):
+    """csrc/cuda/fused_convnet.cu (one cooperative kernel for the forward and one per layer for the backward, grid barriers
+    for the batch statistics) against the per-op kernels on the same weights and data: same TF32 convolution, same fp32
+    rest — only summation orders differ."""
     if B == "sms":
         B = torch.cuda.get_device_properties(0).multi_processor_count
-    monkeypatch.setenv("PDT_WGRAD_MERGED", riders[0])   # conv2 weight gradient inside the layer-1 backward kernel / as its own kernel
-    monkeypatch.setenv("PDT_FC_MERGED", riders[1])      # classifier backward inside the layer-2 backward kernel / as its own kernel
     torch.manual_seed(2)
     a = pdt.models.ConvNet(fused=True).to(dev())
     b = pdt.models.ConvNet(fused=True).to(dev())
@@ -266,20 +263,30 @@ def test_cooperative_layer2_exact_on_small_integers():
     """Integer-valued inputs/weights are exact in TF32 and in fp32 accumulation: the fused conv2 forward (window
     descriptors over the haloed image) and data gradient must reproduce a float64 convolution bit for bit."""
     B = 5
-    p1 = torch.zeros(B, 18, 18, 16, device=dev())   # zero-haloed frame
-    p1[:, 2:16, 2:16, :] = torch.randint(-3, 4, (B, 14, 14, 16), device=dev()).float()
+    # layer 1 with BN1's gamma = 0: the pooled frame p1 is relu(beta) = beta inside an exact zero halo, a distinct small integer
+    # per channel, so that the border rows of both output tiles and every 16-byte swizzle chunk of a patch row carry distinct values
+    x1 = torch.rand(B, 1, 28, 28, device=dev())
+    w1, b1 = torch.randn(16, 1, 5, 5, device=dev()) * 0.2, torch.randn(16, device=dev()) * 0.1
+    be1 = (torch.randperm(16, device=dev()) + 1).float()
     w = torch.randint(-2, 3, (32, 16, 5, 5), device=dev()).float()
     bias = torch.randint(-2, 3, (32,), device=dev()).float()
     gamma, beta = torch.ones(32, device=dev()), torch.zeros(32, device=dev())
-    out, y, saved, logits = _C.convnet_l2_fwd(p1, w, bias, gamma, beta, None, None, None, 0.1, 1e-5, None, None)
+    fcw, fcb = torch.randn(10, 1568, device=dev()) * 0.02, torch.randn(10, device=dev()) * 0.1
+    p1, y1, sv1, out, y, saved, logits, *_ = _C.convnet_fwd(x1, w1, b1, torch.zeros(16, device=dev()), be1, None, None, None, 0.1, 1e-5,
+                                                            w, bias, gamma, beta, None, None, None, 0.1, 1e-5, fcw, fcb)
+    frame = torch.zeros(B, 18, 18, 16, device=dev())
+    frame[:, 2:16, 2:16, :] = be1
+    assert torch.equal(p1, frame)
     ref = F.conv2d(p1[:, 2:16, 2:16, :].permute(0, 3, 1, 2).double(), w.double(), bias.double(), padding=2)
     assert torch.equal(y.permute(0, 3, 1, 2).double(), ref)
     mean = ref.mean((0, 2, 3))
     assert torch.allclose(saved[:32].double(), mean, atol=1e-4, rtol=1e-5)
-    # data gradient: feed a gradient that passes the pool/ReLU/BN backward, compare the conv part through dy
-    dout = torch.randn(B, 32, 7, 7, device=dev())
+    # data gradient: feed a gradient that passes the classifier and pool/ReLU/BN backward, compare the conv part through dy (the
+    # form without p1 writes the dy frame)
+    dlogits = torch.randn(B, 10, device=dev())
+    dfcw, dfcb = torch.empty_like(fcw), torch.empty_like(fcb)
     dg, db = torch.empty(32, device=dev()), torch.empty(32, device=dev())
-    dy, dx, dysum = _C.convnet_l2_bwd(dout, y, saved, gamma, beta, w, dg, db)
+    dy, dx, dysum = _C.convnet_l2_bwd_fc(dlogits, fcw, out, dfcw, dfcb, y, saved, gamma, beta, w, dg, db)
     dyi = dy[:, 2:16, 2:16, :]
     halo = dy.clone()
     halo[:, 2:16, 2:16, :] = 0
@@ -288,36 +295,23 @@ def test_cooperative_layer2_exact_on_small_integers():
     err = (dx[:, 2:16, 2:16, :].permute(0, 3, 1, 2).double() - ref_dx).abs().max().item()
     assert err <= 2e-3 * ref_dx.abs().max().item() + 1e-5, err   # dy is not integer valued: TF32 operand rounding
     assert torch.allclose(dysum.sum(0).double(), dyi.double().sum((0, 1, 2)), atol=1e-4)
-    # weight gradient, window formulation (all operands by TMA): exact on integer-valued frames
+    # weight gradient on integer-valued frames, as the layer-1 backward kernel folds it from the per-image partials of the K-major
+    # operand copies (written here from the frames, as the layer-2 backward kernel writes them from its registers): exact
+    xq = torch.zeros(B, 18, 18, 16, device=dev())   # zero-haloed frame
+    xq[:, 2:16, 2:16, :] = torch.randint(-3, 4, (B, 14, 14, 16), device=dev()).float()
     dyq = torch.zeros(B, 18, 18, 32, device=dev())
     dyq[:, 2:16, 2:16, :] = torch.randint(-2, 3, (B, 14, 14, 32), device=dev()).float()
-    dw, dbias = torch.empty(32, 16, 5, 5, device=dev()), torch.empty(32, device=dev())
-    _C.conv5x5_wgrad_win(dyq, p1, dyq[:, 2:16, 2:16, :].sum((1, 2)).contiguous(), dw, dbias)
-    ref_dw = torch.nn.grad.conv2d_weight(p1[:, 2:16, 2:16, :].permute(0, 3, 1, 2).double(), (32, 16, 5, 5),
+    ref_dw = torch.nn.grad.conv2d_weight(xq[:, 2:16, 2:16, :].permute(0, 3, 1, 2).double(), (32, 16, 5, 5),
                                          dyq[:, 2:16, 2:16, :].permute(0, 3, 1, 2).double(), padding=2)
-    assert torch.equal(dw.double(), ref_dw), (dw.double() - ref_dw).abs().max()
-    assert torch.equal(dbias.double(), dyq.double().sum((0, 1, 2)))
-    # the same weight gradient riding on the layer-1 backward kernel (extra TMA warp, mma.sync): still exact, and the
-    # layer-1 results are those of the plain layer-1 backward kernel, bit for bit
-    x1 = torch.rand(B, 1, 28, 28, device=dev())
-    w1, b1 = torch.randn(16, 1, 5, 5, device=dev()) * 0.2, torch.randn(16, device=dev()) * 0.1
-    g1, be1 = torch.rand(16, device=dev()) + 0.5, torch.randn(16, device=dev()) * 0.1
-    _, y1, sv1 = _C.convnet_l1_fwd(x1, w1, b1, g1, be1, None, None, None, 0.1, 1e-5)
     dp1 = torch.zeros(B, 18, 18, 16, device=dev())
     dp1[:, 2:16, 2:16, :] = torch.randn(B, 14, 14, 16, device=dev())
-
-    def l1_outputs():
-        return [torch.full((16,), 7.0, device=dev()), torch.full((16,), 7.0, device=dev()), torch.full((16, 1, 5, 5), 7.0, device=dev()),
-                torch.full((16,), 7.0, device=dev())]
-
-    plain, riding = l1_outputs(), l1_outputs()
-    _C.convnet_l1_bwd(dp1, y1, x1, sv1, g1, be1, *plain)
+    g1 = torch.rand(16, device=dev()) + 0.5
+    l1_out = [torch.full((16,), 7.0, device=dev()), torch.full((16,), 7.0, device=dev()), torch.full((16, 1, 5, 5), 7.0, device=dev()),
+              torch.full((16,), 7.0, device=dev())]
     dw_m, db_m = torch.full((32, 16, 5, 5), 7.0, device=dev()), torch.full((32,), 7.0, device=dev())
-    _C.convnet_l1_bwd_wgrad(dp1, y1, x1, sv1, g1, be1, *riding, dyq, p1, dyq[:, 2:16, 2:16, :].sum((1, 2)).contiguous(), dw_m, db_m)
+    _C.convnet_l1_bwd_wgrad(dp1, y1, x1, sv1, g1, be1, *l1_out, dyq, xq, dyq[:, 2:16, 2:16, :].sum((1, 2)).contiguous(), dw_m, db_m)
     assert torch.equal(dw_m.double(), ref_dw), (dw_m.double() - ref_dw).abs().max()
     assert torch.equal(db_m.double(), dyq.double().sum((0, 1, 2)))
-    for got, want in zip(riding, plain):
-        assert torch.equal(got, want)
 
 
 def test_generic_bn_kernels_match_torch():

@@ -146,12 +146,15 @@ def _rel(ours, ref):
 
 
 def _assert_grads_match_float64(model, ref):
-    named = list(model.named_parameters())
+    # a frozen parameter gets no gradient (the twin computes every one)
+    assert all(p.grad is None for p in model.parameters() if not p.requires_grad)
+    refs = dict(ref.named_parameters())
+    named = [(n, p, refs[n]) for n, p in model.named_parameters() if p.requires_grad]
     # conv biases feed a BatchNorm: their true gradient is zero and what is left is rounding noise
-    keep = [(p, q) for (n, p), q in zip(named, ref.parameters()) if n not in ("layer1.0.bias", "layer2.0.bias")]
+    keep = [(p, q) for n, p, q in named if n not in ("layer1.0.bias", "layer2.0.bias")]
     err = _rel([p.grad for p, _ in keep], [q.grad for _, q in keep])
     assert err < 2e-2, err
-    for (n, p), q in zip(named, ref.parameters()):
+    for n, p, q in named:
         if n in ("layer1.0.bias", "layer2.0.bias"):
             assert (p.grad.double() - q.grad).abs().max().item() < 1e-4, n
 
@@ -355,15 +358,17 @@ def test_criterion_that_stops_returning_the_cross_entropy_is_refused():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("config", ["PDT_WGRAD_MERGED", "PDT_FC_MERGED", "PDT_FUSED_LAYERS", "above_sms"])
+@pytest.mark.parametrize("config", ["PDT_FUSED_LAYERS", "above_sms", "frozen_conv1"])
 def test_fallback_configurations_accumulate_through_autograd(config, monkeypatch):
     k = 2
     b = _sms() + 18 if config == "above_sms" else 100
-    if config != "above_sms":
+    if config == "PDT_FUSED_LAYERS":
         monkeypatch.setenv(config, "0")
     with _one_gpu():
         torch.manual_seed(0)
         model = pdt.models.ConvNet().to(_dev())
+        if config == "frozen_conv1":   # a partially trainable model takes the per-op kernels
+            model.layer1[0].requires_grad_(False)
         opt = pdt.optim.SGD(model.parameters(), lr=0.0)
         x, t = _batch(k, b, 40)
         step = _graphed(model, opt, x, t, k)

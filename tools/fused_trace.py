@@ -35,7 +35,6 @@ names = {0: ("forward (whole)", ["start", "conv1 done", "stats partial written",
                                  "stats 2 partial written", "barrier 2 passed", "pooled 2 in smem", "logits written", "end (incl. loss)", "prologue done (smem zeroed, weights requested)"]),
          1: ("l1_bwd (+conv2 wgrad fold)", ["start", "partial written", "barrier passed", "folded", "conv1 wgrad partial written", "barrier 2 passed",
                                             "end", "dW2 folded"]),
-         2: ("l2_fwd", ["start", "B built + sync", "epilogue done", "partial written", "barrier passed", "folded", "pooled out written", "end"]),
          3: ("l2_bwd (+conv2 wgrad partials)", ["start", "B built", "partial written", "barrier passed", "folded", "dy written", "end",
                                                 "dW2 atoms done (warp 0)"])}
 def report(t, title):

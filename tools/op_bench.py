@@ -85,7 +85,7 @@ def main():
     w2, b2, g2, be2 = c2.weight.detach(), c2.bias.detach(), bn2.weight.detach(), bn2.bias.detach()
     wf, bf = fc.weight.detach(), fc.bias.detach()
 
-    # ---- ours: the cooperative fused kernels a captured step launches (4 per step), plus the stand-alone variants ----------
+    # ---- ours: the cooperative fused kernels a captured step launches, plus the kernels of the plain-loop and per-op paths ---
     rm1, rv1, nb1 = bn1.running_mean, bn1.running_var, bn1.num_batches_tracked
     rm2, rv2, nb2 = bn2.running_mean, bn2.running_var, bn2.num_batches_tracked
 
@@ -96,30 +96,23 @@ def main():
     dwf, dbf = torch.empty_like(wf), torch.empty_like(bf)
     dg2, dbe2 = torch.empty(32, device=dev), torch.empty(32, device=dev)
 
-    def l2_bwd_fc(p1=None):
+    def l2_bwd_fc():
         return _C.convnet_l2_bwd_fc(dlog, wf, p2, dwf, dbf, y2, sv2, g2, be2, w2, dg2, dbe2, lparts, loss, p1)
 
-    dy2, dp1, dysum = l2_bwd_fc()
+    _, dp1, dysum = l2_bwd_fc()
     dw2, db2 = torch.empty_like(w2), torch.empty_like(b2)
     dg1, dbe1, dw1, db1 = torch.empty(16, device=dev), torch.empty(16, device=dev), torch.empty_like(w1), torch.empty_like(b1)
     params = [w1, b1, g1, be1, w2, b2, g2, be2, wf, bf]
     grads = [torch.randn_like(p) for p in params]
-    dflat = torch.randn(B, 32, 7, 7, device=dev)
     ours = [
         ("forward: conv1+BN+ReLU+pool + conv2(wgmma)+BN+ReLU+pool + fc + cross-entropy (1 kernel)", fwd_whole),
-        ("backward A: classifier bwd + pool/ReLU/BN2 bwd + conv2 dgrad(wgmma) + conv2 wgrad partials(mma.sync, window) (1 kernel)",
-         lambda: l2_bwd_fc(p1)),
+        ("backward A: classifier bwd + pool/ReLU/BN2 bwd + conv2 dgrad(wgmma) + conv2 wgrad partials(wgmma) (1 kernel)",
+         l2_bwd_fc),
         ("backward A + B: the row above, then pool/ReLU/BN1 bwd + conv1 wgrad(mma.sync) + conv2 wgrad fold (2 kernels)",
-         lambda: (l2_bwd_fc(p1), _C.convnet_l1_bwd_wgrad(dp1, y1, x, sv1, g1, be1, dg1, dbe1, dw1, db1, None, None, dysum, dw2, db2))),
-        ("(variant) layer-2 bwd without the conv2 wgrad partials", l2_bwd_fc),
-        ("(variant) conv2 wgrad partials from given frames + layer-1 bwd with the fold (2 kernels)",
-         lambda: _C.convnet_l1_bwd_wgrad(dp1, y1, x, sv1, g1, be1, dg1, dbe1, dw1, db1, dy2, p1, dysum, dw2, db2)),
+         lambda: (l2_bwd_fc(), _C.convnet_l1_bwd_wgrad(dp1, y1, x, sv1, g1, be1, dg1, dbe1, dw1, db1, None, None, dysum, dw2, db2))),
         ("SGD, 10 tensors (1 kernel)", lambda: _C.sgd_multi(params, grads, [], 1e-4, None, 0.0, 0.0, 0.0, False, False, False)),
         ("(variant) cross-entropy fwd (+dlogits) as its own kernel", lambda: _C.cross_entropy_fwd(logits, tgt, True)),
         ("(variant) fc bwd as its own kernel", lambda: _C.linear_bwd(dlog, p2.reshape(B, -1), wf, True, dwf, dbf)),
-        ("(variant) layer-2 bwd without the classifier rider", lambda: _C.convnet_l2_bwd(dflat, y2, sv2, g2, be2, w2, dg2, dbe2)),
-        ("(variant) conv2 wgrad as its own kernel (TMA-materialised tap pairs + in-kernel fold)", lambda: _C.conv5x5_wgrad_win(dy2, p1, dysum, dw2, db2)),
-        ("(variant) layer-1 bwd without the wgrad rider", lambda: _C.convnet_l1_bwd(dp1, y1, x, sv1, g1, be1, dg1, dbe1, dw1, db1)),
     ]
 
     # ---- library: the ATen / cuDNN / cuBLAS ops the reference's modules dispatch to, same shapes -----------------------
