@@ -9,7 +9,8 @@ Extra flags cover what the reference hard-codes: ``--init-method`` (its LAN addr
 ``tcp://10.9.1.2:34567`` only works on the author's network, ref: ddp_example.py:110; we default
 to loopback with a free port), ``--data synthetic|mnist``, ``--model``, ``--comm fused|nccl``, ``--algo``,
 ``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw), ``--lr``,
-``--momentum``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--checkpoint`` / ``--resume``.
+``--momentum``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--checkpoint`` /
+``--resume``.
 """
 from __future__ import annotations
 
@@ -54,6 +55,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--accumulation-steps", default=1, type=int, metavar="K",
                    help="gradient accumulation: K micro-batches of --batch-size images per optimizer step, each backward of loss / K "
                         "(default 1)")
+    p.add_argument("--label-smoothing", default=0.0, type=float, metavar="EPS",
+                   help="label smoothing of the cross-entropy loss, in [0, 1] (default 0)")
     p.add_argument("--steps", default=0, type=int, help="stop each epoch after this many (optimizer) steps (0 = full epoch)")
     p.add_argument("--samples", default=60000, type=int, help="synthetic dataset size")
     p.add_argument("--graph", default=False, action="store_true", help="capture the whole training step in a CUDA graph")
@@ -83,6 +86,8 @@ def check_args(p: argparse.ArgumentParser, args) -> None:
         p.error(f"--clip-grad-norm must be positive (got {args.clip_grad_norm})")
     if args.accumulation_steps < 1:
         p.error(f"--accumulation-steps must be at least 1 (got {args.accumulation_steps})")
+    if not 0.0 <= args.label_smoothing <= 1.0:
+        p.error(f"--label-smoothing must lie in [0, 1] (got {args.label_smoothing})")
     if args.graph and args.gpus >= 2 and args.accumulation_steps > 1:
         p.error("--graph with --accumulation-steps > 1 runs on one GPU only (-g 1)")
 
@@ -118,7 +123,7 @@ def dist_train(gpu: int, args) -> None:
     model.to(device)
     batch_size = args.batch_size
     accum = args.accumulation_steps
-    criterion = pdt.nn.CrossEntropyLoss().to(device)
+    criterion = pdt.nn.CrossEntropyLoss(label_smoothing=args.label_smoothing).to(device)
     optimizer = make_optimizer(args, model.parameters())
     model = pdt.DistributedDataParallel(model, device_ids=[gpu] if use_cuda else None)
 

@@ -41,6 +41,21 @@ float* opt_mut(c10::optional<at::Tensor>& t, const char* name) {
   return t->data_ptr<float>();
 }
 
+// torch's cross-entropy options for C classes of logits on `like`'s device
+CeSpec ce_spec(const c10::optional<at::Tensor>& weight, int64_t ignore_index, double label_smoothing, const std::string& reduction, int64_t C,
+               const at::Tensor& like, const char* who) {
+  TORCH_CHECK(reduction == "mean" || reduction == "sum", who, ": reduction must be 'mean' or 'sum' (got '", reduction, "')");
+  TORCH_CHECK(label_smoothing >= 0.0 && label_smoothing <= 1.0, who, ": label_smoothing must lie in [0, 1] (got ", label_smoothing, ")");
+  CeSpec s;
+  s.weight = opt_ptr(weight, "weight");
+  if (s.weight != nullptr)
+    TORCH_CHECK(weight->dim() == 1 && weight->size(0) == C && weight->device() == like.device(), who, ": weight must be [", C, "] on ", like.device());
+  s.smoothing = static_cast<float>(label_smoothing);
+  s.ignore_index = ignore_index;
+  s.sum = reduction == "sum";
+  return s;
+}
+
 // Per-device scratch for deterministic cross-CTA reductions. Kernels that use it run on one
 // stream at a time (the compute stream), which is what serialises access.
 struct Scratch {
@@ -374,7 +389,8 @@ void register_cuda_bindings(py::module_& m) {
                           double mom1, double eps1, const at::Tensor& w2, c10::optional<at::Tensor> b2, c10::optional<at::Tensor> g2,
                           c10::optional<at::Tensor> be2, c10::optional<at::Tensor> rm2, c10::optional<at::Tensor> rv2, c10::optional<at::Tensor> nbt2,
                           double mom2, double eps2, const at::Tensor& fcw, c10::optional<at::Tensor> fcb, c10::optional<at::Tensor> target,
-                          bool defer_loss_mean, double grad_scale) {
+                          bool defer_loss_mean, double grad_scale, c10::optional<at::Tensor> ce_weight, int64_t ignore_index,
+                          double label_smoothing, const std::string& reduction) {
     chk(x, "x"); chk(w1, "w1"); chk(w2, "w2"); chk(fcw, "fc weight");
     c10::cuda::CUDAGuard g(x.device());
     TORCH_CHECK(x.numel() % 784 == 0 && w1.numel() == 400 && w2.numel() == 12800 && fcw.dim() == 2 && fcw.size(1) == 1568 && fcw.size(0) <= 16,
@@ -392,12 +408,18 @@ void register_cuda_bindings(py::module_& m) {
     ReduceScratch scr = scratch(x);
     TORCH_CHECK(grad_scale > 0.0, "convnet_fwd: grad_scale must be positive");
     // grad_scale (gradient accumulation over k micro-batches: 1/k): the loss is grad_scale · mean cross-entropy, dlogits its gradient
-    ScaledCe ce;
+    SmoothCe ce;
     ce.scale = static_cast<float>(grad_scale);
     at::Tensor loss, dlogits, loss_parts;
     if (target.has_value() && target->defined()) {
       chk(*target, "target", at::kLong);
       TORCH_CHECK(target->numel() == B, "convnet_fwd: one target per image expected");
+      // ce_weight / ignore_index / label_smoothing / reduction: torch's cross-entropy options (a non-default spec runs SmoothCe)
+      const CeSpec spec = ce_spec(ce_weight, ignore_index, label_smoothing, reduction, ncls, x, "convnet_fwd");
+      ce.weight = spec.weight;
+      ce.smoothing = spec.smoothing;
+      ce.ignore_index = spec.ignore_index;
+      ce.sum = spec.sum;
       loss = at::empty({}, x.options());
       dlogits = at::empty({B, ncls}, x.options());
       loss_parts = at::empty({B + 1}, x.options());   // one term per image, then the number of counted images
@@ -417,7 +439,8 @@ void register_cuda_bindings(py::module_& m) {
   }, py::arg("x"), py::arg("w1"), py::arg("b1"), py::arg("g1"), py::arg("be1"), py::arg("rm1"), py::arg("rv1"), py::arg("nbt1"), py::arg("mom1"),
      py::arg("eps1"), py::arg("w2"), py::arg("b2"), py::arg("g2"), py::arg("be2"), py::arg("rm2"), py::arg("rv2"), py::arg("nbt2"), py::arg("mom2"),
      py::arg("eps2"), py::arg("fcw"), py::arg("fcb"), py::arg("target") = py::none(), py::arg("defer_loss_mean") = false,
-     py::arg("grad_scale") = 1.0);
+     py::arg("grad_scale") = 1.0, py::arg("ce_weight") = py::none(), py::arg("ignore_index") = -100, py::arg("label_smoothing") = 0.0,
+     py::arg("reduction") = "mean");
   // p1 (conv2's input frame [B,18,18,16], optional): conv2's per-image weight-gradient partials are computed inside the kernel for
   // convnet_l1_bwd_wgrad(…, None, None, …) to fold, and the dy frame is not written (None in its place).  The training step always
   // passes p1; the dy frame of the form without it, fed to convnet_l1_bwd_wgrad, is the tests' reference for those partials.
@@ -593,22 +616,29 @@ void register_cuda_bindings(py::module_& m) {
                       dw.data_ptr<float>(), opt_mut(db, "db"), x.size(0), x.size(1), w.size(0), cur_stream(x));
     return dx;
   });
-  m.def("cross_entropy_fwd", [](const at::Tensor& logits, const at::Tensor& target, bool emit_grad) {
+  // weight / ignore_index / label_smoothing / reduction: torch's options (ops_kernels.h: CeSpec); the defaults run the plain mean kernels
+  m.def("cross_entropy_fwd", [](const at::Tensor& logits, const at::Tensor& target, bool emit_grad, c10::optional<at::Tensor> weight,
+                                int64_t ignore_index, double label_smoothing, const std::string& reduction) {
     chk(logits, "logits"); chk(target, "target", at::kLong);
     c10::cuda::CUDAGuard g(logits.device());
+    const CeSpec spec = ce_spec(weight, ignore_index, label_smoothing, reduction, logits.size(1), logits, "cross_entropy_fwd");
     at::Tensor loss = at::empty({}, logits.options()), probs = at::empty_like(logits);
     launch_cross_entropy_fwd(logits.data_ptr<float>(), reinterpret_cast<const long long*>(target.data_ptr<int64_t>()), loss.data_ptr<float>(),
-                             probs.data_ptr<float>(), logits.size(0), logits.size(1), cur_stream(logits), emit_grad);
+                             probs.data_ptr<float>(), logits.size(0), logits.size(1), cur_stream(logits), emit_grad, spec);
     return py::make_tuple(loss, probs);  // emit_grad: the second tensor is d(loss)/d(logits) for a unit incoming gradient
-  }, py::arg("logits"), py::arg("target"), py::arg("emit_grad") = false);
-  m.def("cross_entropy_bwd", [](const at::Tensor& probs, const at::Tensor& target, const at::Tensor& dloss) {
+  }, py::arg("logits"), py::arg("target"), py::arg("emit_grad") = false, py::arg("weight") = py::none(), py::arg("ignore_index") = -100,
+     py::arg("label_smoothing") = 0.0, py::arg("reduction") = "mean");
+  m.def("cross_entropy_bwd", [](const at::Tensor& probs, const at::Tensor& target, const at::Tensor& dloss, c10::optional<at::Tensor> weight,
+                                int64_t ignore_index, double label_smoothing, const std::string& reduction) {
     chk(probs, "probs"); chk(target, "target", at::kLong); chk(dloss, "dloss");
     c10::cuda::CUDAGuard g(probs.device());
+    const CeSpec spec = ce_spec(weight, ignore_index, label_smoothing, reduction, probs.size(1), probs, "cross_entropy_bwd");
     at::Tensor d = at::empty_like(probs);
     launch_cross_entropy_bwd(probs.data_ptr<float>(), reinterpret_cast<const long long*>(target.data_ptr<int64_t>()), dloss.data_ptr<float>(),
-                             d.data_ptr<float>(), probs.size(0), probs.size(1), cur_stream(probs));
+                             d.data_ptr<float>(), probs.size(0), probs.size(1), cur_stream(probs), spec);
     return d;
-  });
+  }, py::arg("probs"), py::arg("target"), py::arg("dloss"), py::arg("weight") = py::none(), py::arg("ignore_index") = -100,
+     py::arg("label_smoothing") = 0.0, py::arg("reduction") = "mean");
 
   // ---- optimizer ------------------------------------------------------------------------------------------
   m.def("sgd_multi", [](std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> bufs, double lr,

@@ -826,6 +826,7 @@ struct L2FwdSmem {
 // zero-haloed shared-memory patch the wgmma descriptors read (the global copy is still written: backward needs it) —
 // and the conv2 weights are staged while conv1 computes.  Two grid barriers (BN1 and BN2 batch statistics), one launch.
 // Ce = ScaledCe: the cross-entropy rider computes scale · (mean cross-entropy) and its gradient (gradient accumulation: 1/k).
+// Ce = SmoothCe: the same with class weights, label smoothing, any ignore_index and the sum (fused_convnet.h).
 // =====================================================================================================================
 __device__ __forceinline__ float ce_scale(const FusedCe&) { return 1.f; }
 __device__ __forceinline__ float ce_scale(const ScaledCe& ce) { return ce.scale; }
@@ -839,6 +840,7 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
                    float* rm2, float* rv2, long long* nbt2, float mom2, float eps2, const float* __restrict__ fcw,
                    const float* __restrict__ fcb, float* __restrict__ logits, int ncls, float* partials, GridSync gs, Ce ce) {
   constexpr bool kScaled = std::is_same_v<Ce, ScaledCe>;
+  constexpr bool kSmooth = std::is_same_v<Ce, SmoothCe>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sa = smem;                                  // conv2 input patch, written by this CTA's layer-1 epilogue
@@ -1007,8 +1009,23 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
     for (int i = tid; i < ncls * 392; i += kL1Threads) cp_async_16(smem_u32(fcs + 4 * i), fcw + 4 * i, 16);
     cp_async_commit();
   }
-  __shared__ int s_counted;
-  if (ce.target != nullptr && warp == 0) {
+  __shared__ std::conditional_t<kSmooth, float, int> s_counted;   // SmoothCe: the divisor D
+  if constexpr (kSmooth) {
+    if (ce.target != nullptr && warp == 0) {
+      // in the barrier's shadow: D = Σ w_t over the counted images (their number without weights) for the mean, 1 for the sum;
+      // every CTA sums the same B ≤ #SM terms in the same order, so all agree bit for bit
+      float d = 0.f;
+      if (!ce.sum) {
+        for (int r = lane; r < B; r += 32) {
+          const long long tr = ce.target[r];
+          if (tr >= 0 && tr < ncls && tr != ce.ignore_index) d += ce.weight ? ce.weight[tr] : 1.f;
+        }
+#pragma unroll
+        for (int off = 16; off >= 1; off >>= 1) d += __shfl_xor_sync(0xffffffffu, d, off);
+      }
+      if (lane == 0) s_counted = ce.sum ? 1.f : d;
+    }
+  } else if (ce.target != nullptr && warp == 0) {
     // in the barrier's shadow: the cross-entropy's mean is over the images whose target lies in [0, ncls) (torch's ignore_index);
     // every CTA counts them, B ≤ one per SM
     int counted = 0;
@@ -1099,7 +1116,7 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
       if (ce.target != nullptr) {
         // cross-entropy of this image and its gradient for a unit incoming gradient, divided by the number of counted images; an
         // ignored image adds no term and gets a zero gradient
-        const int counted = s_counted;
+        const auto counted = s_counted;   // SmoothCe: the divisor D
         float mx = lg;
 #pragma unroll
         for (int off = 16; off >= 1; off >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
@@ -1108,18 +1125,42 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
 #pragma unroll
         for (int off = 16; off >= 1; off >>= 1) ssum += __shfl_xor_sync(0xffffffffu, ssum, off);
         const long long t = ce.target[n];
-        const bool t_ok = t >= 0 && t < ncls;
+        bool t_ok = t >= 0 && t < ncls;
+        if constexpr (kSmooth) t_ok = t_ok && t != ce.ignore_index;
         const float lt = __shfl_sync(0xffffffffu, lg, t_ok ? static_cast<int>(t) : 0);
-        if (lane < ncls) {
-          // ScaledCe: the rounding of autograd's grad · scale behind the unscaled loss
-          if constexpr (kScaled)
-            ce.dlogits[static_cast<size_t>(n) * ncls + lane] = (t_ok ? (e / ssum - (t == lane ? 1.f : 0.f)) / static_cast<float>(counted) : 0.f) * ce.scale;
-          else
-            ce.dlogits[static_cast<size_t>(n) * ncls + lane] = t_ok ? (e / ssum - (t == lane ? 1.f : 0.f)) / static_cast<float>(counted) : 0.f;
+        if constexpr (kSmooth) {
+          // term = (1-ε)·w_t·(lse − l_t) + (ε/C)·Σ_c w_c·(lse − l_c), gradient [(1-ε)·w_t·(p_c − [c=t]) + (ε/C)·(W·p_c − w_c)] / D;
+          // lane c holds w_c, the sums over classes are shuffle reductions
+          const float wc = lane < ncls ? (ce.weight ? ce.weight[lane] : 1.f) : 0.f;
+          const float wt = __shfl_sync(0xffffffffu, wc, t_ok ? static_cast<int>(t) : 0);
+          const float lse = mx + __logf(ssum);
+          float wsum = wc, smooth = lane < ncls ? wc * (lse - lg) : 0.f;
+#pragma unroll
+          for (int off = 16; off >= 1; off >>= 1) {
+            wsum += __shfl_xor_sync(0xffffffffu, wsum, off);
+            smooth += __shfl_xor_sync(0xffffffffu, smooth, off);
+          }
+          const float keep = 1.f - ce.smoothing, eps_c = ce.smoothing / static_cast<float>(ncls);
+          if (lane < ncls) {
+            const float p = e / ssum;
+            ce.dlogits[static_cast<size_t>(n) * ncls + lane] =
+                (t_ok ? (keep * wt * (p - (t == lane ? 1.f : 0.f)) + eps_c * (wsum * p - wc)) / counted : 0.f) * ce.scale;
+          }
+          // D = 0 (a mean over zero total weight): no term, so that either fold gives torch's 0 / 0 = NaN
+          if (lane == 0) ce.loss_parts[n] = t_ok && counted != 0.f ? keep * wt * (lse - lt) + eps_c * smooth : 0.f;
+        } else {
+          if (lane < ncls) {
+            // ScaledCe: the rounding of autograd's grad · scale behind the unscaled loss
+            if constexpr (kScaled)
+              ce.dlogits[static_cast<size_t>(n) * ncls + lane] = (t_ok ? (e / ssum - (t == lane ? 1.f : 0.f)) / static_cast<float>(counted) : 0.f) * ce.scale;
+            else
+              ce.dlogits[static_cast<size_t>(n) * ncls + lane] = t_ok ? (e / ssum - (t == lane ? 1.f : 0.f)) / static_cast<float>(counted) : 0.f;
+          }
+          if (lane == 0) ce.loss_parts[n] = t_ok ? mx + __logf(ssum) - lt : 0.f;
         }
-        if (lane == 0) ce.loss_parts[n] = t_ok ? mx + __logf(ssum) - lt : 0.f;
-        // for a mean folded later (ScaledCe: the divisor is the count over the scale)
-        if (lane == 0 && n == 0) ce.loss_parts[B] = kScaled ? static_cast<float>(counted) / ce_scale(ce) : static_cast<float>(counted);
+        // for a mean folded later (ScaledCe: the divisor is the count over the scale; SmoothCe: D over the scale)
+        if (lane == 0 && n == 0)
+          ce.loss_parts[B] = (kScaled || kSmooth) ? static_cast<float>(counted) / ce_scale(ce) : static_cast<float>(counted);
         if (ce.loss != nullptr) {   // batch mean now (otherwise layer-2 backward folds it: ce.loss == nullptr)
           int last = 0;
           if (lane == 0) {
@@ -1134,7 +1175,7 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
 #pragma unroll
             for (int off = 16; off >= 1; off >>= 1) sl += __shfl_xor_sync(0xffffffffu, sl, off);
             if (lane == 0) {
-              *ce.loss = sl / (kScaled ? static_cast<float>(counted) / ce_scale(ce) : static_cast<float>(counted));
+              *ce.loss = sl / ((kScaled || kSmooth) ? static_cast<float>(counted) / ce_scale(ce) : static_cast<float>(counted));
               *ce.counter = 0u;
             }
           }
@@ -1528,14 +1569,21 @@ void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const 
                         float* rm1, float* rv1, long long* nbt1, float mom1, float eps1, const float* w2, const float* b2, const float* g2,
                         const float* be2, float* y2, float* out, float* saved2, float* rm2, float* rv2, long long* nbt2, float mom2, float eps2,
                         const float* fcw, const float* fcb, float* logits, int ncls, int B, float* partials, GridSync gs, cudaStream_t st,
-                        ScaledCe ce) {
+                        SmoothCe ce) {
   if (logits != nullptr && ncls > 16) throw std::invalid_argument("convnet_fwd: the fused classifier handles at most 16 classes");
   if (ce.target != nullptr && logits == nullptr) throw std::invalid_argument("convnet_fwd: the fused cross-entropy needs the fused classifier");
   if (!(ce.scale > 0.f)) throw std::invalid_argument("convnet_fwd: the cross-entropy scale must be positive");
+  if (!(ce.smoothing >= 0.f && ce.smoothing <= 1.f)) throw std::invalid_argument("convnet_fwd: label smoothing must lie in [0, 1]");
+  if (ce.target != nullptr && !ce.is_default(ncls)) {
+    launch_cooperative(convnet_fwd_kernel<SmoothCe>, B, kL1Threads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1,
+                       saved1, rm1, rv1, nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials,
+                       gs, ce);
+    return;
+  }
   if (ce.target != nullptr && ce.scale != 1.f) {
     launch_cooperative(convnet_fwd_kernel<ScaledCe>, B, kL1Threads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1,
                        saved1, rm1, rv1, nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials,
-                       gs, ce);
+                       gs, static_cast<const ScaledCe&>(ce));
     return;
   }
   launch_cooperative(convnet_fwd_kernel<FusedCe>, B, kL1Threads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1, saved1,

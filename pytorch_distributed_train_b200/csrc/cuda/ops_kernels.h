@@ -99,6 +99,23 @@ void launch_cross_entropy_fwd(const float* logits, const long long* target, floa
 void launch_cross_entropy_bwd(const float* probs, const long long* target, const float* dloss, float* dlogits, int B, int C,
                               cudaStream_t st);
 
+// torch's other cross-entropy options.  A row is counted when its target t lies in [0, C) and is not ignore_index; with class
+// weights w (1 without), W = Σ_c w_c and ε = smoothing, a counted row adds
+//   (1-ε)·w_t·(lse − l_t) + (ε/C)·Σ_c w_c·(lse − l_c)        with gradient   [(1-ε)·w_t·(p_c − [c=t]) + (ε/C)·(W·p_c − w_c)] / D
+// and the loss is Σ terms / D: D = Σ_{counted} w_t for the mean (0 ⇒ NaN), 1 for the sum.  D and W are summed in a fixed order.
+struct CeSpec {
+  const float* weight = nullptr;   // [C] or null
+  float smoothing = 0.f;
+  long long ignore_index = -100;
+  bool sum = false;                // reduction 'sum' (else 'mean')
+  // the default spec is the plain mean above, which runs the kernels without the options
+  bool is_default(int C) const { return weight == nullptr && smoothing == 0.f && !sum && (ignore_index < 0 || ignore_index >= C); }
+};
+void launch_cross_entropy_fwd(const float* logits, const long long* target, float* loss, float* probs, int B, int C, cudaStream_t st,
+                              bool emit_grad, const CeSpec& spec);
+void launch_cross_entropy_bwd(const float* probs, const long long* target, const float* dloss, float* dlogits, int B, int C,
+                              cudaStream_t st, const CeSpec& spec);
+
 // ---- optimizer -------------------------------------------------------------------------------------------
 struct SgdTensorList {
   static constexpr int kMax = 48;

@@ -778,6 +778,92 @@ __global__ void __launch_bounds__(256) cross_entropy_bwd_kernel(const float* __r
   dlogits[i] = (t >= 0 && t < C) ? (probs[i] - (t == c ? 1.f : 0.f)) * g : 0.f;
 }
 
+// ---- the same with a CeSpec (class weights, label smoothing, any ignore_index, sum or mean) ------------------------------------
+__device__ __forceinline__ bool ce_spec_counted(long long t, int C, const CeSpec& s) { return t >= 0 && t < C && t != s.ignore_index; }
+
+// Σ of v over the 256 threads of the block in a fixed order (every thread gets the same bits); red: 256 floats of shared memory
+__device__ float ce_block_sum(float v, float* red) {
+  __syncthreads();
+  red[threadIdx.x] = v;
+  __syncthreads();
+  for (int s = blockDim.x >> 1; s > 0; s >>= 1) {
+    if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+    __syncthreads();
+  }
+  const float r = red[0];
+  __syncthreads();
+  return r;
+}
+
+// The divisor D (Σ_{counted} w_t for the mean, 1 for the sum) and W = Σ_c w_c, the same bits in every block and in both kernels
+__device__ __forceinline__ void ce_spec_sums(const long long* __restrict__ target, int B, int C, const CeSpec& s, float* red, float& D,
+                                             float& W) {
+  float d = 0.f, w = 0.f;
+  if (!s.sum) {
+    for (int r = threadIdx.x; r < B; r += blockDim.x) {
+      const long long t = target[r];
+      if (ce_spec_counted(t, C, s)) d += s.weight ? s.weight[t] : 1.f;
+    }
+  }
+  if (s.weight)
+    for (int c = threadIdx.x; c < C; c += blockDim.x) w += s.weight[c];
+  D = s.sum ? 1.f : ce_block_sum(d, red);
+  W = s.weight ? ce_block_sum(w, red) : static_cast<float>(C);
+}
+
+__global__ void __launch_bounds__(256) cross_entropy_fwd_spec_kernel(const float* __restrict__ logits, const long long* __restrict__ target,
+                                                                     float* loss, float* __restrict__ probs, int B, int C, int emit_grad,
+                                                                     CeSpec s) {
+  __shared__ float red[256];
+  float D, W;
+  ce_spec_sums(target, B, C, s, red, D, W);
+  const float keep = 1.f - s.smoothing, eps_c = s.smoothing / static_cast<float>(C);
+  float local = 0.f;
+  for (int r = threadIdx.x; r < B; r += blockDim.x) {
+    const float* l = logits + static_cast<size_t>(r) * C;
+    float m = l[0];
+    for (int c = 1; c < C; ++c) m = fmaxf(m, l[c]);
+    float sx = 0.f;
+    for (int c = 0; c < C; ++c) sx += __expf(l[c] - m);
+    const float inv = 1.f / sx, lse = m + __logf(sx);
+    const long long t = target[r];
+    const bool counted_row = ce_spec_counted(t, C, s);
+    const float wt = counted_row ? (s.weight ? s.weight[t] : 1.f) : 0.f;
+    float smooth = 0.f;   // Σ_c w_c·(lse − l_c): every term non-negative
+    for (int c = 0; c < C; ++c) {
+      const float lc = l[c], wc = s.weight ? s.weight[c] : 1.f;
+      const float p = __expf(lc - m) * inv;
+      smooth += wc * (lse - lc);
+      probs[static_cast<size_t>(r) * C + c] =
+          !emit_grad ? p : counted_row ? (keep * wt * (p - (t == c ? 1.f : 0.f)) + eps_c * (W * p - wc)) / D : 0.f;
+    }
+    if (counted_row) local += keep * wt * (lse - l[t]) + eps_c * smooth;
+  }
+  const float total = ce_block_sum(local, red);
+  // a mean over zero total weight is NaN, as torch's, also when the smoothing terms of zero-weight rows make the sum positive
+  if (threadIdx.x == 0) *loss = (D == 0.f ? 0.f : total) / D;
+}
+
+__global__ void __launch_bounds__(256) cross_entropy_bwd_spec_kernel(const float* __restrict__ probs, const long long* __restrict__ target,
+                                                                     const float* __restrict__ dloss, float* __restrict__ dlogits, int B, int C,
+                                                                     CeSpec s) {
+  __shared__ float red[256];
+  float D, W;
+  ce_spec_sums(target, B, C, s, red, D, W);
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * C) return;
+  const int r = i / C, c = i % C;
+  const long long t = target[r];
+  if (!ce_spec_counted(t, C, s)) {
+    dlogits[i] = 0.f;
+    return;
+  }
+  const float keep = 1.f - s.smoothing, eps_c = s.smoothing / static_cast<float>(C);
+  const float wt = s.weight ? s.weight[t] : 1.f, wc = s.weight ? s.weight[c] : 1.f, p = probs[i];
+  const float g = (dloss ? *dloss : 1.f) / D;
+  dlogits[i] = (keep * wt * (p - (t == c ? 1.f : 0.f)) + eps_c * (W * p - wc)) * g;
+}
+
 // =====================================================================================================
 // Multi-tensor SGD: blockIdx.y = tensor, blockIdx.x strides its elements
 // =====================================================================================================
@@ -1083,6 +1169,18 @@ void launch_cross_entropy_fwd(const float* logits, const long long* target, floa
 void launch_cross_entropy_bwd(const float* probs, const long long* target, const float* dloss, float* dlogits, int B, int C,
                               cudaStream_t st) {
   cross_entropy_bwd_kernel<<<(B * C + 255) / 256, 256, 0, st>>>(probs, target, dloss, dlogits, B, C);
+  check_launch("cross_entropy_bwd");
+}
+void launch_cross_entropy_fwd(const float* logits, const long long* target, float* loss, float* probs, int B, int C, cudaStream_t st,
+                              bool emit_grad, const CeSpec& spec) {
+  if (spec.is_default(C)) return launch_cross_entropy_fwd(logits, target, loss, probs, B, C, st, emit_grad);
+  cross_entropy_fwd_spec_kernel<<<1, 256, 0, st>>>(logits, target, loss, probs, B, C, emit_grad ? 1 : 0, spec);
+  check_launch("cross_entropy_fwd");
+}
+void launch_cross_entropy_bwd(const float* probs, const long long* target, const float* dloss, float* dlogits, int B, int C,
+                              cudaStream_t st, const CeSpec& spec) {
+  if (spec.is_default(C)) return launch_cross_entropy_bwd(probs, target, dloss, dlogits, B, C, st);
+  cross_entropy_bwd_spec_kernel<<<(B * C + 255) / 256, 256, 0, st>>>(probs, target, dloss, dlogits, B, C, spec);
   check_launch("cross_entropy_bwd");
 }
 

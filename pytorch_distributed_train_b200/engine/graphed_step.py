@@ -127,7 +127,8 @@ class GraphedTrainStep:
 
         # the step owns the targets before the model runs: a model whose forward kernel can fold the loss in does so
         # (ops.functional.upcoming_targets); the criterion then finds value and gradient ready
-        with OF.upcoming_targets(inputs[1] if len(inputs) == 2 else None, loss_read_after_backward=True):
+        with OF.upcoming_targets(inputs[1] if len(inputs) == 2 else None, loss_read_after_backward=True,
+                                 spec=OF.ce_spec_of(self.criterion)):
             out = self.model(inputs[0])
         loss = self.criterion(out, *inputs[1:])
         self.optimizer.zero_grad(set_to_none=self.set_to_none)
@@ -168,7 +169,7 @@ class GraphedTrainStep:
             micro = [t[i * b:(i + 1) * b] for t in inputs]
             OF.reset_fused_ce_consumed()
             with OF.upcoming_targets(micro[1] if len(micro) == 2 else None, loss_read_after_backward=bool(self._prescale),
-                                     grad_scale=grad_scale):
+                                     grad_scale=grad_scale, spec=OF.ce_spec_of(self.criterion)):
                 out = self.model(micro[0])
             loss = self.criterion(out, *micro[1:])
             consumed = OF.fused_ce_consumed()

@@ -153,6 +153,24 @@ _upcoming_target: Optional[torch.Tensor] = None
 _loss_read_after_backward = False
 _upcoming_grad_scale = 1.0
 
+# torch's cross-entropy options as (weight, ignore_index, reduction, label_smoothing); the default is the plain mean
+DEFAULT_CE_SPEC = (None, -100, "mean", 0.0)
+_upcoming_spec = DEFAULT_CE_SPEC
+
+
+def ce_spec_of(criterion) -> tuple:
+    """The options of a ``pdt.nn.CrossEntropyLoss`` criterion as a spec for ``upcoming_targets``; the default spec for any other."""
+    from ..nn.loss import CrossEntropyLoss
+
+    if isinstance(criterion, CrossEntropyLoss):
+        return (criterion.weight, criterion.ignore_index, criterion.reduction, criterion.label_smoothing)
+    return DEFAULT_CE_SPEC
+
+
+def _same_spec(a: tuple, b: tuple) -> bool:
+    """The same weight tensor (or none) and equal scalars."""
+    return a[0] is b[0] and a[1] == b[1] and a[2] == b[2] and a[3] == b[3]
+
 
 class upcoming_targets:
     """``loss_read_after_backward=True`` (a captured step: nobody looks at the loss before the whole step has run) lets the
@@ -162,22 +180,26 @@ class upcoming_targets:
     gradient, so backward seeded with one yields torch's ``(loss / k).backward()`` with no scaling kernel.  That is right only when
     the criterion's result IS the cross-entropy ``cross_entropy`` returned (its ``_pdt_loss_scale`` says by how much it is scaled):
     a criterion that computes anything from it (``ce * w``, ``ce + reg``) would see the scaled value.  ``fused_ce_consumed`` lists
-    every fused cross-entropy handed out since ``reset_fused_ce_consumed``, so the caller can check that before it scales."""
+    every fused cross-entropy handed out since ``reset_fused_ce_consumed``, so the caller can check that before it scales.
 
-    def __init__(self, target: Optional[torch.Tensor], loss_read_after_backward: bool = False, grad_scale: float = 1.0):
+    ``spec`` = (weight, ignore_index, reduction, label_smoothing): the options of the criterion that will consume the loss
+    (``ce_spec_of``); the forward kernel computes that loss, and ``cross_entropy`` uses it only when called with the same options."""
+
+    def __init__(self, target: Optional[torch.Tensor], loss_read_after_backward: bool = False, grad_scale: float = 1.0,
+                 spec: tuple = DEFAULT_CE_SPEC):
         if not float(grad_scale) > 0:
             raise ValueError(f"grad_scale must be positive, got {grad_scale}")
-        self.target, self.late, self.scale = target, loss_read_after_backward, float(grad_scale)
+        self.target, self.late, self.scale, self.spec = target, loss_read_after_backward, float(grad_scale), tuple(spec)
 
     def __enter__(self):
-        global _upcoming_target, _loss_read_after_backward, _upcoming_grad_scale
-        self.prev = (_upcoming_target, _loss_read_after_backward, _upcoming_grad_scale)
-        _upcoming_target, _loss_read_after_backward, _upcoming_grad_scale = self.target, self.late, self.scale
+        global _upcoming_target, _loss_read_after_backward, _upcoming_grad_scale, _upcoming_spec
+        self.prev = (_upcoming_target, _loss_read_after_backward, _upcoming_grad_scale, _upcoming_spec)
+        _upcoming_target, _loss_read_after_backward, _upcoming_grad_scale, _upcoming_spec = self.target, self.late, self.scale, self.spec
         return self
 
     def __exit__(self, *exc):
-        global _upcoming_target, _loss_read_after_backward, _upcoming_grad_scale
-        _upcoming_target, _loss_read_after_backward, _upcoming_grad_scale = self.prev
+        global _upcoming_target, _loss_read_after_backward, _upcoming_grad_scale, _upcoming_spec
+        _upcoming_target, _loss_read_after_backward, _upcoming_grad_scale, _upcoming_spec = self.prev
         return False
 
 
@@ -271,10 +293,11 @@ class _FusedLayer1(torch.autograd.Function):
         # classifier of an image run in the same CTA; their results are handed to the next autograd nodes through `whole`
         c2, bn2, fc = whole["conv2"], whole["bn2"], whole["fc"]
         defer = bool(whole.get("defer_loss_mean", False))
+        cw, ignore_index, reduction, smoothing = whole.get("spec", DEFAULT_CE_SPEC)
         out, y, saved, p2, y2, saved2, logits, loss, dlogits, loss_parts = _C.convnet_fwd(
             x, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, c2.weight, c2.bias, bn2.weight, bn2.bias,
             bn2.running_mean, bn2.running_var, bn2.num_batches_tracked, float(bn2.momentum), float(bn2.eps), fc.weight, fc.bias,
-            whole.get("target"), defer, float(whole.get("grad_scale", 1.0)))
+            whole.get("target"), defer, float(whole.get("grad_scale", 1.0)), cw, int(ignore_index), float(smoothing), reduction)
         whole["layer2"] = (p2, y2, saved2, logits)
         whole["ce"] = (loss, dlogits)
         whole["ce_deferred"] = (loss_parts, loss) if defer else None
@@ -376,11 +399,13 @@ def fused_convnet_forward(x: torch.Tensor, model) -> torch.Tensor:
     c1, b1, c2, b2_bn, fc = model.layer1[0], model.layer1[1], model.layer2[0], model.layer2[1], model.fc
     whole = {"conv2": c2, "bn2": b2_bn, "fc": fc}
     t = _upcoming_target
+    spec = _upcoming_spec
     if (t is not None and t.is_cuda and t.dtype == torch.int64 and t.dim() == 1 and t.shape[0] == x.shape[0] and t.is_contiguous()
-            and torch.is_grad_enabled()):
+            and torch.is_grad_enabled() and _rider_spec_ok(spec, fc.weight)):
         whole["target"] = t
         whole["defer_loss_mean"] = bool(_loss_read_after_backward)
         whole["grad_scale"] = _upcoming_grad_scale
+        whole["spec"] = spec
     # conv2's weight gradient is produced by layer 1's backward kernel: layer 1's node owns (w2, b2) for autograd, `link` carries
     # the operands from layer 2's backward to it
     link = {}
@@ -389,9 +414,18 @@ def fused_convnet_forward(x: torch.Tensor, model) -> torch.Tensor:
     _, logits = _FusedLayer2.apply(p1, c2.weight, c2.bias, b2_bn.weight, b2_bn.bias, b2_bn.running_mean, b2_bn.running_var,
                                    b2_bn.num_batches_tracked, float(b2_bn.momentum), float(b2_bn.eps), fc.weight, fc.bias, whole, link)
     if whole.get("target") is not None:
-        # (target, loss, dlogits, scale of loss and gradient, loss folded by layer 2's backward kernel) for ops.cross_entropy
-        logits._pdt_ce = (whole["target"],) + whole["ce"] + (float(whole.get("grad_scale", 1.0)), whole["ce_deferred"] is not None)
+        # (target, loss, dlogits, scale of loss and gradient, loss folded by layer 2's backward kernel, spec) for ops.cross_entropy
+        logits._pdt_ce = (whole["target"],) + whole["ce"] + (float(whole.get("grad_scale", 1.0)), whole["ce_deferred"] is not None,
+                                                             whole["spec"])
     return logits
+
+
+def _rider_spec_ok(spec: tuple, fcw: torch.Tensor) -> bool:
+    """Whether the forward kernel's cross-entropy can take these options (what pdt.nn.CrossEntropyLoss runs natively); a criterion
+    with others computes its loss itself, so the rider is left off."""
+    w, ignore_index, reduction, smoothing = spec
+    return (reduction in ("mean", "sum") and 0.0 <= float(smoothing) <= 1.0 and isinstance(ignore_index, int)
+            and (w is None or (w.dtype == torch.float32 and w.is_contiguous() and w.shape == (fcw.shape[0],) and w.device == fcw.device)))
 
 
 def conv_bn_relu_pool(x: torch.Tensor, conv: torch.nn.Conv2d, bn: torch.nn.Module, out_nchw: Optional[bool] = None,
@@ -474,11 +508,14 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
 class _CrossEntropy(torch.autograd.Function):
     """Mean cross-entropy whose forward launch also produces the gradient w.r.t. the logits for a unit incoming
     gradient, (softmax − onehot)/B.  Backward is then free when the incoming gradient is known to be one
-    (``engine.GraphedTrainStep`` seeds backward with a tensor tagged ``_pdt_unit_seed``) and one scaling kernel otherwise."""
+    (``engine.GraphedTrainStep`` seeds backward with a tensor tagged ``_pdt_unit_seed``) and one scaling kernel otherwise.
+    ``spec`` (weight, ignore_index, reduction, label_smoothing): torch's options, in the same launch."""
 
     @staticmethod
-    def forward(ctx, logits, target):
-        loss, grad0 = _C.cross_entropy_fwd(logits.contiguous(), target.contiguous(), True)
+    def forward(ctx, logits, target, spec=DEFAULT_CE_SPEC):
+        w, ignore_index, reduction, smoothing = spec
+        loss, grad0 = _C.cross_entropy_fwd(logits.contiguous(), target.contiguous(), True, w, int(ignore_index), float(smoothing),
+                                           reduction)
         ctx.save_for_backward(grad0)
         return loss
 
@@ -486,8 +523,8 @@ class _CrossEntropy(torch.autograd.Function):
     def backward(ctx, dloss):
         (grad0,) = ctx.saved_tensors
         if getattr(dloss, "_pdt_unit_seed", False):
-            return grad0, None
-        return grad0 * dloss, None
+            return grad0, None, None
+        return grad0 * dloss, None, None
 
 
 class _CrossEntropyPrecomputed(torch.autograd.Function):
@@ -520,16 +557,20 @@ def fused_ce_consumed() -> list:
     return list(_fused_ce_consumed)
 
 
-def cross_entropy(logits: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
-    """Mean cross-entropy over the batch: fused log-softmax + NLL (ref: ddp_example.py:61,87)."""
+def cross_entropy(logits: torch.Tensor, target: torch.Tensor, weight: Optional[torch.Tensor] = None, ignore_index: int = -100,
+                  reduction: str = "mean", label_smoothing: float = 0.0) -> torch.Tensor:
+    """Cross-entropy over the batch, mean or sum, with torch's class weights, ignore_index and label smoothing: fused log-softmax +
+    NLL (ref: ddp_example.py:61,87).  The value the model's forward kernel computed is used when it was computed for this target
+    tensor with the same options (the same weight tensor, equal scalars)."""
+    spec = (weight, ignore_index, reduction, label_smoothing)
     pre = getattr(logits, "_pdt_ce", None)
-    if pre is not None and pre[0] is target:
+    if pre is not None and pre[0] is target and _same_spec(pre[5], spec):
         loss = _CrossEntropyPrecomputed.apply(logits, pre[1], pre[2])
         loss._pdt_loss_scale = pre[3]   # upcoming_targets(grad_scale=…): the value and its gradient are grad_scale · the mean
         loss._pdt_loss_deferred = pre[4]
         _fused_ce_consumed.append((id(loss), pre[3]))
         return loss
-    return _CrossEntropy.apply(logits, target)
+    return _CrossEntropy.apply(logits, target, spec)
 
 
 def sgd_step(params, grads, momentum_bufs, lr, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False,

@@ -25,6 +25,7 @@ GROUPS = {
     "adam": ["tests/test_adam.py"],
     "clip": ["tests/test_clip_grad.py"],
     "accum": ["tests/test_grad_accumulation.py"],
+    "ce_options": ["tests/test_cross_entropy_options.py"],
 }
 
 
