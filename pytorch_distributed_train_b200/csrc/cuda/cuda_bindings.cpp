@@ -532,16 +532,6 @@ void register_cuda_bindings(py::module_& m) {
   });
 
   // ---- generic NCHW BatchNorm (SyncBatchNorm) ----------------------------------------------------------
-  m.def("bn_stats_nchw", [](const at::Tensor& x) {
-    chk(x, "x");
-    TORCH_CHECK(x.dim() >= 2, "bn_stats: at least 2-D input");
-    c10::cuda::CUDAGuard g(x.device());
-    const int N = x.size(0), C = x.size(1);
-    const int HW = static_cast<int>(x.numel() / std::max<int64_t>(1, static_cast<int64_t>(N) * C));
-    at::Tensor stats = at::zeros({2 * C + 1}, x.options());
-    if (x.numel() > 0) launch_bn_stats_nchw(x.data_ptr<float>(), stats.data_ptr<float>(), N, C, HW, scratch(x), cur_stream(x));
-    return stats;
-  });
   m.def("bn_stats_nchw_f64", [](const at::Tensor& x) {
     chk(x, "x");
     TORCH_CHECK(x.dim() >= 2, "bn_stats: at least 2-D input");

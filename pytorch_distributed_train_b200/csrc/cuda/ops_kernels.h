@@ -69,12 +69,12 @@ void launch_bn_relu_pool_bwd_apply(const float* dout, const float* y, const floa
                                    cudaStream_t st);
 
 // ---- generic NCHW BatchNorm pieces (SyncBatchNorm on arbitrary models) ---------------------------------
-void launch_bn_stats_nchw(const float* x, float* stats, int N, int C, int HW, ReduceScratch scr, cudaStream_t st);
-// same sums accumulated and returned in fp64 (SyncBatchNorm forward: var = E[x²] − μ² needs the headroom)
+// stats [2C+1] ← per-channel Σx, Σx², then the element count per channel, accumulated and returned in fp64 (SyncBatchNorm
+// forward: var = E[x²] − μ² needs the headroom)
+void launch_bn_stats_nchw_f64(const float* x, double* stats, int N, int C, int HW, ReduceScratch scr, cudaStream_t st);
 // fp64 [2C+1(+pad)] all-reduced statistics → mean / invstd / count (fp32) + running-stat update (nullable), one launch
 void launch_bn_finalize(const double* stats, int C, double eps, float momentum, float* mean, float* invstd, float* count_out,
                         float* running_mean, float* running_var, cudaStream_t st);
-void launch_bn_stats_nchw_f64(const float* x, double* stats, int N, int C, int HW, ReduceScratch scr, cudaStream_t st);
 void launch_bn_apply_nchw(const float* x, const float* mean, const float* invstd, const float* gamma, const float* beta, float* out,
                           int N, int C, int HW, cudaStream_t st);
 void launch_bn_bwd_reduce_nchw(const float* dy, const float* x, const float* mean, const float* invstd, float* red4c, int N, int C,

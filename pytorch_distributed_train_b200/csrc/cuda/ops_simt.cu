@@ -445,29 +445,22 @@ __global__ void __launch_bounds__(256) bn_relu_pool_bwd_kernel(const float* __re
 // =====================================================================================================
 // Generic NCHW BatchNorm pieces
 // =====================================================================================================
-template <bool BWD>
-__global__ void __launch_bounds__(256) bn_reduce_nchw_kernel(const float* __restrict__ a, const float* __restrict__ x,
-                                                             const float* __restrict__ mean, const float* __restrict__ invstd,
-                                                             float* out, int N, int C, int HW, int S, ReduceScratch scr) {
-  // FWD: Σx, Σx² of channel c over slice s.  BWD: Σdy, Σdy·(x-μ)   (a = dy)
+__global__ void __launch_bounds__(256) bn_bwd_reduce_nchw_kernel(const float* __restrict__ dy, const float* __restrict__ x,
+                                                                 const float* __restrict__ mean, const float* __restrict__ invstd,
+                                                                 float* out, int N, int C, int HW, int S, ReduceScratch scr) {
+  // Σdy, Σdy·(x-μ) of channel c over slice s
   const int c = blockIdx.x / S, s = blockIdx.x % S;
   const long long total = static_cast<long long>(N) * HW;
   const long long chunk = (total + S - 1) / S;
   const long long lo = chunk * s, hi = min(total, lo + chunk);
-  const float mu = BWD ? mean[c] : 0.f;
+  const float mu = mean[c];
   float s1 = 0.f, s2 = 0.f;
   for (long long e = lo + threadIdx.x; e < hi; e += blockDim.x) {
     const long long n = e / HW, hw = e % HW;
     const size_t off = (static_cast<size_t>(n) * C + c) * HW + hw;
-    if constexpr (BWD) {
-      const float d = a[off];
-      s1 += d;
-      s2 += d * (x[off] - mu);
-    } else {
-      const float v = x[off];
-      s1 += v;
-      s2 += v * v;
-    }
+    const float d = dy[off];
+    s1 += d;
+    s2 += d * (x[off] - mu);
   }
   __shared__ float r1[8], r2[8], blk[2];
   for (int off = 16; off > 0; off >>= 1) {
@@ -497,16 +490,10 @@ __global__ void __launch_bounds__(256) bn_reduce_nchw_kernel(const float* __rest
       t1 += __ldcg(&scr.partials[(static_cast<size_t>(ch) * S + k) * 2]);
       t2 += __ldcg(&scr.partials[(static_cast<size_t>(ch) * S + k) * 2 + 1]);
     }
-    if constexpr (BWD) {
-      out[ch] = t1;                        // Σdy
-      out[C + ch] = t2;                    // Σdy·(x-μ)
-      out[2 * C + ch] = t2 * invstd[ch];   // dγ
-      out[3 * C + ch] = t1;                // dβ
-    } else {
-      out[ch] = t1;
-      out[C + ch] = t2;
-      if (ch == 0) out[2 * C] = static_cast<float>(total);
-    }
+    out[ch] = t1;                        // Σdy
+    out[C + ch] = t2;                    // Σdy·(x-μ)
+    out[2 * C + ch] = t2 * invstd[ch];   // dγ
+    out[3 * C + ch] = t1;                // dβ
   }
   if (threadIdx.x == 0) *scr.counter = 0u;
 }
@@ -1112,12 +1099,6 @@ static int bn_slices(int N, int C, int HW) {
   return std::max(1, S);
 }
 
-void launch_bn_stats_nchw(const float* x, float* stats, int N, int C, int HW, ReduceScratch scr, cudaStream_t st) {
-  const int S = bn_slices(N, C, HW);
-  if (static_cast<long long>(C) * S * 2 > scr.capacity_floats) throw std::invalid_argument("bn_stats: reduction scratch too small");
-  bn_reduce_nchw_kernel<false><<<C * S, 256, 0, st>>>(nullptr, x, nullptr, nullptr, stats, N, C, HW, S, scr);
-  check_launch("bn_stats_nchw");
-}
 void launch_bn_stats_nchw_f64(const float* x, double* stats, int N, int C, int HW, ReduceScratch scr, cudaStream_t st) {
   const int S = bn_slices(N, C, HW);
   if (static_cast<long long>(C) * S * 4 > scr.capacity_floats) throw std::invalid_argument("bn_stats: reduction scratch too small");
@@ -1139,7 +1120,7 @@ void launch_bn_bwd_reduce_nchw(const float* dy, const float* x, const float* mea
                                ReduceScratch scr, cudaStream_t st) {
   const int S = bn_slices(N, C, HW);
   if (static_cast<long long>(C) * S * 2 > scr.capacity_floats) throw std::invalid_argument("bn_bwd_reduce: reduction scratch too small");
-  bn_reduce_nchw_kernel<true><<<C * S, 256, 0, st>>>(dy, x, mean, invstd, red4c, N, C, HW, S, scr);
+  bn_bwd_reduce_nchw_kernel<<<C * S, 256, 0, st>>>(dy, x, mean, invstd, red4c, N, C, HW, S, scr);
   check_launch("bn_bwd_reduce_nchw");
 }
 void launch_bn_bwd_apply_nchw(const float* dy, const float* x, const float* mean, const float* invstd, const float* gamma,

@@ -26,6 +26,7 @@ GROUPS = {
     "clip": ["tests/test_clip_grad.py"],
     "accum": ["tests/test_grad_accumulation.py"],
     "ce_options": ["tests/test_cross_entropy_options.py"],
+    "syncbn": ["tests/test_syncbn_native.py"],
 }
 
 
