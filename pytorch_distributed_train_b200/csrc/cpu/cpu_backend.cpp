@@ -351,7 +351,20 @@ void CpuBackend::do_reduce_scatter(const void* in, void* out, size_t cpr, DType 
 }
 
 // ---- async wrappers --------------------------------------------------------------------
+// On bool, SUM is logical OR and PRODUCT logical AND (torch's NCCL backend maps them to MAX / MIN, and so do the GPU backends);
+// on 0/1 bytes MIN and MAX are AND and OR as well.  AVG has no bool result.  Checked before any byte moves, on every rank alike.
+static ReduceOp checked_op(DType t, ReduceOp op) {
+  if (t != DType::BOOL) return op;
+  switch (op) {
+    case ReduceOp::SUM: case ReduceOp::MAX: case ReduceOp::BOR: return ReduceOp::BOR;
+    case ReduceOp::PRODUCT: case ReduceOp::MIN: case ReduceOp::BAND: return ReduceOp::BAND;
+    case ReduceOp::BXOR: return ReduceOp::BXOR;
+    default: throw std::invalid_argument("AVG is not defined for bool tensors");
+  }
+}
+
 std::shared_ptr<Work> CpuBackend::allreduce(void* buf, size_t count, DType t, ReduceOp op) {
+  op = checked_op(t, op);
   return submit([=] { do_allreduce(buf, count, t, op); });
 }
 std::shared_ptr<Work> CpuBackend::broadcast(void* buf, size_t nbytes, int root) {
@@ -363,9 +376,11 @@ std::shared_ptr<Work> CpuBackend::allgather(const void* in, void* out, size_t nb
 }
 std::shared_ptr<Work> CpuBackend::reduce(void* buf, size_t count, DType t, ReduceOp op, int root) {
   if (root < 0 || root >= size_) throw std::invalid_argument("reduce: invalid root rank");
+  op = checked_op(t, op);
   return submit([=] { do_reduce(buf, count, t, op, root); });
 }
 std::shared_ptr<Work> CpuBackend::reduce_scatter(const void* in, void* out, size_t cpr, DType t, ReduceOp op) {
+  op = checked_op(t, op);
   return submit([=] { do_reduce_scatter(in, out, cpr, t, op); });
 }
 std::shared_ptr<Work> CpuBackend::gather(const void* in, void* out, size_t nb, int root) {

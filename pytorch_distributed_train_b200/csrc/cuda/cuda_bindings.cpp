@@ -5,6 +5,7 @@
 #include <torch/extension.h>
 
 #include <cmath>
+#include <cstring>
 #include <map>
 #include <mutex>
 
@@ -104,6 +105,61 @@ const float* conv2_input(const c10::optional<at::Tensor>& p1, int B, const char*
   return p1->data_ptr<float>();
 }
 
+// Test-only: rank `rank` of a world emulated on one GPU, for launching the collective kernels one at a time.  The W heaps are
+// plain uint8 device tensors laid out like the symmetric heap (the flag pads of every channel first, kSymmFlagPadBytes, then
+// data), and the SymmDev's peer[r] points at heap r; there is no multicast mapping.  Whoever drives it stages what the other
+// ranks would have written (their data, and their barrier flags far enough ahead that no kernel waits) before each launch.
+// Pointer arguments are device addresses (0 = nullptr), so that tests can pass misaligned ones; every launch goes to the current
+// stream of the heaps' device.
+constexpr size_t kSymmFlagPadBytes = sizeof(uint32_t) * kSymmChannels * kSymmMaxBlocks * kSymmMaxWorld;
+
+class SymmEmu {
+ public:
+  SymmEmu(std::vector<at::Tensor> heaps, int rank, int channel, int64_t timeout_ns, at::Tensor epochs, at::Tensor status)
+      : heaps_(std::move(heaps)), epochs_(std::move(epochs)), status_(std::move(status)) {
+    const int world = static_cast<int>(heaps_.size());
+    TORCH_CHECK(world >= 1 && world <= kSymmMaxWorld, "SymmEmu: 1 to ", kSymmMaxWorld, " heaps required");
+    TORCH_CHECK(rank >= 0 && rank < world && channel >= 0 && channel < kSymmChannels && timeout_ns > 0, "SymmEmu: bad rank, channel or timeout");
+    std::memset(&d_, 0, sizeof(d_));
+    for (int r = 0; r < world; ++r) {
+      chk(heaps_[r], "heap", at::kByte);
+      TORCH_CHECK(heaps_[r].device() == heaps_[0].device() && heaps_[r].numel() >= static_cast<int64_t>(kSymmFlagPadBytes) &&
+                      reinterpret_cast<uintptr_t>(heaps_[r].data_ptr()) % 16 == 0,
+                  "SymmEmu: heaps must be 16-byte aligned, on one device, and hold at least the flag pads");
+      d_.peer[r] = static_cast<char*>(heaps_[r].data_ptr());
+    }
+    chk(epochs_, "epochs", at::kInt);
+    chk(status_, "status", at::kInt);
+    TORCH_CHECK(epochs_.numel() == kSymmMaxBlocks && status_.numel() >= 1 && epochs_.device() == heaps_[0].device() &&
+                    status_.device() == heaps_[0].device(),
+                "SymmEmu: epochs [", kSymmMaxBlocks, "] and status [1] on the heaps' device required");
+    d_.mc = nullptr;
+    d_.flags = nullptr;
+    d_.flags_off = static_cast<size_t>(channel) * kSymmMaxBlocks * kSymmMaxWorld * sizeof(uint32_t);
+    d_.epochs = reinterpret_cast<uint32_t*>(epochs_.data_ptr<int>());
+    d_.status = status_.data_ptr<int>();
+    d_.timeout_ns = static_cast<unsigned long long>(timeout_ns);
+    d_.rank = rank;
+    d_.world = world;
+    d_.channel = channel;
+  }
+  const SymmDev& dev() const { return d_; }
+  cudaStream_t stream() const { return c10::cuda::getCurrentCUDAStream(heaps_[0].device().index()).stream(); }
+
+ private:
+  std::vector<at::Tensor> heaps_;
+  at::Tensor epochs_, status_;
+  SymmDev d_;
+};
+
+template <typename P = void> P* dptr(int64_t a) { return reinterpret_cast<P*>(static_cast<uintptr_t>(a)); }
+SymmLaunchCfg launch_cfg(int blocks, int threads) {
+  SymmLaunchCfg c;
+  c.blocks = blocks;
+  c.threads = threads;
+  return c;
+}
+
 // The grid barrier of the cooperative kernels lives in the fixed words behind the fold region.
 GridSync grid_sync(const ReduceScratch& r) { return GridSync{r.counter + kGridEpochWord, r.counter + kGridArrivalWord}; }
 
@@ -174,6 +230,56 @@ void register_cuda_bindings(py::module_& m) {
       })
       .def("heap_bytes_in_use", [](SymmComm& c) { return c.heap().user_bytes_in_use(); })
       .def("is_symmetric", [](SymmComm& c, const at::Tensor& t) { return c.heap().contains(t.data_ptr(), t.nbytes()); });
+
+  // Test-only (see SymmEmu): thin wrappers over every launcher of symm_kernels.h except the multicast forms.
+  m.attr("_symm_max_world") = kSymmMaxWorld;
+  m.attr("_symm_max_blocks") = kSymmMaxBlocks;
+  m.attr("_symm_channels") = kSymmChannels;
+  m.attr("_symm_p2p_blocks") = kSymmP2PBlocks;
+  m.attr("_symm_flag_pad_bytes") = kSymmFlagPadBytes;
+  py::class_<SymmEmu>(m, "_SymmEmu")
+      .def(py::init<std::vector<at::Tensor>, int, int, int64_t, at::Tensor, at::Tensor>(), py::arg("heaps"), py::arg("rank"),
+           py::arg("channel"), py::arg("timeout_ns"), py::arg("epochs"), py::arg("status"))
+      .def("oneshot", [](SymmEmu& e, int64_t in, int64_t out, int64_t stage_off, int64_t count, int dtype, int op, double scale, int blocks,
+                         int threads) {
+        launch_allreduce_oneshot_push(e.dev(), dptr(in), dptr(out), stage_off, count, dtype, op, scale, false, launch_cfg(blocks, threads), e.stream());
+      }, py::arg("inp"), py::arg("out"), py::arg("stage_off"), py::arg("count"), py::arg("dtype"), py::arg("op"), py::arg("scale") = 1.0,
+         py::arg("blocks") = 0, py::arg("threads") = 0)
+      .def("twoshot", [](SymmEmu& e, int64_t buf_off, int64_t count, int dtype, int op, double scale, int blocks, int threads) {
+        launch_allreduce_twoshot(e.dev(), buf_off, count, dtype, op, scale, false, launch_cfg(blocks, threads), e.stream());
+      }, py::arg("buf_off"), py::arg("count"), py::arg("dtype"), py::arg("op"), py::arg("scale") = 1.0, py::arg("blocks") = 0, py::arg("threads") = 0)
+      .def("reduce_pull", [](SymmEmu& e, int64_t stage_off, int64_t begin_vec, int64_t count_vec, int64_t total_vec, int64_t out, int dtype, int op,
+                             double scale, int blocks, int threads) {
+        launch_reduce_pull(e.dev(), stage_off, begin_vec, count_vec, total_vec, dptr(out), dtype, op, scale, launch_cfg(blocks, threads), e.stream());
+      }, py::arg("stage_off"), py::arg("begin_vec"), py::arg("count_vec"), py::arg("total_vec"), py::arg("out"), py::arg("dtype"), py::arg("op"),
+         py::arg("scale") = 1.0, py::arg("blocks") = 0, py::arg("threads") = 0)
+      .def("broadcast", [](SymmEmu& e, int64_t src_off, int64_t dst, int64_t nbytes, int root, bool exit_barrier, int blocks, int threads) {
+        launch_broadcast_pull(e.dev(), src_off, dptr(dst), nbytes, root, exit_barrier, launch_cfg(blocks, threads), e.stream());
+      }, py::arg("src_off"), py::arg("dst"), py::arg("nbytes"), py::arg("root"), py::arg("exit_barrier"), py::arg("blocks") = 0, py::arg("threads") = 0)
+      .def("allgather", [](SymmEmu& e, int64_t src_off, int64_t dst, int64_t nbytes, int64_t dst_stride, bool exit_barrier, int blocks, int threads) {
+        launch_allgather_pull(e.dev(), src_off, dptr(dst), nbytes, dst_stride, exit_barrier, launch_cfg(blocks, threads), e.stream());
+      }, py::arg("src_off"), py::arg("dst"), py::arg("nbytes"), py::arg("dst_stride"), py::arg("exit_barrier"), py::arg("blocks") = 0,
+         py::arg("threads") = 0)
+      .def("alltoall", [](SymmEmu& e, int64_t src_off, int64_t dst, int64_t nbytes, int64_t stride, bool exit_barrier, int blocks, int threads) {
+        launch_alltoall_pull(e.dev(), src_off, dptr(dst), nbytes, stride, exit_barrier, launch_cfg(blocks, threads), e.stream());
+      }, py::arg("src_off"), py::arg("dst"), py::arg("nbytes"), py::arg("stride"), py::arg("exit_barrier"), py::arg("blocks") = 0, py::arg("threads") = 0)
+      .def("allreduce_sgd", [](SymmEmu& e, int64_t grad, int64_t param, int64_t mom, int64_t stage_off, int64_t count, double scale, int64_t lr_dev,
+                               double lr, double momentum, double dampening, double weight_decay, bool nesterov, bool first_step, int64_t bcast,
+                               int64_t bcast_bytes, int bcast_root, int blocks, int threads) {
+        launch_allreduce_sgd_oneshot(e.dev(), dptr<float>(grad), dptr<float>(param), dptr<float>(mom), stage_off, count, static_cast<float>(scale),
+                                     dptr<const float>(lr_dev), static_cast<float>(lr), static_cast<float>(momentum), static_cast<float>(dampening),
+                                     static_cast<float>(weight_decay), nesterov, first_step, false, launch_cfg(blocks, threads), e.stream(),
+                                     dptr(bcast), bcast_bytes, bcast_root);
+      }, py::arg("grad"), py::arg("param"), py::arg("mom"), py::arg("stage_off"), py::arg("count"), py::arg("scale"), py::arg("lr_dev"), py::arg("lr"),
+         py::arg("momentum"), py::arg("dampening"), py::arg("weight_decay"), py::arg("nesterov"), py::arg("first_step"), py::arg("bcast") = 0,
+         py::arg("bcast_bytes") = 0, py::arg("bcast_root") = 0, py::arg("blocks") = 0, py::arg("threads") = 0)
+      .def("p2p_send", [](SymmEmu& e, int64_t src, int64_t nbytes, int dst_rank, int64_t slot_off, uint32_t seq) {
+        launch_p2p_send(e.dev(), dptr(src), nbytes, dst_rank, slot_off, seq, e.stream());
+      }, py::arg("src"), py::arg("nbytes"), py::arg("dst_rank"), py::arg("slot_off"), py::arg("seq"))
+      .def("p2p_recv", [](SymmEmu& e, int64_t dst, int64_t nbytes, int src_rank, int64_t slot_off, uint32_t seq) {
+        launch_p2p_recv(e.dev(), dptr(dst), nbytes, src_rank, slot_off, seq, e.stream());
+      }, py::arg("dst"), py::arg("nbytes"), py::arg("src_rank"), py::arg("slot_off"), py::arg("seq"))
+      .def("barrier", [](SymmEmu& e) { launch_barrier(e.dev(), e.stream()); });
 
   py::class_<NcclComm, Comm, std::shared_ptr<NcclComm>>(m, "NcclComm")
       .def(py::init([](std::shared_ptr<Store> store, int rank, int size, int device, double timeout_s) {

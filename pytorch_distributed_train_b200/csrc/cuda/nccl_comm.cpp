@@ -96,7 +96,14 @@ ncclDataType_t nccl_dtype(at::ScalarType t) {
   }
 }
 
-ncclRedOp_t nccl_op(ReduceOp op) {
+// On bool, SUM is logical OR and PRODUCT logical AND (as torch's NCCL backend maps them): MAX and MIN of 0/1 bytes.  AVG has no
+// bool result.
+ncclRedOp_t nccl_op(ReduceOp op, at::ScalarType t) {
+  if (t == at::kBool) {
+    TORCH_CHECK(op != ReduceOp::AVG, "NCCL: AVG is not defined for bool tensors");
+    if (op == ReduceOp::SUM) return ncclMax;
+    if (op == ReduceOp::PRODUCT) return ncclMin;
+  }
   switch (op) {
     case ReduceOp::SUM: return ncclSum;
     case ReduceOp::AVG: return ncclAvg;
@@ -151,7 +158,7 @@ std::shared_ptr<CommWork> NcclComm::allreduce(at::Tensor t, ReduceOp op, double 
   check(t, "allreduce");
   record("allreduce", &t);
   return enqueue({t}, [&](cudaStream_t s) {
-    nccl_check(api().AllReduce(t.data_ptr(), t.data_ptr(), static_cast<size_t>(t.numel()), nccl_dtype(t.scalar_type()), nccl_op(op),
+    nccl_check(api().AllReduce(t.data_ptr(), t.data_ptr(), static_cast<size_t>(t.numel()), nccl_dtype(t.scalar_type()), nccl_op(op, t.scalar_type()),
                                static_cast<ncclComm_t>(comm_), s),
                "ncclAllReduce");
     if (postscale != 1.0) {
@@ -181,7 +188,7 @@ std::shared_ptr<CommWork> NcclComm::reduce(at::Tensor t, ReduceOp op, int root) 
   check(t, "reduce");
   record("reduce", &t);
   return enqueue({t}, [&](cudaStream_t s) {
-    nccl_check(api().Reduce(t.data_ptr(), t.data_ptr(), static_cast<size_t>(t.numel()), nccl_dtype(t.scalar_type()), nccl_op(op), root,
+    nccl_check(api().Reduce(t.data_ptr(), t.data_ptr(), static_cast<size_t>(t.numel()), nccl_dtype(t.scalar_type()), nccl_op(op, t.scalar_type()), root,
                             static_cast<ncclComm_t>(comm_), s),
                "ncclReduce");
   });
@@ -191,7 +198,7 @@ std::shared_ptr<CommWork> NcclComm::reduce_scatter(at::Tensor out, at::Tensor in
   check(in, "reduce_scatter input");
   record("reduce_scatter", &in);
   return enqueue({out, in}, [&](cudaStream_t s) {
-    nccl_check(api().ReduceScatter(in.data_ptr(), out.data_ptr(), static_cast<size_t>(out.numel()), nccl_dtype(in.scalar_type()), nccl_op(op),
+    nccl_check(api().ReduceScatter(in.data_ptr(), out.data_ptr(), static_cast<size_t>(out.numel()), nccl_dtype(in.scalar_type()), nccl_op(op, in.scalar_type()),
                                    static_cast<ncclComm_t>(comm_), s),
                "ncclReduceScatter");
   });

@@ -442,6 +442,7 @@ std::shared_ptr<CommWork> SymmComm::alltoall(at::Tensor out, at::Tensor in) {
 std::shared_ptr<CommWork> SymmComm::reduce(at::Tensor t, ReduceOp op, int root) {
   check(t, "reduce");
   TORCH_CHECK(root >= 0 && root < size_, "reduce: invalid root");
+  TORCH_CHECK(op != ReduceOp::AVG || at::isFloatingType(t.scalar_type()), "reduce: AVG is only defined for floating-point tensors");
   record("reduce", &t);
   return enqueue({t}, [&](cudaStream_t s) {
     const size_t nbytes = t.nbytes();
@@ -469,6 +470,7 @@ std::shared_ptr<CommWork> SymmComm::reduce_scatter(at::Tensor out, at::Tensor in
   check(out, "reduce_scatter output");
   check(in, "reduce_scatter input");
   TORCH_CHECK(in.numel() == out.numel() * size_ && in.scalar_type() == out.scalar_type(), "reduce_scatter: input must hold world_size × output elements");
+  TORCH_CHECK(op != ReduceOp::AVG || at::isFloatingType(out.scalar_type()), "reduce_scatter: AVG is only defined for floating-point tensors");
   record("reduce_scatter", &in);
   return enqueue({out, in}, [&](cudaStream_t s) {
     const size_t slice = out.nbytes();

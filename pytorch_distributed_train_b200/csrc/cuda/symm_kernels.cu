@@ -34,18 +34,21 @@ template <typename T> __device__ __forceinline__ T from_acc(typename Acc<T>::typ
 template <> __device__ __forceinline__ __half from_acc<__half>(float v) { return __float2half_rn(v); }
 template <> __device__ __forceinline__ __nv_bfloat16 from_acc<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
 
+// MIN / MAX propagate a NaN whichever rank holds it (torch.minimum / torch.maximum): `b != b` is false for integers.
 template <typename A, int OP> __device__ __forceinline__ A combine(A a, A b) {
   if constexpr (OP == SO_SUM || OP == SO_AVG) return a + b;
   else if constexpr (OP == SO_PROD) return a * b;
-  else if constexpr (OP == SO_MIN) return b < a ? b : a;
-  else if constexpr (OP == SO_MAX) return b > a ? b : a;
+  else if constexpr (OP == SO_MIN) return (b < a || b != b) ? b : a;
+  else if constexpr (OP == SO_MAX) return (b > a || b != b) ? b : a;
   else if constexpr (OP == SO_BAND) { if constexpr (std::is_integral<A>::value) return a & b; else return a; }
   else if constexpr (OP == SO_BOR) { if constexpr (std::is_integral<A>::value) return a | b; else return a; }
   else { if constexpr (std::is_integral<A>::value) return a ^ b; else return a; }
 }
 
-template <typename A> __device__ __forceinline__ A apply_scale(A v, float scale) {
-  if constexpr (std::is_floating_point<A>::value) return v * static_cast<A>(scale);
+// The launchers take the scale as a double and reject a scale != 1 on integer types; the kernels convert it once to the
+// accumulator type, so an fp64 reduction is scaled by the fp64 value.
+template <typename A> __device__ __forceinline__ A apply_scale(A v, A scale) {
+  if constexpr (std::is_floating_point<A>::value) return v * scale;
   else return v;
 }
 
@@ -81,7 +84,7 @@ __device__ __forceinline__ void acc_add(typename Acc<T>::type (&a)[VecOf<T>::N],
   for (int k = 0; k < VecOf<T>::N; ++k) a[k] = combine<typename Acc<T>::type, OP>(a[k], to_acc<T>(e[k]));
 }
 template <typename T>
-__device__ __forceinline__ uint4 acc_pack(typename Acc<T>::type (&a)[VecOf<T>::N], float scale) {
+__device__ __forceinline__ uint4 acc_pack(typename Acc<T>::type (&a)[VecOf<T>::N], typename Acc<T>::type scale) {
   uint4 v;
   T* e = reinterpret_cast<T*>(&v);
 #pragma unroll
@@ -93,8 +96,9 @@ __device__ __forceinline__ uint4 acc_pack(typename Acc<T>::type (&a)[VecOf<T>::N
 // nvec: number of 16-byte vectors (host pads the tail into a scratch vector); slot stride = nvec*16.
 template <typename T, int OP, bool MC>
 __global__ void __launch_bounds__(512) allreduce_oneshot_push_kernel(const __grid_constant__ SymmDev d, const uint4* __restrict__ in, uint4* out,
-                                                                      size_t stage_off, size_t nvec, float scale) {
+                                                                      size_t stage_off, size_t nvec, double scale) {
   SymmEpoch ep(d, blockIdx.x);
+  const auto sc = static_cast<typename Acc<T>::type>(scale);
   const size_t slot_bytes = nvec * 16;
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   const size_t first = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -117,7 +121,7 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_push_kernel(const __gri
     typename Acc<T>::type a[VecOf<T>::N];
     acc_init<T, OP>(a, ld_vec_nc(base + i * 16));
     for (int r = 1; r < d.world; ++r) acc_add<T, OP>(a, ld_vec_nc(base + static_cast<size_t>(r) * slot_bytes + i * 16));
-    st_vec(out + i, acc_pack<T>(a, scale));
+    st_vec(out + i, acc_pack<T>(a, sc));
   }
   ep.commit(d, blockIdx.x);
 }
@@ -208,8 +212,9 @@ template <> __device__ __forceinline__ uint4 nvls_ld_reduce<__half>(const void* 
 template <> __device__ __forceinline__ uint4 nvls_ld_reduce<__nv_bfloat16>(const void* p) { return multimem_ld_reduce_bf16x8(p); }
 
 template <typename T, int OP, bool NVLS>
-__global__ void __launch_bounds__(512) allreduce_twoshot_kernel(const __grid_constant__ SymmDev d, size_t buf_off, size_t nvec, float scale) {
+__global__ void __launch_bounds__(512) allreduce_twoshot_kernel(const __grid_constant__ SymmDev d, size_t buf_off, size_t nvec, double scale) {
   SymmEpoch ep(d, blockIdx.x);
+  const auto sc = static_cast<typename Acc<T>::type>(scale);
   const size_t per = (nvec + d.world - 1) / d.world;  // vectors per slice
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   const size_t first = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -220,17 +225,17 @@ __global__ void __launch_bounds__(512) allreduce_twoshot_kernel(const __grid_con
       const size_t off = buf_off + (lo + j) * 16;
       if constexpr (NVLS) {
         uint4 v = nvls_ld_reduce<T>(d.mc + off);
-        if (scale != 1.f) {
+        if (scale != 1.0) {
           typename Acc<T>::type a[VecOf<T>::N];
           acc_init<T, OP>(a, v);
-          v = acc_pack<T>(a, scale);
+          v = acc_pack<T>(a, sc);
         }
         mc_st_vec(d.mc + off, v);  // lands in every rank's buffer
       } else {
         typename Acc<T>::type a[VecOf<T>::N];
         acc_init<T, OP>(a, ld_vec_nc(d.peer[0] + off));
         for (int r = 1; r < d.world; ++r) acc_add<T, OP>(a, ld_vec_nc(d.peer[r] + off));
-        st_vec(d.peer[d.rank] + off, acc_pack<T>(a, scale));
+        st_vec(d.peer[d.rank] + off, acc_pack<T>(a, sc));
       }
     }
   }
@@ -256,8 +261,9 @@ __global__ void __launch_bounds__(512) allreduce_twoshot_kernel(const __grid_con
 // reduce(root): the root takes everything, the others only attend the barrier.
 template <typename T, int OP>
 __global__ void __launch_bounds__(512) reduce_pull_kernel(const __grid_constant__ SymmDev d, size_t stage_off, size_t begin, size_t count, uint4* out,
-                                                          float scale) {
+                                                          double scale) {
   SymmEpoch ep(d, blockIdx.x);
+  const auto sc = static_cast<typename Acc<T>::type>(scale);
   symm_barrier_block(d, blockIdx.x, ep.next());
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < count; i += stride) {
@@ -265,7 +271,7 @@ __global__ void __launch_bounds__(512) reduce_pull_kernel(const __grid_constant_
     typename Acc<T>::type a[VecOf<T>::N];
     acc_init<T, OP>(a, ld_vec_nc(d.peer[0] + off));
     for (int r = 1; r < d.world; ++r) acc_add<T, OP>(a, ld_vec_nc(d.peer[r] + off));
-    st_vec(out + i, acc_pack<T>(a, scale));
+    st_vec(out + i, acc_pack<T>(a, sc));
   }
   ep.commit(d, blockIdx.x);
 }
@@ -426,6 +432,21 @@ template <typename T, int OP> constexpr bool op_supported() {
     default: throw std::invalid_argument("unsupported dtype for NVLink collectives"); \
   }
 
+// The op a launcher runs for (dtype, op), after rejecting what has no defined result.  A scale ≠ 1 on an integer type would be
+// dropped (apply_scale), so it is an error.  On bool, SUM is logical OR and PRODUCT logical AND, as torch's NCCL backend maps them
+// (to MAX / MIN); on 0/1 bytes MIN and MAX are AND and OR as well, and AVG has no bool result.
+int checked_op(int dtype, int op, double scale) {
+  const bool floating = dtype == SD_F32 || dtype == SD_F64 || dtype == SD_F16 || dtype == SD_BF16;
+  if (scale != 1.0 && !floating) throw std::invalid_argument("a reduction scale is only defined for floating-point tensors");
+  if (dtype != SD_BOOL) return op;
+  switch (op) {
+    case SO_SUM: case SO_MAX: case SO_BOR: return SO_BOR;
+    case SO_PROD: case SO_MIN: case SO_BAND: return SO_BAND;
+    case SO_BXOR: return SO_BXOR;
+    default: throw std::invalid_argument("AVG is not defined for bool tensors");
+  }
+}
+
 size_t elem_size(int dtype) {
   switch (dtype) {
     case SD_F32: case SD_I32: return 4;
@@ -441,14 +462,14 @@ void launch_allreduce_oneshot_push(const SymmDev& d, const void* in, void* out, 
                                    int op, double scale, bool use_mc, SymmLaunchCfg cfg, cudaStream_t s) {
   const size_t nbytes = count * elem_size(dtype);
   if (nbytes % 16 != 0) throw std::invalid_argument("oneshot push: byte count must be a multiple of 16 (caller pads)");
+  op = checked_op(dtype, op, scale);
   const size_t nvec = nbytes / 16;
   if (nvec == 0) return;
   const int threads = cfg.threads ? cfg.threads : 256;
   const int blocks = std::min(cfg.blocks ? cfg.blocks : auto_blocks(nvec, threads, 64), kSymmMaxBlocks);
-  const float sc = static_cast<float>(scale);
   PDT_DISPATCH_TYPE(dtype, PDT_DISPATCH_OP(T, op, {
-    if (use_mc) allreduce_oneshot_push_kernel<T, OP, true><<<blocks, threads, 0, s>>>(d, static_cast<const uint4*>(in), static_cast<uint4*>(out), stage_off, nvec, sc);
-    else allreduce_oneshot_push_kernel<T, OP, false><<<blocks, threads, 0, s>>>(d, static_cast<const uint4*>(in), static_cast<uint4*>(out), stage_off, nvec, sc);
+    if (use_mc) allreduce_oneshot_push_kernel<T, OP, true><<<blocks, threads, 0, s>>>(d, static_cast<const uint4*>(in), static_cast<uint4*>(out), stage_off, nvec, scale);
+    else allreduce_oneshot_push_kernel<T, OP, false><<<blocks, threads, 0, s>>>(d, static_cast<const uint4*>(in), static_cast<uint4*>(out), stage_off, nvec, scale);
   }));
   check_launch("allreduce_oneshot_push");
 }
@@ -481,24 +502,24 @@ void launch_allreduce_twoshot(const SymmDev& d, size_t buf_off, size_t count, in
                               SymmLaunchCfg cfg, cudaStream_t s) {
   const size_t nbytes = count * elem_size(dtype);
   if (nbytes % 16 != 0 || buf_off % 16 != 0) throw std::invalid_argument("twoshot: buffer must be 16-byte aligned and sized");
+  op = checked_op(dtype, op, scale);
   const size_t nvec = nbytes / 16;
   if (nvec == 0) return;
   const int threads = cfg.threads ? cfg.threads : 512;
   const size_t per = (nvec + d.world - 1) / d.world;
   // the two-shot kernels use at most one CTA per SM
   const int blocks = std::min(cfg.blocks ? cfg.blocks : auto_blocks(per, threads, sm_count()), kSymmMaxBlocks);
-  const float sc = static_cast<float>(scale);
   if (nvls) {
     if (!d.mc) throw std::runtime_error("twoshot nvls requested but the heap has no multicast mapping");
     if (!(op == SO_SUM || op == SO_AVG)) throw std::invalid_argument("NVLS reduction supports SUM only");
     switch (dtype) {
-      case SD_F32: allreduce_twoshot_kernel<float, SO_SUM, true><<<blocks, threads, 0, s>>>(d, buf_off, nvec, sc); break;
-      case SD_F16: allreduce_twoshot_kernel<__half, SO_SUM, true><<<blocks, threads, 0, s>>>(d, buf_off, nvec, sc); break;
-      case SD_BF16: allreduce_twoshot_kernel<__nv_bfloat16, SO_SUM, true><<<blocks, threads, 0, s>>>(d, buf_off, nvec, sc); break;
+      case SD_F32: allreduce_twoshot_kernel<float, SO_SUM, true><<<blocks, threads, 0, s>>>(d, buf_off, nvec, scale); break;
+      case SD_F16: allreduce_twoshot_kernel<__half, SO_SUM, true><<<blocks, threads, 0, s>>>(d, buf_off, nvec, scale); break;
+      case SD_BF16: allreduce_twoshot_kernel<__nv_bfloat16, SO_SUM, true><<<blocks, threads, 0, s>>>(d, buf_off, nvec, scale); break;
       default: throw std::invalid_argument("NVLS reduction supports f32/f16/bf16 only");
     }
   } else {
-    PDT_DISPATCH_TYPE(dtype, PDT_DISPATCH_OP(T, op, { allreduce_twoshot_kernel<T, OP, false><<<blocks, threads, 0, s>>>(d, buf_off, nvec, sc); }));
+    PDT_DISPATCH_TYPE(dtype, PDT_DISPATCH_OP(T, op, { allreduce_twoshot_kernel<T, OP, false><<<blocks, threads, 0, s>>>(d, buf_off, nvec, scale); }));
   }
   check_launch("allreduce_twoshot");
 }
@@ -525,11 +546,11 @@ void launch_alltoall_pull(const SymmDev& d, size_t src_off, void* dst, size_t nb
 void launch_reduce_pull(const SymmDev& d, size_t stage_off, size_t begin_vec, size_t count_vec, size_t total_vec, void* out, int dtype, int op,
                         double scale, SymmLaunchCfg cfg, cudaStream_t s) {
   if (stage_off % 16 != 0) throw std::invalid_argument("reduce_pull: staging offset must be 16-byte aligned");
+  op = checked_op(dtype, op, scale);
   const int threads = cfg.threads ? cfg.threads : 512;
   // every rank must launch the same grid (the barrier is per block): size it by the whole vector, not by this rank's share
   const int blocks = std::min(cfg.blocks ? cfg.blocks : auto_blocks(total_vec / std::max(1, d.world) + 1, threads, 64), kSymmMaxBlocks);
-  const float sc = static_cast<float>(scale);
-  PDT_DISPATCH_TYPE(dtype, PDT_DISPATCH_OP(T, op, { reduce_pull_kernel<T, OP><<<blocks, threads, 0, s>>>(d, stage_off, begin_vec, count_vec, static_cast<uint4*>(out), sc); }));
+  PDT_DISPATCH_TYPE(dtype, PDT_DISPATCH_OP(T, op, { reduce_pull_kernel<T, OP><<<blocks, threads, 0, s>>>(d, stage_off, begin_vec, count_vec, static_cast<uint4*>(out), scale); }));
   check_launch("reduce_pull");
 }
 

@@ -9,7 +9,9 @@
 
 namespace pdt {
 
-// Must match pdt::DType / pdt::ReduceOp (csrc/cpu/cpu_backend.h).
+// Must match pdt::DType / pdt::ReduceOp (csrc/cpu/cpu_backend.h).  The reducing launchers take AVG as SUM (the caller passes
+// 1/world in `scale`), reject a scale != 1 on integer and bool types, run SUM / MAX on bool as logical OR and PRODUCT / MIN as
+// logical AND, and reject AVG on bool.  MIN / MAX propagate NaN from any rank.
 enum SymmDType : int { SD_F32 = 0, SD_F64 = 1, SD_F16 = 2, SD_BF16 = 3, SD_I8 = 4, SD_U8 = 5, SD_I32 = 6, SD_I64 = 7, SD_BOOL = 8, SD_I16 = 9 };
 enum SymmOp : int { SO_SUM = 0, SO_AVG = 1, SO_PROD = 2, SO_MIN = 3, SO_MAX = 4, SO_BAND = 5, SO_BOR = 6, SO_BXOR = 7 };
 

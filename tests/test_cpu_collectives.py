@@ -26,6 +26,15 @@ def _collectives(rank, world):
         t = torch.ones(33, dtype=dt) * (rank + 1)
         dist.all_reduce(t)
         assert torch.equal(t, torch.ones(33, dtype=dt) * sum(range(1, world + 1))), str(dt)
+    # bool: SUM / MAX are logical OR, PRODUCT / MIN logical AND (torch's NCCL backend), never a byte count; AVG has no bool result
+    col = torch.tensor([rank == 0, True, False, rank % 2 == 1])
+    for op, exp in ((dist.ReduceOp.SUM, [True, True, False, True]), (dist.ReduceOp.MAX, [True, True, False, True]),
+                    (dist.ReduceOp.PRODUCT, [False, True, False, False]), (dist.ReduceOp.MIN, [False, True, False, False])):
+        t = col.clone()
+        dist.all_reduce(t, op)
+        assert t.view(torch.uint8).tolist() == [int(e) for e in exp], (op, t.view(torch.uint8).tolist())
+    with pytest.raises(Exception, match="bool"):
+        dist.all_reduce(col.clone(), dist.ReduceOp.AVG)
     # bitwise identical results on all ranks for a big random vector (ring path)
     g = torch.Generator().manual_seed(rank)
     big = torch.randn(300000, generator=g)

@@ -27,6 +27,7 @@ GROUPS = {
     "accum": ["tests/test_grad_accumulation.py"],
     "ce_options": ["tests/test_cross_entropy_options.py"],
     "syncbn": ["tests/test_syncbn_native.py"],
+    "symm_emu": ["tests/test_symm_kernels_emulated.py"],
 }
 
 
