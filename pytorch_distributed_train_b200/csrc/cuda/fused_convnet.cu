@@ -109,18 +109,24 @@ __device__ __forceinline__ void fold_rows_wide(const float* __restrict__ partial
   __syncthreads();
 }
 
-// Warp-level reduction of 32 per-thread values with 31 shuffles: after the call lane l holds Σ_lanes v[l] in v[0].
-__device__ __forceinline__ void warp_transpose_reduce32(float (&v)[32], int lane) {
+// Warp-level reduction of 32 per-thread values with 31 shuffles: after the call lane l holds Σ_lanes v[l] in v[0].  One step per
+// template instance, so that every index into v is a constant and v stays in registers.
+template <int HALF>
+__device__ __forceinline__ void warp_transpose_reduce_step(float (&v)[32], int lane) {
+  const bool upper = (lane & HALF) != 0;
 #pragma unroll
-  for (int off = 16, half = 16; off >= 1; off >>= 1, half >>= 1) {
-    const bool upper = (lane & off) != 0;
-#pragma unroll
-    for (int i = 0; i < half; ++i) {
-      const float send = upper ? v[i] : v[i + half];
-      const float keep = upper ? v[i + half] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-    }
+  for (int i = 0; i < HALF; ++i) {
+    const float send = upper ? v[i] : v[i + HALF];
+    const float keep = upper ? v[i + HALF] : v[i];
+    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, HALF);
   }
+}
+__device__ __forceinline__ void warp_transpose_reduce32(float (&v)[32], int lane) {
+  warp_transpose_reduce_step<16>(v, lane);
+  warp_transpose_reduce_step<8>(v, lane);
+  warp_transpose_reduce_step<4>(v, lane);
+  warp_transpose_reduce_step<2>(v, lane);
+  warp_transpose_reduce_step<1>(v, lane);
 }
 
 // =====================================================================================================================
@@ -147,12 +153,14 @@ struct L1Map {
   }
 };
 
+// The zero-haloed image by the NT threads of the CTA.
+template <int NT>
 __device__ __forceinline__ void l1_load_image(const float* __restrict__ x, float* xs /*[32][32]*/, int tid) {
-  for (int i = tid; i < 1024; i += kL1Threads) xs[i] = 0.f;
+  for (int i = tid; i < 1024; i += NT) xs[i] = 0.f;
   __syncthreads();
-  if (tid < 784) {
-    const int rr = tid / 28, cc = tid - rr * 28;
-    xs[(rr + 2) * 32 + cc + 2] = x[tid];
+  for (int i = tid; i < 784; i += NT) {
+    const int rr = i / 28, cc = i - rr * 28;
+    xs[(rr + 2) * 32 + cc + 2] = x[i];
   }
 }
 
@@ -384,7 +392,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   TRACE_INIT();
   trace(1, 0);
 
-  l1_load_image(x + static_cast<size_t>(n) * 784, xs, tid);
+  l1_load_image<kL1Threads>(x + static_cast<size_t>(n) * 784, xs, tid);
   if (tid < 16) {
     const float mean = saved[tid], invstd = saved[16 + tid];
     const float g = gamma ? gamma[tid] : 1.f, b = beta ? beta[tid] : 0.f;
@@ -770,46 +778,79 @@ constexpr int kPatchAlloc = 43008;               // + slack rows read by the pad
 
 __device__ __forceinline__ uint32_t sw128_off(int row, int chunk16) { return static_cast<uint32_t>(row) * 128u + (static_cast<uint32_t>(chunk16 ^ (row & 7)) << 4); }
 
-// conv2 of one image on the tensor cores, issued by the warpgroup of warps 4..7 (wt = thread index inside it): per output
-// tile t, 25 taps × 2 K-steps of wgmma m64n32k8 per 64-row half, the A descriptors row-shifted into the haloed patch.  The
-// accumulators go straight into ys [pixel][32] (bias added; 16-byte chunks rotated by the pixel index, as the column reads
-// that follow expect).
-__device__ __forceinline__ void l2_conv_wgmma(const uint8_t* sa, const uint8_t* sb, const float* __restrict__ bias, float* ys, int wt) {
+// Row P of the 128 halo rows of the 18 × 18 patch (h < 128): the top two rows, the two side columns on each side of rows 2..15,
+// the bottom two rows.
+__device__ __forceinline__ int patch_halo_row(int h) {
+  if (h < 36) return h;
+  if (h >= 92) return 16 * kPW + (h - 92);
+  const int s = h - 36, side = s & 3;
+  return (2 + (s >> 2)) * kPW + (side < 2 ? side : 14 + side);
+}
+
+// Output tile t of conv2 of one image on the tensor cores, issued by one warpgroup (wt = thread index inside it; the two tiles run
+// on two warpgroups at once): 25 taps × 2 K-steps of wgmma m64n32k8 per 64-row half, the two halves independent accumulator
+// chains, the A descriptors row-shifted into the haloed patch.  The accumulators go straight into ys [pixel][32] (bias added;
+// 16-byte chunks rotated by the pixel index, as the column reads that follow expect), and the BatchNorm sums of the kept elements
+// are taken while they are still in registers: s_stat[8 warps][64] gets this warp's Σy (columns 0..31) and Σy² (32..63).
+__device__ __forceinline__ void l2_conv_wgmma(const uint8_t* sa, const uint8_t* sb, const float* __restrict__ bias, float* ys, float* s_stat,
+                                              int t, int wt) {
   const uint64_t ad0 = gmma_desc_kmajor<128>(smem_u32(sa)), bd0 = gmma_desc_kmajor<128>(smem_u32(sb));
+  float acc[2][16];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int e = 0; e < 16; ++e) acc[h][e] = 0.f;
+  wgmma_fence();
 #pragma unroll 1
-  for (int t = 0; t < 2; ++t) {
-    float acc[2][16];
+  for (int kh = 0; kh < 5; ++kh) {
+    const uint64_t ad = ad0 + static_cast<uint64_t>(((7 * t + kh) * kPW * 128) >> 4);
+    const uint64_t bd = bd0 + static_cast<uint64_t>((kh * 5 * 4096) >> 4);
 #pragma unroll
-    for (int h = 0; h < 2; ++h)
+    for (int kw = 0; kw < 5; ++kw) {
 #pragma unroll
-      for (int e = 0; e < 16; ++e) acc[h][e] = 0.f;
-    wgmma_fence();
-#pragma unroll 1
-    for (int kh = 0; kh < 5; ++kh) {
-      const uint64_t ad = ad0 + static_cast<uint64_t>(((7 * t + kh) * kPW * 128) >> 4);
-      const uint64_t bd = bd0 + static_cast<uint64_t>((kh * 5 * 4096) >> 4);
+      for (int k = 0; k < 2; ++k)   // K = 16 input channels = two K=8 steps; the zero upper half is never multiplied
 #pragma unroll
-      for (int kw = 0; kw < 5; ++kw) {
+        for (int h = 0; h < 2; ++h)
+          wgmma_m64n32k8_tf32(acc[h], ad + ((h * 64 * 128 + kw * 128 + k * 32) >> 4), bd + ((kw * 4096 + k * 32) >> 4), (kh | kw | k) != 0);
+    }
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  // a thread holds 8 columns, c = 8·(e >> 2) + 2·(wt & 3) + (e & 1): sums slot k = 2·(e >> 2) + (e & 1)
+  float s1[8], s2[8];
 #pragma unroll
-        for (int k = 0; k < 2; ++k)   // K = 16 input channels = two K=8 steps; the zero upper half is never multiplied
+  for (int k = 0; k < 8; ++k) s1[k] = s2[k] = 0.f;
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
-            wgmma_m64n32k8_tf32(acc[h], ad + ((h * 64 * 128 + kw * 128 + k * 32) >> 4), bd + ((kw * 4096 + k * 32) >> 4), (kh | kw | k) != 0);
+  for (int h = 0; h < 2; ++h) {
+#pragma unroll
+    for (int e = 0; e < 16; ++e) {
+      const int rr = 64 * h + wgmma_frag_row(wt, e), c = wgmma_frag_col(wt, e), k = 2 * (e >> 2) + (e & 1);
+      const int orow = rr / kPW, ow = rr - orow * kPW;
+      if (rr < 126 && ow < 14) {
+        const int pix = (7 * t + orow) * 14 + ow;
+        const float v = acc[h][e] + (bias ? __ldg(bias + c) : 0.f);
+        ys[pix * 32 + ((((c >> 2) + pix) & 7) << 2) + (c & 3)] = v;
+        s1[k] += v;
+        s2[k] = fmaf(v, v, s2[k]);
       }
     }
-    wgmma_commit();
-    wgmma_wait<0>();
+  }
+  // lanes 4 apart hold the same columns
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
+  for (int off = 4; off <= 16; off <<= 1)
 #pragma unroll
-      for (int e = 0; e < 16; ++e) {
-        const int rr = 64 * h + wgmma_frag_row(wt, e), c = wgmma_frag_col(wt, e);
-        const int orow = rr / kPW, ow = rr - orow * kPW;
-        if (rr < 126 && ow < 14) {
-          const int pix = (7 * t + orow) * 14 + ow;
-          ys[pix * 32 + ((((c >> 2) + pix) & 7) << 2) + (c & 3)] = acc[h][e] + (bias ? __ldg(bias + c) : 0.f);
-        }
-      }
+    for (int k = 0; k < 8; ++k) {
+      s1[k] += __shfl_xor_sync(0xffffffffu, s1[k], off);
+      s2[k] += __shfl_xor_sync(0xffffffffu, s2[k], off);
+    }
+  const int lane = wt & 31;
+  if (lane < 4) {
+    float* row = s_stat + (4 * t + (wt >> 5)) * 64;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const int c = 8 * (k >> 1) + 2 * lane + (k & 1);
+      row[c] = s1[k];
+      row[32 + c] = s2[k];
     }
   }
 }
@@ -817,8 +858,46 @@ __device__ __forceinline__ void l2_conv_wgmma(const uint8_t* sa, const uint8_t* 
 struct L2FwdSmem {
   static constexpr int kB = 25 * 32 * 128;       // weights: [tap][32 co][128 B] (ci 0..15 used)            102,400
   static constexpr int kYs = 196 * 32 * 4;       // conv output of the image, [pixel][32]                     25,088
-  static constexpr int kTotal = 1024 + kPatchAlloc + kB + kYs + 8192;
+  static constexpr int kMisc = 1024 * 4;         // statistics and classifier scratch                          4,096
+  static constexpr int kTotal = 1024 + kPatchAlloc + kB + kYs + kMisc;
 };
+
+// The forward's CTA: every compute thread owns the same pixel d of two pooling windows, win and win + 98 (392 threads, the
+// 4-lanes-per-window order of L1Map kept), in 13 warps.  The register budget of 416 threads holds both pixels' accumulators and
+// the 32-value statistics reduction without local memory, and every conv1 weight read from shared memory serves two pixels.
+constexpr int kFwdPix = 392;
+constexpr int kFwdThreads = 416;
+constexpr int kFwdWarps = kFwdThreads / 32;
+
+// conv1 output of one pixel → y1 (backward reads it).
+__device__ __forceinline__ void l1_store_y(float* __restrict__ y1, int n, const L1Map& m, const float (&acc)[16]) {
+  float4* yp = reinterpret_cast<float4*>(y1 + ((static_cast<size_t>(n) * 28 + m.r) * 28 + m.c) * 16);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) yp[q] = make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
+}
+
+// BN + ReLU + 2×2 max-pool of one pixel's window (two shuffles; called by every lane) → conv2's patch and the global frame p1n.
+__device__ __forceinline__ void l1_pool_store(const float (&acc)[16], const L1Map& m, const float* s_scale, const float* s_shift, uint8_t* sa,
+                                              float* __restrict__ p1n) {
+  float z[16];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    float t = fmaxf(fmaf(acc[j], s_scale[j], s_shift[j]), 0.f);
+    t = fmaxf(t, __shfl_xor_sync(0xffffffffu, t, 1));
+    t = fmaxf(t, __shfl_xor_sync(0xffffffffu, t, 2));
+    z[j] = t;
+  }
+  if (m.valid) {  // lane d of the window owns channels 4d..4d+3 = one 16-byte chunk of the 128-byte patch row
+    float4 o;
+    if (m.d == 0) o = make_float4(z[0], z[1], z[2], z[3]);
+    else if (m.d == 1) o = make_float4(z[4], z[5], z[6], z[7]);
+    else if (m.d == 2) o = make_float4(z[8], z[9], z[10], z[11]);
+    else o = make_float4(z[12], z[13], z[14], z[15]);
+    const int P = (m.ph + 2) * kPW + m.pw + 2;
+    *reinterpret_cast<float4*>(sa + sw128_off(P, m.d)) = o;   // conv2 reads this one
+    reinterpret_cast<float4*>(p1n + P * 16)[m.d] = o;          // backward (conv2 wgrad) reads this one
+  }
+}
 
 // =====================================================================================================================
 // Whole forward pass in ONE kernel: layer 1 and layer 2 (+ classifier) of an image run in the same CTA, so the pooled
@@ -832,7 +911,7 @@ __device__ __forceinline__ float ce_scale(const FusedCe&) { return 1.f; }
 __device__ __forceinline__ float ce_scale(const ScaledCe& ce) { return ce.scale; }
 
 template <class Ce = FusedCe>
-__global__ void __launch_bounds__(kL1Threads, 1)
+__global__ void __launch_bounds__(kFwdThreads, 1)
 convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ g1,
                    const float* __restrict__ be1, float* __restrict__ y1, float* __restrict__ p1, float* saved1, float* rm1, float* rv1,
                    long long* nbt1, float mom1, float eps1, const float* __restrict__ w2, const float* __restrict__ b2,
@@ -846,73 +925,78 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
   uint8_t* sa = smem;                                  // conv2 input patch, written by this CTA's layer-1 epilogue
   uint8_t* sb = sa + kPatchAlloc;                      // conv2 weights
   float* ys = reinterpret_cast<float*>(sb + L2FwdSmem::kB);
-  float* misc = ys + 196 * 32;                         // 2048 floats
-  float* s_part = misc;                                // [4][64] / [25 warps][16]
-  float* s_tmp2 = misc + 1024;                         // [12][64]
-  float* s_tot2 = misc + 768;                          // [64]
-  float* s_scale2 = misc + 832;                        // [32]
-  float* s_shift2 = misc + 864;                        // [32]
+  float* misc = ys + 196 * 32;                         // 1024 floats
+  float* s_part = misc;                                // [8 warps][64] conv2 statistics / [13 warps][16] classifier partials
+  float* s_tot2 = misc + 512;                          // [64]
+  float* s_scale2 = misc + 576;                        // [32]
+  float* s_shift2 = misc + 608;                        // [32]
+  float* s_tmp2 = misc + 640;                          // [6][64]
   __shared__ float xs[32 * 32];
   __shared__ __align__(16) float ws[25 * 16];
-  __shared__ float red[kL1Warps * 32];
-  __shared__ float s_tmp[kL1Warps * 32];
+  __shared__ float red[kFwdWarps * 32];
+  __shared__ float s_tmp[kFwdWarps * 32];
   __shared__ float s_tot[32];
   __shared__ float s_scale[16], s_shift[16];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = blockIdx.x, B = gridDim.x;
-  const L1Map m(tid);
+  // pixel d of windows win and win + 98; the threads past kFwdPix own none (L1Map(784) is not valid)
+  const L1Map m0(tid < kFwdPix ? tid : 784), m1(tid < kFwdPix ? tid + kFwdPix : 784);
   GridBar bar(gs);
   TRACE_INIT();
   trace(0, 0);
 
-  for (int i = tid; i < kPatchAlloc / 16; i += kL1Threads) reinterpret_cast<float4*>(sa)[i] = make_float4(0.f, 0.f, 0.f, 0.f);   // halo = 0
-  l1_load_image(x + static_cast<size_t>(n) * 784, xs, tid);
+  // conv2 weights [co][ci][tap] → the swizzled K-major tiles [tap][co][ci], one float per cp.async: nothing is held in registers
+  // while they fly, behind conv1.  One (co, ci) pair per thread and its 25 taps, so that the 32 lanes of a copy write 32 different
+  // banks (consecutive taps are 4 KiB apart in shared memory: one bank).
+  for (int pair = tid; pair < 32 * 16; pair += kFwdThreads) {
+    const int co = pair >> 4, ci = pair & 15;
+    const uint32_t dst = smem_u32(sb + sw128_off(co, ci >> 2) + (ci & 3) * 4);
+#pragma unroll
+    for (int tap = 0; tap < 25; ++tap) cp_async_4(dst + tap * 4096, w2 + pair * 25 + tap);
+  }
+  cp_async_commit();
+  // the patch's zero halo: the 64 bytes (channels 0..15) the descriptors read of each halo row.  The slack rows past 324 are left
+  // as they are: only the padding rows of tile 1 read them, and those outputs are dropped.
+  for (int i = tid; i < 128 * 4; i += kFwdThreads)
+    *reinterpret_cast<float4*>(sa + sw128_off(patch_halo_row(i >> 2), i & 3)) = make_float4(0.f, 0.f, 0.f, 0.f);
+  l1_load_image<kFwdThreads>(x + static_cast<size_t>(n) * 784, xs, tid);
   if (tid < 400) {
     const int tap = tid >> 4, co = tid & 15;
     ws[tid] = w1[co * 25 + tap];
   }
-  // conv2 weights: one (co, ci) pair per thread, 25 taps contiguous in global, 4 KiB apart in smem (SWIZZLE_128B K-major tiles);
-  // the loads fly while conv1 computes
-  float wv[25];
-  if (tid < 512) {
-#pragma unroll
-    for (int tap = 0; tap < 25; ++tap) wv[tap] = __ldg(w2 + tid * 25 + tap);
-  }
   __syncthreads();
   trace(0, 11);
 
-  // ---- layer 1 ------------------------------------------------------------------------------------------------------
-  float acc[16];
+  // ---- layer 1: both pixels in the FMA order of one pixel per thread, so y1 does not depend on the CTA shape ---------------
+  float acc0[16], acc1[16];
 #pragma unroll
-  for (int j = 0; j < 16; ++j) acc[j] = b1 ? __ldg(b1 + j) : 0.f;
+  for (int j = 0; j < 16; ++j) acc0[j] = acc1[j] = b1 ? __ldg(b1 + j) : 0.f;
 #pragma unroll 1
   for (int kh = 0; kh < 5; ++kh) {
 #pragma unroll
     for (int kw = 0; kw < 5; ++kw) {
-      const float xv = xs[(m.r + kh) * 32 + m.c + kw];
+      const float xv0 = xs[(m0.r + kh) * 32 + m0.c + kw], xv1 = xs[(m1.r + kh) * 32 + m1.c + kw];
       const float4* wt = reinterpret_cast<const float4*>(ws + (kh * 5 + kw) * 16);
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         const float4 wq = wt[q];
-        acc[4 * q + 0] = fmaf(xv, wq.x, acc[4 * q + 0]);
-        acc[4 * q + 1] = fmaf(xv, wq.y, acc[4 * q + 1]);
-        acc[4 * q + 2] = fmaf(xv, wq.z, acc[4 * q + 2]);
-        acc[4 * q + 3] = fmaf(xv, wq.w, acc[4 * q + 3]);
+        acc0[4 * q + 0] = fmaf(xv0, wq.x, acc0[4 * q + 0]);
+        acc0[4 * q + 1] = fmaf(xv0, wq.y, acc0[4 * q + 1]);
+        acc0[4 * q + 2] = fmaf(xv0, wq.z, acc0[4 * q + 2]);
+        acc0[4 * q + 3] = fmaf(xv0, wq.w, acc0[4 * q + 3]);
+        acc1[4 * q + 0] = fmaf(xv1, wq.x, acc1[4 * q + 0]);
+        acc1[4 * q + 1] = fmaf(xv1, wq.y, acc1[4 * q + 1]);
+        acc1[4 * q + 2] = fmaf(xv1, wq.z, acc1[4 * q + 2]);
+        acc1[4 * q + 3] = fmaf(xv1, wq.w, acc1[4 * q + 3]);
       }
     }
   }
   trace(0, 1);
-  if (tid < 512) {
-    const int co = tid >> 4, ci = tid & 15;
-    uint8_t* dst = sb + sw128_off(co, ci >> 2) + (ci & 3) * 4;
-#pragma unroll
-    for (int tap = 0; tap < 25; ++tap) *reinterpret_cast<float*>(dst + tap * 4096) = wv[tap];
-  }
   {
     float v[32];
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
-      v[j] = m.valid ? acc[j] : 0.f;
-      v[16 + j] = m.valid ? acc[j] * acc[j] : 0.f;
+      v[j] = m0.valid ? acc0[j] + acc1[j] : 0.f;
+      v[16 + j] = m0.valid ? fmaf(acc1[j], acc1[j], acc0[j] * acc0[j]) : 0.f;
     }
     warp_transpose_reduce32(v, lane);
     red[warp * 32 + lane] = v[0];
@@ -920,25 +1004,23 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
   __syncthreads();
   if (tid < 32) {
     float s = 0.f;
-#pragma unroll 5
-    for (int wi = 0; wi < kL1Warps; ++wi) s += red[wi * 32 + tid];
+#pragma unroll
+    for (int wi = 0; wi < kFwdWarps; ++wi) s += red[wi * 32 + tid];
     partials[static_cast<size_t>(n) * 32 + tid] = s;
   }
   trace(0, 2);
   bar.arrive(gs);
   // in the barrier's shadow: everything layer 1 owes to global memory (backward reads it; nothing in this kernel does)
-  if (m.valid) {
-    float4* yp = reinterpret_cast<float4*>(y1 + ((static_cast<size_t>(n) * 28 + m.r) * 28 + m.c) * 16);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) yp[q] = make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
+  if (m0.valid) {
+    l1_store_y(y1, n, m0, acc0);
+    l1_store_y(y1, n, m1, acc1);
   }
-  for (int i = tid; i < 324 * 4; i += kL1Threads) {
-    const int P = i >> 2, pr = P / 18, pc = P - pr * 18;
-    if (pr < 2 || pr >= 16 || pc < 2 || pc >= 16) reinterpret_cast<float4*>(p1 + (static_cast<size_t>(n) * 324 + P) * 16)[i & 3] = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
+  float* p1n = p1 + static_cast<size_t>(n) * 324 * 16;
+  for (int i = tid; i < 128 * 4; i += kFwdThreads)
+    reinterpret_cast<float4*>(p1n + patch_halo_row(i >> 2) * 16)[i & 3] = make_float4(0.f, 0.f, 0.f, 0.f);
   bar.wait(gs);
   trace(0, 3);
-  fold_rows_wide<32, kL1Threads>(partials, B, s_tmp, s_tot);
+  fold_rows_wide<32, kFwdThreads>(partials, B, s_tmp, s_tot);
   if (tid < 16) {
     const float cnt = static_cast<float>(B) * 784.f;
     const float mean = s_tot[tid] / cnt;
@@ -959,54 +1041,31 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
     }
   }
   __syncthreads();
-  {
-    float z[16];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      float t = fmaxf(fmaf(acc[j], s_scale[j], s_shift[j]), 0.f);
-      t = fmaxf(t, __shfl_xor_sync(0xffffffffu, t, 1));
-      t = fmaxf(t, __shfl_xor_sync(0xffffffffu, t, 2));
-      z[j] = t;
-    }
-    if (m.valid) {  // lane d of the window owns channels 4d..4d+3 = one 16-byte chunk of the 128-byte patch row
-      float4 o;
-      if (m.d == 0) o = make_float4(z[0], z[1], z[2], z[3]);
-      else if (m.d == 1) o = make_float4(z[4], z[5], z[6], z[7]);
-      else if (m.d == 2) o = make_float4(z[8], z[9], z[10], z[11]);
-      else o = make_float4(z[12], z[13], z[14], z[15]);
-      const int P = (m.ph + 2) * kPW + m.pw + 2;
-      *reinterpret_cast<float4*>(sa + sw128_off(P, m.d)) = o;                                   // conv2 reads this one
-      reinterpret_cast<float4*>(p1 + (static_cast<size_t>(n) * 324 + P) * 16)[m.d] = o;         // backward (conv2 wgrad) reads this one
-    }
-  }
+  l1_pool_store(acc0, m0, s_scale, s_shift, sa, p1n);
+  l1_pool_store(acc1, m1, s_scale, s_shift, sa, p1n);
+  cp_async_wait<0>();         // this thread's weight copies have landed
   fence_proxy_async_smem();   // generic-proxy writes of the patch and of the weights → visible to the tensor core
   __syncthreads();
   trace(0, 4);
-  // ---- layer 2: 200 wgmma (K = 8, M = 64 each) by the warpgroup of warps 4..7 --------------------------------------------
-  if (warpgroup_index() == 1) l2_conv_wgmma(sa, sb, b2, ys, tid - 128);
+  // ---- layer 2: 2 × 100 wgmma (K = 8, M = 64 each), output tile t by warpgroup t -------------------------------------------
+  const int wg = warpgroup_index();
+  if (wg < 2) l2_conv_wgmma(sa, sb, b2, ys, s_part, wg, tid & 127);
   __syncthreads();
   trace(0, 5);
-  if (tid < 128) {
-    const int c = tid & 31, part = tid >> 5;
-    float s1 = 0.f, s2 = 0.f;
-    for (int p = part * 49; p < part * 49 + 49; ++p) {
-      const float val = ys[p * 32 + ((((c >> 2) + p) & 7) << 2) + (c & 3)];
-      s1 += val;
-      s2 = fmaf(val, val, s2);
-    }
-    s_part[part * 64 + c] = s1;
-    s_part[part * 64 + 32 + c] = s2;
-  }
-  __syncthreads();
   float* partials2 = partials + static_cast<size_t>(B) * 32;
-  if (tid < 64) partials2[static_cast<size_t>(n) * 64 + tid] = (s_part[tid] + s_part[64 + tid]) + (s_part[128 + tid] + s_part[192 + tid]);
+  if (tid < 64) {
+    float s = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) s += s_part[w * 64 + tid];
+    partials2[static_cast<size_t>(n) * 64 + tid] = s;
+  }
   trace(0, 6);
   bar.arrive(gs);
   float* fcs = reinterpret_cast<float*>(sb + 8192);   // classifier weights, staged behind the pooled activations (conv2's weights are dead)
   // only where they fit before ys, which is still being read: up to 15 classes; 16 are read from global memory
   const bool fc_staged = logits != nullptr && (reinterpret_cast<uintptr_t>(fcw) & 15) == 0 && ncls * 1568 * 4 <= L2FwdSmem::kB - 8192;
   if (fc_staged) {
-    for (int i = tid; i < ncls * 392; i += kL1Threads) cp_async_16(smem_u32(fcs + 4 * i), fcw + 4 * i, 16);
+    for (int i = tid; i < ncls * 392; i += kFwdThreads) cp_async_16(smem_u32(fcs + 4 * i), fcw + 4 * i, 16);
     cp_async_commit();
   }
   __shared__ std::conditional_t<kSmooth, float, int> s_counted;   // SmoothCe: the divisor D
@@ -1037,13 +1096,13 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
     counted = __reduce_add_sync(0xffffffffu, counted);
     if (lane == 0) s_counted = counted;
   }
-  for (int i = tid; i < 196 * 8; i += kL1Threads) {   // in the barrier's shadow: conv2's output for the backward pass
+  for (int i = tid; i < 196 * 8; i += kFwdThreads) {   // in the barrier's shadow: conv2's output for the backward pass
     const int pix = i >> 3, q = i & 7;
     reinterpret_cast<float4*>(y2 + (static_cast<size_t>(n) * 196 + pix) * 32)[q] = reinterpret_cast<const float4*>(ys + pix * 32)[(q + pix) & 7];
   }
   bar.wait(gs);
   trace(0, 7);
-  fold_rows_wide<64, kL1Threads>(partials2, B, s_tmp2, s_tot2);
+  fold_rows_wide<64, kFwdThreads>(partials2, B, s_tmp2, s_tot2);
   if (tid < 32) {
     const float cnt = static_cast<float>(B) * 196.f;
     const float mean = s_tot2[tid] / cnt;
@@ -1065,7 +1124,7 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
   }
   __syncthreads();
   float* pool = reinterpret_cast<float*>(sb);   // the weights are dead after the MMAs
-  for (int i = tid; i < 1568; i += kL1Threads) {
+  for (int i = tid; i < 1568; i += kFwdThreads) {
     const int c = i & 31, pp = i >> 5, ph = pp / 7, pw = pp - ph * 7;
     const float sc = s_scale2[c], sh = s_shift2[c];
     float mx = 0.f;
@@ -1079,18 +1138,22 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
   cp_async_wait<0>();
   __syncthreads();
   trace(0, 8);
-  for (int i = tid; i < 1568; i += kL1Threads) out[static_cast<size_t>(n) * 1568 + i] = pool[i];
+  for (int i = tid; i < 1568; i += kFwdThreads) out[static_cast<size_t>(n) * 1568 + i] = pool[i];
   if (logits != nullptr) {
-    // classifier: thread t owns features t and t + 800 for every class (≤ 16): all weight loads independent
-    float accv[16];
-    const float pv0 = pool[tid], pv1 = (tid + kL1Threads < 1568) ? pool[tid + kL1Threads] : 0.f;
+    // classifier: thread t owns features t, t + 416, t + 832 and t + 1248 (< 1568) for every class (≤ 16): all weight loads
+    // independent
+    float accv[16], pv[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) pv[u] = (tid + u * kFwdThreads < 1568) ? pool[tid + u * kFwdThreads] : 0.f;
 #pragma unroll
     for (int c16 = 0; c16 < 16; ++c16) {
       float sacc = 0.f;
       if (c16 < ncls) {
         const float* wr = (fc_staged ? fcs : fcw) + static_cast<size_t>(c16) * 1568 + tid;
-        sacc = pv0 * wr[0];
-        if (tid + kL1Threads < 1568) sacc = fmaf(pv1, wr[kL1Threads], sacc);
+        sacc = pv[0] * wr[0];
+#pragma unroll
+        for (int u = 1; u < 4; ++u)
+          if (tid + u * kFwdThreads < 1568) sacc = fmaf(pv[u], wr[u * kFwdThreads], sacc);
       }
       accv[c16] = sacc;
     }
@@ -1108,8 +1171,8 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
       float lg = -INFINITY;   // lanes < ncls: this image's logits
       if (lane < ncls) {
         lg = fcb ? fcb[lane] : 0.f;
-#pragma unroll 5
-        for (int wi = 0; wi < kL1Warps; ++wi) lg += s_part[wi * 16 + lane];
+#pragma unroll
+        for (int wi = 0; wi < kFwdWarps; ++wi) lg += s_part[wi * 16 + lane];
         logits[static_cast<size_t>(n) * ncls + lane] = lg;
       }
       trace(0, 9);
@@ -1575,18 +1638,18 @@ void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const 
   if (!(ce.scale > 0.f)) throw std::invalid_argument("convnet_fwd: the cross-entropy scale must be positive");
   if (!(ce.smoothing >= 0.f && ce.smoothing <= 1.f)) throw std::invalid_argument("convnet_fwd: label smoothing must lie in [0, 1]");
   if (ce.target != nullptr && !ce.is_default(ncls)) {
-    launch_cooperative(convnet_fwd_kernel<SmoothCe>, B, kL1Threads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1,
+    launch_cooperative(convnet_fwd_kernel<SmoothCe>, B, kFwdThreads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1,
                        saved1, rm1, rv1, nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials,
                        gs, ce);
     return;
   }
   if (ce.target != nullptr && ce.scale != 1.f) {
-    launch_cooperative(convnet_fwd_kernel<ScaledCe>, B, kL1Threads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1,
+    launch_cooperative(convnet_fwd_kernel<ScaledCe>, B, kFwdThreads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1,
                        saved1, rm1, rv1, nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials,
                        gs, static_cast<const ScaledCe&>(ce));
     return;
   }
-  launch_cooperative(convnet_fwd_kernel<FusedCe>, B, kL1Threads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1, saved1,
+  launch_cooperative(convnet_fwd_kernel<FusedCe>, B, kFwdThreads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1, saved1,
                      rm1, rv1, nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials, gs,
                      static_cast<const FusedCe&>(ce));
 }

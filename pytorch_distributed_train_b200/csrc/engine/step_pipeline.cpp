@@ -6,6 +6,22 @@
 
 namespace pdt {
 
+namespace {
+// dst.copy_(src, non_blocking) on `stream`.  A device-resident source of the same dtype and layout is one cudaMemcpyAsync: the
+// dispatcher's copy_ costs microseconds of host time per tensor, and a replayed step's device time is not much larger than the
+// host time of the loop that feeds it — every microsecond the host saves is lead it keeps over the device through a host stall.
+// Anything else (pinned host sources above all, which must stay registered with the caching host allocator) goes through copy_.
+void stage_copy(const at::Tensor& dst, const at::Tensor& src, c10::cuda::CUDAStream stream) {
+  if (src.is_cuda() && dst.is_cuda() && src.get_device() == dst.get_device() && src.scalar_type() == dst.scalar_type() &&
+      src.numel() == dst.numel() && src.is_contiguous() && dst.is_contiguous()) {
+    C10_CUDA_CHECK(cudaMemcpyAsync(dst.data_ptr(), src.data_ptr(), src.nbytes(), cudaMemcpyDeviceToDevice, stream.stream()));
+    return;
+  }
+  c10::cuda::CUDAStreamGuard sg(stream);
+  dst.copy_(src, /*non_blocking=*/true);
+}
+}  // namespace
+
 StepPipeline::StepPipeline(int device, int num_sets, at::ScalarType loss_dtype)
     : device_(device),
       copy_(c10::cuda::getStreamFromPool(/*isHighPriority=*/false, device)),
@@ -39,14 +55,11 @@ void StepPipeline::stage_inputs(int i, const std::vector<at::Tensor>& dst, const
         src_ready_.block(copy_);
       }
     }
-    {
-      c10::cuda::CUDAStreamGuard sg(copy_);
-      for (size_t k = 0; k < dst.size(); ++k) dst[k].copy_(src[k], /*non_blocking=*/true);
-    }
+    for (size_t k = 0; k < dst.size(); ++k) stage_copy(dst[k], src[k], copy_);
     ready_[i]->record(copy_);
     ready_[i]->block(cur);
   } else {
-    for (size_t k = 0; k < dst.size(); ++k) dst[k].copy_(src[k], /*non_blocking=*/true);
+    for (size_t k = 0; k < dst.size(); ++k) stage_copy(dst[k], src[k], cur);
   }
   if (loss_read_[i] != nullptr) {   // loss_to_host() of this graph's previous replay has read the loss buffer
     loss_read_[i]->block(cur);

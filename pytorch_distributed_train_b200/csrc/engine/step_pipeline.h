@@ -8,7 +8,8 @@
 //   copy stream : wait done[i] (the replay that last read set i) → copy batch → record ready[i]
 //   step stream : wait ready[i] → wait loss_read[i] (the previous loss of graph i has left the device) → replay → record done[i]
 //   d2h stream  : wait (event recorded on the step stream after the replay) → copy loss → record slot event
-// Copies go through at::Tensor::copy_, so pinned sources stay registered with the caching host allocator.
+// Host sources are copied through at::Tensor::copy_, so pinned sources stay registered with the caching host allocator; a
+// device-resident source of the destination's dtype and layout is one cudaMemcpyAsync.
 #pragma once
 #include <ATen/ATen.h>
 #include <ATen/cuda/CUDAEvent.h>

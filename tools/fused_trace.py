@@ -31,8 +31,9 @@ with OF.upcoming_targets(y):
 crit(out, y).backward()
 t = _C.fused_convnet_trace_read()[:, :B, :].double()
 _C.fused_convnet_trace_enable(False)
-names = {0: ("forward (whole)", ["start", "conv1 done", "stats partial written", "barrier 1 passed", "pooled patch in smem", "conv2 epilogue done",
-                                 "stats 2 partial written", "barrier 2 passed", "pooled 2 in smem", "logits written", "end (incl. loss)", "prologue done (smem zeroed, weights requested)"]),
+names = {0: ("forward (whole)", ["start", "conv1 done", "stats partial written", "barrier 1 passed", "pooled patch in smem",
+                                 "conv2 done (ys + stats 2 in smem)", "stats 2 partial written", "barrier 2 passed", "pooled 2 in smem",
+                                 "logits written", "end (incl. loss)", "prologue done (halo zeroed, weights requested)"]),
          1: ("l1_bwd (+conv2 wgrad fold)", ["start", "partial written", "barrier passed", "folded", "conv1 wgrad partial written", "barrier 2 passed",
                                             "end", "dW2 folded"]),
          3: ("l2_bwd (+conv2 wgrad partials)", ["start", "B built", "partial written", "barrier passed", "folded", "dy written", "end",
