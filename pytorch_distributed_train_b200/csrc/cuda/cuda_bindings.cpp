@@ -42,6 +42,86 @@ float* opt_mut(c10::optional<at::Tensor>& t, const char* name) {
   return t->data_ptr<float>();
 }
 
+// The hyper-parameters of sgd_multi and of the SGD rider of convnet_l1_bwd_wgrad.
+SgdHyper sgd_hyper(double lr, const c10::optional<at::Tensor>& lr_tensor, double momentum, double dampening, double weight_decay, bool nesterov,
+                   bool maximize, bool first_step) {
+  return SgdHyper{static_cast<float>(lr), static_cast<float>(momentum), static_cast<float>(dampening), static_cast<float>(weight_decay),
+                  nesterov ? 1 : 0, maximize ? 1 : 0, first_step ? 1 : 0, opt_ptr(lr_tensor, "lr_tensor")};
+}
+// The hyper-parameters of adam_multi and of the Adam rider of convnet_l1_bwd_wgrad.
+AdamHyper adam_hyper(double lr, const c10::optional<at::Tensor>& lr_tensor, double beta1, double beta2, double eps, double weight_decay,
+                     bool decoupled, bool maximize) {
+  return AdamHyper{lr, beta1, beta2, static_cast<float>(eps), static_cast<float>(weight_decay), decoupled ? 1 : 0, maximize ? 1 : 0,
+                   opt_ptr(lr_tensor, "lr_tensor")};
+}
+
+using TensorList = std::vector<c10::optional<at::Tensor>>;
+TensorList tensors(const py::dict& d, const char* key) { return d[key].cast<TensorList>(); }
+
+// The parameters of a rider description (dict: "params", the ten parameters in the order conv1.w, conv1.b, bn1.w, bn1.b, conv2.w,
+// conv2.b, fc.w, fc.b, bn2.w, bn2.b, entries may be None; "prev_grads", the gradients of the last four) into r; state(k, param)
+// fills the optimizer state of parameter k.
+template <class R, class State>
+void fill_rider(R& r, const py::dict& d, const char* kind, State state) {
+  static const int64_t want[10] = {400, 16, 16, 16, 12800, 32, -1, -1, 32, 32};
+  const TensorList params = tensors(d, "params"), prev = tensors(d, "prev_grads");
+  TORCH_CHECK(params.size() == 10 && prev.size() == 4, "convnet_l1_bwd_wgrad: ", kind, " lists have the wrong length");
+  for (int k = 0; k < 10; ++k) {
+    if (!params[k].has_value() || !params[k]->defined()) continue;
+    const at::Tensor& p = *params[k];
+    chk(p, "rider param");
+    TORCH_CHECK(want[k] < 0 || p.numel() == want[k], "convnet_l1_bwd_wgrad: ", kind, " parameter ", k, " has the wrong size");
+    r.p[k] = p.data_ptr<float>();
+    state(k, p);
+    if (k >= 6) {
+      TORCH_CHECK(prev[k - 6].has_value() && prev[k - 6]->numel() == p.numel(), "convnet_l1_bwd_wgrad: gradient of ", kind, " parameter ", k, " missing");
+      chk(*prev[k - 6], "rider gradient");
+      r.g_prev[k - 6] = prev[k - 6]->data_ptr<float>();
+      r.n_prev[k - 6] = static_cast<int>(p.numel());
+    }
+  }
+  TORCH_CHECK(r.p[0] && r.p[4], "convnet_l1_bwd_wgrad: the convolution weights must take part in the fused update");
+  r.on = 1;
+}
+
+// {"kind": "sgd", "params", "prev_grads", "momentum_buffer" (ten, or empty when momentum == 0), "lr", "lr_tensor", "momentum",
+// "dampening", "weight_decay", "nesterov", "maximize", "first_step"}
+SgdRider sgd_rider(const py::dict& d) {
+  SgdRider r;
+  const double momentum = d["momentum"].cast<double>();
+  const TensorList bufs = tensors(d, "momentum_buffer");
+  TORCH_CHECK(bufs.empty() || bufs.size() == 10, "convnet_l1_bwd_wgrad: sgd lists have the wrong length");
+  fill_rider(r, d, "sgd", [&](int k, const at::Tensor& p) {
+    if (momentum == 0.0) return;
+    TORCH_CHECK(!bufs.empty() && bufs[k].has_value() && bufs[k]->numel() == p.numel(), "convnet_l1_bwd_wgrad: momentum buffer ", k, " missing");
+    chk(*bufs[k], "momentum buffer");
+    r.m[k] = bufs[k]->data_ptr<float>();
+  });
+  r.h = sgd_hyper(d["lr"].cast<double>(), d["lr_tensor"].cast<c10::optional<at::Tensor>>(), momentum, d["dampening"].cast<double>(),
+                  d["weight_decay"].cast<double>(), d["nesterov"].cast<bool>(), d["maximize"].cast<bool>(), d["first_step"].cast<bool>());
+  return r;
+}
+
+// {"kind": "adam", "params", "prev_grads", "exp_avg", "exp_avg_sq", "step" (fp32 scalars on the device), "lr", "lr_tensor", "beta1",
+// "beta2", "eps", "weight_decay", "decoupled", "maximize"}
+AdamRider adam_rider(const py::dict& d) {
+  AdamRider r;
+  const TensorList ms = tensors(d, "exp_avg"), vs = tensors(d, "exp_avg_sq"), steps = tensors(d, "step");
+  TORCH_CHECK(ms.size() == 10 && vs.size() == 10 && steps.size() == 10, "convnet_l1_bwd_wgrad: adam lists have the wrong length");
+  fill_rider(r, d, "adam", [&](int k, const at::Tensor& p) {
+    TORCH_CHECK(ms[k].has_value() && vs[k].has_value() && steps[k].has_value(), "convnet_l1_bwd_wgrad: adam state of parameter ", k, " missing");
+    chk(*ms[k], "exp_avg"); chk(*vs[k], "exp_avg_sq"); chk(*steps[k], "step");
+    TORCH_CHECK(ms[k]->numel() == p.numel() && vs[k]->numel() == p.numel() && steps[k]->numel() == 1, "convnet_l1_bwd_wgrad: adam state of parameter ",
+                k, " has the wrong size");
+    r.m[k] = ms[k]->data_ptr<float>();
+    r.v[k] = vs[k]->data_ptr<float>();
+    r.step[k] = steps[k]->data_ptr<float>();
+  });
+  r.h = adam_hyper(d["lr"].cast<double>(), d["lr_tensor"].cast<c10::optional<at::Tensor>>(), d["beta1"].cast<double>(), d["beta2"].cast<double>(),
+                   d["eps"].cast<double>(), d["weight_decay"].cast<double>(), d["decoupled"].cast<bool>(), d["maximize"].cast<bool>());
+  return r;
+}
+
 // torch's cross-entropy options for C classes of logits on `like`'s device
 CeSpec ce_spec(const c10::optional<at::Tensor>& weight, int64_t ignore_index, double label_smoothing, const std::string& reduction, int64_t C,
                const at::Tensor& like, const char* who) {
@@ -344,7 +424,8 @@ void register_cuda_bindings(py::module_& m) {
   m.def("convnet_l1_bwd_wgrad", [](const at::Tensor& dp, const at::Tensor& y, const at::Tensor& x, const at::Tensor& saved,
                                    c10::optional<at::Tensor> gamma, c10::optional<at::Tensor> beta, at::Tensor dgamma, at::Tensor dbeta, at::Tensor dw,
                                    c10::optional<at::Tensor> db, c10::optional<at::Tensor> dy2_pad, c10::optional<at::Tensor> x2_pad,
-                                   const at::Tensor& dysum2, at::Tensor dw2, c10::optional<at::Tensor> db2, py::object sgd, bool accumulate) {
+                                   const at::Tensor& dysum2, at::Tensor dw2, c10::optional<at::Tensor> db2, py::object rider, py::object clip,
+                                   bool accumulate) {
     chk(dp, "dp"); chk(y, "y"); chk(x, "x"); chk(saved, "saved"); chk(dgamma, "dgamma"); chk(dbeta, "dbeta"); chk(dw, "dw");
     chk(dysum2, "dysum2"); chk(dw2, "dw2");
     c10::cuda::CUDAGuard g(x.device());
@@ -366,14 +447,10 @@ void register_cuda_bindings(py::module_& m) {
       TORCH_CHECK(entry.wgrad_batch == B, "convnet_l1_bwd_wgrad: without dy2_pad / x2_pad it folds the partials of convnet_l2_bwd_fc(…, p1) "
                   "of the same batch, and none are pending");
     }
-    // sgd = (params[10], prev_grads[4], momentum_bufs[10] or [], lr, lr_tensor, momentum, dampening, weight_decay, nesterov, maximize, first_step):
-    // parameters in the order conv1.w, conv1.b, bn1.w, bn1.b, conv2.w, conv2.b, fc.w, fc.b, bn2.w, bn2.b (entries may be None)
-    // or the Adam rider: ("adam", params[10], prev_grads[4], exp_avgs[10], exp_avg_sqs[10], steps[10], lr, lr_tensor, beta1, beta2,
-    // eps, weight_decay, decoupled, maximize), steps being fp32 scalars on the device.  Either tuple may end in a clip entry
-    // (max_norm, norm_type 2 or inf, norm_out): gradient-norm clipping in front of the update (ClipRider); norm_out receives the norm.
-    // accumulate: gradient accumulation — dgamma, dbeta, dw, db, dw2, db2 are added to (they hold the earlier micro-batches' sum), and
-    // the rider updates with the accumulated gradients.
-    static const int64_t want[10] = {400, 16, 16, 16, 12800, 32, -1, -1, 32, 32};
+    // rider: the optimizer update riding on the kernel, a description with named entries (sgd_rider / adam_rider above), or None.
+    // clip = (max_norm, norm_type 2 or inf, norm_out): gradient-norm clipping in front of the update (ClipRider); norm_out receives the
+    // norm.  accumulate: gradient accumulation — dgamma, dbeta, dw, db, dw2, db2 are added to (they hold the earlier micro-batches' sum),
+    // and the rider updates with the accumulated gradients.
     ReduceScratch scr = scratch(x);
     const size_t l1_floats = static_cast<size_t>(B) * (64 + 512);
     TORCH_CHECK(static_cast<long long>(l1_floats) + B <= scr.capacity_floats, "convnet_l1_bwd_wgrad: scratch too small");
@@ -385,9 +462,10 @@ void register_cuda_bindings(py::module_& m) {
                                   scr.partials + static_cast<size_t>(B) * 64, grid_sync(scr), cur_stream(x), rider, accumulate);
       entry.wgrad_batch = 0;
     };
-    // the clip entry of a rider tuple → the clipping variant of the rider
-    auto clipped = [&](auto base, const py::handle& entry) {
-      auto c = entry.cast<py::tuple>();
+    // the rider with clipping → its clipping variant
+    auto launch_rider = [&](auto base) {
+      if (clip.is_none()) return launch(base);
+      auto c = clip.cast<py::tuple>();
       TORCH_CHECK(c.size() == 3, "convnet_l1_bwd_wgrad: clip entry (max_norm, norm_type, norm_out) expected");
       const double norm_type = c[1].cast<double>();
       TORCH_CHECK(norm_type == 2.0 || (std::isinf(norm_type) && norm_type > 0), "convnet_l1_bwd_wgrad: clip norm_type must be 2 or inf");
@@ -400,96 +478,20 @@ void register_cuda_bindings(py::module_& m) {
       r.norm_inf = std::isinf(norm_type) ? 1 : 0;
       r.norm_out = out.data_ptr<float>();
       r.part = scr.partials + l1_floats;
-      return r;
+      launch(r);
     };
-    if (!sgd.is_none() && py::isinstance<py::tuple>(sgd) && py::len(sgd) > 0 && py::isinstance<py::str>(sgd.cast<py::tuple>()[0])) {
-      auto t = sgd.cast<py::tuple>();
-      TORCH_CHECK((t.size() == 14 || t.size() == 15) && t[0].cast<std::string>() == "adam", "convnet_l1_bwd_wgrad: adam tuple of 14 or 15 entries expected");
-      auto params = t[1].cast<std::vector<c10::optional<at::Tensor>>>();
-      auto prev = t[2].cast<std::vector<c10::optional<at::Tensor>>>();
-      auto ms = t[3].cast<std::vector<c10::optional<at::Tensor>>>();
-      auto vs = t[4].cast<std::vector<c10::optional<at::Tensor>>>();
-      auto steps = t[5].cast<std::vector<c10::optional<at::Tensor>>>();
-      TORCH_CHECK(params.size() == 10 && prev.size() == 4 && ms.size() == 10 && vs.size() == 10 && steps.size() == 10,
-                  "convnet_l1_bwd_wgrad: adam lists have the wrong length");
-      AdamRider rider;
-      for (int k = 0; k < 10; ++k) {
-        if (!params[k].has_value() || !params[k]->defined()) continue;
-        chk(*params[k], "adam param");
-        const int64_t numel = params[k]->numel();
-        TORCH_CHECK(want[k] < 0 || numel == want[k], "convnet_l1_bwd_wgrad: adam parameter ", k, " has the wrong size");
-        TORCH_CHECK(ms[k].has_value() && vs[k].has_value() && steps[k].has_value(), "convnet_l1_bwd_wgrad: adam state of parameter ", k, " missing");
-        chk(*ms[k], "exp_avg"); chk(*vs[k], "exp_avg_sq"); chk(*steps[k], "step");
-        TORCH_CHECK(ms[k]->numel() == numel && vs[k]->numel() == numel && steps[k]->numel() == 1, "convnet_l1_bwd_wgrad: adam state of parameter ", k,
-                    " has the wrong size");
-        rider.p[k] = params[k]->data_ptr<float>();
-        rider.m[k] = ms[k]->data_ptr<float>();
-        rider.v[k] = vs[k]->data_ptr<float>();
-        rider.step[k] = steps[k]->data_ptr<float>();
-        if (k >= 6) {
-          TORCH_CHECK(prev[k - 6].has_value() && prev[k - 6]->numel() == numel, "convnet_l1_bwd_wgrad: gradient of adam parameter ", k, " missing");
-          chk(*prev[k - 6], "adam gradient");
-          rider.g_prev[k - 6] = prev[k - 6]->data_ptr<float>();
-          rider.n_prev[k - 6] = static_cast<int>(numel);
-        }
-      }
-      TORCH_CHECK(rider.p[0] && rider.p[4], "convnet_l1_bwd_wgrad: the convolution weights must take part in the fused update");
-      rider.h = AdamHyper{t[6].cast<double>(), t[8].cast<double>(), t[9].cast<double>(), static_cast<float>(t[10].cast<double>()),
-                          static_cast<float>(t[11].cast<double>()), t[12].cast<bool>() ? 1 : 0, t[13].cast<bool>() ? 1 : 0, nullptr};
-      if (!t[7].is_none()) {
-        at::Tensor lrt = t[7].cast<at::Tensor>();
-        chk(lrt, "lr_tensor");
-        rider.h.lr_dev = lrt.data_ptr<float>();
-      }
-      rider.on = 1;
-      if (t.size() == 15) launch(clipped(rider, t[14]));
-      else launch(rider);
-      return;
+    if (rider.is_none()) {
+      TORCH_CHECK(clip.is_none(), "convnet_l1_bwd_wgrad: clip needs a rider");
+      return launch(SgdRider{});
     }
-    SgdRider rider;
-    if (!sgd.is_none()) {
-      auto t = sgd.cast<py::tuple>();
-      TORCH_CHECK(t.size() == 11 || t.size() == 12, "convnet_l1_bwd_wgrad: sgd tuple of 11 or 12 entries expected");
-      auto params = t[0].cast<std::vector<c10::optional<at::Tensor>>>();
-      auto prev = t[1].cast<std::vector<c10::optional<at::Tensor>>>();
-      auto bufs = t[2].cast<std::vector<c10::optional<at::Tensor>>>();
-      TORCH_CHECK(params.size() == 10 && prev.size() == 4 && (bufs.empty() || bufs.size() == 10), "convnet_l1_bwd_wgrad: sgd lists have the wrong length");
-      const double momentum = t[5].cast<double>();
-      for (int k = 0; k < 10; ++k) {
-        if (!params[k].has_value() || !params[k]->defined()) continue;
-        chk(*params[k], "sgd param");
-        TORCH_CHECK(want[k] < 0 || params[k]->numel() == want[k], "convnet_l1_bwd_wgrad: sgd parameter ", k, " has the wrong size");
-        rider.p[k] = params[k]->data_ptr<float>();
-        if (momentum != 0.0) {
-          TORCH_CHECK(!bufs.empty() && bufs[k].has_value() && bufs[k]->numel() == params[k]->numel(), "convnet_l1_bwd_wgrad: momentum buffer ", k, " missing");
-          chk(*bufs[k], "momentum buffer");
-          rider.m[k] = bufs[k]->data_ptr<float>();
-        }
-        if (k >= 6) {
-          TORCH_CHECK(prev[k - 6].has_value() && prev[k - 6]->numel() == params[k]->numel(), "convnet_l1_bwd_wgrad: gradient of sgd parameter ", k, " missing");
-          chk(*prev[k - 6], "sgd gradient");
-          rider.g_prev[k - 6] = prev[k - 6]->data_ptr<float>();
-          rider.n_prev[k - 6] = static_cast<int>(params[k]->numel());
-        }
-      }
-      TORCH_CHECK(rider.p[0] && rider.p[4], "convnet_l1_bwd_wgrad: the convolution weights must take part in the fused update");
-      rider.h = SgdHyper{static_cast<float>(t[3].cast<double>()), static_cast<float>(momentum), static_cast<float>(t[6].cast<double>()),
-                         static_cast<float>(t[7].cast<double>()), t[8].cast<bool>() ? 1 : 0, t[9].cast<bool>() ? 1 : 0, t[10].cast<bool>() ? 1 : 0, nullptr};
-      if (!t[4].is_none()) {
-        at::Tensor lrt = t[4].cast<at::Tensor>();
-        chk(lrt, "lr_tensor");
-        rider.h.lr_dev = lrt.data_ptr<float>();
-      }
-      rider.on = 1;
-      if (t.size() == 12) {
-        launch(clipped(rider, t[11]));
-        return;
-      }
-    }
-    launch(rider);
+    const auto d = rider.cast<py::dict>();
+    const auto kind = d["kind"].cast<std::string>();
+    TORCH_CHECK(kind == "sgd" || kind == "adam", "convnet_l1_bwd_wgrad: rider kind must be 'sgd' or 'adam' (got '", kind, "')");
+    if (kind == "adam") launch_rider(adam_rider(d));
+    else launch_rider(sgd_rider(d));
   }, py::arg("dp"), py::arg("y"), py::arg("x"), py::arg("saved"), py::arg("gamma"), py::arg("beta"), py::arg("dgamma"), py::arg("dbeta"),
      py::arg("dw"), py::arg("db"), py::arg("dy2_pad"), py::arg("x2_pad"), py::arg("dysum2"), py::arg("dw2"), py::arg("db2"),
-     py::arg("sgd") = py::none(), py::arg("accumulate") = false);
+     py::arg("rider") = py::none(), py::kw_only(), py::arg("clip") = py::none(), py::arg("accumulate") = false);
   m.def("convnet_fwd", [](const at::Tensor& x, const at::Tensor& w1, c10::optional<at::Tensor> b1, c10::optional<at::Tensor> g1,
                           c10::optional<at::Tensor> be1, c10::optional<at::Tensor> rm1, c10::optional<at::Tensor> rv1, c10::optional<at::Tensor> nbt1,
                           double mom1, double eps1, const at::Tensor& w2, c10::optional<at::Tensor> b2, c10::optional<at::Tensor> g2,
@@ -744,9 +746,7 @@ void register_cuda_bindings(py::module_& m) {
     TORCH_CHECK(momentum == 0.0 || bufs.size() == params.size(), "sgd_multi: momentum buffers required");
     if (params.empty()) return;
     c10::cuda::CUDAGuard g(params[0].device());
-    SgdHyper h{static_cast<float>(lr), static_cast<float>(momentum), static_cast<float>(dampening), static_cast<float>(weight_decay),
-               nesterov ? 1 : 0, maximize ? 1 : 0, first_step ? 1 : 0, nullptr};
-    if (lr_tensor.has_value() && lr_tensor->defined()) { chk(*lr_tensor, "lr_tensor"); h.lr_dev = lr_tensor->data_ptr<float>(); }
+    const SgdHyper h = sgd_hyper(lr, lr_tensor, momentum, dampening, weight_decay, nesterov, maximize, first_step);
     cudaStream_t st = cur_stream(params[0]);
     for (size_t base = 0; base < params.size(); base += SgdTensorList::kMax) {
       SgdTensorList tl;
@@ -771,8 +771,7 @@ void register_cuda_bindings(py::module_& m) {
     TORCH_CHECK(grads.size() == n && exp_avgs.size() == n && exp_avg_sqs.size() == n && steps.size() == n, "adam_multi: list lengths differ");
     if (n == 0) return;
     c10::cuda::CUDAGuard g(params[0].device());
-    AdamHyper h{lr, beta1, beta2, static_cast<float>(eps), static_cast<float>(weight_decay), decoupled ? 1 : 0, maximize ? 1 : 0, nullptr};
-    if (lr_tensor.has_value() && lr_tensor->defined()) { chk(*lr_tensor, "lr_tensor"); h.lr_dev = lr_tensor->data_ptr<float>(); }
+    const AdamHyper h = adam_hyper(lr, lr_tensor, beta1, beta2, eps, weight_decay, decoupled, maximize);
     cudaStream_t st = cur_stream(params[0]);
     // the ticket word of the step hand-over (adam_multi_kernel); launches on one device are ordered by the compute stream, and
     // every launch leaves the word at zero

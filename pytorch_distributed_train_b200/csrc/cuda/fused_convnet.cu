@@ -363,6 +363,20 @@ __device__ __forceinline__ float clip_acc(const R& r, float acc, float g) { retu
 template <class R>
 __device__ __forceinline__ float clip_comb(const R& r, float a, float b) { return r.norm_inf ? nan_max(a, b) : a + b; }
 
+template <class R>
+constexpr bool kClipRider = std::is_same_v<R, ClipRider<SgdRider>> || std::is_same_v<R, ClipRider<AdamRider>>;
+template <class R>
+constexpr bool kAdamRider = std::is_same_v<R, AdamRider> || std::is_same_v<R, ClipRider<AdamRider>>;
+
+// Element i of parameter k's gradient is final with value g: a ClipRider adds it to this thread's share ca of the norm (the update
+// waits for the coefficient), the others apply their update.  The caller tests whether the rider is on and the parameter takes part.
+template <class Rider>
+__device__ __forceinline__ void ride(const Rider& sr, float& ca, int k, int i, float g, const float* adam_f, float sgd_lr) {
+  if constexpr (kClipRider<Rider>) ca = clip_acc(sr, ca, g);
+  else if constexpr (kAdamRider<Rider>) adam_apply(sr, k, i, g, adam_f);
+  else sgd_apply(sr.p[k] + i, g, sr.m[k] ? sr.m[k] + i : nullptr, sr.h, sgd_lr);
+}
+
 // ACC (accumulate mode, gradient accumulation over micro-batches): every gradient this kernel writes — dgamma, dbeta, the conv1 fold
 // dw / db and the conv2 fold dw2 / db2 — becomes g = g_old + v, and the rider updates with (and clips) that accumulated value.
 template <class Rider = SgdRider, bool ACC = false>
@@ -372,8 +386,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
                       float* partials, float* partials_w, GridSync gs,
                       // conv2's weight gradient, folded from the per-image partials [B][400][32] and Σdy rows [B][32]
                       const float* __restrict__ wpart, const float* __restrict__ dysum2, float* dw2, float* db2, const __grid_constant__ Rider sr) {
-  constexpr bool kClip = std::is_same_v<Rider, ClipRider<SgdRider>> || std::is_same_v<Rider, ClipRider<AdamRider>>;
-  constexpr bool kAdam = std::is_same_v<Rider, AdamRider> || std::is_same_v<Rider, ClipRider<AdamRider>>;
+  constexpr bool kClip = kClipRider<Rider>, kAdam = kAdamRider<Rider>;
   static_assert(kAdam || std::is_base_of_v<SgdRider, Rider>, "convnet_l1_bwd_kernel: SgdRider or AdamRider, or either in a ClipRider");
   extern __shared__ __align__(16) float dsm[];
   float* dys = dsm;                  // [784][16]
@@ -459,24 +472,15 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   }
   trace(1, 1);
   bar.arrive(gs);
-  // (each update below is spelled out for both riders: the SGD instantiation keeps the code it had before the Adam rider existed)
   const float sgd_lr = sr.on ? (sr.h.lr_dev ? __ldg(sr.h.lr_dev) : static_cast<float>(sr.h.lr)) : 0.f;
   float ca = 0.f;   // ClipRider: this thread's share of the gradient norm
-  if constexpr (kClip) {
-    // in the barrier's shadow: the norm partial of the parameters whose gradients were complete before this kernel started
-    // (classifier, bn2, and below conv2); their update waits for the coefficient
+  if (kClip || sr.on) {   // (a ClipRider is only made around a rider that is on)
+    // in the barrier's shadow: the parameters whose gradients were complete before this kernel started (classifier, bn2, and
+    // below conv2) — nothing in this kernel reads them
 #pragma unroll
     for (int t = 0; t < 4; ++t)
-      if (sr.p[6 + t])
-        for (int i = n * kL1Threads + tid; i < sr.n_prev[t]; i += B * kL1Threads) ca = clip_acc(sr, ca, __ldg(sr.g_prev[t] + i));
-  } else if (sr.on) {
-    // in the barrier's shadow: the optimizer step of the parameters whose gradients were complete before this kernel started
-    // (classifier, bn2) — nothing in this kernel reads them
-#pragma unroll
-    for (int t = 0; t < 4; ++t)
-      for (int i = n * kL1Threads + tid; i < sr.n_prev[t]; i += B * kL1Threads)
-        if constexpr (kAdam) adam_apply(sr, 6 + t, i, __ldg(sr.g_prev[t] + i), adam_f);
-        else sgd_apply(sr.p[6 + t] + i, __ldg(sr.g_prev[t] + i), sr.m[6 + t] ? sr.m[6 + t] + i : nullptr, sr.h, sgd_lr);
+      if (!kClip || sr.p[6 + t])
+        for (int i = n * kL1Threads + tid; i < sr.n_prev[t]; i += B * kL1Threads) ride(sr, ca, 6 + t, i, __ldg(sr.g_prev[t] + i), adam_f, sgd_lr);
   }
   {
     // in the barrier's shadow: conv2's weight gradient, complete before this kernel started (the layer-2 backward kernel wrote the
@@ -531,15 +535,11 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
             const int e = (lane * 16 + (i & 15)) * 25 + (i >> 4);
             if constexpr (ACC) tot = dw2[e] + tot;
             dw2[e] = tot;
-            if constexpr (kClip) ca = clip_acc(sr, ca, tot);
-            else if constexpr (kAdam) { if (sr.on) adam_apply(sr, 4, e, tot, adam_f); }
-            else if (sr.on) sgd_apply(sr.p[4] + e, tot, sr.m[4] ? sr.m[4] + e : nullptr, sr.h, sgd_lr);
+            if (kClip || sr.on) ride(sr, ca, 4, e, tot, adam_f, sgd_lr);
           } else if (db2) {
             if constexpr (ACC) tot = db2[lane] + tot;
             db2[lane] = tot;
-            if constexpr (kClip) { if (sr.p[5]) ca = clip_acc(sr, ca, tot); }
-            else if constexpr (kAdam) { if (sr.on && sr.p[5]) adam_apply(sr, 5, lane, tot, adam_f); }
-            else if (sr.on && sr.p[5]) sgd_apply(sr.p[5] + lane, tot, sr.m[5] ? sr.m[5] + lane : nullptr, sr.h, sgd_lr);
+            if ((kClip || sr.on) && sr.p[5]) ride(sr, ca, 5, lane, tot, adam_f, sgd_lr);
           }
         }
       }
@@ -659,50 +659,21 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
       if (tap < 25) {
         if constexpr (ACC) s = dw[co * 25 + tap] + s;
         dw[co * 25 + tap] = s;
-        if constexpr (kClip) ca = clip_acc(sr, ca, s);
-        else if constexpr (kAdam) { if (sr.on) adam_apply(sr, 0, co * 25 + tap, s, adam_f); }
-        else if (sr.on) sgd_apply(sr.p[0] + co * 25 + tap, s, sr.m[0] ? sr.m[0] + co * 25 + tap : nullptr, sr.h, sgd_lr);
+        if (kClip || sr.on) ride(sr, ca, 0, co * 25 + tap, s, adam_f, sgd_lr);
       } else if (db) {
         if constexpr (ACC) s = db[co] + s;
         db[co] = s;
-        if constexpr (kClip) { if (sr.p[1]) ca = clip_acc(sr, ca, s); }
-        else if constexpr (kAdam) { if (sr.on && sr.p[1]) adam_apply(sr, 1, co, s, adam_f); }
-        else if (sr.on && sr.p[1]) sgd_apply(sr.p[1] + co, s, sr.m[1] ? sr.m[1] + co : nullptr, sr.h, sgd_lr);
+        if ((kClip || sr.on) && sr.p[1]) ride(sr, ca, 1, co, s, adam_f, sgd_lr);
       }
     }
   }
   if (sr.on && n == 0 && tid < 16) {
-    // BatchNorm-1 affine parameters: their gradients are the totals this CTA folded after the first barrier.  Every CTA read
-    // gamma / beta before that barrier, so updating them here (after the second one) races with nobody.
-    if constexpr (ACC) {
-      // accumulate mode: the gradients are what this thread wrote above (batch sums added to the earlier micro-batches')
-      const float gbeta = dbeta ? dbeta[tid] : 0.f, ggamma = dgamma ? dgamma[tid] : 0.f;
-      if constexpr (kClip) {
-        if (sr.p[3]) ca = clip_acc(sr, ca, gbeta);
-        if (sr.p[2]) ca = clip_acc(sr, ca, ggamma);
-      } else if constexpr (kAdam) {
-        if (sr.p[3]) adam_apply(sr, 3, tid, gbeta, adam_f);
-        if (sr.p[2]) adam_apply(sr, 2, tid, ggamma, adam_f);
-      } else {
-        if (sr.p[3]) sgd_apply(sr.p[3] + tid, gbeta, sr.m[3] ? sr.m[3] + tid : nullptr, sr.h, sgd_lr);
-        if (sr.p[2]) sgd_apply(sr.p[2] + tid, ggamma, sr.m[2] ? sr.m[2] + tid : nullptr, sr.h, sgd_lr);
-      }
-    } else if constexpr (kClip) {
-      if (sr.p[3]) ca = clip_acc(sr, ca, s_tot[tid]);
-      if (sr.p[2]) ca = clip_acc(sr, ca, s_tot[16 + tid]);
-    } else if constexpr (kAdam) {
-      if (sr.p[3]) adam_apply(sr, 3, tid, s_tot[tid], adam_f);
-      if (sr.p[2]) adam_apply(sr, 2, tid, s_tot[16 + tid], adam_f);
-    } else {
-      if (sr.p[3]) sgd_apply(sr.p[3] + tid, s_tot[tid], sr.m[3] ? sr.m[3] + tid : nullptr, sr.h, sgd_lr);
-      if (sr.p[2]) sgd_apply(sr.p[2] + tid, s_tot[16 + tid], sr.m[2] ? sr.m[2] + tid : nullptr, sr.h, sgd_lr);
-    }
-  }
-  if constexpr (kAdam && !kClip) {
-    // every CTA read the step counts before the first grid barrier and this is after the last one
-    if (sr.on && n == 0 && tid == 0)
-      for (int k = 0; k < 10; ++k)
-        if (sr.step[k]) *sr.step[k] += 1.f;
+    // BatchNorm-1 affine parameters: their gradients are the totals this CTA folded after the first barrier (in accumulate mode,
+    // what this thread wrote above: those added to the earlier micro-batches').  Every CTA read gamma / beta before that barrier,
+    // so updating them here (after the second one) races with nobody.
+    const float gbeta = ACC && dbeta ? dbeta[tid] : 0.f, ggamma = ACC && dgamma ? dgamma[tid] : 0.f;
+    if (sr.p[3]) ride(sr, ca, 3, tid, ACC ? gbeta : s_tot[tid], adam_f, sgd_lr);
+    if (sr.p[2]) ride(sr, ca, 2, tid, ACC ? ggamma : s_tot[16 + tid], adam_f, sgd_lr);
   }
   if constexpr (kClip) {
     // every gradient has been seen: one partial per CTA, one more grid barrier, then every CTA folds the B partials in the same
@@ -750,12 +721,12 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
         else sgd_apply(sr.p[k] + i, gv, sr.m[k] ? sr.m[k] + i : nullptr, sr.h, sgd_lr);
       }
     }
-    if constexpr (kAdam) {
-      // every CTA read the step counts before the first grid barrier and this is after the last one
-      if (n == 0 && tid == 0)
-        for (int k = 0; k < 10; ++k)
-          if (sr.step[k]) *sr.step[k] += 1.f;
-    }
+  }
+  if constexpr (kAdam) {
+    // every CTA read the step counts before the first grid barrier and this is after the last one
+    if ((kClip || sr.on) && n == 0 && tid == 0)
+      for (int k = 0; k < 10; ++k)
+        if (sr.step[k]) *sr.step[k] += 1.f;
   }
   bar.finish(gs);
   trace(1, 6);

@@ -116,7 +116,8 @@ class GraphedTrainStep:
         """(Re-)arm the riding update; with clipping, the rider stores the norm in the device scalar of graph k."""
         if self.max_grad_norm is None:
             return self.optimizer.ride_on_backward(self.model)
-        return self.optimizer.ride_on_backward(self.model, clip=(self.max_grad_norm, self.norm_type, self._rider_norms[k]))
+        self._rider_norm = self._rider_norms[k]
+        return self.optimizer.ride_on_backward(self.model, clip=(self.max_grad_norm, self.norm_type, self._rider_norm))
 
     def _eager_step(self, inputs=None):
         inputs = self.static_inputs if inputs is None else inputs
@@ -215,12 +216,10 @@ class GraphedTrainStep:
 
     def _finish_step(self, loss):
         """Clipping (unless the riding update did it) and the optimizer step after the backward pass(es)."""
-        from ..ops import functional as OF
-
         norm = None
         if self.max_grad_norm is not None:
             if getattr(self.optimizer, "_rode", False):
-                norm = OF._sgd_rider["clip"][2]   # the backward kernel clipped and updated
+                norm = self._rider_norm   # the backward kernel clipped and updated
             else:
                 from ..nn.utils import clip_grad_norm_
 

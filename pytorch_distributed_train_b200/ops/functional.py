@@ -256,9 +256,8 @@ def _take_accumulated(params) -> Optional[list]:
 
 
 # The optimizer whose update rides on the last backward kernel (optim.SGD / optim.Adam .ride_on_backward, armed by
-# engine.GraphedTrainStep when the gradient reduction does not already carry it, i.e. on one GPU):
-# {"kind": "sgd" | "adam", "params": [...10 parameters...], "args": callable -> the rider tuple of convnet_l1_bwd_wgrad, "owner": optimizer}
-_sgd_rider: Optional[dict] = None
+# engine.GraphedTrainStep when the gradient reduction does not already carry it, i.e. on one GPU): an optim._riding.Rider
+_sgd_rider = None
 _sgd_rider_enabled = False
 
 
@@ -328,18 +327,20 @@ class _FusedLayer1(torch.autograd.Function):
         # layer 2's kernel left conv2's per-image weight-gradient partials; this kernel folds them with its Σdy rows
         dysum2 = ctx.link.pop("dysum")
         prev = ctx.link.pop("prev")
-        sgd = None
+        desc = None
         rider = _sgd_rider if _sgd_rider_enabled else None
         if rider is not None and prev[4] and fresh:
             mine = list(params) + [q for q, _ in prev[:4]]
-            if len(mine) == len(rider["params"]) and all(a is b for a, b in zip(mine, rider["params"])):
+            if len(mine) == len(rider.params) and all(a is b for a, b in zip(mine, rider.params)):
                 # autograd has accumulated layer 2's gradients by now (AccumulateGrad runs as soon as its input is ready): they
                 # must be exactly the tensors layer 2's kernel wrote
                 grads = [q.grad if q is not None else None for q, _ in prev[:4]]
                 if all((g is None and ptr == 0) or (g is not None and g.data_ptr() == ptr) for g, (_, ptr) in zip(grads, prev[:4])):
-                    sgd = rider["args"](grads)   # None when the optimizer cannot ride this iteration
-        _C.convnet_l1_bwd_wgrad(dp.contiguous(), y, x, saved, gamma, beta, dg, dbe, dw, db, None, None, dysum2, dw2, db2, sgd,
-                                accumulate=acc is not None)
+                    desc = rider.build(grads)   # None when the optimizer cannot ride this iteration
+        _C.convnet_l1_bwd_wgrad(dp.contiguous(), y, x, saved, gamma, beta, dg, dbe, dw, db, None, None, dysum2, dw2, db2, desc,
+                                clip=rider.clip if desc is not None else None, accumulate=acc is not None)
+        if desc is not None:
+            rider.owner._rode = True
         _fused_backward_params = list(params) + [q for q, _ in prev[:4]]
         return None, dw, db, dg, dbe, None, None, None, None, None, dw2, db2, None, None
 

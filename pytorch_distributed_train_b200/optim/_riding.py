@@ -4,9 +4,21 @@ from __future__ import annotations
 
 import math
 import os
-from typing import List, Optional
+from dataclasses import dataclass
+from typing import Callable, List, Optional, Tuple
 
 import torch
+
+
+@dataclass
+class Rider:
+    """An optimizer armed to ride on the reference ConvNet's last backward kernel (``ops.functional._sgd_rider``).  ``params``: its ten
+    parameters in the kernel's order; ``clip``: ``(max_norm, norm_type, norm_out)`` or None; ``build(prev_grads)``: the rider
+    description ``convnet_l1_bwd_wgrad`` takes, or None when the optimizer cannot ride this iteration."""
+    owner: "RidingOptimizer"
+    params: List[torch.Tensor]
+    clip: Optional[Tuple[float, float, torch.Tensor]]
+    build: Callable[[list], Optional[dict]]
 
 
 class RidingOptimizer(torch.optim.Optimizer):
@@ -77,27 +89,16 @@ class RidingOptimizer(torch.optim.Optimizer):
         return (float(norm_type) in (2.0, math.inf) and isinstance(out, torch.Tensor) and out.numel() == 1
                 and out.dtype == torch.float32 and out.device == params[0].device)
 
-    def _arm_rider(self, kind: str, params, args, clip=None) -> None:
+    def _arm_rider(self, params, build, clip=None) -> None:
         from ..ops import functional as OF
 
-        if clip is not None:
-            # the rider tuple gains a trailing clip entry: the kernel clips the gradients to max_norm before the update and stores
-            # the total norm in norm_out
-            entry = (float(clip[0]), float(clip[1]), clip[2])
-            plain = args
-
-            def args(prev_grads):
-                t = plain(prev_grads)
-                return None if t is None else tuple(t) + (entry,)
-
-        self._riding_params = params
         self._rode = False
-        OF._sgd_rider = {"kind": kind, "params": params, "args": args, "owner": self, "clip": clip}
+        OF._sgd_rider = Rider(self, params, None if clip is None else (float(clip[0]), float(clip[1]), clip[2]), build)
 
     def stop_riding(self) -> None:
         """Undo :meth:`ride_on_backward`."""
         from ..ops import functional as OF
 
-        if OF._sgd_rider is not None and OF._sgd_rider.get("owner") is self:
+        if OF._sgd_rider is not None and OF._sgd_rider.owner is self:
             OF._sgd_rider = None
         self._rode = False

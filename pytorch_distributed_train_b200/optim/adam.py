@@ -112,21 +112,26 @@ class Adam(RidingOptimizer):
         if group["amsgrad"] or group["fused"] is False:
             return False
 
-        def args(prev_grads):
+        def build(prev_grads):
             g = self.param_groups[0]
             if g["amsgrad"]:
                 return None
             states = [self._state(q, False) for q in params]
             if not all(st["step"].is_cuda and st["step"].dtype == torch.float32 for st in states):
                 return None   # leave this iteration to step()
-            self._rode = True
-            beta1, beta2 = g["betas"]
-            return ("adam", params, list(prev_grads), [st["exp_avg"] for st in states], [st["exp_avg_sq"] for st in states],
-                    [st["step"] for st in states], float(g["lr"]), self._lr_tensor(0, g, params[0].device), float(beta1), float(beta2),
-                    float(g["eps"]), float(g["weight_decay"]), bool(g["decoupled_weight_decay"]), bool(g["maximize"]))
+            return dict(kind="adam", params=params, prev_grads=list(prev_grads), exp_avg=[st["exp_avg"] for st in states],
+                        exp_avg_sq=[st["exp_avg_sq"] for st in states], step=[st["step"] for st in states],
+                        **self._hyper(0, g, params[0].device))
 
-        self._arm_rider("adam", params, args, clip)
+        self._arm_rider(params, build, clip)
         return True
+
+    def _hyper(self, gi: int, group, device) -> dict:
+        """The update's hyper-parameters, as ``ops.adam_step`` and the rider description of the last backward kernel take them."""
+        beta1, beta2 = group["betas"]
+        return dict(lr=float(group["lr"]), lr_tensor=self._lr_tensor(gi, group, device), beta1=float(beta1), beta2=float(beta2),
+                    eps=float(group["eps"]), weight_decay=float(group["weight_decay"]), decoupled=bool(group["decoupled_weight_decay"]),
+                    maximize=bool(group["maximize"]))
 
     # ---- the update ---------------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -153,15 +158,12 @@ class Adam(RidingOptimizer):
                 continue
             amsgrad = group["amsgrad"]
             states = [self._state(p, amsgrad) for p in params]
-            beta1, beta2 = group["betas"]
             native = group["fused"] is not False and not amsgrad and params[0].is_cuda and ops.native_available() and all(
                 p.dtype == torch.float32 and p.is_contiguous() and g.dtype == torch.float32 and g.is_contiguous() and p.device == params[0].device
                 for p, g in zip(params, grads))
             if native:
                 ops.adam_step(params, grads, [st["exp_avg"] for st in states], [st["exp_avg_sq"] for st in states],
-                              [st["step"] for st in states], lr=group["lr"], beta1=beta1, beta2=beta2, eps=group["eps"],
-                              weight_decay=group["weight_decay"], decoupled=group["decoupled_weight_decay"], maximize=group["maximize"],
-                              lr_tensor=self._lr_tensor(gi, group, params[0].device))
+                              [st["step"] for st in states], **self._hyper(gi, group, params[0].device))
                 continue
             if group["fused"]:
                 raise RuntimeError("Adam(fused=True): the native kernel takes fp32 contiguous CUDA parameters without amsgrad")

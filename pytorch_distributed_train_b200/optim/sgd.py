@@ -60,7 +60,7 @@ class SGD(RidingOptimizer):
         if params is None or (clip is not None and not self._clip_qualifies(clip, params)):
             return False
 
-        def args(prev_grads):
+        def build(prev_grads):
             if getattr(self, "_fused_active", False):   # the reduce kernels carry the update (N >= 2)
                 return None
             g = self.param_groups[0]
@@ -76,12 +76,17 @@ class SGD(RidingOptimizer):
                     if st.get("momentum_buffer") is None:
                         st["momentum_buffer"] = torch.zeros_like(q, memory_format=torch.contiguous_format)
                     bufs.append(st["momentum_buffer"])
-            self._rode = True
-            return (params, list(prev_grads), bufs, float(g["lr"]), self._lr_tensor(0, g, params[0].device), float(g["momentum"]),
-                    float(g["dampening"]), float(g["weight_decay"]), bool(g["nesterov"]), bool(g["maximize"]), first)
+            return dict(kind="sgd", params=params, prev_grads=list(prev_grads), momentum_buffer=bufs, first_step=first,
+                        **self._hyper(0, g, params[0].device))
 
-        self._arm_rider("sgd", params, args, clip)
+        self._arm_rider(params, build, clip)
         return True
+
+    def _hyper(self, gi: int, group, device) -> dict:
+        """The update's hyper-parameters, as ``ops.sgd_step`` and the rider description of the last backward kernel take them."""
+        return dict(lr=float(group["lr"]), lr_tensor=self._lr_tensor(gi, group, device), momentum=float(group["momentum"]),
+                    dampening=float(group["dampening"]), weight_decay=float(group["weight_decay"]), nesterov=bool(group["nesterov"]),
+                    maximize=bool(group["maximize"]))
 
     # ---- DDP fusion: the update rides on the gradient reduction ----------------------------------------
     def fuse_with_ddp(self, ddp) -> "SGD":
@@ -225,9 +230,7 @@ class SGD(RidingOptimizer):
                     for p, g in zip(params, grads))
             if use_fused:
                 if momentum == 0:
-                    ops.sgd_step(params, grads, None, lr=group["lr"], momentum=0.0, dampening=group["dampening"],
-                                 weight_decay=group["weight_decay"], nesterov=group["nesterov"], maximize=group["maximize"],
-                                 first_step=False, lr_tensor=self._lr_tensor(gi, group, params[0].device))
+                    ops.sgd_step(params, grads, None, first_step=False, **self._hyper(gi, group, params[0].device))
                     continue
                 # "first step" (buf = g, no dampening) is a per-parameter decision, as in torch: parameters that see
                 # their first gradient now go through one launch with first_step=True, the rest through another
@@ -240,10 +243,8 @@ class SGD(RidingOptimizer):
                     if want_first:
                         for i in sel:
                             bufs[i]["momentum_buffer"] = torch.zeros_like(params[i], memory_format=torch.contiguous_format)
-                    ops.sgd_step(ps, gs_, [bufs[i]["momentum_buffer"] for i in sel], lr=group["lr"], momentum=momentum,
-                                 dampening=group["dampening"], weight_decay=group["weight_decay"], nesterov=group["nesterov"],
-                                 maximize=group["maximize"], first_step=want_first,
-                                 lr_tensor=self._lr_tensor(gi, group, params[0].device))
+                    ops.sgd_step(ps, gs_, [bufs[i]["momentum_buffer"] for i in sel], first_step=want_first,
+                                 **self._hyper(gi, group, params[0].device))
                 continue
             # reference math through foreach ops (CPU / exotic dtypes)
             gs = [(-g if group["maximize"] else g) for g in grads] if group["maximize"] else list(grads)

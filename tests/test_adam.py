@@ -236,7 +236,7 @@ def test_captured_step_advances_the_bias_corrections_on_replay():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("cls", [pdt.optim.Adam, pdt.optim.AdamW])
-def test_adam_rides_on_the_last_backward_kernel(cls):
+def test_adam_rider_rides_on_the_last_backward_kernel(cls):
     """Adam.ride_on_backward: the layer-1 backward kernel applies the update of all ten parameters (fused_convnet.cu: AdamRider);
     parameters and state must follow the separate multi-tensor Adam kernel."""
     from pytorch_distributed_train_b200 import _C
@@ -249,7 +249,7 @@ def test_adam_rides_on_the_last_backward_kernel(cls):
     oa = cls(a.parameters(), 1e-3, weight_decay=1e-2)
     ob = cls(b.parameters(), 1e-3, weight_decay=1e-2)
     crit = pdt.nn.CrossEntropyLoss()
-    assert oa.ride_on_backward(a) and OF._sgd_rider["kind"] == "adam"
+    assert oa.ride_on_backward(a) and OF._sgd_rider.owner is oa
     try:
         for s in range(4):
             x = torch.rand(100, 1, 28, 28, device=_dev(), generator=torch.Generator(device=_dev()).manual_seed(s))
