@@ -9,8 +9,8 @@ Extra flags cover what the reference hard-codes: ``--init-method`` (its LAN addr
 ``tcp://10.9.1.2:34567`` only works on the author's network, ref: ddp_example.py:110; we default
 to loopback with a free port), ``--data synthetic|mnist``, ``--model``, ``--comm fused|nccl``, ``--algo``,
 ``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw), ``--lr``,
-``--momentum``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--checkpoint`` /
-``--resume``.
+``--momentum``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--ema-decay``,
+``--checkpoint`` / ``--resume``.
 """
 from __future__ import annotations
 
@@ -57,6 +57,9 @@ def build_parser() -> argparse.ArgumentParser:
                         "(default 1)")
     p.add_argument("--label-smoothing", default=0.0, type=float, metavar="EPS",
                    help="label smoothing of the cross-entropy loss, in [0, 1] (default 0)")
+    p.add_argument("--ema-decay", default=None, type=float, metavar="D",
+                   help="keep an exponential moving average of the weights and buffers with decay D in [0, 1], updated after every "
+                        "optimizer step and saved with --checkpoint (default: off)")
     p.add_argument("--steps", default=0, type=int, help="stop each epoch after this many (optimizer) steps (0 = full epoch)")
     p.add_argument("--samples", default=60000, type=int, help="synthetic dataset size")
     p.add_argument("--graph", default=False, action="store_true", help="capture the whole training step in a CUDA graph")
@@ -88,6 +91,8 @@ def check_args(p: argparse.ArgumentParser, args) -> None:
         p.error(f"--accumulation-steps must be at least 1 (got {args.accumulation_steps})")
     if not 0.0 <= args.label_smoothing <= 1.0:
         p.error(f"--label-smoothing must lie in [0, 1] (got {args.label_smoothing})")
+    if args.ema_decay is not None and not 0.0 <= args.ema_decay <= 1.0:
+        p.error(f"--ema-decay must lie in [0, 1] (got {args.ema_decay})")
     if args.graph and args.gpus >= 2 and args.accumulation_steps > 1:
         p.error("--graph with --accumulation-steps > 1 runs on one GPU only (-g 1)")
 
@@ -125,6 +130,12 @@ def dist_train(gpu: int, args) -> None:
     accum = args.accumulation_steps
     criterion = pdt.nn.CrossEntropyLoss(label_smoothing=args.label_smoothing).to(device)
     optimizer = make_optimizer(args, model.parameters())
+    ema = None
+    if args.ema_decay is not None:
+        from pytorch_distributed_train_b200.optim import swa_utils
+
+        ema = swa_utils.AveragedModel(model, multi_avg_fn=swa_utils.get_ema_multi_avg_fn(args.ema_decay), use_buffers=True)
+    bare = model
     model = pdt.DistributedDataParallel(model, device_ids=[gpu] if use_cuda else None)
 
     if args.data == "mnist" and args.model == "convnet":
@@ -143,11 +154,11 @@ def dist_train(gpu: int, args) -> None:
 
         step_fn = GraphedTrainStep(model, criterion, optimizer, example_inputs=(
             torch.zeros((accum * batch_size,) + shape, device=device), torch.zeros(accum * batch_size, dtype=torch.int64, device=device)),
-            max_grad_norm=args.clip_grad_norm, accumulation_steps=accum)
+            max_grad_norm=args.clip_grad_norm, accumulation_steps=accum, averaged_model=ema)
 
     first_epoch = 0
     if args.resume:
-        info = pdt.utils.load_checkpoint(args.resume, model, optimizer, sampler=train_sampler)
+        info = pdt.utils.load_checkpoint(args.resume, model, optimizer, sampler=train_sampler, averaged_model=ema)
         first_epoch = info["epoch"]
         if gpu == 0:
             print(f"Resumed from {args.resume} at epoch {first_epoch}")
@@ -187,6 +198,8 @@ def dist_train(gpu: int, args) -> None:
                 if args.clip_grad_norm is not None:
                     pdt.nn.utils.clip_grad_norm_(model.parameters(), args.clip_grad_norm)
                 optimizer.step()
+                if ema is not None:
+                    ema.update_parameters(bare)
                 handle = loss
             if pending is not None and gpu == 0:
                 # the log line of the previous step, printed once this step has been queued: the GPU keeps working while the host waits
@@ -200,7 +213,7 @@ def dist_train(gpu: int, args) -> None:
         if pending is not None and gpu == 0:
             print(fmt.format(epoch + 1, args.epochs, pending[0], total_step, pending[1].item()))
         if args.checkpoint:
-            pdt.utils.save_checkpoint(args.checkpoint, model, optimizer, epoch=epoch + 1, sampler=train_sampler)
+            pdt.utils.save_checkpoint(args.checkpoint, model, optimizer, epoch=epoch + 1, sampler=train_sampler, averaged_model=ema)
     if use_cuda:
         torch.cuda.synchronize()
     if gpu == 0:

@@ -856,6 +856,51 @@ void register_cuda_bindings(py::module_& m) {
       launch_grad_scale_multi(tl, norm.data_ptr<float>() + 1, st);
     }
   });
+  // Weight averaging (AveragedModel.update_parameters with the EMA or SWA multi_avg_fn): averaged[i] follows current[i] (fp32, or
+  // int64 under EMA), copied[i] takes copied_from[i]; n_averaged (int64 scalar on the device) advances by one.  decay < 0: SWA.
+  // One launch per 48 pairs, no host synchronisation.
+  m.def("avg_multi", [](std::vector<at::Tensor> averaged, std::vector<at::Tensor> current, at::Tensor n_averaged, double decay,
+                        std::vector<at::Tensor> copied, std::vector<at::Tensor> copied_from) {
+    TORCH_CHECK(averaged.size() == current.size() && copied.size() == copied_from.size(), "avg_multi: list lengths differ");
+    TORCH_CHECK(!averaged.empty() || !copied.empty(), "avg_multi: no tensors");
+    chk(n_averaged, "n_averaged", at::kLong);
+    TORCH_CHECK(n_averaged.numel() == 1, "avg_multi: n_averaged must be one element");
+    const bool swa = decay < 0.0;
+    TORCH_CHECK(swa || decay <= 1.0, "avg_multi: decay must lie in [0, 1]");
+    c10::cuda::CUDAGuard g(n_averaged.device());
+    std::vector<AvgTensorList> tables;
+    auto add = [&](at::Tensor& d, at::Tensor& s, bool copy) {
+      TORCH_CHECK(d.scalar_type() == at::kFloat || d.scalar_type() == at::kLong, "avg_multi: tensors must be float32 or int64");
+      chk(d, "averaged tensor", d.scalar_type());
+      chk(s, "model tensor", d.scalar_type());
+      TORCH_CHECK(d.device() == n_averaged.device() && s.device() == n_averaged.device(), "avg_multi: all tensors on one device");
+      TORCH_CHECK(d.numel() == s.numel() && d.numel() < (int64_t(1) << 31), "avg_multi: bad tensor sizes");
+      const bool f32 = d.scalar_type() == at::kFloat;
+      TORCH_CHECK(copy || f32 || !swa, "avg_multi: SWA does not average int64 tensors (torch's swa_update raises)");
+      if (tables.empty() || tables.back().count == AvgTensorList::kMax) {
+        tables.emplace_back();
+        tables.back().count = 0;
+      }
+      AvgTensorList& tl = tables.back();
+      tl.avg[tl.count] = d.data_ptr();
+      tl.src[tl.count] = s.data_ptr();
+      tl.n[tl.count] = static_cast<int>(d.numel());
+      tl.mode[tl.count] = f32 ? (copy ? AvgTensorList::kCopyF32 : AvgTensorList::kAvgF32) : (copy ? AvgTensorList::kCopyI64 : AvgTensorList::kAvgI64);
+      ++tl.count;
+    };
+    for (size_t i = 0; i < averaged.size(); ++i) add(averaged[i], current[i], false);
+    for (size_t i = 0; i < copied.size(); ++i) add(copied[i], copied_from[i], true);
+    // the ticket word of the n_averaged hand-over (avg_multi_kernel): launches on one device are ordered by the compute stream,
+    // and every set leaves the word at zero
+    AvgArgs a{reinterpret_cast<long long*>(n_averaged.data_ptr<int64_t>()), swa ? 1 : 0, static_cast<float>(swa ? 0.0 : decay), static_cast<float>(swa ? 0.0 : 1.0 - decay), 0,
+              scratch(n_averaged).counter + kAvgTicketWord};
+    cudaStream_t st = cur_stream(n_averaged);
+    for (size_t k = 0; k < tables.size(); ++k) {
+      a.last = k + 1 == tables.size() ? 1 : 0;
+      launch_avg_multi(tables[k], a, st);
+    }
+  }, py::arg("averaged"), py::arg("current"), py::arg("n_averaged"), py::arg("decay"), py::arg("copied") = std::vector<at::Tensor>{},
+     py::arg("copied_from") = std::vector<at::Tensor>{});
 
   // ---- TF32 wgmma GEMM self-test (D[M,N] = A[M,K]·B[N,K]^T) — validates descriptors/TMA/accumulator layout ---
   m.def("gemm_tf32_wgmma", [](const at::Tensor& a, const at::Tensor& b) {

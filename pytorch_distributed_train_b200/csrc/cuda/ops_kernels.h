@@ -29,7 +29,10 @@ struct ReduceScratch {
 //   kCeCounterWord          arrival counter of the whole-forward kernel's cross-entropy mean
 //   kAdamTicketWord         step hand-over ticket of adam_multi
 //   kClipTicketWord         fold ticket of grad_norm_clip
-// Each fixed word sits in a 32-byte sector of its own.
+//   kAvgTicketWord          n_averaged hand-over ticket of avg_multi
+// Each fixed word sits in a 32-byte sector of its own.  A ticket word serves one launch set at a time: the sets that use it are
+// ordered by the device's compute stream, so no two of them (two adam_multi or two avg_multi sets) may run concurrently on
+// different streams of one device.
 constexpr int kScratchFloats = 4 << 20;                   // 16 MiB
 constexpr int kFoldCounterWords = kScratchFloats / 64;    // a fold of width ≥ 4 fills the partials before it runs out of tickets
 constexpr int kGridEpochWord = kFoldCounterWords;
@@ -37,7 +40,8 @@ constexpr int kGridArrivalWord = kFoldCounterWords + 8;
 constexpr int kCeCounterWord = kFoldCounterWords + 16;
 constexpr int kAdamTicketWord = kFoldCounterWords + 24;
 constexpr int kClipTicketWord = kFoldCounterWords + 32;
-constexpr int kCounterWords = kFoldCounterWords + 40;
+constexpr int kAvgTicketWord = kFoldCounterWords + 40;
+constexpr int kCounterWords = kFoldCounterWords + 48;
 
 // ---- SIMT direct convolution (conv1; conv2 fallback + oracle for the tensor-core kernels) -------------
 // x NHWC [B,H,W,Cin], w torch layout [Cout,Cin,5,5], bias [Cout] (nullable) → y NHWC [B,H,W,Cout].
@@ -179,6 +183,30 @@ int grad_multi_blocks_x(const GradTensorList& tl);   // blockIdx.x extent of a t
 void launch_grad_norm_multi(const GradTensorList& tl, GradNormArgs a, cudaStream_t st);
 // g *= *coef for every tensor of the table
 void launch_grad_scale_multi(const GradTensorList& tl, const float* coef, cudaStream_t st);
+
+// Weight averaging: torch.optim.swa_utils.AveragedModel.update_parameters with the EMA or SWA multi_avg_fn, one table of
+// (averaged, model) tensor pairs per launch.  n = *n_averaged (int64 on the device).  An averaged pair takes the model's value
+// when n == 0 and otherwise, in fp32, torch's CUDA lerp(avg, p, w) with w = fp32(1 − decay) (EMA) or 1 / fp32(n + 1) (SWA); an
+// int64 pair follows torch's EMA branch for integers, fp32(avg)·fp32(decay) + fp32(p)·w truncated (torch's SWA raises there, so no
+// caller sends one).  A copied pair (the buffers when use_buffers=False) takes the model's value on every update.
+struct AvgTensorList {
+  static constexpr int kMax = 48;
+  enum Mode : unsigned char { kAvgF32, kCopyF32, kAvgI64, kCopyI64 };
+  void* avg[kMax];
+  const void* src[kMax];
+  int n[kMax];
+  unsigned char mode[kMax];
+  int count;
+};
+struct AvgArgs {
+  long long* n_averaged;   // read by every block of every table; the last table's last block stores n + 1
+  int swa;                 // 1: SWA weight, 0: EMA
+  float decay;             // EMA: fp32(decay), the integer branch's factor
+  float weight;            // EMA: fp32(1 − decay)
+  int last;                // this is the set's last table
+  unsigned int* ticket;    // one zeroed counter word; the block that takes the last ticket resets it
+};
+void launch_avg_multi(const AvgTensorList& tl, AvgArgs a, cudaStream_t st);
 
 #ifdef __CUDACC__
 // max that keeps a NaN (fmaxf drops it), as torch's inf-norm does

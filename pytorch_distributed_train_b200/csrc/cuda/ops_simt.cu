@@ -984,6 +984,57 @@ __global__ void __launch_bounds__(256) grad_scale_multi_kernel(GradTensorList tl
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) g[i] *= c;
 }
 
+// torch's CUDA lerp (ATen/native/Lerp.h) as nvcc contracts it: a + w·(b − a) for |w| < 0.5, else b − (b − a)·(1 − w)
+__device__ __forceinline__ float torch_lerp(float a, float b, float w) {
+  const float d = b - a;
+  return fabsf(w) < 0.5f ? fmaf(w, d, a) : fmaf(-d, 1.f - w, b);
+}
+
+// =====================================================================================================
+// Weight averaging: same layout as sgd_multi_kernel.  Thread 0 of every block reads n_averaged; on the set's last table it then
+// takes a ticket, and the block that takes the last one stores n + 1 (every block has read n by then) and resets the ticket word.
+// =====================================================================================================
+__global__ void __launch_bounds__(256) avg_multi_kernel(AvgTensorList tl, AvgArgs a) {
+  const int t = blockIdx.y;
+  __shared__ long long s_n;
+  if (threadIdx.x == 0) {
+    const long long na = *a.n_averaged;
+    s_n = na;
+    if (a.last) {
+      __threadfence();
+      if (atomicAdd(a.ticket, 1u) == gridDim.x * gridDim.y - 1) {
+        __threadfence();
+        *a.n_averaged = na + 1;
+        atomicExch(a.ticket, 0u);
+      }
+    }
+  }
+  __syncthreads();
+  const long long na = s_n;
+  const int n = tl.n[t], mode = tl.mode[t];
+  const int i0 = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
+  if (mode == AvgTensorList::kAvgF32 || mode == AvgTensorList::kCopyF32) {
+    float* __restrict__ d = static_cast<float*>(tl.avg[t]);
+    const float* __restrict__ s = static_cast<const float*>(tl.src[t]);
+    if (na == 0 || mode == AvgTensorList::kCopyF32) {
+      for (int i = i0; i < n; i += stride) d[i] = s[i];
+      return;
+    }
+    const float w = a.swa ? 1.f / static_cast<float>(na + 1) : a.weight;
+    for (int i = i0; i < n; i += stride) d[i] = torch_lerp(d[i], s[i], w);
+  } else {
+    long long* __restrict__ d = static_cast<long long*>(tl.avg[t]);
+    const long long* __restrict__ s = static_cast<const long long*>(tl.src[t]);
+    if (na == 0 || mode == AvgTensorList::kCopyI64) {
+      for (int i = i0; i < n; i += stride) d[i] = s[i];
+      return;
+    }
+    // p_ema * decay + p_model * (1 - decay): three separate fp32 ops in torch, then copy_ truncates to int64
+    for (int i = i0; i < n; i += stride)
+      d[i] = static_cast<long long>(__fadd_rn(__fmul_rn(static_cast<float>(d[i]), a.decay), __fmul_rn(static_cast<float>(s[i]), a.weight)));
+  }
+}
+
 size_t conv_smem(int cin, int cout, int th, int w, int threads) {
   return (static_cast<size_t>(cin) * (th + 4) * (w + 4) + 4 + 25 * cin * cout + (threads / 32 + 1) * 2 * cout) * sizeof(float);
 }
@@ -1199,6 +1250,15 @@ void launch_grad_scale_multi(const GradTensorList& tl, const float* coef, cudaSt
   if (tl.count == 0) return;
   grad_scale_multi_kernel<<<dim3(grad_multi_blocks_x(tl), tl.count), 256, 0, st>>>(tl, coef);
   check_launch("grad_scale_multi");
+}
+
+void launch_avg_multi(const AvgTensorList& tl, AvgArgs a, cudaStream_t st) {
+  if (tl.count == 0) return;
+  int maxn = 0;
+  for (int i = 0; i < tl.count; ++i) maxn = std::max(maxn, tl.n[i]);
+  const int bx = std::max(1, std::min(64, (maxn + 1023) / 1024));
+  avg_multi_kernel<<<dim3(bx, tl.count), 256, 0, st>>>(tl, a);
+  check_launch("avg_multi");
 }
 
 }  // namespace pdt

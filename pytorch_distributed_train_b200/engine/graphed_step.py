@@ -37,6 +37,14 @@ gradients of micro-batch 1 (accumulate mode, ops.functional.accumulate_into) and
 last micro-batch's backward: 3k launches, no AccumulateGrad add, no separate optimizer or clip kernel.  Any other model,
 criterion or configuration accumulates through autograd.  One GPU only for now: for a model whose gradients are reduced across
 ranks the micro-batches 1..k−1 would have to skip the reduction (``no_sync``) inside the captured step.
+
+Weight averaging (``averaged_model``, a ``pdt.optim.swa_utils.AveragedModel``): every replay ends with
+``averaged_model.update_parameters(model)`` after the optimizer step, as a training loop calls it after ``optimizer.step()``;
+with accumulation, once per replay, after the last micro-batch.  The native update (``ops.average_update``) is one more launch
+inside the graph, on one GPU too: it reads and advances ``n_averaged`` on the device.  (An averaging rider of the last backward
+kernel was measured slower than this launch: DESIGN.md §7.)  torch's own update reads ``n_averaged`` on the host and
+cannot be captured, so an averaged model that would take it is refused.  The warm-up steps the constructor runs are not
+averaged.
 """
 from __future__ import annotations
 
@@ -55,9 +63,18 @@ class GraphedTrainStep:
 
     def __init__(self, model, criterion, optimizer, example_inputs: Sequence[torch.Tensor], warmup: int = 3,
                  zero_grad_set_to_none: bool = True, fuse_optimizer: bool = True, double_buffer_inputs: bool = True,
-                 max_grad_norm: Optional[float] = None, norm_type: float = 2.0, accumulation_steps: int = 1):
+                 max_grad_norm: Optional[float] = None, norm_type: float = 2.0, accumulation_steps: int = 1, averaged_model=None):
         if not torch.cuda.is_available():
             raise RuntimeError("GraphedTrainStep needs CUDA")
+        self.averaged_model = averaged_model
+        self._averaged_source = getattr(model, "module", model)   # the averaged model was copied from the bare model
+        if averaged_model is not None:
+            plan = averaged_model.native_plan(self._averaged_source) if hasattr(averaged_model, "native_plan") else (
+                "it is not a pdt.optim.swa_utils.AveragedModel")
+            if isinstance(plan, str):
+                raise ValueError(f"GraphedTrainStep(averaged_model=...): the averaged model has no native update ({plan}); torch's "
+                                 "AveragedModel.update_parameters reads n_averaged on the host and cannot be captured in a CUDA graph")
+        self._averaging = False   # True while a graph is captured: the warm-up steps are not averaged
         k = int(accumulation_steps)
         if k != accumulation_steps or k < 1:
             raise ValueError(f"accumulation_steps must be a positive integer, got {accumulation_steps}")
@@ -225,6 +242,8 @@ class GraphedTrainStep:
 
                 norm = clip_grad_norm_(self._clip_params, self.max_grad_norm, self.norm_type)
         self.optimizer.step()
+        if self._averaging:
+            self.averaged_model.update_parameters(self._averaged_source)
         return loss, norm
 
     def _capture(self, warmup: int):
@@ -252,8 +271,10 @@ class GraphedTrainStep:
                 self._ride(k)   # each graph's rider stores the norm in its own scalar
             g = torch.cuda.CUDAGraph()
             before = _C.kernel_launch_count()
+            self._averaging = self.averaged_model is not None
             with torch.cuda.graph(g, stream=side):
                 loss, norm = self._eager_step(self.input_sets[k % len(self.input_sets)])
+            self._averaging = False
             # how many of *our* kernels one replay runs (ATen glue kernels are not counted)
             self.kernels_per_replay = int(_C.kernel_launch_count() - before)
             self.graphs.append(g)

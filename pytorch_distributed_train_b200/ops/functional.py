@@ -601,6 +601,14 @@ def grad_scale(grads, norm: torch.Tensor) -> None:
     _C.grad_scale(list(grads), norm)
 
 
+def average_update(averaged, current, n_averaged: torch.Tensor, decay: Optional[float] = None, copied=(), copied_from=()) -> None:
+    """One ``AveragedModel.update_parameters`` with torch's EMA (``decay``) or SWA (``decay=None``) ``multi_avg_fn``: every
+    ``averaged`` tensor (fp32, or int64 under EMA) takes its ``current`` partner's value when ``n_averaged`` (an int64 device
+    scalar) is 0 and is averaged with it otherwise; every ``copied`` tensor takes its ``copied_from`` partner's value; then
+    ``n_averaged`` advances by one.  One launch per 48 pairs, no host synchronisation, graph-capturable."""
+    _C.avg_multi(list(averaged), list(current), n_averaged, -1.0 if decay is None else float(decay), list(copied), list(copied_from))
+
+
 # ---- generic (NCHW) BatchNorm pieces used by parallel.SyncBatchNorm ------------------------------------------
 def bn_local_stats(x: torch.Tensor) -> torch.Tensor:
     """float64 [2C+2] = per-channel Σx, Σx² (accumulated in fp64), the per-channel element count, one zero pad."""

@@ -11,6 +11,10 @@ exactly that on top of ``state_dict`` / ``load_state_dict``:
 * ``load_checkpoint`` — every rank reads the file and restores in place: parameters stay where DDP put them
   (flat symmetric arenas, bucket-mirroring layout of the fused optimizer step), momentum buffers are copied into
   the optimizer's existing flat buffer, so a resumed run is bit-identical to an uninterrupted one.
+
+Both take an optional ``averaged_model`` (``optim.swa_utils.AveragedModel``, e.g. an EMA of the weights): its state dict,
+``n_averaged`` included, is stored under the payload key ``"averaged_model"``.  A checkpoint without that key loads as before and
+leaves the averaged model untouched.
 """
 from __future__ import annotations
 
@@ -32,7 +36,8 @@ def _to_cpu(obj):
 
 
 def save_checkpoint(path: str, model: torch.nn.Module, optimizer: Optional[torch.optim.Optimizer] = None, *, epoch: int = 0,
-                    step: int = 0, sampler=None, extra: Optional[Dict[str, Any]] = None, group=None) -> None:
+                    step: int = 0, sampler=None, extra: Optional[Dict[str, Any]] = None, group=None,
+                    averaged_model: Optional[torch.nn.Module] = None) -> None:
     from .. import distributed as dist
 
     initialized = dist.is_initialized()
@@ -41,6 +46,8 @@ def save_checkpoint(path: str, model: torch.nn.Module, optimizer: Optional[torch
         payload = {"format": 1, "epoch": int(epoch), "step": int(step), "model": _to_cpu(model.state_dict()),
                    "optimizer": _to_cpu(optimizer.state_dict()) if optimizer is not None else None,
                    "sampler_epoch": getattr(sampler, "epoch", None), "extra": extra or {}}
+        if averaged_model is not None:
+            payload["averaged_model"] = _to_cpu(averaged_model.state_dict())
         d = os.path.dirname(os.path.abspath(path))
         os.makedirs(d, exist_ok=True)
         fd, tmp = tempfile.mkstemp(prefix=".ckpt-", dir=d)
@@ -59,7 +66,7 @@ def save_checkpoint(path: str, model: torch.nn.Module, optimizer: Optional[torch
 
 
 def load_checkpoint(path: str, model: torch.nn.Module, optimizer: Optional[torch.optim.Optimizer] = None, *, sampler=None,
-                    strict: bool = True) -> Dict[str, Any]:
+                    strict: bool = True, averaged_model: Optional[torch.nn.Module] = None) -> Dict[str, Any]:
     """Restores in place and returns ``{"epoch", "step", "extra"}``.  Accepts checkpoints written from the wrapped
     (``module.``-prefixed) or the bare model and loads them into either."""
     payload = torch.load(path, map_location="cpu", weights_only=False)
@@ -73,6 +80,8 @@ def load_checkpoint(path: str, model: torch.nn.Module, optimizer: Optional[torch
     model.load_state_dict(sd, strict=strict)
     if optimizer is not None and payload.get("optimizer") is not None:
         optimizer.load_state_dict(payload["optimizer"])
+    if averaged_model is not None and payload.get("averaged_model") is not None:
+        averaged_model.load_state_dict(payload["averaged_model"], strict=strict)
     if sampler is not None and payload.get("sampler_epoch") is not None and hasattr(sampler, "set_epoch"):
         sampler.set_epoch(payload["sampler_epoch"])
     return {"epoch": payload.get("epoch", 0), "step": payload.get("step", 0), "extra": payload.get("extra", {})}

@@ -24,6 +24,7 @@ GROUPS = {
     "ddp1": ["tests/test_gpu_kernels.py::test_single_gpu_ddp_and_graphed_step"],
     "adam": ["tests/test_adam.py"],
     "clip": ["tests/test_clip_grad.py"],
+    "average": ["tests/test_averaged_model.py"],
     "accum": ["tests/test_grad_accumulation.py"],
     "ce_options": ["tests/test_cross_entropy_options.py"],
     "syncbn": ["tests/test_syncbn_native.py"],
