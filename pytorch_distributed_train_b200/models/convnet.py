@@ -10,12 +10,46 @@ device-side grid barrier inside the kernel instead of a kernel boundary; backwar
 classifier's backward and conv2's weight gradient riding along.  What the fused kernels do not cover (eval mode,
 SyncBatchNorm, batch > #SMs, a partially frozen model) runs each ``layerN`` as two per-op kernels (implicit-GEMM conv with the
 BN statistics in its epilogue, then BN-apply+ReLU+MaxPool) and the classifier as one linear kernel.  The same modules fall back
-to the stock layers on CPU (plumbing tests) or when ``fused=False``.
+to the stock layers on CPU (plumbing tests) or when ``fused=False``.  Other layer configurations (another padding mode,
+dilation or stride, a swapped activation, pool or norm layer, an extra module in a ``Sequential``, module hooks, weight norm)
+run torch's layers, since neither kernel route computes them.
 """
 from __future__ import annotations
 
 import torch
 import torch.nn as nn
+from torch.nn.modules import module as _torch_module
+
+from ..parallel.sync_batchnorm import SyncBatchNorm
+
+
+def _unhooked(m) -> bool:
+    return not (m._forward_hooks or m._forward_pre_hooks or m._backward_hooks or m._backward_pre_hooks)
+
+
+def _native_layer(layer) -> bool:
+    """Exactly Conv2d(5×5, stride 1, pad 2) → BatchNorm2d / pdt.SyncBatchNorm → ReLU → MaxPool2d(2, 2), none of them hooked."""
+    if type(layer) is not nn.Sequential or len(layer._modules) != 4 or not _unhooked(layer):
+        return False
+    conv, bn, act, pool = layer._modules.values()
+    return (type(conv) is nn.Conv2d and conv.kernel_size == (5, 5) and conv.stride == (1, 1) and conv.padding in ((2, 2), "same")
+            and conv.dilation == (1, 1) and conv.groups == 1 and conv.padding_mode == "zeros"
+            and type(bn) in (nn.BatchNorm2d, SyncBatchNorm) and type(act) is nn.ReLU
+            and type(pool) is nn.MaxPool2d and pool.kernel_size in (2, (2, 2)) and pool.stride in (2, (2, 2))
+            and pool.padding in (0, (0, 0)) and pool.dilation in (1, (1, 1)) and not pool.ceil_mode
+            and _unhooked(conv) and _unhooked(bn) and _unhooked(act) and _unhooked(pool))
+
+
+def _native_layers(model) -> bool:
+    """Whether ``model``'s layers are the ones the native kernels compute: the stock layer stack, with no hooks on the modules
+    ``forward`` uses and no global module hooks (the native routes never call the submodules, so their hooks would not run).  The
+    model's own hooks do not matter: ``__call__`` runs them.  Pure host logic on module attributes: it reads no device tensor and
+    never synchronises."""
+    mods = model._modules
+    fc = mods.get("fc")
+    return (type(fc) is nn.Linear and _unhooked(fc) and _native_layer(mods.get("layer1")) and _native_layer(mods.get("layer2"))
+            and not (_torch_module._global_forward_hooks or _torch_module._global_forward_pre_hooks
+                     or _torch_module._global_backward_hooks or _torch_module._global_backward_pre_hooks))
 
 
 class ConvNet(nn.Module):
@@ -45,7 +79,7 @@ class ConvNet(nn.Module):
         return ok
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if self._use_fused(x):
+        if _native_layers(self) and self._use_fused(x):
             from .. import ops
             from ..ops import functional as OF
 

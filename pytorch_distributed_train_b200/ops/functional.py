@@ -432,9 +432,10 @@ def _rider_spec_ok(spec: tuple, fcw: torch.Tensor) -> bool:
 def conv_bn_relu_pool(x: torch.Tensor, conv: torch.nn.Conv2d, bn: torch.nn.Module, out_nchw: Optional[bool] = None,
                       impl: str = "auto") -> torch.Tensor:
     """Conv5×5(pad 2) → BatchNorm (batch stats, optionally synchronised) → ReLU → MaxPool2×2 as two
-    kernels forward / four backward (ref layers: ddp_example.py:25-33)."""
-    if conv.kernel_size != (5, 5) or conv.stride != (1, 1) or conv.padding != (2, 2) or conv.groups != 1:
-        raise ValueError("conv_bn_relu_pool: only 5x5 / stride 1 / pad 2 convolutions are fused")
+    kernels forward / four backward (ref layers: ddp_example.py:25-33).  ``padding="same"`` is pad 2 for a 5×5 kernel."""
+    if (conv.kernel_size != (5, 5) or conv.stride != (1, 1) or conv.padding not in ((2, 2), "same") or conv.dilation != (1, 1)
+            or conv.groups != 1 or conv.padding_mode != "zeros"):
+        raise ValueError("conv_bn_relu_pool: only 5x5 / stride 1 / pad 2 / undilated / zero-padded convolutions are fused")
     if impl == "auto":
         impl = os.environ.get("PDT_CONV_IMPL", "auto")  # auto = tensor cores where implemented, SIMT elsewhere
     group = None
