@@ -1232,9 +1232,78 @@ struct L2BwdSmem {
   // weight gradient in the shadow was the last to read.
   static constexpr int kXT = kPatchAlloc + kB + 4096;
   static constexpr int kDyT = kXT + Conv2Wg::kXBytes;
-  static constexpr int kTotalWg = 1024 + kDyT + Conv2Wg::kDyT;
-  static_assert(Conv2Wg::kXBytes <= kFcW && kTotalWg <= 227 * 1024, "conv2 weight-gradient operand placement");
+  // the data gradient's edge rows (l2_dgrad_edge_slot), behind dyᵀ in both forms (past the end of the FC layout)
+  static constexpr int kDxEdge = kDyT + Conv2Wg::kDyT;
+  static constexpr int kDxEdgeBytes = 9 * 10 * 16 * 4;
+  static constexpr int kTotalWg = 1024 + kDxEdge + kDxEdgeBytes;
+  static_assert(Conv2Wg::kXBytes <= kFcW && kDxEdge >= kTotalFc - 1024 && kTotalWg == 230016 && kTotalWg <= 227 * 1024,
+                "conv2 weight-gradient operand and data-gradient edge placement");
 };
+
+// conv2's data gradient with the filter columns in N.  D'[q][16·kw + ci] = Σ_{kh, co} dy[q + 18·kh][co] · Bd[5·kh + kw][ci][co] over
+// patch rows q = 0..255 (four M = 64 tiles; q + 18·kh ≤ 327 stays inside the zeroed patch), then dx[p][ci] = Σ_kw D'[p + kw][16·kw + ci]
+// with kw = 0, 1, 2, 3, 4 added in that order.  Warp w of the warpgroup holds 16-row range r = 4·tile + w of a tile's accumulators;
+// row p + kw of its own rows comes from a lane of the same warp (shuffles), and the first four rows of range r + 1 (columns kw > row)
+// from the edge buffer: slot l2_dgrad_edge_slot(r) holds range r's rows s = 0..3 at entry kw·(kw − 1)/2 + s, [10][16] floats.
+// Tiles 2 and 3 run first, so range 8 is in the buffer when range 7 needs it.  Range r takes slot (r + 1) mod 9: the first pass
+// (ranges 8..15) fills slots 0..7 and the second (ranges 0..7) slots 1..8, so it keeps range 8's slot 0 and overwrites only slots
+// the first pass has finished reading.
+__device__ __forceinline__ int l2_dgrad_edge_slot(int r) { return (r + 1) % 9; }
+
+// Range r's edge rows from its accumulators a (row s = 16r + s is element half 0 of lanes 4s .. 4s + 3).
+__device__ __forceinline__ void l2_dgrad_edge_store(const float (&a)[40], float* edge, int r, int lane) {
+  const int s = lane >> 2, t4 = lane & 3;
+  if (s >= 4) return;
+  float* slot = edge + l2_dgrad_edge_slot(r) * 160;
+#pragma unroll
+  for (int kw = 1; kw < 5; ++kw)
+    if (kw > s)
+#pragma unroll
+      for (int cg = 0; cg < 2; ++cg) {
+        const int e = 4 * (2 * kw + cg);
+        *reinterpret_cast<float2*>(slot + (kw * (kw - 1) / 2 + s) * 16 + 8 * cg + 2 * t4) = make_float2(a[e], a[e + 1]);
+      }
+}
+
+// dx of range r (dxn = the image's [324][16] frame): the thread's output rows are p = 16r + g + 8·hh (g = lane / 4), its columns
+// ci = 8·cg + 2·(lane mod 4) + b, as in the accumulator fragment.  Row p + kw sits in lane 4·((g + kw) mod 8) + lane mod 4, in the
+// other accumulator half when g + kw wraps past 7 and in range r + 1 when it also wraps past the range (only the dropped rows
+// p ≥ 248 of range 15 reach past row 255).
+__device__ __forceinline__ void l2_dgrad_epilogue(const float (&a)[40], const float* edge, float* __restrict__ dxn, int r, int lane) {
+  const int g = lane >> 2, t4 = lane & 3;
+  float o[2][2][2];   // [hh][cg][b]
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+    for (int cg = 0; cg < 2; ++cg)
+#pragma unroll
+      for (int b = 0; b < 2; ++b) o[hh][cg][b] = a[4 * cg + 2 * hh + b];
+  const float* next = edge + l2_dgrad_edge_slot(r + 1) * 160;
+#pragma unroll
+  for (int kw = 1; kw < 5; ++kw) {
+    const int src = 4 * ((g + kw) & 7) + t4;
+    const bool send_upper = g < kw;       // the row this lane sends to lane g − kw is in its upper half
+    const bool take_next = g + kw >= 8;   // row p + kw of the upper half lies in range r + 1
+#pragma unroll
+    for (int cg = 0; cg < 2; ++cg)
+#pragma unroll
+      for (int b = 0; b < 2; ++b) {
+        const int e = 4 * (2 * kw + cg) + b;
+        const float lo = __shfl_sync(0xffffffffu, send_upper ? a[e + 2] : a[e], src);
+        const float hi = __shfl_sync(0xffffffffu, a[e + 2], src);
+        o[0][cg][b] += lo;
+        o[1][cg][b] += !take_next ? hi : r < 15 ? next[(kw * (kw - 1) / 2 + g + kw - 8) * 16 + 8 * cg + 2 * t4 + b] : 0.f;
+      }
+  }
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int p = 16 * r + g + 8 * hh, oh = p / kPW, ow = p - oh * kPW;
+    if (oh < 14 && ow < 14)
+#pragma unroll
+      for (int cg = 0; cg < 2; ++cg)
+        *reinterpret_cast<float2*>(dxn + ((oh + 2) * kPW + ow + 2) * 16 + 8 * cg + 2 * t4) = make_float2(o[hh][cg][0], o[hh][cg][1]);
+  }
+}
 
 // The classifier's backward rides along: the gradient of the pooled activations is computed on the fly,
 // d(out)[n][k] = Σ_j dlogits[n][j] · Wfc[j][k] (fc weights staged in smem once per CTA); the classifier's weight
@@ -1281,6 +1350,7 @@ convnet_l2_bwd_kernel(const float* __restrict__ y /*[B,14,14,32]*/,
 
   GridBar bar(gs);
   TRACE_INIT();
+  const bool trace_wg1_ = (threadIdx.x == 128) && (*reinterpret_cast<volatile int*>(&g_trace_on) != 0);   // the data gradient's end
   trace(3, 0);
   // WG: the loads of conv2's x copies, written in the grid barrier's shadow (the forward kernel wrote x2)
   Conv2WgX<kL2Threads> xr;
@@ -1349,13 +1419,14 @@ convnet_l2_bwd_kernel(const float* __restrict__ y /*[B,14,14,32]*/,
     arg[k] = 0;
     if (pp < 49) {
       const int ph = pp / 7, pw = pp - ph * 7;
-      float best = -INFINITY;
+      float best = -INFINITY, ya = 0.f;   // ya = y at the arg-max, so that no index into yv depends on data (no local memory)
 #pragma unroll
       for (int d = 0; d < 4; ++d) {
         const int p = (2 * ph + (d >> 1)) * 14 + 2 * pw + (d & 1);
         yv[k][d] = y[(static_cast<size_t>(n) * 196 + p) * 32 + c];
         const float z = fmaf(yv[k][d], sc, sh);
-        if (z > best) { best = z; arg[k] = d; }
+        if (d == 0) ya = yv[k][0];
+        if (z > best) { best = z; arg[k] = d; ya = yv[k][d]; }
       }
       // d(out) of this window from the classifier: Σ_j dlogits[n][j] · Wfc[j][c·49 + pp]
       const float* wk = s_fcw + c * 49 + pp;       // bank = (17·c + pp) mod 32: conflict-free across the warp's 32 channels
@@ -1368,9 +1439,7 @@ convnet_l2_bwd_kernel(const float* __restrict__ y /*[B,14,14,32]*/,
       }
       const float go = g0 + g1;
       dzv[k] = best > 0.f ? go : 0.f;
-      float xh = 0.f;
-#pragma unroll
-      for (int d = 0; d < 4; ++d) if (d == arg[k]) xh = (yv[k][d] - mu) * is;
+      const float xh = (ya - mu) * is;
       s1 += dzv[k];
       s2 = fmaf(dzv[k], xh, s2);
     }
@@ -1502,8 +1571,8 @@ convnet_l2_bwd_kernel(const float* __restrict__ y /*[B,14,14,32]*/,
     dysum[static_cast<size_t>(n) * 32 + tid] = s;
   }
   trace(3, 5);
-  // ---- conv2 data gradient: 400 wgmma m64n16k8 by the warpgroup of warps 4..7, accumulators straight to the dx frame; next to
-  // it (WG) conv2's weight-gradient partial, 320 wgmma m64n32k8 by warps 0..3 ---------------------------------------------------
+  // ---- conv2 data gradient: 80 wgmma m64n80k8 by the warpgroup of warps 4..7, two M tiles at a time (l2_dgrad_epilogue); next to
+  // it (WG) conv2's weight-gradient partial, 320 wgmma m64n32k8 by warps 0..3 -------------------------------------------------------
   const int wg = warpgroup_index();
   if constexpr (WG) {
     if (wg == 0) {
@@ -1512,41 +1581,39 @@ convnet_l2_bwd_kernel(const float* __restrict__ y /*[B,14,14,32]*/,
     }
   }
   if (wg == 1) {
-    const int wt = tid - 128;
+    const int wq = warp - 4;
+    float* edge = reinterpret_cast<float*>(smem + L2BwdSmem::kDxEdge);
+    float* dxn = dx + static_cast<size_t>(n) * 324 * 16;
     const uint64_t ad0 = gmma_desc_kmajor<128>(smem_u32(sa)), bd0 = gmma_desc_kmajor<128>(smem_u32(sb));
 #pragma unroll 1
-    for (int t = 0; t < 2; ++t) {
-      float acc[2][8];
+    for (int pass = 0; pass < 2; ++pass) {
+      const int t0 = 2 - 2 * pass;   // tiles 2, 3, then 0, 1
+      float acc[2][40];
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int e = 0; e < 8; ++e) acc[h][e] = 0.f;
+        for (int e = 0; e < 40; ++e) acc[h][e] = 0.f;
       wgmma_fence();
 #pragma unroll 1
       for (int kh = 0; kh < 5; ++kh) {
-        const uint64_t ad = ad0 + static_cast<uint64_t>(((7 * t + kh) * kPW * 128) >> 4);
+        // A: the patch from row 64·t0 + 18·kh; B: the 80 rows (kw, ci) of taps 5·kh .. 5·kh + 4, one 1024-byte-aligned block
+        const uint64_t ad = ad0 + static_cast<uint64_t>(((64 * t0 + kh * kPW) * 128) >> 4);
         const uint64_t bd = bd0 + static_cast<uint64_t>((kh * 5 * 2048) >> 4);
 #pragma unroll
-        for (int kw = 0; kw < 5; ++kw) {
+        for (int k = 0; k < 4; ++k)   // K = 32 output channels = four K=8 steps
 #pragma unroll
-          for (int k = 0; k < 4; ++k)   // K = 32 output channels = four K=8 steps
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-              wgmma_m64n16k8_tf32(acc[h], ad + ((h * 64 * 128 + kw * 128 + k * 32) >> 4), bd + ((kw * 2048 + k * 32) >> 4), (kh | kw | k) != 0);
-        }
+          for (int h = 0; h < 2; ++h) wgmma_m64n80k8_tf32(acc[h], ad + ((h * 64 * 128 + k * 32) >> 4), bd + ((k * 32) >> 4), (kh | k) != 0);
       }
       wgmma_commit();
       wgmma_wait<0>();
+      if (pass == 1) asm volatile("bar.sync 1, 128;" ::: "memory");   // the first pass has read its edge slots
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
+      for (int h = 0; h < 2; ++h) l2_dgrad_edge_store(acc[h], edge, 4 * (t0 + h) + wq, lane);
+      asm volatile("bar.sync 1, 128;" ::: "memory");
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const int rr = 64 * h + wgmma_frag_row(wt, e), ci = wgmma_frag_col(wt, e);
-          const int orow = rr / kPW, ow = rr - orow * kPW;
-          if (rr < 126 && ow < 14) dx[(static_cast<size_t>(n) * 324 + (7 * t + orow + 2) * 18 + ow + 2) * 16 + ci] = acc[h][e];
-        }
-      }
+      for (int h = 0; h < 2; ++h) l2_dgrad_epilogue(acc[h], edge, dxn, 4 * (t0 + h) + wq, lane);
     }
+    trace_stamp(trace_wg1_, 3, 8);
   }
   __syncthreads();
   bar.finish(gs);
@@ -1633,7 +1700,7 @@ void launch_convnet_l2_bwd_fc(const float* dlogits, const float* fcw, const floa
   if (B > 160) throw std::invalid_argument("convnet_l2_bwd_fc: batch too large for the staged dlogits");
   if (accumulate && x2 == nullptr) throw std::invalid_argument("convnet_l2_bwd_fc: accumulate mode needs conv2's input frame (x2)");
   auto kernel = accumulate ? convnet_l2_bwd_kernel<true, true> : x2 != nullptr ? convnet_l2_bwd_kernel<true> : convnet_l2_bwd_kernel<false>;
-  const int smem = x2 != nullptr ? std::max(L2BwdSmem::kTotalFc, L2BwdSmem::kTotalWg) : L2BwdSmem::kTotalFc;
+  const int smem = std::max(L2BwdSmem::kTotalFc, L2BwdSmem::kTotalWg);   // every form has the data gradient's edge buffer
   launch_cooperative(kernel, B, kL2Threads, static_cast<size_t>(smem), st, "convnet_l2_bwd_fc", y, saved, gamma, beta, w, dgamma, dbeta, dy,
                      dx, dysum, partials, gs, dlogits, fcw, pooled, dfcw, dfcb, ncls, loss_parts, loss_out, x2, wpart);
 }

@@ -37,7 +37,7 @@ names = {0: ("forward (whole)", ["start", "conv1 done", "stats partial written",
          1: ("l1_bwd (+conv2 wgrad fold)", ["start", "partial written", "barrier passed", "folded", "conv1 wgrad partial written", "barrier 2 passed",
                                             "end", "dW2 folded"]),
          3: ("l2_bwd (+conv2 wgrad partials)", ["start", "B built", "partial written", "barrier passed", "folded", "dy written", "end",
-                                                "dW2 atoms done (warp 0)"])}
+                                                "dW2 atoms done (warp 0)", "dx written (warp 4)"])}
 def report(t, title):
     print(f"######## {title}")
     spans = {}
