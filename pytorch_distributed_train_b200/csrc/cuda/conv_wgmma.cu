@@ -1,19 +1,17 @@
-// wgmma / TMA kernels for sm_90a (hand-written PTX; no CUTLASS).
+// wgmma / TMA kernels for sm_90a (hand-written PTX; no CUTLASS): the per-op 5x5 convolution of the ConvNet's conv2
+// (16→32 channels, 88% of the model's FLOPs; ref: ddp_example.py:30).
 //
-//  * gemm_tf32_wgmma_kernel — D[M,N] = A[M,K]·B[N,K]^T: both operands arrive by TMA
-//    (cp.async.bulk.tensor, SWIZZLE_128B), one warpgroup issues wgmma.mma_async ... .tf32,
-//    the fp32 accumulator lives in its registers.  It is the self-test
-//    for every descriptor/barrier convention used below (tests/test_gpu_kernels.py).
-//  * conv5x5_wgmma_gather_kernel — the ConvNet's conv2 (88% of the model's FLOPs; ref:
-//    ddp_example.py:30) and its data gradient as an implicit GEMM: M = output pixels (128 per
-//    tile), N = output channels, K = 25 taps × input channels.  The im2col A-tile is never
-//    materialised in global memory: four producer warps gather it straight from the NHWC
-//    activation with 16-byte cp.async (zero-fill for the padding halo) into the 128B-swizzled
-//    K-major layout the wgmma descriptor expects; the repacked weights (B) are TMA-loaded once
-//    per CTA and stay resident in smem; the epilogue adds the bias, folds the per-channel
-//    Σy/Σy² that BatchNorm needs (saving a full re-read of y) and writes the tile with a TMA
-//    store.  TF32 inputs / fp32 accumulate is the same numerics contract the reference gets from
-//    cuDNN (torch allows TF32 in convolutions by default).
+//  * conv5x5_wgmma_im2col_kernel — forward and data gradient as an implicit GEMM: M = output pixels (128 per tile),
+//    N = output channels, K = 25 taps × input channels.  The im2col A-tile of every filter tap is one
+//    cp.async.bulk.tensor im2col load (the TMA unit zero-fills the padding halo), the repacked weights (B) are TMA-loaded
+//    once per CTA and stay resident in smem, and one warpgroup issues wgmma.mma_async ... .tf32 with the fp32 accumulator
+//    in its registers.  The forward epilogue adds the bias, folds the per-channel Σy/Σy² that BatchNorm needs (saving a
+//    full re-read of y) and writes the tile with a TMA store.
+//  * conv5x5_wgrad_mma_kernel — weight and bias gradient: persistent split-K over pixel tiles on warp-level mma.sync (both
+//    operands are MN-major, which TF32 wgmma does not accept); wgrad_fold_kernel then sums the per-CTA partials in a fixed
+//    order.
+// TF32 inputs / fp32 accumulate is the same numerics contract the reference gets from cuDNN (torch allows TF32 in
+// convolutions by default).
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -37,297 +35,6 @@ namespace {
 using namespace ptx;
 
 constexpr int kTileM = 128;
-constexpr int kChunkK = 32;            // fp32 elements per 128-byte swizzle row
-constexpr int kStageBytes = kTileM * 128;
-
-// =====================================================================================================
-// TF32 GEMM self-test:  one CTA per 128-row × NB-column tile of D; 4-stage TMA ring; 160 threads
-// (warps 0-3 = the wgmma warpgroup, warp 4 = TMA producer)
-// =====================================================================================================
-template <int NB>  // N block = 16, 32 or 64 columns
-struct GemmCfg {
-  static constexpr int kStages = 4;
-  static constexpr int kBBytes = NB * 128;
-  static constexpr size_t kSmem = 1024 + kStages * (kStageBytes + kBBytes) + 256;
-};
-
-template <int NB>
-__global__ void __launch_bounds__(160, 1) gemm_tf32_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,
-                                                                const __grid_constant__ CUtensorMap tm_b, float* __restrict__ d, int M,
-                                                                int N, int K) {
-  using Cfg = GemmCfg<NB>;
-  constexpr int kN = NB < 32 ? NB : 32;   // wgmma N per instruction
-  constexpr int kNI = NB / kN;            // instructions per 64-row half
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sa = smem;
-  uint8_t* sb = smem + Cfg::kStages * kStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sb + Cfg::kStages * Cfg::kBBytes);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + Cfg::kStages;
-
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int m0 = blockIdx.x * kTileM, n0 = blockIdx.y * NB;
-  const int nk = (K + kChunkK - 1) / kChunkK;
-
-  if (tid == 0) {
-    tma_prefetch_desc(&tm_a);
-    tma_prefetch_desc(&tm_b);
-    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 128); }
-    fence_mbar_init();
-  }
-  __syncthreads();
-
-  if (warp == 4) {
-    if (elect_one()) {
-      for (int kc = 0; kc < nk; ++kc) {
-        const int s = kc % Cfg::kStages;
-        mbar_wait(&empty[s], ((kc / Cfg::kStages) & 1) ^ 1);
-        mbar_arrive_expect_tx(&full[s], kStageBytes + Cfg::kBBytes);
-        tma_load_2d(sa + s * kStageBytes, &tm_a, &full[s], kc * kChunkK, m0);
-        tma_load_2d(sb + s * Cfg::kBBytes, &tm_b, &full[s], kc * kChunkK, n0);
-      }
-    }
-    return;
-  }
-  float acc[2][kNI][kN / 2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h)
-#pragma unroll
-    for (int i = 0; i < kNI; ++i)
-#pragma unroll
-      for (int e = 0; e < kN / 2; ++e) acc[h][i][e] = 0.f;
-  for (int kc = 0; kc < nk; ++kc) {
-    const int s = kc % Cfg::kStages;
-    mbar_wait(&full[s], (kc / Cfg::kStages) & 1);
-    const uint32_t a0 = smem_u32(sa + s * kStageBytes), b0 = smem_u32(sb + s * Cfg::kBBytes);
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < kChunkK / 8; ++k)
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int i = 0; i < kNI; ++i)
-          wgmma_tf32<kN>(acc[h][i], gmma_desc_kmajor<128>(a0 + h * 64 * 128 + k * 32), gmma_desc_kmajor<128>(b0 + i * kN * 128 + k * 32),
-                         (kc | k) != 0);
-    wgmma_commit();
-    wgmma_wait<0>();
-    mbar_arrive(&empty[s]);
-  }
-  // epilogue straight from the register fragments
-#pragma unroll
-  for (int h = 0; h < 2; ++h)
-#pragma unroll
-    for (int i = 0; i < kNI; ++i)
-#pragma unroll
-      for (int e = 0; e < kN / 2; ++e) {
-        const int row = m0 + 64 * h + wgmma_frag_row(tid, e), col = n0 + i * kN + wgmma_frag_col(tid, e);
-        if (row < M && col < N) d[static_cast<size_t>(row) * N + col] = acc[h][i][e];
-      }
-}
-
-// =====================================================================================================
-// Weight repack for the implicit GEMM:  Bm[NOUT][NCHUNK*32], K index = tap*CK + c  (zero padded)
-//   FWD : Bm[co][tap*16+ci] = w[co][ci][tap]
-//   DGRAD: Bm[ci][tap*32+co] = w[co][ci][24-tap]
-// =====================================================================================================
-template <bool FWD>
-__global__ void repack_weights_kernel(const float* __restrict__ w, float* __restrict__ bm, int Cout, int Cin) {
-  const int CK = FWD ? Cin : Cout, NOUT = FWD ? Cout : Cin;
-  const int tpc = kChunkK / CK, nchunk = (25 + tpc - 1) / tpc, kpad = nchunk * kChunkK;
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= NOUT * kpad) return;
-  const int n = i / kpad, k = i % kpad, tap = k / CK, c = k % CK;
-  float v = 0.f;
-  if (tap < 25) v = FWD ? w[(n * Cin + c) * 25 + tap] : w[(c * Cin + n) * 25 + (24 - tap)];
-  bm[i] = v;
-}
-
-// =====================================================================================================
-// Implicit-GEMM 5x5 convolution on wgmma
-// =====================================================================================================
-template <int CK, int NOUT>
-struct ConvCfg {
-  static constexpr int kTapsPerChunk = kChunkK / CK;                           // 2 (fwd) / 1 (dgrad)
-  static constexpr int kChunks = (25 + kTapsPerChunk - 1) / kTapsPerChunk;     // 13 / 25
-  // 8 smem stages but only 3 cp.async groups in flight per thread: a chunk is multiplied kLag
-  // iterations after it was issued, so the copies of the next chunks overlap the MMAs.
-  static constexpr int kStages = 8;
-  static constexpr int kLag = 3;
-  static constexpr int kBChunkBytes = NOUT * 128;
-  static constexpr int kAccBytes = kTileM * (NOUT + 1) * 4;
-  static constexpr int kThreads = 160;                                         // 4 producer/MMA/epilogue warps + TMA warp
-  // alignment slack + A ring + resident B + output staging + accumulator rows + (barriers, stat partials)
-  static constexpr size_t kSmem = 1024 + kStages * kStageBytes + kChunks * kBChunkBytes + kTileM * 128 + kAccBytes + 2048;
-};
-
-template <int CK, int NOUT, bool FWD>
-__global__ void __launch_bounds__(160, 1) conv5x5_wgmma_gather_kernel(const float* __restrict__ x, const __grid_constant__ CUtensorMap tm_b,
-                                                              const __grid_constant__ CUtensorMap tm_y, const float* __restrict__ bias,
-                                                              float* __restrict__ y, float* stats, ReduceScratch scr, int B, int H, int W,
-                                                              int num_tiles) {
-  using Cfg = ConvCfg<CK, NOUT>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sa = smem;                                                  // [stages][128 rows][128 B] swizzled
-  uint8_t* sb = sa + Cfg::kStages * kStageBytes;                       // [chunks][NOUT rows][128 B] swizzled (TMA)
-  uint8_t* sy = sb + Cfg::kChunks * Cfg::kBChunkBytes;                 // [128 rows][128 B] swizzled output staging
-  float* sacc = reinterpret_cast<float*>(sy + kTileM * 128);          // [128][NOUT + 1] accumulator rows
-  uint64_t* b_full = reinterpret_cast<uint64_t*>(sacc + kTileM * (NOUT + 1));
-  float* s_part = reinterpret_cast<float*>(b_full + 2);               // [4 warps][2*NOUT] + [2*NOUT]
-  __shared__ int s_last;
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int M = B * H * W;
-
-  if (tid == 0) {
-    tma_prefetch_desc(&tm_b);
-    if (FWD) tma_prefetch_desc(&tm_y);
-    mbar_init(b_full, 1);
-    fence_mbar_init();
-  }
-  __syncthreads();
-
-  if (warp == 4) {
-    // ---- weights: one TMA box per K-chunk, resident for the CTA's lifetime -------------------------
-    if (elect_one()) {
-      mbar_arrive_expect_tx(b_full, Cfg::kChunks * Cfg::kBChunkBytes);
-      for (int c = 0; c < Cfg::kChunks; ++c) tma_load_2d(sb + c * Cfg::kBChunkBytes, &tm_b, b_full, c * kChunkK, 0);
-    }
-  } else {
-    // ---- warps 0-3: im2col producers, wgmma issue (the chunk issued kLag iterations earlier), epilogue --------
-    // A stage is refilled kStages chunks after it was filled; its MMAs completed kStages − kLag iterations before.
-    static_assert(Cfg::kLag < Cfg::kStages, "conv5x5_wgmma_gather: the lag must be shorter than the ring");
-    const uint64_t bdesc0 = gmma_desc_kmajor<128>(smem_u32(sb));
-    auto mma_chunk = [&](float (&acc)[2][NOUT / 2], int c, int s) {
-      const uint32_t a0 = smem_u32(sa + s * kStageBytes);
-      const uint64_t bd = bdesc0 + static_cast<uint64_t>((c * Cfg::kBChunkBytes) >> 4);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < kChunkK / 8; ++k)
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-          wgmma_tf32<NOUT>(acc[h], gmma_desc_kmajor<128>(a0 + h * 64 * 128 + k * 32), bd + ((k * 32) >> 4), (c | k) != 0);
-      wgmma_commit();
-      wgmma_wait<0>();
-    };
-    mbar_wait(b_full, 0);
-    const int u = tid & 7;                       // 16-byte column inside the 128-byte K row
-    const int tap_in_chunk = (u * 4) / CK;       // which tap of the chunk this column belongs to
-    const int c4 = (u * 4) % CK;                 // channel offset inside the tap
-    int g = 0, it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      // the 8 rows this thread fills: r = tid/8 + 16 j
-      int row_off[8], row_h[8], row_w[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int r = (tid >> 3) + 16 * j;
-        const int p = tile * kTileM + r;
-        if (p < M) {
-          const int ow = p % W, oh = (p / W) % H, n = p / (W * H);
-          row_off[j] = ((n * H + oh) * W + ow) * CK;
-          row_h[j] = oh;
-          row_w[j] = ow;
-        } else {
-          row_off[j] = 0;
-          row_h[j] = -100000;  // every tap falls outside → zero fill
-          row_w[j] = 0;
-        }
-      }
-      float acc[2][NOUT / 2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int e = 0; e < NOUT / 2; ++e) acc[h][e] = 0.f;
-      for (int c = 0; c < Cfg::kChunks; ++c, ++g) {
-        const int s = g % Cfg::kStages;
-        const int tap = c * Cfg::kTapsPerChunk + tap_in_chunk;
-        const int kh = tap / 5 - 2, kw = tap % 5 - 2;
-        const int delta = (kh * W + kw) * CK + c4;
-        const uint32_t stage = smem_u32(sa + s * kStageBytes);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int r = (tid >> 3) + 16 * j;
-          const int ih = row_h[j] + kh, iw = row_w[j] + kw;
-          const bool ok = tap < 25 && ih >= 0 && ih < H && iw >= 0 && iw < W;
-          const float* src = ok ? x + row_off[j] + delta : x;
-          cp_async_16(stage + r * 128 + ((u ^ (r & 7)) << 4), src, ok ? 16u : 0u);
-        }
-        cp_async_commit();
-        if (c >= Cfg::kLag) {
-          cp_async_wait<Cfg::kLag>();            // chunk c-kLag of this thread has landed
-          fence_proxy_async_smem();              // generic-proxy writes → visible to the tensor core (async proxy)
-          asm volatile("bar.sync 1, 128;" ::: "memory");   // ... and that of every producer thread
-          mma_chunk(acc, c - Cfg::kLag, (g - Cfg::kLag) % Cfg::kStages);
-        }
-      }
-      // drain this tile (its accumulator is needed now): the kLag chunks still in flight; the lag bookkeeping restarts
-      // with the next tile
-      cp_async_wait<0>();
-      fence_proxy_async_smem();
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-#pragma unroll
-      for (int q = Cfg::kLag; q >= 1; --q) mma_chunk(acc, Cfg::kChunks - q, (g - q) % Cfg::kStages);
-      // ---- epilogue ----------------------------------------------------------------------------------
-#pragma unroll
-      for (int h = 0; h < 2; ++h) wgmma_frag_store<NOUT>(acc[h], sacc, NOUT + 1, 64 * h, tid);
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      float v[NOUT];
-#pragma unroll
-      for (int j = 0; j < NOUT; ++j) v[j] = sacc[tid * (NOUT + 1) + j];
-      const int r = tid;  // 0..127 = tile row
-      const int p = tile * kTileM + r;
-      const bool valid = p < M;
-      if (bias) {
-#pragma unroll
-        for (int j = 0; j < NOUT; ++j) v[j] += bias[j];
-      }
-      if constexpr (FWD) {
-        // stage the tile (swizzled like the tensor map) for the TMA store and the column sums
-        asm volatile("bar.sync 1, 128;" ::: "memory");  // previous tile's TMA store has finished reading sy
-#pragma unroll
-        for (int q = 0; q < NOUT / 4; ++q) {
-          float4 o = valid ? make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]) : make_float4(0.f, 0.f, 0.f, 0.f);
-          *reinterpret_cast<float4*>(sy + r * 128 + ((q ^ (r & 7)) << 4)) = o;
-        }
-        fence_proxy_async_smem();
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (tid == 0) {
-          tma_store_2d(&tm_y, sy, 0, tile * kTileM);
-          tma_store_commit();
-        }
-        if (stats) {
-          // column sums over this warp's 32 rows: lane = channel
-          float s1 = 0.f, s2 = 0.f;
-          const int q = lane >> 2, e = lane & 3;
-          for (int rr = warp * 32; rr < warp * 32 + 32; ++rr) {
-            const float val = reinterpret_cast<const float*>(sy + rr * 128 + ((q ^ (rr & 7)) << 4))[e];
-            s1 += val;
-            s2 += val * val;
-          }
-          s_part[warp * 2 * NOUT + lane] = s1;
-          s_part[warp * 2 * NOUT + NOUT + lane] = s2;
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-          float* tile_sums = s_part + 8 * NOUT;  // [2*NOUT]
-          if (tid < 2 * NOUT) tile_sums[tid] = s_part[tid] + s_part[2 * NOUT + tid] + s_part[4 * NOUT + tid] + s_part[6 * NOUT + tid];
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-          // tiles are the contributors of the two-level deterministic fold (grid_fold.cuh)
-          grid_fold(tile_sums, 2 * NOUT, tile, num_tiles, scr, s_part, &s_last, tid, 128, NamedSync<1, 128>{}, [&](int i, float tot) {
-            stats[i] = tot;
-            if (i == 0) stats[2 * NOUT] = static_cast<float>(M);
-          });
-        }
-        if (tid == 0) tma_store_wait_read();
-      } else {
-        if (valid) {
-          float* o = y + static_cast<size_t>(p) * NOUT;
-#pragma unroll
-          for (int q = 0; q < NOUT / 4; ++q) *reinterpret_cast<float4*>(o + 4 * q) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-        }
-      }
-    }
-  }
-}
 
 // =====================================================================================================
 // Implicit-GEMM 5x5 convolution, fully TMA-fed: the im2col A-tile of every filter tap is ONE
@@ -503,7 +210,9 @@ __global__ void __launch_bounds__(160, 1) conv5x5_wgmma_im2col_kernel(const __gr
   }
 }
 
-// Bm[NOUT][25*CK] without K padding (the TMA-fed kernel loads one [NOUT][CK] box per tap)
+// Weight repack for the implicit GEMM: Bm[NOUT][25*CK], K index = tap*CK + c (the kernel loads one [NOUT][CK] box per tap)
+//   FWD  : Bm[co][tap*16+ci] = w[co][ci][tap]
+//   DGRAD: Bm[ci][tap*32+co] = w[co][ci][24-tap]
 template <bool FWD>
 __global__ void repack_weights_dense_kernel(const float* __restrict__ w, float* __restrict__ bm, int Cout, int Cin) {
   const int CK = FWD ? Cin : Cout, NOUT = FWD ? Cout : Cin;
@@ -712,14 +421,15 @@ CUtensorMap make_tmap_im2col(const float* base, int C, int W, int H, int N, CUte
   return m;
 }
 
-// repacked-weight buffers, one per (device, direction); allocated on first use (outside graph capture)
-float* repack_buffer(int dir, size_t floats) {
+// device buffers, one per (device, slot): 0 = forward weights, 1 = data-gradient weights, 2 = the weight gradient's ones
+// column; allocated on first use (outside graph capture)
+float* repack_buffer(int slot_id, size_t floats) {
   static std::mutex mu;
   static std::map<std::pair<int, int>, std::pair<float*, size_t>> bufs;
   int dev = 0;
   cudaGetDevice(&dev);
   std::lock_guard<std::mutex> g(mu);
-  auto& slot = bufs[{dev, dir}];
+  auto& slot = bufs[{dev, slot_id}];
   if (slot.second < floats) {
     if (slot.first) cudaFree(slot.first);
     cudaError_t e = cudaMalloc(&slot.first, floats * sizeof(float));
@@ -733,44 +443,6 @@ float* repack_buffer(int dir, size_t floats) {
 
 bool conv_wgmma_supported(const ConvShape& s) { return s.Cin == 16 && s.Cout == 32; }
 
-void launch_conv5x5_fwd_gather(const float* x, const float* w, const float* bias, float* y, float* stats, ConvShape s, ReduceScratch scr,
-                               cudaStream_t st) {
-  if (!conv_wgmma_supported(s)) throw std::invalid_argument("conv5x5 gather: only 16→32 channels are implemented");
-  using Cfg = ConvCfg<16, 32>;
-  const int M = s.B * s.H * s.W;
-  const int tiles = (M + kTileM - 1) / kTileM;
-  if (stats && (static_cast<long long>(tiles + tiles / kFoldGroup + 1) * 64 > scr.capacity_floats || tiles / kFoldGroup + 2 > scr.fold_counters))
-    throw std::invalid_argument("conv5x5 gather: scratch too small");
-  const int kpad = Cfg::kChunks * kChunkK;
-  float* bm = repack_buffer(0, static_cast<size_t>(32) * kpad);
-  repack_weights_kernel<true><<<(32 * kpad + 255) / 256, 256, 0, st>>>(w, bm, 32, 16);
-  check_launch("repack_weights(fwd)");
-  CUtensorMap tm_b = make_tmap_2d(bm, kpad, 32, kChunkK, 32);
-  CUtensorMap tm_y = make_tmap_2d(y, 32, static_cast<uint64_t>(M), 32, kTileM);
-  auto kern = conv5x5_wgmma_gather_kernel<16, 32, true>;
-  opt_in_smem(kern, Cfg::kSmem);
-  const int grid = std::min(tiles, sm_count());
-  kern<<<grid, Cfg::kThreads, Cfg::kSmem, st>>>(x, tm_b, tm_y, bias, y, stats, scr, s.B, s.H, s.W, tiles);
-  check_launch("conv5x5_wgmma_gather(fwd)");
-}
-
-void launch_conv5x5_dgrad_gather(const float* dy, const float* w, float* dx, ConvShape s, cudaStream_t st) {
-  if (!conv_wgmma_supported(s)) throw std::invalid_argument("conv5x5 gather dgrad: only 16→32 channels are implemented");
-  using Cfg = ConvCfg<32, 16>;
-  const int M = s.B * s.H * s.W;
-  const int tiles = (M + kTileM - 1) / kTileM;
-  const int kpad = Cfg::kChunks * kChunkK;
-  float* bm = repack_buffer(1, static_cast<size_t>(16) * kpad);
-  repack_weights_kernel<false><<<(16 * kpad + 255) / 256, 256, 0, st>>>(w, bm, 32, 16);
-  check_launch("repack_weights(dgrad)");
-  CUtensorMap tm_b = make_tmap_2d(bm, kpad, 16, kChunkK, 16);
-  auto kern = conv5x5_wgmma_gather_kernel<32, 16, false>;
-  opt_in_smem(kern, Cfg::kSmem);
-  const int grid = std::min(tiles, sm_count());
-  kern<<<grid, Cfg::kThreads, Cfg::kSmem, st>>>(dy, tm_b, tm_b, nullptr, dx, nullptr, ReduceScratch{}, s.B, s.H, s.W, tiles);
-  check_launch("conv5x5_wgmma_gather(dgrad)");
-}
-
 void launch_conv5x5_fwd_im2col(const float* x, const float* w, const float* bias, float* y, float* stats, ConvShape s, ReduceScratch scr,
                                cudaStream_t st) {
   if (!conv_wgmma_supported(s)) throw std::invalid_argument("conv5x5 im2col: only 16→32 channels are implemented");
@@ -779,7 +451,7 @@ void launch_conv5x5_fwd_im2col(const float* x, const float* w, const float* bias
   const int tiles = (M + kTileM - 1) / kTileM;
   if (stats && (static_cast<long long>(tiles + tiles / kFoldGroup + 1) * 64 > scr.capacity_floats || tiles / kFoldGroup + 2 > scr.fold_counters))
     throw std::invalid_argument("conv5x5 im2col: scratch too small");
-  float* bm = repack_buffer(3, static_cast<size_t>(32) * 400);
+  float* bm = repack_buffer(0, static_cast<size_t>(32) * 400);
   repack_weights_dense_kernel<true><<<(32 * 400 + 255) / 256, 256, 0, st>>>(w, bm, 32, 16);
   check_launch("repack_weights_dense(fwd)");
   CUtensorMap tm_x = make_tmap_im2col(x, 16, s.W, s.H, s.B, CU_TENSOR_MAP_SWIZZLE_64B);
@@ -797,7 +469,7 @@ void launch_conv5x5_dgrad_im2col(const float* dy, const float* w, float* dx, Con
   using Cfg = ConvTmaCfg<32, 16>;
   const int M = s.B * s.H * s.W;
   const int tiles = (M + kTileM - 1) / kTileM;
-  float* bm = repack_buffer(4, static_cast<size_t>(16) * 800);
+  float* bm = repack_buffer(1, static_cast<size_t>(16) * 800);
   repack_weights_dense_kernel<false><<<(16 * 800 + 255) / 256, 256, 0, st>>>(w, bm, 32, 16);
   check_launch("repack_weights_dense(dgrad)");
   CUtensorMap tm_x = make_tmap_im2col(dy, 32, s.W, s.H, s.B, CU_TENSOR_MAP_SWIZZLE_128B);
@@ -837,26 +509,6 @@ void launch_conv5x5_wgrad_mma(const float* dy, const float* x, float* dw, float*
   check_launch("conv5x5_wgrad_mma");
   wgrad_fold_kernel<<<401, 256, 0, st>>>(scr.partials, grid, dw, db);
   check_launch("wgrad_fold");
-}
-
-void launch_gemm_tf32_wgmma(const float* a, const float* b, float* d, int M, int N, int K, cudaStream_t st) {
-  if (N % 16 != 0 || N < 16 || N > 256) throw std::invalid_argument("gemm_tf32_wgmma: N must be a multiple of 16 in [16, 256]");
-  if (K % 4 != 0 || K < 4) throw std::invalid_argument("gemm_tf32_wgmma: K must be a positive multiple of 4 (16-byte rows for TMA)");
-  CUtensorMap tm_a = make_tmap_2d(a, static_cast<uint64_t>(K), static_cast<uint64_t>(M), kChunkK, kTileM);
-  const int mtiles = (M + kTileM - 1) / kTileM;
-#define PDT_GEMM_CASE(NB)                                                                    \
-  if (N <= NB || NB == 64) {                                                                 \
-    CUtensorMap tm_b = make_tmap_2d(b, static_cast<uint64_t>(K), static_cast<uint64_t>(N), kChunkK, NB); \
-    auto kern = gemm_tf32_wgmma_kernel<NB>;                                                   \
-    opt_in_smem(kern, GemmCfg<NB>::kSmem);                                                   \
-    kern<<<dim3(mtiles, (N + NB - 1) / NB), 160, GemmCfg<NB>::kSmem, st>>>(tm_a, tm_b, d, M, N, K); \
-    check_launch("gemm_tf32_wgmma");                                                          \
-    return;                                                                                  \
-  }
-  PDT_GEMM_CASE(16)
-  PDT_GEMM_CASE(32)
-  PDT_GEMM_CASE(64)
-#undef PDT_GEMM_CASE
 }
 
 }  // namespace pdt

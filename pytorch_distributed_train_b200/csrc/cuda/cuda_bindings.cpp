@@ -243,21 +243,6 @@ SymmLaunchCfg launch_cfg(int blocks, int threads) {
 // The grid barrier of the cooperative kernels lives in the fixed words behind the fold region.
 GridSync grid_sync(const ReduceScratch& r) { return GridSync{r.counter + kGridEpochWord, r.counter + kGridArrivalWord}; }
 
-// Kernel family of the per-op conv2, selected by the `impl` argument of the conv5x5_* bindings:
-//   auto, tma → TMA-im2col wgmma forward / data gradient;
-//   tcgen05   → the cp.async-gather wgmma kernel for forward / data gradient;
-//   simt      → the CUDA-core kernels for all three.
-// Both tensor-core choices compute the weight gradient with the mma.sync split-K kernel.  Shapes the tensor-core kernels
-// do not cover (conv1: K = 25) always take SIMT.
-enum class ConvImpl { kIm2col, kGather, kSimt };
-
-ConvImpl conv_impl(const std::string& impl) {
-  if (impl == "auto" || impl == "tma") return ConvImpl::kIm2col;
-  if (impl == "tcgen05") return ConvImpl::kGather;
-  TORCH_CHECK(impl == "simt", "conv5x5: impl must be one of auto, tma, tcgen05, simt (got '", impl, "')");
-  return ConvImpl::kSimt;
-}
-
 ConvShape conv_shape(const at::Tensor& x_nhwc, const at::Tensor& w) {
   TORCH_CHECK(x_nhwc.dim() == 4 && w.dim() == 4 && w.size(2) == 5 && w.size(3) == 5, "conv5x5: x [B,H,W,Cin] and w [Cout,Cin,5,5] expected");
   ConvShape s;
@@ -369,9 +354,10 @@ void register_cuda_bindings(py::module_& m) {
            py::arg("store"), py::arg("rank"), py::arg("size"), py::arg("device"), py::arg("timeout") = 600.0);
 
   // ---- convolution ---------------------------------------------------------------------------------
-  m.def("conv5x5_fwd", [](const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> bias, bool want_stats, const std::string& impl,
-                          bool zero_pad) {
-    const ConvImpl family = conv_impl(impl);
+  // The shape picks the kernels: conv2 (16→32) runs on the tensor cores (TMA-im2col wgmma forward and data gradient, mma.sync
+  // weight gradient), every other shape on the SIMT forward and weight gradient, which cover conv1 (1→16) and refuse the rest.
+  // Only conv2 has a data gradient: conv1's input needs none.
+  m.def("conv5x5_fwd", [](const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> bias, bool want_stats, bool zero_pad) {
     chk(x, "x"); chk(w, "w");
     c10::cuda::CUDAGuard g(x.device());
     ConvShape s = conv_shape(x, w);
@@ -382,36 +368,30 @@ void register_cuda_bindings(py::module_& m) {
     // padded temporary (3 extra kernels)
     at::Tensor stats_full = !want_stats ? at::Tensor() : (zero_pad ? at::zeros({2 * s.Cout + 4}, x.options()) : at::empty({2 * s.Cout + 4}, x.options()));
     at::Tensor stats = want_stats ? stats_full.narrow(0, 0, 2 * s.Cout + 1) : at::Tensor();
-    const ConvImpl k = conv_wgmma_supported(s) ? family : ConvImpl::kSimt;
-    auto launch = k == ConvImpl::kIm2col ? launch_conv5x5_fwd_im2col : k == ConvImpl::kGather ? launch_conv5x5_fwd_gather : launch_conv5x5_fwd;
+    auto launch = conv_wgmma_supported(s) ? launch_conv5x5_fwd_im2col : launch_conv5x5_fwd;
     launch(x.data_ptr<float>(), w.data_ptr<float>(), opt_ptr(bias, "bias"), y.data_ptr<float>(), want_stats ? stats.data_ptr<float>() : nullptr, s,
            scratch(x), cur_stream(x));
     return py::make_tuple(y, stats);  // stats is a view of the first 2C+1 entries of the zero-padded vector
-  }, py::arg("x"), py::arg("w"), py::arg("bias") = py::none(), py::arg("want_stats") = true, py::arg("impl") = "auto",
-     py::arg("zero_pad") = false);
+  }, py::arg("x"), py::arg("w"), py::arg("bias") = py::none(), py::arg("want_stats") = true, py::arg("zero_pad") = false);
 
-  m.def("conv5x5_dgrad", [](const at::Tensor& dy, const at::Tensor& w, const std::string& impl) {
-    const ConvImpl family = conv_impl(impl);
+  m.def("conv5x5_dgrad", [](const at::Tensor& dy, const at::Tensor& w) {
     chk(dy, "dy"); chk(w, "w");
     c10::cuda::CUDAGuard g(dy.device());
     ConvShape s = conv_shape(dy, w);
     s.Cin = static_cast<int>(w.size(1));
     TORCH_CHECK(dy.size(3) == s.Cout, "conv5x5_dgrad: dy channels must equal weight Cout");
     at::Tensor dx = at::empty({s.B, s.H, s.W, s.Cin}, dy.options());
-    const ConvImpl k = conv_wgmma_supported(s) ? family : ConvImpl::kSimt;
-    auto launch = k == ConvImpl::kIm2col ? launch_conv5x5_dgrad_im2col : k == ConvImpl::kGather ? launch_conv5x5_dgrad_gather : launch_conv5x5_dgrad;
-    launch(dy.data_ptr<float>(), w.data_ptr<float>(), dx.data_ptr<float>(), s, cur_stream(dy));
+    launch_conv5x5_dgrad_im2col(dy.data_ptr<float>(), w.data_ptr<float>(), dx.data_ptr<float>(), s, cur_stream(dy));
     return dx;
-  }, py::arg("dy"), py::arg("w"), py::arg("impl") = "auto");
+  }, py::arg("dy"), py::arg("w"));
 
-  m.def("conv5x5_wgrad", [](const at::Tensor& dy, const at::Tensor& x, at::Tensor dw, c10::optional<at::Tensor> db, const std::string& impl) {
-    const ConvImpl family = conv_impl(impl);
+  m.def("conv5x5_wgrad", [](const at::Tensor& dy, const at::Tensor& x, at::Tensor dw, c10::optional<at::Tensor> db) {
     chk(dy, "dy"); chk(x, "x"); chk(dw, "dw");
     c10::cuda::CUDAGuard g(dy.device());
     ConvShape s = conv_shape(x, dw);
-    auto launch = conv_wgmma_supported(s) && family != ConvImpl::kSimt ? launch_conv5x5_wgrad_mma : launch_conv5x5_wgrad;
+    auto launch = conv_wgmma_supported(s) ? launch_conv5x5_wgrad_mma : launch_conv5x5_wgrad;
     launch(dy.data_ptr<float>(), x.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"), s, scratch(x), cur_stream(x));
-  }, py::arg("dy"), py::arg("x"), py::arg("dw"), py::arg("db") = py::none(), py::arg("impl") = "auto");
+  }, py::arg("dy"), py::arg("x"), py::arg("dw"), py::arg("db") = py::none());
 
   // ---- cooperative fused ConvNet layers (fused_convnet.cu): one CTA per image, grid barrier for the batch statistics ----
   m.def("fused_convnet_supported", [](int64_t B) { return fused_convnet_supported(static_cast<int>(B)); });
@@ -901,16 +881,6 @@ void register_cuda_bindings(py::module_& m) {
     }
   }, py::arg("averaged"), py::arg("current"), py::arg("n_averaged"), py::arg("decay"), py::arg("copied") = std::vector<at::Tensor>{},
      py::arg("copied_from") = std::vector<at::Tensor>{});
-
-  // ---- TF32 wgmma GEMM self-test (D[M,N] = A[M,K]·B[N,K]^T) — validates descriptors/TMA/accumulator layout ---
-  m.def("gemm_tf32_wgmma", [](const at::Tensor& a, const at::Tensor& b) {
-    chk(a, "a"); chk(b, "b");
-    c10::cuda::CUDAGuard g(a.device());
-    TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && a.size(1) == b.size(1), "gemm_tf32: A [M,K], B [N,K]");
-    at::Tensor d = at::empty({a.size(0), b.size(0)}, a.options());
-    launch_gemm_tf32_wgmma(a.data_ptr<float>(), b.data_ptr<float>(), d.data_ptr<float>(), a.size(0), b.size(0), a.size(1), cur_stream(a));
-    return d;
-  });
 }
 
 }  // namespace pdt

@@ -172,12 +172,5 @@ __device__ __forceinline__ uint64_t gmma_desc_kmajor_noswz(uint32_t smem_addr) {
   return static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4) | static_cast<uint64_t>(LBO >> 4) << 16 | static_cast<uint64_t>(SBO >> 4) << 32;
 }
 
-__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(
-                   smem_u32(smem_dst)),
-               "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-
 }  // namespace ptx
 }  // namespace pdt

@@ -43,13 +43,11 @@ constexpr int kClipTicketWord = kFoldCounterWords + 32;
 constexpr int kAvgTicketWord = kFoldCounterWords + 40;
 constexpr int kCounterWords = kFoldCounterWords + 48;
 
-// ---- SIMT direct convolution (conv1; conv2 fallback + oracle for the tensor-core kernels) -------------
+// ---- SIMT direct convolution (conv1: 1→16 channels; conv2 runs on the tensor-core kernels of conv_wgmma.h) ----
 // x NHWC [B,H,W,Cin], w torch layout [Cout,Cin,5,5], bias [Cout] (nullable) → y NHWC [B,H,W,Cout].
 // stats (nullable): [2*Cout+1] = per-channel Σy, Σy², then the element count per channel.
 void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float* y, float* stats, ConvShape s,
                         ReduceScratch scr, cudaStream_t st);
-// dx NHWC [B,H,W,Cin] = conv_transpose(dy NHWC [B,H,W,Cout], w)
-void launch_conv5x5_dgrad(const float* dy, const float* w, float* dx, ConvShape s, cudaStream_t st);
 // dw [Cout,Cin,5,5], db [Cout] (nullable) from dy NHWC and x NHWC.
 void launch_conv5x5_wgrad(const float* dy, const float* x, float* dw, float* db, ConvShape s, ReduceScratch scr, cudaStream_t st);
 

@@ -4,8 +4,8 @@
 // MaxPool in one pass (no int64 pool indices: the arg-max is recomputed in backward), fused
 // log-softmax/NLL, one multi-tensor SGD launch.  All cross-CTA reductions are deterministic
 // (per-CTA partials + last-CTA fold in fixed order), so runs are bit-reproducible.
-// conv2 (88% of the FLOPs) has a tensor-core implementation in conv_wgmma.cu; the SIMT
-// version here is its fallback and numerical oracle.
+// The SIMT convolution serves conv1 (1→16 channels); conv2 (16→32, 88% of the FLOPs) runs on the
+// tensor-core kernels of conv_wgmma.cu.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -25,9 +25,8 @@ namespace {
 // =====================================================================================================
 // Direct 5x5 "same" convolution, NHWC, one CTA = TH output rows of one image, all output channels.
 //   thread = (pixel, group of CPT output channels); input patch planar in smem, weights [tap][ci][co].
-// TRANSPOSED=true computes the data gradient: weights are read as w[ci_k][co_k][24-tap].
 // =====================================================================================================
-template <int CIN, int COUT, int CPT, int TH, bool STATS, bool TRANSPOSED>
+template <int CIN, int COUT, int CPT, int TH, bool STATS>
 __global__ void __launch_bounds__(448) conv5x5_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
                                                       float* __restrict__ y, float* stats, ReduceScratch scr, int B, int H, int W) {
   constexpr int G = COUT / CPT;
@@ -43,7 +42,7 @@ __global__ void __launch_bounds__(448) conv5x5_kernel(const float* __restrict__ 
 
   for (int i = tid; i < 25 * CIN * COUT; i += blockDim.x) {
     const int tap = i / (CIN * COUT), ci = (i / COUT) % CIN, co = i % COUT;
-    ws[i] = TRANSPOSED ? w[(ci * COUT + co) * 25 + (24 - tap)] : w[(co * CIN + ci) * 25 + tap];
+    ws[i] = w[(co * CIN + ci) * 25 + tap];
   }
   for (int i = tid; i < CIN * PH * PW; i += blockDim.x) {
     const int ci = i % CIN, c = (i / CIN) % PW, r = i / (CIN * PW);
@@ -121,7 +120,8 @@ __global__ void __launch_bounds__(448) conv5x5_kernel(const float* __restrict__ 
 }
 
 // =====================================================================================================
-// Weight gradient: one CTA = TH rows of one image; thread owns (tap,ci) pairs × all COUT.
+// Weight gradient: one CTA = TH rows of one image; a lane owns one (tap,ci) pair × all COUT, the warps split the
+// pixels and smem folds the warps.
 // Partials [CTA][25*CIN*COUT + COUT] are folded by a second kernel (too large for a last-CTA fold).
 // =====================================================================================================
 template <int CIN, int COUT, int TH>
@@ -147,63 +147,38 @@ __global__ void __launch_bounds__(256) conv5x5_wgrad_kernel(const float* __restr
   constexpr int P = 25 * CIN;
   const int width = P * COUT + COUT;
   float* out = partials + static_cast<size_t>(blockIdx.x) * width;
-  if constexpr (P >= 64) {
-    for (int p = tid; p < P; p += blockDim.x) {
-      const int tap = p / CIN, ci = p % CIN, kh = tap / 5, kw = tap % 5;
-      float acc[COUT];
+  static_assert(P <= 32, "conv5x5_wgrad_kernel: one lane per (tap, ci) pair");
+  const int lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+  float acc[COUT];
 #pragma unroll
-      for (int j = 0; j < COUT; ++j) acc[j] = 0.f;
-      for (int pix = 0; pix < npix; ++pix) {
-        const int py = pix / W, px = pix % W;
-        const float xv = xs[(ci * PH + py + kh) * PW + px + kw];
-        const float4* d4 = reinterpret_cast<const float4*>(dys + pix * COUT);
+  for (int j = 0; j < COUT; ++j) acc[j] = 0.f;
+  if (lane < P) {
+    const int tap = lane / CIN, ci = lane % CIN, kh = tap / 5, kw = tap % 5;
+    for (int pix = warp; pix < npix; pix += nwarps) {
+      const int py = pix / W, px = pix % W;
+      const float xv = xs[(ci * PH + py + kh) * PW + px + kw];
+      const float4* d4 = reinterpret_cast<const float4*>(dys + pix * COUT);
 #pragma unroll
-        for (int j4 = 0; j4 < COUT / 4; ++j4) {
-          const float4 d = d4[j4];
-          acc[j4 * 4 + 0] = fmaf(xv, d.x, acc[j4 * 4 + 0]);
-          acc[j4 * 4 + 1] = fmaf(xv, d.y, acc[j4 * 4 + 1]);
-          acc[j4 * 4 + 2] = fmaf(xv, d.z, acc[j4 * 4 + 2]);
-          acc[j4 * 4 + 3] = fmaf(xv, d.w, acc[j4 * 4 + 3]);
-        }
-      }
-      // partial layout matches torch's dw [co][ci][tap]
-#pragma unroll
-      for (int co = 0; co < COUT; ++co) out[(co * CIN + ci) * 25 + tap] = acc[co];
-    }
-  } else {
-    // few (tap,ci) pairs (conv1: 25): lanes own pairs, warps split the pixels, smem folds the warps
-    const int lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
-    float acc[COUT];
-#pragma unroll
-    for (int j = 0; j < COUT; ++j) acc[j] = 0.f;
-    if (lane < P) {
-      const int tap = lane / CIN, ci = lane % CIN, kh = tap / 5, kw = tap % 5;
-      for (int pix = warp; pix < npix; pix += nwarps) {
-        const int py = pix / W, px = pix % W;
-        const float xv = xs[(ci * PH + py + kh) * PW + px + kw];
-        const float4* d4 = reinterpret_cast<const float4*>(dys + pix * COUT);
-#pragma unroll
-        for (int j4 = 0; j4 < COUT / 4; ++j4) {
-          const float4 d = d4[j4];
-          acc[j4 * 4 + 0] = fmaf(xv, d.x, acc[j4 * 4 + 0]);
-          acc[j4 * 4 + 1] = fmaf(xv, d.y, acc[j4 * 4 + 1]);
-          acc[j4 * 4 + 2] = fmaf(xv, d.z, acc[j4 * 4 + 2]);
-          acc[j4 * 4 + 3] = fmaf(xv, d.w, acc[j4 * 4 + 3]);
-        }
+      for (int j4 = 0; j4 < COUT / 4; ++j4) {
+        const float4 d = d4[j4];
+        acc[j4 * 4 + 0] = fmaf(xv, d.x, acc[j4 * 4 + 0]);
+        acc[j4 * 4 + 1] = fmaf(xv, d.y, acc[j4 * 4 + 1]);
+        acc[j4 * 4 + 2] = fmaf(xv, d.z, acc[j4 * 4 + 2]);
+        acc[j4 * 4 + 3] = fmaf(xv, d.w, acc[j4 * 4 + 3]);
       }
     }
-    float* fold = dys + npix * COUT;  // [nwarps][P*COUT], sized by the host
-    if (lane < P)
+  }
+  float* fold = dys + npix * COUT;  // [nwarps][P*COUT], sized by the host
+  if (lane < P)
 #pragma unroll
-      for (int co = 0; co < COUT; ++co) fold[(warp * P + lane) * COUT + co] = acc[co];
-    __syncthreads();
-    for (int i = tid; i < P * COUT; i += blockDim.x) {
-      const int p = i / COUT, co = i % COUT;
-      float s = 0.f;
-      for (int wi = 0; wi < nwarps; ++wi) s += fold[(wi * P + p) * COUT + co];
-      const int tap = p / CIN, ci = p % CIN;
-      out[(co * CIN + ci) * 25 + tap] = s;
-    }
+    for (int co = 0; co < COUT; ++co) fold[(warp * P + lane) * COUT + co] = acc[co];
+  __syncthreads();
+  for (int i = tid; i < P * COUT; i += blockDim.x) {
+    const int p = i / COUT, co = i % COUT;
+    float s = 0.f;
+    for (int wi = 0; wi < nwarps; ++wi) s += fold[(wi * P + p) * COUT + co];
+    const int tap = p / CIN, ci = p % CIN;
+    out[(co * CIN + ci) * 25 + tap] = s;
   }
   // bias gradient partial: Σ_pixels dy[:, co] — 256/COUT pixel slices in parallel, folded in slice order
   {
@@ -1045,58 +1020,29 @@ size_t conv_smem(int cin, int cout, int th, int w, int threads) {
 void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float* y, float* stats, ConvShape s, ReduceScratch scr,
                         cudaStream_t st) {
   constexpr int TH = 7;
+  if (!(s.Cin == 1 && s.Cout == 16)) throw std::invalid_argument("conv5x5_fwd: supported channel config is 1→16");
   if (s.H % TH != 0) throw std::invalid_argument("conv5x5_fwd: H must be a multiple of 7");
   const int blocks = s.B * (s.H / TH);
   if (stats && (static_cast<long long>(blocks + blocks / kFoldGroup + 1) * 2 * s.Cout > scr.capacity_floats || blocks / kFoldGroup + 2 > scr.fold_counters))
     throw std::invalid_argument("conv5x5_fwd: reduction scratch too small");
-  if (s.Cin == 1 && s.Cout == 16) {
-    const int threads = (TH * s.W + 31) / 32 * 32;
-    const size_t sm = conv_smem(1, 16, TH, s.W, threads);
-    if (stats) conv5x5_kernel<1, 16, 16, TH, true, false><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, scr, s.B, s.H, s.W);
-    else conv5x5_kernel<1, 16, 16, TH, false, false><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, scr, s.B, s.H, s.W);
-  } else if (s.Cin == 16 && s.Cout == 32) {
-    const int threads = (TH * s.W * 4 + 31) / 32 * 32;
-    const size_t sm = conv_smem(16, 32, TH, s.W, threads);
-    opt_in_smem(conv5x5_kernel<16, 32, 8, TH, true, false>, sm);
-    opt_in_smem(conv5x5_kernel<16, 32, 8, TH, false, false>, sm);
-    if (stats) conv5x5_kernel<16, 32, 8, TH, true, false><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, scr, s.B, s.H, s.W);
-    else conv5x5_kernel<16, 32, 8, TH, false, false><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, scr, s.B, s.H, s.W);
-  } else {
-    throw std::invalid_argument("conv5x5_fwd: supported channel configs are 1→16 and 16→32");
-  }
+  const int threads = (TH * s.W + 31) / 32 * 32;
+  const size_t sm = conv_smem(1, 16, TH, s.W, threads);
+  if (stats) conv5x5_kernel<1, 16, 16, TH, true><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, scr, s.B, s.H, s.W);
+  else conv5x5_kernel<1, 16, 16, TH, false><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, scr, s.B, s.H, s.W);
   check_launch("conv5x5_fwd");
-}
-
-void launch_conv5x5_dgrad(const float* dy, const float* w, float* dx, ConvShape s, cudaStream_t st) {
-  constexpr int TH = 7;
-  if (!(s.Cin == 16 && s.Cout == 32)) throw std::invalid_argument("conv5x5_dgrad: supported config is 16→32");
-  if (s.H % TH != 0) throw std::invalid_argument("conv5x5_dgrad: H must be a multiple of 7");
-  const int blocks = s.B * (s.H / TH);
-  const int threads = (TH * s.W * 2 + 31) / 32 * 32;
-  const size_t sm = conv_smem(32, 16, TH, s.W, threads);
-  opt_in_smem(conv5x5_kernel<32, 16, 8, TH, false, true>, sm);
-  conv5x5_kernel<32, 16, 8, TH, false, true><<<blocks, threads, sm, st>>>(dy, w, nullptr, dx, nullptr, ReduceScratch{}, s.B, s.H, s.W);
-  check_launch("conv5x5_dgrad");
 }
 
 void launch_conv5x5_wgrad(const float* dy, const float* x, float* dw, float* db, ConvShape s, ReduceScratch scr, cudaStream_t st) {
   constexpr int TH = 7;
+  if (!(s.Cin == 1 && s.Cout == 16)) throw std::invalid_argument("conv5x5_wgrad: supported channel config is 1→16");
   if (s.H % TH != 0) throw std::invalid_argument("conv5x5_wgrad: H must be a multiple of 7");
   const int blocks = s.B * (s.H / TH);
   const int width = 25 * s.Cin * s.Cout + s.Cout;
   if (static_cast<long long>(blocks) * width > scr.capacity_floats) throw std::invalid_argument("conv5x5_wgrad: reduction scratch too small");
   const size_t xs_f = static_cast<size_t>(s.Cin) * (TH + 4) * (s.W + 4);
-  if (s.Cin == 1 && s.Cout == 16) {
-    const size_t fold_f = static_cast<size_t>(8) * 25 * 16;  // [warps][P*COUT] after dys
-    const size_t sm = (xs_f + 4 + static_cast<size_t>(TH) * s.W * s.Cout + fold_f) * sizeof(float);
-    conv5x5_wgrad_kernel<1, 16, TH><<<blocks, 256, sm, st>>>(dy, x, scr.partials, s.B, s.H, s.W);
-  } else if (s.Cin == 16 && s.Cout == 32) {
-    const size_t sm = (xs_f + 4 + static_cast<size_t>(TH) * s.W * s.Cout) * sizeof(float);
-    opt_in_smem(conv5x5_wgrad_kernel<16, 32, TH>, sm);
-    conv5x5_wgrad_kernel<16, 32, TH><<<blocks, 256, sm, st>>>(dy, x, scr.partials, s.B, s.H, s.W);
-  } else {
-    throw std::invalid_argument("conv5x5_wgrad: supported channel configs are 1→16 and 16→32");
-  }
+  const size_t fold_f = static_cast<size_t>(8) * 25 * 16;  // [warps][P*COUT] after dys
+  const size_t sm = (xs_f + 4 + static_cast<size_t>(TH) * s.W * s.Cout + fold_f) * sizeof(float);
+  conv5x5_wgrad_kernel<1, 16, TH><<<blocks, 256, sm, st>>>(dy, x, scr.partials, s.B, s.H, s.W);
   check_launch("conv5x5_wgrad");
   fold_partials_kernel<<<(width + 31) / 32, 256, 0, st>>>(scr.partials, blocks, width, 25 * s.Cin * s.Cout, dw, db);
   check_launch("fold_partials");

@@ -72,23 +72,23 @@ def _to_nhwc(x: torch.Tensor) -> torch.Tensor:
 
 class _ConvBnReluPool(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, training, group, out_nchw, impl):
+    def forward(ctx, x, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, training, group, out_nchw):
         xh = _to_nhwc(x)
         C = w.shape[0]
         if training:
-            y, stats = _C.conv5x5_fwd(xh, w, b, True, impl, group is not None)
+            y, stats = _C.conv5x5_fwd(xh, w, b, True, group is not None)
             if group is not None:
                 _inline_allreduce(group, _padded_stats(stats))   # Σy, Σy², n across the group: SyncBatchNorm
             out, saved = _C.bn_relu_pool_fwd(y, stats, gamma, beta, running_mean, running_var, nbt, momentum, eps, out_nchw)
             count = stats[2 * C:2 * C + 1]
         else:
-            y, _ = _C.conv5x5_fwd(xh, w, b, False, impl)
+            y, _ = _C.conv5x5_fwd(xh, w, b, False)
             # the running mean and variance as they are: no round trip through sums, which would cancel the variance's digits
             out, saved = _C.bn_relu_pool_fwd(y, torch.cat([running_mean, running_var]), gamma, beta, None, None, None, 0.0, eps, out_nchw,
                                              mean_var=True)
             count = None   # backward through eval-mode BatchNorm is refused below
         ctx.save_for_backward(xh, w, y, saved, gamma, beta, count)
-        ctx.group, ctx.out_nchw, ctx.impl, ctx.training = group, out_nchw, impl, training
+        ctx.group, ctx.out_nchw, ctx.training = group, out_nchw, training
         ctx.params = (w, b, gamma, beta)
         ctx.x_is_image = x.shape[1] == 1
         ctx.x_shape = x.shape
@@ -109,11 +109,11 @@ class _ConvBnReluPool(torch.autograd.Function):
         dy = _C.bn_relu_pool_bwd_apply(d, y, saved, gamma, beta, sums, count, ctx.out_nchw)
         dw = _grad_dst(w_p, w)
         db = _grad_dst(b_p, w.new_empty(w.shape[0])) if b_p is not None else None
-        _C.conv5x5_wgrad(dy, xh, dw, db, ctx.impl)
+        _C.conv5x5_wgrad(dy, xh, dw, db)
         dx = None
         if ctx.needs_input_grad[0]:
-            dx = _C.conv5x5_dgrad(dy, w, ctx.impl).permute(0, 3, 1, 2)
-        return dx, dw, db, (dgamma if g_p is not None else None), (dbeta if be_p is not None else None), None, None, None, None, None, None, None, None, None
+            dx = _C.conv5x5_dgrad(dy, w).permute(0, 3, 1, 2)
+        return dx, dw, db, (dgamma if g_p is not None else None), (dbeta if be_p is not None else None), None, None, None, None, None, None, None, None
 
 
 # =====================================================================================================
@@ -429,15 +429,18 @@ def _rider_spec_ok(spec: tuple, fcw: torch.Tensor) -> bool:
             and (w is None or (w.dtype == torch.float32 and w.is_contiguous() and w.shape == (fcw.shape[0],) and w.device == fcw.device)))
 
 
-def conv_bn_relu_pool(x: torch.Tensor, conv: torch.nn.Conv2d, bn: torch.nn.Module, out_nchw: Optional[bool] = None,
-                      impl: str = "auto") -> torch.Tensor:
+def conv_bn_relu_pool(x: torch.Tensor, conv: torch.nn.Conv2d, bn: torch.nn.Module, out_nchw: Optional[bool] = None) -> torch.Tensor:
     """Conv5×5(pad 2) → BatchNorm (batch stats, optionally synchronised) → ReLU → MaxPool2×2 as two
     kernels forward / four backward (ref layers: ddp_example.py:25-33).  ``padding="same"`` is pad 2 for a 5×5 kernel."""
     if (conv.kernel_size != (5, 5) or conv.stride != (1, 1) or conv.padding not in ((2, 2), "same") or conv.dilation != (1, 1)
             or conv.groups != 1 or conv.padding_mode != "zeros"):
         raise ValueError("conv_bn_relu_pool: only 5x5 / stride 1 / pad 2 / undilated / zero-padded convolutions are fused")
-    if impl == "auto":
-        impl = os.environ.get("PDT_CONV_IMPL", "auto")  # auto = tensor cores where implemented, SIMT elsewhere
+    # A PDT_CONV_IMPL that names another conv2 kernel (as bench.py --conv-impl does) is refused rather than ignored, so that no
+    # run reports TMA-im2col numbers under another kernel's name.
+    conv_impl = os.environ.get("PDT_CONV_IMPL", "auto")
+    if conv_impl not in ("auto", "tma"):
+        raise ValueError(f"PDT_CONV_IMPL={conv_impl!r}: the per-op conv2 always runs the TMA-im2col kernels now; "
+                         "unset PDT_CONV_IMPL or set it to 'auto' or 'tma'")
     group = None
     training = bn.training
     if training and type(bn).__name__ == "SyncBatchNorm" and dist.is_initialized():
@@ -452,34 +455,7 @@ def conv_bn_relu_pool(x: torch.Tensor, conv: torch.nn.Conv2d, bn: torch.nn.Modul
     track = bn.track_running_stats
     return _ConvBnReluPool.apply(x, conv.weight, conv.bias, bn.weight, bn.bias, bn.running_mean if track else None,
                                  bn.running_var if track else None, bn.num_batches_tracked if (track and training) else None,
-                                 momentum, bn.eps, training or not track, group, out_nchw, impl)
-
-
-class _Conv5x5(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, w, b, impl):
-        xh = _to_nhwc(x)
-        y, _ = _C.conv5x5_fwd(xh, w, b, False, impl)
-        ctx.save_for_backward(xh, w)
-        ctx.params, ctx.impl = (w, b), impl
-        return y.permute(0, 3, 1, 2)
-
-    @staticmethod
-    def backward(ctx, dout):
-        xh, w = ctx.saved_tensors
-        w_p, b_p = ctx.params
-        dy = dout.permute(0, 2, 3, 1).contiguous()
-        dw = _grad_dst(w_p, w)
-        db = _grad_dst(b_p, w.new_empty(w.shape[0])) if b_p is not None else None
-        _C.conv5x5_wgrad(dy, xh, dw, db, ctx.impl)
-        dx = _C.conv5x5_dgrad(dy, w, ctx.impl).permute(0, 3, 1, 2) if ctx.needs_input_grad[0] else None
-        return dx, dw, db, None
-
-
-def conv2d(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None, impl: str = "auto") -> torch.Tensor:
-    """5×5 / stride 1 / pad 2 convolution on our kernels (tensor cores for 16→32 channels); returns a
-    channels_last tensor."""
-    return _Conv5x5.apply(x, weight, bias, impl)
+                                 momentum, bn.eps, training or not track, group, out_nchw)
 
 
 class _Linear(torch.autograd.Function):

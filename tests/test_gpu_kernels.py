@@ -31,82 +31,57 @@ def nhwc(t):
 
 
 def test_native_cuda_runtime_is_loaded():
-    assert ops.native_available() and hasattr(_C, "SymmComm") and hasattr(_C, "gemm_tf32_wgmma")
+    assert ops.native_available() and hasattr(_C, "SymmComm") and hasattr(_C, "convnet_fwd")
     assert torch.cuda.get_device_capability(0) == (9, 0), "these kernels are built for sm_90a only"
 
 
-@pytest.mark.parametrize("M,N,K", [(128, 32, 32), (128, 32, 416), (256, 16, 800), (19600, 32, 416), (1000, 64, 100), (77, 256, 64)])
-def test_gemm_tf32_wgmma(M, N, K):
-    a = torch.randn(M, K, device=dev())
-    b = torch.randn(N, K, device=dev())
-    d = _C.gemm_tf32_wgmma(a, b)
-    ref = a.double() @ b.double().t()
-    err = (d.double() - ref).abs().max().item()
-    scale = ref.abs().max().item()
-    assert err <= 2e-3 * scale + 1e-3, f"tf32 gemm error {err} (scale {scale})"
-    # exactness on tf32-representable inputs: proves operand layout / descriptors, not just "close"
-    ai = torch.randint(-4, 5, (M, K), device=dev()).float()
-    bi = torch.randint(-4, 5, (N, K), device=dev()).float()
-    assert torch.equal(_C.gemm_tf32_wgmma(ai, bi), ai @ bi.t())
-
-
-@pytest.mark.parametrize("cin,cout,H,impl", [(1, 16, 28, "simt"), (16, 32, 14, "simt"), (16, 32, 14, "tcgen05")])
+# the shape picks the kernel: conv1 (1→16) runs on SIMT, conv2 (16→32) on the TMA-im2col wgmma kernel (TF32 operands)
+@pytest.mark.parametrize("cin,cout,H,kernel", [(1, 16, 28, "simt"), (16, 32, 14, "wgmma")])
 @pytest.mark.parametrize("B", [100, 3])
-def test_conv5x5_forward_and_stats(cin, cout, H, impl, B):
+def test_conv5x5_forward_and_stats(cin, cout, H, kernel, B):
     x = torch.randn(B, cin, H, H, device=dev())
     w = torch.randn(cout, cin, 5, 5, device=dev()) * 0.1
     b = torch.randn(cout, device=dev())
-    y, stats = _C.conv5x5_fwd(nhwc(x), w, b, True, impl)
+    y, stats = _C.conv5x5_fwd(nhwc(x), w, b, True)
     # float64 oracle: cuDNN's fp32 algorithms are not all IEEE-accurate at this size
     ref = F.conv2d(x.double(), w.double(), b.double(), padding=2).float()
-    tol = 2e-2 if impl == "tcgen05" else 1e-4
+    tol = 2e-2 if kernel == "wgmma" else 1e-4
     assert torch.allclose(y.permute(0, 3, 1, 2), ref, atol=tol, rtol=tol), (y.permute(0, 3, 1, 2) - ref).abs().max()
     yn = y.double()
     assert torch.allclose(stats[:cout].double(), yn.sum((0, 1, 2)), rtol=1e-4, atol=1e-2)
     assert torch.allclose(stats[cout:2 * cout].double(), (yn * yn).sum((0, 1, 2)), rtol=1e-4, atol=1e-2)
     assert stats[2 * cout].item() == B * H * H
     # deterministic: bitwise identical on a second run
-    y2, stats2 = _C.conv5x5_fwd(nhwc(x), w, b, True, impl)
+    y2, stats2 = _C.conv5x5_fwd(nhwc(x), w, b, True)
     assert torch.equal(y, y2) and torch.equal(stats, stats2)
-
-
-def test_conv_gather_exact_on_small_integers():
-    x = torch.randint(-3, 4, (5, 16, 14, 14), device=dev()).float()
-    w = torch.randint(-2, 3, (32, 16, 5, 5), device=dev()).float()
-    y, _ = _C.conv5x5_fwd(nhwc(x), w, None, False, "tcgen05")
-    assert torch.equal(y.permute(0, 3, 1, 2), F.conv2d(x, w, padding=2))
-    dy = torch.randint(-3, 4, (5, 32, 14, 14), device=dev()).float()
-    dx = _C.conv5x5_dgrad(nhwc(dy), w, "tcgen05")
-    ref = torch.autograd.grad(F.conv2d(x.requires_grad_(), w, padding=2), x, dy)[0]
-    assert torch.equal(dx.permute(0, 3, 1, 2), ref)
-    # weight/bias gradient: MN-major operands (mma.sync), "ones" column for db
-    wd = w.double().requires_grad_()
-    bd = torch.zeros(32, dtype=torch.float64, device=dev(), requires_grad=True)
-    gw, gb = torch.autograd.grad(F.conv2d(x.detach().double(), wd, bd, padding=2), (wd, bd), dy.double())
-    dw, db = torch.empty_like(w), torch.empty(32, device=dev())
-    _C.conv5x5_wgrad(nhwc(dy), nhwc(x.detach()), dw, db, "tcgen05")
-    assert torch.equal(dw.double(), gw) and torch.equal(db.double(), gb)
 
 
 @pytest.mark.parametrize("B", [5, 100])
 def test_conv_tma_im2col_exact(B):
-    """Fully TMA-fed variant: one im2col bulk-tensor load per filter tap (fwd: SWIZZLE_64B rows, dgrad: 128B)."""
+    """conv2's per-op kernels on TF32-representable integers, so every product and sum is exact: the TMA-im2col forward
+    (SWIZZLE_64B rows, bias, Σy) and data gradient (SWIZZLE_128B rows), and the mma.sync weight gradient (MN-major operands)
+    with the bias gradient from its im2col column of ones."""
     x = torch.randint(-3, 4, (B, 16, 14, 14), device=dev()).float()
     w = torch.randint(-2, 3, (32, 16, 5, 5), device=dev()).float()
     b = torch.randint(-2, 3, (32,), device=dev()).float()
-    y, stats = _C.conv5x5_fwd(nhwc(x), w, b, True, "tma")
+    y, stats = _C.conv5x5_fwd(nhwc(x), w, b, True)
     ref = F.conv2d(x.double(), w.double(), b.double(), padding=2)
     assert torch.equal(y.permute(0, 3, 1, 2).double(), ref)
     assert torch.equal(stats[:32].double(), ref.sum((0, 2, 3))) and stats[64].item() == B * 196
     dy = torch.randint(-3, 4, (B, 32, 14, 14), device=dev()).float()
-    dx = _C.conv5x5_dgrad(nhwc(dy), w, "tma")
+    dx = _C.conv5x5_dgrad(nhwc(dy), w)
     xd = x.double().requires_grad_()
     gx = torch.autograd.grad(F.conv2d(xd, w.double(), padding=2), xd, dy.double())[0]
     assert torch.equal(dx.permute(0, 3, 1, 2).double(), gx)
+    wd = w.double().requires_grad_()
+    bd = torch.zeros(32, dtype=torch.float64, device=dev(), requires_grad=True)
+    gw, gb = torch.autograd.grad(F.conv2d(x.double(), wd, bd, padding=2), (wd, bd), dy.double())
+    dw, db = torch.empty_like(w), torch.empty(32, device=dev())
+    _C.conv5x5_wgrad(nhwc(dy), nhwc(x), dw, db)
+    assert torch.equal(dw.double(), gw) and torch.equal(db.double(), gb)
 
 
-@pytest.mark.parametrize("impl", ["simt", "tcgen05"])
-def test_conv5x5_backward(impl):
+def test_conv5x5_backward():
     B = 100
     x = torch.randn(B, 16, 14, 14, device=dev(), requires_grad=True)
     w = (torch.randn(32, 16, 5, 5, device=dev()) * 0.1).requires_grad_()
@@ -114,15 +89,13 @@ def test_conv5x5_backward(impl):
     dy = torch.randn(B, 32, 14, 14, device=dev())
     xd, wd, bd = (t.detach().double().requires_grad_() for t in (x, w, b))
     gx, gw, gb = (g.float() for g in torch.autograd.grad(F.conv2d(xd, wd, bd, padding=2), (xd, wd, bd), dy.double()))
-    dx = _C.conv5x5_dgrad(nhwc(dy), w.detach(), impl)
-    tol = 3e-2 if impl == "tcgen05" else 2e-4
-    assert torch.allclose(dx.permute(0, 3, 1, 2), gx, atol=tol, rtol=tol)
+    dx = _C.conv5x5_dgrad(nhwc(dy), w.detach())
+    assert torch.allclose(dx.permute(0, 3, 1, 2), gx, atol=3e-2, rtol=3e-2)
     dw, db = torch.empty_like(w), torch.empty_like(b)
-    _C.conv5x5_wgrad(nhwc(dy), nhwc(x.detach()), dw, db, impl)
+    _C.conv5x5_wgrad(nhwc(dy), nhwc(x.detach()), dw, db)
     # TF32 operands: ~1e-3 relative per product, random-walk over 19,600 pixels
-    wa, wr = (1.0, 5e-3) if impl == "tcgen05" else (1e-2, 1e-3)
-    assert torch.allclose(dw, gw, atol=wa, rtol=wr), (dw - gw).abs().max()
-    assert torch.allclose(db, gb, atol=wa, rtol=wr), (db - gb).abs().max()
+    assert torch.allclose(dw, gw, atol=1.0, rtol=5e-3), (dw - gw).abs().max()
+    assert torch.allclose(db, gb, atol=1.0, rtol=5e-3), (db - gb).abs().max()
     # conv1 weight gradient (no data gradient: the input needs none)
     x1 = torch.randn(B, 1, 28, 28, device=dev())
     w1 = torch.randn(16, 1, 5, 5, device=dev(), requires_grad=True)
@@ -131,7 +104,7 @@ def test_conv5x5_backward(impl):
     w1d, b1d = w1.detach().double().requires_grad_(), b1.detach().double().requires_grad_()
     gw1, gb1 = (g.float() for g in torch.autograd.grad(F.conv2d(x1.double(), w1d, b1d, padding=2), (w1d, b1d), dy1.double()))
     dw1, db1 = torch.empty_like(w1), torch.empty_like(b1)
-    _C.conv5x5_wgrad(nhwc(dy1), nhwc(x1), dw1, db1, "simt")
+    _C.conv5x5_wgrad(nhwc(dy1), nhwc(x1), dw1, db1)
     assert torch.allclose(dw1, gw1, atol=5e-3, rtol=1e-3) and torch.allclose(db1, gb1, atol=5e-3, rtol=1e-4)
 
 

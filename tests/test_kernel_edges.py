@@ -94,14 +94,14 @@ def test_conv1_statistics_fold_beyond_512_groups(B):
     x = torch.rand(B, 1, 28, 28, device=dev())
     w = torch.randn(16, 1, 5, 5, device=dev()) * 0.2
     b = torch.randn(16, device=dev()) * 0.1
-    y, stats = _C.conv5x5_fwd(nhwc(x), w, b, True, "simt")
+    y, stats = _C.conv5x5_fwd(nhwc(x), w, b, True)
     ref = F.conv2d(x.double(), w.double(), b.double(), padding=2)
     assert torch.allclose(y.permute(0, 3, 1, 2).double(), ref, atol=1e-5, rtol=1e-5), (y.permute(0, 3, 1, 2).double() - ref).abs().max()
     yd = y.double()
     _assert_sums(stats[:16], yd, (0, 1, 2), "Σy")
     _assert_sums(stats[16:32], yd * yd, (0, 1, 2), "Σy²")
     assert stats[32].item() == B * 784
-    y2, stats2 = _C.conv5x5_fwd(nhwc(x), w, b, True, "simt")
+    y2, stats2 = _C.conv5x5_fwd(nhwc(x), w, b, True)
     assert torch.equal(y, y2) and torch.equal(stats, stats2)
     _assert_fused_matches_per_op()
 

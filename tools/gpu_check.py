@@ -13,11 +13,9 @@ os.makedirs(OUT, exist_ok=True)
 
 GROUPS = {
     "loaded": ["tests/test_gpu_kernels.py::test_native_cuda_runtime_is_loaded"],
-    "gemm": ["tests/test_gpu_kernels.py::test_gemm_tf32_wgmma"],
     "conv_fwd": ["tests/test_gpu_kernels.py::test_conv5x5_forward_and_stats"],
-    "conv_exact": ["tests/test_gpu_kernels.py::test_conv_gather_exact_on_small_integers"],
+    "conv_exact": ["tests/test_gpu_kernels.py::test_conv_tma_im2col_exact"],
     "conv_bwd": ["tests/test_gpu_kernels.py::test_conv5x5_backward"],
-    "conv_tma": ["tests/test_gpu_kernels.py::test_conv_tma_im2col_exact"],
     "bn_pool": ["tests/test_gpu_kernels.py::test_bn_relu_pool_forward_backward", "tests/test_gpu_kernels.py::test_generic_bn_kernels_match_torch"],
     "head_sgd": ["tests/test_gpu_kernels.py::test_linear_and_cross_entropy", "tests/test_gpu_kernels.py::test_fused_sgd_matches_torch"],
     "convnet": ["tests/test_gpu_kernels.py::test_convnet_fused_matches_unfused"],
