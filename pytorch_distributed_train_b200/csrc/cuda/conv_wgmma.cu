@@ -5,7 +5,7 @@
 //    N = output channels, K = 25 taps × input channels.  The im2col A-tile of every filter tap is one
 //    cp.async.bulk.tensor im2col load (the TMA unit zero-fills the padding halo), the repacked weights (B) are TMA-loaded
 //    once per CTA and stay resident in smem, and one warpgroup issues wgmma.mma_async ... .tf32 with the fp32 accumulator
-//    in its registers.  The forward epilogue adds the bias, folds the per-channel Σy/Σy² that BatchNorm needs (saving a
+//    in its registers.  The forward epilogue adds the bias, folds the per-channel statistics BatchNorm needs (saving a
 //    full re-read of y) and writes the tile with a TMA store.
 //  * conv5x5_wgrad_mma_kernel — weight and bias gradient: persistent split-K over pixel tiles on warp-level mma.sync (both
 //    operands are MN-major, which TF32 wgmma does not accept); wgrad_fold_kernel then sums the per-CTA partials in a fixed
@@ -75,8 +75,8 @@ struct ConvTmaCfg {
 template <int CK, int NOUT, bool FWD>
 __global__ void __launch_bounds__(160, 1) conv5x5_wgmma_im2col_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_b,
                                                                   const __grid_constant__ CUtensorMap tm_y, const float* __restrict__ bias,
-                                                                  float* __restrict__ y, float* stats, ReduceScratch scr, int B, int H, int W,
-                                                                  int num_tiles) {
+                                                                  float* __restrict__ y, float* stats, int centred, ReduceScratch scr, int B,
+                                                                  int H, int W, int num_tiles) {
   using Cfg = ConvTmaCfg<CK, NOUT>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -179,13 +179,19 @@ __global__ void __launch_bounds__(160, 1) conv5x5_wgmma_im2col_kernel(const __gr
           tma_store_commit();
         }
         if (stats) {
-          float s1 = 0.f, s2 = 0.f;
+          // the tile's per-channel sums of d = y − K and d² over its valid rows (rows past M are zeros in sy); lane = channel.
+          // K = 0 gives Σy and Σy².  Centred, K is the tile's first row, and the tile's M2 = Σd² − (Σd)²/n then cancels only in
+          // proportion to ((mean − K)/std)², a property of the data's spread rather than of the size of its mean
           const int q = lane >> 2, e = lane & 3;
           const int w4 = et >> 5;  // 0..3: rows 32*w4 .. 32*w4+31
+          const int nvalid = min(kTileM, M - tile * kTileM);
+          const float K = centred ? reinterpret_cast<const float*>(sy + (q << 4))[e] : 0.f;
+          float s1 = 0.f, s2 = 0.f;
           for (int rr = w4 * 32; rr < w4 * 32 + 32; ++rr) {
             const float val = reinterpret_cast<const float*>(sy + rr * 128 + ((q ^ (rr & 7)) << 4))[e];
-            s1 += val;
-            s2 += val * val;
+            const float d = rr < nvalid ? val - K : 0.f;
+            s1 += d;
+            s2 += d * d;
           }
           s_part[w4 * 2 * NOUT + lane] = s1;
           s_part[w4 * 2 * NOUT + NOUT + lane] = s2;
@@ -193,10 +199,25 @@ __global__ void __launch_bounds__(160, 1) conv5x5_wgmma_im2col_kernel(const __gr
           float* tile_sums = s_part + 8 * NOUT;
           if (et < 2 * NOUT) tile_sums[et] = s_part[et] + s_part[2 * NOUT + et] + s_part[4 * NOUT + et] + s_part[6 * NOUT + et];
           asm volatile("bar.sync 1, 128;" ::: "memory");
-          grid_fold(tile_sums, 2 * NOUT, tile, num_tiles, scr, s_part, &s_last, et, 128, NamedSync<1, 128>{}, [&](int i, float tot) {
-            stats[i] = tot;
-            if (i == 0) stats[2 * NOUT] = static_cast<float>(M);
-          });
+          if (centred) {
+            if (et < NOUT) {   // [Σd, Σd²] → [Σy, M2] (thread et < 32 holds channel et's K)
+              const float sd = tile_sums[et], n = static_cast<float>(nvalid);
+              tile_sums[NOUT + et] = fmaxf(tile_sums[NOUT + et] - sd * sd / n, 0.f);
+              tile_sums[et] = fmaf(n, K, sd);
+            }
+            asm volatile("bar.sync 1, 128;" ::: "memory");
+            grid_fold_centred(tile_sums, NOUT, kTileM, M, tile, num_tiles, scr, s_part, &s_last, et, 128, NamedSync<1, 128>{},
+                              [&](int i, float mean, float m2) {
+                                stats[i] = mean;
+                                stats[NOUT + i] = m2;
+                                if (i == 0) stats[2 * NOUT] = static_cast<float>(M);
+                              });
+          } else {
+            grid_fold(tile_sums, 2 * NOUT, tile, num_tiles, scr, s_part, &s_last, et, 128, NamedSync<1, 128>{}, [&](int i, float tot) {
+              stats[i] = tot;
+              if (i == 0) stats[2 * NOUT] = static_cast<float>(M);
+            });
+          }
         }
         if (et == 0) tma_store_wait_read();
       } else {
@@ -443,8 +464,8 @@ float* repack_buffer(int slot_id, size_t floats) {
 
 bool conv_wgmma_supported(const ConvShape& s) { return s.Cin == 16 && s.Cout == 32; }
 
-void launch_conv5x5_fwd_im2col(const float* x, const float* w, const float* bias, float* y, float* stats, ConvShape s, ReduceScratch scr,
-                               cudaStream_t st) {
+void launch_conv5x5_fwd_im2col(const float* x, const float* w, const float* bias, float* y, float* stats, bool centred, ConvShape s,
+                               ReduceScratch scr, cudaStream_t st) {
   if (!conv_wgmma_supported(s)) throw std::invalid_argument("conv5x5 im2col: only 16→32 channels are implemented");
   using Cfg = ConvTmaCfg<16, 32>;
   const int M = s.B * s.H * s.W;
@@ -460,7 +481,7 @@ void launch_conv5x5_fwd_im2col(const float* x, const float* w, const float* bias
   auto kern = conv5x5_wgmma_im2col_kernel<16, 32, true>;
   opt_in_smem(kern, Cfg::kSmem);
   const int grid = std::min(tiles, sm_count());
-  kern<<<grid, Cfg::kThreads, Cfg::kSmem, st>>>(tm_x, tm_b, tm_y, bias, y, stats, scr, s.B, s.H, s.W, tiles);
+  kern<<<grid, Cfg::kThreads, Cfg::kSmem, st>>>(tm_x, tm_b, tm_y, bias, y, stats, centred ? 1 : 0, scr, s.B, s.H, s.W, tiles);
   check_launch("conv5x5_wgmma_im2col(fwd)");
 }
 
@@ -477,7 +498,7 @@ void launch_conv5x5_dgrad_im2col(const float* dy, const float* w, float* dx, Con
   auto kern = conv5x5_wgmma_im2col_kernel<32, 16, false>;
   opt_in_smem(kern, Cfg::kSmem);
   const int grid = std::min(tiles, sm_count());
-  kern<<<grid, Cfg::kThreads, Cfg::kSmem, st>>>(tm_x, tm_b, tm_b, nullptr, dx, nullptr, ReduceScratch{}, s.B, s.H, s.W, tiles);
+  kern<<<grid, Cfg::kThreads, Cfg::kSmem, st>>>(tm_x, tm_b, tm_b, nullptr, dx, nullptr, 0, ReduceScratch{}, s.B, s.H, s.W, tiles);
   check_launch("conv5x5_wgmma_im2col(dgrad)");
 }
 

@@ -357,7 +357,10 @@ void register_cuda_bindings(py::module_& m) {
   // The shape picks the kernels: conv2 (16→32) runs on the tensor cores (TMA-im2col wgmma forward and data gradient, mma.sync
   // weight gradient), every other shape on the SIMT forward and weight gradient, which cover conv1 (1→16) and refuse the rest.
   // Only conv2 has a data gradient: conv1's input needs none.
-  m.def("conv5x5_fwd", [](const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> bias, bool want_stats, bool zero_pad) {
+  // centred: stats = [mean, M2, n] (ops_kernels.h), without the cancellation of Σy² when |mean| ≫ std; the default [Σ, Σ², n] is what
+  // SyncBatchNorm all-reduces
+  m.def("conv5x5_fwd", [](const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> bias, bool want_stats, bool zero_pad,
+                          bool centred) {
     chk(x, "x"); chk(w, "w");
     c10::cuda::CUDAGuard g(x.device());
     ConvShape s = conv_shape(x, w);
@@ -369,10 +372,11 @@ void register_cuda_bindings(py::module_& m) {
     at::Tensor stats_full = !want_stats ? at::Tensor() : (zero_pad ? at::zeros({2 * s.Cout + 4}, x.options()) : at::empty({2 * s.Cout + 4}, x.options()));
     at::Tensor stats = want_stats ? stats_full.narrow(0, 0, 2 * s.Cout + 1) : at::Tensor();
     auto launch = conv_wgmma_supported(s) ? launch_conv5x5_fwd_im2col : launch_conv5x5_fwd;
-    launch(x.data_ptr<float>(), w.data_ptr<float>(), opt_ptr(bias, "bias"), y.data_ptr<float>(), want_stats ? stats.data_ptr<float>() : nullptr, s,
-           scratch(x), cur_stream(x));
+    launch(x.data_ptr<float>(), w.data_ptr<float>(), opt_ptr(bias, "bias"), y.data_ptr<float>(), want_stats ? stats.data_ptr<float>() : nullptr,
+           centred, s, scratch(x), cur_stream(x));
     return py::make_tuple(y, stats);  // stats is a view of the first 2C+1 entries of the zero-padded vector
-  }, py::arg("x"), py::arg("w"), py::arg("bias") = py::none(), py::arg("want_stats") = true, py::arg("zero_pad") = false);
+  }, py::arg("x"), py::arg("w"), py::arg("bias") = py::none(), py::arg("want_stats") = true, py::arg("zero_pad") = false,
+     py::arg("centred") = false);
 
   m.def("conv5x5_dgrad", [](const at::Tensor& dy, const at::Tensor& w) {
     chk(dy, "dy"); chk(w, "w");
@@ -568,11 +572,12 @@ void register_cuda_bindings(py::module_& m) {
   // ---- BN + ReLU + pool ------------------------------------------------------------------------------
   m.def("bn_relu_pool_fwd", [](const at::Tensor& y, const at::Tensor& stats, c10::optional<at::Tensor> gamma, c10::optional<at::Tensor> beta,
                                c10::optional<at::Tensor> running_mean, c10::optional<at::Tensor> running_var,
-                               c10::optional<at::Tensor> nbt, double momentum, double eps, bool out_nchw, bool mean_var) {
+                               c10::optional<at::Tensor> nbt, double momentum, double eps, bool out_nchw, bool mean_var, bool centred) {
     chk(y, "y"); chk(stats, "stats");
     c10::cuda::CUDAGuard g(y.device());
     TORCH_CHECK(y.dim() == 4, "bn_relu_pool_fwd: y [B,H,W,C] expected");
     const int B = y.size(0), H = y.size(1), W = y.size(2), C = y.size(3);
+    TORCH_CHECK(!(mean_var && centred), "bn_relu_pool_fwd: stats are either mean_var or centred");
     if (mean_var) {
       TORCH_CHECK(stats.numel() == 2 * C, "bn_relu_pool_fwd: mean_var stats must have 2C entries (mean, var)");
       TORCH_CHECK(!(running_mean.has_value() && running_mean->defined()) && !(running_var.has_value() && running_var->defined()) &&
@@ -586,10 +591,11 @@ void register_cuda_bindings(py::module_& m) {
     if (nbt.has_value() && nbt->defined()) { chk(*nbt, "num_batches_tracked", at::kLong); nbt_p = reinterpret_cast<long long*>(nbt->data_ptr<int64_t>()); }
     launch_bn_relu_pool_fwd(y.data_ptr<float>(), stats.data_ptr<float>(), opt_ptr(gamma, "gamma"), opt_ptr(beta, "beta"), out.data_ptr<float>(),
                             saved.data_ptr<float>(), opt_mut(running_mean, "running_mean"), opt_mut(running_var, "running_var"), nbt_p,
-                            static_cast<float>(momentum), static_cast<float>(eps), B, H, W, C, out_nchw, mean_var, cur_stream(y));
+                            static_cast<float>(momentum), static_cast<float>(eps), B, H, W, C, out_nchw,
+                            mean_var ? kBnMeanVar : centred ? kBnCentred : kBnSums, cur_stream(y));
     return py::make_tuple(out, saved);
   }, py::arg("y"), py::arg("stats"), py::arg("gamma"), py::arg("beta"), py::arg("running_mean"), py::arg("running_var"), py::arg("nbt"),
-     py::arg("momentum"), py::arg("eps"), py::arg("out_nchw"), py::arg("mean_var") = false);
+     py::arg("momentum"), py::arg("eps"), py::arg("out_nchw"), py::arg("mean_var") = false, py::arg("centred") = false);
   m.def("bn_relu_pool_bwd_reduce", [](const at::Tensor& dout, const at::Tensor& y, const at::Tensor& saved, c10::optional<at::Tensor> gamma,
                                       c10::optional<at::Tensor> beta, bool dout_nchw, c10::optional<at::Tensor> dgamma_out,
                                       c10::optional<at::Tensor> dbeta_out) {

@@ -6,7 +6,7 @@
 // Σdz, Σdz·x̂ sums (backward) and the folds of the weight gradients — are device-side grid barriers in the middle of a
 // kernel instead of kernel boundaries.  A training step is three launches:
 //
-//   convnet_fwd_kernel         conv1 5x5 (1→16) ──barrier (Σy, Σy²)── BN + ReLU + MaxPool2 written straight into conv2's
+//   convnet_fwd_kernel         conv1 5x5 (1→16) ──barrier (Σy, M2)── BN + ReLU + MaxPool2 written straight into conv2's
 //                              swizzled smem patch ── conv2 5x5 (16→32) on wgmma (the 25 taps are row-shifted descriptors
 //                              into that patch; accumulators in registers) ──barrier── BN + ReLU + MaxPool2 + classifier
 //                              (+ cross-entropy term and d(loss)/d(logits) when the targets are known)           (ref :25-34,40)
@@ -127,6 +127,97 @@ __device__ __forceinline__ void warp_transpose_reduce32(float (&v)[32], int lane
   warp_transpose_reduce_step<4>(v, lane);
   warp_transpose_reduce_step<2>(v, lane);
   warp_transpose_reduce_step<1>(v, lane);
+}
+// The same for 16 values (v[16..32) are not read): lanes l and l + 16 both end with Σ_lanes v[l & 15] in v[0].
+__device__ __forceinline__ void warp_transpose_reduce16(float (&v)[32], int lane) {
+  warp_transpose_reduce_step<8>(v, lane);
+  warp_transpose_reduce_step<4>(v, lane);
+  warp_transpose_reduce_step<2>(v, lane);
+  warp_transpose_reduce_step<1>(v, lane);
+  v[0] += __shfl_xor_sync(0xffffffffu, v[0], 16);
+}
+
+// Batch statistics without cancellation.  Each CTA publishes, per channel, the sum of its n_img elements and M2_img, their squared
+// deviations about the CTA's own mean.  The batch's M2 is then exact in form (Chan, Golub & LeVeque):
+//   M2 = Σ_img M2_img + Σ_img d_img² / n_img,   d_img = Σ_img − n_img·mean,   mean = Σ_img Σ_img / (B·n_img),
+// where Σy²/n − mean² in fp32 would lose the variance's digits in proportion to mean²/var (a channel whose mean is 1000 times
+// its spread keeps none).  After the grid barrier every CTA folds the rows [Σ (C) | M2 (C)] in the same fixed order: thread
+// (c, g) sums rows g, g + G, ... of channel c, keeping the first R row sums in registers, so that the deviations d_img from the
+// batch mean need no second trip to L2 for B ≤ R·G (all the rows the cooperative launch can have on an H100).  Σ_img d_img also
+// corrects the mean for the rounding of the first sum, which at large means is worth an ulp.  Leaves the mean in s_stat[0..C)
+// and the biased variance in s_stat[C..2C); s_a, s_b: [THREADS] floats each.
+template <int C, int THREADS, int R>
+__device__ __forceinline__ void fold_centred_stats(const float* __restrict__ partials, int rows, float n_img, float* s_a, float* s_b,
+                                                   float* s_stat) {
+  constexpr int G = THREADS / C;
+  const int tid = threadIdx.x, c = tid % C, g = tid / C;
+  const bool folds = tid < G * C;
+  float sv[R];
+  {
+    float s = 0.f, m = 0.f;
+    if (folds) {
+      float mv[R];
+#pragma unroll
+      for (int j = 0; j < R; ++j) {   // R independent pairs of L2 loads in flight
+        const bool in = g + G * j < rows;
+        sv[j] = in ? __ldcg(partials + static_cast<size_t>(g + G * j) * 2 * C + c) : 0.f;
+        mv[j] = in ? __ldcg(partials + static_cast<size_t>(g + G * j) * 2 * C + C + c) : 0.f;
+      }
+#pragma unroll
+      for (int j = 0; j < R; ++j) {
+        s += sv[j];
+        m += mv[j];
+      }
+      for (int r = g + G * R; r < rows; r += G) {
+        s += __ldcg(partials + static_cast<size_t>(r) * 2 * C + c);
+        m += __ldcg(partials + static_cast<size_t>(r) * 2 * C + C + c);
+      }
+      s_a[tid] = s;
+      s_b[tid] = m;
+    }
+  }
+  __syncthreads();
+  const float cnt = static_cast<float>(rows) * n_img;
+  float m2_rows = 0.f;
+  if (tid < C) {
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < G; ++k) {
+      s += s_a[k * C + tid];
+      m2_rows += s_b[k * C + tid];
+    }
+    s_stat[tid] = s / cnt;
+  }
+  __syncthreads();
+  if (folds) {
+    const float mean = s_stat[c];
+    float ds = 0.f, dq = 0.f;
+#pragma unroll
+    for (int j = 0; j < R; ++j) {
+      const float d = g + G * j < rows ? fmaf(-n_img, mean, sv[j]) : 0.f;
+      ds += d;
+      dq = fmaf(d, d, dq);
+    }
+    for (int r = g + G * R; r < rows; r += G) {
+      const float d = fmaf(-n_img, mean, __ldcg(partials + static_cast<size_t>(r) * 2 * C + c));
+      ds += d;
+      dq = fmaf(d, d, dq);
+    }
+    s_a[tid] = ds;
+    s_b[tid] = dq;
+  }
+  __syncthreads();
+  if (tid < C) {
+    float ds = 0.f, dq = 0.f;
+#pragma unroll
+    for (int k = 0; k < G; ++k) {
+      ds += s_a[k * C + tid];
+      dq += s_b[k * C + tid];
+    }
+    s_stat[tid] += ds / cnt;
+    s_stat[C + tid] = (m2_rows + dq / n_img) / cnt;
+  }
+  __syncthreads();
 }
 
 // =====================================================================================================================
@@ -762,7 +853,7 @@ __device__ __forceinline__ int patch_halo_row(int h) {
 // on two warpgroups at once): 25 taps × 2 K-steps of wgmma m64n32k8 per 64-row half, the two halves independent accumulator
 // chains, the A descriptors row-shifted into the haloed patch.  The accumulators go straight into ys [pixel][32] (bias added;
 // 16-byte chunks rotated by the pixel index, as the column reads that follow expect), and the BatchNorm sums of the kept elements
-// are taken while they are still in registers: s_stat[8 warps][64] gets this warp's Σy (columns 0..31) and Σy² (32..63).
+// are taken while they are still in registers: s_stat[8 warps][32] gets this warp's Σy.
 __device__ __forceinline__ void l2_conv_wgmma(const uint8_t* sa, const uint8_t* sb, const float* __restrict__ bias, float* ys, float* s_stat,
                                               int t, int wt) {
   const uint64_t ad0 = gmma_desc_kmajor<128>(smem_u32(sa)), bd0 = gmma_desc_kmajor<128>(smem_u32(sb));
@@ -788,9 +879,9 @@ __device__ __forceinline__ void l2_conv_wgmma(const uint8_t* sa, const uint8_t* 
   wgmma_commit();
   wgmma_wait<0>();
   // a thread holds 8 columns, c = 8·(e >> 2) + 2·(wt & 3) + (e & 1): sums slot k = 2·(e >> 2) + (e & 1)
-  float s1[8], s2[8];
+  float s1[8];
 #pragma unroll
-  for (int k = 0; k < 8; ++k) s1[k] = s2[k] = 0.f;
+  for (int k = 0; k < 8; ++k) s1[k] = 0.f;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
 #pragma unroll
@@ -802,7 +893,6 @@ __device__ __forceinline__ void l2_conv_wgmma(const uint8_t* sa, const uint8_t* 
         const float v = acc[h][e] + (bias ? __ldg(bias + c) : 0.f);
         ys[pix * 32 + ((((c >> 2) + pix) & 7) << 2) + (c & 3)] = v;
         s1[k] += v;
-        s2[k] = fmaf(v, v, s2[k]);
       }
     }
   }
@@ -810,19 +900,12 @@ __device__ __forceinline__ void l2_conv_wgmma(const uint8_t* sa, const uint8_t* 
 #pragma unroll
   for (int off = 4; off <= 16; off <<= 1)
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      s1[k] += __shfl_xor_sync(0xffffffffu, s1[k], off);
-      s2[k] += __shfl_xor_sync(0xffffffffu, s2[k], off);
-    }
+    for (int k = 0; k < 8; ++k) s1[k] += __shfl_xor_sync(0xffffffffu, s1[k], off);
   const int lane = wt & 31;
   if (lane < 4) {
-    float* row = s_stat + (4 * t + (wt >> 5)) * 64;
+    float* row = s_stat + (4 * t + (wt >> 5)) * 32;
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      const int c = 8 * (k >> 1) + 2 * lane + (k & 1);
-      row[c] = s1[k];
-      row[32 + c] = s2[k];
-    }
+    for (int k = 0; k < 8; ++k) row[8 * (k >> 1) + 2 * lane + (k & 1)] = s1[k];
   }
 }
 
@@ -897,16 +980,14 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
   uint8_t* sb = sa + kPatchAlloc;                      // conv2 weights
   float* ys = reinterpret_cast<float*>(sb + L2FwdSmem::kB);
   float* misc = ys + 196 * 32;                         // 1024 floats
-  float* s_part = misc;                                // [8 warps][64] conv2 statistics / [13 warps][16] classifier partials
-  float* s_tot2 = misc + 512;                          // [64]
+  float* s_part = misc;                                // [8 warps][32] conv2 sums / [13 warps][16] classifier partials
   float* s_scale2 = misc + 576;                        // [32]
   float* s_shift2 = misc + 608;                        // [32]
-  float* s_tmp2 = misc + 640;                          // [6][64]
   __shared__ float xs[32 * 32];
   __shared__ __align__(16) float ws[25 * 16];
   __shared__ float red[kFwdWarps * 32];
   __shared__ float s_tmp[kFwdWarps * 32];
-  __shared__ float s_tot[32];
+  __shared__ float s_stat[64];   // an image's means, then the batch's (mean, var): layer 1 in [0, 32), layer 2 in [0, 64)
   __shared__ float s_scale[16], s_shift[16];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = blockIdx.x, B = gridDim.x;
   // pixel d of windows win and win + 98; the threads past kFwdPix own none (L1Map(784) is not valid)
@@ -962,22 +1043,39 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
     }
   }
   trace(0, 1);
+  // this image's [Σy (16) | M2 (16)] (fold_centred_stats): Σy first, then the squared deviations about the image's mean
+  {
+    float v[32];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) v[j] = m0.valid ? acc0[j] + acc1[j] : 0.f;
+    warp_transpose_reduce16(v, lane);
+    if (lane < 16) red[warp * 16 + lane] = v[0];
+  }
+  __syncthreads();
+  if (tid < 16) {
+    float s = 0.f;
+#pragma unroll
+    for (int wi = 0; wi < kFwdWarps; ++wi) s += red[wi * 16 + tid];
+    partials[static_cast<size_t>(n) * 32 + tid] = s;
+    s_stat[tid] = s / 784.f;
+  }
+  __syncthreads();
   {
     float v[32];
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
-      v[j] = m0.valid ? acc0[j] + acc1[j] : 0.f;
-      v[16 + j] = m0.valid ? fmaf(acc1[j], acc1[j], acc0[j] * acc0[j]) : 0.f;
+      const float d0 = acc0[j] - s_stat[j], d1 = acc1[j] - s_stat[j];
+      v[j] = m0.valid ? fmaf(d1, d1, d0 * d0) : 0.f;
     }
-    warp_transpose_reduce32(v, lane);
-    red[warp * 32 + lane] = v[0];
+    warp_transpose_reduce16(v, lane);
+    if (lane < 16) red[kFwdWarps * 16 + warp * 16 + lane] = v[0];
   }
   __syncthreads();
-  if (tid < 32) {
+  if (tid < 16) {
     float s = 0.f;
 #pragma unroll
-    for (int wi = 0; wi < kFwdWarps; ++wi) s += red[wi * 32 + tid];
-    partials[static_cast<size_t>(n) * 32 + tid] = s;
+    for (int wi = 0; wi < kFwdWarps; ++wi) s += red[kFwdWarps * 16 + wi * 16 + tid];
+    partials[static_cast<size_t>(n) * 32 + 16 + tid] = s;
   }
   trace(0, 2);
   bar.arrive(gs);
@@ -991,11 +1089,10 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
     reinterpret_cast<float4*>(p1n + patch_halo_row(i >> 2) * 16)[i & 3] = make_float4(0.f, 0.f, 0.f, 0.f);
   bar.wait(gs);
   trace(0, 3);
-  fold_rows_wide<32, kFwdThreads>(partials, B, s_tmp, s_tot);
+  fold_centred_stats<16, kFwdThreads, 6>(partials, B, 784.f, s_tmp, red, s_stat);
   if (tid < 16) {
     const float cnt = static_cast<float>(B) * 784.f;
-    const float mean = s_tot[tid] / cnt;
-    const float var = fmaxf(s_tot[16 + tid] / cnt - mean * mean, 0.f);
+    const float mean = s_stat[tid], var = s_stat[16 + tid];
     const float invstd = rsqrtf(var + eps1);
     const float g = g1 ? g1[tid] : 1.f, b = be1 ? be1[tid] : 0.f;
     s_scale[tid] = g * invstd;
@@ -1023,12 +1120,33 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
   if (wg < 2) l2_conv_wgmma(sa, sb, b2, ys, s_part, wg, tid & 127);
   __syncthreads();
   trace(0, 5);
+  // this image's [Σy (32) | M2 (32)] (fold_centred_stats): Σy from the epilogue, the squared deviations about the image's mean
+  // from ys, 15 or 16 pixels of one channel per thread
   float* partials2 = partials + static_cast<size_t>(B) * 32;
-  if (tid < 64) {
+  if (tid < 32) {
     float s = 0.f;
 #pragma unroll
-    for (int w = 0; w < 8; ++w) s += s_part[w * 64 + tid];
+    for (int w = 0; w < 8; ++w) s += s_part[w * 32 + tid];
     partials2[static_cast<size_t>(n) * 64 + tid] = s;
+    s_stat[tid] = s / 196.f;
+  }
+  __syncthreads();
+  {
+    const int c = lane;
+    const float mu = s_stat[c];
+    float q = 0.f;
+    for (int pix = warp; pix < 196; pix += kFwdWarps) {
+      const float d = ys[pix * 32 + ((((c >> 2) + pix) & 7) << 2) + (c & 3)] - mu;
+      q = fmaf(d, d, q);
+    }
+    red[warp * 32 + lane] = q;
+  }
+  __syncthreads();
+  if (tid < 32) {
+    float s = 0.f;
+#pragma unroll
+    for (int wi = 0; wi < kFwdWarps; ++wi) s += red[wi * 32 + tid];
+    partials2[static_cast<size_t>(n) * 64 + 32 + tid] = s;
   }
   trace(0, 6);
   bar.arrive(gs);
@@ -1073,11 +1191,10 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
   }
   bar.wait(gs);
   trace(0, 7);
-  fold_rows_wide<64, kFwdThreads>(partials2, B, s_tmp2, s_tot2);
+  fold_centred_stats<32, kFwdThreads, 11>(partials2, B, 196.f, s_tmp, red, s_stat);
   if (tid < 32) {
     const float cnt = static_cast<float>(B) * 196.f;
-    const float mean = s_tot2[tid] / cnt;
-    const float var = fmaxf(s_tot2[32 + tid] / cnt - mean * mean, 0.f);
+    const float mean = s_stat[tid], var = s_stat[32 + tid];
     const float invstd = rsqrtf(var + eps2);
     const float g = g2 ? g2[tid] : 1.f, b = be2 ? be2[tid] : 0.f;
     s_scale2[tid] = g * invstd;

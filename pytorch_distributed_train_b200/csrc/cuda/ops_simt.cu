@@ -28,7 +28,8 @@ namespace {
 // =====================================================================================================
 template <int CIN, int COUT, int CPT, int TH, bool STATS>
 __global__ void __launch_bounds__(448) conv5x5_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
-                                                      float* __restrict__ y, float* stats, ReduceScratch scr, int B, int H, int W) {
+                                                      float* __restrict__ y, float* stats, int centred, ReduceScratch scr, int B, int H,
+                                                      int W) {
   constexpr int G = COUT / CPT;
   extern __shared__ __align__(16) float smem[];
   const int PW = W + 4, PH = TH + 4;
@@ -87,10 +88,21 @@ __global__ void __launch_bounds__(448) conv5x5_kernel(const float* __restrict__ 
       *reinterpret_cast<float4*>(yp + j4 * 4) = make_float4(acc[j4 * 4], acc[j4 * 4 + 1], acc[j4 * 4 + 2], acc[j4 * 4 + 3]);
   }
   if constexpr (STATS) {
+    // the CTA's per-channel sums of d = y − K and d²: K = 0 gives Σy and Σy².  Centred, K is the CTA's first pixel, and the
+    // CTA's M2 = Σd² − (Σd)²/n then cancels only in proportion to ((mean − K)/std)², whatever the size of the mean
     const int lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+    float* blk = red + nwarps * 2 * COUT;
+    __shared__ float s_k[COUT];
+    if (centred) {
+      if (pix == 0)
+#pragma unroll
+        for (int j = 0; j < CPT; ++j) s_k[cg * CPT + j] = acc[j];
+      __syncthreads();
+    }
 #pragma unroll
     for (int j = 0; j < CPT; ++j) {
-      float s = valid ? acc[j] : 0.f, q = valid ? acc[j] * acc[j] : 0.f;
+      const float d = centred ? acc[j] - s_k[cg * CPT + j] : acc[j];
+      float s = valid ? d : 0.f, q = valid ? d * d : 0.f;
 #pragma unroll
       for (int off = G; off < 32; off <<= 1) {
         s += __shfl_xor_sync(0xffffffffu, s, off);
@@ -102,20 +114,36 @@ __global__ void __launch_bounds__(448) conv5x5_kernel(const float* __restrict__ 
       }
     }
     __syncthreads();
-    float* blk = red + nwarps * 2 * COUT;
     if (tid < 2 * COUT) {
       float s = 0.f;
       for (int wi = 0; wi < nwarps; ++wi) s += red[wi * 2 * COUT + tid];
       blk[tid] = s;
     }
     __syncthreads();
+    if (centred) {
+      if (tid < COUT) {   // [Σd, Σd²] → [Σy, M2]
+        const float sd = blk[tid], n = static_cast<float>(npix);
+        blk[COUT + tid] = fmaxf(blk[COUT + tid] - sd * sd / n, 0.f);
+        blk[tid] = fmaf(n, s_k[tid], sd);
+      }
+      __syncthreads();
+    }
     const float cnt = static_cast<float>(B) * H * W;
     __shared__ float s_tmp[1024];
     __shared__ int s_flag;
-    grid_fold(blk, 2 * COUT, blockIdx.x, gridDim.x, scr, s_tmp, &s_flag, tid, blockDim.x, CtaSync{}, [&](int i, float v) {
-      stats[i] = v;
-      if (i == 0) stats[2 * COUT] = cnt;
-    });
+    if (centred) {
+      grid_fold_centred(blk, COUT, npix, B * H * W, blockIdx.x, gridDim.x, scr, s_tmp, &s_flag, tid, blockDim.x, CtaSync{},
+                        [&](int i, float mean, float m2) {
+                          stats[i] = mean;
+                          stats[COUT + i] = m2;
+                          if (i == 0) stats[2 * COUT] = cnt;
+                        });
+    } else {
+      grid_fold(blk, 2 * COUT, blockIdx.x, gridDim.x, scr, s_tmp, &s_flag, tid, blockDim.x, CtaSync{}, [&](int i, float v) {
+        stats[i] = v;
+        if (i == 0) stats[2 * COUT] = cnt;
+      });
+    }
   }
 }
 
@@ -229,14 +257,20 @@ __global__ void __launch_bounds__(256) fold_partials_kernel(const float* __restr
 // =====================================================================================================
 // BatchNorm(train) + ReLU + MaxPool 2x2
 // =====================================================================================================
-// mean_var: stats = [mean, var] as they are (eval mode), not [Σ, Σ², n]: rebuilding var = E[y²] − mean² from running statistics
-// would cancel away the variance's digits when |mean| ≫ std
-__device__ __forceinline__ void bn_coeffs(const float* stats, const float* gamma, const float* beta, float eps, int C, int mean_var,
+// The batch variance (biased) from stats in the form `form` (BnStats).  kBnSums' E[y²] − mean² cancels the variance's digits when
+// |mean| ≫ std; it is kept for SyncBatchNorm, whose all-reduce can sum Σ and Σ² across GPUs but not M2.  The centred form (M2
+// about the mean) and the eval form (the running statistics as they are) have no such cancellation.
+__device__ __forceinline__ float bn_stats_var(const float* stats, int C, int c, int form, float mean) {
+  if (form == kBnMeanVar) return stats[C + c];
+  const float n = fmaxf(stats[2 * C], 1.f);
+  return form == kBnCentred ? stats[C + c] / n : fmaxf(stats[C + c] / n - mean * mean, 0.f);
+}
+
+__device__ __forceinline__ void bn_coeffs(const float* stats, const float* gamma, const float* beta, float eps, int C, int form,
                                           float* s_scale, float* s_shift, float* s_mean, float* s_invstd) {
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    const float n = mean_var ? 1.f : fmaxf(stats[2 * C], 1.f);
-    const float mean = mean_var ? stats[c] : stats[c] / n;
-    const float var = mean_var ? stats[C + c] : fmaxf(stats[C + c] / n - mean * mean, 0.f);
+    const float mean = form == kBnSums ? stats[c] / fmaxf(stats[2 * C], 1.f) : stats[c];
+    const float var = bn_stats_var(stats, C, c, form, mean);
     const float invstd = rsqrtf(var + eps);
     const float g = gamma ? gamma[c] : 1.f, b = beta ? beta[c] : 0.f;
     s_mean[c] = mean;
@@ -250,9 +284,9 @@ __global__ void __launch_bounds__(256) bn_relu_pool_fwd_kernel(const float* __re
                                                                const float* __restrict__ gamma, const float* __restrict__ beta,
                                                                float* __restrict__ out, float* saved, float* running_mean,
                                                                float* running_var, long long* nbt, float momentum, float eps, int B,
-                                                               int H, int W, int C, int out_nchw, int mean_var) {
+                                                               int H, int W, int C, int out_nchw, int form) {
   __shared__ float s_scale[64], s_shift[64], s_mean[64], s_invstd[64];
-  bn_coeffs(stats, gamma, beta, eps, C, mean_var, s_scale, s_shift, s_mean, s_invstd);
+  bn_coeffs(stats, gamma, beta, eps, C, form, s_scale, s_shift, s_mean, s_invstd);
   __syncthreads();
   if (blockIdx.x == 0) {
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
@@ -260,7 +294,7 @@ __global__ void __launch_bounds__(256) bn_relu_pool_fwd_kernel(const float* __re
       saved[C + c] = s_invstd[c];
       if (running_mean) {
         const float n = fmaxf(stats[2 * C], 1.f);
-        const float var = fmaxf(stats[C + c] / n - s_mean[c] * s_mean[c], 0.f);
+        const float var = bn_stats_var(stats, C, c, form, s_mean[c]);
         const float unbiased = var * (n / fmaxf(n - 1.f, 1.f));
         running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * s_mean[c];
         running_var[c] = (1.f - momentum) * running_var[c] + momentum * unbiased;
@@ -1017,8 +1051,8 @@ size_t conv_smem(int cin, int cout, int th, int w, int threads) {
 }  // namespace
 
 // ---- launchers ---------------------------------------------------------------------------------------
-void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float* y, float* stats, ConvShape s, ReduceScratch scr,
-                        cudaStream_t st) {
+void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float* y, float* stats, bool centred, ConvShape s,
+                        ReduceScratch scr, cudaStream_t st) {
   constexpr int TH = 7;
   if (!(s.Cin == 1 && s.Cout == 16)) throw std::invalid_argument("conv5x5_fwd: supported channel config is 1→16");
   if (s.H % TH != 0) throw std::invalid_argument("conv5x5_fwd: H must be a multiple of 7");
@@ -1027,8 +1061,8 @@ void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float
     throw std::invalid_argument("conv5x5_fwd: reduction scratch too small");
   const int threads = (TH * s.W + 31) / 32 * 32;
   const size_t sm = conv_smem(1, 16, TH, s.W, threads);
-  if (stats) conv5x5_kernel<1, 16, 16, TH, true><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, scr, s.B, s.H, s.W);
-  else conv5x5_kernel<1, 16, 16, TH, false><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, scr, s.B, s.H, s.W);
+  if (stats) conv5x5_kernel<1, 16, 16, TH, true><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, centred ? 1 : 0, scr, s.B, s.H, s.W);
+  else conv5x5_kernel<1, 16, 16, TH, false><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, 0, scr, s.B, s.H, s.W);
   check_launch("conv5x5_fwd");
 }
 
@@ -1057,12 +1091,12 @@ static void check_bn_relu_pool_shape(int C, int H, int W, const char* what) {
 
 void launch_bn_relu_pool_fwd(const float* y, const float* stats, const float* gamma, const float* beta, float* out, float* saved,
                              float* running_mean, float* running_var, long long* nbt, float momentum, float eps, int B, int H, int W,
-                             int C, bool out_nchw, bool mean_var, cudaStream_t st) {
+                             int C, bool out_nchw, BnStats form, cudaStream_t st) {
   check_bn_relu_pool_shape(C, H, W, "bn_relu_pool_fwd");
   const long long total = static_cast<long long>(B) * (H / 2) * (W / 2) * (C / 4);
   bn_relu_pool_fwd_kernel<<<static_cast<int>((total + 255) / 256), 256, 0, st>>>(y, stats, gamma, beta, out, saved, running_mean, running_var,
                                                                                  nbt, momentum, eps, B, H, W, C, out_nchw ? 1 : 0,
-                                                                                 mean_var ? 1 : 0);
+                                                                                 static_cast<int>(form));
   check_launch("bn_relu_pool_fwd");
 }
 

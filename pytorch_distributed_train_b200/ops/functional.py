@@ -76,10 +76,13 @@ class _ConvBnReluPool(torch.autograd.Function):
         xh = _to_nhwc(x)
         C = w.shape[0]
         if training:
-            y, stats = _C.conv5x5_fwd(xh, w, b, True, group is not None)
+            # one GPU: [mean, M2, n], no cancellation when |mean| ≫ std; SyncBatchNorm: [Σy, Σy², n], which the all-reduce can sum
+            centred = group is None
+            y, stats = _C.conv5x5_fwd(xh, w, b, True, not centred, centred=centred)
             if group is not None:
                 _inline_allreduce(group, _padded_stats(stats))   # Σy, Σy², n across the group: SyncBatchNorm
-            out, saved = _C.bn_relu_pool_fwd(y, stats, gamma, beta, running_mean, running_var, nbt, momentum, eps, out_nchw)
+            out, saved = _C.bn_relu_pool_fwd(y, stats, gamma, beta, running_mean, running_var, nbt, momentum, eps, out_nchw,
+                                             centred=centred)
             count = stats[2 * C:2 * C + 1]
         else:
             y, _ = _C.conv5x5_fwd(xh, w, b, False)
