@@ -399,6 +399,19 @@ void register_cuda_bindings(py::module_& m) {
 
   // ---- cooperative fused ConvNet layers (fused_convnet.cu): one CTA per image, grid barrier for the batch statistics ----
   m.def("fused_convnet_supported", [](int64_t B) { return fused_convnet_supported(static_cast<int>(B)); });
+  // A captured launch with programmatic stream serialization becomes a programmatic edge only when the node before it in the
+  // captured stream is a kernel; behind anything else the capture records a full dependency.
+  m.def("graph_programmatic_edges", [](uintptr_t graph) {
+    auto g = reinterpret_cast<cudaGraph_t>(graph);
+    size_t n = 0;
+    PDT_CUDA_CHECK(cudaGraphGetEdges_v2(g, nullptr, nullptr, nullptr, &n));
+    std::vector<cudaGraphNode_t> from(n), to(n);
+    std::vector<cudaGraphEdgeData> data(n);
+    PDT_CUDA_CHECK(cudaGraphGetEdges_v2(g, from.data(), to.data(), data.data(), &n));
+    int64_t programmatic = 0;
+    for (size_t i = 0; i < n; ++i) programmatic += data[i].type == cudaGraphDependencyTypeProgrammatic ? 1 : 0;
+    return programmatic;
+  }, py::arg("graph"), "number of programmatic-dependency edges of a cudaGraph_t (torch.cuda.CUDAGraph(keep_graph=True).raw_cuda_graph())");
   m.def("fused_convnet_trace_enable", [](bool on) { fused_convnet_trace_enable(on); });
   m.def("fused_convnet_trace_read", [] {
     at::Tensor t = at::zeros({4, 160, 12}, at::kLong);

@@ -80,19 +80,25 @@ void opt_in_smem(K kernel, size_t bytes) {
 }
 
 // Cooperative launch: all CTAs are co-resident, so they may wait for each other at a grid barrier (grid_sync.cuh).
+// programmatic: a programmatic dependent launch — the grid may start before the kernel ahead of it in the stream has finished, once
+// that kernel calls griddep_launch_dependents(); the kernel must call griddep_wait() before it reads anything that kernel wrote
+// (hopper_ptx.cuh), and before it touches a grid-barrier word.
 template <typename... KArgs, typename... Args>
-void launch_cooperative(void (*kernel)(KArgs...), int grid, int block, size_t smem, cudaStream_t st, const char* what, Args&&... args) {
+void launch_cooperative(void (*kernel)(KArgs...), int grid, int block, size_t smem, cudaStream_t st, const char* what, bool programmatic,
+                        Args&&... args) {
   opt_in_smem(kernel, smem);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(block);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute attr[1];
+  cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeCooperative;
   attr[0].val.cooperative = 1;
+  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = 1;
+  cfg.numAttrs = programmatic ? 2 : 1;
   cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
   if (e != cudaSuccess) throw std::runtime_error(std::string("launch of ") + what + " failed: " + cudaGetErrorString(e));
   count_kernel_launch();

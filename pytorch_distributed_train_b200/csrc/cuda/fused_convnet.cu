@@ -21,6 +21,8 @@
 // so results are bit-reproducible and identical in every CTA.  The kernels are launched cooperatively (all CTAs
 // co-resident: one per image, at most one per SM); grid barriers are split into arrive / wait so that independent work
 // (stores nobody in the kernel waits for, cp.async staging, gradient slices) runs in their shadow (grid_sync.cuh).
+// The two backward kernels are programmatic dependent launches: each grid is set up once every CTA of the kernel before it has
+// passed its last grid barrier (griddep_launch_dependents), and waits for that kernel's completion at its top (griddep_wait).
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -492,6 +494,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   float* s_clip = red + 512;   // ClipRider: per-warp norm partials + the coefficient (s_db below takes red[0, 512) only)
 
   const L1Map m(tid);
+  griddep_wait();   // programmatic launch behind the layer-2 backward: everything below reads its outputs or the grid-barrier words
   GridBar bar(gs);
   TRACE_INIT();
   trace(1, 0);
@@ -1079,11 +1082,7 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
   }
   trace(0, 2);
   bar.arrive(gs);
-  // in the barrier's shadow: everything layer 1 owes to global memory (backward reads it; nothing in this kernel does)
-  if (m0.valid) {
-    l1_store_y(y1, n, m0, acc0);
-    l1_store_y(y1, n, m1, acc1);
-  }
+  // in the barrier's shadow: the pooled frame's zero halo (backward reads it; nothing in this kernel does)
   float* p1n = p1 + static_cast<size_t>(n) * 324 * 16;
   for (int i = tid; i < 128 * 4; i += kFwdThreads)
     reinterpret_cast<float4*>(p1n + patch_halo_row(i >> 2) * 16)[i & 3] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -1111,6 +1110,10 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
   __syncthreads();
   l1_pool_store(acc0, m0, s_scale, s_shift, sa, p1n);
   l1_pool_store(acc1, m1, s_scale, s_shift, sa, p1n);
+  if (m0.valid) {   // y1 for the backward pass (nothing in this kernel reads it): drains behind conv2
+    l1_store_y(y1, n, m0, acc0);
+    l1_store_y(y1, n, m1, acc1);
+  }
   cp_async_wait<0>();         // this thread's weight copies have landed
   fence_proxy_async_smem();   // generic-proxy writes of the patch and of the weights → visible to the tensor core
   __syncthreads();
@@ -1190,6 +1193,7 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
     reinterpret_cast<float4*>(y2 + (static_cast<size_t>(n) * 196 + pix) * 32)[q] = reinterpret_cast<const float4*>(ys + pix * 32)[(q + pix) & 7];
   }
   bar.wait(gs);
+  griddep_launch_dependents();   // no CTA waits for another from here on: the layer-2 backward's grid may be set up
   trace(0, 7);
   fold_centred_stats<32, kFwdThreads, 11>(partials2, B, 196.f, s_tmp, red, s_stat);
   if (tid < 32) {
@@ -1465,6 +1469,7 @@ convnet_l2_bwd_kernel(const float* __restrict__ y /*[B,14,14,32]*/,
   uint8_t* s_dyt = smem + L2BwdSmem::kDyT;                      // WG: conv2's dyᵀ
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = blockIdx.x, B = gridDim.x;
 
+  griddep_wait();   // programmatic launch behind the forward: everything below reads its outputs or the grid-barrier words
   GridBar bar(gs);
   TRACE_INIT();
   const bool trace_wg1_ = (threadIdx.x == 128) && (*reinterpret_cast<volatile int*>(&g_trace_on) != 0);   // the data gradient's end
@@ -1635,6 +1640,7 @@ convnet_l2_bwd_kernel(const float* __restrict__ y /*[B,14,14,32]*/,
     }
   }
   bar.wait(gs);
+  griddep_launch_dependents();   // the kernel's only grid barrier is behind it: the layer-1 backward's grid may be set up
   trace(3, 3);
   fold_rows<64>(partials, B, s_tmp, s_tot);
   trace(3, 4);
@@ -1770,7 +1776,7 @@ void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* x
                                  float* dgamma, float* dbeta, float* dw, float* db, const float* wpart, const float* dysum2, float* dw2, float* db2,
                                  int B, float* partials, float* partials_w, GridSync gs, cudaStream_t st, Rider rider, bool accumulate) {
   auto kernel = accumulate ? convnet_l1_bwd_kernel<Rider, true> : convnet_l1_bwd_kernel<Rider>;
-  launch_cooperative(kernel, B, kL1Threads, static_cast<size_t>(kL1BwdSmem), st, "convnet_l1_bwd_wgrad", dp, y, x, saved,
+  launch_cooperative(kernel, B, kL1Threads, static_cast<size_t>(kL1BwdSmem), st, "convnet_l1_bwd_wgrad", true, dp, y, x, saved,
                      gamma, beta, dgamma, dbeta, dw, db, partials, partials_w, gs, wpart, dysum2, dw2, db2, rider);
 }
 #define PDT_L1_BWD_WGRAD(R)                                                                                                            \
@@ -1793,18 +1799,18 @@ void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const 
   if (!(ce.scale > 0.f)) throw std::invalid_argument("convnet_fwd: the cross-entropy scale must be positive");
   if (!(ce.smoothing >= 0.f && ce.smoothing <= 1.f)) throw std::invalid_argument("convnet_fwd: label smoothing must lie in [0, 1]");
   if (ce.target != nullptr && !ce.is_default(ncls)) {
-    launch_cooperative(convnet_fwd_kernel<SmoothCe>, B, kFwdThreads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1,
+    launch_cooperative(convnet_fwd_kernel<SmoothCe>, B, kFwdThreads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", false, x, w1, b1, g1, be1, y1, p1,
                        saved1, rm1, rv1, nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials,
                        gs, ce);
     return;
   }
   if (ce.target != nullptr && ce.scale != 1.f) {
-    launch_cooperative(convnet_fwd_kernel<ScaledCe>, B, kFwdThreads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1,
+    launch_cooperative(convnet_fwd_kernel<ScaledCe>, B, kFwdThreads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", false, x, w1, b1, g1, be1, y1, p1,
                        saved1, rm1, rv1, nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials,
                        gs, static_cast<const ScaledCe&>(ce));
     return;
   }
-  launch_cooperative(convnet_fwd_kernel<FusedCe>, B, kFwdThreads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", x, w1, b1, g1, be1, y1, p1, saved1,
+  launch_cooperative(convnet_fwd_kernel<FusedCe>, B, kFwdThreads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", false, x, w1, b1, g1, be1, y1, p1, saved1,
                      rm1, rv1, nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials, gs,
                      static_cast<const FusedCe&>(ce));
 }
@@ -1818,7 +1824,7 @@ void launch_convnet_l2_bwd_fc(const float* dlogits, const float* fcw, const floa
   if (accumulate && x2 == nullptr) throw std::invalid_argument("convnet_l2_bwd_fc: accumulate mode needs conv2's input frame (x2)");
   auto kernel = accumulate ? convnet_l2_bwd_kernel<true, true> : x2 != nullptr ? convnet_l2_bwd_kernel<true> : convnet_l2_bwd_kernel<false>;
   const int smem = std::max(L2BwdSmem::kTotalFc, L2BwdSmem::kTotalWg);   // every form has the data gradient's edge buffer
-  launch_cooperative(kernel, B, kL2Threads, static_cast<size_t>(smem), st, "convnet_l2_bwd_fc", y, saved, gamma, beta, w, dgamma, dbeta, dy,
+  launch_cooperative(kernel, B, kL2Threads, static_cast<size_t>(smem), st, "convnet_l2_bwd_fc", true, y, saved, gamma, beta, w, dgamma, dbeta, dy,
                      dx, dysum, partials, gs, dlogits, fcw, pooled, dfcw, dfcb, ncls, loss_parts, loss_out, x2, wpart);
 }
 

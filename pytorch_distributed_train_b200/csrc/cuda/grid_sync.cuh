@@ -36,6 +36,10 @@ __device__ __forceinline__ void st_release_gpu(unsigned int* p, unsigned int v) 
 // tracks the epoch locally (read once at kernel start, +1 per barrier): no read of the word before arriving, nothing to
 // reset between launches or CUDA-graph replays, any grid size.  A flag-per-CTA variant (every CTA polling every flag)
 // puts ~10^4 pollers on four cache lines and is slower than the counter.
+// Programmatic dependent launch: a grid launched while the kernel before it still runs touches no grid-barrier word — the
+// constructor's epoch read included — before griddep_wait() (hopper_ptx.cuh).  That kernel may still be passing its own barriers on
+// the same two words: a dependent that read the epoch early would start from a stale value and pass its first barrier on the other
+// kernel's epoch store.
 struct GridBar {
   unsigned int e;
   __device__ __forceinline__ explicit GridBar(GridSync gs) : e(gs.epoch ? *reinterpret_cast<volatile unsigned int*>(gs.epoch) : 0u) {}

@@ -1,5 +1,5 @@
-// Hand-written PTX wrappers for the Hopper data path: mbarrier, TMA (cp.async.bulk.tensor), wgmma and the
-// shared-memory matrix descriptors.  Shared by conv_wgmma.cu and fused_convnet.cu.
+// Hand-written PTX wrappers for the Hopper data path: mbarrier, programmatic dependent launch, TMA (cp.async.bulk.tensor), wgmma
+// and the shared-memory matrix descriptors.  Shared by conv_wgmma.cu and fused_convnet.cu.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -50,6 +50,13 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
+
+// Programmatic dependent launch (launch_cooperative(..., programmatic = true)): the grid may start while the kernel before it in the
+// stream still runs.  griddep_wait() blocks until that kernel has completed and its memory operations are visible;
+// griddep_launch_dependents() lets the next kernel's grid start once every CTA of this one has called it (or exited).  Both are
+// no-ops in a grid launched without a programmatic dependency.
+__device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 // TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {

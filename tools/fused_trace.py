@@ -1,5 +1,6 @@
 """Phase timeline of the cooperative fused ConvNet kernels (globaltimer stamps written by thread 0 of every CTA).
     python tools/fused_trace.py            # one eager training step at batch 100, prints per-phase medians in µs
+Then the same inside the replayed CUDA graph of GraphedTrainStep, and the gap between two replays.
 """
 import os
 import sys
@@ -82,8 +83,25 @@ try:
     torch.cuda.synchronize()
     _C.fused_convnet_trace_enable(True)
     step(x, y)
+    step(x, y)   # the stamps are those of the second replay, which starts behind the first one's last kernel
     t2 = _C.fused_convnet_trace_read()[:, :B, :].double()
     _C.fused_convnet_trace_enable(False)
     report(t2, f"inside the replayed CUDA graph ({step.kernels_per_replay} launches)")
+
+    # The launch cost left between two replays.  The stamps of one replay overwrite the other's, so the gap from the layer-1 backward's
+    # end to the next forward's start is the replay period less the stamped span above.  The period is timed with device events around
+    # back-to-back launches of the captured graphs, without the host work of step() (input staging), so that the host stays ahead.
+    span = (t2[1].max() - t2[0][:, 0].min()).item() / 1e3
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    reps = 2000
+    with torch.cuda.stream(step.capture_stream):
+        ev0.record()
+        for r in range(reps):
+            step.graphs[r % len(step.graphs)].replay()
+        ev1.record()
+    torch.cuda.synchronize()
+    period = ev0.elapsed_time(ev1) * 1e3 / reps
+    print(f"-- replay period {period:.2f} us over {reps} replays; gap l1_bwd -> next replay's forward: {period - span:.2f} us "
+          f"(period - first kernel start -> last kernel end)")
 finally:
     pdt.destroy_process_group()
