@@ -75,7 +75,7 @@ struct ConvTmaCfg {
 template <int CK, int NOUT, bool FWD>
 __global__ void __launch_bounds__(160, 1) conv5x5_wgmma_im2col_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_b,
                                                                   const __grid_constant__ CUtensorMap tm_y, const float* __restrict__ bias,
-                                                                  float* __restrict__ y, float* stats, int centred, ReduceScratch scr, int B,
+                                                                  float* __restrict__ y, void* stats, ConvStats form, ReduceScratch scr, int B,
                                                                   int H, int W, int num_tiles) {
   using Cfg = ConvTmaCfg<CK, NOUT>;
   extern __shared__ uint8_t smem_raw[];
@@ -185,6 +185,7 @@ __global__ void __launch_bounds__(160, 1) conv5x5_wgmma_im2col_kernel(const __gr
           const int q = lane >> 2, e = lane & 3;
           const int w4 = et >> 5;  // 0..3: rows 32*w4 .. 32*w4+31
           const int nvalid = min(kTileM, M - tile * kTileM);
+          const bool centred = form != kConvSums;
           const float K = centred ? reinterpret_cast<const float*>(sy + (q << 4))[e] : 0.f;
           float s1 = 0.f, s2 = 0.f;
           for (int rr = w4 * 32; rr < w4 * 32 + 32; ++rr) {
@@ -207,15 +208,12 @@ __global__ void __launch_bounds__(160, 1) conv5x5_wgmma_im2col_kernel(const __gr
             }
             asm volatile("bar.sync 1, 128;" ::: "memory");
             grid_fold_centred(tile_sums, NOUT, kTileM, M, tile, num_tiles, scr, s_part, &s_last, et, 128, NamedSync<1, 128>{},
-                              [&](int i, float mean, float m2) {
-                                stats[i] = mean;
-                                stats[NOUT + i] = m2;
-                                if (i == 0) stats[2 * NOUT] = static_cast<float>(M);
-                              });
+                              [&](int i, float mean, float m2) { store_centred_stats(stats, form, NOUT, i, mean, m2, static_cast<float>(M)); });
           } else {
+            float* sums = static_cast<float*>(stats);
             grid_fold(tile_sums, 2 * NOUT, tile, num_tiles, scr, s_part, &s_last, et, 128, NamedSync<1, 128>{}, [&](int i, float tot) {
-              stats[i] = tot;
-              if (i == 0) stats[2 * NOUT] = static_cast<float>(M);
+              sums[i] = tot;
+              if (i == 0) sums[2 * NOUT] = static_cast<float>(M);
             });
           }
         }
@@ -464,7 +462,7 @@ float* repack_buffer(int slot_id, size_t floats) {
 
 bool conv_wgmma_supported(const ConvShape& s) { return s.Cin == 16 && s.Cout == 32; }
 
-void launch_conv5x5_fwd_im2col(const float* x, const float* w, const float* bias, float* y, float* stats, bool centred, ConvShape s,
+void launch_conv5x5_fwd_im2col(const float* x, const float* w, const float* bias, float* y, void* stats, ConvStats form, ConvShape s,
                                ReduceScratch scr, cudaStream_t st) {
   if (!conv_wgmma_supported(s)) throw std::invalid_argument("conv5x5 im2col: only 16→32 channels are implemented");
   using Cfg = ConvTmaCfg<16, 32>;
@@ -481,7 +479,7 @@ void launch_conv5x5_fwd_im2col(const float* x, const float* w, const float* bias
   auto kern = conv5x5_wgmma_im2col_kernel<16, 32, true>;
   opt_in_smem(kern, Cfg::kSmem);
   const int grid = std::min(tiles, sm_count());
-  kern<<<grid, Cfg::kThreads, Cfg::kSmem, st>>>(tm_x, tm_b, tm_y, bias, y, stats, centred ? 1 : 0, scr, s.B, s.H, s.W, tiles);
+  kern<<<grid, Cfg::kThreads, Cfg::kSmem, st>>>(tm_x, tm_b, tm_y, bias, y, stats, form, scr, s.B, s.H, s.W, tiles);
   check_launch("conv5x5_wgmma_im2col(fwd)");
 }
 
@@ -498,7 +496,7 @@ void launch_conv5x5_dgrad_im2col(const float* dy, const float* w, float* dx, Con
   auto kern = conv5x5_wgmma_im2col_kernel<32, 16, false>;
   opt_in_smem(kern, Cfg::kSmem);
   const int grid = std::min(tiles, sm_count());
-  kern<<<grid, Cfg::kThreads, Cfg::kSmem, st>>>(tm_x, tm_b, tm_b, nullptr, dx, nullptr, 0, ReduceScratch{}, s.B, s.H, s.W, tiles);
+  kern<<<grid, Cfg::kThreads, Cfg::kSmem, st>>>(tm_x, tm_b, tm_b, nullptr, dx, nullptr, kConvSums, ReduceScratch{}, s.B, s.H, s.W, tiles);
   check_launch("conv5x5_wgmma_im2col(dgrad)");
 }
 

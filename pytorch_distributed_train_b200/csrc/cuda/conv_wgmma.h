@@ -10,10 +10,10 @@ namespace pdt {
 // True for the shapes the tensor-core convolution handles (the ConvNet's conv2: 16→32 channels).
 bool conv_wgmma_supported(const ConvShape& s);
 
-// y NHWC [B,H,W,32] = conv5x5(x NHWC [B,H,W,16], w [32,16,5,5]) + bias; stats and centred as in launch_conv5x5_fwd.
+// y NHWC [B,H,W,32] = conv5x5(x NHWC [B,H,W,16], w [32,16,5,5]) + bias; stats and form as in launch_conv5x5_fwd.
 // Fully TMA-fed: every filter tap's A-tile is one cp.async.bulk.tensor im2col load; one warpgroup issues the wgmma and
 // runs the epilogue.
-void launch_conv5x5_fwd_im2col(const float* x, const float* w, const float* bias, float* y, float* stats, bool centred, ConvShape s,
+void launch_conv5x5_fwd_im2col(const float* x, const float* w, const float* bias, float* y, void* stats, ConvStats form, ConvShape s,
                                ReduceScratch scr, cudaStream_t st);
 // dx NHWC [B,H,W,16] = conv_transpose(dy NHWC [B,H,W,32], w [32,16,5,5]), same kernel.
 void launch_conv5x5_dgrad_im2col(const float* dy, const float* w, float* dx, ConvShape s, cudaStream_t st);

@@ -357,26 +357,33 @@ void register_cuda_bindings(py::module_& m) {
   // The shape picks the kernels: conv2 (16→32) runs on the tensor cores (TMA-im2col wgmma forward and data gradient, mma.sync
   // weight gradient), every other shape on the SIMT forward and weight gradient, which cover conv1 (1→16) and refuse the rest.
   // Only conv2 has a data gradient: conv1's input needs none.
-  // centred: stats = [mean, M2, n] (ops_kernels.h), without the cancellation of Σy² when |mean| ≫ std; the default [Σ, Σ², n] is what
-  // SyncBatchNorm all-reduces
+  // centred: stats = [mean, M2, n] (ops_kernels.h), without the cancellation of Σy² when |mean| ≫ std; fp64_sums: the fp64
+  // [Σy, Σy², n, 0] formed from the same centred fold, which SyncBatchNorm all-reduces; the default is the fp32 [Σ, Σ², n]
   m.def("conv5x5_fwd", [](const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> bias, bool want_stats, bool zero_pad,
-                          bool centred) {
+                          bool centred, bool fp64_sums) {
     chk(x, "x"); chk(w, "w");
     c10::cuda::CUDAGuard g(x.device());
     ConvShape s = conv_shape(x, w);
     TORCH_CHECK(x.size(3) == s.Cin, "conv5x5_fwd: x channels ", x.size(3), " != weight Cin ", s.Cin);
+    TORCH_CHECK(!(centred && fp64_sums), "conv5x5_fwd: stats are either centred or fp64_sums");
+    TORCH_CHECK(want_stats || !fp64_sums, "conv5x5_fwd: fp64_sums needs want_stats");
     at::Tensor y = at::empty({s.B, s.H, s.W, s.Cout}, x.options());
-    // [2C+1] statistics live in a [2C+4] vector: a 16-byte multiple goes through the vectorised one-shot allreduce
-    // directly (SyncBatchNorm asks for the three pad entries to be zeroed), an odd length would bounce through a
-    // padded temporary (3 extra kernels)
-    at::Tensor stats_full = !want_stats ? at::Tensor() : (zero_pad ? at::zeros({2 * s.Cout + 4}, x.options()) : at::empty({2 * s.Cout + 4}, x.options()));
-    at::Tensor stats = want_stats ? stats_full.narrow(0, 0, 2 * s.Cout + 1) : at::Tensor();
+    at::Tensor stats;
+    if (fp64_sums) {
+      // [2C+2] doubles, every entry written by the kernel: already a 16-byte multiple for the allreduce
+      stats = at::empty({2 * s.Cout + 2}, x.options().dtype(at::kDouble));
+    } else if (want_stats) {
+      // [2C+1] statistics live in a [2C+4] vector (a 16-byte multiple), the three pad entries zeroed on request
+      at::Tensor stats_full = zero_pad ? at::zeros({2 * s.Cout + 4}, x.options()) : at::empty({2 * s.Cout + 4}, x.options());
+      stats = stats_full.narrow(0, 0, 2 * s.Cout + 1);
+    }
+    const ConvStats form = fp64_sums ? kConvSums64 : centred ? kConvCentred : kConvSums;
     auto launch = conv_wgmma_supported(s) ? launch_conv5x5_fwd_im2col : launch_conv5x5_fwd;
-    launch(x.data_ptr<float>(), w.data_ptr<float>(), opt_ptr(bias, "bias"), y.data_ptr<float>(), want_stats ? stats.data_ptr<float>() : nullptr,
-           centred, s, scratch(x), cur_stream(x));
-    return py::make_tuple(y, stats);  // stats is a view of the first 2C+1 entries of the zero-padded vector
+    launch(x.data_ptr<float>(), w.data_ptr<float>(), opt_ptr(bias, "bias"), y.data_ptr<float>(), want_stats ? stats.data_ptr() : nullptr,
+           form, s, scratch(x), cur_stream(x));
+    return py::make_tuple(y, stats);  // fp32 stats: a view of the first 2C+1 entries of the padded vector
   }, py::arg("x"), py::arg("w"), py::arg("bias") = py::none(), py::arg("want_stats") = true, py::arg("zero_pad") = false,
-     py::arg("centred") = false);
+     py::arg("centred") = false, py::arg("fp64_sums") = false);
 
   m.def("conv5x5_dgrad", [](const at::Tensor& dy, const at::Tensor& w) {
     chk(dy, "dy"); chk(w, "w");
@@ -583,32 +590,38 @@ void register_cuda_bindings(py::module_& m) {
      py::arg("beta"), py::arg("w"), py::arg("dgamma"), py::arg("dbeta"), py::arg("loss_parts") = py::none(), py::arg("loss_out") = py::none(),
      py::arg("p1") = py::none(), py::arg("accumulate") = false);
   // ---- BN + ReLU + pool ------------------------------------------------------------------------------
+  // fp64_sums: stats are conv5x5_fwd's fp64 [Σy, Σy², n, 0] (all-reduced by SyncBatchNorm); saved then has 2C+1 entries, the count
+  // last, for bn_relu_pool_bwd_apply
   m.def("bn_relu_pool_fwd", [](const at::Tensor& y, const at::Tensor& stats, c10::optional<at::Tensor> gamma, c10::optional<at::Tensor> beta,
                                c10::optional<at::Tensor> running_mean, c10::optional<at::Tensor> running_var,
-                               c10::optional<at::Tensor> nbt, double momentum, double eps, bool out_nchw, bool mean_var, bool centred) {
-    chk(y, "y"); chk(stats, "stats");
+                               c10::optional<at::Tensor> nbt, double momentum, double eps, bool out_nchw, bool mean_var, bool centred,
+                               bool fp64_sums) {
+    chk(y, "y"); chk(stats, "stats", fp64_sums ? at::kDouble : at::kFloat);
     c10::cuda::CUDAGuard g(y.device());
     TORCH_CHECK(y.dim() == 4, "bn_relu_pool_fwd: y [B,H,W,C] expected");
     const int B = y.size(0), H = y.size(1), W = y.size(2), C = y.size(3);
-    TORCH_CHECK(!(mean_var && centred), "bn_relu_pool_fwd: stats are either mean_var or centred");
+    TORCH_CHECK(int(mean_var) + int(centred) + int(fp64_sums) <= 1, "bn_relu_pool_fwd: stats are one of mean_var, centred or fp64_sums");
     if (mean_var) {
       TORCH_CHECK(stats.numel() == 2 * C, "bn_relu_pool_fwd: mean_var stats must have 2C entries (mean, var)");
       TORCH_CHECK(!(running_mean.has_value() && running_mean->defined()) && !(running_var.has_value() && running_var->defined()) &&
                       !(nbt.has_value() && nbt->defined()), "bn_relu_pool_fwd: mean_var statistics update no running statistics");
+    } else if (fp64_sums) {
+      TORCH_CHECK(stats.numel() == 2 * C + 2, "bn_relu_pool_fwd: fp64_sums stats must have 2C+2 entries");
     } else {
       TORCH_CHECK(stats.numel() == 2 * C + 1, "bn_relu_pool_fwd: stats must have 2C+1 entries");
     }
     at::Tensor out = out_nchw ? at::empty({B, C, H / 2, W / 2}, y.options()) : at::empty({B, H / 2, W / 2, C}, y.options());
-    at::Tensor saved = at::empty({2 * C}, y.options());
+    at::Tensor saved = at::empty({fp64_sums ? 2 * C + 1 : 2 * C}, y.options());
     long long* nbt_p = nullptr;
     if (nbt.has_value() && nbt->defined()) { chk(*nbt, "num_batches_tracked", at::kLong); nbt_p = reinterpret_cast<long long*>(nbt->data_ptr<int64_t>()); }
-    launch_bn_relu_pool_fwd(y.data_ptr<float>(), stats.data_ptr<float>(), opt_ptr(gamma, "gamma"), opt_ptr(beta, "beta"), out.data_ptr<float>(),
+    launch_bn_relu_pool_fwd(y.data_ptr<float>(), stats.data_ptr(), opt_ptr(gamma, "gamma"), opt_ptr(beta, "beta"), out.data_ptr<float>(),
                             saved.data_ptr<float>(), opt_mut(running_mean, "running_mean"), opt_mut(running_var, "running_var"), nbt_p,
                             static_cast<float>(momentum), static_cast<float>(eps), B, H, W, C, out_nchw,
-                            mean_var ? kBnMeanVar : centred ? kBnCentred : kBnSums, cur_stream(y));
+                            mean_var ? kBnMeanVar : centred ? kBnCentred : fp64_sums ? kBnSums64 : kBnSums, cur_stream(y));
     return py::make_tuple(out, saved);
   }, py::arg("y"), py::arg("stats"), py::arg("gamma"), py::arg("beta"), py::arg("running_mean"), py::arg("running_var"), py::arg("nbt"),
-     py::arg("momentum"), py::arg("eps"), py::arg("out_nchw"), py::arg("mean_var") = false, py::arg("centred") = false);
+     py::arg("momentum"), py::arg("eps"), py::arg("out_nchw"), py::arg("mean_var") = false, py::arg("centred") = false,
+     py::arg("fp64_sums") = false);
   m.def("bn_relu_pool_bwd_reduce", [](const at::Tensor& dout, const at::Tensor& y, const at::Tensor& saved, c10::optional<at::Tensor> gamma,
                                       c10::optional<at::Tensor> beta, bool dout_nchw, c10::optional<at::Tensor> dgamma_out,
                                       c10::optional<at::Tensor> dbeta_out) {

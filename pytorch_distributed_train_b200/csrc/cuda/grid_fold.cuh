@@ -159,4 +159,26 @@ __device__ __forceinline__ void grid_fold_centred(const float* blk_vals, int C, 
   });
 }
 
+// Channel i's result of grid_fold_centred in conv5x5_fwd's centred forms (ConvStats): fp32 [mean, M2, n], or the fp64 sums
+// [Σy, Σy², n, 0] that SyncBatchNorm all-reduces.  n·mean is exact in fp64 and M2 + n·mean² rounds once, so the sums keep the
+// centred fold's digits; Σy²/N − mean² of the group is then taken in fp64 (bn_relu_pool_fwd kBnSums64), where mean²/var up to
+// 10⁷ still leaves the variance good to about 1e-9.
+__device__ __forceinline__ void store_centred_stats(void* stats, ConvStats form, int C, int i, float mean, float m2, float n) {
+  if (form == kConvSums64) {
+    double* s = static_cast<double*>(stats);
+    const double sum = static_cast<double>(n) * mean;
+    s[i] = sum;
+    s[C + i] = fma(sum, static_cast<double>(mean), static_cast<double>(m2));
+    if (i == 0) {
+      s[2 * C] = n;
+      s[2 * C + 1] = 0.0;
+    }
+  } else {
+    float* s = static_cast<float*>(stats);
+    s[i] = mean;
+    s[C + i] = m2;
+    if (i == 0) s[2 * C] = n;
+  }
+}
+
 }  // namespace pdt

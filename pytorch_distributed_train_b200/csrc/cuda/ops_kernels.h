@@ -45,10 +45,15 @@ constexpr int kCounterWords = kFoldCounterWords + 48;
 
 // ---- SIMT direct convolution (conv1: 1→16 channels; conv2 runs on the tensor-core kernels of conv_wgmma.h) ----
 // x NHWC [B,H,W,Cin], w torch layout [Cout,Cin,5,5], bias [Cout] (nullable) → y NHWC [B,H,W,Cout].
-// stats (nullable): [2*Cout+1] = per-channel Σy, Σy², then the element count per channel; centred: the mean, M2 (the sum of squared
-// deviations from the mean, folded without cancellation: grid_fold.cuh), then the count.  Σy² is what an all-reduce across GPUs
-// can sum (SyncBatchNorm); M2 keeps the variance's digits when |mean| ≫ std.
-void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float* y, float* stats, bool centred, ConvShape s,
+// stats (nullable) in the form `form`.  The centred forms fold the mean and M2 (the sum of squared deviations from the mean)
+// without cancellation (grid_fold.cuh), so they keep the variance's digits when |mean| ≫ std.
+enum ConvStats : int {
+  kConvSums = 0,      // fp32 [2C+1] Σy, Σy², then the element count per channel
+  kConvCentred = 1,   // fp32 [2C+1] mean, M2, count
+  kConvSums64 = 2,    // fp64 [2C+2] Σy = n·mean, Σy² = M2 + n·mean², count, 0: formed from the centred fold, summable across GPUs
+                      // (SyncBatchNorm)
+};
+void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float* y, void* stats, ConvStats form, ConvShape s,
                         ReduceScratch scr, cudaStream_t st);
 // dw [Cout,Cin,5,5], db [Cout] (nullable) from dy NHWC and x NHWC.
 void launch_conv5x5_wgrad(const float* dy, const float* x, float* dw, float* db, ConvShape s, ReduceScratch scr, cudaStream_t st);
@@ -56,14 +61,15 @@ void launch_conv5x5_wgrad(const float* dy, const float* x, float* dw, float* db,
 // ---- BatchNorm(train) + ReLU + MaxPool2x2, fused -----------------------------------------------------
 // Every bn_relu_pool launcher takes C ∈ {4, 8, 16, 32, 64} and even H, W.
 // y NHWC [B,H,W,C]; stats in one of the BnStats forms below.
-// out: pooled [B,H/2,W/2,C] NHWC, or NCHW when out_nchw. saved [2C] ← mean, invstd.
+// out: pooled [B,H/2,W/2,C] NHWC, or NCHW when out_nchw. saved [2C] ← mean, invstd; kBnSums64: saved [2C+1], the count last.
 // running_mean/var (nullable) updated with `momentum` (unbiased var), nbt (nullable, int64) += 1.
 enum BnStats : int {
-  kBnSums = 0,      // [2C+1] Σ, Σ², n (conv5x5_fwd's sums, already all-reduced when SyncBN is on)
-  kBnCentred = 1,   // [2C+1] mean, M2, n (conv5x5_fwd centred)
-  kBnMeanVar = 2,   // [2C] mean, variance (eval mode: the running statistics, used as they are)
+  kBnSums = 0,      // fp32 [2C+1] Σ, Σ², n (conv5x5_fwd kConvSums; Σ²/n − mean² loses digits when |mean| ≫ std)
+  kBnCentred = 1,   // fp32 [2C+1] mean, M2, n (conv5x5_fwd kConvCentred: one GPU)
+  kBnMeanVar = 2,   // fp32 [2C] mean, variance (eval mode: the running statistics, used as they are)
+  kBnSums64 = 3,    // fp64 [2C+2] Σ, Σ², n, pad (conv5x5_fwd kConvSums64, all-reduced by SyncBatchNorm): mean and variance in fp64
 };
-void launch_bn_relu_pool_fwd(const float* y, const float* stats, const float* gamma, const float* beta, float* out, float* saved,
+void launch_bn_relu_pool_fwd(const float* y, const void* stats, const float* gamma, const float* beta, float* out, float* saved,
                              float* running_mean, float* running_var, long long* nbt, float momentum, float eps, int B, int H,
                              int W, int C, bool out_nchw, BnStats form, cudaStream_t st);
 // Pass 1 of backward: sums [2C] ← Σdz, Σdz·x̂ over the *local* batch (dz = grad at the BN output,

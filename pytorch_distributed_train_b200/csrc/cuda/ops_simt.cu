@@ -28,7 +28,7 @@ namespace {
 // =====================================================================================================
 template <int CIN, int COUT, int CPT, int TH, bool STATS>
 __global__ void __launch_bounds__(448) conv5x5_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
-                                                      float* __restrict__ y, float* stats, int centred, ReduceScratch scr, int B, int H,
+                                                      float* __restrict__ y, void* stats, ConvStats form, ReduceScratch scr, int B, int H,
                                                       int W) {
   constexpr int G = COUT / CPT;
   extern __shared__ __align__(16) float smem[];
@@ -91,6 +91,7 @@ __global__ void __launch_bounds__(448) conv5x5_kernel(const float* __restrict__ 
     // the CTA's per-channel sums of d = y − K and d²: K = 0 gives Σy and Σy².  Centred, K is the CTA's first pixel, and the
     // CTA's M2 = Σd² − (Σd)²/n then cancels only in proportion to ((mean − K)/std)², whatever the size of the mean
     const int lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+    const bool centred = form != kConvSums;
     float* blk = red + nwarps * 2 * COUT;
     __shared__ float s_k[COUT];
     if (centred) {
@@ -133,15 +134,12 @@ __global__ void __launch_bounds__(448) conv5x5_kernel(const float* __restrict__ 
     __shared__ int s_flag;
     if (centred) {
       grid_fold_centred(blk, COUT, npix, B * H * W, blockIdx.x, gridDim.x, scr, s_tmp, &s_flag, tid, blockDim.x, CtaSync{},
-                        [&](int i, float mean, float m2) {
-                          stats[i] = mean;
-                          stats[COUT + i] = m2;
-                          if (i == 0) stats[2 * COUT] = cnt;
-                        });
+                        [&](int i, float mean, float m2) { store_centred_stats(stats, form, COUT, i, mean, m2, cnt); });
     } else {
+      float* sums = static_cast<float*>(stats);
       grid_fold(blk, 2 * COUT, blockIdx.x, gridDim.x, scr, s_tmp, &s_flag, tid, blockDim.x, CtaSync{}, [&](int i, float v) {
-        stats[i] = v;
-        if (i == 0) stats[2 * COUT] = cnt;
+        sums[i] = v;
+        if (i == 0) sums[2 * COUT] = cnt;
       });
     }
   }
@@ -257,20 +255,39 @@ __global__ void __launch_bounds__(256) fold_partials_kernel(const float* __restr
 // =====================================================================================================
 // BatchNorm(train) + ReLU + MaxPool 2x2
 // =====================================================================================================
-// The batch variance (biased) from stats in the form `form` (BnStats).  kBnSums' E[y²] − mean² cancels the variance's digits when
-// |mean| ≫ std; it is kept for SyncBatchNorm, whose all-reduce can sum Σ and Σ² across GPUs but not M2.  The centred form (M2
-// about the mean) and the eval form (the running statistics as they are) have no such cancellation.
-__device__ __forceinline__ float bn_stats_var(const float* stats, int C, int c, int form, float mean) {
-  if (form == kBnMeanVar) return stats[C + c];
-  const float n = fmaxf(stats[2 * C], 1.f);
-  return form == kBnCentred ? stats[C + c] / n : fmaxf(stats[C + c] / n - mean * mean, 0.f);
+// The batch mean and variance (biased) of channel c from stats in the form `form` (BnStats).  kBnSums' E[y²] − mean² in fp32
+// cancels the variance's digits when |mean| ≫ std; it stays as the plain-sums form of the kernels.  The centred form (M2 about the
+// mean), the eval form (the running statistics as they are) and SyncBatchNorm's fp64 sums, whose E[y²] − mean² in fp64 keeps the
+// variance to about 1e-16·mean²/var, have no such cancellation.
+__device__ __forceinline__ void bn_mean_var(const void* stats, int C, int c, int form, float* mean, float* var) {
+  if (form == kBnSums64) {
+    const double* s = static_cast<const double*>(stats);
+    const double n = fmax(s[2 * C], 1.0), m = s[c] / n;
+    *mean = static_cast<float>(m);
+    *var = static_cast<float>(fmax(s[C + c] / n - m * m, 0.0));
+    return;
+  }
+  const float* s = static_cast<const float*>(stats);
+  if (form == kBnMeanVar) {
+    *mean = s[c];
+    *var = s[C + c];
+    return;
+  }
+  const float n = fmaxf(s[2 * C], 1.f);
+  *mean = form == kBnSums ? s[c] / n : s[c];
+  *var = form == kBnCentred ? s[C + c] / n : fmaxf(s[C + c] / n - *mean * *mean, 0.f);
 }
 
-__device__ __forceinline__ void bn_coeffs(const float* stats, const float* gamma, const float* beta, float eps, int C, int form,
+// the element count per channel (every form but kBnMeanVar)
+__device__ __forceinline__ float bn_stats_count(const void* stats, int C, int form) {
+  return form == kBnSums64 ? static_cast<float>(static_cast<const double*>(stats)[2 * C]) : static_cast<const float*>(stats)[2 * C];
+}
+
+__device__ __forceinline__ void bn_coeffs(const void* stats, const float* gamma, const float* beta, float eps, int C, int form,
                                           float* s_scale, float* s_shift, float* s_mean, float* s_invstd) {
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    const float mean = form == kBnSums ? stats[c] / fmaxf(stats[2 * C], 1.f) : stats[c];
-    const float var = bn_stats_var(stats, C, c, form, mean);
+    float mean, var;
+    bn_mean_var(stats, C, c, form, &mean, &var);
     const float invstd = rsqrtf(var + eps);
     const float g = gamma ? gamma[c] : 1.f, b = beta ? beta[c] : 0.f;
     s_mean[c] = mean;
@@ -280,7 +297,7 @@ __device__ __forceinline__ void bn_coeffs(const float* stats, const float* gamma
   }
 }
 
-__global__ void __launch_bounds__(256) bn_relu_pool_fwd_kernel(const float* __restrict__ y, const float* __restrict__ stats,
+__global__ void __launch_bounds__(256) bn_relu_pool_fwd_kernel(const float* __restrict__ y, const void* __restrict__ stats,
                                                                const float* __restrict__ gamma, const float* __restrict__ beta,
                                                                float* __restrict__ out, float* saved, float* running_mean,
                                                                float* running_var, long long* nbt, float momentum, float eps, int B,
@@ -293,14 +310,18 @@ __global__ void __launch_bounds__(256) bn_relu_pool_fwd_kernel(const float* __re
       saved[c] = s_mean[c];
       saved[C + c] = s_invstd[c];
       if (running_mean) {
-        const float n = fmaxf(stats[2 * C], 1.f);
-        const float var = bn_stats_var(stats, C, c, form, s_mean[c]);
+        const float n = fmaxf(bn_stats_count(stats, C, form), 1.f);
+        float mean, var;
+        bn_mean_var(stats, C, c, form, &mean, &var);
         const float unbiased = var * (n / fmaxf(n - 1.f, 1.f));
         running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * s_mean[c];
         running_var[c] = (1.f - momentum) * running_var[c] + momentum * unbiased;
       }
     }
-    if (nbt && threadIdx.x == 0) *nbt += 1;
+    if (threadIdx.x == 0) {
+      if (nbt) *nbt += 1;
+      if (form == kBnSums64) saved[2 * C] = bn_stats_count(stats, C, form);   // the group's count, for the backward
+    }
   }
   const int Q = C / 4, PH = H / 2, PW = W / 2;
   const long long total = static_cast<long long>(B) * PH * PW * Q;
@@ -1051,7 +1072,7 @@ size_t conv_smem(int cin, int cout, int th, int w, int threads) {
 }  // namespace
 
 // ---- launchers ---------------------------------------------------------------------------------------
-void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float* y, float* stats, bool centred, ConvShape s,
+void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float* y, void* stats, ConvStats form, ConvShape s,
                         ReduceScratch scr, cudaStream_t st) {
   constexpr int TH = 7;
   if (!(s.Cin == 1 && s.Cout == 16)) throw std::invalid_argument("conv5x5_fwd: supported channel config is 1→16");
@@ -1061,8 +1082,8 @@ void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float
     throw std::invalid_argument("conv5x5_fwd: reduction scratch too small");
   const int threads = (TH * s.W + 31) / 32 * 32;
   const size_t sm = conv_smem(1, 16, TH, s.W, threads);
-  if (stats) conv5x5_kernel<1, 16, 16, TH, true><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, centred ? 1 : 0, scr, s.B, s.H, s.W);
-  else conv5x5_kernel<1, 16, 16, TH, false><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, 0, scr, s.B, s.H, s.W);
+  if (stats) conv5x5_kernel<1, 16, 16, TH, true><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, form, scr, s.B, s.H, s.W);
+  else conv5x5_kernel<1, 16, 16, TH, false><<<blocks, threads, sm, st>>>(x, w, bias, y, stats, kConvSums, scr, s.B, s.H, s.W);
   check_launch("conv5x5_fwd");
 }
 
@@ -1089,7 +1110,7 @@ static void check_bn_relu_pool_shape(int C, int H, int W, const char* what) {
     throw std::invalid_argument(std::string(what) + ": C must be 4, 8, 16, 32 or 64, and H and W even");
 }
 
-void launch_bn_relu_pool_fwd(const float* y, const float* stats, const float* gamma, const float* beta, float* out, float* saved,
+void launch_bn_relu_pool_fwd(const float* y, const void* stats, const float* gamma, const float* beta, float* out, float* saved,
                              float* running_mean, float* running_var, long long* nbt, float momentum, float eps, int B, int H, int W,
                              int C, bool out_nchw, BnStats form, cudaStream_t st) {
   check_bn_relu_pool_shape(C, H, W, "bn_relu_pool_fwd");

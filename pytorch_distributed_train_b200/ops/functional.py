@@ -54,15 +54,6 @@ def _inline_allreduce(group, t: torch.Tensor) -> None:
         comm.allreduce(t, dist.ReduceOp.SUM, 1.0).wait()   # NCCL baseline: stream hop + wait
 
 
-def _padded_stats(stats: torch.Tensor) -> torch.Tensor:
-    """conv5x5_fwd hands back the first 2C+1 entries of a zeroed [2C+4] vector; all-reduce the whole padded
-    vector (a 16-byte multiple takes the vectorised kernel, an odd length would bounce through a temporary)."""
-    n = (stats.numel() + 3) // 4 * 4
-    if stats.dim() == 1 and stats.is_contiguous() and stats.untyped_storage().nbytes() >= (stats.storage_offset() + n) * stats.element_size():
-        return stats.as_strided((n,), (1,), stats.storage_offset())
-    return stats
-
-
 def _to_nhwc(x: torch.Tensor) -> torch.Tensor:
     """[B,C,H,W] (any strides) → contiguous [B,H,W,C] without a copy when already channels_last."""
     if x.shape[1] == 1:
@@ -75,15 +66,20 @@ class _ConvBnReluPool(torch.autograd.Function):
     def forward(ctx, x, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, training, group, out_nchw):
         xh = _to_nhwc(x)
         C = w.shape[0]
-        if training:
-            # one GPU: [mean, M2, n], no cancellation when |mean| ≫ std; SyncBatchNorm: [Σy, Σy², n], which the all-reduce can sum
-            centred = group is None
-            y, stats = _C.conv5x5_fwd(xh, w, b, True, not centred, centred=centred)
-            if group is not None:
-                _inline_allreduce(group, _padded_stats(stats))   # Σy, Σy², n across the group: SyncBatchNorm
+        if training and group is None:
+            # one GPU: [mean, M2, n], no cancellation when |mean| ≫ std
+            y, stats = _C.conv5x5_fwd(xh, w, b, True, centred=True)
             out, saved = _C.bn_relu_pool_fwd(y, stats, gamma, beta, running_mean, running_var, nbt, momentum, eps, out_nchw,
-                                             centred=centred)
+                                             centred=True)
             count = stats[2 * C:2 * C + 1]
+        elif training:
+            # SyncBatchNorm: fp64 [Σy = n·mean, Σy² = M2 + n·mean², n, 0] from this rank's centred fold, summed across the group;
+            # the group's mean and variance are then taken in fp64, where Σy²/N − mean² keeps the variance's digits
+            y, stats = _C.conv5x5_fwd(xh, w, b, True, fp64_sums=True)
+            _inline_allreduce(group, stats)
+            out, saved = _C.bn_relu_pool_fwd(y, stats, gamma, beta, running_mean, running_var, nbt, momentum, eps, out_nchw,
+                                             fp64_sums=True)
+            count = saved[2 * C:]   # the group's count, which bn_relu_pool_fwd leaves behind the mean and invstd
         else:
             y, _ = _C.conv5x5_fwd(xh, w, b, False)
             # the running mean and variance as they are: no round trip through sums, which would cancel the variance's digits

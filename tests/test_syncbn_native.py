@@ -7,8 +7,8 @@ whole (concatenated) batch.  Rank r is thus checked against "every other rank ex
 * the generic path (``pdt.SyncBatchNorm`` on any N×C×… input): bn_stats_nchw_f64 → fp64 allreduce of (Σx, Σx², n) → bn_finalize
   (or the same arithmetic in Python) → bn_apply_nchw; backward bn_bwd_reduce_nchw → fp32 allreduce of (Σdy, Σdy·(x−μ)) →
   bn_bwd_apply_nchw;
-* the ConvNet path (``convert_sync_batchnorm(ConvNet())``): conv5x5_fwd's zero-padded [2C+4] fp32 statistics are all-reduced before
-  bn_relu_pool_fwd; backward all-reduces (Σdz, Σdz·x̂) of bn_relu_pool_bwd_reduce before bn_relu_pool_bwd_apply.
+* the ConvNet path (``convert_sync_batchnorm(ConvNet())``): conv5x5_fwd's fp64 [Σy, Σy², n, 0], formed from its centred fold, are
+  all-reduced before bn_relu_pool_fwd; backward all-reduces (Σdz, Σdz·x̂) of bn_relu_pool_bwd_reduce before bn_relu_pool_bwd_apply.
 
 The oracle runs BatchNorm in float64 on the concatenated shards with one copy of every parameter per shard and the loss Σₖ Lₖ:
 shard r's output and input gradient, and the gradients of its own parameter copies, are what rank r must produce.
@@ -477,7 +477,14 @@ def _grad_scale(name, layers, r):
     return None
 
 
-@pytest.mark.parametrize("ns,r", [((37, 63), 0), ((37, 63), 1), ((1, 99), 0), ((1, 99), 1), ((10, 40, 25, 25), 2), ((3, 50, 1, 46), 2)])
+# (per-rank batch sizes, rank under test); after the first six: even shards, a one-image rank under test behind a larger one, two
+# one-image ranks, the first and last rank of four, and worlds of three and eight
+CONVNET_SHARDS = [((37, 63), 0), ((37, 63), 1), ((1, 99), 0), ((1, 99), 1), ((10, 40, 25, 25), 2), ((3, 50, 1, 46), 2),
+                  ((50, 50), 1), ((99, 1), 1), ((1, 1, 98), 1), ((10, 40, 25, 25), 0), ((10, 40, 25, 25), 3),
+                  ((30, 33, 37), 2), ((12, 12, 12, 12, 13, 13, 13, 13), 5)]
+
+
+@pytest.mark.parametrize("ns,r", CONVNET_SHARDS)
 def test_convnet_syncbn_matches_float64(ns, r, fake_dist):
     torch.manual_seed(5)
     gen = torch.Generator(device=dev()).manual_seed(9)
@@ -493,8 +500,8 @@ def test_convnet_syncbn_matches_float64(ns, r, fake_dist):
     others = lambda per: sum(p for k, p in enumerate(per) if k != r)  # noqa: E731
     for l, C in ((1, 16), (2, 32)):
         ys = [y.detach() for y in layers[l]["ys"]]
-        fwd = [torch.cat([y.sum((0, 2, 3)), (y * y).sum((0, 2, 3)), y.new_tensor([float(y.numel() // C), 0.0, 0.0, 0.0])]) for y in ys]
-        group.comm.expected.append((f"layer{l} forward", torch.float32, 2 * C + 4, others(fwd), 2 * C + 1))
+        fwd = [torch.cat([y.sum((0, 2, 3)), (y * y).sum((0, 2, 3)), y.new_tensor([float(y.numel() // C), 0.0])]) for y in ys]
+        group.comm.expected.append((f"layer{l} forward", torch.float64, 2 * C + 2, others(fwd), 2 * C + 1))
     for l in (2, 1):
         L = layers[l]
         xhat = [(y.detach() - L["mean"].detach().view(1, -1, 1, 1)) * L["invstd"].detach().view(1, -1, 1, 1) for y in L["ys"]]

@@ -53,25 +53,6 @@ def test_nvtx_and_clock_sampler_degrade_without_a_gpu():
         assert s["samples"] == 0 and s["sm_mhz"] is None
 
 
-def test_padded_stats_view_logic():
-    """SyncBatchNorm all-reduces the zero-padded [2C+4] vector behind the [2C+1] statistics (a 16-byte multiple takes the
-    vectorised kernel); a tensor that has no padding behind it must be left alone."""
-    from pytorch_distributed_train_b200.ops.functional import _padded_stats
-
-    C = 16
-    full = torch.zeros(2 * C + 4)
-    stats = full.narrow(0, 0, 2 * C + 1)
-    stats.copy_(torch.arange(2 * C + 1, dtype=torch.float32))
-    p = _padded_stats(stats)
-    assert p.numel() == 2 * C + 4 and p.data_ptr() == stats.data_ptr() and p.numel() * 4 % 16 == 0
-    assert torch.equal(p[:2 * C + 1], stats) and p[2 * C + 1:].abs().sum() == 0
-    p[0] = 7.0
-    assert stats[0] == 7.0                                   # same memory: the allreduce result lands in `stats`
-    exact = torch.ones(2 * C + 1)
-    assert _padded_stats(exact) is exact                     # no room behind it
-    assert _padded_stats(torch.ones(8)).numel() == 8         # already a multiple of four
-
-
 def test_upcoming_targets_and_rider_contexts_nest_and_restore():
     """Engine-level announcements (ops.functional): nested contexts restore the outer state; nothing leaks after exit."""
     import torch

@@ -25,7 +25,7 @@ GROUPS = {
     "average": ["tests/test_averaged_model.py"],
     "accum": ["tests/test_grad_accumulation.py"],
     "ce_options": ["tests/test_cross_entropy_options.py"],
-    "syncbn": ["tests/test_syncbn_native.py"],
+    "syncbn": ["tests/test_syncbn_native.py", "tests/test_syncbn_large_mean.py"],
     "symm_emu": ["tests/test_symm_kernels_emulated.py"],
 }
 
