@@ -38,7 +38,7 @@ if hasattr(_C, "_mark_exiting"):
 
     _atexit.register(_C._mark_exiting)
 
-from . import data, distributed, launcher, models, nn, ops, optim, parallel, utils  # noqa: E402
+from . import data, distributed, engine, launcher, models, nn, ops, optim, parallel, utils  # noqa: E402
 from .data import DataLoader, DistributedSampler  # noqa: E402
 from .distributed import (destroy_process_group, get_rank, get_world_size, init_process_group,  # noqa: E402
                           is_initialized)
@@ -46,7 +46,7 @@ from .launcher import spawn  # noqa: E402
 from .parallel import DataParallel, DistributedDataParallel, SyncBatchNorm  # noqa: E402
 
 __all__ = [
-    "data", "distributed", "launcher", "models", "nn", "ops", "optim", "parallel", "utils",
+    "data", "distributed", "engine", "launcher", "models", "nn", "ops", "optim", "parallel", "utils",
     "DataLoader", "DistributedSampler", "DistributedDataParallel", "DataParallel", "SyncBatchNorm",
     "init_process_group", "destroy_process_group", "get_rank", "get_world_size", "is_initialized", "spawn",
 ]

@@ -10,7 +10,7 @@ Extra flags cover what the reference hard-codes: ``--init-method`` (its LAN addr
 to loopback with a free port), ``--data synthetic|mnist``, ``--model``, ``--comm fused|nccl``, ``--algo``,
 ``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw), ``--lr``,
 ``--momentum``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--ema-decay``,
-``--checkpoint`` / ``--resume``.
+``--checkpoint`` / ``--resume``, ``--eval`` (test loss and accuracy after every epoch).
 """
 from __future__ import annotations
 
@@ -66,6 +66,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--log-interval", default=10, type=int)
     p.add_argument("--checkpoint", default=None, type=str, help="write a checkpoint here at the end of every epoch (rank 0, atomic)")
     p.add_argument("--resume", default=None, type=str, help="restore model/optimizer/epoch from this checkpoint before training")
+    p.add_argument("--eval", default=False, action="store_true",
+                   help="after every epoch, print the loss and top-1 accuracy on the test split (and of the --ema-decay average)")
     p.add_argument("--set-epoch", default=False, action="store_true",
                    help="call sampler.set_epoch(e) each epoch (the reference does not)")
     return p
@@ -148,6 +150,16 @@ def dist_train(gpu: int, args) -> None:
     train_loader = pdt.DataLoader(dataset=train_dataset, batch_size=accum * batch_size, shuffle=False, num_workers=0,
                                   pin_memory=use_cuda, sampler=train_sampler)
 
+    if args.eval:
+        # the test split: every image counted once across the ranks (engine.evaluate leaves out the sampler's padding)
+        if args.data == "mnist" and args.model == "convnet":
+            test_dataset = pdata.MNIST(root=args.data_root, train=False, synthetic_fallback=True)
+        else:
+            test_dataset = pdata.SyntheticMNIST(10000 if args.model == "convnet" else 4096, seed=1,
+                                                num_classes=10 if args.model == "convnet" else 1000, image_shape=shape)
+        test_loader = pdt.DataLoader(dataset=test_dataset, batch_size=batch_size, shuffle=False, pin_memory=use_cuda,
+                                     sampler=pdt.DistributedSampler(test_dataset, num_replicas=args.world_size, rank=rank, shuffle=False))
+
     step_fn = None
     if args.graph and use_cuda:
         from pytorch_distributed_train_b200.engine import GraphedTrainStep
@@ -214,6 +226,12 @@ def dist_train(gpu: int, args) -> None:
             print(fmt.format(epoch + 1, args.epochs, pending[0], total_step, pending[1].item()))
         if args.checkpoint:
             pdt.utils.save_checkpoint(args.checkpoint, model, optimizer, epoch=epoch + 1, sampler=train_sampler, averaged_model=ema)
+        if args.eval:
+            for tag, evaluated in [("", model)] + ([("EMA ", ema)] if ema is not None else []):
+                r = pdt.engine.evaluate(evaluated, test_loader, criterion)
+                if gpu == 0:
+                    print(f"Epoch [{epoch + 1}/{args.epochs}], {tag}Test Loss: {r['loss']:.4f}, Accuracy: {100 * r['accuracy']:.2f}% "
+                          f"({r['count']} images)")
     if use_cuda:
         torch.cuda.synchronize()
     if gpu == 0:

@@ -749,6 +749,20 @@ void register_cuda_bindings(py::module_& m) {
     return d;
   }, py::arg("probs"), py::arg("target"), py::arg("dloss"), py::arg("weight") = py::none(), py::arg("ignore_index") = -100,
      py::arg("label_smoothing") = 0.0, py::arg("reduction") = "mean");
+  // acc[0..3] += Σ loss terms, Σ counted target weights, top-1 hits, counted rows of logits[:rows] (ops_kernels.h); no sync
+  m.def("cross_entropy_eval", [](const at::Tensor& logits, const at::Tensor& target, at::Tensor acc, int64_t rows,
+                                 c10::optional<at::Tensor> weight, int64_t ignore_index, double label_smoothing) {
+    chk(logits, "logits"); chk(target, "target", at::kLong); chk(acc, "acc", at::kDouble);
+    TORCH_CHECK(logits.dim() == 2 && logits.size(1) >= 1 && logits.size(1) <= 1024, "cross_entropy_eval: logits must be [B, C <= 1024]");
+    TORCH_CHECK(target.dim() == 1 && target.size(0) == logits.size(0), "cross_entropy_eval: target must be [", logits.size(0), "]");
+    TORCH_CHECK(acc.numel() == 4 && acc.device() == logits.device(), "cross_entropy_eval: acc must be 4 doubles on ", logits.device());
+    TORCH_CHECK(rows >= 0 && rows <= logits.size(0), "cross_entropy_eval: rows must lie in [0, ", logits.size(0), "] (got ", rows, ")");
+    c10::cuda::CUDAGuard g(logits.device());
+    const CeSpec spec = ce_spec(weight, ignore_index, label_smoothing, "mean", logits.size(1), logits, "cross_entropy_eval");
+    launch_cross_entropy_eval(logits.data_ptr<float>(), reinterpret_cast<const long long*>(target.data_ptr<int64_t>()), acc.data_ptr<double>(),
+                              static_cast<int>(rows), logits.size(1), cur_stream(logits), spec);
+  }, py::arg("logits"), py::arg("target"), py::arg("acc"), py::arg("rows"), py::arg("weight") = py::none(), py::arg("ignore_index") = -100,
+     py::arg("label_smoothing") = 0.0);
 
   // ---- optimizer ------------------------------------------------------------------------------------------
   m.def("sgd_multi", [](std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> bufs, double lr,

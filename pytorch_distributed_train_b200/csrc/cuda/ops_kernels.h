@@ -129,6 +129,14 @@ void launch_cross_entropy_fwd(const float* logits, const long long* target, floa
                               bool emit_grad, const CeSpec& spec);
 void launch_cross_entropy_bwd(const float* probs, const long long* target, const float* dloss, float* dlogits, int B, int C,
                               cudaStream_t st, const CeSpec& spec);
+// Evaluation metrics of logits[0:rows, C] (the first `rows` rows of the batch; the rest take no part), added to the fp64 acc[4] by
+// one launch of the forward kernel that writes no loss or softmax:
+//   acc[0] += Σ loss terms (the sum before the division by D)   acc[1] += D = Σ_{counted} w_t, whatever spec.sum says
+//   acc[2] += counted rows whose argmax is the target             acc[3] += counted rows
+// argmax is torch.argmax's: the first maximal index, a NaN counting as the maximum.  Plain adds, one block, stream-ordered: the
+// totals are reproducible bit for bit.
+void launch_cross_entropy_eval(const float* logits, const long long* target, double* acc, int rows, int C, cudaStream_t st,
+                               const CeSpec& spec);
 
 // ---- optimizer -------------------------------------------------------------------------------------------
 struct SgdTensorList {

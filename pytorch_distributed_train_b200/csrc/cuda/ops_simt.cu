@@ -828,14 +828,19 @@ __device__ __forceinline__ void ce_spec_sums(const long long* __restrict__ targe
   W = s.weight ? ce_block_sum(w, red) : static_cast<float>(C);
 }
 
+// acc (accumulate mode, probs == nullptr, a mean spec): instead of the loss, thread 0 adds the block's Σ loss terms, D, the
+// counted rows whose argmax (torch.argmax's: the first maximal index, a NaN counting as the maximum) is the target, and the
+// counted rows to acc[0..3]: plain fp64 adds, ordered by the stream, so the totals are the same bits from run to run.
 __global__ void __launch_bounds__(256) cross_entropy_fwd_spec_kernel(const float* __restrict__ logits, const long long* __restrict__ target,
                                                                      float* loss, float* __restrict__ probs, int B, int C, int emit_grad,
-                                                                     CeSpec s) {
+                                                                     CeSpec s, double* acc) {
   __shared__ float red[256];
+  __shared__ int s_counts[2];   // hits, counted rows (accumulate mode)
   float D, W;
   ce_spec_sums(target, B, C, s, red, D, W);
   const float keep = 1.f - s.smoothing, eps_c = s.smoothing / static_cast<float>(C);
   float local = 0.f;
+  int hits = 0, counted = 0;
   for (int r = threadIdx.x; r < B; r += blockDim.x) {
     const float* l = logits + static_cast<size_t>(r) * C;
     float m = l[0];
@@ -851,12 +856,35 @@ __global__ void __launch_bounds__(256) cross_entropy_fwd_spec_kernel(const float
       const float lc = l[c], wc = s.weight ? s.weight[c] : 1.f;
       const float p = __expf(lc - m) * inv;
       smooth += wc * (lse - lc);
-      probs[static_cast<size_t>(r) * C + c] =
-          !emit_grad ? p : counted_row ? (keep * wt * (p - (t == c ? 1.f : 0.f)) + eps_c * (W * p - wc)) / D : 0.f;
+      if (probs)
+        probs[static_cast<size_t>(r) * C + c] =
+            !emit_grad ? p : counted_row ? (keep * wt * (p - (t == c ? 1.f : 0.f)) + eps_c * (W * p - wc)) / D : 0.f;
     }
     if (counted_row) local += keep * wt * (lse - l[t]) + eps_c * smooth;
+    if (acc && counted_row) {
+      int top = 0;
+      float best = l[0];
+      for (int c = 1; c < C; ++c)
+        if (l[c] > best || (isnan(l[c]) && !isnan(best))) best = l[c], top = c;
+      hits += top == t;
+      ++counted;
+    }
   }
   const float total = ce_block_sum(local, red);
+  if (acc) {
+    if (threadIdx.x == 0) s_counts[0] = s_counts[1] = 0;
+    __syncthreads();
+    atomicAdd(&s_counts[0], hits);   // integer sums: the same whatever the order
+    atomicAdd(&s_counts[1], counted);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      acc[0] += static_cast<double>(total);
+      acc[1] += static_cast<double>(D);
+      acc[2] += static_cast<double>(s_counts[0]);
+      acc[3] += static_cast<double>(s_counts[1]);
+    }
+    return;
+  }
   // a mean over zero total weight is NaN, as torch's, also when the smoothing terms of zero-weight rows make the sum positive
   if (threadIdx.x == 0) *loss = (D == 0.f ? 0.f : total) / D;
 }
@@ -1207,8 +1235,15 @@ void launch_cross_entropy_bwd(const float* probs, const long long* target, const
 void launch_cross_entropy_fwd(const float* logits, const long long* target, float* loss, float* probs, int B, int C, cudaStream_t st,
                               bool emit_grad, const CeSpec& spec) {
   if (spec.is_default(C)) return launch_cross_entropy_fwd(logits, target, loss, probs, B, C, st, emit_grad);
-  cross_entropy_fwd_spec_kernel<<<1, 256, 0, st>>>(logits, target, loss, probs, B, C, emit_grad ? 1 : 0, spec);
+  cross_entropy_fwd_spec_kernel<<<1, 256, 0, st>>>(logits, target, loss, probs, B, C, emit_grad ? 1 : 0, spec, nullptr);
   check_launch("cross_entropy_fwd");
+}
+void launch_cross_entropy_eval(const float* logits, const long long* target, double* acc, int rows, int C, cudaStream_t st,
+                               const CeSpec& spec) {
+  CeSpec mean = spec;
+  mean.sum = false;   // acc takes the sum of the terms and the mean's divisor D whatever the reduction
+  cross_entropy_fwd_spec_kernel<<<1, 256, 0, st>>>(logits, target, nullptr, nullptr, rows, C, 0, mean, acc);
+  check_launch("cross_entropy_eval");
 }
 void launch_cross_entropy_bwd(const float* probs, const long long* target, const float* dloss, float* dlogits, int B, int C,
                               cudaStream_t st, const CeSpec& spec) {

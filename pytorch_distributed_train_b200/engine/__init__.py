@@ -1,3 +1,4 @@
+from .evaluate import evaluate
 from .graphed_step import GraphedTrainStep
 
-__all__ = ["GraphedTrainStep"]
+__all__ = ["GraphedTrainStep", "evaluate"]

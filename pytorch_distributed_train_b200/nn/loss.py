@@ -14,6 +14,17 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 
+def native_ok(input: torch.Tensor, target: torch.Tensor, weight, reduction: str, label_smoothing: float) -> bool:
+    """Whether a cross-entropy of ``input`` and ``target`` with these options runs on the native kernels."""
+    from .. import ops
+
+    return (input.is_cuda and ops.native_available() and input.dim() == 2 and input.dtype == torch.float32
+            and target.dtype == torch.int64 and reduction in ("mean", "sum") and 0.0 <= label_smoothing <= 1.0
+            and input.shape[1] <= 1024
+            and (weight is None or (weight.dtype == torch.float32 and weight.is_contiguous() and weight.shape == (input.shape[1],)
+                                    and weight.device == input.device)))
+
+
 class CrossEntropyLoss(nn.Module):
     def __init__(self, weight=None, ignore_index: int = -100, reduction: str = "mean", label_smoothing: float = 0.0):
         super().__init__()
@@ -22,14 +33,7 @@ class CrossEntropyLoss(nn.Module):
 
     def native_ok(self, input: torch.Tensor, target: torch.Tensor) -> bool:
         """Whether ``forward(input, target)`` runs on the native kernels."""
-        from .. import ops
-
-        w = self.weight
-        return (input.is_cuda and ops.native_available() and input.dim() == 2 and input.dtype == torch.float32
-                and target.dtype == torch.int64 and self.reduction in ("mean", "sum") and 0.0 <= self.label_smoothing <= 1.0
-                and input.shape[1] <= 1024
-                and (w is None or (w.dtype == torch.float32 and w.is_contiguous() and w.shape == (input.shape[1],)
-                                   and w.device == input.device)))
+        return native_ok(input, target, self.weight, self.reduction, self.label_smoothing)
 
     def forward(self, input: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
         from .. import ops

@@ -36,3 +36,6 @@ else:  # CPU-only build of the extension: keep the names importable, fail loudly
     for _n in ("adam_step", "average_update", "bn_apply", "bn_backward_apply", "bn_backward_reduce", "bn_finalize", "bn_local_stats",
                "conv_bn_relu_pool", "cross_entropy", "grad_norm_clip", "grad_scale", "linear", "sgd_step"):
         globals()[_n] = _missing(_n)
+
+# evaluation metrics: the native kernel where it applies, torch ops elsewhere (CPU, gloo, other dtypes), so importable in any build
+from .functional import cross_entropy_accumulate  # noqa: E402,F401

@@ -550,6 +550,32 @@ def cross_entropy(logits: torch.Tensor, target: torch.Tensor, weight: Optional[t
     return _CrossEntropy.apply(logits, target, spec)
 
 
+def cross_entropy_accumulate(logits: torch.Tensor, target: torch.Tensor, acc: torch.Tensor, rows: int,
+                             spec: tuple = DEFAULT_CE_SPEC) -> None:
+    """Add the evaluation metrics of ``logits[:rows]`` against ``target[:rows]`` to ``acc``, a float64 ``[4]`` tensor on the logits'
+    device: Σ of the loss terms, Σ of the counted rows' target weights (the mean's divisor, whatever the reduction), the counted
+    rows whose ``argmax`` is the target, and the counted rows.  A row counts when its target lies in [0, C) and is not
+    ``ignore_index``.  ``spec`` = (weight, ignore_index, reduction, label_smoothing), the criterion's options.
+
+    One launch of the native cross-entropy kernel where ``nn.loss.native_ok`` holds, torch ops otherwise; neither synchronises
+    with the host."""
+    from ..nn.loss import native_ok
+
+    weight, ignore_index, reduction, smoothing = spec
+    if native_ok(logits, target, weight, reduction, smoothing):
+        _C.cross_entropy_eval(logits.contiguous(), target.contiguous(), acc, int(rows), weight, int(ignore_index), float(smoothing))
+        return
+    logits, target = logits[:rows], target[:rows]
+    counted = (target >= 0) & (target < logits.shape[1]) & (target != ignore_index)
+    safe = torch.where(counted, target, 0)   # torch's cross-entropy rejects a target outside [0, C) that is not ignore_index
+    terms = torch.nn.functional.cross_entropy(logits, safe, weight, reduction="none", label_smoothing=smoothing)
+    w_t = weight.index_select(0, safe) if weight is not None else torch.ones_like(terms)
+    hits = counted & (logits.argmax(1) == target)
+    zero = terms.new_zeros(())
+    acc += torch.stack([torch.where(counted, terms, zero).sum(dtype=torch.float64), torch.where(counted, w_t, zero).sum(dtype=torch.float64),
+                        hits.sum().to(torch.float64), counted.sum().to(torch.float64)])
+
+
 def sgd_step(params, grads, momentum_bufs, lr, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False,
              maximize=False, first_step=False, lr_tensor=None) -> None:
     _C.sgd_multi(list(params), list(grads), list(momentum_bufs) if momentum_bufs else [], float(lr), lr_tensor, float(momentum),
