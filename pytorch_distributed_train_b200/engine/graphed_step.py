@@ -21,6 +21,11 @@ safe as is — this is the ConvNet/ResNet case; (b) otherwise the step is captur
 capture starts on the other half) and replays alternate between the two graphs, which reproduces
 exactly the eager alternation.
 
+Learning-rate schedules: with a native optimizer (``pdt.optim.SGD``, ``Adam``, ``AdamW``) every group's lr lives in a device scalar
+that the captured kernels read, whatever the group's ``capturable`` says, and each replay first copies ``param_groups[i]['lr']``
+into it (``sync_lr``), so a ``torch.optim.lr_scheduler`` stepped between replays takes effect on the next one.  The other
+hyper-parameters are baked into the graph: a replay after one of them changed (``OneCycleLR(cycle_momentum=True)``) raises.
+
 Gradient-norm clipping (``max_grad_norm``, as ``torch.nn.utils.clip_grad_norm_`` between backward and ``optimizer.step()``):
 on one GPU, when the update rides on the last backward kernel, that kernel clips before it updates (still three launches);
 otherwise the native clip runs between backward and ``step()`` inside the graph (two launches).  With clipping the optimizer
@@ -97,6 +102,10 @@ class GraphedTrainStep:
         # when the criterion returned the fused cross-entropy itself on every micro-batch (None: not decided yet)
         self._prescale: Optional[bool] = None
         self.model, self.criterion, self.optimizer = model, criterion, optimizer
+        if hasattr(optimizer, "_lr_on_device"):
+            # a native optimizer's kernels read every group's lr from a device scalar from the warm-up steps on, so that sync_lr()
+            # before a replay carries a scheduler's change into the graph (a captured host lr would be replayed forever)
+            optimizer._lr_on_device = True
         self.static_inputs = [t.clone() for t in example_inputs]
         # two input buffers, one captured graph each: the next batch's copy into the step's static inputs (host→device from pinned
         # memory, or device→device) runs on a copy stream while the current replay computes, instead of in front of it
@@ -286,6 +295,8 @@ class GraphedTrainStep:
                 break  # even number of staged collectives per step, or case (a): one graph replays safely
         self.graph, self.static_loss = self.graphs[0], self.losses[0]
         self.grad_norm = None
+        if hasattr(self.optimizer, "_record_captured_hyper"):
+            self.optimizer._record_captured_hyper()   # sync_lr() refuses a replay once any of them has changed
         # the host side of a replay (input staging on a copy stream, ordering against the replays that use the buffers, losses to pinned
         # memory on a side stream) is native: csrc/engine/step_pipeline.cpp
         self._io = _C.StepPipeline(dev.index if dev.index is not None else torch.cuda.current_device(), len(self.graphs), self.static_loss)
@@ -294,10 +305,12 @@ class GraphedTrainStep:
         """One training step on ``inputs`` (pinned host tensors or device tensors).  ``inputs_ready=True``: the caller guarantees
         that device-resident inputs are complete already (a GPU-resident dataset, a batch produced on another stream and
         synchronised) — their copy into the step's buffers then overlaps the previous step instead of queueing behind it."""
+        if hasattr(self.optimizer, "sync_lr"):
+            # scheduler changes of lr reach the captured step through a device scalar; a change of any other hyper-parameter is
+            # refused here, before anything of this step is enqueued
+            self.optimizer.sync_lr()
         i = self.replays % len(self.graphs)
         self._io.stage_inputs(i, self.input_sets[i % len(self.input_sets)], list(inputs), inputs_ready, self.double_buffer)
-        if hasattr(self.optimizer, "sync_lr"):
-            self.optimizer.sync_lr()  # scheduler changes reach the captured step through a device scalar
         self.graphs[i].replay()
         self._io.replayed(i)
         self.replays += 1

@@ -1,8 +1,14 @@
 """What the native optimizers (``SGD``, ``Adam``, ``AdamW``) share: the device-resident learning rate that a captured CUDA
-graph reads, and the checks that decide whether the update may ride on the reference ConvNet's last backward kernel."""
+graph reads, and the checks that decide whether the update may ride on the reference ConvNet's last backward kernel.
+
+The learning rate lives in a device scalar per group when the group says ``capturable=True``, and for every group once
+``engine.GraphedTrainStep`` has taken the optimizer: the captured kernels then read the scalar, and ``sync_lr()`` before each replay
+pushes a scheduler's change into it.  Every other hyper-parameter is a kernel argument baked into the graph; a replay after one of
+them changed is refused (``sync_lr``)."""
 from __future__ import annotations
 
 import math
+import operator
 import os
 from dataclasses import dataclass
 from typing import Callable, List, Optional, Tuple
@@ -25,14 +31,21 @@ class RidingOptimizer(torch.optim.Optimizer):
     """Base of the optimizers with a native multi-tensor update.  Bookkeeping (param_groups / state_dict) comes from
     ``torch.optim.Optimizer``."""
 
+    # the group keys ``_hyper`` reads besides ``lr`` (at least two, so that ``itemgetter`` returns a tuple); a subclass names its own
+    _FIXED_KEYS: Tuple[str, ...] = ()
+
     def __init__(self, params, defaults):
         super().__init__(params, defaults)
         self._lr_dev = {}           # group index -> (device scalar, last host value) when capturable
         self._rode = False
+        # set by engine.GraphedTrainStep: every group's lr in a device scalar, whatever its ``capturable`` says (the group's
+        # ``capturable`` is left alone: it is saved in state_dict)
+        self._lr_on_device = False
+        self._captured_hyper = None   # per group, the values of _FIXED_KEYS when GraphedTrainStep captured its step
 
     # ---- device-resident learning rate (CUDA-graph friendly schedulers) ------------------------------
     def _lr_tensor(self, gi: int, group, device) -> Optional[torch.Tensor]:
-        if not group.get("capturable") or device.type != "cuda":
+        if not (group.get("capturable") or self._lr_on_device) or device.type != "cuda":
             return None
         ent = self._lr_dev.get(gi)
         if ent is None:
@@ -43,10 +56,27 @@ class RidingOptimizer(torch.optim.Optimizer):
             ent[1] = float(group["lr"])
         return ent[0]
 
+    def _record_captured_hyper(self) -> None:
+        """Remember the hyper-parameters a captured step baked into its kernels (``sync_lr`` refuses a replay once they differ)."""
+        self._fixed_of = operator.itemgetter(*self._FIXED_KEYS)
+        self._captured_hyper = [self._fixed_of(g) for g in self.param_groups]
+
     def sync_lr(self) -> None:
         """Push ``param_groups[i]['lr']`` into the device scalars a captured step reads (call between
-        graph replays after a scheduler step; a no-op when nothing changed)."""
+        graph replays after a scheduler step; a no-op when nothing changed).  After ``engine.GraphedTrainStep`` has captured
+        a step, raises RuntimeError when any other hyper-parameter the update reads (momentum, betas, weight decay, …) has
+        changed since: the graph would replay the captured value.  Runs before every replay, so the check is one tuple
+        comparison per group."""
+        captured = self._captured_hyper
         for gi, group in enumerate(self.param_groups):
+            if captured is not None and gi < len(captured):
+                now = self._fixed_of(group)
+                if now != captured[gi]:
+                    key, was, new = next((k, a, b) for k, a, b in zip(self._FIXED_KEYS, captured[gi], now) if a != b)
+                    raise RuntimeError(
+                        f"{type(self).__name__}: hyper-parameter '{key}' of param_groups[{gi}] changed from {was} to {new} after "
+                        "the training step was captured in a CUDA graph, which would replay the captured value; only 'lr' can "
+                        "change between replays (a scheduler that also cycles momentum or betas needs an eager loop)")
             ent = self._lr_dev.get(gi)
             if ent is not None and ent[1] != float(group["lr"]):
                 ent[0].fill_(float(group["lr"]))

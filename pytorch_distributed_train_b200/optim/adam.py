@@ -6,7 +6,9 @@ Constructors, defaults, errors and state keys (``step``, ``exp_avg``, ``exp_avg_
 * the update of *all* fp32 contiguous CUDA parameters of a group is one sm_90a kernel launch (``ops.adam_step``) with the
   arithmetic of torch's single-tensor Adam; it is graph-capturable because ``step`` lives on the parameter's device as an fp32
   scalar (as in torch's capturable mode) and the kernel advances it itself;
-* ``lr`` lives in a device scalar when ``capturable=True`` so schedulers work under CUDA graphs (shared with ``SGD``);
+* ``lr`` lives in a device scalar when ``capturable=True``, and always once ``engine.GraphedTrainStep`` has taken the optimizer,
+  so schedulers work under CUDA graphs (shared with ``SGD``; the betas and the other hyper-parameters must not change between
+  replays: ``sync_lr``);
 * on one GPU the update can ride on the reference ConvNet's last backward kernel (:meth:`Adam.ride_on_backward`).
 
 CPU parameters, other dtypes and ``amsgrad=True`` take the reference math (torch's single-tensor arithmetic, op by op); ``amsgrad``
@@ -126,8 +128,11 @@ class Adam(RidingOptimizer):
         self._arm_rider(params, build, clip)
         return True
 
+    _FIXED_KEYS = ("betas", "eps", "weight_decay", "decoupled_weight_decay", "maximize")
+
     def _hyper(self, gi: int, group, device) -> dict:
-        """The update's hyper-parameters, as ``ops.adam_step`` and the rider description of the last backward kernel take them."""
+        """The update's hyper-parameters, as ``ops.adam_step`` and the rider description of the last backward kernel take them
+        (``lr`` and the group keys ``_FIXED_KEYS``)."""
         beta1, beta2 = group["betas"]
         return dict(lr=float(group["lr"]), lr_tensor=self._lr_tensor(gi, group, device), beta1=float(beta1), beta2=float(beta2),
                     eps=float(group["eps"]), weight_decay=float(group["weight_decay"]), decoupled=bool(group["decoupled_weight_decay"]),

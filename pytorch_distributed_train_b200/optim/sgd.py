@@ -7,7 +7,8 @@ autograd re-allocates them every backward.  Ours:
 * the update for *all* parameters is one sm_90a kernel launch (``ops.sgd_step``) over a pointer
   table — momentum, dampening, Nesterov and weight decay included — so it is graph-capturable
   and launch-count-free as the model grows;
-* ``lr`` lives in a device scalar when ``capturable=True`` so schedulers work under CUDA graphs;
+* ``lr`` lives in a device scalar when ``capturable=True``, and always once ``engine.GraphedTrainStep`` has taken the optimizer,
+  so schedulers work under CUDA graphs (the other hyper-parameters must not change between replays: ``sync_lr``);
 * ``zero_grad(set_to_none=False)`` keeps gradients as views of the DDP bucket (no re-allocation,
   no copy into the bucket next step). ``set_to_none=True`` (the reference's default behaviour)
   still works — the reducer re-homes gradients on the next backward.
@@ -82,8 +83,11 @@ class SGD(RidingOptimizer):
         self._arm_rider(params, build, clip)
         return True
 
+    _FIXED_KEYS = ("momentum", "dampening", "weight_decay", "nesterov", "maximize")
+
     def _hyper(self, gi: int, group, device) -> dict:
-        """The update's hyper-parameters, as ``ops.sgd_step`` and the rider description of the last backward kernel take them."""
+        """The update's hyper-parameters, as ``ops.sgd_step`` and the rider description of the last backward kernel take them
+        (``lr`` and the group keys ``_FIXED_KEYS``)."""
         return dict(lr=float(group["lr"]), lr_tensor=self._lr_tensor(gi, group, device), momentum=float(group["momentum"]),
                     dampening=float(group["dampening"]), weight_decay=float(group["weight_decay"]), nesterov=bool(group["nesterov"]),
                     maximize=bool(group["maximize"]))
@@ -105,7 +109,11 @@ class SGD(RidingOptimizer):
         there sees an already-updated model, and a skipped ``step()`` is not expressible in this mode.  Clipping is expressible
         through ``engine.GraphedTrainStep(max_grad_norm=…)``, which does not fuse the optimizer into the reduction then.  Takes
         effect on the first ``step()`` after the reducer has settled its bucket layout; until then (and whenever the
-        preconditions fail) the ordinary path runs."""
+        preconditions fail) the ordinary path runs.
+
+        The update of a backward uses the hyper-parameters in ``param_groups`` when DDP's forward starts: a scheduler stepped
+        (or a value set) before the forward takes effect in that iteration, as on the unfused path; a change made between the
+        forward and ``backward()`` is not picked up until the next forward."""
         self._ddp = ddp
         return self
 
@@ -140,19 +148,23 @@ class SGD(RidingOptimizer):
         ddp._rearm_fused_optimizer = self._arm_fused
         self._arm_fused()
 
-    def _arm_fused(self) -> None:
-        """(Re-)install the update the reducer applies with every reduce chunk of the *next* backward."""
+    def _arm_fused(self, changed_only: bool = False) -> None:
+        """(Re-)install the update the reducer applies with every reduce chunk of the *next* backward.  DDP calls this when its
+        forward starts with ``changed_only=True``: the reducer is re-armed only when a hyper-parameter or the first-step flag
+        differs from what it holds (a device-resident lr is refreshed here either way)."""
         ddp, group = self._ddp, self.param_groups[0]
         first = False
         if group["momentum"] != 0:
             # zero buffer + "not first" is exact when dampening == 0 (b = μ·0 + g); a uniform first step sets the flag
             first = all(self.state[p].get("momentum_buffer") is None for p in ddp._params)
-        self._armed = (float(group["lr"]), bool(first))
-        ddp.reducer.set_fused_sgd(ddp.param_arena, self._flat_momentum, lr=float(group["lr"]),
-                                  lr_tensor=self._lr_tensor(0, group, ddp.param_arena.device), momentum=float(group["momentum"]),
-                                  dampening=float(group["dampening"]), weight_decay=float(group["weight_decay"]),
-                                  nesterov=bool(group["nesterov"]), first_step=bool(first), bcast=ddp.tail_broadcast_buffer(),
-                                  bcast_root=0)
+        h = self._hyper(0, group, ddp.param_arena.device)
+        armed = (h["lr"], h["lr_tensor"] is not None, h["momentum"], h["dampening"], h["weight_decay"], h["nesterov"], first)
+        if changed_only and armed == self._armed:
+            return
+        self._armed = armed
+        ddp.reducer.set_fused_sgd(ddp.param_arena, self._flat_momentum, lr=h["lr"], lr_tensor=h["lr_tensor"], momentum=h["momentum"],
+                                  dampening=h["dampening"], weight_decay=h["weight_decay"], nesterov=h["nesterov"], first_step=first,
+                                  bcast=ddp.tail_broadcast_buffer(), bcast_root=0)
 
     def _fused_step(self) -> bool:
         ddp = self._ddp
@@ -166,8 +178,7 @@ class SGD(RidingOptimizer):
             for p, off in zip(ddp._params, ddp._param_offsets):
                 if self.state[p].get("momentum_buffer") is None:
                     self.state[p]["momentum_buffer"] = self._flat_momentum[off:off + p.numel()].view(p.shape)
-        if self._armed != (float(group["lr"]), False):
-            self._arm_fused()   # first-step flag drops after one update; a changed learning rate is picked up
+        # the first-step flag drops, and changed hyper-parameters are picked up, when DDP's next forward starts (_arm_fused)
         return True
 
     def load_state_dict(self, state_dict) -> None:

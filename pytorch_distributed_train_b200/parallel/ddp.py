@@ -384,6 +384,9 @@ class DistributedDataParallel(nn.Module):
         if sync:
             self.reducer.prepare_for_forward()
             self._maybe_rebuild_buckets()
+            rearm = getattr(self, "_rearm_fused_optimizer", None)
+            if rearm is not None:
+                rearm(changed_only=True)   # this iteration's update uses the hyper-parameters set before its forward
         if self._join_active:
             self._join_notify_active()
         if self.broadcast_buffers and self.require_forward_param_sync and self.module.training and not self._buffers_ride_on_reduce():
