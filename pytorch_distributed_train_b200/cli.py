@@ -9,7 +9,7 @@ Extra flags cover what the reference hard-codes: ``--init-method`` (its LAN addr
 ``tcp://10.9.1.2:34567`` only works on the author's network, ref: ddp_example.py:110; we default
 to loopback with a free port), ``--data synthetic|mnist``, ``--model``, ``--comm fused|nccl``, ``--algo``,
 ``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw), ``--lr``,
-``--momentum``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--ema-decay``,
+``--momentum``, ``--amsgrad``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--ema-decay``,
 ``--checkpoint`` / ``--resume``, ``--eval`` (test loss and accuracy after every epoch).
 """
 from __future__ import annotations
@@ -48,6 +48,8 @@ def build_parser() -> argparse.ArgumentParser:
                    help="optimizer: SGD (the reference's), Adam or AdamW, each a native multi-tensor kernel")
     p.add_argument("--lr", default=1e-4, type=float, help="learning rate (reference: 1e-4)")
     p.add_argument("--momentum", default=None, type=float, help="SGD momentum (default 0; not accepted with Adam / AdamW)")
+    p.add_argument("--amsgrad", default=False, action="store_true",
+                   help="Adam / AdamW with AMSGrad: the running maximum of exp_avg_sq in the denominator (not accepted with SGD)")
     p.add_argument("--weight-decay", default=None, type=float,
                    help="weight decay (default: 0 for SGD and Adam, 1e-2 for AdamW, torch's defaults)")
     p.add_argument("--clip-grad-norm", default=None, type=float, metavar="MAX",
@@ -74,19 +76,21 @@ def build_parser() -> argparse.ArgumentParser:
 
 
 def make_optimizer(args, params):
-    """The optimizer ``--optimizer`` / ``--lr`` / ``--momentum`` / ``--weight-decay`` describe."""
+    """The optimizer ``--optimizer`` / ``--lr`` / ``--momentum`` / ``--amsgrad`` / ``--weight-decay`` describe."""
     import pytorch_distributed_train_b200 as pdt
 
     kw = {} if args.weight_decay is None else {"weight_decay": args.weight_decay}
     if args.optimizer == "sgd":
         return pdt.optim.SGD(params, args.lr, momentum=args.momentum or 0.0, **kw)
     cls = pdt.optim.Adam if args.optimizer == "adam" else pdt.optim.AdamW
-    return cls(params, args.lr, **kw)
+    return cls(params, args.lr, amsgrad=getattr(args, "amsgrad", False), **kw)
 
 
 def check_args(p: argparse.ArgumentParser, args) -> None:
     if args.optimizer != "sgd" and args.momentum is not None:
         p.error(f"--momentum applies to SGD only; {args.optimizer} takes its moments from its betas")
+    if args.optimizer == "sgd" and getattr(args, "amsgrad", False):
+        p.error("--amsgrad applies to Adam and AdamW only (--optimizer adam | adamw)")
     if args.clip_grad_norm is not None and not args.clip_grad_norm > 0:
         p.error(f"--clip-grad-norm must be positive (got {args.clip_grad_norm})")
     if args.accumulation_steps < 1:

@@ -103,7 +103,7 @@ SgdRider sgd_rider(const py::dict& d) {
 }
 
 // {"kind": "adam", "params", "prev_grads", "exp_avg", "exp_avg_sq", "step" (fp32 scalars on the device), "lr", "lr_tensor", "beta1",
-// "beta2", "eps", "weight_decay", "decoupled", "maximize"}
+// "beta2", "eps", "weight_decay", "decoupled", "maximize"}, and for AMSGrad "max_exp_avg_sq" (ten tensors; amsgrad_rider below)
 AdamRider adam_rider(const py::dict& d) {
   AdamRider r;
   const TensorList ms = tensors(d, "exp_avg"), vs = tensors(d, "exp_avg_sq"), steps = tensors(d, "step");
@@ -119,6 +119,21 @@ AdamRider adam_rider(const py::dict& d) {
   });
   r.h = adam_hyper(d["lr"].cast<double>(), d["lr_tensor"].cast<c10::optional<at::Tensor>>(), d["beta1"].cast<double>(), d["beta2"].cast<double>(),
                    d["eps"].cast<double>(), d["weight_decay"].cast<double>(), d["decoupled"].cast<bool>(), d["maximize"].cast<bool>());
+  return r;
+}
+// the "adam" description with a "max_exp_avg_sq" entry
+AmsgradRider amsgrad_rider(const py::dict& d) {
+  AmsgradRider r;
+  static_cast<AdamRider&>(r) = adam_rider(d);
+  const TensorList vmax = tensors(d, "max_exp_avg_sq"), params = tensors(d, "params");
+  TORCH_CHECK(vmax.size() == 10, "convnet_l1_bwd_wgrad: adam lists have the wrong length");
+  for (int k = 0; k < 10; ++k) {
+    if (!r.p[k]) continue;
+    TORCH_CHECK(vmax[k].has_value() && vmax[k]->numel() == params[k]->numel(), "convnet_l1_bwd_wgrad: max_exp_avg_sq of parameter ", k,
+                " missing or of the wrong size");
+    chk(*vmax[k], "max_exp_avg_sq");
+    r.vmax[k] = vmax[k]->data_ptr<float>();
+  }
   return r;
 }
 
@@ -491,8 +506,9 @@ void register_cuda_bindings(py::module_& m) {
     const auto d = rider.cast<py::dict>();
     const auto kind = d["kind"].cast<std::string>();
     TORCH_CHECK(kind == "sgd" || kind == "adam", "convnet_l1_bwd_wgrad: rider kind must be 'sgd' or 'adam' (got '", kind, "')");
-    if (kind == "adam") launch_rider(adam_rider(d));
-    else launch_rider(sgd_rider(d));
+    if (kind == "sgd") launch_rider(sgd_rider(d));
+    else if (d.contains("max_exp_avg_sq")) launch_rider(amsgrad_rider(d));
+    else launch_rider(adam_rider(d));
   }, py::arg("dp"), py::arg("y"), py::arg("x"), py::arg("saved"), py::arg("gamma"), py::arg("beta"), py::arg("dgamma"), py::arg("dbeta"),
      py::arg("dw"), py::arg("db"), py::arg("dy2_pad"), py::arg("x2_pad"), py::arg("dysum2"), py::arg("dw2"), py::arg("db2"),
      py::arg("rider") = py::none(), py::kw_only(), py::arg("clip") = py::none(), py::arg("accumulate") = false);
@@ -792,9 +808,13 @@ void register_cuda_bindings(py::module_& m) {
   });
   m.def("adam_multi", [](std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avgs,
                          std::vector<at::Tensor> exp_avg_sqs, std::vector<at::Tensor> steps, double lr, c10::optional<at::Tensor> lr_tensor,
-                         double beta1, double beta2, double eps, double weight_decay, bool decoupled, bool maximize) {
+                         double beta1, double beta2, double eps, double weight_decay, bool decoupled, bool maximize,
+                         c10::optional<std::vector<at::Tensor>> max_exp_avg_sqs) {
     const size_t n = params.size();
     TORCH_CHECK(grads.size() == n && exp_avgs.size() == n && exp_avg_sqs.size() == n && steps.size() == n, "adam_multi: list lengths differ");
+    // max_exp_avg_sqs: AMSGrad (amsgrad_multi_kernel)
+    const bool ams = max_exp_avg_sqs.has_value();
+    TORCH_CHECK(!ams || max_exp_avg_sqs->size() == n, "adam_multi: list lengths differ");
     if (n == 0) return;
     c10::cuda::CUDAGuard g(params[0].device());
     const AdamHyper h = adam_hyper(lr, lr_tensor, beta1, beta2, eps, weight_decay, decoupled, maximize);
@@ -803,7 +823,7 @@ void register_cuda_bindings(py::module_& m) {
     // every launch leaves the word at zero
     unsigned int* ticket = scratch(params[0]).counter + kAdamTicketWord;
     for (size_t base = 0; base < n; base += AdamTensorList::kMax) {
-      AdamTensorList tl;
+      AmsgradTensorList tl;
       tl.count = static_cast<int>(std::min<size_t>(AdamTensorList::kMax, n - base));
       for (int i = 0; i < tl.count; ++i) {
         const size_t j = base + i;
@@ -818,8 +838,16 @@ void register_cuda_bindings(py::module_& m) {
         tl.v[i] = exp_avg_sqs[j].data_ptr<float>();
         tl.step[i] = steps[j].data_ptr<float>();
         tl.n[i] = static_cast<int>(numel);
+        if (ams) {
+          const at::Tensor& vm = (*max_exp_avg_sqs)[j];
+          chk(vm, "max_exp_avg_sq");
+          TORCH_CHECK(vm.numel() == numel, "adam_multi: bad tensor sizes");
+          TORCH_CHECK(vm.device() == params[0].device(), "adam_multi: all tensors on one device");
+          tl.vmax[i] = vm.data_ptr<float>();
+        }
       }
-      launch_adam_multi(tl, h, ticket, st);
+      if (ams) launch_adam_multi(tl, h, ticket, st);
+      else launch_adam_multi(static_cast<const AdamTensorList&>(tl), h, ticket, st);
     }
   });
   // Gradient-norm clipping: returns the total norm (a 0-d view of a [2] buffer whose second element is the clip coefficient);

@@ -15,7 +15,7 @@
 //                              wgmma (warps 0..3; K-major copies of x, written in the barrier's shadow, and of dy)
 //   convnet_l1_bwd_kernel      MaxPool/ReLU/BN backward ──barrier── conv1 weight gradient (mma.sync) ──barrier── conv1 fold;
 //                              conv2's weight gradient is folded in the shadow of the first barrier, and — on one GPU — the
-//                              threads that write the folded gradients apply the optimizer update (SgdRider / AdamRider)
+//                              threads that write the folded gradients apply the optimizer update (SgdRider / AdamRider / AmsgradRider)
 //
 // All cross-CTA sums are "every CTA writes one partial row, barrier, every CTA folds the rows in the same fixed order",
 // so results are bit-reproducible and identical in every CTA.  The kernels are launched cooperatively (all CTAs
@@ -432,8 +432,10 @@ __device__ __forceinline__ void adam_factors(const AdamRider& r, float* f, int t
   }
 }
 
-// One Adam update (the arithmetic of adam_multi_kernel, ops_simt.cu) of element i of parameter k with gradient g.
-__device__ __forceinline__ void adam_apply(const AdamRider& r, int k, int i, float g, const float* f) {
+// One Adam update (the arithmetic of adam_multi_kernel / amsgrad_multi_kernel, ops_simt.cu) of element i of parameter k with
+// gradient g.  R: AdamRider or AmsgradRider, possibly in a ClipRider.
+template <class R>
+__device__ __forceinline__ void adam_apply(const R& r, int k, int i, float g, const float* f) {
   float gv = r.h.maximize ? -g : g;
   float* p = r.p[k] + i;
   float* m = r.m[k] + i;
@@ -447,7 +449,13 @@ __device__ __forceinline__ void adam_apply(const AdamRider& r, int k, int i, flo
   const float vv = fmaf(f[kAdamLr + 3] * gv, gv, f[kAdamLr + 2] * *v);
   *m = mv;
   *v = vv;
-  *p = fmaf(-f[k], mv / (sqrtf(vv) / f[10 + k] + r.h.eps), pv);
+  float den = vv;
+  if constexpr (std::is_base_of_v<AmsgradRider, R>) {
+    float* vm = r.vmax[k] + i;
+    den = nan_max(*vm, vv);
+    *vm = den;
+  }
+  *p = fmaf(-f[k], mv / (sqrtf(den) / f[10 + k] + r.h.eps), pv);
 }
 
 // Gradient-norm clipping (ClipRider): one gradient element g into a thread's accumulator — Σg², or max |g| keeping a NaN.
@@ -457,9 +465,11 @@ template <class R>
 __device__ __forceinline__ float clip_comb(const R& r, float a, float b) { return r.norm_inf ? nan_max(a, b) : a + b; }
 
 template <class R>
-constexpr bool kClipRider = std::is_same_v<R, ClipRider<SgdRider>> || std::is_same_v<R, ClipRider<AdamRider>>;
+constexpr bool kClipRider =
+    std::is_same_v<R, ClipRider<SgdRider>> || std::is_same_v<R, ClipRider<AdamRider>> || std::is_same_v<R, ClipRider<AmsgradRider>>;
 template <class R>
-constexpr bool kAdamRider = std::is_same_v<R, AdamRider> || std::is_same_v<R, ClipRider<AdamRider>>;
+constexpr bool kAdamRider = std::is_same_v<R, AdamRider> || std::is_same_v<R, ClipRider<AdamRider>> || std::is_same_v<R, AmsgradRider> ||
+                            std::is_same_v<R, ClipRider<AmsgradRider>>;
 
 // Element i of parameter k's gradient is final with value g: a ClipRider adds it to this thread's share ca of the norm (the update
 // waits for the coefficient), the others apply their update.  The caller tests whether the rider is on and the parameter takes part.
@@ -480,7 +490,8 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
                       // conv2's weight gradient, folded from the per-image partials [B][400][32] and Σdy rows [B][32]
                       const float* __restrict__ wpart, const float* __restrict__ dysum2, float* dw2, float* db2, const __grid_constant__ Rider sr) {
   constexpr bool kClip = kClipRider<Rider>, kAdam = kAdamRider<Rider>;
-  static_assert(kAdam || std::is_base_of_v<SgdRider, Rider>, "convnet_l1_bwd_kernel: SgdRider or AdamRider, or either in a ClipRider");
+  static_assert(kAdam || std::is_base_of_v<SgdRider, Rider>,
+                "convnet_l1_bwd_kernel: SgdRider, AdamRider or AmsgradRider, or one of them in a ClipRider");
   extern __shared__ __align__(16) float dsm[];
   float* dys = dsm;                  // [784][16]
   float* fold = dsm + 784 * 16;      // [25 warps][16][32]
@@ -1787,6 +1798,8 @@ PDT_L1_BWD_WGRAD(SgdRider)
 PDT_L1_BWD_WGRAD(AdamRider)
 PDT_L1_BWD_WGRAD(ClipRider<SgdRider>)
 PDT_L1_BWD_WGRAD(ClipRider<AdamRider>)
+PDT_L1_BWD_WGRAD(AmsgradRider)
+PDT_L1_BWD_WGRAD(ClipRider<AmsgradRider>)
 #undef PDT_L1_BWD_WGRAD
 
 void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const float* g1, const float* be1, float* y1, float* p1, float* saved1,

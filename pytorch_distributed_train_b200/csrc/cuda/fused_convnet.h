@@ -41,7 +41,11 @@ struct AdamRider {
   int n_prev[4] = {};
   AdamHyper h{};
 };
-// Either rider with gradient-norm clipping in front of the update (torch.nn.utils.clip_grad_norm_, norm_type 2 or inf).  Every CTA
+// The Adam rider with AMSGrad (the arithmetic of amsgrad_multi_kernel): vmax = max(vmax, exp_avg_sq), a NaN kept, is the denominator's.
+struct AmsgradRider : AdamRider {
+  float* vmax[10] = {};        // max_exp_avg_sq
+};
+// Any of the riders with gradient-norm clipping in front of the update (torch.nn.utils.clip_grad_norm_, norm_type 2 or inf).  Every CTA
 // adds up the squares (or the max |g|) of the gradient elements it sees — those of parameters 6..9 in the shadow of the first
 // grid barrier, those of 0..5 as it folds them (4, 5 in that shadow too) — and writes one partial; after one more grid barrier every CTA folds the B
 // partials in the same order (fp64), derives the same coefficient, and in a grid-stride pass writes g·coef back to every
@@ -60,7 +64,8 @@ struct ClipRider : Base {
 void launch_conv2_wgrad_partials(const float* dy2_pad, const float* x2_pad, int B, float* wpart, cudaStream_t st);
 // Layer-1 backward: dp [B,18,18,16] frame (interior read) → dgamma/dbeta [16], dw [16,1,5,5], db [16]; it also folds conv2's weight
 // gradient: the per-image partials wpart and Σdy rows dysum2 [B,32] → dw2 [32,16,5,5], db2 [32], in the shadow of the kernel's first
-// grid barrier.  partials: B·32, partials_w: B·512 floats.  Rider: SgdRider or AdamRider, or either one in a ClipRider.
+// grid barrier.  partials: B·32, partials_w: B·512 floats.  Rider: SgdRider, AdamRider or AmsgradRider, or one of them in a
+// ClipRider.
 // accumulate: gradient accumulation — every gradient written (dgamma, dbeta, dw, db, dw2, db2) becomes g_old + this batch's value, and
 // the rider updates with (and clips) the accumulated gradient.
 template <class Rider = SgdRider>

@@ -176,6 +176,12 @@ struct AdamHyper {
 // ticket: one zeroed counter word; every block takes a ticket after it has read its step, the last one advances all steps and
 // resets the word to zero.
 void launch_adam_multi(const AdamTensorList& tl, AdamHyper h, unsigned int* ticket, cudaStream_t st);
+// AMSGrad (torch's amsgrad=True): the same update with the running maximum vmax = max(vmax, exp_avg_sq) (a NaN in either stays,
+// as torch.maximum's) in the denominator.
+struct AmsgradTensorList : AdamTensorList {
+  float* vmax[kMax];  // max_exp_avg_sq
+};
+void launch_adam_multi(const AmsgradTensorList& tl, AdamHyper h, unsigned int* ticket, cudaStream_t st);
 
 // Gradient-norm clipping (torch.nn.utils.clip_grad_norm_ with norm_type 2 or inf) as two launches per table set: the norm, then
 // the scale.  A set of more than kMax tensors is split into tables launched back to back; every block of every table writes one

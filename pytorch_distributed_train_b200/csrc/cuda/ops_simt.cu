@@ -935,9 +935,11 @@ __global__ void __launch_bounds__(256) sgd_multi_kernel(SgdTensorList tl, SgdHyp
 // =====================================================================================================
 // Multi-tensor Adam / AdamW: same layout as sgd_multi_kernel.  Thread 0 of every block reads its tensor's step s and forms
 // the bias corrections of step s + 1 in double; the block that takes the last ticket writes s + 1 back for every tensor
-// (no block reads a step after it has taken its ticket) and resets the ticket word for the next launch.
+// (no block reads a step after it has taken its ticket) and resets the ticket word for the next launch.  AMS (AMSGrad):
+// vmax = max(vmax, v) keeping a NaN, and the denominator is formed from vmax instead of v.
 // =====================================================================================================
-__global__ void __launch_bounds__(256) adam_multi_kernel(AdamTensorList tl, AdamHyper h, unsigned int* ticket) {
+template <bool AMS, class TL>
+__device__ __forceinline__ void adam_multi_body(const TL& tl, const AdamHyper& h, unsigned int* ticket) {
   const int t = blockIdx.y;
   __shared__ float s_f[3];
   if (threadIdx.x == 0) {
@@ -959,6 +961,8 @@ __global__ void __launch_bounds__(256) adam_multi_kernel(AdamTensorList tl, Adam
   const float* __restrict__ g = tl.g[t];
   float* __restrict__ m = tl.m[t];
   float* __restrict__ v = tl.v[t];
+  float* __restrict__ vmax = nullptr;
+  if constexpr (AMS) vmax = tl.vmax[t];
   const float step_size = s_f[0], bc2s = s_f[1], decay = s_f[2];
   const float omb1 = static_cast<float>(1.0 - h.beta1), b2 = static_cast<float>(h.beta2), omb2 = static_cast<float>(1.0 - h.beta2);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -972,9 +976,22 @@ __global__ void __launch_bounds__(256) adam_multi_kernel(AdamTensorList tl, Adam
     const float vv = fmaf(omb2 * gv, gv, b2 * v[i]);
     m[i] = mv;
     v[i] = vv;
-    p[i] = fmaf(-step_size, mv / (sqrtf(vv) / bc2s + h.eps), pv);
+    float den = vv;
+    if constexpr (AMS) {
+      den = nan_max(vmax[i], vv);
+      vmax[i] = den;
+    }
+    p[i] = fmaf(-step_size, mv / (sqrtf(den) / bc2s + h.eps), pv);
   }
 }
+__global__ void __launch_bounds__(256) adam_multi_kernel(AdamTensorList tl, AdamHyper h, unsigned int* ticket) {
+  adam_multi_body<false>(tl, h, ticket);
+}
+__global__ void __launch_bounds__(256) amsgrad_multi_kernel(AmsgradTensorList tl, AdamHyper h, unsigned int* ticket) {
+  adam_multi_body<true>(tl, h, ticket);
+}
+// a kernel's parameters take at most 4 KiB
+static_assert(sizeof(AmsgradTensorList) + sizeof(AdamHyper) + sizeof(unsigned int*) <= 4096, "amsgrad_multi_kernel: parameters too large");
 
 // =====================================================================================================
 // Gradient-norm clipping: same layout as sgd_multi_kernel.  grad_norm_multi_kernel: every block writes one partial (fp32 Σg² or
@@ -1267,6 +1284,14 @@ void launch_adam_multi(const AdamTensorList& tl, AdamHyper h, unsigned int* tick
   for (int i = 0; i < tl.count; ++i) maxn = std::max(maxn, tl.n[i]);
   const int bx = std::max(1, std::min(64, (maxn + 1023) / 1024));
   adam_multi_kernel<<<dim3(bx, tl.count), 256, 0, st>>>(tl, h, ticket);
+  check_launch("adam_multi");
+}
+void launch_adam_multi(const AmsgradTensorList& tl, AdamHyper h, unsigned int* ticket, cudaStream_t st) {
+  if (tl.count == 0) return;
+  int maxn = 0;
+  for (int i = 0; i < tl.count; ++i) maxn = std::max(maxn, tl.n[i]);
+  const int bx = std::max(1, std::min(64, (maxn + 1023) / 1024));
+  amsgrad_multi_kernel<<<dim3(bx, tl.count), 256, 0, st>>>(tl, h, ticket);
   check_launch("adam_multi");
 }
 

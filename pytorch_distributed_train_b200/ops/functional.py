@@ -583,11 +583,14 @@ def sgd_step(params, grads, momentum_bufs, lr, momentum=0.0, dampening=0.0, weig
 
 
 def adam_step(params, grads, exp_avgs, exp_avg_sqs, steps, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0,
-              decoupled=False, maximize=False, lr_tensor=None) -> None:
+              decoupled=False, maximize=False, lr_tensor=None, max_exp_avg_sqs=None) -> None:
     """One Adam (``decoupled=False``) or AdamW update of every tensor, one kernel launch per 48 tensors.  ``steps`` are the fp32
-    step counts on the device: the launch uses step + 1 for the bias corrections and stores it, so a replayed graph advances it."""
+    step counts on the device: the launch uses step + 1 for the bias corrections and stores it, so a replayed graph advances it.
+    ``max_exp_avg_sqs``: AMSGrad — each becomes ``torch.maximum(max_exp_avg_sq, exp_avg_sq)`` (a NaN stays) and the denominator
+    is formed from it."""
     _C.adam_multi(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), list(steps), float(lr), lr_tensor, float(beta1),
-                  float(beta2), float(eps), float(weight_decay), bool(decoupled), bool(maximize))
+                  float(beta2), float(eps), float(weight_decay), bool(decoupled), bool(maximize),
+                  None if max_exp_avg_sqs is None else list(max_exp_avg_sqs))
 
 
 def grad_norm_clip(grads, max_norm, norm_type=2.0, scale=True) -> torch.Tensor:

@@ -9,10 +9,11 @@ Constructors, defaults, errors and state keys (``step``, ``exp_avg``, ``exp_avg_
 * ``lr`` lives in a device scalar when ``capturable=True``, and always once ``engine.GraphedTrainStep`` has taken the optimizer,
   so schedulers work under CUDA graphs (shared with ``SGD``; the betas and the other hyper-parameters must not change between
   replays: ``sync_lr``);
+* ``amsgrad=True`` runs the same kernels with the running maximum ``max_exp_avg_sq`` as a fourth state tensor (``torch.maximum``'s
+  NaN-keeping max, then the denominator from it);
 * on one GPU the update can ride on the reference ConvNet's last backward kernel (:meth:`Adam.ride_on_backward`).
 
-CPU parameters, other dtypes and ``amsgrad=True`` take the reference math (torch's single-tensor arithmetic, op by op); ``amsgrad``
-has no kernel.
+CPU parameters, other dtypes and ``fused=False`` take the reference math (torch's single-tensor arithmetic, op by op).
 """
 from __future__ import annotations
 
@@ -105,38 +106,38 @@ class Adam(RidingOptimizer):
     # ---- single GPU: the update rides on the model's last backward kernel ---------------------------------
     def ride_on_backward(self, model, clip=None) -> bool:
         """Let the reference ConvNet's last backward kernel apply this optimizer's update (csrc/cuda/fused_convnet.cu: AdamRider).
-        Same contract, preconditions and ``clip = (max_norm, norm_type, norm_out)`` as :meth:`SGD.ride_on_backward`; ``amsgrad`` and
-        ``fused=False`` do not ride.  Returns False (and changes nothing) when the model / optimizer combination does not qualify."""
+        Same contract, preconditions and ``clip = (max_norm, norm_type, norm_out)`` as :meth:`SGD.ride_on_backward`; with ``amsgrad``
+        the kernel also keeps ``max_exp_avg_sq`` (AmsgradRider).  ``fused=False`` does not ride.  Returns False (and changes nothing)
+        when the model / optimizer combination does not qualify."""
         params = self._qualify_rider(model)
         if params is None or (clip is not None and not self._clip_qualifies(clip, params)):
             return False
-        group = self.param_groups[0]
-        if group["amsgrad"] or group["fused"] is False:
+        if self.param_groups[0]["fused"] is False:
             return False
 
         def build(prev_grads):
-            g = self.param_groups[0]
-            if g["amsgrad"]:
-                return None
-            states = [self._state(q, False) for q in params]
+            hyper = self._hyper(0, self.param_groups[0], params[0].device)
+            amsgrad = hyper.pop("amsgrad")
+            states = [self._state(q, amsgrad) for q in params]
             if not all(st["step"].is_cuda and st["step"].dtype == torch.float32 for st in states):
                 return None   # leave this iteration to step()
+            if amsgrad:
+                hyper["max_exp_avg_sq"] = [st["max_exp_avg_sq"] for st in states]
             return dict(kind="adam", params=params, prev_grads=list(prev_grads), exp_avg=[st["exp_avg"] for st in states],
-                        exp_avg_sq=[st["exp_avg_sq"] for st in states], step=[st["step"] for st in states],
-                        **self._hyper(0, g, params[0].device))
+                        exp_avg_sq=[st["exp_avg_sq"] for st in states], step=[st["step"] for st in states], **hyper)
 
         self._arm_rider(params, build, clip)
         return True
 
-    _FIXED_KEYS = ("betas", "eps", "weight_decay", "decoupled_weight_decay", "maximize")
+    _FIXED_KEYS = ("betas", "eps", "weight_decay", "decoupled_weight_decay", "maximize", "amsgrad")
 
     def _hyper(self, gi: int, group, device) -> dict:
         """The update's hyper-parameters, as ``ops.adam_step`` and the rider description of the last backward kernel take them
-        (``lr`` and the group keys ``_FIXED_KEYS``)."""
+        (``lr`` and the group keys ``_FIXED_KEYS``; the caller pops ``amsgrad``, which decides whether ``max_exp_avg_sq`` is passed)."""
         beta1, beta2 = group["betas"]
         return dict(lr=float(group["lr"]), lr_tensor=self._lr_tensor(gi, group, device), beta1=float(beta1), beta2=float(beta2),
                     eps=float(group["eps"]), weight_decay=float(group["weight_decay"]), decoupled=bool(group["decoupled_weight_decay"]),
-                    maximize=bool(group["maximize"]))
+                    maximize=bool(group["maximize"]), amsgrad=bool(group["amsgrad"]))
 
     # ---- the update ---------------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -163,21 +164,23 @@ class Adam(RidingOptimizer):
                 continue
             amsgrad = group["amsgrad"]
             states = [self._state(p, amsgrad) for p in params]
-            native = group["fused"] is not False and not amsgrad and params[0].is_cuda and ops.native_available() and all(
+            native = group["fused"] is not False and params[0].is_cuda and ops.native_available() and all(
                 p.dtype == torch.float32 and p.is_contiguous() and g.dtype == torch.float32 and g.is_contiguous() and p.device == params[0].device
                 for p, g in zip(params, grads))
             if native:
+                hyper = self._hyper(gi, group, params[0].device)
+                vmax = [st["max_exp_avg_sq"] for st in states] if hyper.pop("amsgrad") else None
                 ops.adam_step(params, grads, [st["exp_avg"] for st in states], [st["exp_avg_sq"] for st in states],
-                              [st["step"] for st in states], **self._hyper(gi, group, params[0].device))
+                              [st["step"] for st in states], **hyper, max_exp_avg_sqs=vmax)
                 continue
             if group["fused"]:
-                raise RuntimeError("Adam(fused=True): the native kernel takes fp32 contiguous CUDA parameters without amsgrad")
+                raise RuntimeError("Adam(fused=True): the native kernel takes fp32 contiguous CUDA parameters on one device")
             self._reference_step(group, params, grads, states)
         return loss
 
     @staticmethod
     def _reference_step(group, params, grads, states) -> None:
-        """torch's single-tensor Adam, op by op (CPU parameters, other dtypes, amsgrad)."""
+        """torch's single-tensor Adam, op by op (CPU parameters, other dtypes, ``fused=False``)."""
         lr, (beta1, beta2), eps, wd = group["lr"], group["betas"], group["eps"], group["weight_decay"]
         for p, g, st in zip(params, grads, states):
             g = -g if group["maximize"] else g

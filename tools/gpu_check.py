@@ -21,6 +21,7 @@ GROUPS = {
     "convnet": ["tests/test_gpu_kernels.py::test_convnet_fused_matches_unfused"],
     "ddp1": ["tests/test_gpu_kernels.py::test_single_gpu_ddp_and_graphed_step"],
     "adam": ["tests/test_adam.py"],
+    "amsgrad": ["tests/test_adam_amsgrad.py"],
     "clip": ["tests/test_clip_grad.py"],
     "average": ["tests/test_averaged_model.py"],
     "accum": ["tests/test_grad_accumulation.py"],

@@ -1,9 +1,11 @@
 #!/usr/bin/env python
-"""Device time of one graphed training step of the reference ConvNet (batch 100, one GPU) with five optimizers:
+"""Device time of one graphed training step of the reference ConvNet (batch 100, one GPU) with seven optimizers:
 
   pdt SGD, pdt Adam, pdt AdamW               (native update; on one GPU it rides on the last backward kernel)
+  pdt AdamW(amsgrad=True)                    (the same with the running maximum max_exp_avg_sq: AmsgradRider)
   torch AdamW(capturable=True, foreach=True) (torch's multi-tensor kernels, replayed inside the same graph)
   torch AdamW(capturable=True, fused=True)   (torch's fused kernel, replayed inside the same graph)
+  torch AdamW(amsgrad=True, capturable=True, fused=True)
 
 With ``--max-grad-norm X`` four more arms clip the global gradient norm to X in the same rounds:
 
@@ -79,8 +81,10 @@ def main():
         "pdt_sgd": lambda ps: pdt.optim.SGD(ps, lr),
         "pdt_adam": lambda ps: pdt.optim.Adam(ps, lr),
         "pdt_adamw": lambda ps: pdt.optim.AdamW(ps, lr),
+        "pdt_adamw_amsgrad": lambda ps: pdt.optim.AdamW(ps, lr, amsgrad=True),
         "torch_adamw_foreach": lambda ps: torch.optim.AdamW(ps, lr, capturable=True, foreach=True),
         "torch_adamw_fused": lambda ps: torch.optim.AdamW(ps, lr, capturable=True, fused=True),
+        "torch_adamw_amsgrad_fused": lambda ps: torch.optim.AdamW(ps, lr, amsgrad=True, capturable=True, fused=True),
     }
     # name -> GraphedTrainStep keyword arguments of the arm
     kwargs = {name: {} for name in makers}
@@ -137,7 +141,7 @@ def main():
     }
     print(f"{result['card']}, power limit {result['power_limit_w']} W")
     for name in makers:
-        print(f"  {name:22s} {result['ms_per_step_median'][name]:.4f} ms/step (median of {args.rounds} rounds)  "
+        print(f"  {name:26s} {result['ms_per_step_median'][name]:.4f} ms/step (median of {args.rounds} rounds)  "
               f"{result['kernels_per_replay'][name]} own kernels per replay")
     print(json.dumps(result))
 
