@@ -8,7 +8,7 @@ GPU → init_process_group over TCP → seed → model → optional SyncBN → D
 Extra flags cover what the reference hard-codes: ``--init-method`` (its LAN address
 ``tcp://10.9.1.2:34567`` only works on the author's network, ref: ddp_example.py:110; we default
 to loopback with a free port), ``--data synthetic|mnist``, ``--model``, ``--comm fused|nccl``, ``--algo``,
-``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw), ``--lr``,
+``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw | rmsprop | adagrad), ``--lr``,
 ``--momentum``, ``--amsgrad``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--ema-decay``,
 ``--checkpoint`` / ``--resume``, ``--eval`` (test loss and accuracy after every epoch).
 """
@@ -44,14 +44,16 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--data-root", default="./data", type=str)
     p.add_argument("--model", default="convnet", choices=["convnet", "resnet18"])
     p.add_argument("--batch-size", default=100, type=int, help="per-GPU batch size (reference: 100)")
-    p.add_argument("--optimizer", default="sgd", choices=["sgd", "adam", "adamw"],
-                   help="optimizer: SGD (the reference's), Adam or AdamW, each a native multi-tensor kernel")
+    p.add_argument("--optimizer", default="sgd", choices=["sgd", "adam", "adamw", "rmsprop", "adagrad"],
+                   help="optimizer: SGD (the reference's), Adam, AdamW, RMSprop or Adagrad, each a native multi-tensor kernel with "
+                        "torch's defaults")
     p.add_argument("--lr", default=1e-4, type=float, help="learning rate (reference: 1e-4)")
-    p.add_argument("--momentum", default=None, type=float, help="SGD momentum (default 0; not accepted with Adam / AdamW)")
+    p.add_argument("--momentum", default=None, type=float, help="SGD momentum (default 0; not accepted with the other optimizers)")
     p.add_argument("--amsgrad", default=False, action="store_true",
-                   help="Adam / AdamW with AMSGrad: the running maximum of exp_avg_sq in the denominator (not accepted with SGD)")
+                   help="Adam / AdamW with AMSGrad: the running maximum of exp_avg_sq in the denominator (not accepted with the other "
+                        "optimizers)")
     p.add_argument("--weight-decay", default=None, type=float,
-                   help="weight decay (default: 0 for SGD and Adam, 1e-2 for AdamW, torch's defaults)")
+                   help="weight decay (default: 0 for SGD, Adam, RMSprop and Adagrad, 1e-2 for AdamW, torch's defaults)")
     p.add_argument("--clip-grad-norm", default=None, type=float, metavar="MAX",
                    help="clip the global gradient norm (L2) to MAX before every optimizer step (default: off)")
     p.add_argument("--accumulation-steps", default=1, type=int, metavar="K",
@@ -82,14 +84,20 @@ def make_optimizer(args, params):
     kw = {} if args.weight_decay is None else {"weight_decay": args.weight_decay}
     if args.optimizer == "sgd":
         return pdt.optim.SGD(params, args.lr, momentum=args.momentum or 0.0, **kw)
+    if args.optimizer == "rmsprop":
+        return pdt.optim.RMSprop(params, args.lr, **kw)
+    if args.optimizer == "adagrad":
+        return pdt.optim.Adagrad(params, args.lr, **kw)
     cls = pdt.optim.Adam if args.optimizer == "adam" else pdt.optim.AdamW
     return cls(params, args.lr, amsgrad=getattr(args, "amsgrad", False), **kw)
 
 
 def check_args(p: argparse.ArgumentParser, args) -> None:
     if args.optimizer != "sgd" and args.momentum is not None:
-        p.error(f"--momentum applies to SGD only; {args.optimizer} takes its moments from its betas")
-    if args.optimizer == "sgd" and getattr(args, "amsgrad", False):
+        why = {"rmsprop": "RMSprop's momentum is a library option (pdt.optim.RMSprop(..., momentum=...))",
+               "adagrad": "Adagrad has no momentum"}.get(args.optimizer, f"{args.optimizer} takes its moments from its betas")
+        p.error(f"--momentum applies to SGD only; {why}")
+    if args.optimizer not in ("adam", "adamw") and getattr(args, "amsgrad", False):
         p.error("--amsgrad applies to Adam and AdamW only (--optimizer adam | adamw)")
     if args.clip_grad_norm is not None and not args.clip_grad_norm > 0:
         p.error(f"--clip-grad-norm must be positive (got {args.clip_grad_norm})")

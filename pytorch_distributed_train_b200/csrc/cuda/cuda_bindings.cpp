@@ -54,6 +54,16 @@ AdamHyper adam_hyper(double lr, const c10::optional<at::Tensor>& lr_tensor, doub
   return AdamHyper{lr, beta1, beta2, static_cast<float>(eps), static_cast<float>(weight_decay), decoupled ? 1 : 0, maximize ? 1 : 0,
                    opt_ptr(lr_tensor, "lr_tensor")};
 }
+// The hyper-parameters of rmsprop_multi and of the RMSprop rider of convnet_l1_bwd_wgrad.
+RmspropHyper rmsprop_hyper(double lr, const c10::optional<at::Tensor>& lr_tensor, double alpha, double eps, double weight_decay, double momentum,
+                           bool maximize) {
+  return RmspropHyper{static_cast<float>(lr), static_cast<float>(alpha), static_cast<float>(1.0 - alpha), static_cast<float>(eps),
+                      static_cast<float>(weight_decay), static_cast<float>(momentum), maximize ? 1 : 0, opt_ptr(lr_tensor, "lr_tensor")};
+}
+// The hyper-parameters of adagrad_multi and of the Adagrad rider of convnet_l1_bwd_wgrad.
+AdagradHyper adagrad_hyper(double lr, const c10::optional<at::Tensor>& lr_tensor, double lr_decay, double eps, double weight_decay, bool maximize) {
+  return AdagradHyper{lr, lr_decay, static_cast<float>(eps), static_cast<float>(weight_decay), maximize ? 1 : 0, opt_ptr(lr_tensor, "lr_tensor")};
+}
 
 using TensorList = std::vector<c10::optional<at::Tensor>>;
 TensorList tensors(const py::dict& d, const char* key) { return d[key].cast<TensorList>(); }
@@ -134,6 +144,50 @@ AmsgradRider amsgrad_rider(const py::dict& d) {
     chk(*vmax[k], "max_exp_avg_sq");
     r.vmax[k] = vmax[k]->data_ptr<float>();
   }
+  return r;
+}
+
+// State tensor `name` of rider parameter k: present, `numel` elements, fp32 contiguous on the device.
+float* rider_state(const TensorList& ts, int k, int64_t numel, const char* kind, const char* name) {
+  TORCH_CHECK(ts[k].has_value() && ts[k]->defined(), "convnet_l1_bwd_wgrad: ", kind, " state ", name, " of parameter ", k, " missing");
+  chk(*ts[k], name);
+  TORCH_CHECK(ts[k]->numel() == numel, "convnet_l1_bwd_wgrad: ", kind, " state ", name, " of parameter ", k, " has the wrong size");
+  return ts[k]->data_ptr<float>();
+}
+
+// {"kind": "rmsprop", "params", "prev_grads", "square_avg", "step" (fp32 scalars on the device), "momentum_buffer" (ten, or empty when
+// momentum == 0), "grad_avg" (ten, or empty when not centered), "lr", "lr_tensor", "alpha", "eps", "weight_decay", "momentum",
+// "maximize"}
+RmspropRider rmsprop_rider(const py::dict& d) {
+  RmspropRider r;
+  const double momentum = d["momentum"].cast<double>();
+  const TensorList sqs = tensors(d, "square_avg"), steps = tensors(d, "step"), bufs = tensors(d, "momentum_buffer"), gas = tensors(d, "grad_avg");
+  TORCH_CHECK(sqs.size() == 10 && steps.size() == 10 && (bufs.empty() || bufs.size() == 10) && (gas.empty() || gas.size() == 10),
+              "convnet_l1_bwd_wgrad: rmsprop lists have the wrong length");
+  TORCH_CHECK((momentum > 0.0) == !bufs.empty(), "convnet_l1_bwd_wgrad: rmsprop momentum buffers are given exactly when momentum > 0");
+  fill_rider(r, d, "rmsprop", [&](int k, const at::Tensor& p) {
+    r.sq[k] = rider_state(sqs, k, p.numel(), "rmsprop", "square_avg");
+    r.step[k] = rider_state(steps, k, 1, "rmsprop", "step");
+    if (!bufs.empty()) r.buf[k] = rider_state(bufs, k, p.numel(), "rmsprop", "momentum_buffer");
+    if (!gas.empty()) r.ga[k] = rider_state(gas, k, p.numel(), "rmsprop", "grad_avg");
+  });
+  r.h = rmsprop_hyper(d["lr"].cast<double>(), d["lr_tensor"].cast<c10::optional<at::Tensor>>(), d["alpha"].cast<double>(), d["eps"].cast<double>(),
+                      d["weight_decay"].cast<double>(), momentum, d["maximize"].cast<bool>());
+  return r;
+}
+
+// {"kind": "adagrad", "params", "prev_grads", "sum", "step" (fp32 scalars on the device), "lr", "lr_tensor", "lr_decay", "eps",
+// "weight_decay", "maximize"}
+AdagradRider adagrad_rider(const py::dict& d) {
+  AdagradRider r;
+  const TensorList sums = tensors(d, "sum"), steps = tensors(d, "step");
+  TORCH_CHECK(sums.size() == 10 && steps.size() == 10, "convnet_l1_bwd_wgrad: adagrad lists have the wrong length");
+  fill_rider(r, d, "adagrad", [&](int k, const at::Tensor& p) {
+    r.sum[k] = rider_state(sums, k, p.numel(), "adagrad", "sum");
+    r.step[k] = rider_state(steps, k, 1, "adagrad", "step");
+  });
+  r.h = adagrad_hyper(d["lr"].cast<double>(), d["lr_tensor"].cast<c10::optional<at::Tensor>>(), d["lr_decay"].cast<double>(),
+                      d["eps"].cast<double>(), d["weight_decay"].cast<double>(), d["maximize"].cast<bool>());
   return r;
 }
 
@@ -505,8 +559,11 @@ void register_cuda_bindings(py::module_& m) {
     }
     const auto d = rider.cast<py::dict>();
     const auto kind = d["kind"].cast<std::string>();
-    TORCH_CHECK(kind == "sgd" || kind == "adam", "convnet_l1_bwd_wgrad: rider kind must be 'sgd' or 'adam' (got '", kind, "')");
+    TORCH_CHECK(kind == "sgd" || kind == "adam" || kind == "rmsprop" || kind == "adagrad",
+                "convnet_l1_bwd_wgrad: rider kind must be 'sgd', 'adam', 'rmsprop' or 'adagrad' (got '", kind, "')");
     if (kind == "sgd") launch_rider(sgd_rider(d));
+    else if (kind == "rmsprop") launch_rider(rmsprop_rider(d));
+    else if (kind == "adagrad") launch_rider(adagrad_rider(d));
     else if (d.contains("max_exp_avg_sq")) launch_rider(amsgrad_rider(d));
     else launch_rider(adam_rider(d));
   }, py::arg("dp"), py::arg("y"), py::arg("x"), py::arg("saved"), py::arg("gamma"), py::arg("beta"), py::arg("dgamma"), py::arg("dbeta"),
@@ -848,6 +905,84 @@ void register_cuda_bindings(py::module_& m) {
       }
       if (ams) launch_adam_multi(tl, h, ticket, st);
       else launch_adam_multi(static_cast<const AdamTensorList&>(tl), h, ticket, st);
+    }
+  });
+  // RMSprop: momentum_buffers given exactly when momentum > 0, grad_avgs exactly when centered (empty lists otherwise).  The step
+  // counts take adam_multi's ticket word: launches on one device are ordered by the compute stream.
+  m.def("rmsprop_multi", [](std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> square_avgs,
+                            std::vector<at::Tensor> momentum_buffers, std::vector<at::Tensor> grad_avgs, std::vector<at::Tensor> steps,
+                            double lr, c10::optional<at::Tensor> lr_tensor, double alpha, double eps, double weight_decay, double momentum,
+                            bool maximize) {
+    const size_t n = params.size();
+    TORCH_CHECK(grads.size() == n && square_avgs.size() == n && steps.size() == n, "rmsprop_multi: list lengths differ");
+    TORCH_CHECK(momentum > 0.0 ? momentum_buffers.size() == n : momentum_buffers.empty(),
+                "rmsprop_multi: momentum buffers are given exactly when momentum > 0");
+    TORCH_CHECK(grad_avgs.empty() || grad_avgs.size() == n, "rmsprop_multi: list lengths differ");
+    if (n == 0) return;
+    c10::cuda::CUDAGuard g(params[0].device());
+    const RmspropHyper h = rmsprop_hyper(lr, lr_tensor, alpha, eps, weight_decay, momentum, maximize);
+    cudaStream_t st = cur_stream(params[0]);
+    unsigned int* ticket = scratch(params[0]).counter + kAdamTicketWord;
+    const bool centered = !grad_avgs.empty(), mom = !momentum_buffers.empty();
+    for (size_t base = 0; base < n; base += RmspropTensorList::kMax) {
+      RmspropTensorList tl;
+      tl.count = static_cast<int>(std::min<size_t>(RmspropTensorList::kMax, n - base));
+      for (int i = 0; i < tl.count; ++i) {
+        const size_t j = base + i;
+        chk(params[j], "param"); chk(grads[j], "grad"); chk(square_avgs[j], "square_avg"); chk(steps[j], "step");
+        const int64_t numel = params[j].numel();
+        TORCH_CHECK(grads[j].numel() == numel && square_avgs[j].numel() == numel && steps[j].numel() == 1 && numel < (int64_t(1) << 31),
+                    "rmsprop_multi: bad tensor sizes");
+        TORCH_CHECK(params[j].device() == params[0].device() && steps[j].device() == params[0].device(), "rmsprop_multi: all tensors on one device");
+        tl.p[i] = params[j].data_ptr<float>();
+        tl.g[i] = grads[j].data_ptr<float>();
+        tl.sq[i] = square_avgs[j].data_ptr<float>();
+        tl.step[i] = steps[j].data_ptr<float>();
+        tl.n[i] = static_cast<int>(numel);
+        tl.buf[i] = tl.ga[i] = nullptr;
+        if (mom) {
+          chk(momentum_buffers[j], "momentum_buffer");
+          TORCH_CHECK(momentum_buffers[j].numel() == numel, "rmsprop_multi: bad tensor sizes");
+          TORCH_CHECK(momentum_buffers[j].device() == params[0].device(), "rmsprop_multi: all tensors on one device");
+          tl.buf[i] = momentum_buffers[j].data_ptr<float>();
+        }
+        if (centered) {
+          chk(grad_avgs[j], "grad_avg");
+          TORCH_CHECK(grad_avgs[j].numel() == numel, "rmsprop_multi: bad tensor sizes");
+          TORCH_CHECK(grad_avgs[j].device() == params[0].device(), "rmsprop_multi: all tensors on one device");
+          tl.ga[i] = grad_avgs[j].data_ptr<float>();
+        }
+      }
+      launch_rmsprop_multi(tl, h, ticket, st);
+    }
+  });
+  m.def("adagrad_multi", [](std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> sums,
+                            std::vector<at::Tensor> steps, double lr, c10::optional<at::Tensor> lr_tensor, double lr_decay, double eps,
+                            double weight_decay, bool maximize) {
+    const size_t n = params.size();
+    TORCH_CHECK(grads.size() == n && sums.size() == n && steps.size() == n, "adagrad_multi: list lengths differ");
+    if (n == 0) return;
+    c10::cuda::CUDAGuard g(params[0].device());
+    const AdagradHyper h = adagrad_hyper(lr, lr_tensor, lr_decay, eps, weight_decay, maximize);
+    cudaStream_t st = cur_stream(params[0]);
+    unsigned int* ticket = scratch(params[0]).counter + kAdamTicketWord;
+    for (size_t base = 0; base < n; base += AdagradTensorList::kMax) {
+      AdagradTensorList tl;
+      tl.count = static_cast<int>(std::min<size_t>(AdagradTensorList::kMax, n - base));
+      for (int i = 0; i < tl.count; ++i) {
+        const size_t j = base + i;
+        chk(params[j], "param"); chk(grads[j], "grad"); chk(sums[j], "sum"); chk(steps[j], "step");
+        const int64_t numel = params[j].numel();
+        TORCH_CHECK(grads[j].numel() == numel && sums[j].numel() == numel && steps[j].numel() == 1 && numel < (int64_t(1) << 31),
+                    "adagrad_multi: bad tensor sizes");
+        TORCH_CHECK(params[j].device() == params[0].device() && steps[j].device() == params[0].device(), "adagrad_multi: all tensors on one device");
+        tl.p[i] = params[j].data_ptr<float>();
+        tl.g[i] = grads[j].data_ptr<float>();
+        tl.sum[i] = sums[j].data_ptr<float>();
+        tl.step[i] = steps[j].data_ptr<float>();
+        tl.n[i] = static_cast<int>(numel);
+      }
+      launch_adagrad_multi(tl, h, ticket, st);
     }
   });
   // Gradient-norm clipping: returns the total norm (a 0-d view of a [2] buffer whose second element is the clip coefficient);

@@ -15,7 +15,8 @@
 //                              wgmma (warps 0..3; K-major copies of x, written in the barrier's shadow, and of dy)
 //   convnet_l1_bwd_kernel      MaxPool/ReLU/BN backward ──barrier── conv1 weight gradient (mma.sync) ──barrier── conv1 fold;
 //                              conv2's weight gradient is folded in the shadow of the first barrier, and — on one GPU — the
-//                              threads that write the folded gradients apply the optimizer update (SgdRider / AdamRider / AmsgradRider)
+//                              threads that write the folded gradients apply the optimizer update (SgdRider / AdamRider / AmsgradRider /
+//                              RmspropRider / AdagradRider)
 //
 // All cross-CTA sums are "every CTA writes one partial row, barrier, every CTA folds the rows in the same fixed order",
 // so results are bit-reproducible and identical in every CTA.  The kernels are launched cooperatively (all CTAs
@@ -458,6 +459,58 @@ __device__ __forceinline__ void adam_apply(const R& r, int k, int i, float g, co
   *p = fmaf(-f[k], mv / (sqrtf(den) / f[10 + k] + r.h.eps), pv);
 }
 
+// One RMSprop update (the arithmetic of rmsprop_multi_kernel, ops_simt.cu) of element i of parameter k with gradient g.
+// R: RmspropRider, possibly in a ClipRider.
+template <class R>
+__device__ __forceinline__ void rmsprop_apply(const R& r, int k, int i, float g, float lr) {
+  float gv = r.h.maximize ? -g : g;
+  float* p = r.p[k] + i;
+  float* sq = r.sq[k] + i;
+  const float pv = *p;
+  if (r.h.weight_decay != 0.f) gv = fmaf(r.h.weight_decay, pv, gv);
+  const float sv = fmaf(r.h.one_minus_alpha * gv, gv, r.h.alpha * *sq);
+  *sq = sv;
+  float var = sv;
+  if (r.ga[k]) {
+    float* ga = r.ga[k] + i;
+    const float a = fmaf(r.h.one_minus_alpha, gv - *ga, *ga);
+    *ga = a;
+    var = fmaf(-a, a, sv);
+  }
+  const float u = gv / (sqrtf(var) + r.h.eps);
+  if (r.buf[k]) {
+    float* buf = r.buf[k] + i;
+    const float b = fmaf(r.h.momentum, *buf, u);
+    *buf = b;
+    *p = fmaf(-lr, b, pv);
+  } else {
+    *p = fmaf(-lr, u, pv);
+  }
+}
+
+// The Adagrad rider's decayed learning rates clr = lr / (1 + s·lr_decay) of the ten parameters (s: the step before this update),
+// formed in double once per CTA before the first grid barrier.
+__device__ __forceinline__ void adagrad_factors(const AdagradRider& r, float* f, int tid) {
+  if (tid < 10 && r.step[tid]) {
+    const double lr = r.h.lr_dev ? static_cast<double>(__ldg(r.h.lr_dev)) : r.h.lr;
+    f[tid] = static_cast<float>(lr / (1.0 + static_cast<double>(*r.step[tid]) * r.h.lr_decay));
+  }
+}
+
+// One Adagrad update (the arithmetic of adagrad_multi_kernel, ops_simt.cu) of element i of parameter k with gradient g; f: the
+// factors of adagrad_factors.  R: AdagradRider, possibly in a ClipRider.
+template <class R>
+__device__ __forceinline__ void adagrad_apply(const R& r, int k, int i, float g, const float* f) {
+  float gv = r.h.maximize ? -g : g;
+  float* p = r.p[k] + i;
+  float* sum = r.sum[k] + i;
+  const float pv = *p;
+  if (r.h.weight_decay != 0.f) gv = fmaf(r.h.weight_decay, pv, gv);
+  const float s = fmaf(gv, gv, *sum);
+  *sum = s;
+  *p = fmaf(-f[k], gv / (sqrtf(s) + r.h.eps), pv);
+}
+
 // Gradient-norm clipping (ClipRider): one gradient element g into a thread's accumulator — Σg², or max |g| keeping a NaN.
 template <class R>
 __device__ __forceinline__ float clip_acc(const R& r, float acc, float g) { return r.norm_inf ? nan_max(fabsf(g), acc) : fmaf(g, g, acc); }
@@ -466,17 +519,25 @@ __device__ __forceinline__ float clip_comb(const R& r, float a, float b) { retur
 
 template <class R>
 constexpr bool kClipRider =
-    std::is_same_v<R, ClipRider<SgdRider>> || std::is_same_v<R, ClipRider<AdamRider>> || std::is_same_v<R, ClipRider<AmsgradRider>>;
+    std::is_same_v<R, ClipRider<SgdRider>> || std::is_same_v<R, ClipRider<AdamRider>> || std::is_same_v<R, ClipRider<AmsgradRider>> ||
+    std::is_same_v<R, ClipRider<RmspropRider>> || std::is_same_v<R, ClipRider<AdagradRider>>;
 template <class R>
 constexpr bool kAdamRider = std::is_same_v<R, AdamRider> || std::is_same_v<R, ClipRider<AdamRider>> || std::is_same_v<R, AmsgradRider> ||
                             std::is_same_v<R, ClipRider<AmsgradRider>>;
+template <class R>
+constexpr bool kRmspropRider = std::is_same_v<R, RmspropRider> || std::is_same_v<R, ClipRider<RmspropRider>>;
+template <class R>
+constexpr bool kAdagradRider = std::is_same_v<R, AdagradRider> || std::is_same_v<R, ClipRider<AdagradRider>>;
 
 // Element i of parameter k's gradient is final with value g: a ClipRider adds it to this thread's share ca of the norm (the update
 // waits for the coefficient), the others apply their update.  The caller tests whether the rider is on and the parameter takes part.
+// adam_f: the per-launch factors of the Adam or Adagrad rider; sgd_lr: the learning rate of the SGD or RMSprop rider.
 template <class Rider>
 __device__ __forceinline__ void ride(const Rider& sr, float& ca, int k, int i, float g, const float* adam_f, float sgd_lr) {
   if constexpr (kClipRider<Rider>) ca = clip_acc(sr, ca, g);
   else if constexpr (kAdamRider<Rider>) adam_apply(sr, k, i, g, adam_f);
+  else if constexpr (kRmspropRider<Rider>) rmsprop_apply(sr, k, i, g, sgd_lr);
+  else if constexpr (kAdagradRider<Rider>) adagrad_apply(sr, k, i, g, adam_f);
   else sgd_apply(sr.p[k] + i, g, sr.m[k] ? sr.m[k] + i : nullptr, sr.h, sgd_lr);
 }
 
@@ -489,13 +550,14 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
                       float* partials, float* partials_w, GridSync gs,
                       // conv2's weight gradient, folded from the per-image partials [B][400][32] and Σdy rows [B][32]
                       const float* __restrict__ wpart, const float* __restrict__ dysum2, float* dw2, float* db2, const __grid_constant__ Rider sr) {
-  constexpr bool kClip = kClipRider<Rider>, kAdam = kAdamRider<Rider>;
-  static_assert(kAdam || std::is_base_of_v<SgdRider, Rider>,
-                "convnet_l1_bwd_kernel: SgdRider, AdamRider or AmsgradRider, or one of them in a ClipRider");
+  constexpr bool kClip = kClipRider<Rider>, kAdam = kAdamRider<Rider>, kRmsprop = kRmspropRider<Rider>, kAdagrad = kAdagradRider<Rider>;
+  static_assert(kAdam || kRmsprop || kAdagrad || std::is_base_of_v<SgdRider, Rider>,
+                "convnet_l1_bwd_kernel: SgdRider, AdamRider, AmsgradRider, RmspropRider or AdagradRider, or one of them in a ClipRider");
   extern __shared__ __align__(16) float dsm[];
   float* dys = dsm;                  // [784][16]
   float* fold = dsm + 784 * 16;      // [25 warps][16][32]
-  __shared__ float adam_f[kAdam ? kAdamFactors : 1];   // Adam rider: the per-launch factors
+  // Adam rider: the per-launch factors; Adagrad rider: the ten decayed learning rates
+  __shared__ float adam_f[kAdam ? kAdamFactors : kAdagrad ? 10 : 1];
   __shared__ float xs[32 * 32];
   __shared__ float red[kL1Warps * 32];
   __shared__ float s_tmp[kL1Warps * 32];
@@ -521,6 +583,8 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   }
   if constexpr (kAdam) {
     if (sr.on) adam_factors(sr, adam_f, tid);   // reads the step counts: before the first grid barrier
+  } else if constexpr (kAdagrad) {
+    if (sr.on) adagrad_factors(sr, adam_f, tid);
   }
   __syncthreads();
 
@@ -823,11 +887,13 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
         const float gv = __ldcg(gk + i) * coef;
         gk[i] = gv;
         if constexpr (kAdam) adam_apply(sr, k, i, gv, adam_f);
+        else if constexpr (kRmsprop) rmsprop_apply(sr, k, i, gv, sgd_lr);
+        else if constexpr (kAdagrad) adagrad_apply(sr, k, i, gv, adam_f);
         else sgd_apply(sr.p[k] + i, gv, sr.m[k] ? sr.m[k] + i : nullptr, sr.h, sgd_lr);
       }
     }
   }
-  if constexpr (kAdam) {
+  if constexpr (kAdam || kRmsprop || kAdagrad) {
     // every CTA read the step counts before the first grid barrier and this is after the last one
     if ((kClip || sr.on) && n == 0 && tid == 0)
       for (int k = 0; k < 10; ++k)
@@ -1800,6 +1866,10 @@ PDT_L1_BWD_WGRAD(ClipRider<SgdRider>)
 PDT_L1_BWD_WGRAD(ClipRider<AdamRider>)
 PDT_L1_BWD_WGRAD(AmsgradRider)
 PDT_L1_BWD_WGRAD(ClipRider<AmsgradRider>)
+PDT_L1_BWD_WGRAD(RmspropRider)
+PDT_L1_BWD_WGRAD(ClipRider<RmspropRider>)
+PDT_L1_BWD_WGRAD(AdagradRider)
+PDT_L1_BWD_WGRAD(ClipRider<AdagradRider>)
 #undef PDT_L1_BWD_WGRAD
 
 void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const float* g1, const float* be1, float* y1, float* p1, float* saved1,

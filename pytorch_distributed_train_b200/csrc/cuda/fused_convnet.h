@@ -45,6 +45,30 @@ struct AdamRider {
 struct AmsgradRider : AdamRider {
   float* vmax[10] = {};        // max_exp_avg_sq
 };
+// The same rider with the RMSprop update (the arithmetic of rmsprop_multi_kernel).  The step counts do not enter the update; one
+// thread writes step + 1 after the kernel's last grid barrier.
+struct RmspropRider {
+  int on = 0;
+  float* p[10] = {};
+  float* sq[10] = {};          // square_avg
+  float* buf[10] = {};         // momentum_buffer (nullptr: momentum == 0)
+  float* ga[10] = {};          // grad_avg (nullptr: not centered)
+  float* step[10] = {};        // fp32 step counts on the device
+  const float* g_prev[4] = {};
+  int n_prev[4] = {};
+  RmspropHyper h{};
+};
+// The same rider with the Adagrad update (the arithmetic of adagrad_multi_kernel).  Every CTA reads the ten step counts before the
+// kernel's first grid barrier (the decayed learning rates); one thread writes step + 1 after the last one.
+struct AdagradRider {
+  int on = 0;
+  float* p[10] = {};
+  float* sum[10] = {};
+  float* step[10] = {};        // fp32 step counts on the device
+  const float* g_prev[4] = {};
+  int n_prev[4] = {};
+  AdagradHyper h{};
+};
 // Any of the riders with gradient-norm clipping in front of the update (torch.nn.utils.clip_grad_norm_, norm_type 2 or inf).  Every CTA
 // adds up the squares (or the max |g|) of the gradient elements it sees — those of parameters 6..9 in the shadow of the first
 // grid barrier, those of 0..5 as it folds them (4, 5 in that shadow too) — and writes one partial; after one more grid barrier every CTA folds the B
@@ -64,8 +88,8 @@ struct ClipRider : Base {
 void launch_conv2_wgrad_partials(const float* dy2_pad, const float* x2_pad, int B, float* wpart, cudaStream_t st);
 // Layer-1 backward: dp [B,18,18,16] frame (interior read) → dgamma/dbeta [16], dw [16,1,5,5], db [16]; it also folds conv2's weight
 // gradient: the per-image partials wpart and Σdy rows dysum2 [B,32] → dw2 [32,16,5,5], db2 [32], in the shadow of the kernel's first
-// grid barrier.  partials: B·32, partials_w: B·512 floats.  Rider: SgdRider, AdamRider or AmsgradRider, or one of them in a
-// ClipRider.
+// grid barrier.  partials: B·32, partials_w: B·512 floats.  Rider: SgdRider, AdamRider, AmsgradRider, RmspropRider or AdagradRider,
+// or one of them in a ClipRider.
 // accumulate: gradient accumulation — every gradient written (dgamma, dbeta, dw, db, dw2, db2) becomes g_old + this batch's value, and
 // the rider updates with (and clips) the accumulated gradient.
 template <class Rider = SgdRider>

@@ -27,7 +27,7 @@ struct ReduceScratch {
 //   kGridEpochWord          epoch of the cooperative kernels' grid barrier (GridBar): only ever increases, never reset
 //   kGridArrivalWord        arrival count of that barrier
 //   kCeCounterWord          arrival counter of the whole-forward kernel's cross-entropy mean
-//   kAdamTicketWord         step hand-over ticket of adam_multi
+//   kAdamTicketWord         step hand-over ticket of adam_multi, rmsprop_multi and adagrad_multi
 //   kClipTicketWord         fold ticket of grad_norm_clip
 //   kAvgTicketWord          n_averaged hand-over ticket of avg_multi
 // Each fixed word sits in a 32-byte sector of its own.  A ticket word serves one launch set at a time: the sets that use it are
@@ -182,6 +182,48 @@ struct AmsgradTensorList : AdamTensorList {
   float* vmax[kMax];  // max_exp_avg_sq
 };
 void launch_adam_multi(const AmsgradTensorList& tl, AdamHyper h, unsigned int* ticket, cudaStream_t st);
+
+// RMSprop with torch's single-tensor arithmetic (g' = ±g + wd·p):
+//   sq = α·sq + (1 − α)·g'²;  centered: ga = lerp(ga, g', 1 − α), avg = sqrt(sq − ga²) + eps;  else avg = sqrt(sq) + eps
+//   momentum: buf = momentum·buf + g'/avg, p −= lr·buf;  else p −= lr·g'/avg
+// `step` does not enter the arithmetic; it is advanced as torch advances it, with adam_multi's ticket hand-over.
+struct RmspropTensorList {
+  static constexpr int kMax = 48;
+  float* p[kMax];
+  const float* g[kMax];
+  float* sq[kMax];    // square_avg
+  float* buf[kMax];   // momentum_buffer (nullptr: momentum == 0)
+  float* ga[kMax];    // grad_avg (nullptr: not centered)
+  float* step[kMax];
+  int n[kMax];
+  int count;
+};
+struct RmspropHyper {
+  float lr, alpha, one_minus_alpha, eps, weight_decay, momentum;   // 1 − α formed in double, as torch's Python scalar is
+  int maximize;
+  const float* lr_dev;   // optional device-resident learning rate (graph-capturable schedules)
+};
+void launch_rmsprop_multi(const RmspropTensorList& tl, RmspropHyper h, unsigned int* ticket, cudaStream_t st);
+
+// Adagrad with torch's single-tensor arithmetic (g' = ±g + wd·p): with s the step before this update,
+//   clr = lr / (1 + s·lr_decay) (double, rounded to fp32 once per tensor);  sum += g'²;  p −= clr·g' / (sqrt(sum) + eps)
+// The launch leaves step + 1 behind (adam_multi's ticket hand-over).
+struct AdagradTensorList {
+  static constexpr int kMax = 48;
+  float* p[kMax];
+  const float* g[kMax];
+  float* sum[kMax];
+  float* step[kMax];
+  int n[kMax];
+  int count;
+};
+struct AdagradHyper {
+  double lr, lr_decay;   // double, as torch's host-side clr is
+  float eps, weight_decay;
+  int maximize;
+  const float* lr_dev;   // optional device-resident learning rate (graph-capturable schedules)
+};
+void launch_adagrad_multi(const AdagradTensorList& tl, AdagradHyper h, unsigned int* ticket, cudaStream_t st);
 
 // Gradient-norm clipping (torch.nn.utils.clip_grad_norm_ with norm_type 2 or inf) as two launches per table set: the norm, then
 // the scale.  A set of more than kMax tensors is split into tables launched back to back; every block of every table writes one

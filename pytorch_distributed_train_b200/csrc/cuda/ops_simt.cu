@@ -993,6 +993,86 @@ __global__ void __launch_bounds__(256) amsgrad_multi_kernel(AmsgradTensorList tl
 // a kernel's parameters take at most 4 KiB
 static_assert(sizeof(AmsgradTensorList) + sizeof(AdamHyper) + sizeof(unsigned int*) <= 4096, "amsgrad_multi_kernel: parameters too large");
 
+// The step hand-over of adam_multi_kernel for the tables of rmsprop / adagrad (thread 0 of every block, after it has read its step):
+// the block that takes the last ticket writes s + 1 back for every tensor and resets the ticket word.
+template <class TL>
+__device__ __forceinline__ void advance_steps_last(const TL& tl, unsigned int* ticket) {
+  __threadfence();
+  if (atomicAdd(ticket, 1u) == gridDim.x * gridDim.y - 1) {
+    __threadfence();
+    for (int i = 0; i < tl.count; ++i) *tl.step[i] += 1.f;
+    atomicExch(ticket, 0u);
+  }
+}
+
+// =====================================================================================================
+// Multi-tensor RMSprop: same layout as sgd_multi_kernel.  The step count does not enter the update; thread 0 of every block takes a
+// ticket, and the block that takes the last one advances every step.  buf / ga of a tensor are null when momentum == 0 / not
+// centered: one kernel for the four combinations.
+// =====================================================================================================
+__global__ void __launch_bounds__(256) rmsprop_multi_kernel(RmspropTensorList tl, RmspropHyper h, unsigned int* ticket) {
+  const int t = blockIdx.y;
+  if (threadIdx.x == 0) advance_steps_last(tl, ticket);
+  const int n = tl.n[t];
+  float* __restrict__ p = tl.p[t];
+  const float* __restrict__ g = tl.g[t];
+  float* __restrict__ sq = tl.sq[t];
+  float* __restrict__ buf = tl.buf[t];
+  float* __restrict__ ga = tl.ga[t];
+  const float lr = h.lr_dev ? *h.lr_dev : h.lr;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float gv = h.maximize ? -g[i] : g[i];
+    const float pv = p[i];
+    if (h.weight_decay != 0.f) gv = fmaf(h.weight_decay, pv, gv);
+    const float sv = fmaf(h.one_minus_alpha * gv, gv, h.alpha * sq[i]);
+    sq[i] = sv;
+    float var = sv;
+    if (ga) {
+      const float a = fmaf(h.one_minus_alpha, gv - ga[i], ga[i]);
+      ga[i] = a;
+      var = fmaf(-a, a, sv);
+    }
+    const float u = gv / (sqrtf(var) + h.eps);
+    if (buf) {
+      const float b = fmaf(h.momentum, buf[i], u);
+      buf[i] = b;
+      p[i] = fmaf(-lr, b, pv);
+    } else {
+      p[i] = fmaf(-lr, u, pv);
+    }
+  }
+}
+static_assert(sizeof(RmspropTensorList) + sizeof(RmspropHyper) + sizeof(unsigned int*) <= 4096, "rmsprop_multi_kernel: parameters too large");
+
+// =====================================================================================================
+// Multi-tensor Adagrad: same layout as sgd_multi_kernel.  Thread 0 of every block reads its tensor's step s and forms
+// clr = lr / (1 + s·lr_decay) in double; the step hand-over is adam_multi_kernel's.
+// =====================================================================================================
+__global__ void __launch_bounds__(256) adagrad_multi_kernel(AdagradTensorList tl, AdagradHyper h, unsigned int* ticket) {
+  const int t = blockIdx.y;
+  __shared__ float s_clr;
+  if (threadIdx.x == 0) {
+    const double lr = h.lr_dev ? static_cast<double>(*h.lr_dev) : h.lr;
+    s_clr = static_cast<float>(lr / (1.0 + static_cast<double>(*tl.step[t]) * h.lr_decay));
+    advance_steps_last(tl, ticket);
+  }
+  __syncthreads();
+  const int n = tl.n[t];
+  float* __restrict__ p = tl.p[t];
+  const float* __restrict__ g = tl.g[t];
+  float* __restrict__ sum = tl.sum[t];
+  const float clr = s_clr;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float gv = h.maximize ? -g[i] : g[i];
+    const float pv = p[i];
+    if (h.weight_decay != 0.f) gv = fmaf(h.weight_decay, pv, gv);
+    const float s = fmaf(gv, gv, sum[i]);
+    sum[i] = s;
+    p[i] = fmaf(-clr, gv / (sqrtf(s) + h.eps), pv);
+  }
+}
+static_assert(sizeof(AdagradTensorList) + sizeof(AdagradHyper) + sizeof(unsigned int*) <= 4096, "adagrad_multi_kernel: parameters too large");
+
 // =====================================================================================================
 // Gradient-norm clipping: same layout as sgd_multi_kernel.  grad_norm_multi_kernel: every block writes one partial (fp32 Σg² or
 // max |g| of the elements it strides over, reduced over the block in a fixed order); on the set's last table, the block that
@@ -1293,6 +1373,22 @@ void launch_adam_multi(const AmsgradTensorList& tl, AdamHyper h, unsigned int* t
   const int bx = std::max(1, std::min(64, (maxn + 1023) / 1024));
   amsgrad_multi_kernel<<<dim3(bx, tl.count), 256, 0, st>>>(tl, h, ticket);
   check_launch("adam_multi");
+}
+void launch_rmsprop_multi(const RmspropTensorList& tl, RmspropHyper h, unsigned int* ticket, cudaStream_t st) {
+  if (tl.count == 0) return;
+  int maxn = 0;
+  for (int i = 0; i < tl.count; ++i) maxn = std::max(maxn, tl.n[i]);
+  const int bx = std::max(1, std::min(64, (maxn + 1023) / 1024));
+  rmsprop_multi_kernel<<<dim3(bx, tl.count), 256, 0, st>>>(tl, h, ticket);
+  check_launch("rmsprop_multi");
+}
+void launch_adagrad_multi(const AdagradTensorList& tl, AdagradHyper h, unsigned int* ticket, cudaStream_t st) {
+  if (tl.count == 0) return;
+  int maxn = 0;
+  for (int i = 0; i < tl.count; ++i) maxn = std::max(maxn, tl.n[i]);
+  const int bx = std::max(1, std::min(64, (maxn + 1023) / 1024));
+  adagrad_multi_kernel<<<dim3(bx, tl.count), 256, 0, st>>>(tl, h, ticket);
+  check_launch("adagrad_multi");
 }
 
 int grad_multi_blocks_x(const GradTensorList& tl) {

@@ -593,6 +593,24 @@ def adam_step(params, grads, exp_avgs, exp_avg_sqs, steps, lr, beta1=0.9, beta2=
                   None if max_exp_avg_sqs is None else list(max_exp_avg_sqs))
 
 
+def rmsprop_step(params, grads, square_avgs, steps, lr, alpha=0.99, eps=1e-8, weight_decay=0.0, momentum=0.0, maximize=False,
+                 momentum_buffers=None, grad_avgs=None, lr_tensor=None) -> None:
+    """One RMSprop update of every tensor (torch's single-tensor arithmetic), one kernel launch per 48 tensors.  ``momentum_buffers``
+    are required when ``momentum > 0``; ``grad_avgs`` make it centered.  ``steps`` (fp32 scalars on the device) do not enter the
+    update; the launch advances them, as torch's step does."""
+    _C.rmsprop_multi(list(params), list(grads), list(square_avgs), list(momentum_buffers) if momentum_buffers else [],
+                     list(grad_avgs) if grad_avgs else [], list(steps), float(lr), lr_tensor, float(alpha), float(eps),
+                     float(weight_decay), float(momentum), bool(maximize))
+
+
+def adagrad_step(params, grads, sums, steps, lr, lr_decay=0.0, eps=1e-10, weight_decay=0.0, maximize=False, lr_tensor=None) -> None:
+    """One Adagrad update of every tensor (torch's single-tensor arithmetic), one kernel launch per 48 tensors.  ``steps`` are the
+    fp32 step counts s on the device: the launch decays the learning rate to lr / (1 + s·lr_decay) and stores s + 1, so a replayed
+    graph advances it."""
+    _C.adagrad_multi(list(params), list(grads), list(sums), list(steps), float(lr), lr_tensor, float(lr_decay), float(eps),
+                     float(weight_decay), bool(maximize))
+
+
 def grad_norm_clip(grads, max_norm, norm_type=2.0, scale=True) -> torch.Tensor:
     """The total ``norm_type`` norm (2 or inf) of fp32 contiguous gradients on one device, and — with ``scale`` — every gradient
     multiplied by torch's clip coefficient ``min(max_norm / (norm + 1e-6), 1)``: two launches per 48 tensors, graph-capturable,

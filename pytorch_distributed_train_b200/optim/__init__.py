@@ -1,5 +1,7 @@
 from . import swa_utils
+from .adagrad import Adagrad
 from .adam import Adam, AdamW
+from .rmsprop import RMSprop
 from .sgd import SGD
 
-__all__ = ["Adam", "AdamW", "SGD", "swa_utils"]
+__all__ = ["Adagrad", "Adam", "AdamW", "RMSprop", "SGD", "swa_utils"]

@@ -95,13 +95,7 @@ class Adam(RidingOptimizer):
         """Standard behaviour, plus: every ``step`` goes to its parameter's device as fp32.  torch leaves it on the CPU unless
         the saved group says ``capturable`` or ``fused``; the kernels need it where the parameter is."""
         super().load_state_dict(state_dict)
-        for group in self.param_groups:
-            for p in group["params"]:
-                st = self.state.get(p)
-                if st and "step" in st:
-                    s = st["step"]
-                    s = s if isinstance(s, torch.Tensor) else torch.tensor(float(s))
-                    st["step"] = s.to(device=p.device, dtype=torch.float32).reshape(())
+        self._steps_to_param_device()
 
     # ---- single GPU: the update rides on the model's last backward kernel ---------------------------------
     def ride_on_backward(self, model, clip=None) -> bool:

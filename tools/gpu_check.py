@@ -22,6 +22,7 @@ GROUPS = {
     "ddp1": ["tests/test_gpu_kernels.py::test_single_gpu_ddp_and_graphed_step"],
     "adam": ["tests/test_adam.py"],
     "amsgrad": ["tests/test_adam_amsgrad.py"],
+    "rmsprop_adagrad": ["tests/test_rmsprop_adagrad.py"],
     "clip": ["tests/test_clip_grad.py"],
     "average": ["tests/test_averaged_model.py"],
     "accum": ["tests/test_grad_accumulation.py"],
