@@ -28,6 +28,7 @@ GROUPS = {
     "accum": ["tests/test_grad_accumulation.py"],
     "ce_options": ["tests/test_cross_entropy_options.py"],
     "syncbn": ["tests/test_syncbn_native.py", "tests/test_syncbn_large_mean.py"],
+    "maxpool_ties": ["tests/test_maxpool_ties.py"],
     "symm_emu": ["tests/test_symm_kernels_emulated.py"],
 }
 
