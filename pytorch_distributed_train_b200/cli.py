@@ -9,8 +9,8 @@ Extra flags cover what the reference hard-codes: ``--init-method`` (its LAN addr
 ``tcp://10.9.1.2:34567`` only works on the author's network, ref: ddp_example.py:110; we default
 to loopback with a free port), ``--data synthetic|mnist``, ``--model``, ``--comm fused|nccl``, ``--algo``,
 ``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw | rmsprop | adagrad), ``--lr``,
-``--momentum``, ``--amsgrad``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--ema-decay``,
-``--checkpoint`` / ``--resume``, ``--eval`` (test loss and accuracy after every epoch).
+``--momentum``, ``--amsgrad``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--mixup``,
+``--ema-decay``, ``--checkpoint`` / ``--resume``, ``--eval`` (test loss and accuracy after every epoch).
 """
 from __future__ import annotations
 
@@ -61,6 +61,9 @@ def build_parser() -> argparse.ArgumentParser:
                         "(default 1)")
     p.add_argument("--label-smoothing", default=0.0, type=float, metavar="EPS",
                    help="label smoothing of the cross-entropy loss, in [0, 1] (default 0)")
+    p.add_argument("--mixup", default=None, type=float, metavar="ALPHA",
+                   help="MixUp every training batch with lambda ~ Beta(ALPHA, ALPHA), ALPHA > 0, and train on the mixed class "
+                        "probabilities (default: off)")
     p.add_argument("--ema-decay", default=None, type=float, metavar="D",
                    help="keep an exponential moving average of the weights and buffers with decay D in [0, 1], updated after every "
                         "optimizer step and saved with --checkpoint (default: off)")
@@ -105,6 +108,8 @@ def check_args(p: argparse.ArgumentParser, args) -> None:
         p.error(f"--accumulation-steps must be at least 1 (got {args.accumulation_steps})")
     if not 0.0 <= args.label_smoothing <= 1.0:
         p.error(f"--label-smoothing must lie in [0, 1] (got {args.label_smoothing})")
+    if args.mixup is not None and not args.mixup > 0:
+        p.error(f"--mixup must be positive (got {args.mixup})")
     if args.ema_decay is not None and not 0.0 <= args.ema_decay <= 1.0:
         p.error(f"--ema-decay must lie in [0, 1] (got {args.ema_decay})")
     if args.graph and args.gpus >= 2 and args.accumulation_steps > 1:
@@ -130,10 +135,10 @@ def dist_train(gpu: int, args) -> None:
     torch.manual_seed(0)
     if args.model == "convnet":
         model = pdt.models.ConvNet()
-        shape = (1, 28, 28)
+        shape, num_classes = (1, 28, 28), 10
     else:
         model = pdt.models.resnet18(num_classes=1000)
-        shape = (3, 224, 224)
+        shape, num_classes = (3, 224, 224), 1000
     if args.syncbn:
         model = pdt.SyncBatchNorm.convert_sync_batchnorm(model)
         if gpu == 0:
@@ -156,7 +161,7 @@ def dist_train(gpu: int, args) -> None:
         train_dataset = pdata.MNIST(root=args.data_root, train=True, download=True, synthetic_fallback=True)
     else:
         n = args.samples if args.model == "convnet" else min(args.samples, 4096)
-        train_dataset = pdata.SyntheticMNIST(n, seed=0, num_classes=10 if args.model == "convnet" else 1000, image_shape=shape)
+        train_dataset = pdata.SyntheticMNIST(n, seed=0, num_classes=num_classes, image_shape=shape)
     train_sampler = pdt.DistributedSampler(train_dataset, num_replicas=args.world_size, rank=rank)
     # one loader batch = one optimizer step: `accum` micro-batches of batch_size images
     train_loader = pdt.DataLoader(dataset=train_dataset, batch_size=accum * batch_size, shuffle=False, num_workers=0,
@@ -167,18 +172,26 @@ def dist_train(gpu: int, args) -> None:
         if args.data == "mnist" and args.model == "convnet":
             test_dataset = pdata.MNIST(root=args.data_root, train=False, synthetic_fallback=True)
         else:
-            test_dataset = pdata.SyntheticMNIST(10000 if args.model == "convnet" else 4096, seed=1,
-                                                num_classes=10 if args.model == "convnet" else 1000, image_shape=shape)
+            test_dataset = pdata.SyntheticMNIST(10000 if args.model == "convnet" else 4096, seed=1, num_classes=num_classes,
+                                                image_shape=shape)
         test_loader = pdt.DataLoader(dataset=test_dataset, batch_size=batch_size, shuffle=False, pin_memory=use_cuda,
                                      sampler=pdt.DistributedSampler(test_dataset, num_replicas=args.world_size, rank=rank, shuffle=False))
+
+    mix_gen = None
+    if args.mixup is not None:
+        # MixUp on the host, before the batch's copy to the device: one λ per loader batch, each rank drawing its own (seeded per
+        # epoch below)
+        mix_gen = torch.Generator()
 
     step_fn = None
     if args.graph and use_cuda:
         from pytorch_distributed_train_b200.engine import GraphedTrainStep
 
-        step_fn = GraphedTrainStep(model, criterion, optimizer, example_inputs=(
-            torch.zeros((accum * batch_size,) + shape, device=device), torch.zeros(accum * batch_size, dtype=torch.int64, device=device)),
-            max_grad_norm=args.clip_grad_norm, accumulation_steps=accum, averaged_model=ema)
+        rows = accum * batch_size
+        example_targets = (torch.zeros(rows, dtype=torch.int64, device=device) if mix_gen is None else
+                           torch.zeros(rows, num_classes, device=device))
+        step_fn = GraphedTrainStep(model, criterion, optimizer, example_inputs=(torch.zeros((rows,) + shape, device=device), example_targets),
+                                   max_grad_norm=args.clip_grad_norm, accumulation_steps=accum, averaged_model=ema)
 
     first_epoch = 0
     if args.resume:
@@ -192,11 +205,19 @@ def dist_train(gpu: int, args) -> None:
     for epoch in range(first_epoch, args.epochs):
         if args.set_epoch:
             train_sampler.set_epoch(epoch)
+        if mix_gen is not None:
+            # from (epoch, rank): a run resumed from an epoch's checkpoint draws the λ sequence of an uninterrupted run
+            mix_gen.manual_seed(epoch * args.world_size + rank)
         pending = None   # (step index, loss handle) of a log line whose value is still on its way to the host
         fmt = "Epoch [{}/{}], Step [{}/{}], Loss: {:.4f}"
         for i, (images, labels) in enumerate(train_loader):
             if args.steps and i >= args.steps:
                 break
+            if mix_gen is not None:
+                # the images are mixed in place and stay pinned; the targets are pinned too, so their copy stays asynchronous
+                labels = pdata.mixup(images, labels, num_classes, args.mixup, mix_gen)
+                if use_cuda:
+                    labels = labels.pin_memory()
             graphed = step_fn is not None and images.shape[0] == accum * batch_size
             if graphed:
                 # the (pinned) host batch goes straight into the captured step's input buffers; the copy overlaps the previous step

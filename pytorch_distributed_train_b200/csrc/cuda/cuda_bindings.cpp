@@ -206,6 +206,21 @@ CeSpec ce_spec(const c10::optional<at::Tensor>& weight, int64_t ignore_index, do
   return s;
 }
 
+// Whether `target` holds class probabilities (a floating-point tensor, which must then be fp32 and shaped like the [B, C] `logits`)
+// rather than int64 class indices
+bool soft_target(const at::Tensor& target, const at::Tensor& logits, int64_t ignore_index, const char* who) {
+  if (!at::isFloatingType(target.scalar_type())) {
+    chk(target, "target", at::kLong);
+    return false;
+  }
+  chk(target, "target");
+  TORCH_CHECK(logits.dim() == 2 && target.sizes() == logits.sizes(), who, ": a probability target must have the logits' shape ",
+              logits.sizes(), " (got ", target.sizes(), ")");
+  TORCH_CHECK(target.device() == logits.device(), who, ": target must be on ", logits.device());
+  TORCH_CHECK(ignore_index == -100, who, ": ignore_index is not supported for floating point target");
+  return true;
+}
+
 // Per-device scratch for deterministic cross-CTA reductions. Kernels that use it run on one
 // stream at a time (the compute stream), which is what serialises access.
 struct Scratch {
@@ -593,12 +608,13 @@ void register_cuda_bindings(py::module_& m) {
     ReduceScratch scr = scratch(x);
     TORCH_CHECK(grad_scale > 0.0, "convnet_fwd: grad_scale must be positive");
     // grad_scale (gradient accumulation over k micro-batches: 1/k): the loss is grad_scale · mean cross-entropy, dlogits its gradient
-    SmoothCe ce;
+    SoftCe ce;
     ce.scale = static_cast<float>(grad_scale);
     at::Tensor loss, dlogits, loss_parts;
     if (target.has_value() && target->defined()) {
-      chk(*target, "target", at::kLong);
-      TORCH_CHECK(target->numel() == B, "convnet_fwd: one target per image expected");
+      // int64 class indices [B], or fp32 class probabilities [B, ncls] (SoftCe)
+      const bool soft = soft_target(*target, logits, ignore_index, "convnet_fwd");
+      TORCH_CHECK(soft || target->numel() == B, "convnet_fwd: one target per image expected");
       // ce_weight / ignore_index / label_smoothing / reduction: torch's cross-entropy options (a non-default spec runs SmoothCe)
       const CeSpec spec = ce_spec(ce_weight, ignore_index, label_smoothing, reduction, ncls, x, "convnet_fwd");
       ce.weight = spec.weight;
@@ -608,7 +624,8 @@ void register_cuda_bindings(py::module_& m) {
       loss = at::empty({}, x.options());
       dlogits = at::empty({B, ncls}, x.options());
       loss_parts = at::empty({B + 1}, x.options());   // one term per image, then the number of counted images
-      ce.target = reinterpret_cast<const long long*>(target->data_ptr<int64_t>());
+      if (soft) ce.target_probs = target->data_ptr<float>();
+      else ce.target = reinterpret_cast<const long long*>(target->data_ptr<int64_t>());
       ce.loss_parts = loss_parts.data_ptr<float>();
       ce.loss = defer_loss_mean ? nullptr : loss.data_ptr<float>();   // deferred: convnet_l2_bwd_fc(…, loss_parts, loss) writes it
       ce.dlogits = dlogits.data_ptr<float>();
@@ -799,26 +816,37 @@ void register_cuda_bindings(py::module_& m) {
                       dw.data_ptr<float>(), opt_mut(db, "db"), x.size(0), x.size(1), w.size(0), cur_stream(x));
     return dx;
   });
-  // weight / ignore_index / label_smoothing / reduction: torch's options (ops_kernels.h: CeSpec); the defaults run the plain mean kernels
+  // weight / ignore_index / label_smoothing / reduction: torch's options (ops_kernels.h: CeSpec); the defaults run the plain mean kernels.
+  // target: int64 class indices [B], or fp32 class probabilities shaped like the logits (soft_target)
   m.def("cross_entropy_fwd", [](const at::Tensor& logits, const at::Tensor& target, bool emit_grad, c10::optional<at::Tensor> weight,
                                 int64_t ignore_index, double label_smoothing, const std::string& reduction) {
-    chk(logits, "logits"); chk(target, "target", at::kLong);
+    chk(logits, "logits");
+    const bool soft = soft_target(target, logits, ignore_index, "cross_entropy_fwd");
     c10::cuda::CUDAGuard g(logits.device());
     const CeSpec spec = ce_spec(weight, ignore_index, label_smoothing, reduction, logits.size(1), logits, "cross_entropy_fwd");
     at::Tensor loss = at::empty({}, logits.options()), probs = at::empty_like(logits);
-    launch_cross_entropy_fwd(logits.data_ptr<float>(), reinterpret_cast<const long long*>(target.data_ptr<int64_t>()), loss.data_ptr<float>(),
-                             probs.data_ptr<float>(), logits.size(0), logits.size(1), cur_stream(logits), emit_grad, spec);
+    if (soft)
+      launch_cross_entropy_fwd_soft(logits.data_ptr<float>(), target.data_ptr<float>(), loss.data_ptr<float>(), probs.data_ptr<float>(),
+                                    logits.size(0), logits.size(1), cur_stream(logits), emit_grad, spec);
+    else
+      launch_cross_entropy_fwd(logits.data_ptr<float>(), reinterpret_cast<const long long*>(target.data_ptr<int64_t>()), loss.data_ptr<float>(),
+                               probs.data_ptr<float>(), logits.size(0), logits.size(1), cur_stream(logits), emit_grad, spec);
     return py::make_tuple(loss, probs);  // emit_grad: the second tensor is d(loss)/d(logits) for a unit incoming gradient
   }, py::arg("logits"), py::arg("target"), py::arg("emit_grad") = false, py::arg("weight") = py::none(), py::arg("ignore_index") = -100,
      py::arg("label_smoothing") = 0.0, py::arg("reduction") = "mean");
   m.def("cross_entropy_bwd", [](const at::Tensor& probs, const at::Tensor& target, const at::Tensor& dloss, c10::optional<at::Tensor> weight,
                                 int64_t ignore_index, double label_smoothing, const std::string& reduction) {
-    chk(probs, "probs"); chk(target, "target", at::kLong); chk(dloss, "dloss");
+    chk(probs, "probs"); chk(dloss, "dloss");
+    const bool soft = soft_target(target, probs, ignore_index, "cross_entropy_bwd");
     c10::cuda::CUDAGuard g(probs.device());
     const CeSpec spec = ce_spec(weight, ignore_index, label_smoothing, reduction, probs.size(1), probs, "cross_entropy_bwd");
     at::Tensor d = at::empty_like(probs);
-    launch_cross_entropy_bwd(probs.data_ptr<float>(), reinterpret_cast<const long long*>(target.data_ptr<int64_t>()), dloss.data_ptr<float>(),
-                             d.data_ptr<float>(), probs.size(0), probs.size(1), cur_stream(probs), spec);
+    if (soft)
+      launch_cross_entropy_bwd_soft(probs.data_ptr<float>(), target.data_ptr<float>(), dloss.data_ptr<float>(), d.data_ptr<float>(),
+                                    probs.size(0), probs.size(1), cur_stream(probs), spec);
+    else
+      launch_cross_entropy_bwd(probs.data_ptr<float>(), reinterpret_cast<const long long*>(target.data_ptr<int64_t>()), dloss.data_ptr<float>(),
+                               d.data_ptr<float>(), probs.size(0), probs.size(1), cur_stream(probs), spec);
     return d;
   }, py::arg("probs"), py::arg("target"), py::arg("dloss"), py::arg("weight") = py::none(), py::arg("ignore_index") = -100,
      py::arg("label_smoothing") = 0.0, py::arg("reduction") = "mean");

@@ -1040,9 +1040,13 @@ __device__ __forceinline__ void l1_pool_store(const float (&acc)[16], const L1Ma
 // and the conv2 weights are staged while conv1 computes.  Two grid barriers (BN1 and BN2 batch statistics), one launch.
 // Ce = ScaledCe: the cross-entropy rider computes scale · (mean cross-entropy) and its gradient (gradient accumulation: 1/k).
 // Ce = SmoothCe: the same with class weights, label smoothing, any ignore_index and the sum (fused_convnet.h).
+// Ce = SoftCe: the SmoothCe options with class-probability targets.
 // =====================================================================================================================
 __device__ __forceinline__ float ce_scale(const FusedCe&) { return 1.f; }
 __device__ __forceinline__ float ce_scale(const ScaledCe& ce) { return ce.scale; }
+// whether the cross-entropy rider is on
+__device__ __forceinline__ bool ce_on(const FusedCe& ce) { return ce.target != nullptr; }
+__device__ __forceinline__ bool ce_on(const SoftCe& ce) { return ce.target_probs != nullptr; }
 
 template <class Ce = FusedCe>
 __global__ void __launch_bounds__(kFwdThreads, 1)
@@ -1054,6 +1058,7 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
                    const float* __restrict__ fcb, float* __restrict__ logits, int ncls, float* partials, GridSync gs, Ce ce) {
   constexpr bool kScaled = std::is_same_v<Ce, ScaledCe>;
   constexpr bool kSmooth = std::is_same_v<Ce, SmoothCe>;
+  constexpr bool kSoft = std::is_same_v<Ce, SoftCe>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sa = smem;                                  // conv2 input patch, written by this CTA's layer-1 epilogue
@@ -1237,8 +1242,10 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
     for (int i = tid; i < ncls * 392; i += kFwdThreads) cp_async_16(smem_u32(fcs + 4 * i), fcw + 4 * i, 16);
     cp_async_commit();
   }
-  __shared__ std::conditional_t<kSmooth, float, int> s_counted;   // SmoothCe: the divisor D
-  if constexpr (kSmooth) {
+  __shared__ std::conditional_t<kSmooth || kSoft, float, int> s_counted;   // SmoothCe, SoftCe: the divisor D
+  if constexpr (kSoft) {
+    if (tid == 0) s_counted = ce.sum ? 1.f : static_cast<float>(B);   // every image counts
+  } else if constexpr (kSmooth) {
     if (ce.target != nullptr && warp == 0) {
       // in the barrier's shadow: D = Σ w_t over the counted images (their number without weights) for the mean, 1 for the sum;
       // every CTA sums the same B ≤ #SM terms in the same order, so all agree bit for bit
@@ -1345,10 +1352,10 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
         logits[static_cast<size_t>(n) * ncls + lane] = lg;
       }
       trace(0, 9);
-      if (ce.target != nullptr) {
+      if (ce_on(ce)) {
         // cross-entropy of this image and its gradient for a unit incoming gradient, divided by the number of counted images; an
         // ignored image adds no term and gets a zero gradient
-        const auto counted = s_counted;   // SmoothCe: the divisor D
+        const auto counted = s_counted;   // SmoothCe, SoftCe: the divisor D
         float mx = lg;
 #pragma unroll
         for (int off = 16; off >= 1; off >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
@@ -1356,43 +1363,61 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
         float ssum = e;
 #pragma unroll
         for (int off = 16; off >= 1; off >>= 1) ssum += __shfl_xor_sync(0xffffffffu, ssum, off);
-        const long long t = ce.target[n];
-        bool t_ok = t >= 0 && t < ncls;
-        if constexpr (kSmooth) t_ok = t_ok && t != ce.ignore_index;
-        const float lt = __shfl_sync(0xffffffffu, lg, t_ok ? static_cast<int>(t) : 0);
-        if constexpr (kSmooth) {
-          // term = (1-ε)·w_t·(lse − l_t) + (ε/C)·Σ_c w_c·(lse − l_c), gradient [(1-ε)·w_t·(p_c − [c=t]) + (ε/C)·(W·p_c − w_c)] / D;
-          // lane c holds w_c, the sums over classes are shuffle reductions
-          const float wc = lane < ncls ? (ce.weight ? ce.weight[lane] : 1.f) : 0.f;
-          const float wt = __shfl_sync(0xffffffffu, wc, t_ok ? static_cast<int>(t) : 0);
+        if constexpr (kSoft) {
+          // term = Σ_c a_c·(lse − l_c), gradient (p_c·S − a_c) / D, with a_c = w_c·q'_c, q' = q·(1−ε) + ε/C and S = Σ_c a_c; lane c
+          // reads q_c and w_c, the sums over classes are shuffle reductions
+          float a = 0.f;
+          if (lane < ncls)
+            a = (ce.weight ? ce.weight[lane] : 1.f) *
+                (ce.target_probs[static_cast<size_t>(n) * ncls + lane] * (1.f - ce.smoothing) + ce.smoothing / static_cast<float>(ncls));
           const float lse = mx + __logf(ssum);
-          float wsum = wc, smooth = lane < ncls ? wc * (lse - lg) : 0.f;
+          float S = a, term = lane < ncls ? a * (lse - lg) : 0.f;
 #pragma unroll
           for (int off = 16; off >= 1; off >>= 1) {
-            wsum += __shfl_xor_sync(0xffffffffu, wsum, off);
-            smooth += __shfl_xor_sync(0xffffffffu, smooth, off);
+            S += __shfl_xor_sync(0xffffffffu, S, off);
+            term += __shfl_xor_sync(0xffffffffu, term, off);
           }
-          const float keep = 1.f - ce.smoothing, eps_c = ce.smoothing / static_cast<float>(ncls);
-          if (lane < ncls) {
-            const float p = e / ssum;
-            ce.dlogits[static_cast<size_t>(n) * ncls + lane] =
-                (t_ok ? (keep * wt * (p - (t == lane ? 1.f : 0.f)) + eps_c * (wsum * p - wc)) / counted : 0.f) * ce.scale;
-          }
-          // D = 0 (a mean over zero total weight): no term, so that either fold gives torch's 0 / 0 = NaN
-          if (lane == 0) ce.loss_parts[n] = t_ok && counted != 0.f ? keep * wt * (lse - lt) + eps_c * smooth : 0.f;
+          if (lane < ncls) ce.dlogits[static_cast<size_t>(n) * ncls + lane] = (e / ssum * S - a) / counted * ce.scale;
+          if (lane == 0) ce.loss_parts[n] = term;
         } else {
-          if (lane < ncls) {
-            // ScaledCe: the rounding of autograd's grad · scale behind the unscaled loss
-            if constexpr (kScaled)
-              ce.dlogits[static_cast<size_t>(n) * ncls + lane] = (t_ok ? (e / ssum - (t == lane ? 1.f : 0.f)) / static_cast<float>(counted) : 0.f) * ce.scale;
-            else
-              ce.dlogits[static_cast<size_t>(n) * ncls + lane] = t_ok ? (e / ssum - (t == lane ? 1.f : 0.f)) / static_cast<float>(counted) : 0.f;
+          const long long t = ce.target[n];
+          bool t_ok = t >= 0 && t < ncls;
+          if constexpr (kSmooth) t_ok = t_ok && t != ce.ignore_index;
+          const float lt = __shfl_sync(0xffffffffu, lg, t_ok ? static_cast<int>(t) : 0);
+          if constexpr (kSmooth) {
+            // term = (1-ε)·w_t·(lse − l_t) + (ε/C)·Σ_c w_c·(lse − l_c), gradient [(1-ε)·w_t·(p_c − [c=t]) + (ε/C)·(W·p_c − w_c)] / D;
+            // lane c holds w_c, the sums over classes are shuffle reductions
+            const float wc = lane < ncls ? (ce.weight ? ce.weight[lane] : 1.f) : 0.f;
+            const float wt = __shfl_sync(0xffffffffu, wc, t_ok ? static_cast<int>(t) : 0);
+            const float lse = mx + __logf(ssum);
+            float wsum = wc, smooth = lane < ncls ? wc * (lse - lg) : 0.f;
+#pragma unroll
+            for (int off = 16; off >= 1; off >>= 1) {
+              wsum += __shfl_xor_sync(0xffffffffu, wsum, off);
+              smooth += __shfl_xor_sync(0xffffffffu, smooth, off);
+            }
+            const float keep = 1.f - ce.smoothing, eps_c = ce.smoothing / static_cast<float>(ncls);
+            if (lane < ncls) {
+              const float p = e / ssum;
+              ce.dlogits[static_cast<size_t>(n) * ncls + lane] =
+                  (t_ok ? (keep * wt * (p - (t == lane ? 1.f : 0.f)) + eps_c * (wsum * p - wc)) / counted : 0.f) * ce.scale;
+            }
+            // D = 0 (a mean over zero total weight): no term, so that either fold gives torch's 0 / 0 = NaN
+            if (lane == 0) ce.loss_parts[n] = t_ok && counted != 0.f ? keep * wt * (lse - lt) + eps_c * smooth : 0.f;
+          } else {
+            if (lane < ncls) {
+              // ScaledCe: the rounding of autograd's grad · scale behind the unscaled loss
+              if constexpr (kScaled)
+                ce.dlogits[static_cast<size_t>(n) * ncls + lane] = (t_ok ? (e / ssum - (t == lane ? 1.f : 0.f)) / static_cast<float>(counted) : 0.f) * ce.scale;
+              else
+                ce.dlogits[static_cast<size_t>(n) * ncls + lane] = t_ok ? (e / ssum - (t == lane ? 1.f : 0.f)) / static_cast<float>(counted) : 0.f;
+            }
+            if (lane == 0) ce.loss_parts[n] = t_ok ? mx + __logf(ssum) - lt : 0.f;
           }
-          if (lane == 0) ce.loss_parts[n] = t_ok ? mx + __logf(ssum) - lt : 0.f;
         }
-        // for a mean folded later (ScaledCe: the divisor is the count over the scale; SmoothCe: D over the scale)
+        // for a mean folded later (ScaledCe: the divisor is the count over the scale; SmoothCe, SoftCe: D over the scale)
         if (lane == 0 && n == 0)
-          ce.loss_parts[B] = (kScaled || kSmooth) ? static_cast<float>(counted) / ce_scale(ce) : static_cast<float>(counted);
+          ce.loss_parts[B] = (kScaled || kSmooth || kSoft) ? static_cast<float>(counted) / ce_scale(ce) : static_cast<float>(counted);
         if (ce.loss != nullptr) {   // batch mean now (otherwise layer-2 backward folds it: ce.loss == nullptr)
           int last = 0;
           if (lane == 0) {
@@ -1407,7 +1432,7 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
 #pragma unroll
             for (int off = 16; off >= 1; off >>= 1) sl += __shfl_xor_sync(0xffffffffu, sl, off);
             if (lane == 0) {
-              *ce.loss = sl / ((kScaled || kSmooth) ? static_cast<float>(counted) / ce_scale(ce) : static_cast<float>(counted));
+              *ce.loss = sl / ((kScaled || kSmooth || kSoft) ? static_cast<float>(counted) / ce_scale(ce) : static_cast<float>(counted));
               *ce.counter = 0u;
             }
           }
@@ -1876,15 +1901,24 @@ void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const 
                         float* rm1, float* rv1, long long* nbt1, float mom1, float eps1, const float* w2, const float* b2, const float* g2,
                         const float* be2, float* y2, float* out, float* saved2, float* rm2, float* rv2, long long* nbt2, float mom2, float eps2,
                         const float* fcw, const float* fcb, float* logits, int ncls, int B, float* partials, GridSync gs, cudaStream_t st,
-                        SmoothCe ce) {
+                        SoftCe ce) {
   if (logits != nullptr && ncls > 16) throw std::invalid_argument("convnet_fwd: the fused classifier handles at most 16 classes");
-  if (ce.target != nullptr && logits == nullptr) throw std::invalid_argument("convnet_fwd: the fused cross-entropy needs the fused classifier");
+  if ((ce.target != nullptr || ce.target_probs != nullptr) && logits == nullptr)
+    throw std::invalid_argument("convnet_fwd: the fused cross-entropy needs the fused classifier");
+  if (ce.target != nullptr && ce.target_probs != nullptr)
+    throw std::invalid_argument("convnet_fwd: class-index and class-probability targets are exclusive");
   if (!(ce.scale > 0.f)) throw std::invalid_argument("convnet_fwd: the cross-entropy scale must be positive");
   if (!(ce.smoothing >= 0.f && ce.smoothing <= 1.f)) throw std::invalid_argument("convnet_fwd: label smoothing must lie in [0, 1]");
+  if (ce.target_probs != nullptr) {
+    launch_cooperative(convnet_fwd_kernel<SoftCe>, B, kFwdThreads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", false, x, w1, b1, g1, be1, y1, p1,
+                       saved1, rm1, rv1, nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials,
+                       gs, ce);
+    return;
+  }
   if (ce.target != nullptr && !ce.is_default(ncls)) {
     launch_cooperative(convnet_fwd_kernel<SmoothCe>, B, kFwdThreads, static_cast<size_t>(L2FwdSmem::kTotal), st, "convnet_fwd", false, x, w1, b1, g1, be1, y1, p1,
                        saved1, rm1, rv1, nbt1, mom1, eps1, w2, b2, g2, be2, y2, out, saved2, rm2, rv2, nbt2, mom2, eps2, fcw, fcb, logits, ncls, partials,
-                       gs, ce);
+                       gs, static_cast<const SmoothCe&>(ce));
     return;
   }
   if (ce.target != nullptr && ce.scale != 1.f) {

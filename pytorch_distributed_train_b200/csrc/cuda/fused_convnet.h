@@ -124,18 +124,24 @@ struct SmoothCe : ScaledCe {
   bool sum = false;                // reduction 'sum' (else 'mean')
   bool is_default(int ncls) const { return weight == nullptr && smoothing == 0.f && !sum && (ignore_index < 0 || ignore_index >= ncls); }
 };
+// The rider with class-probability targets q [B, ncls] in place of `target` (ops_kernels.h: launch_cross_entropy_fwd_soft): class
+// weights, label smoothing, sum or mean; ignore_index plays no part.  Every image counts, so loss_parts[B] holds D = B (the mean)
+// or 1 (the sum) over the scale, and nothing is summed before the image's term.
+struct SoftCe : SmoothCe {
+  const float* target_probs = nullptr;   // [B, ncls]; nullptr: `target` (class indices) or off
+};
 
 // The whole training forward in one launch: layer 1 and layer 2 (+ classifier, ncls ≤ 16) of an image in the same CTA; the
 // pooled layer-1 activations go into conv2's shared-memory patch directly.  x [B,28,28] → y1 [B,28,28,16] (conv1 + bias, kept for
 // backward), p1 [B,18,18,16] frame (BN + ReLU + pool), saved1 [32] = mean, invstd; y2 [B,14,14,32], out [B,32,7,7] NCHW, saved2
 // [64]; logits [B,ncls].  partials: B·(32 + 64) floats.
-// With targets, a non-default spec runs the SmoothCe instantiation, else ce.scale != 1 the ScaledCe one; otherwise the kernel without
-// the scale.
+// With probability targets the SoftCe instantiation runs; with class-index targets a non-default spec runs the SmoothCe one, else
+// ce.scale != 1 the ScaledCe one; otherwise the kernel without the scale.
 void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const float* g1, const float* be1, float* y1, float* p1, float* saved1,
                         float* rm1, float* rv1, long long* nbt1, float mom1, float eps1, const float* w2, const float* b2, const float* g2,
                         const float* be2, float* y2, float* out, float* saved2, float* rm2, float* rv2, long long* nbt2, float mom2, float eps2,
                         const float* fcw, const float* fcb, float* logits, int ncls, int B, float* partials, GridSync gs, cudaStream_t st,
-                        SmoothCe ce = SmoothCe{});
+                        SoftCe ce = SoftCe{});
 // Layer-2 backward with the classifier's backward riding along: d(out) is computed from dlogits [B,ncls] and the fc weights
 // [ncls,1568] inside the kernel; dfcw [ncls,1568] / dfcb [ncls] are produced from `pooled` = the forward's out [B,1568].  ncls ≤ 16.
 // → dgamma/dbeta [32], dy [B,18,18,32] frame with zero halo (gradient at the conv2 output), dx [B,18,18,16] frame (data gradient,

@@ -129,6 +129,16 @@ void launch_cross_entropy_fwd(const float* logits, const long long* target, floa
                               bool emit_grad, const CeSpec& spec);
 void launch_cross_entropy_bwd(const float* probs, const long long* target, const float* dloss, float* dlogits, int B, int C,
                               cudaStream_t st, const CeSpec& spec);
+// Class-probability targets q [B, C] (torch's floating-point target).  With q' = q·(1−ε) + ε/C, a_c = w_c·q'_c and S = Σ_c a_c,
+// a row adds
+//   Σ_c a_c·(lse − l_c)        with gradient   (p_c·S − a_c) / D
+// and the loss is Σ terms / D: D = B for the mean whatever the weights (B = 0 ⇒ NaN), 1 for the sum.  Entries are not validated
+// (negative ones, rows that do not sum to one), and spec.ignore_index plays no part: torch refuses any but −100 with such targets.
+// One thread per row sums S in class order, and the forward's batch sum is in a fixed order.
+void launch_cross_entropy_fwd_soft(const float* logits, const float* q, float* loss, float* probs, int B, int C, cudaStream_t st,
+                                   bool emit_grad, const CeSpec& spec);
+void launch_cross_entropy_bwd_soft(const float* probs, const float* q, const float* dloss, float* dlogits, int B, int C, cudaStream_t st,
+                                   const CeSpec& spec);
 // Evaluation metrics of logits[0:rows, C] (the first `rows` rows of the batch; the rest take no part), added to the fp64 acc[4] by
 // one launch of the forward kernel that writes no loss or softmax:
 //   acc[0] += Σ loss terms (the sum before the division by D)   acc[1] += D = Σ_{counted} w_t, whatever spec.sum says

@@ -909,6 +909,62 @@ __global__ void __launch_bounds__(256) cross_entropy_bwd_spec_kernel(const float
   dlogits[i] = (keep * wt * (p - (t == c ? 1.f : 0.f)) + eps_c * (W * p - wc)) * g;
 }
 
+// ---- class-probability targets (ops_kernels.h: launch_cross_entropy_fwd_soft) ---------------------------------------------------
+// w_c·q'_c with q' = q·(1−ε) + ε/C, torch's smoothing of a probability target
+__device__ __forceinline__ float ce_soft_a(const float* __restrict__ qr, int c, const CeSpec& s, float keep, float eps_c) {
+  return (s.weight ? s.weight[c] : 1.f) * (qr[c] * keep + eps_c);
+}
+
+// One thread per row: the row's term Σ_c a_c·(lse − l_c), a_c = w_c·q'_c, and S = Σ_c a_c in class order; emit_grad as in
+// cross_entropy_fwd_kernel, with the gradient (p_c·S − a_c) / D.
+__global__ void __launch_bounds__(256) cross_entropy_fwd_soft_kernel(const float* __restrict__ logits, const float* __restrict__ q,
+                                                                     float* loss, float* __restrict__ probs, int B, int C, int emit_grad,
+                                                                     CeSpec s) {
+  __shared__ float red[256];
+  const float D = s.sum ? 1.f : static_cast<float>(B);
+  const float keep = 1.f - s.smoothing, eps_c = s.smoothing / static_cast<float>(C);
+  float local = 0.f;
+  for (int r = threadIdx.x; r < B; r += blockDim.x) {
+    const float* l = logits + static_cast<size_t>(r) * C;
+    const float* qr = q + static_cast<size_t>(r) * C;
+    float m = l[0];
+    for (int c = 1; c < C; ++c) m = fmaxf(m, l[c]);
+    float sx = 0.f;
+    for (int c = 0; c < C; ++c) sx += __expf(l[c] - m);
+    const float inv = 1.f / sx, lse = m + __logf(sx);
+    float S = 0.f, term = 0.f;
+    for (int c = 0; c < C; ++c) {
+      const float a = ce_soft_a(qr, c, s, keep, eps_c);
+      S += a;
+      term += a * (lse - l[c]);
+    }
+    for (int c = 0; c < C; ++c) {
+      const float p = __expf(l[c] - m) * inv;
+      probs[static_cast<size_t>(r) * C + c] = !emit_grad ? p : (p * S - ce_soft_a(qr, c, s, keep, eps_c)) / D;
+    }
+    local += term;
+  }
+  const float total = ce_block_sum(local, red);
+  if (threadIdx.x == 0) *loss = total / D;   // an empty batch's mean is 0 / 0 = NaN, as torch's
+}
+
+// One thread per row: S in the forward kernel's order, then dlogits = (p_c·S − a_c) · dloss / D
+__global__ void __launch_bounds__(256) cross_entropy_bwd_soft_kernel(const float* __restrict__ probs, const float* __restrict__ q,
+                                                                     const float* __restrict__ dloss, float* __restrict__ dlogits, int B, int C,
+                                                                     CeSpec s) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= B) return;
+  const float keep = 1.f - s.smoothing, eps_c = s.smoothing / static_cast<float>(C);
+  const float* qr = q + static_cast<size_t>(r) * C;
+  float S = 0.f;
+  for (int c = 0; c < C; ++c) S += ce_soft_a(qr, c, s, keep, eps_c);
+  const float g = (dloss ? *dloss : 1.f) / (s.sum ? 1.f : static_cast<float>(B));
+  for (int c = 0; c < C; ++c) {
+    const size_t i = static_cast<size_t>(r) * C + c;
+    dlogits[i] = (probs[i] * S - ce_soft_a(qr, c, s, keep, eps_c)) * g;
+  }
+}
+
 // =====================================================================================================
 // Multi-tensor SGD: blockIdx.y = tensor, blockIdx.x strides its elements
 // =====================================================================================================
@@ -1346,6 +1402,17 @@ void launch_cross_entropy_bwd(const float* probs, const long long* target, const
                               cudaStream_t st, const CeSpec& spec) {
   if (spec.is_default(C)) return launch_cross_entropy_bwd(probs, target, dloss, dlogits, B, C, st);
   cross_entropy_bwd_spec_kernel<<<(B * C + 255) / 256, 256, 0, st>>>(probs, target, dloss, dlogits, B, C, spec);
+  check_launch("cross_entropy_bwd");
+}
+void launch_cross_entropy_fwd_soft(const float* logits, const float* q, float* loss, float* probs, int B, int C, cudaStream_t st,
+                                   bool emit_grad, const CeSpec& spec) {
+  cross_entropy_fwd_soft_kernel<<<1, 256, 0, st>>>(logits, q, loss, probs, B, C, emit_grad ? 1 : 0, spec);
+  check_launch("cross_entropy_fwd");
+}
+void launch_cross_entropy_bwd_soft(const float* probs, const float* q, const float* dloss, float* dlogits, int B, int C, cudaStream_t st,
+                                   const CeSpec& spec) {
+  if (B == 0) return;
+  cross_entropy_bwd_soft_kernel<<<(B + 255) / 256, 256, 0, st>>>(probs, q, dloss, dlogits, B, C, spec);
   check_launch("cross_entropy_bwd");
 }
 

@@ -1,10 +1,11 @@
-"""Input pipeline: samplers, DataLoader, MNIST (idx parser) and synthetic datasets."""
+"""Input pipeline: samplers, DataLoader, MNIST (idx parser), synthetic datasets and MixUp."""
 from .dataloader import DataLoader, DevicePrefetcher, default_collate
+from .mixup import mixup
 from .mnist import MNIST, SyntheticMNIST, TensorDataset, read_idx, synthesize_mnist_files, write_idx
 from .sampler import BatchSampler, DistributedSampler, RandomSampler, Sampler, SequentialSampler
 
 __all__ = [
     "DataLoader", "DevicePrefetcher", "default_collate", "MNIST", "SyntheticMNIST", "TensorDataset",
     "read_idx", "write_idx", "synthesize_mnist_files", "BatchSampler", "DistributedSampler",
-    "RandomSampler", "Sampler", "SequentialSampler",
+    "RandomSampler", "Sampler", "SequentialSampler", "mixup",
 ]

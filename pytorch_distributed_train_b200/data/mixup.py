@@ -1,0 +1,29 @@
+"""MixUp (Zhang et al., 2018) on one batch, with torchvision's ``transforms.v2.MixUp`` definition."""
+from __future__ import annotations
+
+from typing import Optional
+
+import torch
+import torch.nn.functional as F
+
+
+def mixup(images: torch.Tensor, labels: torch.Tensor, num_classes: int, alpha: float,
+          generator: Optional[torch.Generator] = None) -> torch.Tensor:
+    """Mix every image of the batch with the one before it (the first with the last) and return the matching class-probability
+    targets.  λ ~ Beta(α, α) is drawn once for the batch, on the host from ``generator`` (a CPU generator; torch's default one when
+    None), and then
+
+        images ← λ·images + (1 − λ)·images.roll(1, 0)             in place
+        targets = λ·onehot(labels) + (1 − λ)·onehot(labels).roll(1, 0)    fp32 [B, num_classes]
+
+    rounded as torchvision computes them.  ``labels`` are int64 class indices in [0, num_classes).  The arithmetic runs on the
+    tensors' own device and nothing waits for it: in place, pinned host images stay pinned."""
+    if not alpha > 0:
+        raise ValueError(f"mixup: alpha must be positive (got {alpha})")
+    # what torch.distributions.Beta(α, α).sample() draws (torchvision's λ), here from the caller's generator: torch.distributions
+    # takes no generator, so the private sampler Beta.sample calls is called directly (test_mixup_cli.py pins the equivalence)
+    lam = float(torch._sample_dirichlet(torch.tensor([alpha, alpha]), generator=generator)[0])
+    rolled = images.roll(1, 0)
+    images.mul_(lam).add_(rolled.mul_(1.0 - lam))
+    onehot = F.one_hot(labels, num_classes).to(torch.float32)
+    return onehot.roll(1, 0).mul_(1.0 - lam).add_(onehot.mul_(lam))

@@ -400,8 +400,11 @@ def fused_convnet_forward(x: torch.Tensor, model) -> torch.Tensor:
     whole = {"conv2": c2, "bn2": b2_bn, "fc": fc}
     t = _upcoming_target
     spec = _upcoming_spec
-    if (t is not None and t.is_cuda and t.dtype == torch.int64 and t.dim() == 1 and t.shape[0] == x.shape[0] and t.is_contiguous()
-            and torch.is_grad_enabled() and _rider_spec_ok(spec, fc.weight)):
+    # class indices [B], or class probabilities [B, ncls] (fp32, as pdt.nn.CrossEntropyLoss runs them natively)
+    index = t is not None and t.dtype == torch.int64 and t.dim() == 1 and t.shape[0] == x.shape[0]
+    soft = t is not None and t.dtype == torch.float32 and t.shape == (x.shape[0], fc.weight.shape[0])
+    if ((index or soft) and t.is_cuda and t.is_contiguous() and torch.is_grad_enabled()
+            and _rider_spec_ok(spec, fc.weight, soft)):
         whole["target"] = t
         whole["defer_loss_mean"] = bool(_loss_read_after_backward)
         whole["grad_scale"] = _upcoming_grad_scale
@@ -420,11 +423,13 @@ def fused_convnet_forward(x: torch.Tensor, model) -> torch.Tensor:
     return logits
 
 
-def _rider_spec_ok(spec: tuple, fcw: torch.Tensor) -> bool:
+def _rider_spec_ok(spec: tuple, fcw: torch.Tensor, soft: bool = False) -> bool:
     """Whether the forward kernel's cross-entropy can take these options (what pdt.nn.CrossEntropyLoss runs natively); a criterion
-    with others computes its loss itself, so the rider is left off."""
+    with others computes its loss itself, so the rider is left off.  ``soft``: class-probability targets, which torch takes with
+    the default ``ignore_index`` only."""
     w, ignore_index, reduction, smoothing = spec
     return (reduction in ("mean", "sum") and 0.0 <= float(smoothing) <= 1.0 and isinstance(ignore_index, int)
+            and (not soft or ignore_index == -100)
             and (w is None or (w.dtype == torch.float32 and w.is_contiguous() and w.shape == (fcw.shape[0],) and w.device == fcw.device)))
 
 
@@ -537,8 +542,9 @@ def fused_ce_consumed() -> list:
 def cross_entropy(logits: torch.Tensor, target: torch.Tensor, weight: Optional[torch.Tensor] = None, ignore_index: int = -100,
                   reduction: str = "mean", label_smoothing: float = 0.0) -> torch.Tensor:
     """Cross-entropy over the batch, mean or sum, with torch's class weights, ignore_index and label smoothing: fused log-softmax +
-    NLL (ref: ddp_example.py:61,87).  The value the model's forward kernel computed is used when it was computed for this target
-    tensor with the same options (the same weight tensor, equal scalars)."""
+    NLL (ref: ddp_example.py:61,87).  ``target``: int64 class indices [B], or fp32 class probabilities [B, C].  The value the
+    model's forward kernel computed is used when it was computed for this target tensor with the same options (the same weight
+    tensor, equal scalars)."""
     spec = (weight, ignore_index, reduction, label_smoothing)
     pre = getattr(logits, "_pdt_ce", None)
     if pre is not None and pre[0] is target and _same_spec(pre[5], spec):
@@ -562,7 +568,7 @@ def cross_entropy_accumulate(logits: torch.Tensor, target: torch.Tensor, acc: to
     from ..nn.loss import native_ok
 
     weight, ignore_index, reduction, smoothing = spec
-    if native_ok(logits, target, weight, reduction, smoothing):
+    if target.dtype == torch.int64 and native_ok(logits, target, weight, reduction, smoothing):
         _C.cross_entropy_eval(logits.contiguous(), target.contiguous(), acc, int(rows), weight, int(ignore_index), float(smoothing))
         return
     logits, target = logits[:rows], target[:rows]

@@ -7,6 +7,10 @@ lr 1e-4):
   pdt_smooth_weighted  the same with class weights
   torch_smooth         torch.nn.CrossEntropyLoss(label_smoothing=0.1): the loss and its backward are ATen kernels in the graph
   k2_pdt_plain, k2_pdt_smooth   the first two with accumulation_steps=2 (two micro-batches of 100 per step)
+  pdt_soft             pdt.nn.CrossEntropyLoss() on class-probability targets with two non-zeros per row, as MixUp makes them
+  pdt_soft_smooth_weighted      the same with label smoothing 0.1 and class weights
+  torch_soft           torch.nn.CrossEntropyLoss() on the same targets
+  k2_pdt_soft          pdt_soft with accumulation_steps=2
 
 The pdt criteria take their loss from the forward kernel's cross-entropy rider; torch's criterion computes its own, next to the
 rider's unused one.  Every arm gets its own model (same initial weights) and its own GraphedTrainStep.  Inputs rotate through a
@@ -47,37 +51,45 @@ def main():
     xs = torch.rand((POOL_IMAGES,) + IMG, generator=g).to(dev)
     ys = torch.randint(0, 10, (POOL_IMAGES,), generator=g).to(dev)
     w = (torch.rand(10, generator=g) + 0.5).to(dev)
+    # MixUp-like probability targets: λ·onehot(y) + (1 − λ)·onehot(y of the previous image), λ drawn per image
+    lam = torch.rand(POOL_IMAGES, 1, generator=g).to(dev)
+    onehot = torch.nn.functional.one_hot(ys, 10).float()
+    qs = (lam * onehot + (1 - lam) * onehot.roll(1, 0)).contiguous()
     torch.manual_seed(0)
     init = pdt.models.ConvNet().to(dev).state_dict()
-    criteria = {
-        "pdt_plain": (lambda: pdt.nn.CrossEntropyLoss(), 1),
-        "pdt_smooth": (lambda: pdt.nn.CrossEntropyLoss(label_smoothing=0.1), 1),
-        "pdt_smooth_weighted": (lambda: pdt.nn.CrossEntropyLoss(label_smoothing=0.1, weight=w), 1),
-        "torch_smooth": (lambda: torch.nn.CrossEntropyLoss(label_smoothing=0.1), 1),
-        "k2_pdt_plain": (lambda: pdt.nn.CrossEntropyLoss(), 2),
-        "k2_pdt_smooth": (lambda: pdt.nn.CrossEntropyLoss(label_smoothing=0.1), 2),
+    criteria = {   # name: (criterion factory, accumulation steps, targets)
+        "pdt_plain": (lambda: pdt.nn.CrossEntropyLoss(), 1, ys),
+        "pdt_smooth": (lambda: pdt.nn.CrossEntropyLoss(label_smoothing=0.1), 1, ys),
+        "pdt_smooth_weighted": (lambda: pdt.nn.CrossEntropyLoss(label_smoothing=0.1, weight=w), 1, ys),
+        "torch_smooth": (lambda: torch.nn.CrossEntropyLoss(label_smoothing=0.1), 1, ys),
+        "k2_pdt_plain": (lambda: pdt.nn.CrossEntropyLoss(), 2, ys),
+        "k2_pdt_smooth": (lambda: pdt.nn.CrossEntropyLoss(label_smoothing=0.1), 2, ys),
+        "pdt_soft": (lambda: pdt.nn.CrossEntropyLoss(), 1, qs),
+        "pdt_soft_smooth_weighted": (lambda: pdt.nn.CrossEntropyLoss(label_smoothing=0.1, weight=w), 1, qs),
+        "torch_soft": (lambda: torch.nn.CrossEntropyLoss(), 1, qs),
+        "k2_pdt_soft": (lambda: pdt.nn.CrossEntropyLoss(), 2, qs),
     }
     arms = {}
-    for name, (make, k) in criteria.items():
+    for name, (make, k, ts) in criteria.items():
         model = pdt.models.ConvNet().to(dev)
         model.load_state_dict(init)
         opt = pdt.optim.SGD(list(model.parameters()), 1e-4)
-        step = GraphedTrainStep(model, make(), opt, (xs[:k * MICRO], ys[:k * MICRO]), warmup=3, accumulation_steps=k)
+        step = GraphedTrainStep(model, make(), opt, (xs[:k * MICRO], ts[:k * MICRO]), warmup=3, accumulation_steps=k)
         if hasattr(opt, "stop_riding"):
             opt.stop_riding()   # the captured graph keeps the rider; disarm it so that the next model captures on its own
-        arms[name] = (step, k)
+        arms[name] = (step, k, ts)
 
     def run(name, n, base):
-        step, k = arms[name]
+        step, k, ts = arms[name]
         rows = k * MICRO
         for i in range(n):
             j = ((base + i) * rows) % (POOL_IMAGES - rows + 1)
-            step(xs[j:j + rows], ys[j:j + rows], inputs_ready=True)
+            step(xs[j:j + rows], ts[j:j + rows], inputs_ready=True)
 
     per = {name: [] for name in arms}
     for r in range(args.rounds):
         for name in arms:
-            step, _ = arms[name]
+            step = arms[name][0]
             run(name, args.warmup, 0)
             torch.cuda.synchronize()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -102,7 +114,7 @@ def main():
     }
     print(f"{result['card']}, power limit {result['power_limit_w']} W")
     for name in arms:
-        print(f"  {name:20s} {result['us_per_step_median'][name]:8.2f} us/step (median of {args.rounds} rounds, min "
+        print(f"  {name:24s} {result['us_per_step_median'][name]:8.2f} us/step (median of {args.rounds} rounds, min "
               f"{result['us_per_step_min'][name]:.2f})  {result['kernels_per_replay'][name]} own kernels per replay")
     print(json.dumps(result))
 
