@@ -509,17 +509,26 @@ void register_cuda_bindings(py::module_& m) {
     fused_convnet_trace_read(reinterpret_cast<unsigned long long*>(t.data_ptr<int64_t>()));
     return t;
   });
-  m.def("convnet_l1_bwd_wgrad", [](const at::Tensor& dp, const at::Tensor& y, const at::Tensor& x, const at::Tensor& saved,
+  m.def("convnet_l1_bwd_wgrad", [](const at::Tensor& dp, c10::optional<at::Tensor> y, const at::Tensor& x, const at::Tensor& saved,
                                    c10::optional<at::Tensor> gamma, c10::optional<at::Tensor> beta, at::Tensor dgamma, at::Tensor dbeta, at::Tensor dw,
                                    c10::optional<at::Tensor> db, c10::optional<at::Tensor> dy2_pad, c10::optional<at::Tensor> x2_pad,
                                    const at::Tensor& dysum2, at::Tensor dw2, c10::optional<at::Tensor> db2, py::object rider, py::object clip,
-                                   bool accumulate) {
-    chk(dp, "dp"); chk(y, "y"); chk(x, "x"); chk(saved, "saved"); chk(dgamma, "dgamma"); chk(dbeta, "dbeta"); chk(dw, "dw");
+                                   bool accumulate, c10::optional<at::Tensor> w1, c10::optional<at::Tensor> b1) {
+    chk(dp, "dp"); chk(x, "x"); chk(saved, "saved"); chk(dgamma, "dgamma"); chk(dbeta, "dbeta"); chk(dw, "dw");
     chk(dysum2, "dysum2"); chk(dw2, "dw2");
     c10::cuda::CUDAGuard g(x.device());
-    const int B = static_cast<int>(y.size(0));
-    TORCH_CHECK(dp.numel() == static_cast<int64_t>(B) * 5184 && x.numel() == static_cast<int64_t>(B) * 784 && dw.numel() == 400 &&
-                    dgamma.numel() == 16 && dbeta.numel() == 16, "convnet_l1_bwd_wgrad: layer-1 shape mismatch");
+    TORCH_CHECK(x.numel() % 784 == 0, "convnet_l1_bwd_wgrad: x [B,1,28,28] expected");
+    const int B = static_cast<int>(x.numel() / 784);
+    TORCH_CHECK(dp.numel() == static_cast<int64_t>(B) * 5184 && dw.numel() == 400 && dgamma.numel() == 16 && dbeta.numel() == 16,
+                "convnet_l1_bwd_wgrad: layer-1 shape mismatch");
+    // y: conv1's output as convnet_fwd(…, keep_y1=True) returns it, or None: the kernel recomputes it from x and w1 / b1 (bit for bit)
+    const float* y_ptr = opt_ptr(y, "y");
+    const float* w1_ptr = opt_ptr(w1, "w1");
+    const float* b1_ptr = opt_ptr(b1, "b1");
+    TORCH_CHECK(y_ptr != nullptr || w1_ptr != nullptr, "convnet_l1_bwd_wgrad: without y, conv1's weights w1 are needed to recompute it");
+    TORCH_CHECK(y_ptr == nullptr || y->numel() == static_cast<int64_t>(B) * 12544, "convnet_l1_bwd_wgrad: y [B,28,28,16] expected");
+    TORCH_CHECK(w1_ptr == nullptr || w1->numel() == 400, "convnet_l1_bwd_wgrad: w1 [16,1,5,5] expected");
+    TORCH_CHECK(b1_ptr == nullptr || b1->numel() == 16, "convnet_l1_bwd_wgrad: b1 [16] expected");
     TORCH_CHECK(dysum2.numel() == static_cast<int64_t>(B) * 32 && dw2.numel() == 12800, "convnet_l1_bwd_wgrad: layer-2 shape mismatch");
     // conv2's per-image weight-gradient partials: from the given frames (the tests' reference), or (both None) left by
     // convnet_l2_bwd_fc(…, p1) of this batch
@@ -544,7 +553,7 @@ void register_cuda_bindings(py::module_& m) {
     TORCH_CHECK(static_cast<long long>(l1_floats) + B <= scr.capacity_floats, "convnet_l1_bwd_wgrad: scratch too small");
     auto launch = [&](auto rider) {
       if (frames) launch_conv2_wgrad_partials(dy2_pad->data_ptr<float>(), x2_pad->data_ptr<float>(), B, wpart, cur_stream(x));
-      launch_convnet_l1_bwd_wgrad(dp.data_ptr<float>(), y.data_ptr<float>(), x.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"),
+      launch_convnet_l1_bwd_wgrad(dp.data_ptr<float>(), y_ptr, w1_ptr, b1_ptr, x.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"),
                                   opt_ptr(beta, "beta"), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), dw.data_ptr<float>(), opt_mut(db, "db"),
                                   wpart, dysum2.data_ptr<float>(), dw2.data_ptr<float>(), opt_mut(db2, "db2"), B, scr.partials,
                                   scr.partials + static_cast<size_t>(B) * 64, grid_sync(scr), cur_stream(x), rider, accumulate);
@@ -583,21 +592,24 @@ void register_cuda_bindings(py::module_& m) {
     else launch_rider(adam_rider(d));
   }, py::arg("dp"), py::arg("y"), py::arg("x"), py::arg("saved"), py::arg("gamma"), py::arg("beta"), py::arg("dgamma"), py::arg("dbeta"),
      py::arg("dw"), py::arg("db"), py::arg("dy2_pad"), py::arg("x2_pad"), py::arg("dysum2"), py::arg("dw2"), py::arg("db2"),
-     py::arg("rider") = py::none(), py::kw_only(), py::arg("clip") = py::none(), py::arg("accumulate") = false);
+     py::arg("rider") = py::none(), py::kw_only(), py::arg("clip") = py::none(), py::arg("accumulate") = false, py::arg("w1") = py::none(),
+     py::arg("b1") = py::none());
   m.def("convnet_fwd", [](const at::Tensor& x, const at::Tensor& w1, c10::optional<at::Tensor> b1, c10::optional<at::Tensor> g1,
                           c10::optional<at::Tensor> be1, c10::optional<at::Tensor> rm1, c10::optional<at::Tensor> rv1, c10::optional<at::Tensor> nbt1,
                           double mom1, double eps1, const at::Tensor& w2, c10::optional<at::Tensor> b2, c10::optional<at::Tensor> g2,
                           c10::optional<at::Tensor> be2, c10::optional<at::Tensor> rm2, c10::optional<at::Tensor> rv2, c10::optional<at::Tensor> nbt2,
                           double mom2, double eps2, const at::Tensor& fcw, c10::optional<at::Tensor> fcb, c10::optional<at::Tensor> target,
                           bool defer_loss_mean, double grad_scale, c10::optional<at::Tensor> ce_weight, int64_t ignore_index,
-                          double label_smoothing, const std::string& reduction) {
+                          double label_smoothing, const std::string& reduction, bool keep_y1) {
     chk(x, "x"); chk(w1, "w1"); chk(w2, "w2"); chk(fcw, "fc weight");
     c10::cuda::CUDAGuard g(x.device());
     TORCH_CHECK(x.numel() % 784 == 0 && w1.numel() == 400 && w2.numel() == 12800 && fcw.dim() == 2 && fcw.size(1) == 1568 && fcw.size(0) <= 16,
                 "convnet_fwd: x [B,1,28,28], w1 [16,1,5,5], w2 [32,16,5,5], fc weight [<=16, 1568] expected");
     const int B = static_cast<int>(x.numel() / 784), ncls = static_cast<int>(fcw.size(0));
     TORCH_CHECK(fused_convnet_supported(B), "convnet_fwd: batch ", B, " exceeds one CTA per SM");
-    at::Tensor y1 = at::empty({B, 28, 28, 16}, x.options()), p1 = at::empty({B, 18, 18, 16}, x.options()), saved1 = at::empty({32}, x.options());
+    // keep_y1=False: conv1's output is not stored (None in its place); convnet_l1_bwd_wgrad(y=None, w1=…, b1=…) recomputes it
+    at::Tensor y1 = keep_y1 ? at::empty({B, 28, 28, 16}, x.options()) : at::Tensor();
+    at::Tensor p1 = at::empty({B, 18, 18, 16}, x.options()), saved1 = at::empty({32}, x.options());
     at::Tensor y2 = at::empty({B, 14, 14, 32}, x.options()), out = at::empty({B, 32, 7, 7}, x.options()), saved2 = at::empty({64}, x.options());
     at::Tensor logits = at::empty({B, ncls}, x.options());
     auto nbt_ptr = [](c10::optional<at::Tensor>& t) -> long long* {
@@ -631,7 +643,7 @@ void register_cuda_bindings(py::module_& m) {
       ce.dlogits = dlogits.data_ptr<float>();
       ce.counter = scr.counter + kCeCounterWord;
     }
-    launch_convnet_fwd(x.data_ptr<float>(), w1.data_ptr<float>(), opt_ptr(b1, "b1"), opt_ptr(g1, "g1"), opt_ptr(be1, "be1"), y1.data_ptr<float>(),
+    launch_convnet_fwd(x.data_ptr<float>(), w1.data_ptr<float>(), opt_ptr(b1, "b1"), opt_ptr(g1, "g1"), opt_ptr(be1, "be1"), keep_y1 ? y1.data_ptr<float>() : nullptr,
                        p1.data_ptr<float>(), saved1.data_ptr<float>(), opt_mut(rm1, "rm1"), opt_mut(rv1, "rv1"), nbt_ptr(nbt1), static_cast<float>(mom1),
                        static_cast<float>(eps1), w2.data_ptr<float>(), opt_ptr(b2, "b2"), opt_ptr(g2, "g2"), opt_ptr(be2, "be2"), y2.data_ptr<float>(),
                        out.data_ptr<float>(), saved2.data_ptr<float>(), opt_mut(rm2, "rm2"), opt_mut(rv2, "rv2"), nbt_ptr(nbt2), static_cast<float>(mom2),
@@ -642,7 +654,7 @@ void register_cuda_bindings(py::module_& m) {
      py::arg("eps1"), py::arg("w2"), py::arg("b2"), py::arg("g2"), py::arg("be2"), py::arg("rm2"), py::arg("rv2"), py::arg("nbt2"), py::arg("mom2"),
      py::arg("eps2"), py::arg("fcw"), py::arg("fcb"), py::arg("target") = py::none(), py::arg("defer_loss_mean") = false,
      py::arg("grad_scale") = 1.0, py::arg("ce_weight") = py::none(), py::arg("ignore_index") = -100, py::arg("label_smoothing") = 0.0,
-     py::arg("reduction") = "mean");
+     py::arg("reduction") = "mean", py::arg("keep_y1") = true);
   // p1 (conv2's input frame [B,18,18,16], optional): conv2's per-image weight-gradient partials are computed inside the kernel for
   // convnet_l1_bwd_wgrad(…, None, None, …) to fold, and the dy frame is not written (None in its place).  The training step always
   // passes p1; the dy frame of the form without it, fed to convnet_l1_bwd_wgrad, is the tests' reference for those partials.

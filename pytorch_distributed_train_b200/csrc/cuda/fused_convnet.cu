@@ -13,7 +13,8 @@
 //   convnet_l2_bwd_kernel<WG>  classifier backward + MaxPool/ReLU/BN backward ──barrier (Σdz, Σdz·x̂)── dy → conv2 data
 //                              gradient on wgmma (warps 4..7), next to it conv2's weight-gradient partial of the image on
 //                              wgmma (warps 0..3; K-major copies of x, written in the barrier's shadow, and of dy)
-//   convnet_l1_bwd_kernel      MaxPool/ReLU/BN backward ──barrier── conv1 weight gradient (mma.sync) ──barrier── conv1 fold;
+//   convnet_l1_bwd_kernel      conv1 recomputed (the forward stores no conv1 output: the same FMA order gives the same bits)
+//                              MaxPool/ReLU/BN backward ──barrier── conv1 weight gradient (mma.sync) ──barrier── conv1 fold;
 //                              conv2's weight gradient is folded in the shadow of the first barrier, and — on one GPU — the
 //                              threads that write the folded gradients apply the optimizer update (SgdRider / AdamRider / AmsgradRider /
 //                              RmspropRider / AdagradRider)
@@ -247,14 +248,79 @@ struct L1Map {
   }
 };
 
-// The zero-haloed image by the NT threads of the CTA.
+// The zero-haloed image by the NT threads of the CTA, in two halves: load() requests this thread's pixels, so that their latency
+// overlaps the other prologue loads (conv1's weights) instead of following them; store() zeroes the frame, waits for the CTA and
+// writes them (the caller syncs before reading xs).
 template <int NT>
-__device__ __forceinline__ void l1_load_image(const float* __restrict__ x, float* xs /*[32][32]*/, int tid) {
-  for (int i = tid; i < 1024; i += NT) xs[i] = 0.f;
-  __syncthreads();
-  for (int i = tid; i < 784; i += NT) {
-    const int rr = i / 28, cc = i - rr * 28;
-    xs[(rr + 2) * 32 + cc + 2] = x[i];
+struct L1Image {
+  static constexpr int kPer = (784 + NT - 1) / NT;
+  float v[kPer];
+  __device__ __forceinline__ void load(const float* __restrict__ x, int tid) {
+#pragma unroll
+    for (int u = 0; u < kPer; ++u) v[u] = tid + u * NT < 784 ? x[tid + u * NT] : 0.f;
+  }
+  __device__ __forceinline__ void store(float* xs /*[32][32]*/, int tid) const {
+    for (int i = tid; i < 1024; i += NT) xs[i] = 0.f;
+    __syncthreads();
+#pragma unroll
+    for (int u = 0; u < kPer; ++u) {
+      const int i = tid + u * NT, rr = i / 28, cc = i - rr * 28;
+      if (i < 784) xs[(rr + 2) * 32 + cc + 2] = v[u];
+    }
+  }
+};
+
+// conv1 of P pixels of one image, channels c0 .. c0 + C of them: pixel i at xoff[i] = r·32 + c in the haloed image xs, ws = the weights
+// [25 taps][16 co] in shared memory + c0, b1 = the bias + c0 (or null).  acc[i][j] = b1[j], then one fmaf per tap, kh outer, kw inner.
+// Every caller accumulates in this one order whatever its CTA shape or channel split, so the forward's y1 and backward B's recompute
+// of it are the same bits.
+template <int P, int C>
+__device__ __forceinline__ void conv1_pixels(const float* xs, const float* ws, const float* b1, const int (&xoff)[P], float (&acc)[P][C]) {
+  static_assert(C % 4 == 0, "conv1_pixels: whole float4 weight groups");
+#pragma unroll
+  for (int j = 0; j < C; ++j) {
+    const float b = b1 ? __ldg(b1 + j) : 0.f;
+#pragma unroll
+    for (int i = 0; i < P; ++i) acc[i][j] = b;
+  }
+#pragma unroll 1
+  for (int kh = 0; kh < 5; ++kh) {
+#pragma unroll
+    for (int kw = 0; kw < 5; ++kw) {
+      float xv[P];
+#pragma unroll
+      for (int i = 0; i < P; ++i) xv[i] = xs[xoff[i] + kh * 32 + kw];
+      const float4* wt = reinterpret_cast<const float4*>(ws + (kh * 5 + kw) * 16);
+#pragma unroll
+      for (int q = 0; q < C / 4; ++q) {
+        const float4 wq = wt[q];
+#pragma unroll
+        for (int i = 0; i < P; ++i) {
+          acc[i][4 * q + 0] = fmaf(xv[i], wq.x, acc[i][4 * q + 0]);
+          acc[i][4 * q + 1] = fmaf(xv[i], wq.y, acc[i][4 * q + 1]);
+          acc[i][4 * q + 2] = fmaf(xv[i], wq.z, acc[i][4 * q + 2]);
+          acc[i][4 * q + 3] = fmaf(xv[i], wq.w, acc[i][4 * q + 3]);
+        }
+      }
+    }
+  }
+}
+
+// One butterfly stage of a 4 × 4 block transpose over the four lanes of a pooling window (lanes 4w .. 4w + 3): lanes S apart swap
+// the blocks whose index differs from theirs in bit S.  Constant indices only, so a stays in registers.
+template <int S>
+__device__ __forceinline__ void window_transpose_step(float (&a)[4][4], int lane) {
+  const bool upper = (lane & S) != 0;
+#pragma unroll
+  for (int i0 = 0; i0 < 4; ++i0) {
+    if (i0 & S) continue;
+    const int i1 = i0 | S;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float got = __shfl_xor_sync(0xffffffffu, upper ? a[i0][j] : a[i1][j], S);
+      a[i0][j] = upper ? got : a[i0][j];
+      a[i1][j] = upper ? a[i1][j] : got;
+    }
   }
 }
 
@@ -543,9 +609,12 @@ __device__ __forceinline__ void ride(const Rider& sr, float& ca, int k, int i, f
 
 // ACC (accumulate mode, gradient accumulation over micro-batches): every gradient this kernel writes — dgamma, dbeta, the conv1 fold
 // dw / db and the conv2 fold dw2 / db2 — becomes g = g_old + v, and the rider updates with (and clips) that accumulated value.
+// y: conv1's output [B][28][28][16], or null: then the CTA recomputes its pixel's values from the image and w1 / b1 (conv1_pixels, the
+// forward's order, so the same bits) instead of loading 50 KB per image that the forward would have had to store.
 template <class Rider = SgdRider, bool ACC = false>
 __global__ void __launch_bounds__(kL1Threads, 1)
-convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y, const float* __restrict__ x, const float* __restrict__ saved,
+convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y, const float* w1, const float* b1, const float* __restrict__ x,
+                      const float* __restrict__ saved,
                       const float* __restrict__ gamma, const float* __restrict__ beta, float* dgamma, float* dbeta, float* dw, float* db,
                       float* partials, float* partials_w, GridSync gs,
                       // conv2's weight gradient, folded from the per-image partials [B][400][32] and Σdy rows [B][32]
@@ -559,6 +628,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   // Adam rider: the per-launch factors; Adagrad rider: the ten decayed learning rates
   __shared__ float adam_f[kAdam ? kAdamFactors : kAdagrad ? 10 : 1];
   __shared__ float xs[32 * 32];
+  __shared__ __align__(16) float ws[25 * 16];   // conv1's weights [tap][co] when y is recomputed
   __shared__ float red[kL1Warps * 32];
   __shared__ float s_tmp[kL1Warps * 32];
   __shared__ float s_tot[32];
@@ -572,7 +642,24 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   TRACE_INIT();
   trace(1, 0);
 
-  l1_load_image<kL1Threads>(x + static_cast<size_t>(n) * 784, xs, tid);
+  // the image and conv1's weights are requested together (one round trip, not two in a row), then the pooled gradient, whose loads
+  // are in flight while the image is staged and y is loaded or recomputed.  conv1's weights and bias (here and in conv1_pixels) are
+  // read before the first grid barrier, and the rider updates them (parameters 0 and 1) only after the second one, so no CTA reads an
+  // updated weight
+  L1Image<kL1Threads> img;
+  img.load(x + static_cast<size_t>(n) * 784, tid);
+  const float w1v = y == nullptr && tid < 400 ? w1[(tid & 15) * 25 + (tid >> 4)] : 0.f;
+  float dz[16];
+  {
+    const float4* gp = reinterpret_cast<const float4*>(dp + ((static_cast<size_t>(n) * 18 + m.ph + 2) * 18 + m.pw + 2) * 16);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const float4 g4 = m.valid ? gp[q] : make_float4(0.f, 0.f, 0.f, 0.f);
+      dz[4 * q] = g4.x; dz[4 * q + 1] = g4.y; dz[4 * q + 2] = g4.z; dz[4 * q + 3] = g4.w;
+    }
+  }
+  img.store(xs, tid);
+  if (y == nullptr && tid < 400) ws[tid] = w1v;
   if (tid < 16) {
     const float mean = saved[tid], invstd = saved[16 + tid];
     const float g = gamma ? gamma[tid] : 1.f, b = beta ? beta[tid] : 0.f;
@@ -588,18 +675,29 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   }
   __syncthreads();
 
-  float yv[16], dz[16];
-  {
+  float yv[16];
+  if (y != nullptr) {
     const float4* yp = reinterpret_cast<const float4*>(y + ((static_cast<size_t>(n) * 28 + m.r) * 28 + m.c) * 16);
-    const float4* gp = reinterpret_cast<const float4*>(dp + ((static_cast<size_t>(n) * 18 + m.ph + 2) * 18 + m.pw + 2) * 16);
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const float4 a = m.valid ? yp[q] : make_float4(0.f, 0.f, 0.f, 0.f);
-      const float4 g4 = m.valid ? gp[q] : make_float4(0.f, 0.f, 0.f, 0.f);
       yv[4 * q] = a.x; yv[4 * q + 1] = a.y; yv[4 * q + 2] = a.z; yv[4 * q + 3] = a.w;
-      dz[4 * q] = g4.x; dz[4 * q + 1] = g4.y; dz[4 * q + 2] = g4.z; dz[4 * q + 3] = g4.w;
     }
+  } else {
+    // the window's four lanes share the recompute: lane d computes channels 4d .. 4d + 3 of the window's four pixels, so that every
+    // weight read from shared memory serves four pixels, then the lanes transpose the 4 × 4 blocks: lane d gets its pixel's 16
+    const int x0 = 2 * m.ph * 32 + 2 * m.pw;
+    const int xoff[4] = {x0, x0 + 1, x0 + 32, x0 + 33};   // pixel d of the window: row 2·ph + (d >> 1), column 2·pw + (d & 1)
+    float blk[4][4];
+    conv1_pixels<4, 4>(xs, ws + 4 * m.d, b1 ? b1 + 4 * m.d : nullptr, xoff, blk);
+    window_transpose_step<2>(blk, lane);
+    window_transpose_step<1>(blk, lane);
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) yv[4 * e + j] = m.valid ? blk[e][j] : 0.f;   // the padding threads hold zeros, as when y is loaded
   }
+  trace(1, 8);
   // route the pooled gradient to the arg-max of the window (first maximum wins, like torch) and through the ReLU
   unsigned int mine = 0;
   float zmax[16];
@@ -1003,7 +1101,7 @@ constexpr int kFwdPix = 392;
 constexpr int kFwdThreads = 416;
 constexpr int kFwdWarps = kFwdThreads / 32;
 
-// conv1 output of one pixel → y1 (backward reads it).
+// conv1 output of one pixel → y1 (for direct callers of convnet_fwd).
 __device__ __forceinline__ void l1_store_y(float* __restrict__ y1, int n, const L1Map& m, const float (&acc)[16]) {
   float4* yp = reinterpret_cast<float4*>(y1 + ((static_cast<size_t>(n) * 28 + m.r) * 28 + m.c) * 16);
 #pragma unroll
@@ -1095,37 +1193,23 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
   // as they are: only the padding rows of tile 1 read them, and those outputs are dropped.
   for (int i = tid; i < 128 * 4; i += kFwdThreads)
     *reinterpret_cast<float4*>(sa + sw128_off(patch_halo_row(i >> 2), i & 3)) = make_float4(0.f, 0.f, 0.f, 0.f);
-  l1_load_image<kFwdThreads>(x + static_cast<size_t>(n) * 784, xs, tid);
-  if (tid < 400) {
-    const int tap = tid >> 4, co = tid & 15;
-    ws[tid] = w1[co * 25 + tap];
+  {   // the image and conv1's weights are requested together: one round trip, not two in a row
+    L1Image<kFwdThreads> img;
+    img.load(x + static_cast<size_t>(n) * 784, tid);
+    const float w1v = tid < 400 ? w1[(tid & 15) * 25 + (tid >> 4)] : 0.f;
+    img.store(xs, tid);
+    if (tid < 400) ws[tid] = w1v;   // [tap][co]
   }
   __syncthreads();
   trace(0, 11);
 
   // ---- layer 1: both pixels in the FMA order of one pixel per thread, so y1 does not depend on the CTA shape ---------------
-  float acc0[16], acc1[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) acc0[j] = acc1[j] = b1 ? __ldg(b1 + j) : 0.f;
-#pragma unroll 1
-  for (int kh = 0; kh < 5; ++kh) {
-#pragma unroll
-    for (int kw = 0; kw < 5; ++kw) {
-      const float xv0 = xs[(m0.r + kh) * 32 + m0.c + kw], xv1 = xs[(m1.r + kh) * 32 + m1.c + kw];
-      const float4* wt = reinterpret_cast<const float4*>(ws + (kh * 5 + kw) * 16);
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float4 wq = wt[q];
-        acc0[4 * q + 0] = fmaf(xv0, wq.x, acc0[4 * q + 0]);
-        acc0[4 * q + 1] = fmaf(xv0, wq.y, acc0[4 * q + 1]);
-        acc0[4 * q + 2] = fmaf(xv0, wq.z, acc0[4 * q + 2]);
-        acc0[4 * q + 3] = fmaf(xv0, wq.w, acc0[4 * q + 3]);
-        acc1[4 * q + 0] = fmaf(xv1, wq.x, acc1[4 * q + 0]);
-        acc1[4 * q + 1] = fmaf(xv1, wq.y, acc1[4 * q + 1]);
-        acc1[4 * q + 2] = fmaf(xv1, wq.z, acc1[4 * q + 2]);
-        acc1[4 * q + 3] = fmaf(xv1, wq.w, acc1[4 * q + 3]);
-      }
-    }
+  float acc[2][16];
+  float(&acc0)[16] = acc[0];
+  float(&acc1)[16] = acc[1];
+  {
+    const int xoff[2] = {m0.r * 32 + m0.c, m1.r * 32 + m1.c};
+    conv1_pixels<2, 16>(xs, ws, b1, xoff, acc);
   }
   trace(0, 1);
   // this image's [Σy (16) | M2 (16)] (fold_centred_stats): Σy first, then the squared deviations about the image's mean
@@ -1192,7 +1276,7 @@ convnet_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w1, co
   __syncthreads();
   l1_pool_store(acc0, m0, s_scale, s_shift, sa, p1n);
   l1_pool_store(acc1, m1, s_scale, s_shift, sa, p1n);
-  if (m0.valid) {   // y1 for the backward pass (nothing in this kernel reads it): drains behind conv2
+  if (y1 && m0.valid) {   // y1 for direct callers (nothing in this kernel reads it; backward B recomputes it): drains behind conv2
     l1_store_y(y1, n, m0, acc0);
     l1_store_y(y1, n, m1, acc1);
   }
@@ -1874,17 +1958,18 @@ void launch_conv2_wgrad_partials(const float* dy2_pad, const float* x2_pad, int 
 }
 
 template <class Rider>
-void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
-                                 float* dgamma, float* dbeta, float* dw, float* db, const float* wpart, const float* dysum2, float* dw2, float* db2,
-                                 int B, float* partials, float* partials_w, GridSync gs, cudaStream_t st, Rider rider, bool accumulate) {
+void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* w1, const float* b1, const float* x, const float* saved,
+                                 const float* gamma, const float* beta, float* dgamma, float* dbeta, float* dw, float* db, const float* wpart,
+                                 const float* dysum2, float* dw2, float* db2, int B, float* partials, float* partials_w, GridSync gs, cudaStream_t st,
+                                 Rider rider, bool accumulate) {
   auto kernel = accumulate ? convnet_l1_bwd_kernel<Rider, true> : convnet_l1_bwd_kernel<Rider>;
-  launch_cooperative(kernel, B, kL1Threads, static_cast<size_t>(kL1BwdSmem), st, "convnet_l1_bwd_wgrad", true, dp, y, x, saved,
+  launch_cooperative(kernel, B, kL1Threads, static_cast<size_t>(kL1BwdSmem), st, "convnet_l1_bwd_wgrad", true, dp, y, w1, b1, x, saved,
                      gamma, beta, dgamma, dbeta, dw, db, partials, partials_w, gs, wpart, dysum2, dw2, db2, rider);
 }
 #define PDT_L1_BWD_WGRAD(R)                                                                                                            \
-  template void launch_convnet_l1_bwd_wgrad<R>(const float*, const float*, const float*, const float*, const float*, const float*, float*, \
-                                               float*, float*, float*, const float*, const float*, float*, float*, int, float*, float*,       \
-                                               GridSync, cudaStream_t, R, bool);
+  template void launch_convnet_l1_bwd_wgrad<R>(const float*, const float*, const float*, const float*, const float*, const float*,       \
+                                               const float*, const float*, float*, float*, float*, float*, const float*, const float*, float*, \
+                                               float*, int, float*, float*, GridSync, cudaStream_t, R, bool);
 PDT_L1_BWD_WGRAD(SgdRider)
 PDT_L1_BWD_WGRAD(AdamRider)
 PDT_L1_BWD_WGRAD(ClipRider<SgdRider>)

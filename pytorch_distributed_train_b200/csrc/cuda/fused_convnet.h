@@ -92,11 +92,13 @@ void launch_conv2_wgrad_partials(const float* dy2_pad, const float* x2_pad, int 
 // or one of them in a ClipRider.
 // accumulate: gradient accumulation — every gradient written (dgamma, dbeta, dw, db, dw2, db2) becomes g_old + this batch's value, and
 // the rider updates with (and clips) the accumulated gradient.
+// y: conv1's output [B,28,28,16] (conv1 + bias) as launch_convnet_fwd wrote it, or nullptr: then each CTA recomputes it from x and
+// conv1's weights w1 [16,1,5,5] and bias b1 [16] (nullable) in the forward's order, bit for bit; w1 is required then.
 template <class Rider = SgdRider>
-void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* x, const float* saved, const float* gamma, const float* beta,
-                                 float* dgamma, float* dbeta, float* dw, float* db, const float* wpart, const float* dysum2, float* dw2, float* db2,
-                                 int B, float* partials, float* partials_w, GridSync gs, cudaStream_t st, Rider rider = Rider{},
-                                 bool accumulate = false);
+void launch_convnet_l1_bwd_wgrad(const float* dp, const float* y, const float* w1, const float* b1, const float* x, const float* saved,
+                                 const float* gamma, const float* beta, float* dgamma, float* dbeta, float* dw, float* db, const float* wpart,
+                                 const float* dysum2, float* dw2, float* db2, int B, float* partials, float* partials_w, GridSync gs, cudaStream_t st,
+                                 Rider rider = Rider{}, bool accumulate = false);
 // Optional rider of the whole-forward kernel: the mean cross-entropy of the logits against `target` and its gradient
 // (softmax − onehot)/n, computed by the CTA that owns the image; the batch mean is folded by the CTA that finishes last
 // (arrival counter, fixed summation order).  n counts the images whose target is in [0, ncls); the others (ignore_index) add
@@ -132,8 +134,8 @@ struct SoftCe : SmoothCe {
 };
 
 // The whole training forward in one launch: layer 1 and layer 2 (+ classifier, ncls ≤ 16) of an image in the same CTA; the
-// pooled layer-1 activations go into conv2's shared-memory patch directly.  x [B,28,28] → y1 [B,28,28,16] (conv1 + bias, kept for
-// backward), p1 [B,18,18,16] frame (BN + ReLU + pool), saved1 [32] = mean, invstd; y2 [B,14,14,32], out [B,32,7,7] NCHW, saved2
+// pooled layer-1 activations go into conv2's shared-memory patch directly.  x [B,28,28] → y1 [B,28,28,16] (conv1 + bias; nullptr:
+// not stored — the layer-1 backward recomputes it), p1 [B,18,18,16] frame (BN + ReLU + pool), saved1 [32] = mean, invstd; y2 [B,14,14,32], out [B,32,7,7] NCHW, saved2
 // [64]; logits [B,ncls].  partials: B·(32 + 64) floats.
 // With probability targets the SoftCe instantiation runs; with class-index targets a non-default spec runs the SmoothCe one, else
 // ce.scale != 1 the ScaledCe one; otherwise the kernel without the scale.

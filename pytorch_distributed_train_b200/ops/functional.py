@@ -292,14 +292,17 @@ class _FusedLayer1(torch.autograd.Function):
         c2, bn2, fc = whole["conv2"], whole["bn2"], whole["fc"]
         defer = bool(whole.get("defer_loss_mean", False))
         cw, ignore_index, reduction, smoothing = whole.get("spec", DEFAULT_CE_SPEC)
-        out, y, saved, p2, y2, saved2, logits, loss, dlogits, loss_parts = _C.convnet_fwd(
+        out, _, saved, p2, y2, saved2, logits, loss, dlogits, loss_parts = _C.convnet_fwd(
             x, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, c2.weight, c2.bias, bn2.weight, bn2.bias,
             bn2.running_mean, bn2.running_var, bn2.num_batches_tracked, float(bn2.momentum), float(bn2.eps), fc.weight, fc.bias,
-            whole.get("target"), defer, float(whole.get("grad_scale", 1.0)), cw, int(ignore_index), float(smoothing), reduction)
+            whole.get("target"), defer, float(whole.get("grad_scale", 1.0)), cw, int(ignore_index), float(smoothing), reduction,
+            keep_y1=False)
         whole["layer2"] = (p2, y2, saved2, logits)
         whole["ce"] = (loss, dlogits)
         whole["ce_deferred"] = (loss_parts, loss) if defer else None
-        ctx.save_for_backward(x, y, saved, gamma, beta)
+        # conv1's output is not kept: the backward kernel recomputes it from x, w and b, bit for bit.  w and b are saved tensors, so an
+        # in-place change to them before backward fails autograd's version check instead of recomputing from other weights.
+        ctx.save_for_backward(x, w, b, saved, gamma, beta)
         ctx.params = (w, b, gamma, beta, w2, b2)
         ctx.link = link
         return out  # [B,18,18,16]: zero-haloed NHWC frame
@@ -307,7 +310,7 @@ class _FusedLayer1(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dp):
         global _fused_backward_params
-        x, y, saved, gamma, beta = ctx.saved_tensors
+        x, w, b, saved, gamma, beta = ctx.saved_tensors
         params = ctx.params   # w, b, gamma, beta, w2, b2
         # gradient accumulation (accumulate_into): the buffers of the earlier micro-batches, added to by the kernel
         # (only when layer 2's kernel accumulated too)
@@ -336,8 +339,8 @@ class _FusedLayer1(torch.autograd.Function):
                 grads = [q.grad if q is not None else None for q, _ in prev[:4]]
                 if all((g is None and ptr == 0) or (g is not None and g.data_ptr() == ptr) for g, (_, ptr) in zip(grads, prev[:4])):
                     desc = rider.build(grads)   # None when the optimizer cannot ride this iteration
-        _C.convnet_l1_bwd_wgrad(dp.contiguous(), y, x, saved, gamma, beta, dg, dbe, dw, db, None, None, dysum2, dw2, db2, desc,
-                                clip=rider.clip if desc is not None else None, accumulate=acc is not None)
+        _C.convnet_l1_bwd_wgrad(dp.contiguous(), None, x, saved, gamma, beta, dg, dbe, dw, db, None, None, dysum2, dw2, db2, desc,
+                                clip=rider.clip if desc is not None else None, accumulate=acc is not None, w1=w, b1=b)
         if desc is not None:
             rider.owner._rode = True
         _fused_backward_params = list(params) + [q for q, _ in prev[:4]]

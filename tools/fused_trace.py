@@ -36,7 +36,7 @@ names = {0: ("forward (whole)", ["start", "conv1 done", "stats partial written",
                                  "conv2 done (ys + stats 2 in smem)", "stats 2 partial written", "barrier 2 passed", "pooled 2 in smem",
                                  "logits written", "end (incl. loss)", "prologue done (halo zeroed, weights requested)"]),
          1: ("l1_bwd (+conv2 wgrad fold)", ["start", "partial written", "barrier passed", "folded", "conv1 wgrad partial written", "barrier 2 passed",
-                                            "end", "dW2 folded"]),
+                                            "end", "dW2 folded", "y recomputed (conv1)"]),
          3: ("l2_bwd (+conv2 wgrad partials)", ["start", "B built", "partial written", "barrier passed", "folded", "dy written", "end",
                                                 "dW2 atoms done (warp 0)", "dx written (warp 4)"])}
 def report(t, title):
