@@ -439,8 +439,8 @@ void register_cuda_bindings(py::module_& m) {
 
   // ---- convolution ---------------------------------------------------------------------------------
   // The shape picks the kernels: conv2 (16→32) runs on the tensor cores (TMA-im2col wgmma forward and data gradient, mma.sync
-  // weight gradient), every other shape on the SIMT forward and weight gradient, which cover conv1 (1→16) and refuse the rest.
-  // Only conv2 has a data gradient: conv1's input needs none.
+  // weight gradient), every other shape on the SIMT kernels, which cover conv1 (1→16: forward, weight gradient, and the data
+  // gradient an input that requires grad takes) and refuse the rest.
   // centred: stats = [mean, M2, n] (ops_kernels.h), without the cancellation of Σy² when |mean| ≫ std; fp64_sums: the fp64
   // [Σy, Σy², n, 0] formed from the same centred fold, which SyncBatchNorm all-reduces; the default is the fp32 [Σ, Σ², n]
   m.def("conv5x5_fwd", [](const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> bias, bool want_stats, bool zero_pad,
@@ -476,7 +476,8 @@ void register_cuda_bindings(py::module_& m) {
     s.Cin = static_cast<int>(w.size(1));
     TORCH_CHECK(dy.size(3) == s.Cout, "conv5x5_dgrad: dy channels must equal weight Cout");
     at::Tensor dx = at::empty({s.B, s.H, s.W, s.Cin}, dy.options());
-    launch_conv5x5_dgrad_im2col(dy.data_ptr<float>(), w.data_ptr<float>(), dx.data_ptr<float>(), s, cur_stream(dy));
+    auto launch = conv_wgmma_supported(s) ? launch_conv5x5_dgrad_im2col : launch_conv5x5_dgrad;
+    launch(dy.data_ptr<float>(), w.data_ptr<float>(), dx.data_ptr<float>(), s, cur_stream(dy));
     return dx;
   }, py::arg("dy"), py::arg("w"));
 
@@ -741,17 +742,24 @@ void register_cuda_bindings(py::module_& m) {
     return py::make_tuple(sums, dgamma, dbeta);
   }, py::arg("dout"), py::arg("y"), py::arg("saved"), py::arg("gamma"), py::arg("beta"), py::arg("dout_nchw"),
      py::arg("dgamma_out") = py::none(), py::arg("dbeta_out") = py::none());
+  // Batch statistics take bn_relu_pool_bwd_reduce's (possibly all-reduced) sums and the element count.  mean_var=True: the forward
+  // ran with mean_var=True (eval: the running statistics, constants of the graph), so dy has no batch-mean terms and takes neither.
   m.def("bn_relu_pool_bwd_apply", [](const at::Tensor& dout, const at::Tensor& y, const at::Tensor& saved, c10::optional<at::Tensor> gamma,
-                                     c10::optional<at::Tensor> beta, const at::Tensor& sums, const at::Tensor& count, bool dout_nchw) {
-    chk(dout, "dout"); chk(y, "y"); chk(saved, "saved"); chk(sums, "sums"); chk(count, "count");
+                                     c10::optional<at::Tensor> beta, c10::optional<at::Tensor> sums, c10::optional<at::Tensor> count,
+                                     bool dout_nchw, bool mean_var) {
+    chk(dout, "dout"); chk(y, "y"); chk(saved, "saved");
+    const bool has_sums = sums.has_value() && sums->defined(), has_count = count.has_value() && count->defined();
+    TORCH_CHECK(has_sums != mean_var && has_count != mean_var,
+                "bn_relu_pool_bwd_apply: batch statistics take sums and count, mean_var=True takes neither");
     c10::cuda::CUDAGuard g(y.device());
     const int B = y.size(0), H = y.size(1), W = y.size(2), C = y.size(3);
     at::Tensor dy = at::empty_like(y);
     launch_bn_relu_pool_bwd_apply(dout.data_ptr<float>(), y.data_ptr<float>(), saved.data_ptr<float>(), opt_ptr(gamma, "gamma"),
-                                  opt_ptr(beta, "beta"), sums.data_ptr<float>(), count.data_ptr<float>(), dy.data_ptr<float>(), B, H, W, C,
-                                  dout_nchw, cur_stream(y));
+                                  opt_ptr(beta, "beta"), opt_ptr(sums, "sums"), opt_ptr(count, "count"), dy.data_ptr<float>(), B, H, W, C,
+                                  dout_nchw, mean_var, cur_stream(y));
     return dy;
-  });
+  }, py::arg("dout"), py::arg("y"), py::arg("saved"), py::arg("gamma"), py::arg("beta"), py::arg("sums"), py::arg("count"),
+     py::arg("dout_nchw"), py::arg("mean_var") = false);
 
   // ---- generic NCHW BatchNorm (SyncBatchNorm) ----------------------------------------------------------
   m.def("bn_stats_nchw_f64", [](const at::Tensor& x) {

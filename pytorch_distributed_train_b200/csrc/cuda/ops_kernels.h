@@ -57,6 +57,9 @@ void launch_conv5x5_fwd(const float* x, const float* w, const float* bias, float
                         ReduceScratch scr, cudaStream_t st);
 // dw [Cout,Cin,5,5], db [Cout] (nullable) from dy NHWC and x NHWC.
 void launch_conv5x5_wgrad(const float* dy, const float* x, float* dw, float* db, ConvShape s, ReduceScratch scr, cudaStream_t st);
+// dx NHWC [B,H,W,1] from dy NHWC [B,H,W,16] and w [16,1,5,5] (conv1's input gradient): one thread per pixel, fp32 fmaf in a
+// fixed order, so the result is deterministic at any B.
+void launch_conv5x5_dgrad(const float* dy, const float* w, float* dx, ConvShape s, cudaStream_t st);
 
 // ---- BatchNorm(train) + ReLU + MaxPool2x2, fused -----------------------------------------------------
 // Every bn_relu_pool launcher takes C ∈ {4, 8, 16, 32, 64} and even H, W.
@@ -77,10 +80,11 @@ void launch_bn_relu_pool_fwd(const float* y, const void* stats, const float* gam
 void launch_bn_relu_pool_bwd_reduce(const float* dout, const float* y, const float* saved, const float* gamma, const float* beta,
                                     float* sums, float* dgamma, float* dbeta, int B, int H, int W, int C, bool dout_nchw,
                                     ReduceScratch scr, cudaStream_t st);
-// Pass 2: dy NHWC [B,H,W,C] from the (possibly all-reduced) sums and the global count n.
+// Pass 2: dy NHWC [B,H,W,C] from the (possibly all-reduced) sums and the global count n.  mean_var: the forward ran on kBnMeanVar
+// statistics (eval), constants of the graph: dy = γ·invstd·dz at the arg-max and 0 elsewhere, and sums and count are not read.
 void launch_bn_relu_pool_bwd_apply(const float* dout, const float* y, const float* saved, const float* gamma, const float* beta,
                                    const float* sums, const float* count, float* dy, int B, int H, int W, int C, bool dout_nchw,
-                                   cudaStream_t st);
+                                   bool mean_var, cudaStream_t st);
 
 // ---- generic NCHW BatchNorm pieces (SyncBatchNorm on arbitrary models) ---------------------------------
 // stats [2C+1] ← per-channel Σx, Σx², then the element count per channel, accumulated and returned in fp64 (SyncBatchNorm

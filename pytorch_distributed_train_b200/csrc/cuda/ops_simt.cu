@@ -225,6 +225,49 @@ __global__ void __launch_bounds__(256) conv5x5_wgrad_kernel(const float* __restr
   }
 }
 
+// =====================================================================================================
+// conv1's data gradient (COUT→1), the transposed 5x5 convolution dx[h][w] = Σ_{kh,kw,co} dy[h+2−kh][w+2−kw][co]·w[co][kh][kw].
+// One CTA = TH rows of one image, one thread per dx pixel; the dy patch planar in smem (zero halo), the flipped filter [tap][co].
+// A pixel is one thread's chain of 25·COUT fmaf in a fixed order (taps row-major, channels inner), with no reduction across
+// threads or CTAs: the result does not depend on B or the launch, and repeats bit for bit.
+// =====================================================================================================
+template <int COUT, int TH>
+__global__ void __launch_bounds__(448) conv5x5_dgrad_cin1_kernel(const float* __restrict__ dy, const float* __restrict__ w,
+                                                                 float* __restrict__ dx, int H, int W) {
+  extern __shared__ __align__(16) float smem[];
+  const int PW = W + 4, PH = TH + 4;
+  float* ds = smem;                    // [COUT][PH][PW]: patch row r is dy row tile·TH + r − 2
+  float* ws = smem + COUT * PH * PW;   // [25][COUT]: ws[(fh·5 + fw)·COUT + co] = w[co][4−fh][4−fw]
+  const int tiles = H / TH;
+  const int n = blockIdx.x / tiles, tile = blockIdx.x % tiles, tid = threadIdx.x;
+  for (int i = tid; i < 25 * COUT; i += blockDim.x) {
+    const int tap = i / COUT, co = i % COUT;
+    ws[i] = w[co * 25 + 24 - tap];
+  }
+  for (int i = tid; i < COUT * PH * PW; i += blockDim.x) {
+    const int co = i % COUT, c = (i / COUT) % PW, r = i / (COUT * PW);
+    const int ih = tile * TH + r - 2, iw = c - 2;
+    float v = 0.f;
+    if (ih >= 0 && ih < H && iw >= 0 && iw < W) v = dy[((static_cast<size_t>(n) * H + ih) * W + iw) * COUT + co];
+    ds[(co * PH + r) * PW + c] = v;
+  }
+  __syncthreads();
+  if (tid >= TH * W) return;
+  const int py = tid / W, px = tid % W;
+  float acc = 0.f;
+#pragma unroll 1
+  for (int fh = 0; fh < 5; ++fh) {
+#pragma unroll
+    for (int fw = 0; fw < 5; ++fw) {
+      const float* wt = ws + (fh * 5 + fw) * COUT;
+      const float* dp = ds + (py + fh) * PW + px + fw;   // dy row tile·TH + py + 2 − kh with kh = 4 − fh
+#pragma unroll
+      for (int co = 0; co < COUT; ++co) acc = fmaf(dp[co * PH * PW], wt[co], acc);
+    }
+  }
+  dx[(static_cast<size_t>(n) * H + tile * TH + py) * W + px] = acc;
+}
+
 // out[i] = Σ_b partials[b][i] in a fixed order: a CTA owns 32 outputs (lane = output), its 8 warps
 // stride over the partial rows (coalesced 128-byte reads), then the 8 sub-sums are added in warp order.
 __global__ void __launch_bounds__(256) fold_partials_kernel(const float* __restrict__ partials, int nblk, int width, int split,
@@ -366,7 +409,9 @@ __device__ __forceinline__ void route(const float v[4], float scale, float shift
   *xhat = (v[a] - mean) * invstd;
 }
 
-template <bool APPLY>
+// MEAN_VAR (APPLY only): the forward normalised with kBnMeanVar statistics, which are constants of the graph, so the apply pass has
+// no batch-mean terms and reads neither sums nor count.
+template <bool APPLY, bool MEAN_VAR = false>
 __global__ void __launch_bounds__(256) bn_relu_pool_bwd_kernel(const float* __restrict__ dout, const float* __restrict__ y,
                                                                const float* __restrict__ saved, const float* __restrict__ gamma,
                                                                const float* __restrict__ beta, float* sums, float* dgamma,
@@ -381,7 +426,7 @@ __global__ void __launch_bounds__(256) bn_relu_pool_bwd_kernel(const float* __re
     s_invstd[c] = invstd;
     s_scale[c] = g * invstd;
     s_shift[c] = b - mean * g * invstd;
-    if (APPLY) {
+    if (APPLY && !MEAN_VAR) {
       const float n = fmaxf(*count, 1.f);
       s_m1[c] = sums[c] / n;
       s_m2[c] = sums[C + c] / n;
@@ -425,6 +470,10 @@ __global__ void __launch_bounds__(256) bn_relu_pool_bwd_kernel(const float* __re
       if constexpr (!APPLY) {
         a1[k] = dz;
         a2[k] = dz * xhat;
+      } else if constexpr (MEAN_VAR) {
+        // dy = γ·invstd·dz at the arg-max, 0 at the window's other positions
+#pragma unroll
+        for (int d = 0; d < 4; ++d) reinterpret_cast<float*>(&o4[d])[k] = d == arg ? s_scale[c] * dz : 0.f;
       } else {
         // dy = γ·invstd·(dz_pos − mean(dz) − x̂_pos·mean(dz·x̂)) at every position of the window
 #pragma unroll
@@ -1284,6 +1333,18 @@ void launch_conv5x5_wgrad(const float* dy, const float* x, float* dw, float* db,
   check_launch("fold_partials");
 }
 
+void launch_conv5x5_dgrad(const float* dy, const float* w, float* dx, ConvShape s, cudaStream_t st) {
+  constexpr int TH = 7;
+  if (!(s.Cin == 1 && s.Cout == 16)) throw std::invalid_argument("conv5x5_dgrad: supported channel configs are 16→32 and 1→16");
+  if (s.H % TH != 0) throw std::invalid_argument("conv5x5_dgrad: H must be a multiple of 7");
+  const size_t sm = (static_cast<size_t>(s.Cout) * (TH + 4) * (s.W + 4) + 25 * s.Cout) * sizeof(float);
+  if (TH * s.W > 448 || sm > 48 * 1024) throw std::invalid_argument("conv5x5_dgrad: W must be at most 63");
+  const int blocks = s.B * (s.H / TH);
+  if (blocks == 0) return;
+  conv5x5_dgrad_cin1_kernel<16, TH><<<blocks, (TH * s.W + 31) / 32 * 32, sm, st>>>(dy, w, dx, s.H, s.W);
+  check_launch("conv5x5_dgrad");
+}
+
 // The backward kernel takes a thread's channel quad from threadIdx.x % (C/4), which needs 256 % (C/4) == 0, and reduces the
 // quads of a warp with a shuffle tree over C/4 lanes, which needs a power of two: C ∈ {4, 8, 16, 32, 64}.  Pooling takes even H, W.
 static void check_bn_relu_pool_shape(int C, int H, int W, const char* what) {
@@ -1317,12 +1378,12 @@ void launch_bn_relu_pool_bwd_reduce(const float* dout, const float* y, const flo
 
 void launch_bn_relu_pool_bwd_apply(const float* dout, const float* y, const float* saved, const float* gamma, const float* beta,
                                    const float* sums, const float* count, float* dy, int B, int H, int W, int C, bool dout_nchw,
-                                   cudaStream_t st) {
+                                   bool mean_var, cudaStream_t st) {
   check_bn_relu_pool_shape(C, H, W, "bn_relu_pool_bwd_apply");
   const long long total = static_cast<long long>(B) * (H / 2) * (W / 2) * (C / 4);
-  bn_relu_pool_bwd_kernel<true><<<static_cast<int>((total + 255) / 256), 256, 0, st>>>(dout, y, saved, gamma, beta, const_cast<float*>(sums), nullptr,
-                                                                                       nullptr, count, dy, B, H, W, C, dout_nchw ? 1 : 0,
-                                                                                       ReduceScratch{});
+  auto kern = mean_var ? bn_relu_pool_bwd_kernel<true, true> : bn_relu_pool_bwd_kernel<true, false>;
+  kern<<<static_cast<int>((total + 255) / 256), 256, 0, st>>>(dout, y, saved, gamma, beta, const_cast<float*>(sums), nullptr, nullptr, count, dy,
+                                                              B, H, W, C, dout_nchw ? 1 : 0, ReduceScratch{});
   check_launch("bn_relu_pool_bwd_apply");
 }
 

@@ -8,7 +8,7 @@ sm_90a kernel with one CTA per image (``csrc/cuda/fused_convnet.cu``): conv1+BN1
 accumulators, haloed image in shared memory) +BN2+ReLU+pool2+classifier — the BatchNorm batch statistics cross a
 device-side grid barrier inside the kernel instead of a kernel boundary; backward is one such kernel per layer, with the
 classifier's backward and conv2's weight gradient riding along.  What the fused kernels do not cover (eval mode,
-SyncBatchNorm, batch > #SMs, a partially frozen model) runs each ``layerN`` as two per-op kernels (implicit-GEMM conv with the
+SyncBatchNorm, batch > #SMs, a partially frozen model, an input that requires grad) runs each ``layerN`` as two per-op kernels (implicit-GEMM conv with the
 BN statistics in its epilogue, then BN-apply+ReLU+MaxPool) and the classifier as one linear kernel.  The same modules fall back
 to the stock layers on CPU (plumbing tests) or when ``fused=False``.  Other layer configurations (another padding mode,
 dilation or stride, a swapped activation, pool or norm layer, an extra module in a ``Sequential``, module hooks, weight norm)

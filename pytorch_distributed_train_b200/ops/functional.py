@@ -61,6 +61,15 @@ def _to_nhwc(x: torch.Tensor) -> torch.Tensor:
     return x.permute(0, 2, 3, 1).contiguous()
 
 
+def _refuse_double_backward(op: str) -> None:
+    """Called first in every native backward.  Autograd runs a backward in grad mode only under ``create_graph=True`` (gradient
+    penalties, Hessian-vector products); the kernels' gradients carry no graph, so a loss built from them would silently train
+    without its gradient term.  Refuse instead."""
+    if torch.is_grad_enabled():
+        raise RuntimeError(f"{op}: the native kernels have no double backward (create_graph=True); torch's layers have one: "
+                           "ConvNet(fused=False), torch.nn.CrossEntropyLoss")
+
+
 class _ConvBnReluPool(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w, b, gamma, beta, running_mean, running_var, nbt, momentum, eps, training, group, out_nchw):
@@ -85,7 +94,7 @@ class _ConvBnReluPool(torch.autograd.Function):
             # the running mean and variance as they are: no round trip through sums, which would cancel the variance's digits
             out, saved = _C.bn_relu_pool_fwd(y, torch.cat([running_mean, running_var]), gamma, beta, None, None, None, 0.0, eps, out_nchw,
                                              mean_var=True)
-            count = None   # backward through eval-mode BatchNorm is refused below
+            count = None   # the running statistics are constants: backward has no batch-mean terms
         ctx.save_for_backward(xh, w, y, saved, gamma, beta, count)
         ctx.group, ctx.out_nchw, ctx.training = group, out_nchw, training
         ctx.params = (w, b, gamma, beta)
@@ -95,17 +104,20 @@ class _ConvBnReluPool(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dout):
+        _refuse_double_backward("conv_bn_relu_pool")
         xh, w, y, saved, gamma, beta, count = ctx.saved_tensors
         w_p, b_p, g_p, be_p = ctx.params
-        if not ctx.training:
-            raise RuntimeError("conv_bn_relu_pool: backward through eval-mode BatchNorm is not supported by the fused op")
         d = dout.contiguous() if ctx.out_nchw else dout.permute(0, 2, 3, 1).contiguous()
         gview = _grad_dst(g_p, gamma) if g_p is not None else None
         bview = _grad_dst(be_p, beta) if be_p is not None else None
+        # dγ = Σdz·x̂ and dβ = Σdz in either mode: `saved` holds the mean and invstd the forward normalised with
         sums, dgamma, dbeta = _C.bn_relu_pool_bwd_reduce(d, y, saved, gamma, beta, ctx.out_nchw, gview, bview)
-        if ctx.group is not None:
-            _inline_allreduce(ctx.group, sums)     # Σdz, Σdz·x̂ across the group
-        dy = _C.bn_relu_pool_bwd_apply(d, y, saved, gamma, beta, sums, count, ctx.out_nchw)
+        if not ctx.training:
+            dy = _C.bn_relu_pool_bwd_apply(d, y, saved, gamma, beta, None, None, ctx.out_nchw, mean_var=True)
+        else:
+            if ctx.group is not None:
+                _inline_allreduce(ctx.group, sums)     # Σdz, Σdz·x̂ across the group
+            dy = _C.bn_relu_pool_bwd_apply(d, y, saved, gamma, beta, sums, count, ctx.out_nchw)
         dw = _grad_dst(w_p, w)
         db = _grad_dst(b_p, w.new_empty(w.shape[0])) if b_p is not None else None
         _C.conv5x5_wgrad(dy, xh, dw, db)
@@ -310,6 +322,7 @@ class _FusedLayer1(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dp):
         global _fused_backward_params
+        _refuse_double_backward("fused ConvNet layer 1")
         x, w, b, saved, gamma, beta = ctx.saved_tensors
         params = ctx.params   # w, b, gamma, beta, w2, b2
         # gradient accumulation (accumulate_into): the buffers of the earlier micro-batches, added to by the kernel
@@ -365,6 +378,7 @@ class _FusedLayer2(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dout, dlogits):
+        _refuse_double_backward("fused ConvNet layer 2")
         w_p, b_p, g_p, be_p, fcw_p, fcb_p = ctx.params
         p1, y, saved, gamma, beta, w, out, fcw = ctx.saved_tensors
         if dout is not None:
@@ -475,6 +489,7 @@ class _Linear(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dout):
+        _refuse_double_backward("linear")
         x, w = ctx.saved_tensors
         w_p, b_p = ctx.params
         dw = _grad_dst(w_p, w)
@@ -506,6 +521,7 @@ class _CrossEntropy(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dloss):
+        _refuse_double_backward("cross_entropy")
         (grad0,) = ctx.saved_tensors
         if getattr(dloss, "_pdt_unit_seed", False):
             return grad0, None, None
@@ -522,6 +538,7 @@ class _CrossEntropyPrecomputed(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dloss):
+        _refuse_double_backward("cross_entropy (computed by the fused forward)")
         (grad0,) = ctx.saved_tensors
         if getattr(dloss, "_pdt_unit_seed", False):
             return grad0, None, None

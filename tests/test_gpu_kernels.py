@@ -56,7 +56,7 @@ def test_conv5x5_forward_and_stats(cin, cout, H, kernel, B):
     assert torch.equal(y, y2) and torch.equal(stats, stats2)
 
 
-@pytest.mark.parametrize("B", [5, 100])
+@pytest.mark.parametrize("B", [1, 5, 100, 2048])   # 2 tiles of 128 pixels, …, 3136 tiles: more than the grid
 def test_conv_tma_im2col_exact(B):
     """conv2's per-op kernels on TF32-representable integers, so every product and sum is exact: the TMA-im2col forward
     (SWIZZLE_64B rows, bias, Σy) and data gradient (SWIZZLE_128B rows), and the mma.sync weight gradient (MN-major operands)
@@ -96,7 +96,7 @@ def test_conv5x5_backward():
     # TF32 operands: ~1e-3 relative per product, random-walk over 19,600 pixels
     assert torch.allclose(dw, gw, atol=1.0, rtol=5e-3), (dw - gw).abs().max()
     assert torch.allclose(db, gb, atol=1.0, rtol=5e-3), (db - gb).abs().max()
-    # conv1 weight gradient (no data gradient: the input needs none)
+    # conv1 weight gradient (its data gradient: test_convnet_input_grads.py)
     x1 = torch.randn(B, 1, 28, 28, device=dev())
     w1 = torch.randn(16, 1, 5, 5, device=dev(), requires_grad=True)
     b1 = torch.randn(16, device=dev(), requires_grad=True)

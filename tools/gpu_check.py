@@ -29,6 +29,7 @@ GROUPS = {
     "ce_options": ["tests/test_cross_entropy_options.py"],
     "syncbn": ["tests/test_syncbn_native.py", "tests/test_syncbn_large_mean.py"],
     "maxpool_ties": ["tests/test_maxpool_ties.py"],
+    "input_grads": ["tests/test_convnet_input_grads.py"],
     "symm_emu": ["tests/test_symm_kernels_emulated.py"],
 }
 
