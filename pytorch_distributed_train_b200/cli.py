@@ -8,8 +8,8 @@ GPU → init_process_group over TCP → seed → model → optional SyncBN → D
 Extra flags cover what the reference hard-codes: ``--init-method`` (its LAN address
 ``tcp://10.9.1.2:34567`` only works on the author's network, ref: ddp_example.py:110; we default
 to loopback with a free port), ``--data synthetic|mnist``, ``--model``, ``--comm fused|nccl``, ``--algo``,
-``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw | rmsprop | adagrad), ``--lr``,
-``--momentum``, ``--amsgrad``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--mixup``,
+``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw | nadam | radam | rmsprop |
+adagrad), ``--lr``, ``--momentum``, ``--amsgrad``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--mixup``,
 ``--ema-decay``, ``--checkpoint`` / ``--resume``, ``--eval`` (test loss and accuracy after every epoch).
 """
 from __future__ import annotations
@@ -44,16 +44,17 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--data-root", default="./data", type=str)
     p.add_argument("--model", default="convnet", choices=["convnet", "resnet18"])
     p.add_argument("--batch-size", default=100, type=int, help="per-GPU batch size (reference: 100)")
-    p.add_argument("--optimizer", default="sgd", choices=["sgd", "adam", "adamw", "rmsprop", "adagrad"],
-                   help="optimizer: SGD (the reference's), Adam, AdamW, RMSprop or Adagrad, each a native multi-tensor kernel with "
-                        "torch's defaults")
+    p.add_argument("--optimizer", default="sgd", choices=["sgd", "adam", "adamw", "nadam", "radam", "rmsprop", "adagrad"],
+                   help="optimizer: SGD (the reference's), Adam, AdamW, NAdam, RAdam, RMSprop or Adagrad, each a native multi-tensor "
+                        "kernel with torch's defaults")
     p.add_argument("--lr", default=1e-4, type=float, help="learning rate (reference: 1e-4)")
     p.add_argument("--momentum", default=None, type=float, help="SGD momentum (default 0; not accepted with the other optimizers)")
     p.add_argument("--amsgrad", default=False, action="store_true",
                    help="Adam / AdamW with AMSGrad: the running maximum of exp_avg_sq in the denominator (not accepted with the other "
                         "optimizers)")
     p.add_argument("--weight-decay", default=None, type=float,
-                   help="weight decay (default: 0 for SGD, Adam, RMSprop and Adagrad, 1e-2 for AdamW, torch's defaults)")
+                   help="weight decay (default: 0 for SGD, Adam, NAdam, RAdam, RMSprop and Adagrad, 1e-2 for AdamW, torch's defaults; "
+                        "NAdam and RAdam take it as L2 decay added to the gradient)")
     p.add_argument("--clip-grad-norm", default=None, type=float, metavar="MAX",
                    help="clip the global gradient norm (L2) to MAX before every optimizer step (default: off)")
     p.add_argument("--accumulation-steps", default=1, type=int, metavar="K",
@@ -91,6 +92,10 @@ def make_optimizer(args, params):
         return pdt.optim.RMSprop(params, args.lr, **kw)
     if args.optimizer == "adagrad":
         return pdt.optim.Adagrad(params, args.lr, **kw)
+    if args.optimizer == "nadam":
+        return pdt.optim.NAdam(params, args.lr, **kw)
+    if args.optimizer == "radam":
+        return pdt.optim.RAdam(params, args.lr, **kw)
     cls = pdt.optim.Adam if args.optimizer == "adam" else pdt.optim.AdamW
     return cls(params, args.lr, amsgrad=getattr(args, "amsgrad", False), **kw)
 

@@ -113,16 +113,18 @@ SgdRider sgd_rider(const py::dict& d) {
 }
 
 // {"kind": "adam", "params", "prev_grads", "exp_avg", "exp_avg_sq", "step" (fp32 scalars on the device), "lr", "lr_tensor", "beta1",
-// "beta2", "eps", "weight_decay", "decoupled", "maximize"}, and for AMSGrad "max_exp_avg_sq" (ten tensors; amsgrad_rider below)
-AdamRider adam_rider(const py::dict& d) {
+// "beta2", "eps", "weight_decay", "decoupled", "maximize"}, and for AMSGrad "max_exp_avg_sq" (ten tensors; amsgrad_rider below).
+// The "nadam" and "radam" descriptions have the same entries (nadam_rider, radam_rider below); kind names them in errors.
+AdamRider adam_rider(const py::dict& d, const char* kind = "adam") {
   AdamRider r;
   const TensorList ms = tensors(d, "exp_avg"), vs = tensors(d, "exp_avg_sq"), steps = tensors(d, "step");
-  TORCH_CHECK(ms.size() == 10 && vs.size() == 10 && steps.size() == 10, "convnet_l1_bwd_wgrad: adam lists have the wrong length");
-  fill_rider(r, d, "adam", [&](int k, const at::Tensor& p) {
-    TORCH_CHECK(ms[k].has_value() && vs[k].has_value() && steps[k].has_value(), "convnet_l1_bwd_wgrad: adam state of parameter ", k, " missing");
+  TORCH_CHECK(ms.size() == 10 && vs.size() == 10 && steps.size() == 10, "convnet_l1_bwd_wgrad: ", kind, " lists have the wrong length");
+  fill_rider(r, d, kind, [&](int k, const at::Tensor& p) {
+    TORCH_CHECK(ms[k].has_value() && vs[k].has_value() && steps[k].has_value(), "convnet_l1_bwd_wgrad: ", kind, " state of parameter ", k,
+                " missing");
     chk(*ms[k], "exp_avg"); chk(*vs[k], "exp_avg_sq"); chk(*steps[k], "step");
-    TORCH_CHECK(ms[k]->numel() == p.numel() && vs[k]->numel() == p.numel() && steps[k]->numel() == 1, "convnet_l1_bwd_wgrad: adam state of parameter ",
-                k, " has the wrong size");
+    TORCH_CHECK(ms[k]->numel() == p.numel() && vs[k]->numel() == p.numel() && steps[k]->numel() == 1, "convnet_l1_bwd_wgrad: ", kind,
+                " state of parameter ", k, " has the wrong size");
     r.m[k] = ms[k]->data_ptr<float>();
     r.v[k] = vs[k]->data_ptr<float>();
     r.step[k] = steps[k]->data_ptr<float>();
@@ -153,6 +155,25 @@ float* rider_state(const TensorList& ts, int k, int64_t numel, const char* kind,
   chk(*ts[k], name);
   TORCH_CHECK(ts[k]->numel() == numel, "convnet_l1_bwd_wgrad: ", kind, " state ", name, " of parameter ", k, " has the wrong size");
   return ts[k]->data_ptr<float>();
+}
+
+// {"kind": "nadam", the "adam" entries, "mu_product" (ten fp32 scalars on the device), "momentum_decay"}
+NadamRider nadam_rider(const py::dict& d) {
+  NadamRider r;
+  static_cast<AdamRider&>(r) = adam_rider(d, "nadam");
+  const TensorList mps = tensors(d, "mu_product");
+  TORCH_CHECK(mps.size() == 10, "convnet_l1_bwd_wgrad: nadam lists have the wrong length");
+  for (int k = 0; k < 10; ++k)
+    if (r.p[k]) r.mu_product[k] = rider_state(mps, k, 1, "nadam", "mu_product");
+  r.momentum_decay = d["momentum_decay"].cast<double>();
+  return r;
+}
+
+// {"kind": "radam", the "adam" entries}
+RadamRider radam_rider(const py::dict& d) {
+  RadamRider r;
+  static_cast<AdamRider&>(r) = adam_rider(d, "radam");
+  return r;
 }
 
 // {"kind": "rmsprop", "params", "prev_grads", "square_avg", "step" (fp32 scalars on the device), "momentum_buffer" (ten, or empty when
@@ -584,9 +605,11 @@ void register_cuda_bindings(py::module_& m) {
     }
     const auto d = rider.cast<py::dict>();
     const auto kind = d["kind"].cast<std::string>();
-    TORCH_CHECK(kind == "sgd" || kind == "adam" || kind == "rmsprop" || kind == "adagrad",
-                "convnet_l1_bwd_wgrad: rider kind must be 'sgd', 'adam', 'rmsprop' or 'adagrad' (got '", kind, "')");
+    TORCH_CHECK(kind == "sgd" || kind == "adam" || kind == "nadam" || kind == "radam" || kind == "rmsprop" || kind == "adagrad",
+                "convnet_l1_bwd_wgrad: rider kind must be 'sgd', 'adam', 'nadam', 'radam', 'rmsprop' or 'adagrad' (got '", kind, "')");
     if (kind == "sgd") launch_rider(sgd_rider(d));
+    else if (kind == "nadam") launch_rider(nadam_rider(d));
+    else if (kind == "radam") launch_rider(radam_rider(d));
     else if (kind == "rmsprop") launch_rider(rmsprop_rider(d));
     else if (kind == "adagrad") launch_rider(adagrad_rider(d));
     else if (d.contains("max_exp_avg_sq")) launch_rider(amsgrad_rider(d));
@@ -954,6 +977,64 @@ void register_cuda_bindings(py::module_& m) {
       if (ams) launch_adam_multi(tl, h, ticket, st);
       else launch_adam_multi(static_cast<const AdamTensorList&>(tl), h, ticket, st);
     }
+  });
+  // NAdam (mu_products given) and RAdam (mu_products empty, momentum_decay unused): adam_multi's tables and checks; the step counts
+  // and mu_products take adam_multi's ticket word.
+  auto nadam_radam = [](bool nadam, std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avgs,
+                        std::vector<at::Tensor> exp_avg_sqs, std::vector<at::Tensor> steps, std::vector<at::Tensor> mu_products, double lr,
+                        c10::optional<at::Tensor> lr_tensor, double beta1, double beta2, double eps, double weight_decay, bool decoupled,
+                        bool maximize, double momentum_decay) {
+    const size_t n = params.size();
+    const char* who = nadam ? "nadam_multi" : "radam_multi";
+    TORCH_CHECK(grads.size() == n && exp_avgs.size() == n && exp_avg_sqs.size() == n && steps.size() == n &&
+                    mu_products.size() == (nadam ? n : 0), who, ": list lengths differ");
+    if (n == 0) return;
+    c10::cuda::CUDAGuard g(params[0].device());
+    NadamHyper h;
+    static_cast<AdamHyper&>(h) = adam_hyper(lr, lr_tensor, beta1, beta2, eps, weight_decay, decoupled, maximize);
+    h.momentum_decay = momentum_decay;
+    cudaStream_t st = cur_stream(params[0]);
+    unsigned int* ticket = scratch(params[0]).counter + kAdamTicketWord;
+    for (size_t base = 0; base < n; base += AdamTensorList::kMax) {
+      NadamTensorList tl;
+      tl.count = static_cast<int>(std::min<size_t>(AdamTensorList::kMax, n - base));
+      for (int i = 0; i < tl.count; ++i) {
+        const size_t j = base + i;
+        chk(params[j], "param"); chk(grads[j], "grad"); chk(exp_avgs[j], "exp_avg"); chk(exp_avg_sqs[j], "exp_avg_sq"); chk(steps[j], "step");
+        const int64_t numel = params[j].numel();
+        TORCH_CHECK(grads[j].numel() == numel && exp_avgs[j].numel() == numel && exp_avg_sqs[j].numel() == numel && steps[j].numel() == 1 &&
+                        numel < (int64_t(1) << 31), who, ": bad tensor sizes");
+        TORCH_CHECK(params[j].device() == params[0].device() && steps[j].device() == params[0].device(), who, ": all tensors on one device");
+        tl.p[i] = params[j].data_ptr<float>();
+        tl.g[i] = grads[j].data_ptr<float>();
+        tl.m[i] = exp_avgs[j].data_ptr<float>();
+        tl.v[i] = exp_avg_sqs[j].data_ptr<float>();
+        tl.step[i] = steps[j].data_ptr<float>();
+        tl.n[i] = static_cast<int>(numel);
+        if (nadam) {
+          chk(mu_products[j], "mu_product");
+          TORCH_CHECK(mu_products[j].numel() == 1, who, ": bad tensor sizes");
+          TORCH_CHECK(mu_products[j].device() == params[0].device(), who, ": all tensors on one device");
+          tl.mu_product[i] = mu_products[j].data_ptr<float>();
+        }
+      }
+      if (nadam) launch_nadam_multi(tl, h, ticket, st);
+      else launch_radam_multi(static_cast<const AdamTensorList&>(tl), static_cast<const AdamHyper&>(h), ticket, st);
+    }
+  };
+  m.def("nadam_multi", [nadam_radam](std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avgs,
+                                     std::vector<at::Tensor> exp_avg_sqs, std::vector<at::Tensor> steps, std::vector<at::Tensor> mu_products,
+                                     double lr, c10::optional<at::Tensor> lr_tensor, double beta1, double beta2, double eps, double weight_decay,
+                                     bool decoupled, bool maximize, double momentum_decay) {
+    nadam_radam(true, params, grads, exp_avgs, exp_avg_sqs, steps, mu_products, lr, lr_tensor, beta1, beta2, eps, weight_decay,
+                decoupled, maximize, momentum_decay);
+  });
+  m.def("radam_multi", [nadam_radam](std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avgs,
+                                     std::vector<at::Tensor> exp_avg_sqs, std::vector<at::Tensor> steps, double lr,
+                                     c10::optional<at::Tensor> lr_tensor, double beta1, double beta2, double eps, double weight_decay,
+                                     bool decoupled, bool maximize) {
+    nadam_radam(false, params, grads, exp_avgs, exp_avg_sqs, steps, {}, lr, lr_tensor, beta1, beta2, eps, weight_decay, decoupled,
+                maximize, 0.0);
   });
   // RMSprop: momentum_buffers given exactly when momentum > 0, grad_avgs exactly when centered (empty lists otherwise).  The step
   // counts take adam_multi's ticket word: launches on one device are ordered by the compute stream.

@@ -17,7 +17,7 @@
 //                              MaxPool/ReLU/BN backward ──barrier── conv1 weight gradient (mma.sync) ──barrier── conv1 fold;
 //                              conv2's weight gradient is folded in the shadow of the first barrier, and — on one GPU — the
 //                              threads that write the folded gradients apply the optimizer update (SgdRider / AdamRider / AmsgradRider /
-//                              RmspropRider / AdagradRider)
+//                              NadamRider / RadamRider / RmspropRider / AdagradRider)
 //
 // All cross-CTA sums are "every CTA writes one partial row, barrier, every CTA folds the rows in the same fixed order",
 // so results are bit-reproducible and identical in every CTA.  The kernels are launched cooperatively (all CTAs
@@ -525,6 +525,113 @@ __device__ __forceinline__ void adam_apply(const R& r, int k, int i, float g, co
   *p = fmaf(-f[k], mv / (sqrtf(den) / f[10 + k] + r.h.eps), pv);
 }
 
+// NAdam's momentum schedule μ_t = β1·(1 − ½·0.96^(t·ψ)), in torch's order of operations (as nadam_multi_kernel forms it).
+__device__ __forceinline__ double nadam_mu(double beta1, double psi, double t) { return beta1 * (1.0 - 0.5 * pow(0.96, t * psi)); }
+
+// Per-launch factors of the NAdam rider, formed once per CTA before the first grid barrier from each parameter's step s and
+// mu_product Π (t = s + 1, in double as nadam_multi_kernel forms them): the gradient's step size lr·(1 − μ_t)/(1 − Π_t) [10],
+// exp_avg's lr·μ_{t+1}/(1 − Π_t·μ_{t+1}) [10], bc2 [10], the new mu_product Π_t = fp32(Π·fp32(μ_t)) [10] (stored after the last
+// grid barrier), then (kNadamLr) AdamW's decay 1 − lr·wd, 1 − β1, β2, 1 − β2.  Threads k, 10 + k and 20 + k share parameter k's
+// work (c_g and Π_t; c_m; bc2), so that no thread holds more than two pow results: with all of it in one thread
+// ClipRider<NadamRider> spills more than the Adam rider's clipping instantiation.
+constexpr int kNadamLr = 40, kNadamFactors = 44;
+__device__ __forceinline__ void nadam_factors(const NadamRider& r, float* f, int tid) {
+  const int k = tid % 10, part = tid / 10;
+  if (part < 3 && r.step[k]) {
+    const double lr = r.h.lr_dev ? static_cast<double>(__ldg(r.h.lr_dev)) : r.h.lr;
+    const double s = static_cast<double>(*r.step[k] + 1.f);
+    if (part == 2) {
+      f[20 + k] = static_cast<float>(1.0 - pow(r.h.beta2, s));
+    } else {
+      const double mu = nadam_mu(r.h.beta1, r.momentum_decay, s);
+      const float prod = *r.mu_product[k] * static_cast<float>(mu);
+      if (part == 0) {
+        f[k] = static_cast<float>(lr * (1.0 - mu) / (1.0 - static_cast<double>(prod)));
+        f[30 + k] = prod;
+      } else {
+        const double mu_next = nadam_mu(r.h.beta1, r.momentum_decay, s + 1.0);
+        f[10 + k] = static_cast<float>(lr * mu_next / (1.0 - static_cast<double>(prod) * mu_next));
+      }
+    }
+    if (tid == 0) {
+      f[kNadamLr] = static_cast<float>(1.0 - lr * r.h.weight_decay);
+      f[kNadamLr + 1] = static_cast<float>(1.0 - r.h.beta1);
+      f[kNadamLr + 2] = static_cast<float>(r.h.beta2);
+      f[kNadamLr + 3] = static_cast<float>(1.0 - r.h.beta2);
+    }
+  }
+}
+
+// One NAdam update (the arithmetic of nadam_multi_kernel, ops_simt.cu) of element i of parameter k with gradient g; f: the factors
+// of nadam_factors.  R: NadamRider, possibly in a ClipRider.
+template <class R>
+__device__ __forceinline__ void nadam_apply(const R& r, int k, int i, float g, const float* f) {
+  float gv = r.h.maximize ? -g : g;
+  float* p = r.p[k] + i;
+  float* m = r.m[k] + i;
+  float* v = r.v[k] + i;
+  float pv = *p;
+  if (r.h.weight_decay != 0.f) {
+    if (r.h.decoupled) pv *= f[kNadamLr];
+    else gv = fmaf(r.h.weight_decay, pv, gv);
+  }
+  const float mv = fmaf(f[kNadamLr + 1], gv - *m, *m);
+  const float vv = fmaf(f[kNadamLr + 3] * gv, gv, f[kNadamLr + 2] * *v);
+  *m = mv;
+  *v = vv;
+  // torch's two addcdiv terms over one division: a second inlined IEEE division makes ClipRider<NadamRider> spill more than the
+  // Adam rider's clipping instantiation
+  const float d = sqrtf(vv / f[20 + k]) + r.h.eps;
+  *p = pv - fmaf(f[k], gv, f[10 + k] * mv) / d;
+}
+
+// Per-launch factors of the RAdam rider, formed once per CTA before the first grid barrier in Adam's layout (kAdamLr): the step
+// size [10] — lr·rect·sqrt(bc2)/bc1 where ρ_t > 5, else lr/bc1 — and which of the two applies [10] (1 rectified, 0 not), from each
+// parameter's step in double as radam_multi_kernel decides it; then AdamW's decay 1 − lr·wd, 1 − β1, β2, 1 − β2.
+__device__ __forceinline__ void radam_factors(const RadamRider& r, float* f, int tid) {
+  if (tid < 10 && r.step[tid]) {
+    const double lr = r.h.lr_dev ? static_cast<double>(__ldg(r.h.lr_dev)) : r.h.lr;
+    const double s = static_cast<double>(*r.step[tid] + 1.f);
+    const double bc1 = 1.0 - pow(r.h.beta1, s), b2t = pow(r.h.beta2, s), bc2 = 1.0 - b2t;
+    const double rho_inf = 2.0 / (1.0 - r.h.beta2) - 1.0;
+    const double rho_t = rho_inf - 2.0 * s * b2t / bc2;
+    if (rho_t > 5.0) {
+      const double rect = sqrt((rho_t - 4.0) * (rho_t - 2.0) * rho_inf / ((rho_inf - 4.0) * (rho_inf - 2.0) * rho_t));
+      f[tid] = static_cast<float>(lr * rect * sqrt(bc2) / bc1);
+      f[10 + tid] = 1.f;
+    } else {
+      f[tid] = static_cast<float>(lr / bc1);
+      f[10 + tid] = 0.f;
+    }
+    if (tid == 0) {
+      f[kAdamLr] = static_cast<float>(1.0 - lr * r.h.weight_decay);
+      f[kAdamLr + 1] = static_cast<float>(1.0 - r.h.beta1);
+      f[kAdamLr + 2] = static_cast<float>(r.h.beta2);
+      f[kAdamLr + 3] = static_cast<float>(1.0 - r.h.beta2);
+    }
+  }
+}
+
+// One RAdam update (the arithmetic of radam_multi_kernel, ops_simt.cu) of element i of parameter k with gradient g; f: the factors
+// of radam_factors.  R: RadamRider, possibly in a ClipRider.
+template <class R>
+__device__ __forceinline__ void radam_apply(const R& r, int k, int i, float g, const float* f) {
+  float gv = r.h.maximize ? -g : g;
+  float* p = r.p[k] + i;
+  float* m = r.m[k] + i;
+  float* v = r.v[k] + i;
+  float pv = *p;
+  if (r.h.weight_decay != 0.f) {
+    if (r.h.decoupled) pv *= f[kAdamLr];
+    else gv = fmaf(r.h.weight_decay, pv, gv);
+  }
+  const float mv = fmaf(f[kAdamLr + 1], gv - *m, *m);
+  const float vv = fmaf(f[kAdamLr + 3] * gv, gv, f[kAdamLr + 2] * *v);
+  *m = mv;
+  *v = vv;
+  *p = fmaf(-f[k], f[10 + k] != 0.f ? mv / (sqrtf(vv) + r.h.eps) : mv, pv);
+}
+
 // One RMSprop update (the arithmetic of rmsprop_multi_kernel, ops_simt.cu) of element i of parameter k with gradient g.
 // R: RmspropRider, possibly in a ClipRider.
 template <class R>
@@ -586,10 +693,15 @@ __device__ __forceinline__ float clip_comb(const R& r, float a, float b) { retur
 template <class R>
 constexpr bool kClipRider =
     std::is_same_v<R, ClipRider<SgdRider>> || std::is_same_v<R, ClipRider<AdamRider>> || std::is_same_v<R, ClipRider<AmsgradRider>> ||
-    std::is_same_v<R, ClipRider<RmspropRider>> || std::is_same_v<R, ClipRider<AdagradRider>>;
+    std::is_same_v<R, ClipRider<RmspropRider>> || std::is_same_v<R, ClipRider<AdagradRider>> || std::is_same_v<R, ClipRider<NadamRider>> ||
+    std::is_same_v<R, ClipRider<RadamRider>>;
 template <class R>
 constexpr bool kAdamRider = std::is_same_v<R, AdamRider> || std::is_same_v<R, ClipRider<AdamRider>> || std::is_same_v<R, AmsgradRider> ||
                             std::is_same_v<R, ClipRider<AmsgradRider>>;
+template <class R>
+constexpr bool kNadamRider = std::is_same_v<R, NadamRider> || std::is_same_v<R, ClipRider<NadamRider>>;
+template <class R>
+constexpr bool kRadamRider = std::is_same_v<R, RadamRider> || std::is_same_v<R, ClipRider<RadamRider>>;
 template <class R>
 constexpr bool kRmspropRider = std::is_same_v<R, RmspropRider> || std::is_same_v<R, ClipRider<RmspropRider>>;
 template <class R>
@@ -597,11 +709,13 @@ constexpr bool kAdagradRider = std::is_same_v<R, AdagradRider> || std::is_same_v
 
 // Element i of parameter k's gradient is final with value g: a ClipRider adds it to this thread's share ca of the norm (the update
 // waits for the coefficient), the others apply their update.  The caller tests whether the rider is on and the parameter takes part.
-// adam_f: the per-launch factors of the Adam or Adagrad rider; sgd_lr: the learning rate of the SGD or RMSprop rider.
+// adam_f: the per-launch factors of the Adam, NAdam, RAdam or Adagrad rider; sgd_lr: the learning rate of the SGD or RMSprop rider.
 template <class Rider>
 __device__ __forceinline__ void ride(const Rider& sr, float& ca, int k, int i, float g, const float* adam_f, float sgd_lr) {
   if constexpr (kClipRider<Rider>) ca = clip_acc(sr, ca, g);
   else if constexpr (kAdamRider<Rider>) adam_apply(sr, k, i, g, adam_f);
+  else if constexpr (kNadamRider<Rider>) nadam_apply(sr, k, i, g, adam_f);
+  else if constexpr (kRadamRider<Rider>) radam_apply(sr, k, i, g, adam_f);
   else if constexpr (kRmspropRider<Rider>) rmsprop_apply(sr, k, i, g, sgd_lr);
   else if constexpr (kAdagradRider<Rider>) adagrad_apply(sr, k, i, g, adam_f);
   else sgd_apply(sr.p[k] + i, g, sr.m[k] ? sr.m[k] + i : nullptr, sr.h, sgd_lr);
@@ -619,14 +733,16 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
                       float* partials, float* partials_w, GridSync gs,
                       // conv2's weight gradient, folded from the per-image partials [B][400][32] and Σdy rows [B][32]
                       const float* __restrict__ wpart, const float* __restrict__ dysum2, float* dw2, float* db2, const __grid_constant__ Rider sr) {
-  constexpr bool kClip = kClipRider<Rider>, kAdam = kAdamRider<Rider>, kRmsprop = kRmspropRider<Rider>, kAdagrad = kAdagradRider<Rider>;
-  static_assert(kAdam || kRmsprop || kAdagrad || std::is_base_of_v<SgdRider, Rider>,
-                "convnet_l1_bwd_kernel: SgdRider, AdamRider, AmsgradRider, RmspropRider or AdagradRider, or one of them in a ClipRider");
+  constexpr bool kClip = kClipRider<Rider>, kAdam = kAdamRider<Rider>, kRmsprop = kRmspropRider<Rider>, kAdagrad = kAdagradRider<Rider>,
+                 kNadam = kNadamRider<Rider>, kRadam = kRadamRider<Rider>;
+  static_assert(kAdam || kNadam || kRadam || kRmsprop || kAdagrad || std::is_base_of_v<SgdRider, Rider>,
+                "convnet_l1_bwd_kernel: SgdRider, AdamRider, AmsgradRider, NadamRider, RadamRider, RmspropRider or AdagradRider, or one "
+                "of them in a ClipRider");
   extern __shared__ __align__(16) float dsm[];
   float* dys = dsm;                  // [784][16]
   float* fold = dsm + 784 * 16;      // [25 warps][16][32]
-  // Adam rider: the per-launch factors; Adagrad rider: the ten decayed learning rates
-  __shared__ float adam_f[kAdam ? kAdamFactors : kAdagrad ? 10 : 1];
+  // Adam, NAdam and RAdam riders: the per-launch factors; Adagrad rider: the ten decayed learning rates
+  __shared__ float adam_f[kAdam || kRadam ? kAdamFactors : kNadam ? kNadamFactors : kAdagrad ? 10 : 1];
   __shared__ float xs[32 * 32];
   __shared__ __align__(16) float ws[25 * 16];   // conv1's weights [tap][co] when y is recomputed
   __shared__ float red[kL1Warps * 32];
@@ -670,6 +786,10 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   }
   if constexpr (kAdam) {
     if (sr.on) adam_factors(sr, adam_f, tid);   // reads the step counts: before the first grid barrier
+  } else if constexpr (kNadam) {
+    if (sr.on) nadam_factors(sr, adam_f, tid);   // reads the step counts and mu_products
+  } else if constexpr (kRadam) {
+    if (sr.on) radam_factors(sr, adam_f, tid);
   } else if constexpr (kAdagrad) {
     if (sr.on) adagrad_factors(sr, adam_f, tid);
   }
@@ -985,17 +1105,22 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
         const float gv = __ldcg(gk + i) * coef;
         gk[i] = gv;
         if constexpr (kAdam) adam_apply(sr, k, i, gv, adam_f);
+        else if constexpr (kNadam) nadam_apply(sr, k, i, gv, adam_f);
+        else if constexpr (kRadam) radam_apply(sr, k, i, gv, adam_f);
         else if constexpr (kRmsprop) rmsprop_apply(sr, k, i, gv, sgd_lr);
         else if constexpr (kAdagrad) adagrad_apply(sr, k, i, gv, adam_f);
         else sgd_apply(sr.p[k] + i, gv, sr.m[k] ? sr.m[k] + i : nullptr, sr.h, sgd_lr);
       }
     }
   }
-  if constexpr (kAdam || kRmsprop || kAdagrad) {
-    // every CTA read the step counts before the first grid barrier and this is after the last one
+  if constexpr (kAdam || kNadam || kRadam || kRmsprop || kAdagrad) {
+    // every CTA read the step counts (and NAdam's mu_products) before the first grid barrier and this is after the last one
     if ((kClip || sr.on) && n == 0 && tid == 0)
       for (int k = 0; k < 10; ++k)
-        if (sr.step[k]) *sr.step[k] += 1.f;
+        if (sr.step[k]) {
+          *sr.step[k] += 1.f;
+          if constexpr (kNadam) *sr.mu_product[k] = adam_f[30 + k];
+        }
   }
   bar.finish(gs);
   trace(1, 6);
@@ -1980,6 +2105,10 @@ PDT_L1_BWD_WGRAD(RmspropRider)
 PDT_L1_BWD_WGRAD(ClipRider<RmspropRider>)
 PDT_L1_BWD_WGRAD(AdagradRider)
 PDT_L1_BWD_WGRAD(ClipRider<AdagradRider>)
+PDT_L1_BWD_WGRAD(NadamRider)
+PDT_L1_BWD_WGRAD(ClipRider<NadamRider>)
+PDT_L1_BWD_WGRAD(RadamRider)
+PDT_L1_BWD_WGRAD(ClipRider<RadamRider>)
 #undef PDT_L1_BWD_WGRAD
 
 void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const float* g1, const float* be1, float* y1, float* p1, float* saved1,

@@ -45,6 +45,15 @@ struct AdamRider {
 struct AmsgradRider : AdamRider {
   float* vmax[10] = {};        // max_exp_avg_sq
 };
+// The Adam rider's state with the NAdam update (the arithmetic of nadam_multi_kernel).  Every CTA reads the ten step counts and
+// mu_products before the kernel's first grid barrier; one thread writes step + 1 and the new mu_product after the last one.
+struct NadamRider : AdamRider {
+  float* mu_product[10] = {};  // fp32 scalars on the device
+  double momentum_decay = 0.0;
+};
+// The Adam rider's state with the RAdam update (the arithmetic of radam_multi_kernel): every CTA decides from the step counts it
+// reads before the first grid barrier which parameters take the rectified step.
+struct RadamRider : AdamRider {};
 // The same rider with the RMSprop update (the arithmetic of rmsprop_multi_kernel).  The step counts do not enter the update; one
 // thread writes step + 1 after the kernel's last grid barrier.
 struct RmspropRider {
@@ -88,8 +97,8 @@ struct ClipRider : Base {
 void launch_conv2_wgrad_partials(const float* dy2_pad, const float* x2_pad, int B, float* wpart, cudaStream_t st);
 // Layer-1 backward: dp [B,18,18,16] frame (interior read) → dgamma/dbeta [16], dw [16,1,5,5], db [16]; it also folds conv2's weight
 // gradient: the per-image partials wpart and Σdy rows dysum2 [B,32] → dw2 [32,16,5,5], db2 [32], in the shadow of the kernel's first
-// grid barrier.  partials: B·32, partials_w: B·512 floats.  Rider: SgdRider, AdamRider, AmsgradRider, RmspropRider or AdagradRider,
-// or one of them in a ClipRider.
+// grid barrier.  partials: B·32, partials_w: B·512 floats.  Rider: SgdRider, AdamRider, AmsgradRider, NadamRider, RadamRider,
+// RmspropRider or AdagradRider, or one of them in a ClipRider.
 // accumulate: gradient accumulation — every gradient written (dgamma, dbeta, dw, db, dw2, db2) becomes g_old + this batch's value, and
 // the rider updates with (and clips) the accumulated gradient.
 // y: conv1's output [B,28,28,16] (conv1 + bias) as launch_convnet_fwd wrote it, or nullptr: then each CTA recomputes it from x and

@@ -27,7 +27,7 @@ struct ReduceScratch {
 //   kGridEpochWord          epoch of the cooperative kernels' grid barrier (GridBar): only ever increases, never reset
 //   kGridArrivalWord        arrival count of that barrier
 //   kCeCounterWord          arrival counter of the whole-forward kernel's cross-entropy mean
-//   kAdamTicketWord         step hand-over ticket of adam_multi, rmsprop_multi and adagrad_multi
+//   kAdamTicketWord         step hand-over ticket of adam_multi, nadam_multi, radam_multi, rmsprop_multi and adagrad_multi
 //   kClipTicketWord         fold ticket of grad_norm_clip
 //   kAvgTicketWord          n_averaged hand-over ticket of avg_multi
 // Each fixed word sits in a 32-byte sector of its own.  A ticket word serves one launch set at a time: the sets that use it are
@@ -196,6 +196,27 @@ struct AmsgradTensorList : AdamTensorList {
   float* vmax[kMax];  // max_exp_avg_sq
 };
 void launch_adam_multi(const AmsgradTensorList& tl, AdamHyper h, unsigned int* ticket, cudaStream_t st);
+
+// NAdam with torch's single-tensor arithmetic (g' = ±g + wd·p, or AdamW's p *= 1 − lr·wd with decoupled): with t = step + 1,
+//   μ_t = β1·(1 − ½·0.96^(t·ψ)), μ_{t+1} likewise (double);  Π_t = fp32(Π·fp32(μ_t)) (torch's fp32 mu_product *= μ_t)
+//   m = lerp(m, g', 1 − β1);  v = β2·v + (1 − β2)·g'²;  d = sqrt(v / bc2) + eps
+//   p −= (c_g·g' + c_m·m) / d,  c_g = lr·(1 − μ_t)/(1 − Π_t),  c_m = lr·μ_{t+1}/(1 − Π_t·μ_{t+1})   (c_g, c_m in double, rounded
+//   to fp32; torch's two addcdiv terms over one division)
+// The launch leaves t and Π_t behind (adam_multi's ticket hand-over), so a replayed CUDA graph advances both.
+struct NadamTensorList : AdamTensorList {
+  float* mu_product[kMax];
+};
+struct NadamHyper : AdamHyper {
+  double momentum_decay;   // ψ
+};
+void launch_nadam_multi(const NadamTensorList& tl, NadamHyper h, unsigned int* ticket, cudaStream_t st);
+
+// RAdam with torch's single-tensor arithmetic (weight decay as in NAdam): with t = step + 1, bc1 = 1 − β1^t, bc2 = 1 − β2^t,
+// ρ∞ = 2/(1 − β2) − 1 and ρ_t = ρ∞ − 2t·β2^t / bc2 (double), m and v as in Adam, then
+//   ρ_t > 5:  p −= lr·rect·sqrt(bc2)/bc1 · m / (sqrt(v) + eps),  rect = sqrt((ρ_t − 4)(ρ_t − 2)ρ∞ / ((ρ∞ − 4)(ρ∞ − 2)ρ_t))
+//   else:     p −= lr/bc1 · m
+// The branch is taken per tensor on the device from its step count; the launch leaves t behind (adam_multi's ticket hand-over).
+void launch_radam_multi(const AdamTensorList& tl, AdamHyper h, unsigned int* ticket, cudaStream_t st);
 
 // RMSprop with torch's single-tensor arithmetic (g' = ±g + wd·p):
 //   sq = α·sq + (1 − α)·g'²;  centered: ga = lerp(ga, g', 1 − α), avg = sqrt(sq − ga²) + eps;  else avg = sqrt(sq) + eps

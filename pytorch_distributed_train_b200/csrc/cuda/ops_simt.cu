@@ -1178,6 +1178,116 @@ __global__ void __launch_bounds__(256) adagrad_multi_kernel(AdagradTensorList tl
 }
 static_assert(sizeof(AdagradTensorList) + sizeof(AdagradHyper) + sizeof(unsigned int*) <= 4096, "adagrad_multi_kernel: parameters too large");
 
+// NAdam's momentum schedule μ_t = β1·(1 − ½·0.96^(t·ψ)), in torch's order of operations.
+__device__ __forceinline__ double nadam_mu(double beta1, double psi, double t) { return beta1 * (1.0 - 0.5 * pow(0.96, t * psi)); }
+
+// =====================================================================================================
+// Multi-tensor NAdam: same layout as adam_multi_kernel.  Thread 0 of every block reads its tensor's step s and mu_product Π and
+// forms, with t = s + 1, the two step sizes and bc2 in double (ops_kernels.h).  Π_t = fp32(Π·fp32(μ_t)) is torch's in-place product
+// on its fp32 state.  The block that takes the last ticket writes t and Π_t back for every tensor, one tensor per thread, and
+// resets the ticket word.
+// =====================================================================================================
+__global__ void __launch_bounds__(256) nadam_multi_kernel(NadamTensorList tl, NadamHyper h, unsigned int* ticket) {
+  const int t = blockIdx.y;
+  __shared__ float s_f[4];
+  __shared__ int s_last;
+  if (threadIdx.x == 0) {
+    const double lr = h.lr_dev ? static_cast<double>(*h.lr_dev) : h.lr;
+    const double s = static_cast<double>(*tl.step[t] + 1.f);
+    const double mu = nadam_mu(h.beta1, h.momentum_decay, s), mu_next = nadam_mu(h.beta1, h.momentum_decay, s + 1.0);
+    const double prod = static_cast<double>(*tl.mu_product[t] * static_cast<float>(mu));
+    s_f[0] = static_cast<float>(lr * (1.0 - mu) / (1.0 - prod));             // the gradient's step size
+    s_f[1] = static_cast<float>(lr * mu_next / (1.0 - prod * mu_next));      // exp_avg's step size
+    s_f[2] = static_cast<float>(1.0 - pow(h.beta2, s));                      // bc2
+    s_f[3] = static_cast<float>(1.0 - lr * h.weight_decay);                  // the decoupled decay factor
+    __threadfence();
+    s_last = atomicAdd(ticket, 1u) == gridDim.x * gridDim.y - 1;
+  }
+  __syncthreads();
+  if (s_last) {   // every block has read its step and mu_product
+    __threadfence();
+    for (int i = threadIdx.x; i < tl.count; i += blockDim.x) {
+      const float s = *tl.step[i] + 1.f;
+      *tl.mu_product[i] *= static_cast<float>(nadam_mu(h.beta1, h.momentum_decay, static_cast<double>(s)));
+      *tl.step[i] = s;
+    }
+    if (threadIdx.x == 0) atomicExch(ticket, 0u);
+  }
+  const int n = tl.n[t];
+  float* __restrict__ p = tl.p[t];
+  const float* __restrict__ g = tl.g[t];
+  float* __restrict__ m = tl.m[t];
+  float* __restrict__ v = tl.v[t];
+  const float c_g = s_f[0], c_m = s_f[1], bc2 = s_f[2], decay = s_f[3];
+  const float omb1 = static_cast<float>(1.0 - h.beta1), b2 = static_cast<float>(h.beta2), omb2 = static_cast<float>(1.0 - h.beta2);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float gv = h.maximize ? -g[i] : g[i];
+    float pv = p[i];
+    if (h.weight_decay != 0.f) {
+      if (h.decoupled) pv *= decay;
+      else gv = fmaf(h.weight_decay, pv, gv);
+    }
+    const float mv = fmaf(omb1, gv - m[i], m[i]);
+    const float vv = fmaf(omb2 * gv, gv, b2 * v[i]);
+    m[i] = mv;
+    v[i] = vv;
+    // torch's two addcdiv terms over one quotient, (c_g·g' + c_m·m) / d, as the rider forms it (fused_convnet.cu: nadam_apply)
+    const float d = sqrtf(vv / bc2) + h.eps;
+    p[i] = pv - fmaf(c_g, gv, c_m * mv) / d;
+  }
+}
+static_assert(sizeof(NadamTensorList) + sizeof(NadamHyper) + sizeof(unsigned int*) <= 4096, "nadam_multi_kernel: parameters too large");
+
+// =====================================================================================================
+// Multi-tensor RAdam: same layout as adam_multi_kernel.  Thread 0 of every block reads its tensor's step s and decides, with
+// t = s + 1 and ρ_t in double as torch forms it, whether this step is rectified (ρ_t > 5); the step size lr·rect·sqrt(bc2)/bc1 or
+// lr/bc1 goes to fp32.  The step hand-over is adam_multi_kernel's.
+// =====================================================================================================
+__global__ void __launch_bounds__(256) radam_multi_kernel(AdamTensorList tl, AdamHyper h, unsigned int* ticket) {
+  const int t = blockIdx.y;
+  __shared__ float s_f[3];
+  if (threadIdx.x == 0) {
+    const double lr = h.lr_dev ? static_cast<double>(*h.lr_dev) : h.lr;
+    const double s = static_cast<double>(*tl.step[t] + 1.f);
+    const double bc1 = 1.0 - pow(h.beta1, s), b2t = pow(h.beta2, s), bc2 = 1.0 - b2t;
+    const double rho_inf = 2.0 / (1.0 - h.beta2) - 1.0;
+    const double rho_t = rho_inf - 2.0 * s * b2t / bc2;
+    if (rho_t > 5.0) {
+      const double rect = sqrt((rho_t - 4.0) * (rho_t - 2.0) * rho_inf / ((rho_inf - 4.0) * (rho_inf - 2.0) * rho_t));
+      s_f[0] = static_cast<float>(lr * rect * sqrt(bc2) / bc1);
+      s_f[1] = 1.f;
+    } else {
+      s_f[0] = static_cast<float>(lr / bc1);
+      s_f[1] = 0.f;
+    }
+    s_f[2] = static_cast<float>(1.0 - lr * h.weight_decay);
+    advance_steps_last(tl, ticket);
+  }
+  __syncthreads();
+  const int n = tl.n[t];
+  float* __restrict__ p = tl.p[t];
+  const float* __restrict__ g = tl.g[t];
+  float* __restrict__ m = tl.m[t];
+  float* __restrict__ v = tl.v[t];
+  const float step_size = s_f[0], decay = s_f[2];
+  const bool rect = s_f[1] != 0.f;
+  const float omb1 = static_cast<float>(1.0 - h.beta1), b2 = static_cast<float>(h.beta2), omb2 = static_cast<float>(1.0 - h.beta2);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float gv = h.maximize ? -g[i] : g[i];
+    float pv = p[i];
+    if (h.weight_decay != 0.f) {
+      if (h.decoupled) pv *= decay;
+      else gv = fmaf(h.weight_decay, pv, gv);
+    }
+    const float mv = fmaf(omb1, gv - m[i], m[i]);
+    const float vv = fmaf(omb2 * gv, gv, b2 * v[i]);
+    m[i] = mv;
+    v[i] = vv;
+    p[i] = fmaf(-step_size, rect ? mv / (sqrtf(vv) + h.eps) : mv, pv);
+  }
+}
+static_assert(sizeof(AdamTensorList) + sizeof(AdamHyper) + sizeof(unsigned int*) <= 4096, "radam_multi_kernel: parameters too large");
+
 // =====================================================================================================
 // Gradient-norm clipping: same layout as sgd_multi_kernel.  grad_norm_multi_kernel: every block writes one partial (fp32 Σg² or
 // max |g| of the elements it strides over, reduced over the block in a fixed order); on the set's last table, the block that
@@ -1517,6 +1627,22 @@ void launch_adagrad_multi(const AdagradTensorList& tl, AdagradHyper h, unsigned 
   const int bx = std::max(1, std::min(64, (maxn + 1023) / 1024));
   adagrad_multi_kernel<<<dim3(bx, tl.count), 256, 0, st>>>(tl, h, ticket);
   check_launch("adagrad_multi");
+}
+void launch_nadam_multi(const NadamTensorList& tl, NadamHyper h, unsigned int* ticket, cudaStream_t st) {
+  if (tl.count == 0) return;
+  int maxn = 0;
+  for (int i = 0; i < tl.count; ++i) maxn = std::max(maxn, tl.n[i]);
+  const int bx = std::max(1, std::min(64, (maxn + 1023) / 1024));
+  nadam_multi_kernel<<<dim3(bx, tl.count), 256, 0, st>>>(tl, h, ticket);
+  check_launch("nadam_multi");
+}
+void launch_radam_multi(const AdamTensorList& tl, AdamHyper h, unsigned int* ticket, cudaStream_t st) {
+  if (tl.count == 0) return;
+  int maxn = 0;
+  for (int i = 0; i < tl.count; ++i) maxn = std::max(maxn, tl.n[i]);
+  const int bx = std::max(1, std::min(64, (maxn + 1023) / 1024));
+  radam_multi_kernel<<<dim3(bx, tl.count), 256, 0, st>>>(tl, h, ticket);
+  check_launch("radam_multi");
 }
 
 int grad_multi_blocks_x(const GradTensorList& tl) {

@@ -637,6 +637,25 @@ def adagrad_step(params, grads, sums, steps, lr, lr_decay=0.0, eps=1e-10, weight
                      float(weight_decay), bool(maximize))
 
 
+def nadam_step(params, grads, exp_avgs, exp_avg_sqs, mu_products, steps, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0,
+               momentum_decay=4e-3, decoupled=False, maximize=False, lr_tensor=None) -> None:
+    """One NAdam update of every tensor (torch's single-tensor arithmetic), one kernel launch per 48 tensors.  ``steps`` and
+    ``mu_products`` are fp32 scalars on the device: the launch forms the momentum schedule of step + 1 from them and stores step + 1
+    and the advanced product, so a replayed graph advances both.  ``decoupled``: the weight decay scales the parameter
+    (``decoupled_weight_decay=True``) instead of adding to the gradient."""
+    _C.nadam_multi(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), list(steps), list(mu_products), float(lr), lr_tensor,
+                   float(beta1), float(beta2), float(eps), float(weight_decay), bool(decoupled), bool(maximize), float(momentum_decay))
+
+
+def radam_step(params, grads, exp_avgs, exp_avg_sqs, steps, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0, decoupled=False,
+               maximize=False, lr_tensor=None) -> None:
+    """One RAdam update of every tensor (torch's single-tensor arithmetic), one kernel launch per 48 tensors.  ``steps`` are the fp32
+    step counts on the device: the launch decides from step + 1 whether the update is rectified (ρ_t > 5) and stores it, so a
+    replayed graph crosses into the rectified update when torch's step would."""
+    _C.radam_multi(list(params), list(grads), list(exp_avgs), list(exp_avg_sqs), list(steps), float(lr), lr_tensor, float(beta1),
+                   float(beta2), float(eps), float(weight_decay), bool(decoupled), bool(maximize))
+
+
 def grad_norm_clip(grads, max_norm, norm_type=2.0, scale=True) -> torch.Tensor:
     """The total ``norm_type`` norm (2 or inf) of fp32 contiguous gradients on one device, and — with ``scale`` — every gradient
     multiplied by torch's clip coefficient ``min(max_norm / (norm + 1e-6), 1)``: two launches per 48 tensors, graph-capturable,

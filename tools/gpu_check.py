@@ -23,6 +23,7 @@ GROUPS = {
     "adam": ["tests/test_adam.py"],
     "amsgrad": ["tests/test_adam_amsgrad.py"],
     "rmsprop_adagrad": ["tests/test_rmsprop_adagrad.py"],
+    "nadam_radam": ["tests/test_nadam_radam.py"],
     "clip": ["tests/test_clip_grad.py"],
     "average": ["tests/test_averaged_model.py"],
     "accum": ["tests/test_grad_accumulation.py"],
