@@ -9,7 +9,7 @@ Extra flags cover what the reference hard-codes: ``--init-method`` (its LAN addr
 ``tcp://10.9.1.2:34567`` only works on the author's network, ref: ddp_example.py:110; we default
 to loopback with a free port), ``--data synthetic|mnist``, ``--model``, ``--comm fused|nccl``, ``--algo``,
 ``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw | nadam | radam | rmsprop |
-adagrad), ``--lr``, ``--momentum``, ``--amsgrad``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--mixup``,
+adagrad | adamax | adadelta | asgd | rprop), ``--lr``, ``--momentum``, ``--amsgrad``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--mixup``,
 ``--ema-decay``, ``--checkpoint`` / ``--resume``, ``--eval`` (test loss and accuracy after every epoch).
 """
 from __future__ import annotations
@@ -44,17 +44,19 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--data-root", default="./data", type=str)
     p.add_argument("--model", default="convnet", choices=["convnet", "resnet18"])
     p.add_argument("--batch-size", default=100, type=int, help="per-GPU batch size (reference: 100)")
-    p.add_argument("--optimizer", default="sgd", choices=["sgd", "adam", "adamw", "nadam", "radam", "rmsprop", "adagrad"],
-                   help="optimizer: SGD (the reference's), Adam, AdamW, NAdam, RAdam, RMSprop or Adagrad, each a native multi-tensor "
-                        "kernel with torch's defaults")
+    p.add_argument("--optimizer", default="sgd",
+                   choices=["sgd", "adam", "adamw", "nadam", "radam", "rmsprop", "adagrad", "adamax", "adadelta", "asgd", "rprop"],
+                   help="optimizer: SGD (the reference's), Adam, AdamW, NAdam, RAdam, RMSprop, Adagrad, Adamax, Adadelta, ASGD or Rprop, "
+                        "each a native multi-tensor kernel with torch's defaults")
     p.add_argument("--lr", default=1e-4, type=float, help="learning rate (reference: 1e-4)")
     p.add_argument("--momentum", default=None, type=float, help="SGD momentum (default 0; not accepted with the other optimizers)")
     p.add_argument("--amsgrad", default=False, action="store_true",
                    help="Adam / AdamW with AMSGrad: the running maximum of exp_avg_sq in the denominator (not accepted with the other "
                         "optimizers)")
     p.add_argument("--weight-decay", default=None, type=float,
-                   help="weight decay (default: 0 for SGD, Adam, NAdam, RAdam, RMSprop and Adagrad, 1e-2 for AdamW, torch's defaults; "
-                        "NAdam and RAdam take it as L2 decay added to the gradient)")
+                   help="weight decay (default: 0 for SGD, Adam, NAdam, RAdam, RMSprop, Adagrad, Adamax, Adadelta and ASGD, 1e-2 for "
+                        "AdamW, torch's defaults; NAdam, RAdam, Adamax, Adadelta and ASGD take it as L2 decay added to the gradient; not "
+                        "accepted with Rprop, which has none)")
     p.add_argument("--clip-grad-norm", default=None, type=float, metavar="MAX",
                    help="clip the global gradient norm (L2) to MAX before every optimizer step (default: off)")
     p.add_argument("--accumulation-steps", default=1, type=int, metavar="K",
@@ -96,6 +98,14 @@ def make_optimizer(args, params):
         return pdt.optim.NAdam(params, args.lr, **kw)
     if args.optimizer == "radam":
         return pdt.optim.RAdam(params, args.lr, **kw)
+    if args.optimizer == "adamax":
+        return pdt.optim.Adamax(params, args.lr, **kw)
+    if args.optimizer == "adadelta":
+        return pdt.optim.Adadelta(params, args.lr, **kw)
+    if args.optimizer == "asgd":
+        return pdt.optim.ASGD(params, args.lr, **kw)
+    if args.optimizer == "rprop":
+        return pdt.optim.Rprop(params, args.lr)
     cls = pdt.optim.Adam if args.optimizer == "adam" else pdt.optim.AdamW
     return cls(params, args.lr, amsgrad=getattr(args, "amsgrad", False), **kw)
 
@@ -103,10 +113,13 @@ def make_optimizer(args, params):
 def check_args(p: argparse.ArgumentParser, args) -> None:
     if args.optimizer != "sgd" and args.momentum is not None:
         why = {"rmsprop": "RMSprop's momentum is a library option (pdt.optim.RMSprop(..., momentum=...))",
-               "adagrad": "Adagrad has no momentum"}.get(args.optimizer, f"{args.optimizer} takes its moments from its betas")
+               "adagrad": "Adagrad has no momentum", "adadelta": "Adadelta has no momentum", "asgd": "ASGD has no momentum",
+               "rprop": "Rprop has no momentum"}.get(args.optimizer, f"{args.optimizer} takes its moments from its betas")
         p.error(f"--momentum applies to SGD only; {why}")
     if args.optimizer not in ("adam", "adamw") and getattr(args, "amsgrad", False):
         p.error("--amsgrad applies to Adam and AdamW only (--optimizer adam | adamw)")
+    if args.optimizer == "rprop" and args.weight_decay is not None:
+        p.error("--weight-decay does not apply to Rprop, which has no weight decay")
     if args.clip_grad_norm is not None and not args.clip_grad_norm > 0:
         p.error(f"--clip-grad-norm must be positive (got {args.clip_grad_norm})")
     if args.accumulation_steps < 1:

@@ -68,6 +68,22 @@ AdagradHyper adagrad_hyper(double lr, const c10::optional<at::Tensor>& lr_tensor
 using TensorList = std::vector<c10::optional<at::Tensor>>;
 TensorList tensors(const py::dict& d, const char* key) { return d[key].cast<TensorList>(); }
 
+// The hyper-parameters of adadelta_multi and of the Adadelta rider of convnet_l1_bwd_wgrad.
+AdadeltaHyper adadelta_hyper(double lr, const c10::optional<at::Tensor>& lr_tensor, double rho, double eps, double weight_decay, bool maximize) {
+  return AdadeltaHyper{static_cast<float>(lr), static_cast<float>(rho), static_cast<float>(1.0 - rho), static_cast<float>(eps),
+                       static_cast<float>(weight_decay), maximize ? 1 : 0, opt_ptr(lr_tensor, "lr_tensor")};
+}
+// The hyper-parameters of asgd_multi and of the ASGD rider of convnet_l1_bwd_wgrad.
+AsgdHyper asgd_hyper(double lr, const c10::optional<at::Tensor>& lr_tensor, double lambd, double alpha, double t0, double weight_decay,
+                     bool maximize) {
+  return AsgdHyper{lr, lambd, alpha, t0, static_cast<float>(weight_decay), maximize ? 1 : 0, opt_ptr(lr_tensor, "lr_tensor")};
+}
+// The hyper-parameters of rprop_multi and of the Rprop rider of convnet_l1_bwd_wgrad.
+RpropHyper rprop_hyper(double etaminus, double etaplus, double step_min, double step_max, bool maximize) {
+  return RpropHyper{static_cast<float>(etaminus), static_cast<float>(etaplus), static_cast<float>(step_min), static_cast<float>(step_max),
+                    maximize ? 1 : 0};
+}
+
 // The parameters of a rider description (dict: "params", the ten parameters in the order conv1.w, conv1.b, bn1.w, bn1.b, conv2.w,
 // conv2.b, fc.w, fc.b, bn2.w, bn2.b, entries may be None; "prev_grads", the gradients of the last four) into r; state(k, param)
 // fills the optimizer state of parameter k.
@@ -209,6 +225,70 @@ AdagradRider adagrad_rider(const py::dict& d) {
   });
   r.h = adagrad_hyper(d["lr"].cast<double>(), d["lr_tensor"].cast<c10::optional<at::Tensor>>(), d["lr_decay"].cast<double>(),
                       d["eps"].cast<double>(), d["weight_decay"].cast<double>(), d["maximize"].cast<bool>());
+  return r;
+}
+
+// {"kind": "adamax", the "adam" entries with "exp_inf" in place of "exp_avg_sq" ("decoupled" unused)}
+AdamaxRider adamax_rider(const py::dict& d) {
+  AdamaxRider r;
+  const TensorList ms = tensors(d, "exp_avg"), us = tensors(d, "exp_inf"), steps = tensors(d, "step");
+  TORCH_CHECK(ms.size() == 10 && us.size() == 10 && steps.size() == 10, "convnet_l1_bwd_wgrad: adamax lists have the wrong length");
+  fill_rider(r, d, "adamax", [&](int k, const at::Tensor& p) {
+    r.m[k] = rider_state(ms, k, p.numel(), "adamax", "exp_avg");
+    r.v[k] = rider_state(us, k, p.numel(), "adamax", "exp_inf");
+    r.step[k] = rider_state(steps, k, 1, "adamax", "step");
+  });
+  r.h = adam_hyper(d["lr"].cast<double>(), d["lr_tensor"].cast<c10::optional<at::Tensor>>(), d["beta1"].cast<double>(), d["beta2"].cast<double>(),
+                   d["eps"].cast<double>(), d["weight_decay"].cast<double>(), false, d["maximize"].cast<bool>());
+  return r;
+}
+
+// {"kind": "adadelta", "params", "prev_grads", "square_avg", "acc_delta", "step" (fp32 scalars on the device), "lr", "lr_tensor", "rho",
+// "eps", "weight_decay", "maximize"}
+AdadeltaRider adadelta_rider(const py::dict& d) {
+  AdadeltaRider r;
+  const TensorList sqs = tensors(d, "square_avg"), accs = tensors(d, "acc_delta"), steps = tensors(d, "step");
+  TORCH_CHECK(sqs.size() == 10 && accs.size() == 10 && steps.size() == 10, "convnet_l1_bwd_wgrad: adadelta lists have the wrong length");
+  fill_rider(r, d, "adadelta", [&](int k, const at::Tensor& p) {
+    r.sq[k] = rider_state(sqs, k, p.numel(), "adadelta", "square_avg");
+    r.acc[k] = rider_state(accs, k, p.numel(), "adadelta", "acc_delta");
+    r.step[k] = rider_state(steps, k, 1, "adadelta", "step");
+  });
+  r.h = adadelta_hyper(d["lr"].cast<double>(), d["lr_tensor"].cast<c10::optional<at::Tensor>>(), d["rho"].cast<double>(), d["eps"].cast<double>(),
+                       d["weight_decay"].cast<double>(), d["maximize"].cast<bool>());
+  return r;
+}
+
+// {"kind": "asgd", "params", "prev_grads", "ax", "step", "eta", "mu" (fp32 scalars on the device), "lr", "lr_tensor", "lambd", "alpha",
+// "t0", "weight_decay", "maximize"}
+AsgdRider asgd_rider(const py::dict& d) {
+  AsgdRider r;
+  const TensorList axs = tensors(d, "ax"), steps = tensors(d, "step"), etas = tensors(d, "eta"), mus = tensors(d, "mu");
+  TORCH_CHECK(axs.size() == 10 && steps.size() == 10 && etas.size() == 10 && mus.size() == 10, "convnet_l1_bwd_wgrad: asgd lists have the wrong length");
+  fill_rider(r, d, "asgd", [&](int k, const at::Tensor& p) {
+    r.ax[k] = rider_state(axs, k, p.numel(), "asgd", "ax");
+    r.step[k] = rider_state(steps, k, 1, "asgd", "step");
+    r.eta[k] = rider_state(etas, k, 1, "asgd", "eta");
+    r.mu[k] = rider_state(mus, k, 1, "asgd", "mu");
+  });
+  r.h = asgd_hyper(d["lr"].cast<double>(), d["lr_tensor"].cast<c10::optional<at::Tensor>>(), d["lambd"].cast<double>(), d["alpha"].cast<double>(),
+                   d["t0"].cast<double>(), d["weight_decay"].cast<double>(), d["maximize"].cast<bool>());
+  return r;
+}
+
+// {"kind": "rprop", "params", "prev_grads", "prev", "step_size", "step" (fp32 scalars on the device), "etaminus", "etaplus",
+// "step_size_min", "step_size_max", "maximize"}
+RpropRider rprop_rider(const py::dict& d) {
+  RpropRider r;
+  const TensorList prevs = tensors(d, "prev"), sizes = tensors(d, "step_size"), steps = tensors(d, "step");
+  TORCH_CHECK(prevs.size() == 10 && sizes.size() == 10 && steps.size() == 10, "convnet_l1_bwd_wgrad: rprop lists have the wrong length");
+  fill_rider(r, d, "rprop", [&](int k, const at::Tensor& p) {
+    r.prev[k] = rider_state(prevs, k, p.numel(), "rprop", "prev");
+    r.step_size[k] = rider_state(sizes, k, p.numel(), "rprop", "step_size");
+    r.step[k] = rider_state(steps, k, 1, "rprop", "step");
+  });
+  r.h = rprop_hyper(d["etaminus"].cast<double>(), d["etaplus"].cast<double>(), d["step_size_min"].cast<double>(), d["step_size_max"].cast<double>(),
+                    d["maximize"].cast<bool>());
   return r;
 }
 
@@ -605,9 +685,15 @@ void register_cuda_bindings(py::module_& m) {
     }
     const auto d = rider.cast<py::dict>();
     const auto kind = d["kind"].cast<std::string>();
-    TORCH_CHECK(kind == "sgd" || kind == "adam" || kind == "nadam" || kind == "radam" || kind == "rmsprop" || kind == "adagrad",
-                "convnet_l1_bwd_wgrad: rider kind must be 'sgd', 'adam', 'nadam', 'radam', 'rmsprop' or 'adagrad' (got '", kind, "')");
+    TORCH_CHECK(kind == "sgd" || kind == "adam" || kind == "nadam" || kind == "radam" || kind == "rmsprop" || kind == "adagrad" ||
+                    kind == "adamax" || kind == "adadelta" || kind == "asgd" || kind == "rprop",
+                "convnet_l1_bwd_wgrad: rider kind must be 'sgd', 'adam', 'nadam', 'radam', 'rmsprop', 'adagrad', 'adamax', 'adadelta', 'asgd' "
+                "or 'rprop' (got '", kind, "')");
     if (kind == "sgd") launch_rider(sgd_rider(d));
+    else if (kind == "adamax") launch_rider(adamax_rider(d));
+    else if (kind == "adadelta") launch_rider(adadelta_rider(d));
+    else if (kind == "asgd") launch_rider(asgd_rider(d));
+    else if (kind == "rprop") launch_rider(rprop_rider(d));
     else if (kind == "nadam") launch_rider(nadam_rider(d));
     else if (kind == "radam") launch_rider(radam_rider(d));
     else if (kind == "rmsprop") launch_rider(rmsprop_rider(d));
@@ -1112,6 +1198,129 @@ void register_cuda_bindings(py::module_& m) {
         tl.n[i] = static_cast<int>(numel);
       }
       launch_adagrad_multi(tl, h, ticket, st);
+    }
+  });
+  // Adamax: adam_multi's tables (exp_infs in place of exp_avg_sqs), checks and ticket word.
+  m.def("adamax_multi", [](std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> exp_avgs,
+                           std::vector<at::Tensor> exp_infs, std::vector<at::Tensor> steps, double lr, c10::optional<at::Tensor> lr_tensor,
+                           double beta1, double beta2, double eps, double weight_decay, bool maximize) {
+    const size_t n = params.size();
+    TORCH_CHECK(grads.size() == n && exp_avgs.size() == n && exp_infs.size() == n && steps.size() == n, "adamax_multi: list lengths differ");
+    if (n == 0) return;
+    c10::cuda::CUDAGuard g(params[0].device());
+    const AdamHyper h = adam_hyper(lr, lr_tensor, beta1, beta2, eps, weight_decay, false, maximize);
+    cudaStream_t st = cur_stream(params[0]);
+    unsigned int* ticket = scratch(params[0]).counter + kAdamTicketWord;
+    for (size_t base = 0; base < n; base += AdamTensorList::kMax) {
+      AdamTensorList tl;
+      tl.count = static_cast<int>(std::min<size_t>(AdamTensorList::kMax, n - base));
+      for (int i = 0; i < tl.count; ++i) {
+        const size_t j = base + i;
+        chk(params[j], "param"); chk(grads[j], "grad"); chk(exp_avgs[j], "exp_avg"); chk(exp_infs[j], "exp_inf"); chk(steps[j], "step");
+        const int64_t numel = params[j].numel();
+        TORCH_CHECK(grads[j].numel() == numel && exp_avgs[j].numel() == numel && exp_infs[j].numel() == numel && steps[j].numel() == 1 &&
+                        numel < (int64_t(1) << 31), "adamax_multi: bad tensor sizes");
+        TORCH_CHECK(params[j].device() == params[0].device() && steps[j].device() == params[0].device(), "adamax_multi: all tensors on one device");
+        tl.p[i] = params[j].data_ptr<float>();
+        tl.g[i] = grads[j].data_ptr<float>();
+        tl.m[i] = exp_avgs[j].data_ptr<float>();
+        tl.v[i] = exp_infs[j].data_ptr<float>();
+        tl.step[i] = steps[j].data_ptr<float>();
+        tl.n[i] = static_cast<int>(numel);
+      }
+      launch_adamax_multi(tl, h, ticket, st);
+    }
+  });
+  m.def("adadelta_multi", [](std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> square_avgs,
+                             std::vector<at::Tensor> acc_deltas, std::vector<at::Tensor> steps, double lr, c10::optional<at::Tensor> lr_tensor,
+                             double rho, double eps, double weight_decay, bool maximize) {
+    const size_t n = params.size();
+    TORCH_CHECK(grads.size() == n && square_avgs.size() == n && acc_deltas.size() == n && steps.size() == n, "adadelta_multi: list lengths differ");
+    if (n == 0) return;
+    c10::cuda::CUDAGuard g(params[0].device());
+    const AdadeltaHyper h = adadelta_hyper(lr, lr_tensor, rho, eps, weight_decay, maximize);
+    cudaStream_t st = cur_stream(params[0]);
+    unsigned int* ticket = scratch(params[0]).counter + kAdamTicketWord;
+    for (size_t base = 0; base < n; base += AdadeltaTensorList::kMax) {
+      AdadeltaTensorList tl;
+      tl.count = static_cast<int>(std::min<size_t>(AdadeltaTensorList::kMax, n - base));
+      for (int i = 0; i < tl.count; ++i) {
+        const size_t j = base + i;
+        chk(params[j], "param"); chk(grads[j], "grad"); chk(square_avgs[j], "square_avg"); chk(acc_deltas[j], "acc_delta"); chk(steps[j], "step");
+        const int64_t numel = params[j].numel();
+        TORCH_CHECK(grads[j].numel() == numel && square_avgs[j].numel() == numel && acc_deltas[j].numel() == numel && steps[j].numel() == 1 &&
+                        numel < (int64_t(1) << 31), "adadelta_multi: bad tensor sizes");
+        TORCH_CHECK(params[j].device() == params[0].device() && steps[j].device() == params[0].device(), "adadelta_multi: all tensors on one device");
+        tl.p[i] = params[j].data_ptr<float>();
+        tl.g[i] = grads[j].data_ptr<float>();
+        tl.sq[i] = square_avgs[j].data_ptr<float>();
+        tl.acc[i] = acc_deltas[j].data_ptr<float>();
+        tl.step[i] = steps[j].data_ptr<float>();
+        tl.n[i] = static_cast<int>(numel);
+      }
+      launch_adadelta_multi(tl, h, ticket, st);
+    }
+  });
+  m.def("asgd_multi", [](std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> axs, std::vector<at::Tensor> steps,
+                         std::vector<at::Tensor> etas, std::vector<at::Tensor> mus, double lr, c10::optional<at::Tensor> lr_tensor, double lambd,
+                         double alpha, double t0, double weight_decay, bool maximize) {
+    const size_t n = params.size();
+    TORCH_CHECK(grads.size() == n && axs.size() == n && steps.size() == n && etas.size() == n && mus.size() == n, "asgd_multi: list lengths differ");
+    if (n == 0) return;
+    c10::cuda::CUDAGuard g(params[0].device());
+    const AsgdHyper h = asgd_hyper(lr, lr_tensor, lambd, alpha, t0, weight_decay, maximize);
+    cudaStream_t st = cur_stream(params[0]);
+    unsigned int* ticket = scratch(params[0]).counter + kAdamTicketWord;
+    for (size_t base = 0; base < n; base += AsgdTensorList::kMax) {
+      AsgdTensorList tl;
+      tl.count = static_cast<int>(std::min<size_t>(AsgdTensorList::kMax, n - base));
+      for (int i = 0; i < tl.count; ++i) {
+        const size_t j = base + i;
+        chk(params[j], "param"); chk(grads[j], "grad"); chk(axs[j], "ax"); chk(steps[j], "step"); chk(etas[j], "eta"); chk(mus[j], "mu");
+        const int64_t numel = params[j].numel();
+        TORCH_CHECK(grads[j].numel() == numel && axs[j].numel() == numel && steps[j].numel() == 1 && etas[j].numel() == 1 && mus[j].numel() == 1 &&
+                        numel < (int64_t(1) << 31), "asgd_multi: bad tensor sizes");
+        TORCH_CHECK(params[j].device() == params[0].device() && steps[j].device() == params[0].device() && etas[j].device() == params[0].device() &&
+                        mus[j].device() == params[0].device(), "asgd_multi: all tensors on one device");
+        tl.p[i] = params[j].data_ptr<float>();
+        tl.g[i] = grads[j].data_ptr<float>();
+        tl.ax[i] = axs[j].data_ptr<float>();
+        tl.step[i] = steps[j].data_ptr<float>();
+        tl.eta[i] = etas[j].data_ptr<float>();
+        tl.mu[i] = mus[j].data_ptr<float>();
+        tl.n[i] = static_cast<int>(numel);
+      }
+      launch_asgd_multi(tl, h, ticket, st);
+    }
+  });
+  m.def("rprop_multi", [](std::vector<at::Tensor> params, std::vector<at::Tensor> grads, std::vector<at::Tensor> prevs,
+                          std::vector<at::Tensor> step_sizes, std::vector<at::Tensor> steps, double etaminus, double etaplus, double step_min,
+                          double step_max, bool maximize) {
+    const size_t n = params.size();
+    TORCH_CHECK(grads.size() == n && prevs.size() == n && step_sizes.size() == n && steps.size() == n, "rprop_multi: list lengths differ");
+    if (n == 0) return;
+    c10::cuda::CUDAGuard g(params[0].device());
+    const RpropHyper h = rprop_hyper(etaminus, etaplus, step_min, step_max, maximize);
+    cudaStream_t st = cur_stream(params[0]);
+    unsigned int* ticket = scratch(params[0]).counter + kAdamTicketWord;
+    for (size_t base = 0; base < n; base += RpropTensorList::kMax) {
+      RpropTensorList tl;
+      tl.count = static_cast<int>(std::min<size_t>(RpropTensorList::kMax, n - base));
+      for (int i = 0; i < tl.count; ++i) {
+        const size_t j = base + i;
+        chk(params[j], "param"); chk(grads[j], "grad"); chk(prevs[j], "prev"); chk(step_sizes[j], "step_size"); chk(steps[j], "step");
+        const int64_t numel = params[j].numel();
+        TORCH_CHECK(grads[j].numel() == numel && prevs[j].numel() == numel && step_sizes[j].numel() == numel && steps[j].numel() == 1 &&
+                        numel < (int64_t(1) << 31), "rprop_multi: bad tensor sizes");
+        TORCH_CHECK(params[j].device() == params[0].device() && steps[j].device() == params[0].device(), "rprop_multi: all tensors on one device");
+        tl.p[i] = params[j].data_ptr<float>();
+        tl.g[i] = grads[j].data_ptr<float>();
+        tl.prev[i] = prevs[j].data_ptr<float>();
+        tl.step_size[i] = step_sizes[j].data_ptr<float>();
+        tl.step[i] = steps[j].data_ptr<float>();
+        tl.n[i] = static_cast<int>(numel);
+      }
+      launch_rprop_multi(tl, h, ticket, st);
     }
   });
   // Gradient-norm clipping: returns the total norm (a 0-d view of a [2] buffer whose second element is the clip coefficient);

@@ -17,7 +17,7 @@
 //                              MaxPool/ReLU/BN backward ──barrier── conv1 weight gradient (mma.sync) ──barrier── conv1 fold;
 //                              conv2's weight gradient is folded in the shadow of the first barrier, and — on one GPU — the
 //                              threads that write the folded gradients apply the optimizer update (SgdRider / AdamRider / AmsgradRider /
-//                              NadamRider / RadamRider / RmspropRider / AdagradRider)
+//                              NadamRider / RadamRider / RmspropRider / AdagradRider / AdamaxRider / AdadeltaRider / AsgdRider / RpropRider)
 //
 // All cross-CTA sums are "every CTA writes one partial row, barrier, every CTA folds the rows in the same fixed order",
 // so results are bit-reproducible and identical in every CTA.  The kernels are launched cooperatively (all CTAs
@@ -39,6 +39,7 @@
 #include "fused_convnet.h"
 #include "grid_sync.cuh"
 #include "hopper_ptx.cuh"
+#include "optim_update.cuh"
 #include "wgrad_win.cuh"
 
 namespace pdt {
@@ -684,41 +685,124 @@ __device__ __forceinline__ void adagrad_apply(const R& r, int k, int i, float g,
   *p = fmaf(-f[k], gv / (sqrtf(s) + r.h.eps), pv);
 }
 
+// Per-launch factors of the Adamax rider, formed once per CTA before the first grid barrier in Adam's layout (kAdamLr): the
+// bias-corrected learning rate clr = lr / (1 − β1^t) [10] from each parameter's step in double, as adamax_multi_kernel forms it,
+// then 1 − β1 and β2 at kAdamLr + 1 and kAdamLr + 2.
+__device__ __forceinline__ void adamax_factors(const AdamaxRider& r, float* f, int tid) {
+  if (tid < 10 && r.step[tid]) {
+    const double lr = r.h.lr_dev ? static_cast<double>(__ldg(r.h.lr_dev)) : r.h.lr;
+    f[tid] = static_cast<float>(lr / (1.0 - pow(r.h.beta1, static_cast<double>(*r.step[tid] + 1.f))));
+    if (tid == 0) {
+      f[kAdamLr + 1] = static_cast<float>(1.0 - r.h.beta1);
+      f[kAdamLr + 2] = static_cast<float>(r.h.beta2);
+    }
+  }
+}
+// One Adamax update of element i of parameter k with gradient g; f: the factors of adamax_factors.  R: AdamaxRider, possibly in a
+// ClipRider.
+template <class R>
+__device__ __forceinline__ void adamax_apply(const R& r, int k, int i, float g, const float* f) {
+  adamax_update(r.p[k] + i, r.h.maximize ? -g : g, r.m[k] + i, r.v[k] + i, r.h.weight_decay, f[kAdamLr + 1], f[kAdamLr + 2], r.h.eps, f[k]);
+}
+
+// One Adadelta update of element i of parameter k with gradient g.  R: AdadeltaRider, possibly in a ClipRider.
+template <class R>
+__device__ __forceinline__ void adadelta_apply(const R& r, int k, int i, float g, float lr) {
+  adadelta_update(r.p[k] + i, r.h.maximize ? -g : g, r.sq[k] + i, r.acc[k] + i, r.h.weight_decay, r.h.rho, r.h.one_minus_rho, r.h.eps, lr);
+}
+
+// Per-launch factors of the ASGD rider, formed once per CTA before the first grid barrier from each parameter's eta, mu and step s,
+// as asgd_multi_kernel forms them: eta [10], fp32(1 − λ·eta) [10], mu [10], then the eta and mu of the count s + 1 [10] [10], which
+// one thread stores after the last grid barrier.
+constexpr int kAsgdFactors = 50;
+__device__ __forceinline__ void asgd_factors(const AsgdRider& r, float* f, int tid) {
+  if (tid < 10 && r.step[tid]) {
+    const float eta = *r.eta[tid];
+    f[tid] = eta;
+    f[10 + tid] = static_cast<float>(1.0 - r.h.lambd * static_cast<double>(eta));
+    f[20 + tid] = *r.mu[tid];
+    const double lr = r.h.lr_dev ? static_cast<double>(__ldg(r.h.lr_dev)) : r.h.lr;
+    const double t = static_cast<double>(*r.step[tid] + 1.f);
+    f[30 + tid] = asgd_eta(lr, r.h.lambd, r.h.alpha, t);
+    f[40 + tid] = asgd_mu(r.h.t0, t);
+  }
+}
+// One ASGD update of element i of parameter k with gradient g; f: the factors of asgd_factors.  R: AsgdRider, possibly in a ClipRider.
+template <class R>
+__device__ __forceinline__ void asgd_apply(const R& r, int k, int i, float g, const float* f) {
+  asgd_update(r.p[k] + i, r.h.maximize ? -g : g, r.ax[k] + i, r.h.weight_decay, f[k], f[10 + k], f[20 + k]);
+}
+
+// One Rprop update of element i of parameter k with gradient g.  R: RpropRider, possibly in a ClipRider.
+template <class R>
+__device__ __forceinline__ void rprop_apply(const R& r, int k, int i, float g) {
+  rprop_update(r.p[k] + i, r.h.maximize ? -g : g, r.prev[k] + i, r.step_size[k] + i, r.h.etaminus, r.h.etaplus, r.h.step_min, r.h.step_max);
+}
+
 // Gradient-norm clipping (ClipRider): one gradient element g into a thread's accumulator — Σg², or max |g| keeping a NaN.
 template <class R>
 __device__ __forceinline__ float clip_acc(const R& r, float acc, float g) { return r.norm_inf ? nan_max(fabsf(g), acc) : fmaf(g, g, acc); }
 template <class R>
 __device__ __forceinline__ float clip_comb(const R& r, float a, float b) { return r.norm_inf ? nan_max(a, b) : a + b; }
 
+// What the kernel knows of its rider: the optimizer's rider (Base: the one inside a ClipRider) and whether the gradients are clipped
+// first.  kRiderOf<R, X, …>: R's optimizer rider is one of X, ….
 template <class R>
-constexpr bool kClipRider =
-    std::is_same_v<R, ClipRider<SgdRider>> || std::is_same_v<R, ClipRider<AdamRider>> || std::is_same_v<R, ClipRider<AmsgradRider>> ||
-    std::is_same_v<R, ClipRider<RmspropRider>> || std::is_same_v<R, ClipRider<AdagradRider>> || std::is_same_v<R, ClipRider<NadamRider>> ||
-    std::is_same_v<R, ClipRider<RadamRider>>;
+struct RiderTraits {
+  using Base = R;
+  static constexpr bool clip = false;
+};
+template <class B>
+struct RiderTraits<ClipRider<B>> {
+  using Base = B;
+  static constexpr bool clip = true;
+};
+template <class R, class... Of>
+constexpr bool kRiderOf = (std::is_same_v<typename RiderTraits<R>::Base, Of> || ...);
+template <class R> constexpr bool kClipRider = RiderTraits<R>::clip;
+template <class R> constexpr bool kSgdRider = kRiderOf<R, SgdRider>;
+template <class R> constexpr bool kAdamRider = kRiderOf<R, AdamRider, AmsgradRider>;
+template <class R> constexpr bool kNadamRider = kRiderOf<R, NadamRider>;
+template <class R> constexpr bool kRadamRider = kRiderOf<R, RadamRider>;
+template <class R> constexpr bool kRmspropRider = kRiderOf<R, RmspropRider>;
+template <class R> constexpr bool kAdagradRider = kRiderOf<R, AdagradRider>;
+template <class R> constexpr bool kAdamaxRider = kRiderOf<R, AdamaxRider>;
+template <class R> constexpr bool kAdadeltaRider = kRiderOf<R, AdadeltaRider>;
+template <class R> constexpr bool kAsgdRider = kRiderOf<R, AsgdRider>;
+template <class R> constexpr bool kRpropRider = kRiderOf<R, RpropRider>;
 template <class R>
-constexpr bool kAdamRider = std::is_same_v<R, AdamRider> || std::is_same_v<R, ClipRider<AdamRider>> || std::is_same_v<R, AmsgradRider> ||
-                            std::is_same_v<R, ClipRider<AmsgradRider>>;
-template <class R>
-constexpr bool kNadamRider = std::is_same_v<R, NadamRider> || std::is_same_v<R, ClipRider<NadamRider>>;
-template <class R>
-constexpr bool kRadamRider = std::is_same_v<R, RadamRider> || std::is_same_v<R, ClipRider<RadamRider>>;
-template <class R>
-constexpr bool kRmspropRider = std::is_same_v<R, RmspropRider> || std::is_same_v<R, ClipRider<RmspropRider>>;
-template <class R>
-constexpr bool kAdagradRider = std::is_same_v<R, AdagradRider> || std::is_same_v<R, ClipRider<AdagradRider>>;
+constexpr bool kKnownRider = kSgdRider<R> || kAdamRider<R> || kNadamRider<R> || kRadamRider<R> || kRmspropRider<R> || kAdagradRider<R> ||
+                             kAdamaxRider<R> || kAdadeltaRider<R> || kAsgdRider<R> || kRpropRider<R>;
 
-// Element i of parameter k's gradient is final with value g: a ClipRider adds it to this thread's share ca of the norm (the update
-// waits for the coefficient), the others apply their update.  The caller tests whether the rider is on and the parameter takes part.
-// adam_f: the per-launch factors of the Adam, NAdam, RAdam or Adagrad rider; sgd_lr: the learning rate of the SGD or RMSprop rider.
+// The learning rate the SGD, RMSprop and Adadelta riders apply as it is (the device scalar when there is one); Rprop has none.
+template <class R>
+__device__ __forceinline__ float rider_lr(const R& sr) {
+  if constexpr (kRpropRider<R>) return 0.f;
+  else return sr.on ? (sr.h.lr_dev ? __ldg(sr.h.lr_dev) : static_cast<float>(sr.h.lr)) : 0.f;
+}
+
+// The update of element i of parameter k with its final gradient g.  adam_f: the per-launch factors of the riders that have them;
+// sgd_lr: rider_lr.
 template <class Rider>
-__device__ __forceinline__ void ride(const Rider& sr, float& ca, int k, int i, float g, const float* adam_f, float sgd_lr) {
-  if constexpr (kClipRider<Rider>) ca = clip_acc(sr, ca, g);
-  else if constexpr (kAdamRider<Rider>) adam_apply(sr, k, i, g, adam_f);
+__device__ __forceinline__ void rider_update(const Rider& sr, int k, int i, float g, const float* adam_f, float sgd_lr) {
+  if constexpr (kAdamRider<Rider>) adam_apply(sr, k, i, g, adam_f);
   else if constexpr (kNadamRider<Rider>) nadam_apply(sr, k, i, g, adam_f);
   else if constexpr (kRadamRider<Rider>) radam_apply(sr, k, i, g, adam_f);
   else if constexpr (kRmspropRider<Rider>) rmsprop_apply(sr, k, i, g, sgd_lr);
   else if constexpr (kAdagradRider<Rider>) adagrad_apply(sr, k, i, g, adam_f);
+  else if constexpr (kAdamaxRider<Rider>) adamax_apply(sr, k, i, g, adam_f);
+  else if constexpr (kAdadeltaRider<Rider>) adadelta_apply(sr, k, i, g, sgd_lr);
+  else if constexpr (kAsgdRider<Rider>) asgd_apply(sr, k, i, g, adam_f);
+  else if constexpr (kRpropRider<Rider>) rprop_apply(sr, k, i, g);
   else sgd_apply(sr.p[k] + i, g, sr.m[k] ? sr.m[k] + i : nullptr, sr.h, sgd_lr);
+}
+
+// Element i of parameter k's gradient is final with value g: a ClipRider adds it to this thread's share ca of the norm (the update
+// waits for the coefficient), the others apply their update.  The caller tests whether the rider is on and the parameter takes part.
+template <class Rider>
+__device__ __forceinline__ void ride(const Rider& sr, float& ca, int k, int i, float g, const float* adam_f, float sgd_lr) {
+  if constexpr (kClipRider<Rider>) ca = clip_acc(sr, ca, g);
+  else rider_update(sr, k, i, g, adam_f, sgd_lr);
 }
 
 // ACC (accumulate mode, gradient accumulation over micro-batches): every gradient this kernel writes — dgamma, dbeta, the conv1 fold
@@ -733,16 +817,16 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
                       float* partials, float* partials_w, GridSync gs,
                       // conv2's weight gradient, folded from the per-image partials [B][400][32] and Σdy rows [B][32]
                       const float* __restrict__ wpart, const float* __restrict__ dysum2, float* dw2, float* db2, const __grid_constant__ Rider sr) {
-  constexpr bool kClip = kClipRider<Rider>, kAdam = kAdamRider<Rider>, kRmsprop = kRmspropRider<Rider>, kAdagrad = kAdagradRider<Rider>,
-                 kNadam = kNadamRider<Rider>, kRadam = kRadamRider<Rider>;
-  static_assert(kAdam || kNadam || kRadam || kRmsprop || kAdagrad || std::is_base_of_v<SgdRider, Rider>,
-                "convnet_l1_bwd_kernel: SgdRider, AdamRider, AmsgradRider, NadamRider, RadamRider, RmspropRider or AdagradRider, or one "
-                "of them in a ClipRider");
+  constexpr bool kClip = kClipRider<Rider>, kAdam = kAdamRider<Rider>, kAdagrad = kAdagradRider<Rider>, kNadam = kNadamRider<Rider>,
+                 kRadam = kRadamRider<Rider>, kAdamax = kAdamaxRider<Rider>, kAsgd = kAsgdRider<Rider>;
+  static_assert(kKnownRider<Rider>,
+                "convnet_l1_bwd_kernel: SgdRider, AdamRider, AmsgradRider, NadamRider, RadamRider, RmspropRider, AdagradRider, AdamaxRider, "
+                "AdadeltaRider, AsgdRider or RpropRider, or one of them in a ClipRider");
   extern __shared__ __align__(16) float dsm[];
   float* dys = dsm;                  // [784][16]
   float* fold = dsm + 784 * 16;      // [25 warps][16][32]
-  // Adam, NAdam and RAdam riders: the per-launch factors; Adagrad rider: the ten decayed learning rates
-  __shared__ float adam_f[kAdam || kRadam ? kAdamFactors : kNadam ? kNadamFactors : kAdagrad ? 10 : 1];
+  // Adam, NAdam, RAdam, Adamax and ASGD riders: the per-launch factors; Adagrad rider: the ten decayed learning rates
+  __shared__ float adam_f[kAdam || kRadam || kAdamax ? kAdamFactors : kNadam ? kNadamFactors : kAsgd ? kAsgdFactors : kAdagrad ? 10 : 1];
   __shared__ float xs[32 * 32];
   __shared__ __align__(16) float ws[25 * 16];   // conv1's weights [tap][co] when y is recomputed
   __shared__ float red[kL1Warps * 32];
@@ -792,6 +876,10 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
     if (sr.on) radam_factors(sr, adam_f, tid);
   } else if constexpr (kAdagrad) {
     if (sr.on) adagrad_factors(sr, adam_f, tid);
+  } else if constexpr (kAdamax) {
+    if (sr.on) adamax_factors(sr, adam_f, tid);
+  } else if constexpr (kAsgd) {
+    if (sr.on) asgd_factors(sr, adam_f, tid);   // reads the step counts, etas and mus
   }
   __syncthreads();
 
@@ -859,7 +947,7 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
   }
   trace(1, 1);
   bar.arrive(gs);
-  const float sgd_lr = sr.on ? (sr.h.lr_dev ? __ldg(sr.h.lr_dev) : static_cast<float>(sr.h.lr)) : 0.f;
+  const float sgd_lr = rider_lr(sr);
   float ca = 0.f;   // ClipRider: this thread's share of the gradient norm
   if (kClip || sr.on) {   // (a ClipRider is only made around a rider that is on)
     // in the barrier's shadow: the parameters whose gradients were complete before this kernel started (classifier, bn2, and
@@ -1104,22 +1192,22 @@ convnet_l1_bwd_kernel(const float* __restrict__ dp, const float* __restrict__ y,
       for (int i = n * kL1Threads + tid; i < nk; i += B * kL1Threads) {
         const float gv = __ldcg(gk + i) * coef;
         gk[i] = gv;
-        if constexpr (kAdam) adam_apply(sr, k, i, gv, adam_f);
-        else if constexpr (kNadam) nadam_apply(sr, k, i, gv, adam_f);
-        else if constexpr (kRadam) radam_apply(sr, k, i, gv, adam_f);
-        else if constexpr (kRmsprop) rmsprop_apply(sr, k, i, gv, sgd_lr);
-        else if constexpr (kAdagrad) adagrad_apply(sr, k, i, gv, adam_f);
-        else sgd_apply(sr.p[k] + i, gv, sr.m[k] ? sr.m[k] + i : nullptr, sr.h, sgd_lr);
+        rider_update(sr, k, i, gv, adam_f, sgd_lr);
       }
     }
   }
-  if constexpr (kAdam || kNadam || kRadam || kRmsprop || kAdagrad) {
-    // every CTA read the step counts (and NAdam's mu_products) before the first grid barrier and this is after the last one
+  if constexpr (!kSgdRider<Rider>) {
+    // every CTA read the step counts (and NAdam's mu_products, ASGD's etas and mus) before the first grid barrier and this is after
+    // the last one
     if ((kClip || sr.on) && n == 0 && tid == 0)
       for (int k = 0; k < 10; ++k)
         if (sr.step[k]) {
           *sr.step[k] += 1.f;
           if constexpr (kNadam) *sr.mu_product[k] = adam_f[30 + k];
+          if constexpr (kAsgd) {
+            *sr.eta[k] = adam_f[30 + k];
+            *sr.mu[k] = adam_f[40 + k];
+          }
         }
   }
   bar.finish(gs);
@@ -2109,6 +2197,14 @@ PDT_L1_BWD_WGRAD(NadamRider)
 PDT_L1_BWD_WGRAD(ClipRider<NadamRider>)
 PDT_L1_BWD_WGRAD(RadamRider)
 PDT_L1_BWD_WGRAD(ClipRider<RadamRider>)
+PDT_L1_BWD_WGRAD(AdamaxRider)
+PDT_L1_BWD_WGRAD(ClipRider<AdamaxRider>)
+PDT_L1_BWD_WGRAD(AdadeltaRider)
+PDT_L1_BWD_WGRAD(ClipRider<AdadeltaRider>)
+PDT_L1_BWD_WGRAD(AsgdRider)
+PDT_L1_BWD_WGRAD(ClipRider<AsgdRider>)
+PDT_L1_BWD_WGRAD(RpropRider)
+PDT_L1_BWD_WGRAD(ClipRider<RpropRider>)
 #undef PDT_L1_BWD_WGRAD
 
 void launch_convnet_fwd(const float* x, const float* w1, const float* b1, const float* g1, const float* be1, float* y1, float* p1, float* saved1,

@@ -78,6 +78,46 @@ struct AdagradRider {
   int n_prev[4] = {};
   AdagradHyper h{};
 };
+// The Adam rider's state with the Adamax update (optim_update.cuh: adamax_update), v holding exp_inf: every CTA forms the ten
+// bias-corrected learning rates from the step counts it reads before the first grid barrier; one thread writes step + 1 after the last.
+struct AdamaxRider : AdamRider {};
+// The rider with the Adadelta update (optim_update.cuh: adadelta_update).  The step counts do not enter the update; one thread
+// writes step + 1 after the kernel's last grid barrier.
+struct AdadeltaRider {
+  int on = 0;
+  float* p[10] = {};
+  float* sq[10] = {};          // square_avg
+  float* acc[10] = {};         // acc_delta
+  float* step[10] = {};        // fp32 step counts on the device
+  const float* g_prev[4] = {};
+  int n_prev[4] = {};
+  AdadeltaHyper h{};
+};
+// The rider with the ASGD update (optim_update.cuh: asgd_update).  Every CTA reads the ten step counts, etas and mus before the
+// kernel's first grid barrier; one thread writes step + 1 and the next eta and mu after the last one.
+struct AsgdRider {
+  int on = 0;
+  float* p[10] = {};
+  float* ax[10] = {};
+  float* step[10] = {};        // fp32 scalars on the device
+  float* eta[10] = {};
+  float* mu[10] = {};
+  const float* g_prev[4] = {};
+  int n_prev[4] = {};
+  AsgdHyper h{};
+};
+// The rider with the Rprop update (optim_update.cuh: rprop_update).  The step counts do not enter the update; one thread writes
+// step + 1 after the kernel's last grid barrier.
+struct RpropRider {
+  int on = 0;
+  float* p[10] = {};
+  float* prev[10] = {};
+  float* step_size[10] = {};
+  float* step[10] = {};        // fp32 step counts on the device
+  const float* g_prev[4] = {};
+  int n_prev[4] = {};
+  RpropHyper h{};
+};
 // Any of the riders with gradient-norm clipping in front of the update (torch.nn.utils.clip_grad_norm_, norm_type 2 or inf).  Every CTA
 // adds up the squares (or the max |g|) of the gradient elements it sees — those of parameters 6..9 in the shadow of the first
 // grid barrier, those of 0..5 as it folds them (4, 5 in that shadow too) — and writes one partial; after one more grid barrier every CTA folds the B
@@ -98,7 +138,7 @@ void launch_conv2_wgrad_partials(const float* dy2_pad, const float* x2_pad, int 
 // Layer-1 backward: dp [B,18,18,16] frame (interior read) → dgamma/dbeta [16], dw [16,1,5,5], db [16]; it also folds conv2's weight
 // gradient: the per-image partials wpart and Σdy rows dysum2 [B,32] → dw2 [32,16,5,5], db2 [32], in the shadow of the kernel's first
 // grid barrier.  partials: B·32, partials_w: B·512 floats.  Rider: SgdRider, AdamRider, AmsgradRider, NadamRider, RadamRider,
-// RmspropRider or AdagradRider, or one of them in a ClipRider.
+// RmspropRider, AdagradRider, AdamaxRider, AdadeltaRider, AsgdRider or RpropRider, or one of them in a ClipRider.
 // accumulate: gradient accumulation — every gradient written (dgamma, dbeta, dw, db, dw2, db2) becomes g_old + this batch's value, and
 // the rider updates with (and clips) the accumulated gradient.
 // y: conv1's output [B,28,28,16] (conv1 + bias) as launch_convnet_fwd wrote it, or nullptr: then each CTA recomputes it from x and

@@ -27,7 +27,8 @@ struct ReduceScratch {
 //   kGridEpochWord          epoch of the cooperative kernels' grid barrier (GridBar): only ever increases, never reset
 //   kGridArrivalWord        arrival count of that barrier
 //   kCeCounterWord          arrival counter of the whole-forward kernel's cross-entropy mean
-//   kAdamTicketWord         step hand-over ticket of adam_multi, nadam_multi, radam_multi, rmsprop_multi and adagrad_multi
+//   kAdamTicketWord         step hand-over ticket of adam_multi, nadam_multi, radam_multi, rmsprop_multi, adagrad_multi, adamax_multi,
+//                           adadelta_multi, asgd_multi and rprop_multi
 //   kClipTicketWord         fold ticket of grad_norm_clip
 //   kAvgTicketWord          n_averaged hand-over ticket of avg_multi
 // Each fixed word sits in a 32-byte sector of its own.  A ticket word serves one launch set at a time: the sets that use it are
@@ -259,6 +260,70 @@ struct AdagradHyper {
   const float* lr_dev;   // optional device-resident learning rate (graph-capturable schedules)
 };
 void launch_adagrad_multi(const AdagradTensorList& tl, AdagradHyper h, unsigned int* ticket, cudaStream_t st);
+
+// Adamax with torch's single-tensor arithmetic (optim_update.cuh: adamax_update; AdamHyper's decoupled is unused): with t = step + 1,
+// clr = lr / (1 − β1^t) in double, rounded to fp32 once per tensor.  The tables are Adam's, v holding exp_inf; the launch leaves t
+// behind (adam_multi's ticket hand-over).
+void launch_adamax_multi(const AdamTensorList& tl, AdamHyper h, unsigned int* ticket, cudaStream_t st);
+
+// Adadelta with torch's single-tensor arithmetic (optim_update.cuh: adadelta_update).  `step` does not enter the arithmetic; it is
+// advanced with adam_multi's ticket hand-over.
+struct AdadeltaTensorList {
+  static constexpr int kMax = 48;
+  float* p[kMax];
+  const float* g[kMax];
+  float* sq[kMax];    // square_avg
+  float* acc[kMax];   // acc_delta
+  float* step[kMax];
+  int n[kMax];
+  int count;
+};
+struct AdadeltaHyper {
+  float lr, rho, one_minus_rho, eps, weight_decay;   // 1 − ρ formed in double, as torch's Python scalar is
+  int maximize;
+  const float* lr_dev;   // optional device-resident learning rate (graph-capturable schedules)
+};
+void launch_adadelta_multi(const AdadeltaTensorList& tl, AdadeltaHyper h, unsigned int* ticket, cudaStream_t st);
+
+// ASGD with torch's single-tensor, non-capturable arithmetic (optim_update.cuh: asgd_update), from each tensor's fp32 eta and mu on
+// the device.  The block that takes the last ticket stores, with t = step + 1, step = t, eta = fp32(lr / (1 + λ·lr·t)^α) and
+// mu = fp32(1 / max(1, t − t0)) (double, from the device lr when there is one), so a replayed graph follows torch's schedules.
+struct AsgdTensorList {
+  static constexpr int kMax = 48;
+  float* p[kMax];
+  const float* g[kMax];
+  float* ax[kMax];
+  float* step[kMax];
+  float* eta[kMax];
+  float* mu[kMax];
+  int n[kMax];
+  int count;
+};
+struct AsgdHyper {
+  double lr, lambd, alpha, t0;   // double, as torch's host-side eta and mu are
+  float weight_decay;
+  int maximize;
+  const float* lr_dev;   // optional device-resident learning rate (graph-capturable schedules)
+};
+void launch_asgd_multi(const AsgdTensorList& tl, AsgdHyper h, unsigned int* ticket, cudaStream_t st);
+
+// Rprop with torch's single-tensor arithmetic (optim_update.cuh: rprop_update); no learning rate (step_size starts at lr) and no
+// weight decay.  `step` is advanced with adam_multi's ticket hand-over.
+struct RpropTensorList {
+  static constexpr int kMax = 48;
+  float* p[kMax];
+  const float* g[kMax];
+  float* prev[kMax];
+  float* step_size[kMax];
+  float* step[kMax];
+  int n[kMax];
+  int count;
+};
+struct RpropHyper {
+  float etaminus, etaplus, step_min, step_max;
+  int maximize;
+};
+void launch_rprop_multi(const RpropTensorList& tl, RpropHyper h, unsigned int* ticket, cudaStream_t st);
 
 // Gradient-norm clipping (torch.nn.utils.clip_grad_norm_ with norm_type 2 or inf) as two launches per table set: the norm, then
 // the scale.  A set of more than kMax tensors is split into tables launched back to back; every block of every table writes one

@@ -15,6 +15,7 @@
 #include "cuda_utils.h"
 #include "grid_fold.cuh"
 #include "ops_kernels.h"
+#include "optim_update.cuh"
 
 namespace pdt {
 
@@ -1289,6 +1290,102 @@ __global__ void __launch_bounds__(256) radam_multi_kernel(AdamTensorList tl, Ada
 static_assert(sizeof(AdamTensorList) + sizeof(AdamHyper) + sizeof(unsigned int*) <= 4096, "radam_multi_kernel: parameters too large");
 
 // =====================================================================================================
+// Multi-tensor Adamax: same layout as adam_multi_kernel (v holds exp_inf).  Thread 0 of every block reads its tensor's step s and
+// forms clr = lr / (1 − β1^(s + 1)) in double; the step hand-over is adam_multi_kernel's.
+// =====================================================================================================
+__global__ void __launch_bounds__(256) adamax_multi_kernel(AdamTensorList tl, AdamHyper h, unsigned int* ticket) {
+  const int t = blockIdx.y;
+  __shared__ float s_clr;
+  if (threadIdx.x == 0) {
+    const double lr = h.lr_dev ? static_cast<double>(*h.lr_dev) : h.lr;
+    s_clr = static_cast<float>(lr / (1.0 - pow(h.beta1, static_cast<double>(*tl.step[t] + 1.f))));
+    advance_steps_last(tl, ticket);
+  }
+  __syncthreads();
+  const int n = tl.n[t];
+  float* __restrict__ p = tl.p[t];
+  const float* __restrict__ g = tl.g[t];
+  float* __restrict__ m = tl.m[t];
+  float* __restrict__ u = tl.v[t];
+  const float clr = s_clr;
+  const float omb1 = static_cast<float>(1.0 - h.beta1), b2 = static_cast<float>(h.beta2);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    adamax_update(p + i, h.maximize ? -g[i] : g[i], m + i, u + i, h.weight_decay, omb1, b2, h.eps, clr);
+}
+
+// =====================================================================================================
+// Multi-tensor Adadelta: same layout as rmsprop_multi_kernel (the step count does not enter the update).
+// =====================================================================================================
+__global__ void __launch_bounds__(256) adadelta_multi_kernel(AdadeltaTensorList tl, AdadeltaHyper h, unsigned int* ticket) {
+  const int t = blockIdx.y;
+  if (threadIdx.x == 0) advance_steps_last(tl, ticket);
+  const int n = tl.n[t];
+  float* __restrict__ p = tl.p[t];
+  const float* __restrict__ g = tl.g[t];
+  float* __restrict__ sq = tl.sq[t];
+  float* __restrict__ acc = tl.acc[t];
+  const float lr = h.lr_dev ? *h.lr_dev : h.lr;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    adadelta_update(p + i, h.maximize ? -g[i] : g[i], sq + i, acc + i, h.weight_decay, h.rho, h.one_minus_rho, h.eps, lr);
+}
+static_assert(sizeof(AdadeltaTensorList) + sizeof(AdadeltaHyper) + sizeof(unsigned int*) <= 4096, "adadelta_multi_kernel: parameters too large");
+
+// =====================================================================================================
+// Multi-tensor ASGD: same layout as adam_multi_kernel.  Thread 0 of every block reads its tensor's eta and mu and takes a ticket; the
+// block that takes the last one stores every tensor's step + 1 and the eta and mu of that count, one tensor per thread (no block
+// reads them after it has taken its ticket), and resets the ticket word.
+// =====================================================================================================
+__global__ void __launch_bounds__(256) asgd_multi_kernel(AsgdTensorList tl, AsgdHyper h, unsigned int* ticket) {
+  const int t = blockIdx.y;
+  __shared__ float s_f[3];
+  __shared__ int s_last;
+  if (threadIdx.x == 0) {
+    const float eta = *tl.eta[t];
+    s_f[0] = eta;
+    s_f[1] = static_cast<float>(1.0 - h.lambd * static_cast<double>(eta));   // torch's p.mul_(1 − λ·η)
+    s_f[2] = *tl.mu[t];
+    __threadfence();
+    s_last = atomicAdd(ticket, 1u) == gridDim.x * gridDim.y - 1;
+  }
+  __syncthreads();
+  if (s_last) {   // every block has read its eta and mu
+    __threadfence();
+    const double lr = h.lr_dev ? static_cast<double>(*h.lr_dev) : h.lr;
+    for (int i = threadIdx.x; i < tl.count; i += blockDim.x) {
+      const float s = *tl.step[i] + 1.f;
+      *tl.step[i] = s;
+      *tl.eta[i] = asgd_eta(lr, h.lambd, h.alpha, static_cast<double>(s));
+      *tl.mu[i] = asgd_mu(h.t0, static_cast<double>(s));
+    }
+    if (threadIdx.x == 0) atomicExch(ticket, 0u);
+  }
+  const int n = tl.n[t];
+  float* __restrict__ p = tl.p[t];
+  const float* __restrict__ g = tl.g[t];
+  float* __restrict__ ax = tl.ax[t];
+  const float eta = s_f[0], decay = s_f[1], mu = s_f[2];
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    asgd_update(p + i, h.maximize ? -g[i] : g[i], ax + i, h.weight_decay, eta, decay, mu);
+}
+static_assert(sizeof(AsgdTensorList) + sizeof(AsgdHyper) + sizeof(unsigned int*) <= 4096, "asgd_multi_kernel: parameters too large");
+
+// =====================================================================================================
+// Multi-tensor Rprop: same layout as rmsprop_multi_kernel (the step count does not enter the update).
+// =====================================================================================================
+__global__ void __launch_bounds__(256) rprop_multi_kernel(RpropTensorList tl, RpropHyper h, unsigned int* ticket) {
+  const int t = blockIdx.y;
+  if (threadIdx.x == 0) advance_steps_last(tl, ticket);
+  const int n = tl.n[t];
+  float* __restrict__ p = tl.p[t];
+  const float* __restrict__ g = tl.g[t];
+  float* __restrict__ prev = tl.prev[t];
+  float* __restrict__ ss = tl.step_size[t];
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    rprop_update(p + i, h.maximize ? -g[i] : g[i], prev + i, ss + i, h.etaminus, h.etaplus, h.step_min, h.step_max);
+}
+static_assert(sizeof(RpropTensorList) + sizeof(RpropHyper) + sizeof(unsigned int*) <= 4096, "rprop_multi_kernel: parameters too large");
+
+// =====================================================================================================
 // Gradient-norm clipping: same layout as sgd_multi_kernel.  grad_norm_multi_kernel: every block writes one partial (fp32 Σg² or
 // max |g| of the elements it strides over, reduced over the block in a fixed order); on the set's last table, the block that
 // takes the last ticket folds the partials of every table in index order in fp64 and stores the norm and torch's clip
@@ -1643,6 +1740,33 @@ void launch_radam_multi(const AdamTensorList& tl, AdamHyper h, unsigned int* tic
   const int bx = std::max(1, std::min(64, (maxn + 1023) / 1024));
   radam_multi_kernel<<<dim3(bx, tl.count), 256, 0, st>>>(tl, h, ticket);
   check_launch("radam_multi");
+}
+// blockIdx.x extent of an optimizer table's launch: one block per 1024 elements of the largest tensor, at most 64
+template <class TL>
+static int optim_blocks_x(const TL& tl) {
+  int maxn = 0;
+  for (int i = 0; i < tl.count; ++i) maxn = std::max(maxn, tl.n[i]);
+  return std::max(1, std::min(64, (maxn + 1023) / 1024));
+}
+void launch_adamax_multi(const AdamTensorList& tl, AdamHyper h, unsigned int* ticket, cudaStream_t st) {
+  if (tl.count == 0) return;
+  adamax_multi_kernel<<<dim3(optim_blocks_x(tl), tl.count), 256, 0, st>>>(tl, h, ticket);
+  check_launch("adamax_multi");
+}
+void launch_adadelta_multi(const AdadeltaTensorList& tl, AdadeltaHyper h, unsigned int* ticket, cudaStream_t st) {
+  if (tl.count == 0) return;
+  adadelta_multi_kernel<<<dim3(optim_blocks_x(tl), tl.count), 256, 0, st>>>(tl, h, ticket);
+  check_launch("adadelta_multi");
+}
+void launch_asgd_multi(const AsgdTensorList& tl, AsgdHyper h, unsigned int* ticket, cudaStream_t st) {
+  if (tl.count == 0) return;
+  asgd_multi_kernel<<<dim3(optim_blocks_x(tl), tl.count), 256, 0, st>>>(tl, h, ticket);
+  check_launch("asgd_multi");
+}
+void launch_rprop_multi(const RpropTensorList& tl, RpropHyper h, unsigned int* ticket, cudaStream_t st) {
+  if (tl.count == 0) return;
+  rprop_multi_kernel<<<dim3(optim_blocks_x(tl), tl.count), 256, 0, st>>>(tl, h, ticket);
+  check_launch("rprop_multi");
 }
 
 int grad_multi_blocks_x(const GradTensorList& tl) {

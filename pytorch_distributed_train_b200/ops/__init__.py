@@ -24,9 +24,9 @@ def require_native(what: str) -> None:
 
 
 if _HAS_NATIVE:
-    from .functional import (adagrad_step, adam_step, average_update, bn_apply, bn_backward_apply, bn_backward_reduce,  # noqa: F401
-                             bn_finalize, bn_local_stats, conv_bn_relu_pool, cross_entropy, grad_norm_clip, grad_scale, linear,
-                             nadam_step, radam_step, rmsprop_step, sgd_step)
+    from .functional import (adadelta_step, adagrad_step, adam_step, adamax_step, asgd_step, average_update, bn_apply,  # noqa: F401
+                             bn_backward_apply, bn_backward_reduce, bn_finalize, bn_local_stats, conv_bn_relu_pool, cross_entropy,
+                             grad_norm_clip, grad_scale, linear, nadam_step, radam_step, rmsprop_step, rprop_step, sgd_step)
 else:  # CPU-only build of the extension: keep the names importable, fail loudly on use
     def _missing(name):
         def f(*a, **k):
@@ -34,9 +34,9 @@ else:  # CPU-only build of the extension: keep the names importable, fail loudly
         f.__name__ = name
         return f
 
-    for _n in ("adagrad_step", "adam_step", "average_update", "bn_apply", "bn_backward_apply", "bn_backward_reduce", "bn_finalize",
-               "bn_local_stats", "conv_bn_relu_pool", "cross_entropy", "grad_norm_clip", "grad_scale", "linear", "nadam_step", "radam_step",
-               "rmsprop_step", "sgd_step"):
+    for _n in ("adadelta_step", "adagrad_step", "adam_step", "adamax_step", "asgd_step", "average_update", "bn_apply", "bn_backward_apply",
+               "bn_backward_reduce", "bn_finalize", "bn_local_stats", "conv_bn_relu_pool", "cross_entropy", "grad_norm_clip", "grad_scale",
+               "linear", "nadam_step", "radam_step", "rmsprop_step", "rprop_step", "sgd_step"):
         globals()[_n] = _missing(_n)
 
 # evaluation metrics: the native kernel where it applies, torch ops elsewhere (CPU, gloo, other dtypes), so importable in any build

@@ -656,6 +656,39 @@ def radam_step(params, grads, exp_avgs, exp_avg_sqs, steps, lr, beta1=0.9, beta2
                    float(beta2), float(eps), float(weight_decay), bool(decoupled), bool(maximize))
 
 
+def adamax_step(params, grads, exp_avgs, exp_infs, steps, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0, maximize=False,
+                lr_tensor=None) -> None:
+    """One Adamax update of every tensor (torch's single-tensor arithmetic), one kernel launch per 48 tensors.  ``steps`` are the fp32
+    step counts on the device: the launch forms the bias correction of step + 1 from them and stores step + 1."""
+    _C.adamax_multi(list(params), list(grads), list(exp_avgs), list(exp_infs), list(steps), float(lr), lr_tensor, float(beta1),
+                    float(beta2), float(eps), float(weight_decay), bool(maximize))
+
+
+def adadelta_step(params, grads, square_avgs, acc_deltas, steps, lr, rho=0.9, eps=1e-6, weight_decay=0.0, maximize=False,
+                  lr_tensor=None) -> None:
+    """One Adadelta update of every tensor (torch's single-tensor arithmetic), one kernel launch per 48 tensors; ``steps`` (fp32 on the
+    device) are advanced as torch advances them."""
+    _C.adadelta_multi(list(params), list(grads), list(square_avgs), list(acc_deltas), list(steps), float(lr), lr_tensor, float(rho),
+                      float(eps), float(weight_decay), bool(maximize))
+
+
+def asgd_step(params, grads, axs, steps, etas, mus, lr, lambd=1e-4, alpha=0.75, t0=1e6, weight_decay=0.0, maximize=False,
+              lr_tensor=None) -> None:
+    """One ASGD update of every tensor (torch's single-tensor, non-capturable arithmetic), one kernel launch per 48 tensors.
+    ``steps``, ``etas`` and ``mus`` are fp32 scalars on the device: the launch updates with eta and mu and stores step + 1 and the
+    eta and mu of that count (from ``lr``, or ``lr_tensor`` when given), so a replayed graph follows torch's schedules."""
+    _C.asgd_multi(list(params), list(grads), list(axs), list(steps), list(etas), list(mus), float(lr), lr_tensor, float(lambd),
+                  float(alpha), float(t0), float(weight_decay), bool(maximize))
+
+
+def rprop_step(params, grads, prevs, step_sizes, steps, etaminus=0.5, etaplus=1.2, step_size_min=1e-6, step_size_max=50.0,
+               maximize=False) -> None:
+    """One Rprop update of every tensor (torch's single-tensor arithmetic, bit for bit), one kernel launch per 48 tensors; ``steps``
+    (fp32 on the device) are advanced as torch advances them."""
+    _C.rprop_multi(list(params), list(grads), list(prevs), list(step_sizes), list(steps), float(etaminus), float(etaplus),
+                   float(step_size_min), float(step_size_max), bool(maximize))
+
+
 def grad_norm_clip(grads, max_norm, norm_type=2.0, scale=True) -> torch.Tensor:
     """The total ``norm_type`` norm (2 or inf) of fp32 contiguous gradients on one device, and — with ``scale`` — every gradient
     multiplied by torch's clip coefficient ``min(max_norm / (norm + 1e-6), 1)``: two launches per 48 tensors, graph-capturable,

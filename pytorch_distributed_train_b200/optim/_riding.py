@@ -1,6 +1,7 @@
-"""What the native optimizers (``SGD``, ``Adam``, ``AdamW``, ``NAdam``, ``RAdam``, ``RMSprop``, ``Adagrad``) share: the
-device-resident learning rate that a captured CUDA graph reads, the device-resident step counts (and NAdam's ``mu_product``) that
-its kernels advance, and the checks that decide whether the update may ride on the reference ConvNet's last backward kernel.
+"""What the native optimizers (``SGD``, ``Adam``, ``AdamW``, ``NAdam``, ``RAdam``, ``RMSprop``, ``Adagrad``, ``Adamax``, ``Adadelta``,
+``ASGD``, ``Rprop``) share: the device-resident learning rate that a captured CUDA graph reads, the device-resident step counts (and
+NAdam's ``mu_product``, ASGD's ``eta`` and ``mu``) that its kernels advance, and the checks that decide whether the update may ride on
+the reference ConvNet's last backward kernel.
 
 The learning rate lives in a device scalar per group when the group says ``capturable=True``, and for every group once
 ``engine.GraphedTrainStep`` has taken the optimizer: the captured kernels then read the scalar, and ``sync_lr()`` before each replay
@@ -84,13 +85,13 @@ class RidingOptimizer(torch.optim.Optimizer):
                 ent[1] = float(group["lr"])
 
     def _steps_to_param_device(self) -> None:
-        """Move every state's ``step`` (and NAdam's ``mu_product``) to its parameter's device as an fp32 scalar, after
-        ``load_state_dict``: torch keeps ``step`` on the CPU unless the saved group says ``capturable`` or ``fused``, casts
-        ``mu_product`` to the parameter's dtype, and the kernels that count steps read both where the parameter is, in fp32."""
+        """Move every state's ``step`` (and NAdam's ``mu_product``, ASGD's ``eta`` and ``mu``) to its parameter's device as an fp32
+        scalar, after ``load_state_dict``: torch keeps ``step`` on the CPU unless the saved group says ``capturable`` or ``fused``,
+        casts the other scalars to the parameter's dtype, and the kernels read them where the parameter is, in fp32."""
         for group in self.param_groups:
             for p in group["params"]:
                 st = self.state.get(p)
-                for key in ("step", "mu_product"):
+                for key in ("step", "mu_product", "eta", "mu"):
                     if st and key in st:
                         s = st[key]
                         s = s if isinstance(s, torch.Tensor) else torch.tensor(float(s))

@@ -24,6 +24,7 @@ GROUPS = {
     "amsgrad": ["tests/test_adam_amsgrad.py"],
     "rmsprop_adagrad": ["tests/test_rmsprop_adagrad.py"],
     "nadam_radam": ["tests/test_nadam_radam.py"],
+    "adamax_adadelta_asgd_rprop": ["tests/test_adamax_adadelta_asgd_rprop.py"],
     "clip": ["tests/test_clip_grad.py"],
     "average": ["tests/test_averaged_model.py"],
     "accum": ["tests/test_grad_accumulation.py"],

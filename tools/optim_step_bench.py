@@ -1,23 +1,27 @@
 #!/usr/bin/env python
-"""Device time of one graphed training step of the reference ConvNet (batch 100, one GPU) with seventeen optimizers:
+"""Device time of one graphed training step of the reference ConvNet (batch 100, one GPU) with twenty-nine optimizers:
 
   pdt SGD, pdt Adam, pdt AdamW               (native update; on one GPU it rides on the last backward kernel)
   pdt AdamW(amsgrad=True)                    (the same with the running maximum max_exp_avg_sq: AmsgradRider)
   pdt RMSprop, pdt RMSprop(momentum=0.9, centered=True), pdt Adagrad   (RmspropRider, AdagradRider)
   pdt NAdam, pdt RAdam                       (NadamRider, RadamRider)
   pdt NAdam, pdt RAdam, not riding           (GraphedTrainStep(fuse_optimizer=False): the multi-tensor kernel after backward)
+  pdt Adamax, Adadelta, ASGD, Rprop          (AdamaxRider, AdadeltaRider, AsgdRider, RpropRider)
+  pdt Adamax, Adadelta, ASGD, Rprop, not riding
   torch AdamW(capturable=True, foreach=True) (torch's multi-tensor kernels, replayed inside the same graph)
   torch AdamW(capturable=True, fused=True)   (torch's fused kernel, replayed inside the same graph)
   torch AdamW(amsgrad=True, capturable=True, fused=True)
   torch RMSprop(capturable=True, foreach=True)
   torch NAdam(capturable=True, foreach=True), torch RAdam(capturable=True, foreach=True)
+  torch Adamax / Adadelta / ASGD / Rprop(capturable=True, foreach=True)
 
 torch's Adagrad has no arm: it computes its decayed learning rate on the host from a CPU step count, so a captured step would
 replay the captured rate.
 
-With ``--max-grad-norm X`` six more arms clip the global gradient norm to X in the same rounds:
+With ``--max-grad-norm X`` ten more arms clip the global gradient norm to X in the same rounds:
 
-  pdt SGD / AdamW / NAdam / RAdam with clipping, riding   (the last backward kernel clips, then updates: still 3 launches)
+  pdt SGD / AdamW / NAdam / RAdam / Adamax / Adadelta / ASGD / Rprop with clipping, riding   (the last backward kernel clips, then
+                                                                                            updates: still 3 launches)
   pdt AdamW with clipping, not riding          (GraphedTrainStep(fuse_optimizer=False): native clip + Adam kernel after backward)
   torch clip_grad_norm_(foreach=True) + AdamW(capturable=True, fused=True) in the same graph
 
@@ -97,16 +101,28 @@ def main():
         "pdt_radam": lambda ps: pdt.optim.RAdam(ps, lr),
         "pdt_nadam_unfused": lambda ps: pdt.optim.NAdam(ps, lr),
         "pdt_radam_unfused": lambda ps: pdt.optim.RAdam(ps, lr),
+        "pdt_adamax": lambda ps: pdt.optim.Adamax(ps, lr),
+        "pdt_adadelta": lambda ps: pdt.optim.Adadelta(ps, lr),
+        "pdt_asgd": lambda ps: pdt.optim.ASGD(ps, lr),
+        "pdt_rprop": lambda ps: pdt.optim.Rprop(ps, lr),
+        "pdt_adamax_unfused": lambda ps: pdt.optim.Adamax(ps, lr),
+        "pdt_adadelta_unfused": lambda ps: pdt.optim.Adadelta(ps, lr),
+        "pdt_asgd_unfused": lambda ps: pdt.optim.ASGD(ps, lr),
+        "pdt_rprop_unfused": lambda ps: pdt.optim.Rprop(ps, lr),
         "torch_adamw_foreach": lambda ps: torch.optim.AdamW(ps, lr, capturable=True, foreach=True),
         "torch_adamw_fused": lambda ps: torch.optim.AdamW(ps, lr, capturable=True, fused=True),
         "torch_adamw_amsgrad_fused": lambda ps: torch.optim.AdamW(ps, lr, amsgrad=True, capturable=True, fused=True),
         "torch_rmsprop_foreach": lambda ps: torch.optim.RMSprop(ps, lr, capturable=True, foreach=True),
         "torch_nadam_foreach": lambda ps: torch.optim.NAdam(ps, lr, capturable=True, foreach=True),
         "torch_radam_foreach": lambda ps: torch.optim.RAdam(ps, lr, capturable=True, foreach=True),
+        "torch_adamax_foreach": lambda ps: torch.optim.Adamax(ps, lr, capturable=True, foreach=True),
+        "torch_adadelta_foreach": lambda ps: torch.optim.Adadelta(ps, lr, capturable=True, foreach=True),
+        "torch_asgd_foreach": lambda ps: torch.optim.ASGD(ps, lr, capturable=True, foreach=True),
+        "torch_rprop_foreach": lambda ps: torch.optim.Rprop(ps, lr, capturable=True, foreach=True),
     }
     # name -> GraphedTrainStep keyword arguments of the arm
     kwargs = {name: {} for name in makers}
-    kwargs.update({"pdt_nadam_unfused": {"fuse_optimizer": False}, "pdt_radam_unfused": {"fuse_optimizer": False}})
+    kwargs.update({name: {"fuse_optimizer": False} for name in makers if name.endswith("_unfused")})
     if args.max_grad_norm is not None:
         mg = args.max_grad_norm
         makers.update({
@@ -114,11 +130,17 @@ def main():
             "pdt_adamw_clip": lambda ps: pdt.optim.AdamW(ps, lr),
             "pdt_nadam_clip": lambda ps: pdt.optim.NAdam(ps, lr),
             "pdt_radam_clip": lambda ps: pdt.optim.RAdam(ps, lr),
+            "pdt_adamax_clip": lambda ps: pdt.optim.Adamax(ps, lr),
+            "pdt_adadelta_clip": lambda ps: pdt.optim.Adadelta(ps, lr),
+            "pdt_asgd_clip": lambda ps: pdt.optim.ASGD(ps, lr),
+            "pdt_rprop_clip": lambda ps: pdt.optim.Rprop(ps, lr),
             "pdt_adamw_clip_unfused": lambda ps: pdt.optim.AdamW(ps, lr),
             "torch_clip_adamw_fused": lambda ps: _TorchClip(torch.optim.AdamW(ps, lr, capturable=True, fused=True), ps, mg),
         })
         kwargs.update({"pdt_sgd_clip": {"max_grad_norm": mg}, "pdt_adamw_clip": {"max_grad_norm": mg},
                        "pdt_nadam_clip": {"max_grad_norm": mg}, "pdt_radam_clip": {"max_grad_norm": mg},
+                       "pdt_adamax_clip": {"max_grad_norm": mg}, "pdt_adadelta_clip": {"max_grad_norm": mg},
+                       "pdt_asgd_clip": {"max_grad_norm": mg}, "pdt_rprop_clip": {"max_grad_norm": mg},
                        "pdt_adamw_clip_unfused": {"max_grad_norm": mg, "fuse_optimizer": False}, "torch_clip_adamw_fused": {}})
     crit = pdt.nn.CrossEntropyLoss()
     steps = {}
