@@ -10,7 +10,7 @@ Extra flags cover what the reference hard-codes: ``--init-method`` (its LAN addr
 to loopback with a free port), ``--data synthetic|mnist``, ``--model``, ``--comm fused|nccl``, ``--algo``,
 ``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw | nadam | radam | rmsprop |
 adagrad | adamax | adadelta | asgd | rprop), ``--lr``, ``--momentum``, ``--amsgrad``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--mixup``,
-``--ema-decay``, ``--checkpoint`` / ``--resume``, ``--eval`` (test loss and accuracy after every epoch).
+``--rotate`` / ``--translate`` / ``--scale-range`` / ``--shear`` / ``--affine-interpolation`` (per-image random affine augmentation), ``--ema-decay``, ``--checkpoint`` / ``--resume``, ``--eval`` (test loss and accuracy after every epoch).
 """
 from __future__ import annotations
 
@@ -67,6 +67,17 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--mixup", default=None, type=float, metavar="ALPHA",
                    help="MixUp every training batch with lambda ~ Beta(ALPHA, ALPHA), ALPHA > 0, and train on the mixed class "
                         "probabilities (default: off)")
+    p.add_argument("--rotate", default=None, type=float, metavar="DEG",
+                   help="random affine augmentation: rotate every training image by an angle ~ U[-DEG, DEG) (default: off)")
+    p.add_argument("--translate", default=None, type=float, metavar="FRAC",
+                   help="random affine augmentation: shift every training image by up to FRAC of its width and height, FRAC in [0, 1] "
+                        "(default: off)")
+    p.add_argument("--scale-range", default=None, type=float, nargs=2, metavar=("LO", "HI"),
+                   help="random affine augmentation: scale every training image by a factor ~ U[LO, HI), 0 < LO <= HI (default: off)")
+    p.add_argument("--shear", default=None, type=float, metavar="DEG",
+                   help="random affine augmentation: shear every training image along x by an angle ~ U[-DEG, DEG) (default: off)")
+    p.add_argument("--affine-interpolation", default="nearest", choices=["nearest", "bilinear"],
+                   help="resampling of the random affine augmentation (default: nearest, torchvision's)")
     p.add_argument("--ema-decay", default=None, type=float, metavar="D",
                    help="keep an exponential moving average of the weights and buffers with decay D in [0, 1], updated after every "
                         "optimizer step and saved with --checkpoint (default: off)")
@@ -110,6 +121,23 @@ def make_optimizer(args, params):
     return cls(params, args.lr, amsgrad=getattr(args, "amsgrad", False), **kw)
 
 
+def affine_requested(args) -> bool:
+    return any(getattr(args, k, None) is not None for k in ("rotate", "translate", "scale_range", "shear"))
+
+
+def make_augment(args, generator):
+    """The per-image random affine augmentation ``--rotate`` / ``--translate`` / ``--scale-range`` / ``--shear`` describe, or None."""
+    if not affine_requested(args):
+        return None
+    from pytorch_distributed_train_b200 import data as pdata
+
+    return pdata.RandomAffine(degrees=(-args.rotate, args.rotate) if args.rotate is not None else 0,
+                              translate=None if args.translate is None else (args.translate, args.translate),
+                              scale=None if args.scale_range is None else tuple(args.scale_range),
+                              shear=None if args.shear is None else (-args.shear, args.shear),
+                              interpolation=args.affine_interpolation, generator=generator)
+
+
 def check_args(p: argparse.ArgumentParser, args) -> None:
     if args.optimizer != "sgd" and args.momentum is not None:
         why = {"rmsprop": "RMSprop's momentum is a library option (pdt.optim.RMSprop(..., momentum=...))",
@@ -128,6 +156,17 @@ def check_args(p: argparse.ArgumentParser, args) -> None:
         p.error(f"--label-smoothing must lie in [0, 1] (got {args.label_smoothing})")
     if args.mixup is not None and not args.mixup > 0:
         p.error(f"--mixup must be positive (got {args.mixup})")
+    if args.rotate is not None and not args.rotate >= 0:
+        p.error(f"--rotate must be non-negative (got {args.rotate})")
+    if args.translate is not None and not 0.0 <= args.translate <= 1.0:
+        p.error(f"--translate must lie in [0, 1] (got {args.translate})")
+    if args.scale_range is not None and not 0 < args.scale_range[0] <= args.scale_range[1]:
+        p.error(f"--scale-range needs 0 < LO <= HI (got {args.scale_range[0]} {args.scale_range[1]})")
+    if args.shear is not None and not args.shear >= 0:
+        p.error(f"--shear must be non-negative (got {args.shear})")
+    if args.mixup is not None and affine_requested(args):
+        p.error("--mixup cannot be combined with --rotate, --translate, --scale-range or --shear: MixUp mixes on the host before the "
+                "batch reaches the device, where the affine would warp the mixed image with one parameter set")
     if args.ema_decay is not None and not 0.0 <= args.ema_decay <= 1.0:
         p.error(f"--ema-decay must lie in [0, 1] (got {args.ema_decay})")
     if args.graph and args.gpus >= 2 and args.accumulation_steps > 1:
@@ -201,6 +240,10 @@ def dist_train(gpu: int, args) -> None:
         # epoch below)
         mix_gen = torch.Generator()
 
+    # every training image warped with its own parameters, on the batch's device after its copy (inside the captured step with
+    # --graph); each rank draws from its own generator, seeded per epoch below
+    augment = make_augment(args, torch.Generator(device=device))
+
     step_fn = None
     if args.graph and use_cuda:
         from pytorch_distributed_train_b200.engine import GraphedTrainStep
@@ -209,7 +252,7 @@ def dist_train(gpu: int, args) -> None:
         example_targets = (torch.zeros(rows, dtype=torch.int64, device=device) if mix_gen is None else
                            torch.zeros(rows, num_classes, device=device))
         step_fn = GraphedTrainStep(model, criterion, optimizer, example_inputs=(torch.zeros((rows,) + shape, device=device), example_targets),
-                                   max_grad_norm=args.clip_grad_norm, accumulation_steps=accum, averaged_model=ema)
+                                   max_grad_norm=args.clip_grad_norm, accumulation_steps=accum, averaged_model=ema, augment=augment)
 
     first_epoch = 0
     if args.resume:
@@ -226,6 +269,8 @@ def dist_train(gpu: int, args) -> None:
         if mix_gen is not None:
             # from (epoch, rank): a run resumed from an epoch's checkpoint draws the λ sequence of an uninterrupted run
             mix_gen.manual_seed(epoch * args.world_size + rank)
+        if augment is not None:
+            augment.generator.manual_seed(epoch * args.world_size + rank)   # as MixUp's: a resumed run draws what an uninterrupted one does
         pending = None   # (step index, loss handle) of a log line whose value is still on its way to the host
         fmt = "Epoch [{}/{}], Step [{}/{}], Loss: {:.4f}"
         for i, (images, labels) in enumerate(train_loader):
@@ -244,6 +289,8 @@ def dist_train(gpu: int, args) -> None:
             else:
                 images = images.to(device, non_blocking=True)
                 labels = labels.to(device, non_blocking=True)
+                if augment is not None:
+                    images = augment(images)
                 optimizer.zero_grad()
                 if accum == 1:
                     outputs = model(images)

@@ -1,0 +1,119 @@
+// Per-image random affine augmentation (torchvision's RandomAffine on a batch, every image with its own parameters), one launch.
+// One CTA per image, one thread per pixel up to 1024: thread 0 draws the image's parameters from Philox subsequence b and forms
+// torchvision's inverse matrix in double into shared memory; then every thread maps its output pixels to source coordinates once
+// and samples all channels there.
+#include <cuda_runtime.h>
+#include <curand_kernel.h>
+
+#include <algorithm>
+#include <stdexcept>
+
+#include "cuda_utils.h"
+#include "ops_kernels.h"
+
+namespace pdt {
+
+namespace {
+
+// one thread per output pixel up to 1024 (a 28×28 image in one pass: each thread's source loads are the kernel's latency)
+constexpr int kAffineMaxThreads = 1024;
+
+// torch's CUDA uniform_: curand's (0, 1] with 1 mapped to 0, then u·range + from in fp32: U[from, to)
+__device__ __forceinline__ float draw(float r, float from, float range) { return (r == 1.f ? 0.f : r) * range + from; }
+
+__global__ void __launch_bounds__(kAffineMaxThreads) random_affine_kernel(const float* __restrict__ x, float* __restrict__ y,
+                                                                        float* __restrict__ params, int C, int H, int W, AffineSpec s,
+                                                                        PhiloxSeed rng) {
+  __shared__ double m[6];
+  const int b = blockIdx.x;
+  if (threadIdx.x == 0) {
+    unsigned long long seed = rng.seed, offset = rng.offset;
+    if (rng.seed_ptr != nullptr) {   // captured: the graph's replay writes seed and base offset before it launches us
+      seed = static_cast<unsigned long long>(*rng.seed_ptr);
+      offset = static_cast<unsigned long long>(*rng.offset_ptr) + rng.offset;
+    }
+    curandStatePhilox4_32_10_t st;
+    curand_init(seed, b, offset, &st);
+    const float4 r0 = curand_uniform4(&st);
+    const float4 r1 = curand_uniform4(&st);
+    const float angle = draw(r0.x, s.angle_from, s.angle_range);
+    const float tx = rintf(draw(r0.y, s.tx_from, s.tx_range));   // round half to even, as Python's round
+    const float ty = rintf(draw(r0.z, s.ty_from, s.ty_range));
+    const float scale = draw(r0.w, s.scale_from, s.scale_range);
+    const float shear_x = draw(r1.x, s.shear_x_from, s.shear_x_range);
+    const float shear_y = draw(r1.y, s.shear_y_from, s.shear_y_range);
+    if (params != nullptr) {
+      float* p = params + 6 * static_cast<long long>(b);
+      p[0] = angle, p[1] = tx, p[2] = ty, p[3] = scale, p[4] = shear_x, p[5] = shear_y;
+    }
+    // torchvision's _get_inverse_affine_matrix(center=[0, 0], angle, (tx, ty), scale, (shear_x, shear_y)), in double
+    constexpr double kRad = 3.14159265358979323846 / 180.0;
+    const double rot = angle * kRad, sx = shear_x * kRad, sy = shear_y * kRad;
+    const double a = cos(rot - sy) / cos(sy);
+    const double bb = -cos(rot - sy) * tan(sx) / cos(sy) - sin(rot);
+    const double c = sin(rot - sy) / cos(sy);
+    const double d = -sin(rot - sy) * tan(sx) / cos(sy) + cos(rot);
+    const double sc = scale;
+    m[0] = d / sc, m[1] = -bb / sc, m[3] = -c / sc, m[4] = a / sc;
+    m[2] = m[0] * -static_cast<double>(tx) + m[1] * -static_cast<double>(ty);
+    m[5] = m[3] * -static_cast<double>(tx) + m[4] * -static_cast<double>(ty);
+  }
+  __syncthreads();
+  const double m0 = m[0], m1 = m[1], m2 = m[2], m3 = m[3], m4 = m[4], m5 = m[5];
+  const double cw = 0.5 * (W - 1), ch = 0.5 * (H - 1);
+  const int hw = H * W;
+  const float* __restrict__ src = x + static_cast<long long>(b) * C * hw;
+  float* __restrict__ dst = y + static_cast<long long>(b) * C * hw;
+  const float fill = s.fill;
+  for (int p = threadIdx.x; p < hw; p += blockDim.x) {
+    const int i = p / W, j = p - (p / W) * W;
+    // the source coordinate of output pixel (i, j): torchvision's _affine_grid + grid_sample(align_corners=False), unnormalised
+    const double xj = j - cw, yi = i - ch;
+    const double sxp = m0 * xj + m1 * yi + m2 + cw;
+    const double syp = m3 * xj + m4 * yi + m5 + ch;
+    if (!s.bilinear) {
+      const double rx = rint(sxp), ry = rint(syp);   // ties to even, as grid_sample's nearbyint
+      const bool in = rx >= 0.0 && rx <= W - 1 && ry >= 0.0 && ry <= H - 1;   // false for NaN
+      const int o = in ? static_cast<int>(ry) * W + static_cast<int>(rx) : 0;
+      for (int ci = 0; ci < C; ++ci) dst[ci * hw + p] = in ? __ldg(src + ci * hw + o) : fill;
+      continue;
+    }
+    const double x0 = floor(sxp), y0 = floor(syp);
+    const double fx = sxp - x0, fy = syp - y0;
+    const bool vx0 = x0 >= 0.0 && x0 <= W - 1, vx1 = x0 >= -1.0 && x0 <= W - 2;
+    const bool vy0 = y0 >= 0.0 && y0 <= H - 1, vy1 = y0 >= -1.0 && y0 <= H - 2;
+    // taps nw, ne, sw, se; out-of-bounds taps read 0 and add nothing to the mask
+    const bool v[4] = {vx0 && vy0, vx1 && vy0, vx0 && vy1, vx1 && vy1};
+    const float w[4] = {static_cast<float>((1.0 - fx) * (1.0 - fy)), static_cast<float>(fx * (1.0 - fy)),
+                        static_cast<float>((1.0 - fx) * fy), static_cast<float>(fx * fy)};
+    int o[4];
+    const int ix = vx0 || vx1 ? static_cast<int>(x0) : 0, iy = vy0 || vy1 ? static_cast<int>(y0) : 0;
+    o[0] = iy * W + ix, o[1] = o[0] + 1, o[2] = o[0] + W, o[3] = o[0] + W + 1;
+    float mask = 0.f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) mask += v[k] ? w[k] : 0.f;
+    for (int ci = 0; ci < C; ++ci) {
+      const float* __restrict__ plane = src + ci * hw;
+      float acc = 0.f;
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        if (v[k]) acc += w[k] * __ldg(plane + o[k]);
+      // torchvision's fill: (img − fill)·mask + fill, the mask being grid_sample's bilinear weight of the in-bounds taps
+      dst[ci * hw + p] = (acc - fill) * mask + fill;
+    }
+  }
+}
+
+}  // namespace
+
+void launch_random_affine(const float* x, float* y, float* params, int B, int C, int H, int W, const AffineSpec& s, PhiloxSeed rng,
+                          cudaStream_t st) {
+  if (B < 0 || C < 1 || H < 1 || W < 1) throw std::invalid_argument("random_affine: bad shape");
+  if (static_cast<long long>(C) * H * W >= (1LL << 31)) throw std::invalid_argument("random_affine: an image must have fewer than 2^31 elements");
+  if (B == 0) return;
+  const int threads = static_cast<int>(std::min<long long>(kAffineMaxThreads, (static_cast<long long>(H) * W + 31) / 32 * 32));
+  random_affine_kernel<<<B, threads, 0, st>>>(x, y, params, C, H, W, s, rng);
+  check_launch("random_affine");
+}
+
+}  // namespace pdt

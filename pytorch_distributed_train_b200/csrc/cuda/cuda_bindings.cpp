@@ -1,5 +1,6 @@
 // CUDA-side bindings: GPU communicators and the sm_90a operator library.
 #include <ATen/cuda/CUDAContext.h>
+#include <ATen/cuda/CUDAGeneratorImpl.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <pybind11/stl.h>
 #include <torch/extension.h>
@@ -1428,6 +1429,64 @@ void register_cuda_bindings(py::module_& m) {
     }
   }, py::arg("averaged"), py::arg("current"), py::arg("n_averaged"), py::arg("decay"), py::arg("copied") = std::vector<at::Tensor>{},
      py::arg("copied_from") = std::vector<at::Tensor>{});
+  // Random affine augmentation (torchvision's RandomAffine per image): x fp32 [B, C, H, W] → a new tensor of the same shape, and
+  // the [B, 6] parameters when record_params.  The Philox state comes from `generator` (a CUDA generator on x's device; the device's
+  // default one when None) as torch's own random kernels take it: under stream capture through the graph-safe seed and offset
+  // pointers, so that every replay draws new values.
+  m.def("random_affine", [](const at::Tensor& x, std::vector<double> degrees, std::vector<double> translate, std::vector<double> scale,
+                            std::vector<double> shear, bool bilinear, double fill, c10::optional<at::Generator> generator,
+                            bool record_params) {
+    chk(x, "x");
+    TORCH_CHECK(x.dim() == 4, "random_affine: x must be [B, C, H, W] (got ", x.dim(), " dimensions)");
+    TORCH_CHECK(degrees.size() == 2 && (translate.empty() || translate.size() == 2) && (scale.empty() || scale.size() == 2) &&
+                (shear.empty() || shear.size() == 2 || shear.size() == 4), "random_affine: bad parameter ranges");
+    c10::cuda::CUDAGuard g(x.device());
+    const int B = static_cast<int>(x.size(0)), C = static_cast<int>(x.size(1)), H = static_cast<int>(x.size(2)), W = static_cast<int>(x.size(3));
+    // torch's uniform_(from, to): the range is formed in double, then both go to fp32
+    auto range = [](double from, double to, float& f, float& r) {
+      TORCH_CHECK(from <= to, "random_affine: uniform_ expects to return a [from, to) range, but found from=", from, " > to=", to);
+      f = static_cast<float>(from);
+      r = static_cast<float>(to - from);
+    };
+    AffineSpec s{};
+    range(degrees[0], degrees[1], s.angle_from, s.angle_range);
+    if (!translate.empty()) {
+      const double max_dx = translate[0] * W, max_dy = translate[1] * H;
+      range(-max_dx, max_dx, s.tx_from, s.tx_range);
+      range(-max_dy, max_dy, s.ty_from, s.ty_range);
+    }
+    s.scale_from = 1.f;
+    if (!scale.empty()) range(scale[0], scale[1], s.scale_from, s.scale_range);
+    if (!shear.empty()) range(shear[0], shear[1], s.shear_x_from, s.shear_x_range);
+    if (shear.size() == 4) range(shear[2], shear[3], s.shear_y_from, s.shear_y_range);
+    s.fill = static_cast<float>(fill);
+    s.bilinear = bilinear ? 1 : 0;
+    auto y = at::empty_like(x);
+    at::Tensor params;
+    if (record_params) params = at::empty({x.size(0), 6}, x.options());
+    if (B == 0) return py::make_tuple(y, record_params ? py::cast(params) : py::none());
+    auto* gen = at::get_generator_or_default<at::CUDAGeneratorImpl>(generator, at::cuda::detail::getDefaultCUDAGenerator(x.device().index()));
+    TORCH_CHECK(!generator.has_value() || generator->device() == x.device(), "random_affine: the generator is on ", generator->device(),
+                ", x on ", x.device());
+    at::PhiloxCudaState ps;
+    {
+      std::lock_guard<std::mutex> lock(gen->mutex_);
+      ps = gen->philox_cuda_state(kAffineOffsetIncrement);
+    }
+    PhiloxSeed rng{};
+    if (ps.captured_) {
+      rng.seed_ptr = reinterpret_cast<const long long*>(ps.seed_.ptr);
+      rng.offset_ptr = reinterpret_cast<const long long*>(ps.offset_.ptr);
+      rng.offset = ps.offset_intragraph_;
+    } else {
+      rng.seed = ps.seed_.val;
+      rng.offset = ps.offset_.val;
+    }
+    launch_random_affine(x.data_ptr<float>(), y.data_ptr<float>(), record_params ? params.data_ptr<float>() : nullptr, B, C, H, W, s, rng,
+                         cur_stream(x));
+    return py::make_tuple(y, record_params ? py::cast(params) : py::none());
+  }, py::arg("x"), py::arg("degrees"), py::arg("translate"), py::arg("scale"), py::arg("shear"), py::arg("bilinear"), py::arg("fill"),
+     py::arg("generator"), py::arg("record_params"));
 }
 
 }  // namespace pdt

@@ -374,6 +374,37 @@ struct AvgArgs {
 };
 void launch_avg_multi(const AvgTensorList& tl, AvgArgs a, cudaStream_t st);
 
+// ---- data augmentation ---------------------------------------------------------------------------------
+// The Philox seed and offset of one launch: torch's PhiloxCudaState without torch's types.  Under CUDA-graph capture the seed and
+// the base offset are read from device memory (seed_ptr, offset_ptr + offset), which the graph's replay refreshes, so every replay
+// draws new values; otherwise seed and offset are used as they are.
+struct PhiloxSeed {
+  unsigned long long seed, offset;
+  const long long* seed_ptr;     // null unless captured
+  const long long* offset_ptr;
+};
+// Every parameter is drawn as U[from, from + range) in fp32, torch's uniform_; a range of 0 gives `from` (1 for an absent scale,
+// 0 for the others).  fill: the value of pixels whose source lies outside the image.
+struct AffineSpec {
+  float angle_from, angle_range;
+  float tx_from, tx_range, ty_from, ty_range;   // before the rounding to whole pixels
+  float scale_from, scale_range;
+  float shear_x_from, shear_x_range, shear_y_from, shear_y_range;
+  float fill;
+  int bilinear;   // 0: nearest
+};
+// Philox values each image consumes (two curand_uniform4 from subsequence b): the generator's offset increment per launch
+constexpr int kAffineOffsetIncrement = 8;
+// torchvision's RandomAffine applied to each image of x [B, C, H, W] (fp32 contiguous NCHW) with its own parameters, into y of the
+// same shape.  Image b draws (angle, tx, ty, scale, shear_x, shear_y) from Philox subsequence b, tx and ty rounded half to even,
+// and stores them in params[b, 0:6] (fp32, nullable).  The inverse matrix is torchvision's _get_inverse_affine_matrix with
+// center (0, 0) in double; output pixel (i, j) samples the source at
+//   sx = m0·(j − cw) + m1·(i − ch) + m2 + cw,   sy = m3·(j − cw) + m4·(i − ch) + m5 + ch,   cw = (W − 1)/2, ch = (H − 1)/2
+// (double): nearest rounds half to even and takes `fill` outside the image; bilinear reads 0 outside and returns
+// (v − fill)·mask + fill, mask being the bilinear weight of the in-bounds taps.  One launch (none when B = 0).
+void launch_random_affine(const float* x, float* y, float* params, int B, int C, int H, int W, const AffineSpec& s, PhiloxSeed rng,
+                          cudaStream_t st);
+
 #ifdef __CUDACC__
 // max that keeps a NaN (fmaxf drops it), as torch's inf-norm does
 __device__ __forceinline__ float nan_max(float a, float b) { return (a != a || a > b) ? a : b; }

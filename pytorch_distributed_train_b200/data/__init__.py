@@ -1,4 +1,5 @@
-"""Input pipeline: samplers, DataLoader, MNIST (idx parser), synthetic datasets and MixUp."""
+"""Input pipeline: samplers, DataLoader, MNIST (idx parser), synthetic datasets, MixUp and random affine augmentation."""
+from .augment import RandomAffine
 from .dataloader import DataLoader, DevicePrefetcher, default_collate
 from .mixup import mixup
 from .mnist import MNIST, SyntheticMNIST, TensorDataset, read_idx, synthesize_mnist_files, write_idx
@@ -7,5 +8,5 @@ from .sampler import BatchSampler, DistributedSampler, RandomSampler, Sampler, S
 __all__ = [
     "DataLoader", "DevicePrefetcher", "default_collate", "MNIST", "SyntheticMNIST", "TensorDataset",
     "read_idx", "write_idx", "synthesize_mnist_files", "BatchSampler", "DistributedSampler",
-    "RandomSampler", "Sampler", "SequentialSampler", "mixup",
+    "RandomSampler", "Sampler", "SequentialSampler", "mixup", "RandomAffine",
 ]

@@ -50,6 +50,14 @@ inside the graph, on one GPU too: it reads and advances ``n_averaged`` on the de
 kernel was measured slower than this launch: DESIGN.md §7.)  torch's own update reads ``n_averaged`` on the host and
 cannot be captured, so an averaged model that would take it is refused.  The warm-up steps the constructor runs are not
 averaged.
+
+Augmentation (``augment``, a callable on the image batch such as ``pdt.data.RandomAffine``): every step runs
+``x = augment(inputs[0])`` before the model; with accumulation, once on all k·b rows before the micro-batches are sliced.  A
+``RandomAffine`` on a CUDA batch is one more launch inside the graph that draws its parameters on the device, so every replay
+augments with fresh ones.  Its generator, when it is not the device's default one (which every capture registers), is registered
+with each captured graph, so its ``manual_seed`` between replays takes effect.  The model sees a plain contiguous fp32 batch.  After
+each call, an augmentation's ``last_params`` (``RandomAffine(record_params=True)``) is the replayed graph's, so it holds that step's
+draws.
 """
 from __future__ import annotations
 
@@ -68,9 +76,11 @@ class GraphedTrainStep:
 
     def __init__(self, model, criterion, optimizer, example_inputs: Sequence[torch.Tensor], warmup: int = 3,
                  zero_grad_set_to_none: bool = True, fuse_optimizer: bool = True, double_buffer_inputs: bool = True,
-                 max_grad_norm: Optional[float] = None, norm_type: float = 2.0, accumulation_steps: int = 1, averaged_model=None):
+                 max_grad_norm: Optional[float] = None, norm_type: float = 2.0, accumulation_steps: int = 1, averaged_model=None,
+                 augment=None):
         if not torch.cuda.is_available():
             raise RuntimeError("GraphedTrainStep needs CUDA")
+        self.augment = augment
         self.averaged_model = averaged_model
         self._averaged_source = getattr(model, "module", model)   # the averaged model was copied from the bare model
         if averaged_model is not None:
@@ -149,6 +159,8 @@ class GraphedTrainStep:
         inputs = self.static_inputs if inputs is None else inputs
         from ..ops import functional as OF
 
+        if self.augment is not None:
+            inputs = [self.augment(inputs[0])] + list(inputs[1:])   # all k·b rows at once under accumulation
         if self.accumulation_steps > 1:
             return self._finish_step(self._accumulate(inputs))
 
@@ -274,11 +286,18 @@ class GraphedTrainStep:
         comm = getattr(self.model, "comm", None)
         parity = (lambda: list(comm.parity_state())) if hasattr(comm, "parity_state") else (lambda: [])
         self.graphs, self.losses, self.norms = [], [], []
+        self._augment_params = []   # the static parameter record of each graph's augmentation (RandomAffine(record_params=True))
         p0 = parity()
         for k in range(2):
             if self._riding and self.max_grad_norm is not None:
                 self._ride(k)   # each graph's rider stores the norm in its own scalar
             g = torch.cuda.CUDAGraph()
+            gen = getattr(self.augment, "generator", None)
+            if (isinstance(gen, torch.Generator) and gen.device.type == "cuda"
+                    and gen is not torch.cuda.default_generators[gen.device.index if gen.device.index is not None else torch.cuda.current_device()]):
+                # the capture registers the default generator itself; any other one that the step draws from must be registered, so
+                # that each replay advances its offset (and its manual_seed reaches the graph)
+                g.register_generator_state(gen)
             before = _C.kernel_launch_count()
             self._averaging = self.averaged_model is not None
             with torch.cuda.graph(g, stream=side):
@@ -289,6 +308,7 @@ class GraphedTrainStep:
             self.graphs.append(g)
             self.losses.append(loss)
             self.norms.append(norm)
+            self._augment_params.append(getattr(self.augment, "last_params", None))
             torch.cuda.synchronize(dev)
             ordered = getattr(self.model, "syncs_buffers_every_step", None)
             if not self.double_buffer and (parity() == p0 or (ordered is not None and ordered())):
@@ -317,6 +337,8 @@ class GraphedTrainStep:
         self._last = i
         self.static_loss = self.losses[i]
         self.grad_norm = self.norms[i]
+        if self._augment_params[i] is not None:
+            self.augment.last_params = self._augment_params[i]   # the draws of this replay, not of the graph captured last
         return self.static_loss
 
     def loss_to_host(self) -> "HostLoss":

@@ -710,6 +710,19 @@ def average_update(averaged, current, n_averaged: torch.Tensor, decay: Optional[
     _C.avg_multi(list(averaged), list(current), n_averaged, -1.0 if decay is None else float(decay), list(copied), list(copied_from))
 
 
+def random_affine(x: torch.Tensor, degrees, translate=None, scale=None, shear=None, bilinear: bool = False, fill: float = 0.0,
+                  generator: Optional[torch.Generator] = None, record_params: bool = False):
+    """torchvision's ``RandomAffine`` on every image of ``x`` (fp32 contiguous CUDA ``[B, C, H, W]``) with its own parameters,
+    drawn on the device from ``generator``'s Philox state (the device's default CUDA generator when None): one launch,
+    graph-capturable, every replay drawing new values.  ``degrees``, ``scale`` and ``shear`` are (lo, hi) ranges (``shear`` 2 or 4
+    values), ``translate`` the (x, y) fractions, each None when absent.  Returns ``(out, params)``: ``params`` is the fp32
+    ``[B, 6]`` (angle, tx, ty, scale, shear_x, shear_y) with ``record_params``, None otherwise.  ``pdt.data.RandomAffine`` is the
+    user-facing transform that validates the arguments."""
+    return _C.random_affine(x, [float(d) for d in degrees], [] if translate is None else [float(t) for t in translate],
+                            [] if scale is None else [float(s) for s in scale], [] if shear is None else [float(s) for s in shear],
+                            bool(bilinear), float(fill), generator, bool(record_params))
+
+
 # ---- generic (NCHW) BatchNorm pieces used by parallel.SyncBatchNorm ------------------------------------------
 def bn_local_stats(x: torch.Tensor) -> torch.Tensor:
     """float64 [2C+2] = per-channel Σx, Σx² (accumulated in fp64), the per-channel element count, one zero pad."""

@@ -33,6 +33,7 @@ GROUPS = {
     "maxpool_ties": ["tests/test_maxpool_ties.py"],
     "input_grads": ["tests/test_convnet_input_grads.py"],
     "symm_emu": ["tests/test_symm_kernels_emulated.py"],
+    "random_affine": ["tests/test_random_affine.py"],
 }
 
 
