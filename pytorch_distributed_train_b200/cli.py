@@ -10,7 +10,7 @@ Extra flags cover what the reference hard-codes: ``--init-method`` (its LAN addr
 to loopback with a free port), ``--data synthetic|mnist``, ``--model``, ``--comm fused|nccl``, ``--algo``,
 ``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw | nadam | radam | rmsprop |
 adagrad | adamax | adadelta | asgd | rprop), ``--lr``, ``--momentum``, ``--amsgrad``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--mixup``,
-``--rotate`` / ``--translate`` / ``--scale-range`` / ``--shear`` / ``--affine-interpolation`` (per-image random affine augmentation), ``--ema-decay``, ``--checkpoint`` / ``--resume``, ``--eval`` (test loss and accuracy after every epoch).
+``--cutmix`` (CutMix drawn on the device, inside the captured step with ``--graph``), ``--rotate`` / ``--translate`` / ``--scale-range`` / ``--shear`` / ``--affine-interpolation`` (per-image random affine augmentation), ``--ema-decay``, ``--checkpoint`` / ``--resume``, ``--eval`` (test loss and accuracy after every epoch).
 """
 from __future__ import annotations
 
@@ -67,6 +67,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--mixup", default=None, type=float, metavar="ALPHA",
                    help="MixUp every training batch with lambda ~ Beta(ALPHA, ALPHA), ALPHA > 0, and train on the mixed class "
                         "probabilities (default: off)")
+    p.add_argument("--cutmix", default=None, type=float, metavar="ALPHA",
+                   help="CutMix every training batch on the device with lambda ~ Beta(ALPHA, ALPHA), ALPHA > 0: a box of the previous "
+                        "image pasted into each image, trained on the mixed class probabilities (default: off)")
     p.add_argument("--rotate", default=None, type=float, metavar="DEG",
                    help="random affine augmentation: rotate every training image by an angle ~ U[-DEG, DEG) (default: off)")
     p.add_argument("--translate", default=None, type=float, metavar="FRAC",
@@ -167,6 +170,12 @@ def check_args(p: argparse.ArgumentParser, args) -> None:
     if args.mixup is not None and affine_requested(args):
         p.error("--mixup cannot be combined with --rotate, --translate, --scale-range or --shear: MixUp mixes on the host before the "
                 "batch reaches the device, where the affine would warp the mixed image with one parameter set")
+    cutmix = getattr(args, "cutmix", None)
+    if cutmix is not None and not cutmix > 0:
+        p.error(f"--cutmix must be positive (got {cutmix})")
+    if cutmix is not None and args.mixup is not None:
+        p.error("--cutmix cannot be combined with --mixup: each replaces the batch's targets with its own mixture (a random choice "
+                "between the two per batch is not implemented)")
     if args.ema_decay is not None and not 0.0 <= args.ema_decay <= 1.0:
         p.error(f"--ema-decay must lie in [0, 1] (got {args.ema_decay})")
     if args.graph and args.gpus >= 2 and args.accumulation_steps > 1:
@@ -243,6 +252,11 @@ def dist_train(gpu: int, args) -> None:
     # every training image warped with its own parameters, on the batch's device after its copy (inside the captured step with
     # --graph); each rank draws from its own generator, seeded per epoch below
     augment = make_augment(args, torch.Generator(device=device))
+    # CutMix on the batch's device after the copy and the affine (inside the captured step with --graph); its own generator per rank,
+    # seeded per epoch below
+    cutmix = None
+    if getattr(args, "cutmix", None) is not None:
+        cutmix = pdata.CutMix(alpha=args.cutmix, num_classes=num_classes, generator=torch.Generator(device=device))
 
     step_fn = None
     if args.graph and use_cuda:
@@ -252,7 +266,8 @@ def dist_train(gpu: int, args) -> None:
         example_targets = (torch.zeros(rows, dtype=torch.int64, device=device) if mix_gen is None else
                            torch.zeros(rows, num_classes, device=device))
         step_fn = GraphedTrainStep(model, criterion, optimizer, example_inputs=(torch.zeros((rows,) + shape, device=device), example_targets),
-                                   max_grad_norm=args.clip_grad_norm, accumulation_steps=accum, averaged_model=ema, augment=augment)
+                                   max_grad_norm=args.clip_grad_norm, accumulation_steps=accum, averaged_model=ema, augment=augment,
+                                   mix=cutmix)
 
     first_epoch = 0
     if args.resume:
@@ -271,6 +286,8 @@ def dist_train(gpu: int, args) -> None:
             mix_gen.manual_seed(epoch * args.world_size + rank)
         if augment is not None:
             augment.generator.manual_seed(epoch * args.world_size + rank)   # as MixUp's: a resumed run draws what an uninterrupted one does
+        if cutmix is not None:
+            cutmix.generator.manual_seed(epoch * args.world_size + rank)
         pending = None   # (step index, loss handle) of a log line whose value is still on its way to the host
         fmt = "Epoch [{}/{}], Step [{}/{}], Loss: {:.4f}"
         for i, (images, labels) in enumerate(train_loader):
@@ -291,6 +308,8 @@ def dist_train(gpu: int, args) -> None:
                 labels = labels.to(device, non_blocking=True)
                 if augment is not None:
                     images = augment(images)
+                if cutmix is not None:
+                    images, labels = cutmix(images, labels)   # the whole loader batch, as the graphed step mixes it
                 optimizer.zero_grad()
                 if accum == 1:
                     outputs = model(images)

@@ -2,6 +2,8 @@
 // One CTA per image, one thread per pixel up to 1024: thread 0 draws the image's parameters from Philox subsequence b and forms
 // torchvision's inverse matrix in double into shared memory; then every thread maps its output pixels to source coordinates once
 // and samples all channels there.
+// Batch-level MixUp and CutMix (torchvision's v2 transforms), one launch: one CTA per image, each drawing the batch's λ (and box)
+// from the same Philox values, then mixing its image with its roll-by-one partner and writing its target row.
 #include <cuda_runtime.h>
 #include <curand_kernel.h>
 
@@ -18,6 +20,17 @@ namespace {
 // one thread per output pixel up to 1024 (a 28×28 image in one pass: each thread's source loads are the kernel's latency)
 constexpr int kAffineMaxThreads = 1024;
 
+// Philox subsequence `subsequence` at the launch's offset.  Captured: the graph's replay writes seed and base offset before it
+// launches us.
+__device__ __forceinline__ void philox_init(const PhiloxSeed& rng, unsigned long long subsequence, curandStatePhilox4_32_10_t* st) {
+  unsigned long long seed = rng.seed, offset = rng.offset;
+  if (rng.seed_ptr != nullptr) {
+    seed = static_cast<unsigned long long>(*rng.seed_ptr);
+    offset = static_cast<unsigned long long>(*rng.offset_ptr) + rng.offset;
+  }
+  curand_init(seed, subsequence, offset, st);
+}
+
 // torch's CUDA uniform_: curand's (0, 1] with 1 mapped to 0, then u·range + from in fp32: U[from, to)
 __device__ __forceinline__ float draw(float r, float from, float range) { return (r == 1.f ? 0.f : r) * range + from; }
 
@@ -27,13 +40,8 @@ __global__ void __launch_bounds__(kAffineMaxThreads) random_affine_kernel(const 
   __shared__ double m[6];
   const int b = blockIdx.x;
   if (threadIdx.x == 0) {
-    unsigned long long seed = rng.seed, offset = rng.offset;
-    if (rng.seed_ptr != nullptr) {   // captured: the graph's replay writes seed and base offset before it launches us
-      seed = static_cast<unsigned long long>(*rng.seed_ptr);
-      offset = static_cast<unsigned long long>(*rng.offset_ptr) + rng.offset;
-    }
     curandStatePhilox4_32_10_t st;
-    curand_init(seed, b, offset, &st);
+    philox_init(rng, b, &st);
     const float4 r0 = curand_uniform4(&st);
     const float4 r1 = curand_uniform4(&st);
     const float angle = draw(r0.x, s.angle_from, s.angle_range);
@@ -104,6 +112,95 @@ __global__ void __launch_bounds__(kAffineMaxThreads) random_affine_kernel(const 
   }
 }
 
+constexpr int kMixThreads = 256;
+
+// log of one Gamma(alpha) draw: Marsaglia & Tsang (2000) in double, for alpha < 1 boosted as Gamma(alpha + 1)·U^(1/alpha) with the
+// power kept as a logarithm (at small alpha the draw itself underflows).  Every attempt consumes 8 Philox values whether it is
+// accepted or not, so a draw never reads past its kGammaMaxAttempts · 8; a draw that exhausts them (probability < 1e-21) returns
+// log d, the distribution's mode region.
+__device__ double log_gamma_draw(curandStatePhilox4_32_10_t* st, double alpha) {
+  const bool boost = alpha < 1.0;
+  const double d = (boost ? alpha + 1.0 : alpha) - 1.0 / 3.0;
+  const double c = 1.0 / sqrt(9.0 * d);
+  const double log_d = log(d);
+  for (int k = 0; k < kGammaMaxAttempts; ++k) {
+    const double2 n = curand_normal2_double(st);
+    const double2 u = curand_uniform2_double(st);   // (0, 1): u.x decides, u.y is the boost's U
+    const double t = 1.0 + c * n.x;
+    if (t <= 0.0) continue;
+    const double log_v = 3.0 * log(t);
+    if (log(u.x) < 0.5 * n.x * n.x + d - d * (t * t * t) + d * log_v) return log_d + log_v + (boost ? log(u.y) / alpha : 0.0);
+  }
+  return log_d;
+}
+
+// One CTA per image i: thread 0 draws the batch's parameters (every CTA draws the same ones, from Philox subsequence 0), then the
+// CTA writes image i and target row i.
+__global__ void __launch_bounds__(kMixThreads, 1) mix_batch_kernel(const float* __restrict__ x, const long long* __restrict__ labels,
+                                                                const float* __restrict__ probs, float* __restrict__ y,
+                                                                float* __restrict__ q, double* __restrict__ record, int B, int C, int H,
+                                                                int W, int K, double alpha, int cutmix, PhiloxSeed rng) {
+  __shared__ double s_lam;
+  __shared__ int s_box[4];
+  const int i = blockIdx.x;
+  if (threadIdx.x == 0) {
+    curandStatePhilox4_32_10_t st;
+    philox_init(rng, 0, &st);
+    const double2 r = curand_uniform2_double(&st);   // (0, 1), drawn by MixUp too so that both modes read the stream alike
+    const double lg1 = log_gamma_draw(&st, alpha);
+    const double lg2 = log_gamma_draw(&st, alpha);
+    // λ = G₁/(G₁ + G₂), never 0/0 when both draws underflow
+    const double lam = 1.0 / (1.0 + exp(lg2 - lg1));
+    double lam_mix = lam;
+    int x1 = 0, y1 = 0, x2 = 0, y2 = 0;
+    if (cutmix) {
+      // torchvision's CutMix.make_params from (λ, r_x, r_y), in double
+      const int rx = min(static_cast<int>((1.0 - r.x) * W), W - 1), ry = min(static_cast<int>((1.0 - r.y) * H), H - 1);
+      const double rr = 0.5 * sqrt(1.0 - lam);
+      const int rw_half = static_cast<int>(rr * W), rh_half = static_cast<int>(rr * H);
+      x1 = max(rx - rw_half, 0), y1 = max(ry - rh_half, 0), x2 = min(rx + rw_half, W), y2 = min(ry + rh_half, H);
+      lam_mix = 1.0 - static_cast<double>(static_cast<long long>(x2 - x1) * (y2 - y1)) / static_cast<double>(static_cast<long long>(W) * H);
+      if (record != nullptr && i == 0) {
+        record[0] = lam, record[1] = rx, record[2] = ry, record[3] = x1, record[4] = y1, record[5] = x2, record[6] = y2;
+        record[7] = lam_mix;
+      }
+    } else if (record != nullptr && i == 0) {
+      record[0] = lam;
+    }
+    s_lam = lam_mix;
+    s_box[0] = x1, s_box[1] = y1, s_box[2] = x2, s_box[3] = y2;
+  }
+  __syncthreads();
+  const double lam = s_lam;
+  // torchvision's tensor ops: the Python float λ and 1 − λ (formed in double) each rounded to fp32 as a scalar operand
+  const float lf = static_cast<float>(lam), omf = static_cast<float>(1.0 - lam);
+  const int prev = i == 0 ? B - 1 : i - 1;
+  float* __restrict__ qi = q + static_cast<long long>(i) * K;
+  if (labels != nullptr) {
+    const long long li = labels[i], lp = labels[prev];
+    for (int k = threadIdx.x; k < K; k += blockDim.x) qi[k] = __fadd_rn(k == lp ? omf : 0.f, k == li ? lf : 0.f);
+  } else {
+    const float* __restrict__ pi = probs + static_cast<long long>(i) * K;
+    const float* __restrict__ pp = probs + static_cast<long long>(prev) * K;
+    for (int k = threadIdx.x; k < K; k += blockDim.x) qi[k] = __fadd_rn(__fmul_rn(__ldg(pp + k), omf), __fmul_rn(__ldg(pi + k), lf));
+  }
+  const int hw = H * W, n = C * hw;
+  const float* __restrict__ xi = x + static_cast<long long>(i) * n;
+  const float* __restrict__ xp = x + static_cast<long long>(prev) * n;
+  float* __restrict__ yi = y + static_cast<long long>(i) * n;
+  if (cutmix) {
+    const int x1 = s_box[0], y1 = s_box[1], x2 = s_box[2], y2 = s_box[3];
+    for (int e = threadIdx.x; e < n; e += blockDim.x) {
+      const int p = e % hw, h = p / W, w = p - h * W;
+      const bool inside = h >= y1 && h < y2 && w >= x1 && w < x2;
+      yi[e] = __ldg((inside ? xp : xi) + e);
+    }
+  } else {
+    // two roundings, no FMA: fl(fl(x[i−1]·(1 − λ)) + fl(x[i]·λ))
+    for (int e = threadIdx.x; e < n; e += blockDim.x) yi[e] = __fadd_rn(__fmul_rn(__ldg(xp + e), omf), __fmul_rn(__ldg(xi + e), lf));
+  }
+}
+
 }  // namespace
 
 void launch_random_affine(const float* x, float* y, float* params, int B, int C, int H, int W, const AffineSpec& s, PhiloxSeed rng,
@@ -114,6 +211,16 @@ void launch_random_affine(const float* x, float* y, float* params, int B, int C,
   const int threads = static_cast<int>(std::min<long long>(kAffineMaxThreads, (static_cast<long long>(H) * W + 31) / 32 * 32));
   random_affine_kernel<<<B, threads, 0, st>>>(x, y, params, C, H, W, s, rng);
   check_launch("random_affine");
+}
+
+void launch_mix_batch(const float* x, const long long* labels, const float* probs, float* y, float* q, double* record, int B, int C, int H,
+                      int W, int K, double alpha, bool cutmix, PhiloxSeed rng, cudaStream_t st) {
+  if (B < 0 || C < 1 || H < 1 || W < 1 || K < 1) throw std::invalid_argument("mix_batch: bad shape");
+  if (static_cast<long long>(C) * H * W >= (1LL << 31)) throw std::invalid_argument("mix_batch: an image must have fewer than 2^31 elements");
+  if (!(alpha > 0.0)) throw std::invalid_argument("mix_batch: alpha must be positive");
+  if (B == 0) return;
+  mix_batch_kernel<<<B, kMixThreads, 0, st>>>(x, labels, probs, y, q, record, B, C, H, W, K, alpha, cutmix ? 1 : 0, rng);
+  check_launch("mix_batch");
 }
 
 }  // namespace pdt

@@ -7,6 +7,7 @@
 
 #include <cmath>
 #include <cstring>
+#include <limits>
 #include <map>
 #include <mutex>
 
@@ -30,6 +31,30 @@ void chk(const at::Tensor& t, const char* name, at::ScalarType dt = at::kFloat) 
   TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor");
   TORCH_CHECK(t.scalar_type() == dt, name, " must have dtype ", c10::toString(dt), " (got ", c10::toString(t.scalar_type()), ")");
   TORCH_CHECK(t.is_contiguous(), name, " must be contiguous");
+}
+
+// The Philox seed and offset of one launch that consumes `increment` values per subsequence, taken from `generator` (a CUDA generator
+// on x's device; the device's default one when None) as torch's own random kernels take them: under stream capture through the
+// graph-safe seed and offset pointers, so that every replay draws new values.
+PhiloxSeed philox_seed(const c10::optional<at::Generator>& generator, const at::Tensor& x, uint64_t increment, const char* what) {
+  auto* gen = at::get_generator_or_default<at::CUDAGeneratorImpl>(generator, at::cuda::detail::getDefaultCUDAGenerator(x.device().index()));
+  TORCH_CHECK(!generator.has_value() || generator->device() == x.device(), what, ": the generator is on ", generator->device(),
+              ", x on ", x.device());
+  at::PhiloxCudaState ps;
+  {
+    std::lock_guard<std::mutex> lock(gen->mutex_);
+    ps = gen->philox_cuda_state(increment);
+  }
+  PhiloxSeed rng{};
+  if (ps.captured_) {
+    rng.seed_ptr = reinterpret_cast<const long long*>(ps.seed_.ptr);
+    rng.offset_ptr = reinterpret_cast<const long long*>(ps.offset_.ptr);
+    rng.offset = ps.offset_intragraph_;
+  } else {
+    rng.seed = ps.seed_.val;
+    rng.offset = ps.offset_.val;
+  }
+  return rng;
 }
 
 const float* opt_ptr(const c10::optional<at::Tensor>& t, const char* name) {
@@ -1465,28 +1490,51 @@ void register_cuda_bindings(py::module_& m) {
     at::Tensor params;
     if (record_params) params = at::empty({x.size(0), 6}, x.options());
     if (B == 0) return py::make_tuple(y, record_params ? py::cast(params) : py::none());
-    auto* gen = at::get_generator_or_default<at::CUDAGeneratorImpl>(generator, at::cuda::detail::getDefaultCUDAGenerator(x.device().index()));
-    TORCH_CHECK(!generator.has_value() || generator->device() == x.device(), "random_affine: the generator is on ", generator->device(),
-                ", x on ", x.device());
-    at::PhiloxCudaState ps;
-    {
-      std::lock_guard<std::mutex> lock(gen->mutex_);
-      ps = gen->philox_cuda_state(kAffineOffsetIncrement);
-    }
-    PhiloxSeed rng{};
-    if (ps.captured_) {
-      rng.seed_ptr = reinterpret_cast<const long long*>(ps.seed_.ptr);
-      rng.offset_ptr = reinterpret_cast<const long long*>(ps.offset_.ptr);
-      rng.offset = ps.offset_intragraph_;
-    } else {
-      rng.seed = ps.seed_.val;
-      rng.offset = ps.offset_.val;
-    }
+    const PhiloxSeed rng = philox_seed(generator, x, kAffineOffsetIncrement, "random_affine");
     launch_random_affine(x.data_ptr<float>(), y.data_ptr<float>(), record_params ? params.data_ptr<float>() : nullptr, B, C, H, W, s, rng,
                          cur_stream(x));
     return py::make_tuple(y, record_params ? py::cast(params) : py::none());
   }, py::arg("x"), py::arg("degrees"), py::arg("translate"), py::arg("scale"), py::arg("shear"), py::arg("bilinear"), py::arg("fill"),
      py::arg("generator"), py::arg("record_params"));
+  // Batch MixUp / CutMix (torchvision's v2 transforms): x fp32 [B, C, H, W] and targets (int64 class indices [B] over num_classes,
+  // or fp32 probabilities [B, K]) → (a new image tensor, fp32 targets [B, K], the fp64 parameter record or None).  λ (and the box)
+  // are drawn on the device from `generator`, as random_affine draws.
+  m.def("mix_batch", [](const at::Tensor& x, const at::Tensor& targets, int64_t num_classes, double alpha, bool cutmix,
+                        c10::optional<at::Generator> generator, bool record_params) {
+    chk(x, "x");
+    TORCH_CHECK(x.dim() == 4, "mix_batch: x must be [B, C, H, W] (got ", x.dim(), " dimensions)");
+    TORCH_CHECK(alpha > 0.0, "mix_batch: alpha must be positive (got ", alpha, ")");
+    TORCH_CHECK(targets.device() == x.device(), "mix_batch: targets are on ", targets.device(), ", x on ", x.device());
+    const bool index = targets.dim() == 1;
+    if (index) {
+      chk(targets, "targets", at::kLong);
+      TORCH_CHECK(num_classes >= 1, "mix_batch: index targets need num_classes >= 1 (got ", num_classes, ")");
+    } else {
+      TORCH_CHECK(targets.dim() == 2, "mix_batch: targets must be [B] class indices or [B, K] probabilities (got ", targets.dim(),
+                  " dimensions)");
+      chk(targets, "targets");
+      TORCH_CHECK(targets.size(1) >= 1, "mix_batch: probability targets need at least one class");
+    }
+    TORCH_CHECK(targets.size(0) == x.size(0), "mix_batch: ", targets.size(0), " targets for ", x.size(0), " images");
+    c10::cuda::CUDAGuard g(x.device());
+    const int B = static_cast<int>(x.size(0)), C = static_cast<int>(x.size(1)), H = static_cast<int>(x.size(2)), W = static_cast<int>(x.size(3));
+    const int64_t K = index ? num_classes : targets.size(1);
+    TORCH_CHECK(K < (1LL << 31), "mix_batch: too many classes");
+    auto y = at::empty_like(x);
+    auto q = at::empty({x.size(0), K}, x.options());
+    at::Tensor record;
+    if (record_params) record = at::empty({cutmix ? 8 : 1}, x.options().dtype(at::kDouble));
+    if (B == 0) {
+      if (record_params) record.fill_(std::numeric_limits<double>::quiet_NaN());   // nothing drawn
+      return py::make_tuple(y, q, record_params ? py::cast(record) : py::none());
+    }
+    const PhiloxSeed rng = philox_seed(generator, x, kMixOffsetIncrement, "mix_batch");
+    const long long* labels = index ? reinterpret_cast<const long long*>(targets.data_ptr<int64_t>()) : nullptr;
+    launch_mix_batch(x.data_ptr<float>(), labels, index ? nullptr : targets.data_ptr<float>(), y.data_ptr<float>(), q.data_ptr<float>(), record_params ? record.data_ptr<double>() : nullptr, B, C, H, W,
+                     static_cast<int>(K), alpha, cutmix, rng, cur_stream(x));
+    return py::make_tuple(y, q, record_params ? py::cast(record) : py::none());
+  }, py::arg("x"), py::arg("targets"), py::arg("num_classes"), py::arg("alpha"), py::arg("cutmix"), py::arg("generator"),
+     py::arg("record_params"));
 }
 
 }  // namespace pdt

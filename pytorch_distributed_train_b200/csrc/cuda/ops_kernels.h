@@ -404,6 +404,24 @@ constexpr int kAffineOffsetIncrement = 8;
 // (v − fill)·mask + fill, mask being the bilinear weight of the in-bounds taps.  One launch (none when B = 0).
 void launch_random_affine(const float* x, float* y, float* params, int B, int C, int H, int W, const AffineSpec& s, PhiloxSeed rng,
                           cudaStream_t st);
+// Attempts each Gamma draw of mix_batch_kernel may make before it gives up (Marsaglia–Tsang rejects at most 4.9% of attempts for a
+// shape ≥ 1, so a draw reaches the cap with probability below 0.049^16 ≈ 1e-21)
+constexpr int kGammaMaxAttempts = 16;
+// Philox values one mix_batch launch consumes at most, every CTA reading the same ones from subsequence 0: 4 for (r_x, r_y), then per
+// Gamma draw 8 per attempt (a curand_normal2_double and a curand_uniform2_double), two draws.  The generator's offset increment per
+// launch, so consecutive launches never read overlapping parts of the stream.
+constexpr int kMixOffsetIncrement = 4 + 2 * kGammaMaxAttempts * 8;
+// torchvision's MixUp (cutmix = 0) or CutMix (cutmix = 1) on the batch x [B, C, H, W] (fp32 contiguous NCHW), image i paired with
+// image i − 1 (image 0 with image B − 1), into the new tensor y and the fp32 targets q [B, K].  The targets are int64 class
+// indices `labels` [B] (one-hot over K classes; an index outside [0, K) adds no mass to its row) or, when `labels` is null, fp32
+// probabilities `probs` [B, K].  λ ~ Beta(α, α) = G₁/(G₁ + G₂) from two Gamma(α) draws (Marsaglia–Tsang in double; for α < 1,
+// Gamma(α + 1)·U^(1/α) in logarithms), λ = 1/(1 + exp(log G₂ − log G₁)).  CutMix draws r_x in {0..W−1} and r_y in {0..H−1} and
+// forms torchvision's box (x1, y1, x2, y2) and λ_adj = 1 − (x2 − x1)(y2 − y1)/(W·H) in double; pixels in [y1:y2, x1:x2] come from
+// the partner on every channel.  MixUp gives y = fl(fl(x[i−1]·fp32(1 − λ)) + fl(x[i]·fp32(λ))); the targets take the same formula
+// with λ (MixUp) or λ_adj (CutMix).  record (fp64, nullable): (λ) for MixUp, (λ, r_x, r_y, x1, y1, x2, y2, λ_adj) for CutMix.  One
+// launch of B CTAs (none when B = 0); every CTA draws the batch's parameters itself.
+void launch_mix_batch(const float* x, const long long* labels, const float* probs, float* y, float* q, double* record, int B, int C, int H,
+                      int W, int K, double alpha, bool cutmix, PhiloxSeed rng, cudaStream_t st);
 
 #ifdef __CUDACC__
 // max that keeps a NaN (fmaxf drops it), as torch's inf-norm does

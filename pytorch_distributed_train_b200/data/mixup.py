@@ -20,10 +20,20 @@ def mixup(images: torch.Tensor, labels: torch.Tensor, num_classes: int, alpha: f
     tensors' own device and nothing waits for it: in place, pinned host images stay pinned."""
     if not alpha > 0:
         raise ValueError(f"mixup: alpha must be positive (got {alpha})")
-    # what torch.distributions.Beta(α, α).sample() draws (torchvision's λ), here from the caller's generator: torch.distributions
-    # takes no generator, so the private sampler Beta.sample calls is called directly (test_mixup_cli.py pins the equivalence)
-    lam = float(torch._sample_dirichlet(torch.tensor([alpha, alpha]), generator=generator)[0])
-    rolled = images.roll(1, 0)
-    images.mul_(lam).add_(rolled.mul_(1.0 - lam))
-    onehot = F.one_hot(labels, num_classes).to(torch.float32)
-    return onehot.roll(1, 0).mul_(1.0 - lam).add_(onehot.mul_(lam))
+    lam = draw_lambda(alpha, generator)
+    mix_rows_(images, lam)
+    return mix_rows_(F.one_hot(labels, num_classes).to(torch.float32), lam)
+
+
+def draw_lambda(alpha: float, generator: Optional[torch.Generator] = None) -> float:
+    """λ ~ Beta(α, α) on the host: what torch.distributions.Beta(α, α).sample() draws (torchvision's λ), here from the caller's
+    generator.  torch.distributions takes no generator, so the private sampler Beta.sample calls is called directly
+    (test_mixup_cli.py pins the equivalence)."""
+    return float(torch._sample_dirichlet(torch.tensor([alpha, alpha]), generator=generator)[0])
+
+
+def mix_rows_(t: torch.Tensor, lam: float) -> torch.Tensor:
+    """t ← λ·t + (1 − λ)·t.roll(1, 0) in place, rounded as torchvision's MixUp: fl(fl(t·fp32(λ)) + fl(t.roll(1, 0)·fp32(1 − λ))), with
+    1 − λ formed in double.  Returns t."""
+    rolled = t.roll(1, 0)
+    return t.mul_(lam).add_(rolled.mul_(1.0 - lam))

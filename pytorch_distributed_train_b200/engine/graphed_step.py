@@ -58,6 +58,15 @@ augments with fresh ones.  Its generator, when it is not the device's default on
 with each captured graph, so its ``manual_seed`` between replays takes effect.  The model sees a plain contiguous fp32 batch.  After
 each call, an augmentation's ``last_params`` (``RandomAffine(record_params=True)``) is the replayed graph's, so it holds that step's
 draws.
+
+Batch mixing (``mix``, a callable ``(images, targets) -> (images, targets)`` such as ``pdt.data.CutMix`` or ``pdt.data.MixUp``): every
+step runs ``x, t = mix(x, t)`` after ``augment``; with accumulation, once on all k·b rows before the micro-batches are sliced, as an
+eager loop mixes a loader batch, so the first row of micro-batch i is paired with the last row of micro-batch i − 1.  The mixed fp32
+class probabilities are what ``upcoming_targets`` and the criterion see: the forward kernel's probability-target rider computes the
+loss.  On a CUDA batch ``CutMix`` / ``MixUp`` are one more launch inside the graph that draws λ (and the box) on the device, so every
+replay mixes anew.  The step's example targets stay what the loader delivers (int64 class indices).  Every distinct non-default
+CUDA generator of ``augment`` and ``mix`` is registered with each captured graph, and after each call every transform's
+``last_params`` is the replayed graph's record.
 """
 from __future__ import annotations
 
@@ -77,10 +86,11 @@ class GraphedTrainStep:
     def __init__(self, model, criterion, optimizer, example_inputs: Sequence[torch.Tensor], warmup: int = 3,
                  zero_grad_set_to_none: bool = True, fuse_optimizer: bool = True, double_buffer_inputs: bool = True,
                  max_grad_norm: Optional[float] = None, norm_type: float = 2.0, accumulation_steps: int = 1, averaged_model=None,
-                 augment=None):
+                 augment=None, mix=None):
         if not torch.cuda.is_available():
             raise RuntimeError("GraphedTrainStep needs CUDA")
         self.augment = augment
+        self.mix = mix
         self.averaged_model = averaged_model
         self._averaged_source = getattr(model, "module", model)   # the averaged model was copied from the bare model
         if averaged_model is not None:
@@ -161,6 +171,8 @@ class GraphedTrainStep:
 
         if self.augment is not None:
             inputs = [self.augment(inputs[0])] + list(inputs[1:])   # all k·b rows at once under accumulation
+        if self.mix is not None:
+            inputs = list(self.mix(inputs[0], inputs[1])) + list(inputs[2:])   # likewise, before the micro-batches are sliced
         if self.accumulation_steps > 1:
             return self._finish_step(self._accumulate(inputs))
 
@@ -286,15 +298,14 @@ class GraphedTrainStep:
         comm = getattr(self.model, "comm", None)
         parity = (lambda: list(comm.parity_state())) if hasattr(comm, "parity_state") else (lambda: [])
         self.graphs, self.losses, self.norms = [], [], []
-        self._augment_params = []   # the static parameter record of each graph's augmentation (RandomAffine(record_params=True))
+        transforms = [t for t in (self.augment, self.mix) if t is not None]
+        self._records = []   # per graph: (transform, its static parameter record) for each transform that records (record_params=True)
         p0 = parity()
         for k in range(2):
             if self._riding and self.max_grad_norm is not None:
                 self._ride(k)   # each graph's rider stores the norm in its own scalar
             g = torch.cuda.CUDAGraph()
-            gen = getattr(self.augment, "generator", None)
-            if (isinstance(gen, torch.Generator) and gen.device.type == "cuda"
-                    and gen is not torch.cuda.default_generators[gen.device.index if gen.device.index is not None else torch.cuda.current_device()]):
+            for gen in _own_cuda_generators(transforms):
                 # the capture registers the default generator itself; any other one that the step draws from must be registered, so
                 # that each replay advances its offset (and its manual_seed reaches the graph)
                 g.register_generator_state(gen)
@@ -308,7 +319,7 @@ class GraphedTrainStep:
             self.graphs.append(g)
             self.losses.append(loss)
             self.norms.append(norm)
-            self._augment_params.append(getattr(self.augment, "last_params", None))
+            self._records.append([(t, t.last_params) for t in transforms if getattr(t, "last_params", None) is not None])
             torch.cuda.synchronize(dev)
             ordered = getattr(self.model, "syncs_buffers_every_step", None)
             if not self.double_buffer and (parity() == p0 or (ordered is not None and ordered())):
@@ -337,8 +348,8 @@ class GraphedTrainStep:
         self._last = i
         self.static_loss = self.losses[i]
         self.grad_norm = self.norms[i]
-        if self._augment_params[i] is not None:
-            self.augment.last_params = self._augment_params[i]   # the draws of this replay, not of the graph captured last
+        for t, record in self._records[i]:
+            t.last_params = record   # the draws of this replay, not of the graph captured last
         return self.static_loss
 
     def loss_to_host(self) -> "HostLoss":
@@ -347,6 +358,19 @@ class GraphedTrainStep:
         replay is not held up by the copy — call it every step and read the handles you want to log whenever convenient
         (reading a handle *after* the next step has been enqueued keeps the device busy while the host waits)."""
         return HostLoss(self._io, self._io.loss_to_host(self._last, self.static_loss))
+
+
+def _own_cuda_generators(transforms):
+    """The distinct CUDA generators the transforms draw from, other than their device's default one."""
+    out = []
+    for t in transforms:
+        gen = getattr(t, "generator", None)
+        if not (isinstance(gen, torch.Generator) and gen.device.type == "cuda"):
+            continue
+        index = gen.device.index if gen.device.index is not None else torch.cuda.current_device()
+        if gen is not torch.cuda.default_generators[index] and all(gen is not o for o in out):
+            out.append(gen)
+    return out
 
 
 class HostLoss:

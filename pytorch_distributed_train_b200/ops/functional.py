@@ -723,6 +723,18 @@ def random_affine(x: torch.Tensor, degrees, translate=None, scale=None, shear=No
                             bool(bilinear), float(fill), generator, bool(record_params))
 
 
+def mix_batch(x: torch.Tensor, targets: torch.Tensor, num_classes: Optional[int], alpha: float, cutmix: bool,
+              generator: Optional[torch.Generator] = None, record_params: bool = False):
+    """torchvision's ``MixUp`` (``cutmix=False``) or ``CutMix`` on ``x`` (fp32 contiguous CUDA ``[B, C, H, W]``), image i paired with
+    image i − 1, with λ ~ Beta(α, α) (and the box) drawn on the device from ``generator``'s Philox state (the device's default CUDA
+    generator when None): one launch, graph-capturable, every replay drawing new values.  ``targets`` are int64 class indices ``[B]``
+    (one-hot over ``num_classes``; an index outside [0, num_classes) adds no mass to its row) or fp32 probabilities ``[B, K]``.
+    Returns ``(images, fp32 targets [B, K], record)``: ``record`` is fp64 (λ) for MixUp, (λ, r_x, r_y, x1, y1, x2, y2, λ_adj) for
+    CutMix, with ``record_params``, else None.  ``pdt.data.MixUp`` and ``pdt.data.CutMix`` are the user-facing transforms."""
+    return _C.mix_batch(x, targets, -1 if num_classes is None else int(num_classes), float(alpha), bool(cutmix), generator,
+                        bool(record_params))
+
+
 # ---- generic (NCHW) BatchNorm pieces used by parallel.SyncBatchNorm ------------------------------------------
 def bn_local_stats(x: torch.Tensor) -> torch.Tensor:
     """float64 [2C+2] = per-channel Σx, Σx² (accumulated in fp64), the per-channel element count, one zero pad."""

@@ -34,6 +34,7 @@ GROUPS = {
     "input_grads": ["tests/test_convnet_input_grads.py"],
     "symm_emu": ["tests/test_symm_kernels_emulated.py"],
     "random_affine": ["tests/test_random_affine.py"],
+    "mix": ["tests/test_mix.py"],
 }
 
 
