@@ -10,7 +10,7 @@ Extra flags cover what the reference hard-codes: ``--init-method`` (its LAN addr
 to loopback with a free port), ``--data synthetic|mnist``, ``--model``, ``--comm fused|nccl``, ``--algo``,
 ``--steps``, ``--graph`` (whole-step CUDA graph), ``--batch-size``, ``--optimizer`` (sgd | adam | adamw | nadam | radam | rmsprop |
 adagrad | adamax | adadelta | asgd | rprop), ``--lr``, ``--momentum``, ``--amsgrad``, ``--weight-decay``, ``--clip-grad-norm``, ``--accumulation-steps``, ``--label-smoothing``, ``--mixup``,
-``--cutmix`` (CutMix drawn on the device, inside the captured step with ``--graph``), ``--rotate`` / ``--translate`` / ``--scale-range`` / ``--shear`` / ``--affine-interpolation`` (per-image random affine augmentation), ``--ema-decay``, ``--checkpoint`` / ``--resume``, ``--eval`` (test loss and accuracy after every epoch).
+``--cutmix`` (CutMix drawn on the device, inside the captured step with ``--graph``), ``--rotate`` / ``--translate`` / ``--scale-range`` / ``--shear`` / ``--affine-interpolation`` (per-image random affine augmentation), ``--elastic-alpha`` / ``--elastic-sigma`` (per-image elastic deformation, after the affine), ``--ema-decay``, ``--checkpoint`` / ``--resume``, ``--eval`` (test loss and accuracy after every epoch).
 """
 from __future__ import annotations
 
@@ -81,6 +81,11 @@ def build_parser() -> argparse.ArgumentParser:
                    help="random affine augmentation: shear every training image along x by an angle ~ U[-DEG, DEG) (default: off)")
     p.add_argument("--affine-interpolation", default="nearest", choices=["nearest", "bilinear"],
                    help="resampling of the random affine augmentation (default: nearest, torchvision's)")
+    p.add_argument("--elastic-alpha", default=None, type=float, metavar="A",
+                   help="elastic deformation (torchvision's ElasticTransform, bilinear): displace every training image by its own "
+                        "smoothed random field of magnitude A, after the random affine augmentation (default: off)")
+    p.add_argument("--elastic-sigma", default=None, type=float, metavar="S",
+                   help="smoothness of the --elastic-alpha field: the sigma of its Gaussian blur (default 5.0, torchvision's)")
     p.add_argument("--ema-decay", default=None, type=float, metavar="D",
                    help="keep an exponential moving average of the weights and buffers with decay D in [0, 1], updated after every "
                         "optimizer step and saved with --checkpoint (default: off)")
@@ -141,6 +146,16 @@ def make_augment(args, generator):
                               interpolation=args.affine_interpolation, generator=generator)
 
 
+def make_elastic(args, generator):
+    """The per-image elastic deformation ``--elastic-alpha`` / ``--elastic-sigma`` describe, or None."""
+    if getattr(args, "elastic_alpha", None) is None:
+        return None
+    from pytorch_distributed_train_b200 import data as pdata
+
+    sigma = 5.0 if args.elastic_sigma is None else args.elastic_sigma
+    return pdata.ElasticTransform(alpha=args.elastic_alpha, sigma=sigma, generator=generator)
+
+
 def check_args(p: argparse.ArgumentParser, args) -> None:
     if args.optimizer != "sgd" and args.momentum is not None:
         why = {"rmsprop": "RMSprop's momentum is a library option (pdt.optim.RMSprop(..., momentum=...))",
@@ -170,6 +185,12 @@ def check_args(p: argparse.ArgumentParser, args) -> None:
     if args.mixup is not None and affine_requested(args):
         p.error("--mixup cannot be combined with --rotate, --translate, --scale-range or --shear: MixUp mixes on the host before the "
                 "batch reaches the device, where the affine would warp the mixed image with one parameter set")
+    elastic_alpha, elastic_sigma = getattr(args, "elastic_alpha", None), getattr(args, "elastic_sigma", None)
+    if elastic_sigma is not None and elastic_alpha is None:
+        p.error("--elastic-sigma needs --elastic-alpha, which turns the elastic deformation on")
+    if elastic_alpha is not None and args.mixup is not None:
+        p.error("--mixup cannot be combined with --elastic-alpha: MixUp mixes on the host before the batch reaches the device, where "
+                "the elastic deformation would warp the mixed image with one field")
     cutmix = getattr(args, "cutmix", None)
     if cutmix is not None and not cutmix > 0:
         p.error(f"--cutmix must be positive (got {cutmix})")
@@ -250,8 +271,11 @@ def dist_train(gpu: int, args) -> None:
         mix_gen = torch.Generator()
 
     # every training image warped with its own parameters, on the batch's device after its copy (inside the captured step with
-    # --graph); each rank draws from its own generator, seeded per epoch below
-    augment = make_augment(args, torch.Generator(device=device))
+    # --graph): the affine, then the elastic deformation.  Each rank draws both from one generator of its own, seeded per epoch
+    # below; the affine's launch advances its offset before the elastic one draws (two generators seeded alike would repeat the
+    # same Philox values).
+    augment_gen = torch.Generator(device=device)
+    augments = [t for t in (make_augment(args, augment_gen), make_elastic(args, augment_gen)) if t is not None]
     # CutMix on the batch's device after the copy and the affine (inside the captured step with --graph); its own generator per rank,
     # seeded per epoch below
     cutmix = None
@@ -266,8 +290,8 @@ def dist_train(gpu: int, args) -> None:
         example_targets = (torch.zeros(rows, dtype=torch.int64, device=device) if mix_gen is None else
                            torch.zeros(rows, num_classes, device=device))
         step_fn = GraphedTrainStep(model, criterion, optimizer, example_inputs=(torch.zeros((rows,) + shape, device=device), example_targets),
-                                   max_grad_norm=args.clip_grad_norm, accumulation_steps=accum, averaged_model=ema, augment=augment,
-                                   mix=cutmix)
+                                   max_grad_norm=args.clip_grad_norm, accumulation_steps=accum, averaged_model=ema,
+                                   augment=augments or None, mix=cutmix)
 
     first_epoch = 0
     if args.resume:
@@ -284,8 +308,8 @@ def dist_train(gpu: int, args) -> None:
         if mix_gen is not None:
             # from (epoch, rank): a run resumed from an epoch's checkpoint draws the λ sequence of an uninterrupted run
             mix_gen.manual_seed(epoch * args.world_size + rank)
-        if augment is not None:
-            augment.generator.manual_seed(epoch * args.world_size + rank)   # as MixUp's: a resumed run draws what an uninterrupted one does
+        if augments:
+            augment_gen.manual_seed(epoch * args.world_size + rank)   # as MixUp's: a resumed run draws what an uninterrupted one does
         if cutmix is not None:
             cutmix.generator.manual_seed(epoch * args.world_size + rank)
         pending = None   # (step index, loss handle) of a log line whose value is still on its way to the host
@@ -306,8 +330,8 @@ def dist_train(gpu: int, args) -> None:
             else:
                 images = images.to(device, non_blocking=True)
                 labels = labels.to(device, non_blocking=True)
-                if augment is not None:
-                    images = augment(images)
+                for t in augments:
+                    images = t(images)
                 if cutmix is not None:
                     images, labels = cutmix(images, labels)   # the whole loader batch, as the graphed step mixes it
                 optimizer.zero_grad()

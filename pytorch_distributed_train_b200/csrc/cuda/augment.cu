@@ -4,11 +4,18 @@
 // and samples all channels there.
 // Batch-level MixUp and CutMix (torchvision's v2 transforms), one launch: one CTA per image, each drawing the batch's λ (and box)
 // from the same Philox values, then mixing its image with its roll-by-one partner and writing its target row.
+// Per-image elastic deformation (torchvision's v2.ElasticTransform, every image with its own field), one launch: one CTA per image
+// holds the image's two noise planes and one scratch plane in shared memory (12 B per pixel), draws the noise, blurs it
+// separably and warps the image with the shared sampler.  Philox layout: the noise value of pixel p (p = 4q + e, e in 0..3) of
+// plane c (0: dx0, 1: dy0) of image b is component e of the one curand_uniform4 drawn from subsequence (2b + c)·⌈HW/4⌉ + q at
+// the launch's offset, so no two images, planes or pixels share a value, and each subsequence consumes 4 values: the launch's
+// offset increment (kElasticOffsetIncrement).
 #include <cuda_runtime.h>
 #include <curand_kernel.h>
 
 #include <algorithm>
 #include <stdexcept>
+#include <string>
 
 #include "cuda_utils.h"
 #include "ops_kernels.h"
@@ -33,6 +40,44 @@ __device__ __forceinline__ void philox_init(const PhiloxSeed& rng, unsigned long
 
 // torch's CUDA uniform_: curand's (0, 1] with 1 mapped to 0, then u·range + from in fp32: U[from, to)
 __device__ __forceinline__ float draw(float r, float from, float range) { return (r == 1.f ? 0.f : r) * range + from; }
+
+// Output pixel p of every channel of one image (src, dst: its first plane, C planes of H·W) from the source coordinate (sx, sy):
+// grid_sample(align_corners=False, padding_mode="zeros") unnormalised.  Nearest rounds half to even and writes `fill` outside the
+// image; bilinear reads 0 outside and returns torchvision's (v − fill)·mask + fill.
+__device__ __forceinline__ void sample_pixel(const float* __restrict__ src, float* __restrict__ dst, int C, int H, int W, int p,
+                                             double sxp, double syp, int bilinear, float fill) {
+  const int hw = H * W;
+  if (!bilinear) {
+    const double rx = rint(sxp), ry = rint(syp);   // ties to even, as grid_sample's nearbyint
+    const bool in = rx >= 0.0 && rx <= W - 1 && ry >= 0.0 && ry <= H - 1;   // false for NaN
+    const int o = in ? static_cast<int>(ry) * W + static_cast<int>(rx) : 0;
+    for (int ci = 0; ci < C; ++ci) dst[ci * hw + p] = in ? __ldg(src + ci * hw + o) : fill;
+    return;
+  }
+  const double x0 = floor(sxp), y0 = floor(syp);
+  const double fx = sxp - x0, fy = syp - y0;
+  const bool vx0 = x0 >= 0.0 && x0 <= W - 1, vx1 = x0 >= -1.0 && x0 <= W - 2;
+  const bool vy0 = y0 >= 0.0 && y0 <= H - 1, vy1 = y0 >= -1.0 && y0 <= H - 2;
+  // taps nw, ne, sw, se; out-of-bounds taps read 0 and add nothing to the mask
+  const bool v[4] = {vx0 && vy0, vx1 && vy0, vx0 && vy1, vx1 && vy1};
+  const float w[4] = {static_cast<float>((1.0 - fx) * (1.0 - fy)), static_cast<float>(fx * (1.0 - fy)),
+                      static_cast<float>((1.0 - fx) * fy), static_cast<float>(fx * fy)};
+  int o[4];
+  const int ix = vx0 || vx1 ? static_cast<int>(x0) : 0, iy = vy0 || vy1 ? static_cast<int>(y0) : 0;
+  o[0] = iy * W + ix, o[1] = o[0] + 1, o[2] = o[0] + W, o[3] = o[0] + W + 1;
+  float mask = 0.f;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) mask += v[k] ? w[k] : 0.f;
+  for (int ci = 0; ci < C; ++ci) {
+    const float* __restrict__ plane = src + ci * hw;
+    float acc = 0.f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (v[k]) acc += w[k] * __ldg(plane + o[k]);
+    // torchvision's fill: (img − fill)·mask + fill, the mask being grid_sample's bilinear weight of the in-bounds taps
+    dst[ci * hw + p] = (acc - fill) * mask + fill;
+  }
+}
 
 __global__ void __launch_bounds__(kAffineMaxThreads) random_affine_kernel(const float* __restrict__ x, float* __restrict__ y,
                                                                         float* __restrict__ params, int C, int H, int W, AffineSpec s,
@@ -77,38 +122,74 @@ __global__ void __launch_bounds__(kAffineMaxThreads) random_affine_kernel(const 
     const int i = p / W, j = p - (p / W) * W;
     // the source coordinate of output pixel (i, j): torchvision's _affine_grid + grid_sample(align_corners=False), unnormalised
     const double xj = j - cw, yi = i - ch;
-    const double sxp = m0 * xj + m1 * yi + m2 + cw;
-    const double syp = m3 * xj + m4 * yi + m5 + ch;
-    if (!s.bilinear) {
-      const double rx = rint(sxp), ry = rint(syp);   // ties to even, as grid_sample's nearbyint
-      const bool in = rx >= 0.0 && rx <= W - 1 && ry >= 0.0 && ry <= H - 1;   // false for NaN
-      const int o = in ? static_cast<int>(ry) * W + static_cast<int>(rx) : 0;
-      for (int ci = 0; ci < C; ++ci) dst[ci * hw + p] = in ? __ldg(src + ci * hw + o) : fill;
-      continue;
+    sample_pixel(src, dst, C, H, W, p, m0 * xj + m1 * yi + m2 + cw, m3 * xj + m4 * yi + m5 + ch, s.bilinear, fill);
+  }
+}
+
+// one thread per pixel up to 1024, as random_affine_kernel
+constexpr int kElasticMaxThreads = 1024;
+
+// torch's reflect padding of an index in [−(n − 1), 2(n − 1)]
+__device__ __forceinline__ int reflect(int i, int n) { return i < 0 ? -i : (i > n - 1 ? 2 * (n - 1) - i : i); }
+
+// out = blur(in) with weights w (k taps, centred) along x (step 1, extent W) or y (step W, extent H), in fp32
+__device__ __forceinline__ void blur_pass(const float* in, float* out, const float* __restrict__ w, int k, int H, int W, bool along_x) {
+  const int r = k / 2;
+  for (int p = threadIdx.x; p < H * W; p += blockDim.x) {
+    const int i = p / W, j = p - i * W;
+    float acc = 0.f;
+    if (along_x) {
+      for (int t = 0; t < k; ++t) acc += __ldg(w + t) * in[i * W + reflect(j + t - r, W)];
+    } else {
+      for (int t = 0; t < k; ++t) acc += __ldg(w + t) * in[reflect(i + t - r, H) * W + j];
     }
-    const double x0 = floor(sxp), y0 = floor(syp);
-    const double fx = sxp - x0, fy = syp - y0;
-    const bool vx0 = x0 >= 0.0 && x0 <= W - 1, vx1 = x0 >= -1.0 && x0 <= W - 2;
-    const bool vy0 = y0 >= 0.0 && y0 <= H - 1, vy1 = y0 >= -1.0 && y0 <= H - 2;
-    // taps nw, ne, sw, se; out-of-bounds taps read 0 and add nothing to the mask
-    const bool v[4] = {vx0 && vy0, vx1 && vy0, vx0 && vy1, vx1 && vy1};
-    const float w[4] = {static_cast<float>((1.0 - fx) * (1.0 - fy)), static_cast<float>(fx * (1.0 - fy)),
-                        static_cast<float>((1.0 - fx) * fy), static_cast<float>(fx * fy)};
-    int o[4];
-    const int ix = vx0 || vx1 ? static_cast<int>(x0) : 0, iy = vy0 || vy1 ? static_cast<int>(y0) : 0;
-    o[0] = iy * W + ix, o[1] = o[0] + 1, o[2] = o[0] + W, o[3] = o[0] + W + 1;
-    float mask = 0.f;
+    out[p] = acc;
+  }
+}
+
+// One CTA per image b: draws the two noise planes into shared memory (and into noise[b] when recording), blurs each (x pass into
+// the scratch plane, y pass back), scales it to the displacement and warps all channels of the image through it.
+__global__ void __launch_bounds__(kElasticMaxThreads) elastic_kernel(const float* __restrict__ x, float* __restrict__ y,
+                                                                     float* __restrict__ noise, int C, int H, int W, ElasticSpec s,
+                                                                     PhiloxSeed rng) {
+  extern __shared__ float sm[];   // dx plane, dy plane, scratch: 3·H·W
+  const int b = blockIdx.x;
+  const int hw = H * W, groups = (hw + 3) / 4;
+  for (int g = threadIdx.x; g < 2 * groups; g += blockDim.x) {
+    const int c = g < groups ? 0 : 1, q = g - c * groups;
+    curandStatePhilox4_32_10_t st;
+    philox_init(rng, (2ull * b + c) * groups + q, &st);
+    const float4 r = curand_uniform4(&st);
+    const float v[4] = {draw(r.x, -1.f, 2.f), draw(r.y, -1.f, 2.f), draw(r.z, -1.f, 2.f), draw(r.w, -1.f, 2.f)};   // torch.rand·2 − 1
 #pragma unroll
-    for (int k = 0; k < 4; ++k) mask += v[k] ? w[k] : 0.f;
-    for (int ci = 0; ci < C; ++ci) {
-      const float* __restrict__ plane = src + ci * hw;
-      float acc = 0.f;
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        if (v[k]) acc += w[k] * __ldg(plane + o[k]);
-      // torchvision's fill: (img − fill)·mask + fill, the mask being grid_sample's bilinear weight of the in-bounds taps
-      dst[ci * hw + p] = (acc - fill) * mask + fill;
+    for (int e = 0; e < 4; ++e) {
+      const int p = 4 * q + e;
+      if (p >= hw) break;
+      sm[c * hw + p] = v[e];
+      if (noise != nullptr) noise[(2ll * b + c) * hw + p] = v[e];
     }
+  }
+  __syncthreads();
+  float* tmp = sm + 2 * hw;
+  const float* w = s.weights;
+  for (int c = 0; c < 2; ++c) {
+    const int k = s.k[c];
+    if (k == 0) continue;   // the same for the whole CTA
+    // plane c: x weights (k, sigma[0]), then y weights (k, sigma[1])
+    blur_pass(sm + c * hw, tmp, w, k, H, W, true);
+    __syncthreads();
+    blur_pass(tmp, sm + c * hw, w + k, k, H, W, false);
+    __syncthreads();
+    w += 2 * k;
+  }
+  const float* __restrict__ src = x + static_cast<long long>(b) * C * hw;
+  float* __restrict__ dst = y + static_cast<long long>(b) * C * hw;
+  const float fw = static_cast<float>(W), fh = static_cast<float>(H);
+  for (int p = threadIdx.x; p < hw; p += blockDim.x) {
+    const int i = p / W, j = p - i * W;
+    // torchvision's dx = blurred · alpha[0] / W in fp32 (dy likewise with H); the grid's identity plus displacement, unnormalised
+    const float dx = __fdiv_rn(__fmul_rn(sm[p], s.alpha_x), fw), dy = __fdiv_rn(__fmul_rn(sm[hw + p], s.alpha_y), fh);
+    sample_pixel(src, dst, C, H, W, p, j + 0.5 * W * static_cast<double>(dx), i + 0.5 * H * static_cast<double>(dy), s.bilinear, s.fill);
   }
 }
 
@@ -221,6 +302,33 @@ void launch_mix_batch(const float* x, const long long* labels, const float* prob
   if (B == 0) return;
   mix_batch_kernel<<<B, kMixThreads, 0, st>>>(x, labels, probs, y, q, record, B, C, H, W, K, alpha, cutmix ? 1 : 0, rng);
   check_launch("mix_batch");
+}
+
+size_t elastic_smem_bytes(int H, int W) { return 3 * sizeof(float) * static_cast<size_t>(H) * W; }
+
+void check_elastic_size(int H, int W) {
+  if (H < 1 || W < 1) throw std::invalid_argument("elastic: bad shape");
+  const size_t need = elastic_smem_bytes(H, W), limit = smem_optin_limit();
+  if (need > limit)
+    throw std::invalid_argument("elastic: a " + std::to_string(H) + "x" + std::to_string(W) + " image needs " + std::to_string(need) +
+                                " bytes of shared memory (12 per pixel), above the device's opt-in limit of " + std::to_string(limit) +
+                                " bytes per block");
+}
+
+void launch_elastic(const float* x, float* y, float* noise, int B, int C, int H, int W, const ElasticSpec& s, PhiloxSeed rng,
+                    cudaStream_t st) {
+  if (B < 0 || C < 1) throw std::invalid_argument("elastic: bad shape");
+  if (static_cast<long long>(C) * H * W >= (1LL << 31)) throw std::invalid_argument("elastic: an image must have fewer than 2^31 elements");
+  check_elastic_size(H, W);
+  for (int c = 0; c < 2; ++c)
+    if (s.k[c] != 0 && (s.k[c] < 1 || s.k[c] % 2 == 0 || s.k[c] / 2 >= H || s.k[c] / 2 >= W))
+      throw std::invalid_argument("elastic: the blur needs an odd kernel size whose half is below the image's height and width");
+  if (B == 0) return;
+  const size_t smem = elastic_smem_bytes(H, W);
+  opt_in_smem(elastic_kernel, smem);
+  const int threads = static_cast<int>(std::min<long long>(kElasticMaxThreads, (static_cast<long long>(H) * W + 31) / 32 * 32));
+  elastic_kernel<<<B, threads, smem, st>>>(x, y, noise, C, H, W, s, rng);
+  check_launch("elastic");
 }
 
 }  // namespace pdt

@@ -1496,6 +1496,40 @@ void register_cuda_bindings(py::module_& m) {
     return py::make_tuple(y, record_params ? py::cast(params) : py::none());
   }, py::arg("x"), py::arg("degrees"), py::arg("translate"), py::arg("scale"), py::arg("shear"), py::arg("bilinear"), py::arg("fill"),
      py::arg("generator"), py::arg("record_params"));
+  // Elastic deformation (torchvision's v2.ElasticTransform per image): x fp32 [B, C, H, W] → a new tensor of the same shape, and the
+  // fp32 [B, 2, H, W] noise (dx0, dy0 before the blur) when record_params.  weights: the fp32 1-D blur weights on x's device
+  // (ElasticSpec's layout; ignored when kx = ky = 0).  The noise is drawn from `generator` as random_affine draws.  A size whose
+  // planes exceed the device's opt-in shared memory raises ValueError before anything is drawn.
+  m.def("elastic", [](const at::Tensor& x, const c10::optional<at::Tensor>& weights, int64_t kx, int64_t ky, double alpha_x,
+                      double alpha_y, bool bilinear, double fill, c10::optional<at::Generator> generator, bool record_params) {
+    chk(x, "x");
+    TORCH_CHECK(x.dim() == 4, "elastic: x must be [B, C, H, W] (got ", x.dim(), " dimensions)");
+    TORCH_CHECK(kx >= 0 && ky >= 0 && kx < (1 << 20) && ky < (1 << 20), "elastic: bad kernel sizes");
+    c10::cuda::CUDAGuard g(x.device());
+    const int B = static_cast<int>(x.size(0)), C = static_cast<int>(x.size(1)), H = static_cast<int>(x.size(2)), W = static_cast<int>(x.size(3));
+    ElasticSpec s{};
+    s.k[0] = static_cast<int>(kx), s.k[1] = static_cast<int>(ky);
+    if (kx > 0 || ky > 0) {
+      TORCH_CHECK(weights.has_value() && weights->defined(), "elastic: a blur needs its weights");
+      chk(*weights, "weights");
+      TORCH_CHECK(weights->device() == x.device(), "elastic: weights are on ", weights->device(), ", x on ", x.device());
+      TORCH_CHECK(weights->numel() == 2 * (kx + ky), "elastic: ", weights->numel(), " weights for kernel sizes ", kx, " and ", ky);
+      s.weights = weights->data_ptr<float>();
+    }
+    s.alpha_x = static_cast<float>(alpha_x), s.alpha_y = static_cast<float>(alpha_y);
+    s.fill = static_cast<float>(fill);
+    s.bilinear = bilinear ? 1 : 0;
+    check_elastic_size(H, W);
+    auto y = at::empty_like(x);
+    at::Tensor noise;
+    if (record_params) noise = at::empty({x.size(0), 2, x.size(2), x.size(3)}, x.options());
+    if (B == 0) return py::make_tuple(y, record_params ? py::cast(noise) : py::none());
+    const PhiloxSeed rng = philox_seed(generator, x, kElasticOffsetIncrement, "elastic");
+    launch_elastic(x.data_ptr<float>(), y.data_ptr<float>(), record_params ? noise.data_ptr<float>() : nullptr, B, C, H, W, s, rng,
+                   cur_stream(x));
+    return py::make_tuple(y, record_params ? py::cast(noise) : py::none());
+  }, py::arg("x"), py::arg("weights"), py::arg("kx"), py::arg("ky"), py::arg("alpha_x"), py::arg("alpha_y"), py::arg("bilinear"),
+     py::arg("fill"), py::arg("generator"), py::arg("record_params"));
   // Batch MixUp / CutMix (torchvision's v2 transforms): x fp32 [B, C, H, W] and targets (int64 class indices [B] over num_classes,
   // or fp32 probabilities [B, K]) → (a new image tensor, fp32 targets [B, K], the fp64 parameter record or None).  λ (and the box)
   // are drawn on the device from `generator`, as random_affine draws.

@@ -73,17 +73,28 @@ void check_launch(const char* what) {
   count_kernel_launch();
 }
 
-int sm_count() {
-  constexpr int kMaxDevices = 64;
-  static std::atomic<int> cached[kMaxDevices];   // 0 = not queried yet
+constexpr int kMaxDevices = 64;
+
+// attribute `attr` of the current device, queried once per device into cached[device] (0 = not queried yet)
+static int cached_attribute(cudaDeviceAttr attr, std::atomic<int>* cached) {
   int dev = 0;
   PDT_CUDA_CHECK(cudaGetDevice(&dev));
   int n = dev < kMaxDevices ? cached[dev].load(std::memory_order_relaxed) : 0;
   if (n == 0) {
-    PDT_CUDA_CHECK(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
+    PDT_CUDA_CHECK(cudaDeviceGetAttribute(&n, attr, dev));
     if (dev < kMaxDevices) cached[dev].store(n, std::memory_order_relaxed);
   }
   return n;
+}
+
+int sm_count() {
+  static std::atomic<int> cached[kMaxDevices];
+  return cached_attribute(cudaDevAttrMultiProcessorCount, cached);
+}
+
+size_t smem_optin_limit() {
+  static std::atomic<int> cached[kMaxDevices];
+  return static_cast<size_t>(cached_attribute(cudaDevAttrMaxSharedMemoryPerBlockOptin, cached));
 }
 
 std::string cu_error(CUresult r) {

@@ -72,6 +72,8 @@ void check_launch(const char* what);
 
 // Multiprocessor count of the current device (queried once per device).
 int sm_count();
+// Dynamic shared memory one block of the current device may opt in to (queried once per device): the bound of opt_in_smem.
+size_t smem_optin_limit();
 
 // Kernels that use more than the default 48 KB of dynamic shared memory must opt in first.
 template <typename K>

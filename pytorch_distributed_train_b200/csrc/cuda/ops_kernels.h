@@ -404,6 +404,29 @@ constexpr int kAffineOffsetIncrement = 8;
 // (v − fill)·mask + fill, mask being the bilinear weight of the in-bounds taps.  One launch (none when B = 0).
 void launch_random_affine(const float* x, float* y, float* params, int B, int C, int H, int W, const AffineSpec& s, PhiloxSeed rng,
                           cudaStream_t st);
+// The blur weights and scales of one elastic launch.  weights (device, fp32): for dx, the k[0] x weights (kernel size k[0], sigma[0])
+// then its k[0] y weights (k[0], sigma[1]); then the same for dy with k[1]; k[c] = 0: plane c is not blurred.
+struct ElasticSpec {
+  const float* weights;
+  int k[2];
+  float alpha_x, alpha_y;   // fp32(alpha[0]), fp32(alpha[1])
+  float fill;
+  int bilinear;   // 0: nearest
+};
+// Philox values each subsequence of an elastic launch consumes (one curand_uniform4): the generator's offset increment per launch
+constexpr int kElasticOffsetIncrement = 4;
+// Shared memory of one elastic CTA: the dx and dy noise planes and one scratch plane, fp32.
+size_t elastic_smem_bytes(int H, int W);
+// Throws std::invalid_argument (naming the limit) unless an H×W image's planes fit the current device's opt-in shared memory.
+void check_elastic_size(int H, int W);
+// torchvision's v2.ElasticTransform applied to each image of x [B, C, H, W] (fp32 contiguous NCHW) with its own field, into y of
+// the same shape.  Image b draws dx0, dy0 ~ U[-1, 1) over H×W (torch.rand·2 − 1; Philox layout in augment.cu) and stores them in
+// noise[b, 0:2] (fp32 [B, 2, H, W], nullable).  Plane c with k[c] > 0 is blurred separably in fp32 with reflect indexing (x pass,
+// then y pass); then dx = fl(fl(blurred_dx · alpha_x) / W), dy = fl(fl(blurred_dy · alpha_y) / H), and output pixel (i, j)
+// samples the source at (j + dx·W/2, i + dy·H/2) in double with random_affine's sampling (nearest: ties to even, `fill` outside;
+// bilinear: (v − fill)·mask + fill).  Every channel shares the image's field.  One launch of B CTAs (none when B = 0).
+void launch_elastic(const float* x, float* y, float* noise, int B, int C, int H, int W, const ElasticSpec& s, PhiloxSeed rng,
+                    cudaStream_t st);
 // Attempts each Gamma draw of mix_batch_kernel may make before it gives up (Marsaglia–Tsang rejects at most 4.9% of attempts for a
 // shape ≥ 1, so a draw reaches the cap with probability below 0.049^16 ≈ 1e-21)
 constexpr int kGammaMaxAttempts = 16;

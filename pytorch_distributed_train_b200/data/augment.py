@@ -140,6 +140,14 @@ def _random_affine_cpu(x, degrees, translate, scale, shear, bilinear, fill, gene
     col = lambda v: v.view(B, 1, 1)   # noqa: E731
     src_x = col(m0) * xj + col(m1) * yi + col(m2) + cw
     src_y = col(m3) * xj + col(m4) * yi + col(m5) + ch
+    return _sample_cpu(x, src_x, src_y, bilinear, fill), params
+
+
+def _sample_cpu(x, src_x, src_y, bilinear, fill):
+    """Every channel of x [B, C, H, W] sampled at the float64 source coordinates src_x, src_y [B, H, W]: grid_sample
+    (align_corners=False, padding_mode="zeros") unnormalised; nearest rounds half to even and takes ``fill`` outside the image,
+    bilinear (in float64) returns torchvision's (v − fill)·mask + fill."""
+    B, C, H, W = x.shape
     flat = x.reshape(B, C, H * W)
 
     def tap(ix, iy):
@@ -151,7 +159,7 @@ def _random_affine_cpu(x, degrees, translate, scale, shear, bilinear, fill, gene
 
     if not bilinear:
         inside, v = tap(torch.round(src_x), torch.round(src_y))
-        return torch.where(inside.unsqueeze(1), v, torch.tensor(fill, dtype=x.dtype)), params
+        return torch.where(inside.unsqueeze(1), v, torch.tensor(fill, dtype=x.dtype))
     x0, y0 = torch.floor(src_x), torch.floor(src_y)
     fx, fy = src_x - x0, src_y - y0
     acc = torch.zeros(B, C, H, W, dtype=torch.float64)
@@ -161,4 +169,4 @@ def _random_affine_cpu(x, degrees, translate, scale, shear, bilinear, fill, gene
         w = torch.where(inside, w, 0)
         acc += w.unsqueeze(1) * v.double()
         mask += w
-    return ((acc - fill) * mask.unsqueeze(1) + fill).to(x.dtype), params
+    return ((acc - fill) * mask.unsqueeze(1) + fill).to(x.dtype)

@@ -51,13 +51,14 @@ kernel was measured slower than this launch: DESIGN.md §7.)  torch's own update
 cannot be captured, so an averaged model that would take it is refused.  The warm-up steps the constructor runs are not
 averaged.
 
-Augmentation (``augment``, a callable on the image batch such as ``pdt.data.RandomAffine``): every step runs
-``x = augment(inputs[0])`` before the model; with accumulation, once on all k·b rows before the micro-batches are sliced.  A
-``RandomAffine`` on a CUDA batch is one more launch inside the graph that draws its parameters on the device, so every replay
-augments with fresh ones.  Its generator, when it is not the device's default one (which every capture registers), is registered
-with each captured graph, so its ``manual_seed`` between replays takes effect.  The model sees a plain contiguous fp32 batch.  After
-each call, an augmentation's ``last_params`` (``RandomAffine(record_params=True)``) is the replayed graph's, so it holds that step's
-draws.
+Augmentation (``augment``, a callable on the image batch such as ``pdt.data.RandomAffine`` or ``pdt.data.ElasticTransform``, or a
+list or tuple of them applied in order, such as an affine warp followed by an elastic one): every step runs ``x = augment(inputs[0])``
+(each transform in turn) before the model; with accumulation, once on all k·b rows before the micro-batches are sliced.  A
+``RandomAffine`` or ``ElasticTransform`` on a CUDA batch is one more launch inside the graph that draws its parameters on the device,
+so every replay augments with fresh ones.  Every generator of the transforms, when it is not the device's default one (which every
+capture registers), is registered with each captured graph, so its ``manual_seed`` between replays takes effect.  The model sees a
+plain contiguous fp32 batch.  After each call, every augmentation's ``last_params`` (``record_params=True``) is the replayed graph's,
+so it holds that step's draws.
 
 Batch mixing (``mix``, a callable ``(images, targets) -> (images, targets)`` such as ``pdt.data.CutMix`` or ``pdt.data.MixUp``): every
 step runs ``x, t = mix(x, t)`` after ``augment``; with accumulation, once on all k·b rows before the micro-batches are sliced, as an
@@ -90,6 +91,10 @@ class GraphedTrainStep:
         if not torch.cuda.is_available():
             raise RuntimeError("GraphedTrainStep needs CUDA")
         self.augment = augment
+        self._augments = list(augment) if isinstance(augment, (list, tuple)) else ([] if augment is None else [augment])
+        for t in self._augments:
+            if not callable(t):
+                raise TypeError(f"GraphedTrainStep(augment=...): {t!r} is not callable")
         self.mix = mix
         self.averaged_model = averaged_model
         self._averaged_source = getattr(model, "module", model)   # the averaged model was copied from the bare model
@@ -169,8 +174,8 @@ class GraphedTrainStep:
         inputs = self.static_inputs if inputs is None else inputs
         from ..ops import functional as OF
 
-        if self.augment is not None:
-            inputs = [self.augment(inputs[0])] + list(inputs[1:])   # all k·b rows at once under accumulation
+        for t in self._augments:
+            inputs = [t(inputs[0])] + list(inputs[1:])   # all k·b rows at once under accumulation
         if self.mix is not None:
             inputs = list(self.mix(inputs[0], inputs[1])) + list(inputs[2:])   # likewise, before the micro-batches are sliced
         if self.accumulation_steps > 1:
@@ -298,7 +303,7 @@ class GraphedTrainStep:
         comm = getattr(self.model, "comm", None)
         parity = (lambda: list(comm.parity_state())) if hasattr(comm, "parity_state") else (lambda: [])
         self.graphs, self.losses, self.norms = [], [], []
-        transforms = [t for t in (self.augment, self.mix) if t is not None]
+        transforms = self._augments + ([self.mix] if self.mix is not None else [])
         self._records = []   # per graph: (transform, its static parameter record) for each transform that records (record_params=True)
         p0 = parity()
         for k in range(2):

@@ -26,7 +26,7 @@ def require_native(what: str) -> None:
 if _HAS_NATIVE:
     from .functional import (adadelta_step, adagrad_step, adam_step, adamax_step, asgd_step, average_update, bn_apply,  # noqa: F401
                              bn_backward_apply, bn_backward_reduce, bn_finalize, bn_local_stats, conv_bn_relu_pool, cross_entropy,
-                             grad_norm_clip, grad_scale, linear, mix_batch, nadam_step, radam_step, random_affine, rmsprop_step,
+                             elastic, grad_norm_clip, grad_scale, linear, mix_batch, nadam_step, radam_step, random_affine, rmsprop_step,
                              rprop_step, sgd_step)
 else:  # CPU-only build of the extension: keep the names importable, fail loudly on use
     def _missing(name):
@@ -36,7 +36,7 @@ else:  # CPU-only build of the extension: keep the names importable, fail loudly
         return f
 
     for _n in ("adadelta_step", "adagrad_step", "adam_step", "adamax_step", "asgd_step", "average_update", "bn_apply", "bn_backward_apply",
-               "bn_backward_reduce", "bn_finalize", "bn_local_stats", "conv_bn_relu_pool", "cross_entropy", "grad_norm_clip", "grad_scale",
+               "bn_backward_reduce", "bn_finalize", "bn_local_stats", "conv_bn_relu_pool", "cross_entropy", "elastic", "grad_norm_clip", "grad_scale",
                "linear", "mix_batch", "nadam_step", "radam_step", "random_affine", "rmsprop_step", "rprop_step", "sgd_step"):
         globals()[_n] = _missing(_n)
 

@@ -723,6 +723,19 @@ def random_affine(x: torch.Tensor, degrees, translate=None, scale=None, shear=No
                             bool(bilinear), float(fill), generator, bool(record_params))
 
 
+def elastic(x: torch.Tensor, weights: Optional[torch.Tensor], kernel_sizes, alpha, bilinear: bool = True, fill: float = 0.0,
+            generator: Optional[torch.Generator] = None, record_params: bool = False):
+    """torchvision's ``v2.ElasticTransform`` on every image of ``x`` (fp32 contiguous CUDA ``[B, C, H, W]``) with its own field: the
+    noise ``dx0``, ``dy0`` ~ U[-1, 1) drawn on the device from ``generator``'s Philox state (the device's default CUDA generator when
+    None), blurred separably with ``weights`` (fp32 on ``x``'s device: for dx the (kx, sigma[0]) then (kx, sigma[1]) 1-D weights,
+    then the same for dy with ky; None when ``kernel_sizes`` is (0, 0), no blur), scaled by ``alpha`` / (W, H), then sampled: one
+    launch, graph-capturable, every replay drawing new values.  Returns ``(out, noise)``: ``noise`` is the fp32 ``[B, 2, H, W]``
+    (dx0, dy0) with ``record_params``, None otherwise.  ``pdt.data.ElasticTransform`` is the user-facing transform that validates
+    the arguments and builds the weights."""
+    return _C.elastic(x, weights, int(kernel_sizes[0]), int(kernel_sizes[1]), float(alpha[0]), float(alpha[1]), bool(bilinear),
+                      float(fill), generator, bool(record_params))
+
+
 def mix_batch(x: torch.Tensor, targets: torch.Tensor, num_classes: Optional[int], alpha: float, cutmix: bool,
               generator: Optional[torch.Generator] = None, record_params: bool = False):
     """torchvision's ``MixUp`` (``cutmix=False``) or ``CutMix`` on ``x`` (fp32 contiguous CUDA ``[B, C, H, W]``), image i paired with

@@ -35,6 +35,7 @@ GROUPS = {
     "symm_emu": ["tests/test_symm_kernels_emulated.py"],
     "random_affine": ["tests/test_random_affine.py"],
     "mix": ["tests/test_mix.py"],
+    "elastic": ["tests/test_elastic.py"],
 }
 
 
